@@ -2,13 +2,13 @@
 """bench.py — suggestions/sec at (N=8192 trials, M=1,048,576 candidates, D=32), Matérn-5/2 GP, EI  (BASELINE.json cfg 3).
 
 One "step" = one full suggestion at fixed θ: Gram → Cholesky → L⁻¹/alpha → sweep of this rank's candidate rows (stratified
-calibration rows, tensor-core K*, cta_group::2 ranking contraction, acquisition bounds, FP64 decision among the survivors) →
+calibration rows, tensor-core K*, wgmma ranking contraction, acquisition bounds, FP64 decision among the survivors) →
 first-index argmax (→ one 32-byte-per-rank NCCL all-gather inside libkbo when N > 1).
 
   value     device-resident inputs, CUDA-event timed, max over ranks.
   e2e       the same through kbo_suggest_host: HOST buffers in (pinned), H2D + 32-byte D2H inside the timed region.
   roofline  the dominant kernel (tc_rank_kernel): algorithmic flops (rows·N² per launch) ÷ its mean launch time (CUDA events
-            recorded around every launch inside libkbo) against the measured bf16 tensor peak; `kstar_hbm` the K* generation
+            recorded around every launch inside libkbo) against the bf16 tensor peak (MEASURED_PEAKS.json, else the H100 SXM data sheet); `kstar_hbm` the K* generation
             kernel against the measured HBM bandwidth; `acquisition_hbm` the standalone acquisition pass ("acquisition HBM
             GB/s vs peak").
   cpu_baseline / --impl reference   the oracle (fp64 NumPy/SciPy port of the sklearn path; scikit-optimize itself is not
@@ -19,6 +19,9 @@ Multi-GPU (torchrun, one rank per GPU): weak scaling — every rank runs the ful
 sweeps its own 1,048,576-row shard of an R·1,048,576 grid; `value` counts R (N=8192, M=1M)-suggestion units per step and
 `suggestions_per_s_actual` the suggestions over the R·M grid actually produced.  `other_configs` adds what BASELINE.json asks
 beyond that: the SAME 1M grid split R ways (strong scaling) and, at R = 8, config 5 (one 16M grid, 2M rows per rank).
+
+--dump-outputs DIR writes what the timed path returned in its last step (the suggestion: index, value, mu, std) as float64 .npy
+files, so two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -48,22 +51,8 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]), src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, src="fallback")
-
-
-def kernel_traffic(name, rows_per_launch):
-    """dram bytes per launch from the committed `ncu --set full` capture of that kernel (profiles/), scaled by rows."""
-    p = os.path.join(ROOT, "profiles", name)
-    if not os.path.exists(p):
-        return None
-    d = json.load(open(p))
-    out = {"bytes_per_launch": (d["dram_read_bytes"] + d["dram_write_bytes"]) * rows_per_launch / d["rows"], "source": d["source"],
-           "captured_rows_per_launch": d["rows"]}
-    for k in ("algorithmic_bytes_per_launch", "ncu_tensor_pipe_active_pct_of_active", "ncu_dram_pct_of_peak", "ncu_l2_hit_pct", "ncu_l2_to_sm_bytes",
-              "why_traffic_exceeds_algorithmic"):
-        if k in d:
-            out[k] = d[k] * rows_per_launch / d["rows"] if k in ("algorithmic_bytes_per_launch", "ncu_l2_to_sm_bytes") else d[k]
-    return out
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense BF16 989 TFLOP/s — not reached figures, upper bounds
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -195,6 +184,7 @@ def main():
     ap.add_argument("--k-span", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the last timed step's suggestion as DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -263,6 +253,8 @@ def main():
     if rank == 0:
         sampler.start()
     ms_step, best = timed(step_device, args.steps, 0)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, best)
     survivors, rank_err, rank_mu_err, unrefined = eng.last_contenders(), eng.last_rank_error(), eng.last_rank_mu_error(), eng.last_unrefined()
 
     # ---- end to end: host buffers through kbo_suggest_host (the exchange is inside the call when N > 1) ---------------
@@ -285,7 +277,7 @@ def main():
     mean = lambda k: float(np.mean([t[k] for t in tims]))   # noqa: E731
 
     # ---- standalone acquisition pass: the HBM-bound kernel (8 B/candidate in + 4 B out), at this rank's M and at cfg5's 16M ----
-    flush64 = torch.zeros((256 << 20) // 8, dtype=torch.int64, device=dev)   # > 126 MB L2
+    flush64 = torch.zeros((256 << 20) // 8, dtype=torch.int64, device=dev)   # > 50 MB L2
     flush_sink = torch.zeros((), dtype=torch.int64, device=dev)
 
     def acq_bw(Ma):
@@ -294,7 +286,7 @@ def main():
         acq_o = torch.empty(Ma, device=dev, dtype=torch.float32)
         ts = []
         for i in range(10):
-            # evict with READS of a 256 MiB buffer: a write-based flush leaves ~126 MB of dirty L2 lines whose write-back then
+            # evict with READS of a 256 MiB buffer: a write-based flush leaves ~50 MB of dirty L2 lines whose write-back then
             # competes with the timed kernel for DRAM bandwidth
             flush_sink.copy_(flush64.sum())
             a0, a1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -348,7 +340,7 @@ def main():
         other["full_ranking_pass"] = {"ms_per_step_e2e": float(np.mean([t["total_ms"] for t in full_tims])),
                                       "variance_kernel_ms": float(np.mean([t["var_kernel_ms"] for t in full_tims])),
                                       "kstar_kernel_ms": float(np.mean([t["cross_kernel_ms"] for t in full_tims])),
-                                      "note": "kbo_set_rank_prefix(h, 0): no pruning pass — tensor-core K* and cta_group::2 contraction over the whole grid "
+                                      "note": "kbo_set_rank_prefix(h, 0): no pruning pass — tensor-core K* and wgmma contraction over the whole grid "
                                               "(also what a landscape too flat to prune costs, before any three-product redo)"}
     if rank == 0 and world == 1 and not args.no_extras:
         try:
@@ -407,7 +399,7 @@ def main():
         fit_flops = N ** 3 / 3.0 + (lead ** 3 / 3.0 + 4.0 * N * N if lazy_fit else N ** 3 / 3.0)
         fit_tflops = fit_flops / (mean("fit_ms") * 1e-3) / 1e12
         fp64_peak = eng.fp64_peak_tflops()
-        kernel = "tc_rank_kernel" if rank_tc else ("tc_variance_pair_kernel" if os.environ.get("KBO_TC_PAIR", "1") != "0" else "tc_variance_kernel")
+        kernel = "tc_rank_kernel" if rank_tc else ("tc_variance_kernel<true> (2-CTA cluster)" if os.environ.get("KBO_TC_PAIR", "1") != "0" else "tc_variance_kernel<false>")
         Npad = (N + 255) // 256 * 256
         kstar_bytes = rows_per_launch * Npad * 2.0
         line = {
@@ -415,14 +407,14 @@ def main():
             "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None,
             "suggestions_per_s_actual": 1e3 / ms_step,
-            "dtype": ("f64 fit / ranking pass: fp16 hi+lo tcgen05 dot products -> fp32 kernel values -> fp16 K* plane, fp16 cta_group::2 contraction "
+            "dtype": ("f64 fit / ranking pass: fp16 hi+lo wgmma dot products -> fp32 kernel values -> fp16 K* plane, fp16 wgmma contraction "
                       "(fp32 accumulate), fp32 mean / FP64 K*, mean and variance for the calibration rows and the survivors that decide"
-                      if rank_tc else "f64 fit+mean / fp16 tcgen05 ranking pass over sigma² (1 product, fp32 accumulate) + FP64 decision among the survivors"
-                      if fast_rank else "f64 fit+mean / fp16x3-split tcgen05 variance (fp32 accumulate)") if args.var_mode == "tc" else "f64",
+                      if rank_tc else "f64 fit+mean / fp16 wgmma ranking pass over sigma² (1 product, fp32 accumulate) + FP64 decision among the survivors"
+                      if fast_rank else "f64 fit+mean / fp16x3-split wgmma variance (fp32 accumulate)") if args.var_mode == "tc" else "f64",
             "data": "synthetic",
             "config": {"workload": W.describe(N, M, D, world, KERNEL, ACQ),
                        "kernel": KERNEL, "acq": ACQ, "per_gpu_candidates": M, "grid_candidates": world * M, "var_mode": args.var_mode,
-                       "l2": "inputs larger than L2 (Xc 128 MiB, W plane 128 MiB, K* scratch 4 GiB per chunk)",
+                       "l2": "inputs larger than the 50 MB L2 (Xc 128 MiB, W plane 128 MiB, K* scratch up to 4 GiB per chunk)",
                        "argmax_index": best.index, "argmax_value": best.value, "argmax_mu": best.mu, "argmax_std": best.std,
                        "survivors_decided_in_fp64": survivors, "decision": unrefined,
                        "pruning_pass": ({"prefix_of_trial_tiles": "first eighth (1/64 of the contraction's MMAs)", "candidates_kept": prefix_survivors,
@@ -439,12 +431,11 @@ def main():
                          "frac": achieved_tf / pk["tf_sus"], "peak_source": f"bf16_tflops_sustained, {pk['src']}",
                          "frac_of_burst_peak": achieved_tf / pk["tf_burst"],
                          "issued_mma_tflops": mma_products * achieved_tf * (1.0 + 256.0 / N), "mma_products_per_term": mma_products,
-                         "traffic": kernel_traffic("tcrank_traffic.json" if rank_tc else "tcvar_traffic.json", rows_per_launch) if (rank_tc or not fast_rank) else None,
                          "launch_ms": var_launch_ms, "launches_per_step": chunks, "flops_per_launch": flops_launch,
-                         "launch_note": "variance phase time / chunks (CUDA events inside libkbo around tc_rank_kernel + its 6 µs finish kernel)",
+                         "launch_note": "variance phase time / chunks (CUDA events inside libkbo around tc_rank_kernel + its finish kernel)",
                          "share_of_step": {"note": "where the product path's step goes (phases_ms / ms_per_step); this object rates the kernel that carries "
                                                    "the path's M·N² term, which the pruning pass shrinks to 1/64 — the step's largest kernels are rated in "
-                                                   "fit_fp64 (dgemm64_kernel, FP64 DMMA) and kstar_hbm / profiles (tc_kstar_kernel, MUFU-bound)",
+                                                   "fit_fp64 (dgemm64_kernel, FP64 DMMA) and kstar_hbm (tc_kstar_kernel, MUFU-bound)",
                                            "fit": mean("fit_ms") / ms_step, "kstar_kernel": mean("cross_kernel_ms") / ms_step,
                                            "prefix_contraction_this_kernel": mean("var_kernel_ms") / ms_step, "calibration": mean("calib_ms") / ms_step,
                                            "bounds_and_fp64_decision": mean("acq_kernel_ms") / ms_step},
@@ -456,14 +447,13 @@ def main():
                          "peak_source": "measured in this run: DMMA m8n8k4 on register operands, one 256-thread CTA per SM (kbo_debug_fp64_peak; "
                                         "MEASURED_PEAKS.json has no FP64 entry)",
                          "inverse": "lazy: leading %d rows of L^-1 + two panel solves" % lead if lazy_fit else "full",
-                         "note": "the step's largest phase; FP64 by contract (fp32 Cholesky / alpha move EI by up to 4e-4). The trailing updates run at "
-                                 "~24 TFLOP/s (K = 256 GEMMs, tests/studies/dgemm_probe.cu); the rest of the gap is the dependent chain of 128 "
-                                 "single-CTA diagonal blocks, which the second half of the factorisation waits on"},
+                         "note": "FP64 by contract (fp32 Cholesky / alpha move EI by up to 4e-4); the dependent chain of single-CTA diagonal "
+                                 "blocks, which the second half of the factorisation waits on, keeps it below the FP64 peak"},
             "kstar_hbm": {"bound": "hbm", "kernel": "tc_kstar_kernel" if rank_tc else "cross_mean_kernel", "bytes_per_launch": kstar_bytes,
                           "launch_ms": cross_launch_ms, "achieved": kstar_bytes / (cross_launch_ms * 1e-3) / 1e9, "peak": pk["hbm"], "unit": "GB/s",
                           "frac": kstar_bytes / (cross_launch_ms * 1e-3) / 1e9 / pk["hbm"],
                           "note": "algorithmic bytes = the fp16 K* plane written once (rows x Npad x 2 B); the kernel is MUFU/issue-bound (2 MUFU + ~15 "
-                                  "instructions per pair), not bandwidth-bound — profiles/r9_tckstar_cfg3_summary.csv"},
+                                  "instructions per pair), not bandwidth-bound"},
             "acquisition_hbm": {"kernel": "acq_kernel<float>", "bytes_per_candidate": 12, "candidates": M, "achieved": acq_gbs, "peak": pk["hbm"],
                                 "unit": "GB/s", "frac": acq_gbs / pk["hbm"], "peak_source": f"hbm_gbs, {pk['src']}", "launch_ms": acq_launch_ms,
                                 "at_16M_candidates": {"achieved": acq_gbs16, "frac": acq_gbs16 / pk["hbm"], "launch_ms": acq_launch_ms16},
@@ -479,6 +469,13 @@ def main():
     eng.close()
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, best):
+    """The suggestion the timed path returned in its last step, one float64 array per field (the grid index is exact in float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name in ("index", "value", "mu", "std"):
+        np.save(os.path.join(out_dir, f"suggestion_{name}.npy"), np.array([getattr(best, name)], dtype=np.float64))
 
 
 def grpc_cfg3_request(local, X, y, N, M, D):

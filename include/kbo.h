@@ -1,5 +1,5 @@
 /*
- * kbo.h — C ABI of libkbo.so, the B200 (sm_100a) GP-suggestion engine.
+ * kbo.h — C ABI of libkbo.so, the H100 (sm_90a) GP-suggestion engine.
  *
  * This is the drop-in boundary (SURVEY.md §8(b) "B-inner").  The reference platform repo
  * (/root/reference = kubeflow/kubeflow @ 6d6b78bc) reaches the suggestion service only through
@@ -55,7 +55,7 @@ typedef enum kbo_acq_kind {
 
 typedef enum kbo_var_mode {
   KBO_VAR_F64 = 0,     /* variance contraction V = K* W^T on the FP64 SIMT pipe (checker precision) */
-  KBO_VAR_TC_F16X3 = 1, /* tcgen05 tensor cores, fp16 hi/lo split (3 MMAs per product), fp32 accum */
+  KBO_VAR_TC_F16X3 = 1, /* wgmma tensor cores, fp16 hi/lo split (3 MMAs per product), fp32 accum */
   KBO_VAR_AUTO = 2      /* FP64 while M·N² <= 2e11 (a few ms of FP64 pipe), tensor cores above that    */
 } kbo_var_mode;
 
@@ -73,7 +73,7 @@ typedef struct kbo_params {
   double kappa;            /* LCB weight (skopt default 1.96) */
   const double* length_scale; /* HOST pointer, n_length_scale entries */
   int32_t n_length_scale;  /* 1 (isotropic) or D (anisotropic) */
-  int32_t tc_k_span;       /* TC mode: trials accumulated in TMEM before a drain to fp32 registers; 0 = default */
+  int32_t tc_k_span;       /* TC mode: trials accumulated by the tensor cores before a drain into a second fp32 register sum; 0 = default */
 } kbo_params;
 
 /* Result of one sweep: best acquisition value and its GLOBAL candidate index (lowest index wins ties,
@@ -121,8 +121,8 @@ int kbo_last_contenders(kbo_handle* h);
  * largest |sigma²(1 product) - sigma²(3 products)| seen on the calibration rows of the last such sweep. */
 int kbo_set_tc_fast(kbo_handle* h, int enabled);
 double kbo_last_rank_error(kbo_handle* h);
-/* The ranking pass builds its K* plane on the tensor cores (c·x as tcgen05 MMAs of fp16 hi/lo splits, kernel values in fp32,
- * only the hi plane written, the mean accumulated on the fly) and contracts it with cta_group::2 MMAs; 0 selects the FP64 K*
+/* The ranking pass builds its K* plane on the tensor cores (c·x as wgmma MMAs of fp16 hi/lo splits, kernel values in fp32,
+ * only the hi plane written, the mean accumulated on the fly) and contracts it with wgmma m64n256k16 MMAs; 0 selects the FP64 K*
  * kernel + single-CTA-MMA cluster kernel of round 1 for that pass.  Default 1 (needs D <= 128; wider spaces use the FP64
  * kernel).  Either way the calibration rows are STRATIFIED over the grid (row i*M/n) and go through the FP64 K* kernel and
  * the three-product contraction; kbo_last_rank_mu_error is the largest |mean(ranking) - mean(FP64)| seen on them, in

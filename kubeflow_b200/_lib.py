@@ -72,7 +72,7 @@ def load() -> C.CDLL:
             _build.build()
         if not os.path.exists(LIB_PATH):
             raise ImportError(f"{LIB_PATH} is missing and could not be built: run `python -c 'import __graft_entry__ as g; "
-                              "g.build()'` (nvcc, sm_100a). There is no CPU fallback.")
+                              "g.build()'` (nvcc, sm_90a). There is no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, i32, i64, dbl = C.c_void_p, C.c_int32, C.c_int64, C.c_double
     pd = C.POINTER(C.c_double)

@@ -1,4 +1,4 @@
-"""Build libkbo.so in-tree with nvcc for sm_100a (the only target).  Used by __graft_entry__.build()."""
+"""Build libkbo.so in-tree with nvcc for sm_90a (the only target).  Used by __graft_entry__.build()."""
 from __future__ import annotations
 
 import glob
@@ -9,7 +9,7 @@ import subprocess
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libkbo.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 
 
 def sources():
@@ -25,7 +25,7 @@ def needs_build() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile csrc/*.cu into kubeflow_b200/libkbo.so (sm_100a only).  Safe under torchrun: ranks serialise on a lock
+    """Compile csrc/*.cu into kubeflow_b200/libkbo.so (sm_90a only).  Safe under torchrun: ranks serialise on a lock
     file and the library is written to a temporary name first, so no rank ever dlopens a half-written .so."""
     import fcntl
     if not force and not needs_build():

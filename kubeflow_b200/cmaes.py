@@ -13,7 +13,7 @@ from . import _lib as L
 class CmaEs:
     def __init__(self, mean, sigma: float, popsize: int | None = None, seed: int = 0, device: int = 0):
         if not torch.cuda.is_available():
-            raise RuntimeError("kubeflow_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         mean = np.ascontiguousarray(np.asarray(mean, dtype=np.float64))
         self.D = int(mean.shape[0])
         self.popsize = int(popsize) if popsize else 4 + int(3 * np.log(self.D))

@@ -27,9 +27,9 @@ int kbo_create(kbo_handle** out, int device) {
   if (const char* e = getenv("KBO_RANK_TC")) h->rank_tc = atoi(e) != 0;
   if (const char* e = getenv("KBO_RANK_PREFIX")) h->rank_prefix = atoi(e);
   if (const char* e = getenv("KBO_LAZY_W")) h->lazy_w = atoi(e) != 0;
-  if (prop.major != 10) {
-    // sm_100a cubin only: refuse politely instead of failing at the first launch
-    h->err = "libkbo is built for sm_100a (B200) only";
+  if (prop.major != 9) {
+    // sm_90a cubin only: refuse politely instead of failing at the first launch
+    h->err = "libkbo is built for sm_90a (H100) only";
   }
   for (auto& ev : h->ev) cudaEventCreate(&ev);
   *out = h;
@@ -401,7 +401,7 @@ int kbo_debug_fp64_peak(kbo_handle* h, double* tflops_out) {
 }
 
 // Test hook (not in kbo.h): the ranking pass alone over M candidates (device pointer), normalised mean / variance copied to
-// caller-owned DEVICE float arrays.  mode 0 = FP64 K* kernel + one-product cluster kernel, 1 = tensor-core K* + cta_group::2
+// caller-owned DEVICE float arrays.  mode 0 = FP64 K* kernel + one-product cluster kernel, 1 = tensor-core K* + wgmma
 // ranking kernel.  plane_out (optional, M × Npad fp16, M <= one chunk) receives the K* hi plane the contraction consumed.
 int kbo_debug_rank_pass(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, int32_t mode, float* mun_out, float* varn_out, void* plane_out,
                         void* stream) {

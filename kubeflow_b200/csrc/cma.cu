@@ -337,7 +337,7 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
                                        (const double*)c->Dv.p, (double*)c->ps.p, (double*)c->pc.p, (double*)c->scal.p, (double*)c->yw.p);
   KBO_LAUNCH_CHECK(h);
   // R = Σ w°_i y_i y_iᵀ  (D×D = YwT[D×λ]·Ys[λ×D]) as split-K over 256-sample slices: a 128×128 output is only two
-  // tiles of the GEMM, so without the split a K = 4096 product ran on 2 CTAs (337 µs); the slices fill 2·λ/256 CTAs
+  // tiles of the GEMM, so without the split a K = 4096 product ran on 2 CTAs; the slices fill 2·λ/256 CTAs
   const int nsl = c->lam_pad / 256;
   dgemm64_launch<false, EPI_STORE>(s, D, D, 256, (const double*)c->YwT.p, c->lam_pad, (const double*)c->Ys.p, D, (double*)c->R.p, D, 1.0, 0.0, KM_FULL,
                                    0, TS_NONE, nsl, 256, 256LL * D, (long long)D * D);

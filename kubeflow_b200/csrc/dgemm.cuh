@@ -17,7 +17,7 @@ enum { TS_NONE = 0, TS_LOWER = 1 };
 //  * the slab store — lanes = 16 consecutive k of one row — is contiguous;
 //  * the DMMA fragment load — lanes (g, t) = (row, k) — lands on bank (g·pitch + t) mod 16 = 4g + t for g < 4: distinct.
 // (The first layout, [k][row] with pitch ≡ 8, had the loads 2-way and the stores 8-way conflicted: ncu showed the tensor pipe 53 %
-// active, `mio_throttle` the top stall — profiles/README.md.)
+// active, `mio_throttle` the top stall.)
 #define DG_LDK (DG_BK + 4)
 #define DG_LDB (DG_BN + 4)
 #define DG_A_DOUBLES (DG_BM * DG_LDK)
@@ -26,7 +26,7 @@ enum { TS_NONE = 0, TS_LOWER = 1 };
 #define DG_SMEM_BYTES (2 * DG_STAGE_DOUBLES * 8 + 2 * DG_BM * 8)   // two slabs + the row-sum epilogue's scratch
 
 // FP64 tensor-core MMA (DMMA), warp-level: D(8×8) += A(8×4)·B(4×8).  Fragments (lane = 4g + t): a = A[g][t], b = B[t][g],
-// c/d = C[g][2t], C[g][2t+1].  On B200 DMMA and plain DFMA reach the same 37 TFLOP/s (tests/studies/dmma_probe.cu); the point of
+// c/d = C[g][2t], C[g][2t+1].  DMMA and plain DFMA peak rates: tests/studies/dmma_probe.cu; the point of
 // the tensor form is that one fragment load feeds 256 FMAs, so the FP64 GEMM-shaped work (potrf / trtri updates, FP64 variance
 // contraction, CMA-ES products) is not bound by shared-memory loads.
 __device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, double b) {

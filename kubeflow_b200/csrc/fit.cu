@@ -3,7 +3,7 @@
 //   $SK/kernels.py:1559-1570 RBF, :1713-1729 Matern(nu=2.5)
 // Why FP64 here (not fp32/tensor cores): the posterior mean is K*·alpha with |alpha|₂ up to ~3e3 for the
 // workloads of record; fp32 L/alpha moves EI by 1e-4 (measured, DESIGN.md §numerics) against a 1e-5 contract.
-// B200 has a full FP64 pipe, and the fit is O(N³/3) once per suggestion next to the O(M·N²) sweep.
+// H100 has a full FP64 pipe, and the fit is O(N³/3) once per suggestion next to the O(M·N²) sweep.
 #include <stdlib.h>
 
 #include "kbo_internal.cuh"
@@ -332,7 +332,7 @@ static int fit_streams(kbo_handle* h, int n_panels) {
 // between — most of the GPU idles — and the inverse W_i,<i = −W_ii·(L_i,<i·W_<i,<i) of row panel i needs only the rows of L the
 // Cholesky has already finished, so it runs on another stream under the chain.  In potrf_impl every 64-block step touches all
 // N−k rows below it (panel solve + in-panel update: ~125 CTAs each), so when a trailing update runs beside the chain those kernels
-// queue for SM slots behind 70 µs GEMM blocks and the chain doubles in length.  Here the dependent chain
+// queue for SM slots behind long GEMM blocks and the chain doubles in length.  Here the dependent chain
 // of a 256-column panel works on its 256×256 DIAGONAL block only — four single-CTA factorisations, ≤ 3-CTA solves, ≤ 9-CTA
 // updates — then inverts that block (needed for L⁻¹ anyway) and solves the whole panel below it with ONE GEMM against the
 // inverse.  The trailing update is issued on a second stream as [next column block | rest]: the next panel's chain starts as
@@ -516,11 +516,11 @@ static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double
 
 // ------------------------------------------------------------------------------------------------
 // Version 3: the chain on its OWN SMs, the panel below it solved in its shadow.
-// What v2's chain-stream trace showed (KBO_FIT_TRACE, N = 8192): the four single-CTA factorisations of a panel take 0.21 ms
-// on an idle GPU and up to 0.55 ms while trailing updates run — the update GEMMs hold two 128-register CTAs per SM, i.e. the
+// What v2's chain-stream trace showed (KBO_FIT_TRACE, N = 8192): the four single-CTA factorisations of a panel take more
+// than twice as long while trailing updates run as on an idle GPU — the update GEMMs hold two 128-register CTAs per SM, i.e. the
 // whole register file, so a chain kernel waits until an SM drains (stream priority orders pending CTAs; it does not preempt) —
-// and W_PP plus the one-GEMM panel solve add 0.2 ms of dependent launches per panel.  Here
-//  * a GREEN CONTEXT (CUDA 12.4+) gives the chain stream 8 SMs of its own; everything else runs on the other 140.  If the
+// and W_PP plus the one-GEMM panel solve add dependent launches per panel.  Here
+//  * a GREEN CONTEXT (CUDA 12.4+) gives the chain stream 8 SMs of its own; everything else runs on the rest.  If the
 //    driver cannot split the device the same streams are created unpartitioned and only the second point applies;
 //  * the rows below the diagonal block are solved column block by column block on a second stream AS the chain produces the
 //    64×64 inverses (four buffers): after the last factorisation only one 64-column solve remains before the trailing update
@@ -651,7 +651,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   // trailing update covers the rest — the chain can run `depth` − 1 panels ahead of the bulk (KBO_FIT_DEPTH=1: [next block | rest])
   static const int depth_env = getenv("KBO_FIT_DEPTH") ? atoi(getenv("KBO_FIT_DEPTH")) : 0;
   const int Dn = OW == 256 ? (depth_env >= 1 && depth_env <= 6 ? depth_env : 3) : 1;
-  // merged bulks: the bulk updates of panels (P, P+1), P even, run as ONE K = 512 GEMM after panel P+1 (26 instead of 24 TFLOP/s, half
+  // merged bulks: the bulk updates of panels (P, P+1), P even, run as ONE K = 512 GEMM after panel P+1 (a faster GEMM shape, half
   // the passes over the trailing matrix); the even panel covers the column block the merged region misses with one more distance GEMM
   static const bool pair_env = !(getenv("KBO_FIT_PAIR") && atoi(getenv("KBO_FIT_PAIR")) == 0);
   const bool pairs = pair_env && OW == 256 && Dn >= 2 && Dn <= 5;
@@ -695,9 +695,8 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   cudaEvent_t *ev_mid = ev_wpp + n_panels, *ev_t1 = ev_mid + n_panels, *ev_t2 = ev_t1 + n_panels;   // MID rows solved; their two 256×256 updates done
   // MID rows (KBO_FIT_MID=1, off by default) = the second block below the diagonal block, solved against W_PP on the chain's partition
   // together with their updates of blocks (P+2,P+1) and (P+2,P+2), so that the next panel's near shadow and the chain two panels on
-  // do not wait for the FAR shadow and the distance-1 update.  Measured (KBO_FIT_TRACE=2): the dependency does move, the factorisation
-  // does not get faster (12.2 vs 11.7 ms) — the big partition is saturated by the updates (2.2e11 flop in ~11 ms = 18 of the 22 TFLOP/s
-  // its K = 256 GEMM delivers on 140 SMs), so the far GEMMs are slow whichever chain waits for them.  Kept as a tested variant.
+  // do not wait for the FAR shadow and the distance-1 update.  The dependency moves (KBO_FIT_TRACE=2), but the big partition is
+  // saturated by the updates, so the far GEMMs are slow whichever chain waits for them.  Kept as a tested variant.
   static const bool mid_env = getenv("KBO_FIT_MID") && atoi(getenv("KBO_FIT_MID")) != 0;
   const bool midmode = mid_env && OW == 256 && Dn >= 2;
   for (int k = 1; k <= (pairs ? Dn + 1 : Dn); k++) all_streams.push_back(colS[k]);
@@ -866,7 +865,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
         }
         if (n_far > 0) {
           // FAR rows: one GEMM against W_PP (L_far = A_far·W_PPᵀ, out of place + copy) instead of seven 64-column steps — under the bulk
-          // updates every small kernel of the big partition waits for SM slots (KBO_FIT_TRACE=2 timeline: 0.44 ms for the seven steps,
+          // updates every small kernel of the big partition waits for SM slots (KBO_FIT_TRACE=2 timeline: the seven steps queue,
           // 0.2 for this)
           if (P > 0) KBO_CUDA(h, cudaStreamWaitEvent(ss, ev_col[P], 0));
           KBO_CUDA(h, cudaStreamWaitEvent(ss, ev_wpp[P], 0));
@@ -1120,7 +1119,7 @@ int kbo_i_gram(kbo_handle* h, const double* Xs, int N, int D, int kernel, double
   return KBO_OK;
 }
 // The Gram matrix in two launches: the first `tiles_first` 64-column tiles (all the first panel's chain and shadows read), an event,
-// then the rest — the factorisation starts 0.3 ms earlier (fit.cu: factor_and_invert_v3, e_early).
+// then the rest — the factorisation starts earlier (fit.cu: factor_and_invert_v3, e_early).
 static int gram_two_parts(kbo_handle* h, const double* Xs, int N, int D, int kernel, double amp, double noise, double* K, int ldk, int tiles_first,
                           cudaEvent_t e_first, cudaStream_t s) {
   const int nt = (N + 63) / 64, t1 = min(tiles_first, nt);
@@ -1306,7 +1305,7 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
 
 // ------------------------------------------------------------------------------------------------
 // The rows of W a lazy fit left out (and the full fp16 planes): row panels [w_lead, N) of W_i,<i = −W_ii·(L_i,<i·W_<i,<i), the
-// 512-wide diagonal blocks first.  ~10 ms at N = 8192 — what the fit saved; paid only by callers that need all of W.
+// 512-wide diagonal blocks first.  What the lazy fit saved; paid only by callers that need all of W.
 int kbo_i_ensure_w(kbo_handle* h, cudaStream_t s) {
   if (!h->fitted && !h->w_lead) return KBO_OK;
   if (h->w_full) return KBO_OK;

@@ -20,7 +20,7 @@ struct DevBuf {
 
 struct kbo_handle {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   std::string err;
   uint64_t scratch_limit = 4ull << 30;
 
@@ -61,8 +61,8 @@ struct kbo_handle {
   bool time_kernels = false;
   bool attr_fit = false, attr_tc = false;
   int tc_pair = 1;  // variance kernel variant (kbo_set_tc_pair)  // cudaFuncSetAttribute done for this handle's device
-  // ---- tensor-core K* generation (tc_kstar.cu) and cta_group::2 ranking kernel (tc_rank.cu) ---------------------------
-  bool rank_tc = true;        // kbo_set_rank_tc: the ranking pass builds K̃* on the tensor cores and contracts with cta_group::2 MMAs
+  // ---- tensor-core K* generation (tc_kstar.cu) and wgmma ranking kernel (tc_rank.cu) ---------------------------
+  bool rank_tc = true;        // kbo_set_rank_tc: the ranking pass builds K̃* on the tensor cores and contracts with wgmma MMAs
   bool ks_ready = false;      // trial-side operands below match the current fit
   DevBuf ks_center;           // D doubles: centre subtracted from the scaled coordinates (any fixed vector is valid)
   DevBuf ks_Xh, ks_Xl;        // trials, fp16 hi/lo planes, round_up(N,256) × round_up(D,32)
@@ -70,7 +70,7 @@ struct kbo_handle {
   DevBuf ks_Ch, ks_Cl, ks_nc; // candidate planes / squared norms of the current chunk
   DevBuf rk_part;             // [tile pairs][rows] partial Σ v² of the ranking kernel
   struct RkSched {
-    int key[5] = {-1, -1, -1, -1, -1};  // (row groups, j-tiles, clusters, first tile pair, end tile pair)
+    int key[5] = {-1, -1, -1, -1, -1};  // (row groups, j-tiles, CTAs, first tile pair, end tile pair)
     DevBuf dev;
     std::vector<int> host;
   } rk_sched[8];
@@ -195,6 +195,6 @@ int kbo_i_tc_kstar(kbo_handle* h, const void* Xc, int xc_dtype, int64_t rows, __
 int kbo_i_tc_rank(kbo_handle* h, const __half* Ksh, int64_t rows, const __half* Wh, int Npad, double amp, float* var_n_out, cudaStream_t s,
                   int p_begin = 0, int p_end = -1);
 // ---- tc_var.cu ---------------------------------------------------------------------------------
-// var_n[m] = amp − Σ_j (Σ_k K*[m,k] W[j,k])²  for the rows of one chunk, on tcgen05 tensor cores.
+// var_n[m] = amp − Σ_j (Σ_k K*[m,k] W[j,k])²  for the rows of one chunk, on the wgmma tensor cores.
 int kbo_i_tc_variance(kbo_handle* h, const __half* Ksh, const __half* Ksl, int64_t rows, const __half* Wh, const __half* Wl,
                       int Npad, double w_scale_inv, double amp, float* var_n_out, int k_span, cudaStream_t s, int nprod = 3, int jtiles = -1);

@@ -1,6 +1,6 @@
 // Kernel function k = f(d²) in FP64, branch-free, in registers.
 // (A Taylor-table variant was measured first: two data-dependent 16-byte loads per element made the kernel L1-gather
-//  bound — 104 ms vs 77 ms at cfg3 — so the table is gone; see profiles/README.md "r1 dead ends".)
+//  bound, slower than this polynomial — so the table is gone.)
 //   exp(x), x <= 0:  n = rint(x·log2e) by the 1.5·2⁵² trick, f = x·log2e − n (two-term log2e), 2^f by a degree-11
 //   polynomial in f (|f·ln2| ≤ 0.3466, truncation 6e-15 relative), scaled by 2ⁿ through the exponent bits.
 //   Results below 2⁻¹⁰²⁰ flush to 0 (irrelevant next to the 1e-5 contract).

@@ -1,8 +1,8 @@
 // Request ingestion (SURVEY.md §8(f)3): a serialized api.v1.beta1.GetSuggestionsRequest goes straight from wire bytes to
 // flat arrays — trial names (spans + 64-bit hashes), conditions, the objective metric and one double per (trial, parameter) —
 // without building a message tree.  Katib resends EVERY finished trial as strings on every call (8192 trials × 32 parameters
-// = 7.5 MB, 540k sub-messages at cfg3): protobuf-python (upb) takes 25 ms to parse that and Python 360 ms more to walk it
-// when the experiment is new to the service; this scan takes a few ms and hands NumPy the matrix.
+// = 7.5 MB, 540k sub-messages at cfg3): protobuf-python (upb) parsing it and a Python walk over it cost far more than the GPU step
+// when the experiment is new to the service; this scan hands NumPy the matrix directly.
 //
 // Host-only code (no device work): it lives in libkbo.so so the suggestion service has one native dependency.
 // Field numbers are those of kubeflow_b200/suggestion/api_pb.py's SCHEMA table (UNVERIFIED against upstream's api.proto, as

@@ -2,7 +2,7 @@
 // inverse W = L⁻¹ ($SK/_gpr.py:363 alpha_ = cho_solve(L, y); :460 V = solve_triangular(L, K*ᵀ)).
 //
 // The pruned sweep needs exact variances for a handful of candidates and alpha for one right-hand side; forming W costs N³/3
-// FP64 flop (10 ms at N = 8192, a third of the fit) to serve them.  A solve needs the factor L and the inverses of its 256×256
+// FP64 flop (a large share of the fit) to serve them.  A solve needs the factor L and the inverses of its 256×256
 // diagonal blocks, which the look-ahead factorisation computes anyway (fit.cu: W_PP, kept in the diagonal blocks of the W
 // buffer).  Forward, right-looking:   v_P = W_PP·b_P ;  b_>P −= L_>P,P·v_P      (P = 0, 1, …)
 // backward (alpha = L⁻ᵀ z):            a_P = W_PPᵀ·z_P ; z_<P −= (L_P,<P)ᵀ·a_P   (P = last, …, 0)

@@ -2,7 +2,7 @@
 //   $SK/_gpr.py:446 K* = k(Xc,X) | :447-450 mean | :460 V = L⁻¹K*ᵀ (here V = K*·Wᵀ, W = L⁻¹) | :480-500 variance
 //   skopt.acquisition.gaussian_ei / gaussian_lcb / gaussian_pi ; Optimizer._tell: X_cand[np.argmin(values)]
 // Per candidate chunk:  cross_mean_kernel (FP64: K*, μ = K*·alpha)  →  variance contraction (FP64 SIMT GEMM with a
-// fused Σv² epilogue, or the tcgen05 kernel in tc_var.cu)  →  once per sweep: acquisition + argmax.
+// fused Σv² epilogue, or the wgmma kernel in tc_var.cu)  →  once per sweep: acquisition + argmax.
 #include <type_traits>
 
 #include "kbo_internal.cuh"
@@ -483,7 +483,7 @@ acq_kernel(const T* __restrict__ mun, const T* __restrict__ varn, int64_t M, int
 // fp16×3 contraction; a near-tie could therefore pick a different index than the fp64 reference.  Every candidate whose
 // (recomputed, bit-identical) fp32 value is within `delta` of the maximum is a contender: its row goes through the FP64
 // K*/variance path again and the first-index argmax is taken over those FP64 values.  Contenders are a handful, so this is
-// one 14 µs pass plus a few small launches; the arrays returned for parity tests are not touched.
+// one pass plus a few small launches; the arrays returned for parity tests are not touched.
 #define KBO_REFINE_CAP 4096
 __global__ void __launch_bounds__(256)
 contender_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int64_t M, int acq, const double* __restrict__ scal, double xi,
@@ -707,7 +707,7 @@ static int launch_cross(kbo_handle* h, const XT* Xc, int64_t rows, int64_t rows_
   KBO_CUDA(h, cudaFuncSetAttribute(cross_mean_kernel<XT, MT, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const unsigned gx = (unsigned)((rows_grid + CM_BM - 1) / CM_BM);
   // fewer CTAs than one wave (two per SM): split the trial tiles so every SM works — the 74 CTAs of the calibration rows left half
-  // of the GPU idle for 1.5 ms
+  // of the GPU idle
   const int ntiles = (h->N + CM_BN - 1) / CM_BN;
   int nsplit = 1;
   if (gx < 2u * h->sm_count) nsplit = (int)min((unsigned)min(ntiles, 16), max(1u, 2u * h->sm_count / gx));
@@ -1291,7 +1291,7 @@ static int fast_pick(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int
 // cal_idx (row indices), cal_mu (normalised mean), var_cal (normalised variance).  Uses the K* scratch planes, so it runs
 // before the first chunk.
 static int calibration_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int* cal_n_out, cudaStream_t s, int jtiles) {
-  // one wave of the three-product cluster kernel: 74 clusters × 128 rows on a B200.  The bounds are 8 × the largest error seen on
+  // one wave of the three-product cluster kernel: sm_count / 2 clusters × 128 rows.  The bounds are 8 × the largest error seen on
   // these rows; the errors are sums of thousands of rounding terms (light-tailed: the maximum over 1e6 rows of a Gaussian exceeds
   // the maximum over 1e4 by ~1.2×), so the sample size is not what the margin hinges on — its being stratified is.
   int64_t want = (int64_t)h->sm_count * 64;
@@ -1346,7 +1346,7 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
   const double* scal = (const double*)h->scal.p;
   // array-free tensor-core sweeps rank with one fp16 product and let the FP64 refinement decide (fast_pick above)
   const bool fast = tc && !force_three && h->tc_fast && h->tc_refine && h->tc_pair && !mu_out && !std_out && !acq_out && M < 0x7fffffff;
-  // ... and, by default, build that pass's K̃* on the tensor cores and contract it with cta_group::2 MMAs (tc_kstar.cu, tc_rank.cu)
+  // ... and, by default, build that pass's K̃* on the tensor cores and contract it with wgmma MMAs (tc_kstar.cu, tc_rank.cu)
   const bool rank_tc = fast && h->rank_tc && h->ks_ready;
   int cal_n = 0;
   int64_t chunk;
@@ -1365,7 +1365,7 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
       KBO_TRY(kbo_reserve(h, h->Ksl, sizeof(__half) * (size_t)cal_pad * Npad));   // the lo plane exists for the calibration rows only
     } else {
       // wave-aligned chunks: the variance kernel runs one 128-row CTA per SM, the K* kernel two — a chunk that is a multiple
-      // of sm_count·128 rows leaves no partial wave (512 CTAs on 148 SMs idled 13 % of the tensor time; profiles/README.md)
+      // of sm_count·128 rows leaves no partial wave
       chunk = (int64_t)(h->scratch_limit / ((size_t)Npad * 4));
       chunk = chunk >= wave ? chunk / wave * wave : chunk / 128 * 128;
       if (chunk < 128) chunk = 128;

@@ -1,10 +1,9 @@
-// tcgen05 / TMEM / TMA / mbarrier helpers shared by the sm_100a tensor-core kernels (tc_var.cu, tc_kstar.cu, tc_rank.cu).
-// Inline PTX only; descriptor bit layouts follow the sm_100 UMMA shared-memory / instruction descriptors.
+// wgmma / TMA / mbarrier helpers shared by the sm_90a tensor-core kernels (tc_var.cu, tc_kstar.cu, tc_rank.cu).
+// Inline PTX only; the shared-memory matrix descriptor follows the sm_90 GMMA descriptor layout.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
-#include <stdio.h>
 
 namespace tcx {
 
@@ -51,26 +50,19 @@ __device__ __forceinline__ bool mbar_try_wait_cluster(uint32_t bar, uint32_t par
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU.
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, int tag) {
+// Bounded waits: a protocol bug traps (the launch fails with an error) instead of hanging the GPU.  No printf here: a function call
+// inside a warp that has wgmma groups in flight makes ptxas serialise the wgmma pipeline.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("kbo tcgen05 kernel: mbarrier wait timed out (tag %d, block %d, thread %d, parity %u)\n", tag, blockIdx.x, threadIdx.x, parity);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > 4000000000LL) __trap();
 }
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity, int tag) {
+__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait_cluster(bar, parity)) return;
   const long long t0 = clock64();
-  while (!mbar_try_wait_cluster(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {
-      printf("kbo tcgen05 kernel: mbarrier wait timed out (tag %d, block %d, thread %d, parity %u)\n", tag, blockIdx.x, threadIdx.x, parity);
-      __trap();
-    }
-  }
+  while (!mbar_try_wait_cluster(bar, parity))
+    if (clock64() - t0 > 4000000000LL) __trap();
 }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
@@ -84,69 +76,51 @@ __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* 
       "l"(map), "r"(bar), "h"(mask), "r"(c0), "r"(c1)
       : "memory");
 }
-// 2-CTA (cta_group::2) load: the data lands in THIS CTA's shared memory, the transaction bytes are counted on the barrier at
-// the same offset in the LEADER CTA (peer bit of the shared::cluster address cleared) — where the pair's MMA thread waits.
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-               "l"(map), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-               : "memory");
-}
-
-// K-major, SWIZZLE_64B shared-memory matrix descriptor (sm_100 UMMA descriptor, version 1):
-// rows are 64 B (32 fp16), 8-row groups 512 B apart (SBO), LBO unused for swizzled K-major (canonical value 1).
-__device__ __forceinline__ uint64_t umma_desc_sw64(uint32_t saddr) {
+// K-major, SWIZZLE_64B shared-memory matrix descriptor (sm_90 GMMA): rows are 64 B (32 fp16), 8-row groups 512 B apart
+// (SBO), LBO unused for swizzled K-major (canonical value 1).  A k16 step inside the 64 B row advances the start address by 32 B.
+__device__ __forceinline__ uint64_t gmma_desc_sw64(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);        // start address  [0,14)
   d |= (uint64_t)1 << 16;                          // LBO            [16,30)
   d |= (uint64_t)(512 >> 4) << 32;                 // SBO            [32,46)
-  d |= (uint64_t)1 << 46;                          // version        [46,48)
-  d |= (uint64_t)4 << 61;                          // SWIZZLE_64B    [61,64)
+  d |= (uint64_t)2 << 62;                          // SWIZZLE_64B    [62,64)
   return d;
 }
-// kind::f16 instruction descriptor: D=F32, A=B=F16, both K-major, N (multiple of 16, ≤ 256), M (128, or 256 with cta_group::2)
-__device__ __forceinline__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+// Warpgroup MMA, D[64 × N] (fp32, registers) (+)= A[64 × 16] · B[N × 16]ᵀ, A and B fp16 K-major in shared memory.
+// Fragment of thread (warp w of the warpgroup, lane = 4g + t): d[4i + e] is row 16w + g + 8·(e >> 1), column 8i + 2t + (e & 1).
+__device__ __forceinline__ void wgmma_f16_n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// issued by the leader CTA of a pair only: D[256 × N] over both CTAs' TMEM, A = each CTA's own 128 rows, B = each CTA's N/2 rows
-__device__ __forceinline__ void umma_f16_2sm(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
+
+__device__ __forceinline__ void wgmma_f16_n256(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// the accumulator registers are read by ordinary code only after wgmma_wait<0>(); this keeps the compiler from moving those reads
+template <int R>
+__device__ __forceinline__ void acc_fence(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm_mc(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;

@@ -1,38 +1,37 @@
 // K* = amp·k(Xc, X) on the tensor cores, for the RANKING pass of the sweep ($SK/_gpr.py:446, $SK/kernels.py:1559-1570 RBF,
-// :1713-1729 Matérn-5/2).  sm_100a only: tcgen05.mma + TMEM + TMA.
+// :1713-1729 Matérn-5/2).  sm_90a: wgmma + TMA + mbarrier.
 //
-// The FP64 cross kernel (sweep.cu) spends ~75 FP64 operations per (candidate, trial) pair: 59 ms per suggestion at cfg3, on a
+// The FP64 cross kernel (sweep.cu) spends ~75 FP64 operations per (candidate, trial) pair, on a
 // pass whose output the ranking pass then rounds to fp16.  Here the pairwise distances are the dense product they are:
 //     d²(c, x) = |c|² + |x|² − 2 c·x ,   c·x = Σ_d ĉ_d x̂_d   (ĉ, x̂: coordinates / ℓ_d, centred on the trials' mean, pre-scaled
 //                                                              by √5 (Matérn) or 1/√2 (RBF) so the epilogue needs no constant)
 // with c·x on the tensor cores.  Coordinates are split into fp16 hi + lo (|x̂ − hi − lo| ≤ 2⁻²²|x̂|) and all four partial
-// products are accumulated in fp32 TMEM (small ones first), so c·x carries ~1e-7 relative error — the kernel value is then
+// products are accumulated in fp32 (small ones first), so c·x carries ~1e-7 relative error — the kernel value is then
 // evaluated in fp32 (MUFU sqrt / ex2) per element by the epilogue warps, written ONCE as the fp16 hi plane the ranking kernel
 // consumes (no lo plane, no FP64), and the normalised mean μ̃ = Σ_n K̃*[m,n]·alpha[n] is accumulated on the fly (four fp32 FMA
 // chains of four trials, summed and added in FP64 once per 16 trials).  Both μ̃ and the variance built from this plane are only used to RANK: their error
 // is measured per sweep on stratified calibration rows against the FP64 path and every candidate that could still be the
 // maximum is re-evaluated in FP64 (sweep.cu).
 //
-// CTA = 128 candidate rows (TMEM lanes); it walks all 256-trial tiles.  Candidate planes (128 × Dp, hi and lo) stay in shared
-// memory; trial planes stream through a 3-stage TMA ring one 32-feature slab at a time (SWIZZLE_64B);
-//   warp 0      TMA producer
-//   warp 1      MMA issuer (one thread): per (tile, slab) 2 k-steps × 4 products of M128 N256 K16 → one of two TMEM accumulators
-//   warps 2-17  epilogue: tcgen05.ld 16 columns → d² → kernel → fp16 → one 32-byte store per thread per batch; μ̃ partials
-// Per 128×256 tile the epilogue (~12 instructions and 2 MUFU per element: MUFU-bound, profiles/r11_tckstar_cfg3_summary.csv) is the
-// limiter, the MMAs take a sixth of that.
+// CTA = 128 candidate rows; it walks all 128-trial tiles.  Candidate planes (128 × Dp, hi and lo) stay in shared memory; trial
+// planes stream through a 4-stage TMA ring one 32-feature slab at a time (SWIZZLE_64B);
+//   warps 0-7  two consumer warpgroups (rows 64·wg …): per (tile, slab) 2 k-steps × 4 products of wgmma m64n128k16 into 64 fp32
+//              registers, then the epilogue on those registers: d² → kernel → fp16 K* plane; μ̃ partials
+//   warp 8     TMA producer
+// The epilogue (~12 instructions and 2 MUFU per element) is the limiter; the MMAs take a fraction of that.
 #include "kbo_internal.cuh"
 #include <type_traits>
 
 #include "tc_common.cuh"
 
 #define KS_BM 128
-#define KS_BN 256
+#define KS_BN 128
 #define KS_BK 32
-#define KS_STAGES 3
-#define KS_EPI_WARPS 16
-#define KS_THREADS (64 + 32 * KS_EPI_WARPS)
+#define KS_STAGES 4
+#define KS_CONSUMERS 256                        // two warpgroups
+#define KS_THREADS (KS_CONSUMERS + 32)
 #define KS_A_PLANE_BYTES (KS_BM * KS_BK * 2)    // 8 KB: one plane of one slab of the candidate tile
-#define KS_B_PLANE_BYTES (KS_BN * KS_BK * 2)    // 16 KB
+#define KS_B_PLANE_BYTES (KS_BN * KS_BK * 2)    // 8 KB
 #define KS_STAGE_BYTES (2 * KS_B_PLANE_BYTES)   // hi + lo
 #define KS_MAX_SLABS 4                          // D <= 128
 
@@ -43,15 +42,9 @@ struct KsSmem {
   uint64_t full[KS_STAGES];
   uint64_t empty[KS_STAGES];
   uint64_t a_full;
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
 };
 
-static size_t ks_smem_bytes(int ns) {
-  return 1024 + (size_t)ns * 2 * KS_A_PLANE_BYTES + (size_t)KS_STAGES * KS_STAGE_BYTES + (size_t)KS_EPI_WARPS * 2 * 512 + 4 * KS_BM * sizeof(double) +
-         256;
-}
+static size_t ks_smem_bytes(int ns) { return 1024 + (size_t)ns * 2 * KS_A_PLANE_BYTES + (size_t)KS_STAGES * KS_STAGE_BYTES + 256; }
 
 __device__ __forceinline__ float ex2_ftz(float x) {
   float r;
@@ -86,39 +79,26 @@ tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant_
   extern __shared__ unsigned char ks_smem_raw[];
   unsigned char* base = (unsigned char*)(((uintptr_t)ks_smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* smA = base;                                            // [ns][hi 8 KB | lo 8 KB]
-  unsigned char* ring = smA + (size_t)ns * 2 * KS_A_PLANE_BYTES;        // [KS_STAGES][hi 16 KB | lo 16 KB]
-  float4* nxs = (float4*)(ring + KS_STAGES * KS_STAGE_BYTES);           // [16 warps][2][32 lanes]
-  double* musum = (double*)(nxs + KS_EPI_WARPS * 2 * 32);               // [4][128]
-  KsSmem* S = (KsSmem*)(musum + 4 * KS_BM);
+  unsigned char* ring = smA + (size_t)ns * 2 * KS_A_PLANE_BYTES;        // [KS_STAGES][hi 8 KB | lo 8 KB]
+  KsSmem* S = (KsSmem*)(ring + KS_STAGES * KS_STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * KS_BM;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == KS_CONSUMERS) {
     prefetch_tmap(&tmCh);
     prefetch_tmap(&tmCl);
     prefetch_tmap(&tmXh);
     prefetch_tmap(&tmXl);
     for (int i = 0; i < KS_STAGES; i++) {
       mbar_init(smem_u32(&S->full[i]), 1);
-      mbar_init(smem_u32(&S->empty[i]), 1);
+      mbar_init(smem_u32(&S->empty[i]), 2);   // one arrive per consumer warpgroup
     }
     mbar_init(smem_u32(&S->a_full), 1);
-    for (int i = 0; i < 2; i++) {
-      mbar_init(smem_u32(&S->tmem_full[i]), 1);
-      mbar_init(smem_u32(&S->tmem_empty[i]), KS_EPI_WARPS);
-    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&S->tmem_base)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = S->tmem_base;
 
-  if (warp == 0) {
+  if (warp == KS_CONSUMERS / 32) {
     // ===================================== TMA producer ===========================================
     if (lane == 0) {
       const uint32_t abar = smem_u32(&S->a_full);
@@ -131,7 +111,7 @@ tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant_
       for (int t = 0; t < ntiles; t++)
         for (int sl = 0; sl < ns; sl++, c++) {
           const uint32_t st = c % KS_STAGES, use = c / KS_STAGES;
-          mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1, 21);
+          mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1);
           const uint32_t bar = smem_u32(&S->full[st]);
           mbar_expect_tx(bar, KS_STAGE_BYTES);
           const uint32_t dst = smem_u32(ring + (size_t)st * KS_STAGE_BYTES);
@@ -140,118 +120,91 @@ tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant_
         }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =============================================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_f16(KS_BM, KS_BN);
-      mbar_wait(smem_u32(&S->a_full), 0, 22);
-      tc_fence_after();
-      uint32_t c = 0;
-      for (int t = 0; t < ntiles; t++) {
-        const uint32_t buf = t & 1;
-        mbar_wait(smem_u32(&S->tmem_empty[buf]), ((t >> 1) & 1) ^ 1, 23);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + buf * KS_BN;
-        for (int sl = 0; sl < ns; sl++, c++) {
-          const uint32_t st = c % KS_STAGES, suse = c / KS_STAGES;
-          mbar_wait(smem_u32(&S->full[st]), suse & 1, 24);
-          tc_fence_after();
-          const uint32_t a_hi = smem_u32(smA + (size_t)sl * 2 * KS_A_PLANE_BYTES), a_lo = a_hi + KS_A_PLANE_BYTES;
-          const uint32_t b_hi = smem_u32(ring + (size_t)st * KS_STAGE_BYTES), b_lo = b_hi + KS_B_PLANE_BYTES;
-          // small products first: the accumulator is still tiny when they are added, so their bits are not truncated away
-#pragma unroll
-          for (int prod = 0; prod < 4; prod++) {
-            const uint32_t a = (prod < 2) ? a_lo : a_hi;
-            const uint32_t b = (prod & 1) ? b_hi : b_lo;   // lo·lo, lo·hi, hi·lo, hi·hi
-#pragma unroll
-            for (int k = 0; k < KS_BK / 16; k++)
-              umma_f16(d_tmem, umma_desc_sw64(a + k * 32), umma_desc_sw64(b + k * 32), idesc, (sl > 0 || prod > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(smem_u32(&S->empty[st]));
-        }
-        umma_commit(smem_u32(&S->tmem_full[buf]));
-      }
-    }
-    __syncwarp();
   } else {
-    // ===================================== epilogue warps =========================================
-    const int ew = warp - 2;
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may access
-    const int cg = ew >> 2;              // which 64 of the tile's 256 trial columns
-    const int row = quarter * 32 + lane;
-    const float ncr = ncand[m0 + row];
-    float4* slot = nxs + (size_t)ew * 2 * 32;
-    __half* out_row = Ksh + (size_t)(m0 + row) * Npad + cg * 64;
-    double mu_d = 0.0;
-    float4 pf = nxal4[(size_t)(cg * 64) / 2 + lane];
+    // ===================================== consumer warpgroups ====================================
+    const int wg = threadIdx.x >> 7, wl = (threadIdx.x >> 5) & 3, q = lane & 3;
+    const int r0 = m0 + wg * 64 + wl * 16 + (lane >> 2), r1 = r0 + 8;
+    const bool signal = (threadIdx.x & 127) == 0;
+    const float nc0 = ncand[r0], nc1 = ncand[r1];
+    __half* out0 = Ksh + (size_t)r0 * Npad;
+    __half* out1 = Ksh + (size_t)r1 * Npad;
+    double mu0 = 0.0, mu1 = 0.0;
+    float acc[64];
+    mbar_wait(smem_u32(&S->a_full), 0);
+    uint32_t c = 0;
     for (int t = 0; t < ntiles; t++) {
-      const uint32_t buf = t & 1;
-      slot[(t & 1) * 32 + lane] = pf;
-      __syncwarp();
-      if (t + 1 < ntiles) pf = nxal4[(size_t)((t + 1) * KS_BN + cg * 64) / 2 + lane];
-      const float4* sl4 = slot + (t & 1) * 32;
-      mbar_wait(smem_u32(&S->tmem_full[buf]), (t >> 1) & 1, 25);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * KS_BN + cg * 64;
-      const int n_base = t * KS_BN + cg * 64;
-      const bool edge = n_base + 64 > N;   // warp-uniform: only the last tile(s) mask trials >= N
-      // EDGE: only the last tile(s) mask trials >= N.  Two instantiations behind one warp-uniform branch: as a runtime flag inside the
-      // body the mask compiled to ISETP + FSEL + IADD per element — 3 of 15 instructions on every tile.
+      int pending = -1;
+      for (int sl = 0; sl < ns; sl++, c++) {
+        const uint32_t st = c % KS_STAGES, use = c / KS_STAGES;
+        mbar_wait(smem_u32(&S->full[st]), use & 1);
+        const uint32_t a_hi = smem_u32(smA + (size_t)sl * 2 * KS_A_PLANE_BYTES) + wg * (KS_A_PLANE_BYTES / 2), a_lo = a_hi + KS_A_PLANE_BYTES;
+        const uint32_t b_hi = smem_u32(ring + (size_t)st * KS_STAGE_BYTES), b_lo = b_hi + KS_B_PLANE_BYTES;
+        wgmma_fence();
+        // small products first: the accumulator is still tiny when they are added, so their bits are not truncated away
+#pragma unroll
+        for (int prod = 0; prod < 4; prod++) {
+          const uint32_t a = (prod < 2) ? a_lo : a_hi;
+          const uint32_t b = (prod & 1) ? b_hi : b_lo;   // lo·lo, lo·hi, hi·lo, hi·hi
+#pragma unroll
+          for (int k = 0; k < KS_BK / 16; k++)
+            wgmma_f16_n128(acc, gmma_desc_sw64(a + k * 32), gmma_desc_sw64(b + k * 32), (sl > 0 || prod > 0 || k > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (pending >= 0 && signal) mbar_arrive(smem_u32(&S->empty[pending]));
+        pending = (int)st;
+      }
+      wgmma_wait<0>();
+      acc_fence(acc);
+      if (signal) mbar_arrive(smem_u32(&S->empty[pending]));   // everything this warpgroup needs is in registers
+      const int n_base = t * KS_BN;
+      const bool store = t < store_tiles;   // a pruning pass contracts a prefix of the trials only: the mean needs every column, the plane does not
+      // EDGE: only the last tile(s) mask trials >= N.  Two instantiations behind one warp-uniform branch keep the mask out of the
+      // per-element code of every other tile.
       auto tile_body = [&](auto edge_tag) {
         constexpr bool EDGE = decltype(edge_tag)::value;
-        uint32_t rr[2][16];
-        tmem_ld16(taddr, rr[0]);
+        float ma0 = 0.f, mb0 = 0.f, ma1 = 0.f, mb1 = 0.f;   // two fp32 chains per row, added in FP64 once per tile
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
-          uint32_t(&r)[16] = rr[q & 1];
-          tmem_ld_wait();
-          if (q < 3) tmem_ld16(taddr + (q + 1) * 16, rr[(q + 1) & 1]);   // the next 16 columns travel while these are evaluated
-          if (q == 3) {   // everything this warp needs from the accumulator is in registers: hand it back to the MMA thread
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&S->tmem_empty[buf]));
+        for (int i = 0; i < KS_BN / 8; i++) {
+          const int n = n_base + 8 * i + 2 * q;
+          const float4 na = (EDGE && n >= N) ? make_float4(0.f, 0.f, 0.f, 0.f) : __ldg(nxal4 + (n >> 1));
+          float k00 = ks_kernel_value<KIND>(acc[4 * i], nc0 + na.x, log2amp);
+          float k01 = ks_kernel_value<KIND>(acc[4 * i + 1], nc0 + na.z, log2amp);
+          float k10 = ks_kernel_value<KIND>(acc[4 * i + 2], nc1 + na.x, log2amp);
+          float k11 = ks_kernel_value<KIND>(acc[4 * i + 3], nc1 + na.z, log2amp);
+          if (EDGE) {
+            k00 = n < N ? k00 : 0.f;
+            k10 = n < N ? k10 : 0.f;
+            k01 = n + 1 < N ? k01 : 0.f;
+            k11 = n + 1 < N ? k11 : 0.f;
           }
-          uint32_t o[8];
-          float macc[4];   // four independent fp32 chains of four trials each, summed in FP64 once per 16 trials
-#pragma unroll
-          for (int g = 0; g < 4; g++) {
-            macc[g] = 0.f;
-#pragma unroll
-            for (int e = 0; e < 4; e += 2) {
-              const int i = g * 4 + e;
-              const float4 na = sl4[(q * 16 + i) >> 1];   // broadcast: every lane reads the same word
-              float k0 = ks_kernel_value<KIND>(__uint_as_float(r[i]), ncr + na.x, log2amp);
-              float k1 = ks_kernel_value<KIND>(__uint_as_float(r[i + 1]), ncr + na.z, log2amp);
-              if (EDGE) {
-                k0 = (n_base + q * 16 + i < N) ? k0 : 0.f;
-                k1 = (n_base + q * 16 + i + 1 < N) ? k1 : 0.f;
-              }
-              macc[g] = fmaf(k0, na.y, macc[g]);
-              macc[g] = fmaf(k1, na.w, macc[g]);
-              const __half2 h2 = __floats2half2_rn(k0, k1);
-              o[i >> 1] = *reinterpret_cast<const uint32_t*>(&h2);
-            }
+          ma0 = fmaf(k00, na.y, ma0);
+          mb0 = fmaf(k01, na.w, mb0);
+          ma1 = fmaf(k10, na.y, ma1);
+          mb1 = fmaf(k11, na.w, mb1);
+          if (store) {
+            *reinterpret_cast<__half2*>(out0 + n) = __floats2half2_rn(k00, k01);
+            *reinterpret_cast<__half2*>(out1 + n) = __floats2half2_rn(k10, k11);
           }
-          mu_d += (double)((macc[0] + macc[1]) + (macc[2] + macc[3]));
-          if (t < store_tiles)   // a pruning pass contracts a prefix of the trials only: the mean needs every column, the plane does not
-            asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(out_row + (size_t)t * KS_BN + q * 16), "r"(o[0]), "r"(o[1]),
-                         "r"(o[2]), "r"(o[3]), "r"(o[4]), "r"(o[5]), "r"(o[6]), "r"(o[7])
-                         : "memory");
         }
+        mu0 += (double)(ma0 + mb0);
+        mu1 += (double)(ma1 + mb1);
       };
-      if (edge)
+      if (n_base + KS_BN > N)
         tile_body(std::true_type{});
       else
         tile_body(std::false_type{});
     }
-    musum[cg * KS_BM + row] = mu_d;
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * KS_EPI_WARPS) : "memory");
-    if (cg == 0) mun[m0 + row] = (float)(((musum[row] + musum[KS_BM + row]) + musum[2 * KS_BM + row]) + musum[3 * KS_BM + row]);
+    // the four lanes of a quad hold the same two rows: fixed-order butterfly
+    mu0 += __shfl_xor_sync(0xffffffffu, mu0, 1);
+    mu1 += __shfl_xor_sync(0xffffffffu, mu1, 1);
+    mu0 += __shfl_xor_sync(0xffffffffu, mu0, 2);
+    mu1 += __shfl_xor_sync(0xffffffffu, mu1, 2);
+    if (q == 0) {
+      mun[r0] = (float)mu0;
+      mun[r1] = (float)mu1;
+    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------------------------

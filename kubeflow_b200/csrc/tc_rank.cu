@@ -1,23 +1,15 @@
-// Ranking pass of the variance contraction with cta_group::2 MMAs (sm_100a: tcgen05 + TMEM + TMA, 2-CTA clusters).
+// Ranking pass of the variance contraction on the Hopper tensor cores (sm_90a: wgmma + TMA + mbarrier).
 //
 //   Σ_j ṽ[m,j]²,   ṽ[m,j] = Σ_{k≤j} K̃*h[m,k]·Wh[j,k]          (hi planes only: ONE fp16 product per term, $SK/_gpr.py:460,:480)
 //
-// The single-CTA MMA of tc_var.cu reads 12 KB of operands from shared memory per 128-cycle MMA while TMA writes the same
-// 12 KB: 192 B/clk against a 128 B/clk shared-memory port — the one-product pass stalled at 60 % of the tensor peak there.
-// Here a CTA PAIR issues M256×N256×K16 MMAs: each CTA feeds its own 128 candidate rows (A) and HALF of the W tile (B), so a
-// CTA moves 8 KB per MMA through shared memory instead of 12, and both TMEM accumulators hold a different j-tile fed by the
-// SAME K* chunk (16 KB of MMA reads + 12 KB of TMA writes per 256 cycles = 112 B/clk).
-//
-// Work item = (256-row group, pair of j-tiles); the K range of a pair is its triangular extent k < 256·(2p+2).  Items are dealt
-// round-robin to the resident clusters in row-group-major order, so the ~74 clusters running at any moment work on the same
-// 4–5 row groups: their K* rows (4 MB per group) and all of W's triangle (68 MB) stay in the 126 MB L2 and each K* byte is read
-// from DRAM once — the single-cluster-per-panel kernel re-streamed the panel from DRAM for every tile pair (8.5×).
-// No intermediate drains: a ranking pass does not care about the ~5e-9/term truncation of TMEM accumulation, so each
-// accumulator is read exactly once per item; accumulator 0 (the shorter K range) is drained while accumulator 1 still
-// receives its last 256 trials, and the next item's first MMAs overlap the drain of accumulator 1.
-//   warp 0      TMA producer (both CTAs; loads land locally, bytes are counted on the leader's barrier)
-//   warp 1      MMA issuer (leader CTA only, one thread), tcgen05.mma.cta_group::2.kind::f16
-//   warps 2-17  epilogue (both CTAs): tcgen05.ld → Σ v² per row → part[pair][row]
+// Work item = (128-row group, pair of 256-column j-tiles); the K range of tile t is its triangular extent k < 256·(t+1).  Items
+// are dealt to persistent CTAs (one per SM) in row-group-major order, so the CTAs running at any moment work on neighbouring
+// row groups: their K* rows and the part of W's triangle in use stay in the 50 MB L2 and each K* byte is read from DRAM about
+// once.  No intermediate drains: a ranking pass does not care about the truncation of long fp32 accumulation chains, so each
+// accumulator is read once per tile.
+//   warps 0-7  two consumer warpgroups: rows 64·wg … 64·wg + 63 of the item, wgmma m64n256k16 into 128 fp32 registers per
+//              thread, then Σ v² per row → part[pair][row]
+//   warp 8     TMA producer (one thread): A (K̃*, 128 × 32) and B (W, 256 × 32) per stage, SWIZZLE_64B, 8-stage ring
 #include "kbo_internal.cuh"
 #include "tc_common.cuh"
 
@@ -25,11 +17,12 @@
 #define RK_BN 256
 #define RK_BK 32
 #define RK_STAGES 8
-#define RK_TILE_BYTES (RK_BM * RK_BK * 2)        // 8 KB: A tile, or this CTA's half of a W tile
-#define RK_STAGE_BYTES (3 * RK_TILE_BYTES)       // A | B0 half | B1 half
-#define RK_EPI_WARPS 16
-#define RK_THREADS (64 + 32 * RK_EPI_WARPS)
-#define RK_SMEM_BYTES (1024 + RK_STAGES * RK_STAGE_BYTES + 2 * 4 * RK_BM * 4 + 256)
+#define RK_A_BYTES (RK_BM * RK_BK * 2)           // 8 KB
+#define RK_B_BYTES (RK_BN * RK_BK * 2)           // 16 KB
+#define RK_STAGE_BYTES (RK_A_BYTES + RK_B_BYTES)
+#define RK_CONSUMERS 256                         // two warpgroups
+#define RK_THREADS (RK_CONSUMERS + 32)
+#define RK_SMEM_BYTES (1024 + RK_STAGES * RK_STAGE_BYTES + 256)
 #define RK_CPT (RK_BN / RK_BK)                   // chunks per 256 trials
 
 namespace {
@@ -38,175 +31,113 @@ using namespace tcx;
 struct RkSmem {
   uint64_t full[RK_STAGES];
   uint64_t empty[RK_STAGES];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
 };
 
 struct RkItem {
-  int rg, p, t0, lim0, nch;
-  bool live1;
+  int rg, p, t0, ntiles;
 };
-// Work item (256-row group rg, tile pair p) and the chunk limits of its two tiles.  The item lists are built on the host
-// (rk_schedule below): every role of both CTAs of a cluster walks the same list sched[off[c] .. off[c+1]).
+// Work item (128-row group rg, tile pair p).  The item lists are built on the host (rk_schedule below): every role of a CTA
+// walks the same list sched[off[c] .. off[c+1]).
 __device__ __forceinline__ RkItem rk_item(int code, int n_jtiles) {
   RkItem w;
   w.rg = code >> 8;
   w.p = code & 255;
   w.t0 = 2 * w.p;
-  w.live1 = w.t0 + 1 < n_jtiles;
-  w.lim0 = (w.t0 + 1) * RK_CPT;
-  w.nch = w.live1 ? (w.t0 + 2) * RK_CPT : w.lim0;
+  w.ntiles = w.t0 + 1 < n_jtiles ? 2 : 1;
   return w;
 }
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(RK_THREADS, 1)
-tc_rank_kernel(const __grid_constant__ CUtensorMap tmA /* K̃* hi plane, box 32 × 128 */, const __grid_constant__ CUtensorMap tmW /* W hi plane, box 32 × 128 */,
-               int n_jtiles, const int* __restrict__ sched /* [n_clusters + 1 offsets | item codes] */, float* __restrict__ part /* [n_pairs][rows] Σ v² over the pair's 512 columns (scaled units) */,
+__global__ void __launch_bounds__(RK_THREADS, 1)
+tc_rank_kernel(const __grid_constant__ CUtensorMap tmA /* K̃* hi plane, box 32 × 128 */, const __grid_constant__ CUtensorMap tmW /* W hi plane, box 32 × 256 */,
+               int n_jtiles, const int* __restrict__ sched /* [n_ctas + 1 offsets | item codes] */, float* __restrict__ part /* [n_pairs][rows] Σ v² over the pair's 512 columns (scaled units) */,
                int64_t rows) {
   extern __shared__ unsigned char rk_smem_raw[];
   unsigned char* ring = (unsigned char*)(((uintptr_t)rk_smem_raw + 1023) & ~(uintptr_t)1023);
-  float* partsum = (float*)(ring + RK_STAGES * RK_STAGE_BYTES);   // [2 item parities][4 column groups][128 rows]
-  RkSmem* S = (RkSmem*)(partsum + 2 * 4 * RK_BM);
+  RkSmem* S = (RkSmem*)(ring + RK_STAGES * RK_STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int cluster_id = blockIdx.x >> 1;
-  const int it_begin = __ldg(sched + cluster_id), it_end = __ldg(sched + cluster_id + 1);
+  const int it_begin = __ldg(sched + blockIdx.x), it_end = __ldg(sched + blockIdx.x + 1);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == RK_CONSUMERS) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmW);
     for (int i = 0; i < RK_STAGES; i++) {
-      mbar_init(smem_u32(&S->full[i]), 1);    // the leader's producer arms it; bytes arrive from both CTAs' loads
-      mbar_init(smem_u32(&S->empty[i]), 1);   // one multicast commit per use
-    }
-    for (int i = 0; i < 2; i++) {
-      mbar_init(smem_u32(&S->tmem_full[i]), 1);
-      mbar_init(smem_u32(&S->tmem_empty[i]), 2 * RK_EPI_WARPS);   // every epilogue warp of both CTAs (used on the leader only)
+      mbar_init(smem_u32(&S->full[i]), 1);    // the producer's expect_tx; the bytes complete the phase
+      mbar_init(smem_u32(&S->empty[i]), 2);   // one arrive per consumer warpgroup
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {   // both CTAs, same warp: 512 columns in each CTA's TMEM = two M256×N256 fp32 accumulators across the pair
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&S->tmem_base)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();   // the peer's barriers exist before any load, commit or arrive targets them
-  tc_fence_after();
-  const uint32_t tmem_base = S->tmem_base;
 
-  if (warp == 0) {
-    // ===================================== TMA producer (both CTAs) ===============================
+  if (warp == RK_CONSUMERS / 32) {
+    // ===================================== TMA producer ==========================================
     if (lane == 0) {
       uint32_t c = 0;
       for (int it = it_begin; it < it_end; it++) {
         const RkItem w = rk_item(__ldg(sched + it), n_jtiles);
-        const int m0 = w.rg * 2 * RK_BM + (int)rank * RK_BM;
-        const int j0 = w.t0 * RK_BN + (int)rank * (RK_BN / 2), j1 = j0 + RK_BN;
-        for (int ch = 0; ch < w.nch; ch++, c++) {
-          const uint32_t st = c % RK_STAGES, use = c / RK_STAGES;
-          mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1, 31);
-          const uint32_t bar = smem_u32(&S->full[st]);
-          const bool b0 = ch < w.lim0;
-          if (rank == 0) mbar_expect_tx(bar, 2u * (RK_TILE_BYTES + (b0 ? RK_TILE_BYTES : 0) + (w.live1 ? RK_TILE_BYTES : 0)));
-          const uint32_t dst = smem_u32(ring + (size_t)st * RK_STAGE_BYTES);
-          const int k0 = ch * RK_BK;
-          tma_load_2d_2sm(dst, &tmA, bar, k0, m0);
-          if (b0) tma_load_2d_2sm(dst + RK_TILE_BYTES, &tmW, bar, k0, j0);
-          if (w.live1) tma_load_2d_2sm(dst + 2 * RK_TILE_BYTES, &tmW, bar, k0, j1);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================================== MMA issuer (leader CTA) ================================
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = umma_idesc_f16(2 * RK_BM, RK_BN);
-      uint32_t c = 0, u0 = 0, u1 = 0;
-      for (int it = it_begin; it < it_end; it++) {
-        const RkItem w = rk_item(__ldg(sched + it), n_jtiles);
-        mbar_wait(smem_u32(&S->tmem_empty[0]), (u0 & 1) ^ 1, 32);
-        u0++;
-        tc_fence_after();
-        for (int ch = 0; ch < w.nch; ch++, c++) {
-          const uint32_t st = c % RK_STAGES, suse = c / RK_STAGES;
-          mbar_wait(smem_u32(&S->full[st]), suse & 1, 34);
-          tc_fence_after();
-          const uint32_t a = smem_u32(ring + (size_t)st * RK_STAGE_BYTES), b0 = a + RK_TILE_BYTES, b1 = a + 2 * RK_TILE_BYTES;
-          if (ch < w.lim0) {
-#pragma unroll
-            for (int k = 0; k < RK_BK / 16; k++)
-              umma_f16_2sm(tmem_base, umma_desc_sw64(a + k * 32), umma_desc_sw64(b0 + k * 32), idesc, (ch > 0 || k > 0) ? 1u : 0u);
+        const int m0 = w.rg * RK_BM;
+        for (int tt = 0; tt < w.ntiles; tt++) {
+          const int t = w.t0 + tt, nch = (t + 1) * RK_CPT;
+          for (int ch = 0; ch < nch; ch++, c++) {
+            const uint32_t st = c % RK_STAGES, use = c / RK_STAGES;
+            mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1);
+            const uint32_t bar = smem_u32(&S->full[st]);
+            mbar_expect_tx(bar, RK_STAGE_BYTES);
+            const uint32_t dst = smem_u32(ring + (size_t)st * RK_STAGE_BYTES);
+            tma_load_2d(dst, &tmA, bar, ch * RK_BK, m0);
+            tma_load_2d(dst + RK_A_BYTES, &tmW, bar, ch * RK_BK, t * RK_BN);
           }
-          if (w.live1) {
-            if (ch == 0) {   // accumulator 1 may still be draining the previous item: its first MMA waits, accumulator 0's are already in flight
-              mbar_wait(smem_u32(&S->tmem_empty[1]), (u1 & 1) ^ 1, 33);
-              u1++;
-              tc_fence_after();
-            }
-#pragma unroll
-            for (int k = 0; k < RK_BK / 16; k++)
-              umma_f16_2sm(tmem_base + RK_BN, umma_desc_sw64(a + k * 32), umma_desc_sw64(b1 + k * 32), idesc, (ch > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit_2sm_mc(smem_u32(&S->empty[st]), (uint16_t)3);   // the stage is free in BOTH CTAs once these MMAs retire
-          if (ch == w.lim0 - 1) umma_commit_2sm_mc(smem_u32(&S->tmem_full[0]), (uint16_t)3);
         }
-        if (w.live1) umma_commit_2sm_mc(smem_u32(&S->tmem_full[1]), (uint16_t)3);
       }
     }
     __syncwarp();
   } else {
-    // ===================================== epilogue warps (both CTAs) =============================
-    const int ew = warp - 2;
-    const int quarter = warp & 3;
-    const int cg = ew >> 2;
-    const int row = quarter * 32 + lane;
-    uint32_t u0 = 0, u1 = 0, nit = 0;
-    for (int it = it_begin; it < it_end; it++, nit++) {
+    // ===================================== consumer warpgroups ===================================
+    const int wg = threadIdx.x >> 7, wl = (threadIdx.x >> 5) & 3;
+    const int row0 = wg * 64 + wl * 16 + (lane >> 2);   // and row0 + 8
+    const bool signal = (threadIdx.x & 127) == 0;
+    float acc[128];
+    uint32_t c = 0;
+    for (int it = it_begin; it < it_end; it++) {
       const RkItem w = rk_item(__ldg(sched + it), n_jtiles);
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;   // rows row0 (s0, s1) and row0 + 8 (s2, s3)
+      for (int tt = 0; tt < w.ntiles; tt++) {
+        const int nch = (w.t0 + tt + 1) * RK_CPT;
+        uint32_t prev = 0;
+        for (int ch = 0; ch < nch; ch++, c++) {
+          const uint32_t st = c % RK_STAGES, use = c / RK_STAGES;
+          mbar_wait(smem_u32(&S->full[st]), use & 1);
+          const uint32_t a = smem_u32(ring + (size_t)st * RK_STAGE_BYTES) + wg * (RK_A_BYTES / 2), b = smem_u32(ring + (size_t)st * RK_STAGE_BYTES) + RK_A_BYTES;
+          wgmma_fence();
 #pragma unroll
-      for (int a = 0; a < 2; a++) {
-        if (a == 1 && !w.live1) break;
-        const uint32_t par = a == 0 ? (u0 & 1) : (u1 & 1);
-        mbar_wait(smem_u32(&S->tmem_full[a]), par, 35 + a);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + a * RK_BN + cg * 64;
+          for (int k = 0; k < RK_BK / 16; k++) wgmma_f16_n256(acc, gmma_desc_sw64(a + k * 32), gmma_desc_sw64(b + k * 32), (ch > 0 || k > 0) ? 1u : 0u);
+          wgmma_commit();
+          wgmma_wait<1>();   // the previous chunk's MMAs are done: its stage may be refilled
+          if (ch > 0 && signal) mbar_arrive(smem_u32(&S->empty[prev]));
+          prev = st;
+        }
+        wgmma_wait<0>();
+        acc_fence(acc);
+        if (signal) mbar_arrive(smem_u32(&S->empty[prev]));
 #pragma unroll
-        for (int q = 0; q < 4; q++) {
-          uint32_t r[16];
-          tmem_ld16(taddr + q * 16, r);
-          tmem_ld_wait();
-          if (q == 3) {   // this warp holds everything it needs of accumulator a: release it to the leader's MMA thread
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_remote(smem_u32(&S->tmem_empty[a]), 0);
-          }
-#pragma unroll
-          for (int i = 0; i < 16; i += 4) {
-            const float v0 = __uint_as_float(r[i]), v1 = __uint_as_float(r[i + 1]), v2 = __uint_as_float(r[i + 2]), v3 = __uint_as_float(r[i + 3]);
-            s0 = fmaf(v0, v0, s0);
-            s1 = fmaf(v1, v1, s1);
-            s2 = fmaf(v2, v2, s2);
-            s3 = fmaf(v3, v3, s3);
-          }
+        for (int i = 0; i < 128; i += 4) {
+          s0 = fmaf(acc[i], acc[i], s0);
+          s1 = fmaf(acc[i + 1], acc[i + 1], s1);
+          s2 = fmaf(acc[i + 2], acc[i + 2], s2);
+          s3 = fmaf(acc[i + 3], acc[i + 3], s3);
         }
       }
-      u0++;
-      if (w.live1) u1++;
-      float* ps = partsum + (nit & 1) * 4 * RK_BM;
-      ps[cg * RK_BM + row] = (s0 + s1) + (s2 + s3);
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * RK_EPI_WARPS) : "memory");
-      if (cg == 0)
-        part[(size_t)w.p * rows + (size_t)w.rg * 2 * RK_BM + rank * RK_BM + row] = ((ps[row] + ps[RK_BM + row]) + ps[2 * RK_BM + row]) + ps[3 * RK_BM + row];
+      float r0 = s0 + s1, r1 = s2 + s3;   // the four lanes of a quad hold the same two rows: fixed-order butterfly
+      r0 += __shfl_xor_sync(0xffffffffu, r0, 1);
+      r1 += __shfl_xor_sync(0xffffffffu, r1, 1);
+      r0 += __shfl_xor_sync(0xffffffffu, r0, 2);
+      r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
+      if ((lane & 3) == 0) {
+        float* out = part + (size_t)w.p * rows + (size_t)w.rg * RK_BM;
+        out[row0] = r0;
+        out[row0 + 8] = r1;
+      }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();   // nobody leaves while the peer may still load into, commit to or arrive on this CTA
-  if (warp == 1) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
 }
 
 __global__ void rank_finish_kernel(const float* __restrict__ part, int p_begin, int p_end, int64_t rows, const double* __restrict__ w_scale, double amp,
@@ -219,43 +150,43 @@ __global__ void rank_finish_kernel(const float* __restrict__ part, int p_begin, 
   var_out[m] = (float)(amp - tot * sc * sc);
 }
 
-// Item lists: items in row-group-major order (largest tile pair of a group first), each dealt to the least-loaded cluster.
-// Loads stay level (≤ 1 % spread on a full chunk), and because they do, the clusters consume the row groups in step: the
-// ~74 items in flight always belong to 4–5 neighbouring row groups, whose K* rows therefore stay in L2.
-int rk_schedule(kbo_handle* h, int n_rg, int n_jtiles, int clusters, int p_begin, int p_end, const int** sched_dev, cudaStream_t s) {
+// Item lists: items in row-group-major order (largest tile pair of a group first), each dealt to the least-loaded CTA.  Loads
+// stay level, and because they do, the CTAs consume the row groups in step: the items in flight always belong to a few
+// neighbouring row groups, whose K* rows therefore stay in L2.
+int rk_schedule(kbo_handle* h, int n_rg, int n_jtiles, int ctas, int p_begin, int p_end, const int** sched_dev, cudaStream_t s) {
   for (auto& e : h->rk_sched)
-    if (e.key[0] == n_rg && e.key[1] == n_jtiles && e.key[2] == clusters && e.key[3] == p_begin && e.key[4] == p_end) {
+    if (e.key[0] == n_rg && e.key[1] == n_jtiles && e.key[2] == ctas && e.key[3] == p_begin && e.key[4] == p_end) {
       *sched_dev = (const int*)e.dev.p;
       return KBO_OK;
     }
   kbo_handle::RkSched& e = h->rk_sched[h->rk_sched_next];
   h->rk_sched_next = (h->rk_sched_next + 1) % 8;
   e.key[0] = -1;
-  std::vector<std::vector<int>> lists(clusters);
-  std::vector<long long> load(clusters, 0);
+  std::vector<std::vector<int>> lists(ctas);
+  std::vector<long long> load(ctas, 0);
   for (int rg = 0; rg < n_rg; rg++)
     for (int p = p_end - 1; p >= p_begin; p--) {
       int best = 0;
-      for (int c = 1; c < clusters; c++)
+      for (int c = 1; c < ctas; c++)
         if (load[c] < load[best]) best = c;
       const bool live1 = 2 * p + 1 < n_jtiles;
       load[best] += (2 * p + 1) * RK_CPT + (live1 ? (2 * p + 2) * RK_CPT : 0) + 3;   // MMA chunk-units + the drain
       lists[best].push_back((rg << 8) | p);
     }
-  e.host.assign(clusters + 1, 0);
-  int off = clusters + 1;
-  for (int c = 0; c < clusters; c++) {
+  e.host.assign(ctas + 1, 0);
+  int off = ctas + 1;
+  for (int c = 0; c < ctas; c++) {
     e.host[c] = off;
     off += (int)lists[c].size();
   }
-  e.host[clusters] = off;
-  for (int c = 0; c < clusters; c++) e.host.insert(e.host.end(), lists[c].begin(), lists[c].end());
+  e.host[ctas] = off;
+  for (int c = 0; c < ctas; c++) e.host.insert(e.host.end(), lists[c].begin(), lists[c].end());
   KBO_TRY(kbo_reserve(h, e.dev, sizeof(int) * e.host.size()));
   // pageable source: the runtime stages it before returning, and earlier launches reading this buffer precede the copy on s
   KBO_CUDA(h, cudaMemcpyAsync(e.dev.p, e.host.data(), sizeof(int) * e.host.size(), cudaMemcpyHostToDevice, s));
   e.key[0] = n_rg;
   e.key[1] = n_jtiles;
-  e.key[2] = clusters;
+  e.key[2] = ctas;
   e.key[3] = p_begin;
   e.key[4] = p_end;
   *sched_dev = (const int*)e.dev.p;
@@ -269,25 +200,25 @@ int rk_schedule(kbo_handle* h, int n_rg, int n_jtiles, int clusters, int p_begin
 // (every (W k*)_j² is non-negative) at the cost of the prefix's share of the triangle: the first eighth of the trials costs 1/64.
 int kbo_i_tc_rank(kbo_handle* h, const __half* Ksh, int64_t rows, const __half* Wh, int Npad, double amp, float* var_n_out, cudaStream_t s,
                   int p_begin, int p_end) {
-  if (rows % (2 * RK_BM) != 0 || Npad % RK_BN != 0) KBO_FAIL(h, KBO_ERR_INVALID, "tc_rank: rows %% 256 and Npad %% 256 must be 0");
+  if (rows % 256 != 0 || Npad % RK_BN != 0) KBO_FAIL(h, KBO_ERR_INVALID, "tc_rank: rows %% 256 and Npad %% 256 must be 0");
   CUtensorMap tmA, tmW;
   KBO_TRY(kbo_i_encode_map_f16(h, &tmA, Ksh, (uint64_t)Npad, (uint64_t)rows, RK_BK, RK_BM));
-  KBO_TRY(kbo_i_encode_map_f16(h, &tmW, Wh, (uint64_t)Npad, (uint64_t)Npad, RK_BK, RK_BM));
+  KBO_TRY(kbo_i_encode_map_f16(h, &tmW, Wh, (uint64_t)Npad, (uint64_t)Npad, RK_BK, RK_BN));
   if (!h->attr_rank) {
     KBO_CUDA(h, cudaFuncSetAttribute(tc_rank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, RK_SMEM_BYTES));
     h->attr_rank = true;
   }
   const int n_jtiles = Npad / RK_BN, n_pairs = (n_jtiles + 1) / 2;
-  const int64_t n_rg = rows / (2 * RK_BM);
+  const int64_t n_rg = rows / RK_BM;
   if (p_end < 0 || p_end > n_pairs) p_end = n_pairs;
   if (p_begin < 0 || p_begin >= p_end) KBO_FAIL(h, KBO_ERR_INVALID, "tc_rank: empty tile-pair range [%d, %d)", p_begin, p_end);
   if (n_pairs > 256 || n_rg >= (1 << 23)) KBO_FAIL(h, KBO_ERR_INVALID, "tc_rank: problem too large for the item encoding (Npad %d, rows %lld)", Npad, (long long)rows);
   KBO_TRY(kbo_reserve(h, h->rk_part, sizeof(float) * (size_t)n_pairs * rows));
-  int clusters = h->sm_count / 2;
-  if ((int64_t)clusters > n_rg * (p_end - p_begin)) clusters = (int)(n_rg * (p_end - p_begin));
+  int ctas = h->sm_count;
+  if ((int64_t)ctas > n_rg * (p_end - p_begin)) ctas = (int)(n_rg * (p_end - p_begin));
   const int* sched = nullptr;
-  KBO_TRY(rk_schedule(h, (int)n_rg, n_jtiles, clusters, p_begin, p_end, &sched, s));
-  tc_rank_kernel<<<(unsigned)(2 * clusters), RK_THREADS, RK_SMEM_BYTES, s>>>(tmA, tmW, n_jtiles, sched, (float*)h->rk_part.p, rows);
+  KBO_TRY(rk_schedule(h, (int)n_rg, n_jtiles, ctas, p_begin, p_end, &sched, s));
+  tc_rank_kernel<<<(unsigned)ctas, RK_THREADS, RK_SMEM_BYTES, s>>>(tmA, tmW, n_jtiles, sched, (float*)h->rk_part.p, rows);
   KBO_LAUNCH_CHECK(h);
   rank_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>((const float*)h->rk_part.p, p_begin, p_end, rows, (const double*)h->scal.p + 6, amp, var_n_out);
   KBO_LAUNCH_CHECK(h);

@@ -1,24 +1,20 @@
-// Variance contraction on the 5th-gen tensor cores (tcgen05 + TMEM + TMA), sm_100a only.
+// Variance contraction on the Hopper tensor cores (wgmma + TMA + mbarrier, 2-CTA clusters), sm_90a.
 //
 //   var_n[m] = amp − Σ_j v[m,j]²,   v[m,j] = Σ_{k≤j} K*[m,k]·W[j,k]      ($SK/_gpr.py:460, :480-481 with W = L⁻¹)
 //
 // This is the M·N² term that sets the suggestion rate (SURVEY.md §8(d)).  Operands are fp16 hi/lo splits
 // (x ≈ hi + lo, |x − hi − lo| ≤ 2⁻²²|x|) and each product is three MMAs  Ah·Bh + Ah·Bl + Al·Bh  into one
-// fp32 TMEM accumulator: bf16/fp16 single-pass moves σ² by 1e-2 and bf16×3 by 1e-5..1e-4 (measured,
-// DESIGN.md §numerics) — fp16×3 stays at ~3e-7.
+// fp32 accumulator: bf16/fp16 single-pass moves σ² by 1e-2 and bf16×3 by 1e-5..1e-4 (DESIGN.md §numerics) — fp16×3
+// stays at ~3e-7.
 //
-// Two kernels share the pipeline below: tc_variance_kernel (one CTA per 128-row panel, all j-tiles) and the default
-// tc_variance_pair_kernel (a 2-CTA cluster per panel, j-tiles split by parity, K* chunks TMA-multicast to both CTAs).
-// CTA = 128 candidate rows (TMEM lanes) × its j-tiles of 256 trial columns, walked in order; for j-tile t only
-// k < 256(t+1) is issued (W is lower triangular).  K is consumed in 32-wide chunks, 4-stage TMA→smem ring:
-//   warp 0     TMA producer (A hi/lo 128×32, B hi/lo 256×32 per stage, SWIZZLE_64B, mbarrier expect_tx)
-//   warp 1     MMA issuer  (single thread, tcgen05.mma.cta_group::1.kind::f16, M=128 N=256 K=16)
-//   warps 2-17 epilogue: TMEM → registers every `k_span` trials (two 256-column TMEM buffers ping-pong) and
-//              accumulate in fp32 registers with round-to-nearest — bounds the length of the in-TMEM
-//              accumulation chain — then Σv² per row at the end of each j-tile.  16 warps (one row × 64 columns
-//              per thread, 4 tcgen05.ld.x16 per drain).  Measured: the per-span cost (~350 cycles) is TMEM read-port
-//              contention between the drains and the MMAs' own accumulator traffic, not epilogue latency (8 vs 16
-//              epilogue warps time the same), so k_span trades accuracy against tensor time directly.
+// One kernel template, two launch shapes: tc_variance_kernel<false> (one CTA per 128-row panel, all j-tiles) and the default
+// tc_variance_kernel<true> (a 2-CTA cluster per panel, j-tiles split by parity, K* chunks TMA-multicast to both CTAs).
+// CTA = 128 candidate rows × its j-tiles of 128 trial columns, walked in order; for j-tile t only k < 128(t+1) is issued (W is
+// lower triangular).  K is consumed in 32-wide chunks through a 6-stage TMA→smem ring:
+//   warps 0-7  two consumer warpgroups (rows 64·wg …): wgmma m64n128k16 into 64 fp32 registers per thread.  Every `k_span`
+//              trials the accumulator is added into a second register array with round-to-nearest — this bounds the length
+//              of the tensor-core accumulation chain — and Σv² per row is taken at the end of each j-tile.
+//   warp 8     TMA producer (A hi/lo 128×32, B hi/lo 128×32 per stage, SWIZZLE_64B, mbarrier expect_tx)
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -26,250 +22,90 @@
 #include "tc_common.cuh"
 
 #define TC_BM 128
-#define TC_BN 256
+#define TC_BN 128
 #define TC_BK 32
-#define TC_STAGES 4
+#define TC_CPT (TC_BN / TC_BK)                // chunks per j-tile of K
+#define TC_STAGES 6
 #define TC_A_BYTES (TC_BM * TC_BK * 2)        // 8 KB per plane
-#define TC_B_BYTES (TC_BN * TC_BK * 2)        // 16 KB per plane
-#define TC_STAGE_BYTES (2 * TC_A_BYTES + 2 * TC_B_BYTES)  // 48 KB
-#define TC_EPI_WARPS 16                       // 4 lane quarters × 4 column groups of 64
-#define TC_THREADS (64 + 32 * TC_EPI_WARPS)
+#define TC_B_BYTES (TC_BN * TC_BK * 2)        // 8 KB per plane
+#define TC_STAGE_BYTES (2 * TC_A_BYTES + 2 * TC_B_BYTES)  // 32 KB
+#define TC_CONSUMERS 256
+#define TC_THREADS (TC_CONSUMERS + 32)
 #define TC_SMEM_BYTES (TC_STAGES * TC_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/)
 
 namespace {
 using namespace tcx;
 
-__device__ __forceinline__ constexpr uint32_t umma_idesc_f16_m128_n256() { return umma_idesc_f16(TC_BM, TC_BN); }
-
 struct TcSmem {
   uint64_t full[TC_STAGES];
   uint64_t empty[TC_STAGES];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
 };
 
+// PAIR: the cluster variant.  The j-tiles are split by parity (CTA r owns tiles 2p + r) and both CTAs walk the K chunks of a
+// tile pair in lockstep, so every A (K*) chunk is fetched ONCE and TMA-multicast into both CTAs' shared memory (each CTA
+// issues the load for its 64-row half with ctaMask = 0b11); B (W) chunks stay private.  That halves the K* panel re-reads.
+//   full[st]  (per CTA): 1 arrival (own producer's expect_tx) + A bytes from both multicast halves + own B bytes
+//   empty[st] (per CTA): one arrival per consumer warpgroup of BOTH CTAs, so a stage is refilled only when both CTAs are done
+// Per-row Σv² of the two CTAs' tile sets goes to part[rank][row]; tc_pair_finish_kernel adds them in a fixed order.
+// nprod 3: Al·Bh + Ah·Bl + Ah·Bh; 1: Ah·Bh only (ranking pass, lo planes never loaded; cluster variant only).
+template <bool PAIR>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_variance_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                    const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, int n_jtiles,
-                   int span_chunks, const double* __restrict__ w_scale /* [0]=2^s, [1]=2^-s */, double amp,
-                   float* __restrict__ var_out, double* __restrict__ sumsq_out /* optional raw Σv² (tests) */) {
+                   int span_chunks, int nprod, const double* __restrict__ w_scale /* [0]=2^s, [1]=2^-s */, double amp,
+                   float* __restrict__ var_out, double* __restrict__ sumsq_out /* optional raw Σv² (tests) */,
+                   double* __restrict__ part /* PAIR: [2][rows] raw Σv² (scaled units) */, int64_t rows) {
   extern __shared__ unsigned char tc_smem_raw[];
   // SWIZZLE_64B tiles need 512 B alignment of each plane; keep the whole ring 1024 B aligned.
   unsigned char* ring = (unsigned char*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
   TcSmem* S = (TcSmem*)(ring + TC_STAGES * TC_STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int m0 = blockIdx.x * TC_BM;
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0;
+  const int m0 = (PAIR ? (blockIdx.x >> 1) : blockIdx.x) * TC_BM;
+  constexpr int STRIDE = PAIR ? 2 : 1;
+  const int n_groups = (n_jtiles + STRIDE - 1) / STRIDE;
+  const uint32_t planes = nprod == 3 ? 2u : 1u;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAh) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAl) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBh) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBl) : "memory");
+  if (threadIdx.x == TC_CONSUMERS) {
+    prefetch_tmap(&tmAh);
+    prefetch_tmap(&tmAl);
+    prefetch_tmap(&tmBh);
+    prefetch_tmap(&tmBl);
     for (int i = 0; i < TC_STAGES; i++) {
       mbar_init(smem_u32(&S->full[i]), 1);
-      mbar_init(smem_u32(&S->empty[i]), 1);
-    }
-    for (int i = 0; i < 2; i++) {
-      mbar_init(smem_u32(&S->tmem_full[i]), 1);
-      mbar_init(smem_u32(&S->tmem_empty[i]), TC_EPI_WARPS);  // one arrive per epilogue warp
+      mbar_init(smem_u32(&S->empty[i]), 2 * STRIDE);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {  // the MMA warp owns the TMEM allocation: all 512 columns = two 128×256 fp32 accumulators
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&S->tmem_base)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = S->tmem_base;
+  if (PAIR) cluster_sync_all();  // the peer's barriers exist before anything is multicast into them
 
-  if (warp == 0) {
+  if (warp == TC_CONSUMERS / 32) {
     // ===================================== TMA producer ===========================================
     if (lane == 0) {
       uint32_t c = 0;
-      for (int jt = 0; jt < n_jtiles; jt++) {
-        const int nch = (jt + 1) * (TC_BN / TC_BK);
+      for (int p = 0; p < n_groups; p++) {
+        const int my_tile = STRIDE * p + (int)rank;
+        const int my_nch = my_tile < n_jtiles ? (my_tile + 1) * TC_CPT : 0;
+        const int nch = PAIR ? min(2 * p + 2, n_jtiles) * TC_CPT : my_nch;  // a pair streams the longer of its two K ranges
         for (int ch = 0; ch < nch; ch++, c++) {
           const uint32_t st = c % TC_STAGES, use = c / TC_STAGES;
-          mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1, 1);
+          if (PAIR)
+            mbar_wait_cluster(smem_u32(&S->empty[st]), (use & 1) ^ 1);
+          else
+            mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1);
           const uint32_t bar = smem_u32(&S->full[st]);
-          mbar_expect_tx(bar, TC_STAGE_BYTES);
-          const uint32_t base = smem_u32(ring + st * TC_STAGE_BYTES);
-          const int k0 = ch * TC_BK;
-          tma_load_2d(base, &tmAh, bar, k0, m0);
-          tma_load_2d(base + TC_A_BYTES, &tmAl, bar, k0, m0);
-          tma_load_2d(base + 2 * TC_A_BYTES, &tmBh, bar, k0, jt * TC_BN);
-          tma_load_2d(base + 2 * TC_A_BYTES + TC_B_BYTES, &tmBl, bar, k0, jt * TC_BN);
-        }
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =============================================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_f16_m128_n256();
-      uint32_t c = 0, span = 0;
-      for (int jt = 0; jt < n_jtiles; jt++) {
-        const int nch = (jt + 1) * (TC_BN / TC_BK);
-        for (int ch0 = 0; ch0 < nch; ch0 += span_chunks, span++) {
-          const uint32_t buf = span & 1, use = span >> 1;
-          mbar_wait(smem_u32(&S->tmem_empty[buf]), (use & 1) ^ 1, 2);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + buf * TC_BN;
-          const int che = min(nch, ch0 + span_chunks);
-          for (int ch = ch0; ch < che; ch++, c++) {
-            const uint32_t st = c % TC_STAGES, suse = c / TC_STAGES;
-            mbar_wait(smem_u32(&S->full[st]), suse & 1, 3);
-            tc_fence_after();
-            const uint32_t base = smem_u32(ring + st * TC_STAGE_BYTES);
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; k++) {
-              const uint32_t koff = k * 32;  // 16 fp16 = 32 B inside the 64 B swizzle row
-              const uint64_t ah = umma_desc_sw64(base + koff);
-              const uint64_t al = umma_desc_sw64(base + TC_A_BYTES + koff);
-              const uint64_t bh = umma_desc_sw64(base + 2 * TC_A_BYTES + koff);
-              const uint64_t bl = umma_desc_sw64(base + 2 * TC_A_BYTES + TC_B_BYTES + koff);
-              umma_f16(d_tmem, al, bh, idesc, (ch > ch0 || k > 0) ? 1u : 0u);  // small terms first
-              umma_f16(d_tmem, ah, bl, idesc, 1u);
-              umma_f16(d_tmem, ah, bh, idesc, 1u);
-            }
-            umma_commit(smem_u32(&S->empty[st]));  // frees the smem stage when these MMAs retire
-          }
-          umma_commit(smem_u32(&S->tmem_full[buf]));  // accumulator span complete → epilogue
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // ===================================== epilogue warps =========================================
-    const int ew = warp - 2;             // 0..15
-    const int quarter = warp & 3;        // TMEM lane quarter this warp may access
-    const int cg = ew >> 2;              // which 64 of the 256 accumulator columns
-    const int row = quarter * 32 + lane; // candidate row within the CTA tile (= TMEM lane)
-    float acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; i++) acc[i] = 0.f;
-    double rowacc = 0.0;
-    uint32_t span = 0;
-    for (int jt = 0; jt < n_jtiles; jt++) {
-      const int nch = (jt + 1) * (TC_BN / TC_BK);
-      for (int ch0 = 0; ch0 < nch; ch0 += span_chunks, span++) {
-        const uint32_t buf = span & 1, use = span >> 1;
-        mbar_wait(smem_u32(&S->tmem_full[buf]), use & 1, 4);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * TC_BN + cg * 64;
-#pragma unroll
-        for (int p = 0; p < 4; p++) {
-          uint32_t r[16];
-          tmem_ld16(taddr + p * 16, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; i++) acc[p * 16 + i] += __uint_as_float(r[i]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&S->tmem_empty[buf]));
-      }
-      // j-tile complete: Σ v² over this thread's 64 columns (4 partial sums, then fp64 across tiles)
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 64; i += 4) {
-        s0 = fmaf(acc[i], acc[i], s0);
-        s1 = fmaf(acc[i + 1], acc[i + 1], s1);
-        s2 = fmaf(acc[i + 2], acc[i + 2], s2);
-        s3 = fmaf(acc[i + 3], acc[i + 3], s3);
-        acc[i] = acc[i + 1] = acc[i + 2] = acc[i + 3] = 0.f;
-      }
-      rowacc += (double)((s0 + s1) + (s2 + s3));
-    }
-    const double sc = w_scale[1];
-    // combine the four column groups through shared memory in a fixed order
-    __shared__ double partsum[4][TC_BM];
-    partsum[cg][row] = rowacc * sc * sc;
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * TC_EPI_WARPS) : "memory");  // the epilogue warps only
-    if (cg == 0) {
-      const double tot = ((partsum[0][row] + partsum[1][row]) + partsum[2][row]) + partsum[3][row];
-      var_out[m0 + row] = (float)(amp - tot);
-      if (sumsq_out) sumsq_out[m0 + row] = tot;
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Cluster variant: TWO CTAs (a 2-CTA cluster, one SM each) share one 128-row candidate panel.  The j-tiles are split by
-// parity (CTA r owns tiles 2p + r) and both CTAs walk the K chunks of a tile pair in lockstep, so every A (K*) chunk is
-// fetched ONCE and TMA-multicast into both CTAs' shared memory (each CTA issues the load for its 64-row half with
-// ctaMask = 0b11); B (W) chunks stay private.  That halves the K* panel re-reads — the kernel's dominant DRAM/L2 traffic.
-//   full[st]  (per CTA): 1 arrival (own producer's expect_tx) + A bytes from both multicast halves + own B bytes
-//   empty[st] (per CTA): 2 arrivals — each CTA's MMA thread commits with .multicast::cluster to BOTH CTAs' barrier, so a
-//             stage is refilled only when both consumers are done with it.
-// Per-row Σv² of the two CTAs' tile sets goes to part[rank][row]; tc_pair_finish_kernel adds them in a fixed order.
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(TC_THREADS, 1)
-tc_variance_pair_kernel(const __grid_constant__ CUtensorMap tmAh64, const __grid_constant__ CUtensorMap tmAl64,
-                        const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, int n_jtiles,
-                        int span_chunks, double* __restrict__ part /* [2][rows] raw Σv² (scaled units) */, int64_t rows,
-                        int nprod /* 3: Al·Bh + Ah·Bl + Ah·Bh; 1: Ah·Bh only (ranking pass, lo planes never loaded) */) {
-  extern __shared__ unsigned char tc_smem_raw[];
-  unsigned char* ring = (unsigned char*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
-  TcSmem* S = (TcSmem*)(ring + TC_STAGES * TC_STAGE_BYTES);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int m0 = (blockIdx.x >> 1) * TC_BM;
-  const int n_pairs = (n_jtiles + 1) >> 1;
-  constexpr int CPT = TC_BN / TC_BK;  // chunks per 256-column block of K
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAh64) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmAl64) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBh) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmBl) : "memory");
-    for (int i = 0; i < TC_STAGES; i++) {
-      mbar_init(smem_u32(&S->full[i]), 1);
-      mbar_init(smem_u32(&S->empty[i]), 2);  // both CTAs' MMA threads release a stage
-    }
-    for (int i = 0; i < 2; i++) {
-      mbar_init(smem_u32(&S->tmem_full[i]), 1);
-      mbar_init(smem_u32(&S->tmem_empty[i]), TC_EPI_WARPS);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(&S->tmem_base)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // the peer's barriers exist before anything is multicast into them
-  tc_fence_after();
-  const uint32_t tmem_base = S->tmem_base;
-
-  if (warp == 0) {
-    // ===================================== TMA producer ===========================================
-    if (lane == 0) {
-      uint32_t c = 0;
-      for (int p = 0; p < n_pairs; p++) {
-        const int my_tile = 2 * p + (int)rank;
-        const int my_nch = my_tile < n_jtiles ? (my_tile + 1) * CPT : 0;
-        const int nch = min(2 * p + 2, n_jtiles) * CPT;  // the pair streams the longer of its two K ranges
-        for (int ch = 0; ch < nch; ch++, c++) {
-          const uint32_t st = c % TC_STAGES, use = c / TC_STAGES;
-          mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1, 11);
-          const uint32_t bar = smem_u32(&S->full[st]);
-          const uint32_t planes = nprod == 3 ? 2u : 1u;
           mbar_expect_tx(bar, planes * TC_A_BYTES + (ch < my_nch ? planes * TC_B_BYTES : 0));
           const uint32_t base = smem_u32(ring + st * TC_STAGE_BYTES);
           const int k0 = ch * TC_BK;
-          const uint32_t half_off = rank * (TC_A_BYTES / 2);  // rows 64·rank … of the 128-row A tile
-          tma_load_2d_mc(base + half_off, &tmAh64, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
-          if (nprod == 3) tma_load_2d_mc(base + TC_A_BYTES + half_off, &tmAl64, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
+          if (PAIR) {
+            const uint32_t half_off = rank * (TC_A_BYTES / 2);  // rows 64·rank … of the 128-row A tile
+            tma_load_2d_mc(base + half_off, &tmAh, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
+            if (nprod == 3) tma_load_2d_mc(base + TC_A_BYTES + half_off, &tmAl, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
+          } else {
+            tma_load_2d(base, &tmAh, bar, k0, m0);
+            if (nprod == 3) tma_load_2d(base + TC_A_BYTES, &tmAl, bar, k0, m0);
+          }
           if (ch < my_nch) {
             tma_load_2d(base + 2 * TC_A_BYTES, &tmBh, bar, k0, my_tile * TC_BN);
             if (nprod == 3) tma_load_2d(base + 2 * TC_A_BYTES + TC_B_BYTES, &tmBl, bar, k0, my_tile * TC_BN);
@@ -278,112 +114,105 @@ tc_variance_pair_kernel(const __grid_constant__ CUtensorMap tmAh64, const __grid
       }
     }
     __syncwarp();
-  } else if (warp == 1) {
-    // ===================================== MMA issuer =============================================
-    if (lane == 0) {
-      const uint32_t idesc = umma_idesc_f16_m128_n256();
-      uint32_t c = 0, span = 0;
-      for (int p = 0; p < n_pairs; p++) {
-        const int my_tile = 2 * p + (int)rank;
-        const int my_nch = my_tile < n_jtiles ? (my_tile + 1) * CPT : 0;
-        const int nch = min(2 * p + 2, n_jtiles) * CPT;
-        for (int ch0 = 0; ch0 < nch; ch0 += span_chunks) {
-          const int che = min(nch, ch0 + span_chunks);
-          const bool live = ch0 < my_nch;  // this span holds MMAs of my tile
-          uint32_t buf = 0, d_tmem = 0;
-          if (live) {
-            buf = span & 1;
-            mbar_wait(smem_u32(&S->tmem_empty[buf]), ((span >> 1) & 1) ^ 1, 12);
-            tc_fence_after();
-            d_tmem = tmem_base + buf * TC_BN;
-          }
-          for (int ch = ch0; ch < che; ch++, c++) {
-            const uint32_t st = c % TC_STAGES, suse = c / TC_STAGES;
-            mbar_wait(smem_u32(&S->full[st]), suse & 1, 13);
-            tc_fence_after();
-            if (ch < my_nch) {
-              const uint32_t base = smem_u32(ring + st * TC_STAGE_BYTES);
+  } else {
+    // ===================================== consumer warpgroups ====================================
+    const int wg = threadIdx.x >> 7, wl = (threadIdx.x >> 5) & 3;
+    const int row0 = wg * 64 + wl * 16 + (lane >> 2);  // and row0 + 8
+    const bool signal = (threadIdx.x & 127) == 0;
+    auto release = [&](uint32_t st) {
+      if (!signal) return;
+      mbar_arrive(smem_u32(&S->empty[st]));
+      if (PAIR) mbar_arrive_remote(smem_u32(&S->empty[st]), rank ^ 1u);
+    };
+    float acc[64], sum[64];
 #pragma unroll
-              for (int k = 0; k < TC_BK / 16; k++) {
-                const uint32_t koff = k * 32;
-                const uint64_t ah = umma_desc_sw64(base + koff);
-                const uint64_t al = umma_desc_sw64(base + TC_A_BYTES + koff);
-                const uint64_t bh = umma_desc_sw64(base + 2 * TC_A_BYTES + koff);
-                const uint64_t bl = umma_desc_sw64(base + 2 * TC_A_BYTES + TC_B_BYTES + koff);
-                if (nprod == 3) {
-                  umma_f16(d_tmem, al, bh, idesc, (ch > ch0 || k > 0) ? 1u : 0u);
-                  umma_f16(d_tmem, ah, bl, idesc, 1u);
-                  umma_f16(d_tmem, ah, bh, idesc, 1u);
-                } else {
-                  umma_f16(d_tmem, ah, bh, idesc, (ch > ch0 || k > 0) ? 1u : 0u);
-                }
+    for (int i = 0; i < 64; i++) sum[i] = 0.f;
+    double rowacc0 = 0.0, rowacc1 = 0.0;
+    uint32_t c = 0;
+    for (int p = 0; p < n_groups; p++) {
+      const int my_tile = STRIDE * p + (int)rank;
+      const int my_nch = my_tile < n_jtiles ? (my_tile + 1) * TC_CPT : 0;
+      const int nch = PAIR ? min(2 * p + 2, n_jtiles) * TC_CPT : my_nch;
+      for (int ch0 = 0; ch0 < nch; ch0 += span_chunks) {
+        const int che = min(nch, ch0 + span_chunks);
+        int pending = -1;   // stage whose MMAs are committed but not yet known complete
+        for (int ch = ch0; ch < che; ch++, c++) {
+          const uint32_t st = c % TC_STAGES, use = c / TC_STAGES;
+          mbar_wait(smem_u32(&S->full[st]), use & 1);
+          if (ch < my_nch) {
+            const uint32_t base = smem_u32(ring + st * TC_STAGE_BYTES);
+            const uint32_t ah = base + wg * (TC_A_BYTES / 2), al = ah + TC_A_BYTES;
+            const uint32_t bh = base + 2 * TC_A_BYTES, bl = bh + TC_B_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < TC_BK / 16; k++) {
+              const uint32_t koff = k * 32;  // 16 fp16 = 32 B inside the 64 B swizzle row
+              const uint32_t first = (ch > ch0 || k > 0) ? 1u : 0u;
+              if (nprod == 3) {
+                wgmma_f16_n128(acc, gmma_desc_sw64(al + koff), gmma_desc_sw64(bh + koff), first);  // small terms first
+                wgmma_f16_n128(acc, gmma_desc_sw64(ah + koff), gmma_desc_sw64(bl + koff), 1u);
+                wgmma_f16_n128(acc, gmma_desc_sw64(ah + koff), gmma_desc_sw64(bh + koff), 1u);
+              } else {
+                wgmma_f16_n128(acc, gmma_desc_sw64(ah + koff), gmma_desc_sw64(bh + koff), first);
               }
             }
-            umma_commit_mc(smem_u32(&S->empty[st]), (uint16_t)3);  // release the stage in BOTH CTAs
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (pending >= 0) release((uint32_t)pending);
+            pending = (int)st;
+          } else {   // the peer's tile needs this chunk, this CTA's does not
+            wgmma_wait<0>();
+            if (pending >= 0) release((uint32_t)pending);
+            pending = -1;
+            release(st);
           }
-          if (live) {
-            umma_commit(smem_u32(&S->tmem_full[buf]));
-            span++;
-          }
+        }
+        if (ch0 < my_nch) {   // this span holds MMAs of my tile: drain the accumulator
+          wgmma_wait<0>();
+          acc_fence(acc);
+          if (pending >= 0) release((uint32_t)pending);
+#pragma unroll
+          for (int i = 0; i < 64; i++) sum[i] += acc[i];
+        }
+      }
+      if (my_nch > 0) {
+        // j-tile complete: Σ v² over this thread's 32 columns of each of its two rows (partial chains, then fp64 across tiles)
+        float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+#pragma unroll
+        for (int i = 0; i < 64; i += 4) {
+          s0 = fmaf(sum[i], sum[i], s0);
+          s1 = fmaf(sum[i + 1], sum[i + 1], s1);
+          s2 = fmaf(sum[i + 2], sum[i + 2], s2);
+          s3 = fmaf(sum[i + 3], sum[i + 3], s3);
+          sum[i] = sum[i + 1] = sum[i + 2] = sum[i + 3] = 0.f;
+        }
+        rowacc0 += (double)(s0 + s1);
+        rowacc1 += (double)(s2 + s3);
+      }
+    }
+    // the four lanes of a quad hold the same two rows: fixed-order butterfly
+    rowacc0 += __shfl_xor_sync(0xffffffffu, rowacc0, 1);
+    rowacc1 += __shfl_xor_sync(0xffffffffu, rowacc1, 1);
+    rowacc0 += __shfl_xor_sync(0xffffffffu, rowacc0, 2);
+    rowacc1 += __shfl_xor_sync(0xffffffffu, rowacc1, 2);
+    if ((lane & 3) == 0) {
+      if (PAIR) {
+        part[(size_t)rank * rows + m0 + row0] = rowacc0;
+        part[(size_t)rank * rows + m0 + row0 + 8] = rowacc1;
+      } else {
+        const double sc = w_scale[1];
+        const double t0 = rowacc0 * sc * sc, t1 = rowacc1 * sc * sc;
+        var_out[m0 + row0] = (float)(amp - t0);
+        var_out[m0 + row0 + 8] = (float)(amp - t1);
+        if (sumsq_out) {
+          sumsq_out[m0 + row0] = t0;
+          sumsq_out[m0 + row0 + 8] = t1;
         }
       }
     }
-    __syncwarp();
-  } else {
-    // ===================================== epilogue warps =========================================
-    const int ew = warp - 2;
-    const int quarter = warp & 3;
-    const int cg = ew >> 2;
-    const int row = quarter * 32 + lane;
-    float acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; i++) acc[i] = 0.f;
-    double rowacc = 0.0;
-    uint32_t span = 0;
-    for (int p = 0; p < n_pairs; p++) {
-      const int my_tile = 2 * p + (int)rank;
-      if (my_tile >= n_jtiles) break;
-      const int my_nch = (my_tile + 1) * CPT;
-      for (int ch0 = 0; ch0 < my_nch; ch0 += span_chunks, span++) {
-        const uint32_t buf = span & 1, use = span >> 1;
-        mbar_wait(smem_u32(&S->tmem_full[buf]), use & 1, 14);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + buf * TC_BN + cg * 64;
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-          uint32_t r[16];
-          tmem_ld16(taddr + q * 16, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 16; i++) acc[q * 16 + i] += __uint_as_float(r[i]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&S->tmem_empty[buf]));
-      }
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-#pragma unroll
-      for (int i = 0; i < 64; i += 4) {
-        s0 = fmaf(acc[i], acc[i], s0);
-        s1 = fmaf(acc[i + 1], acc[i + 1], s1);
-        s2 = fmaf(acc[i + 2], acc[i + 2], s2);
-        s3 = fmaf(acc[i + 3], acc[i + 3], s3);
-        acc[i] = acc[i + 1] = acc[i + 2] = acc[i + 3] = 0.f;
-      }
-      rowacc += (double)((s0 + s1) + (s2 + s3));
-    }
-    __shared__ double partsum[4][TC_BM];
-    partsum[cg][row] = rowacc;
-    asm volatile("bar.sync 1, %0;" ::"n"(32 * TC_EPI_WARPS) : "memory");
-    if (cg == 0) part[(size_t)rank * rows + m0 + row] = ((partsum[0][row] + partsum[1][row]) + partsum[2][row]) + partsum[3][row];
   }
 
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();  // no CTA leaves while its peer may still multicast into it or arrive on its barriers
-  if (warp == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
-  }
+  if (PAIR) cluster_sync_all();  // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
 __global__ void tc_pair_finish_kernel(const double* __restrict__ part, int64_t rows, const double* __restrict__ w_scale, double amp,
@@ -402,39 +231,50 @@ int encode_map(kbo_handle* h, CUtensorMap* out, const void* base, uint64_t inner
 
 int tc_launch(kbo_handle* h, const __half* Ksh, const __half* Ksl, int64_t rows, const __half* Wh, const __half* Wl, int Npad,
               const double* w_scale_dev, double amp, float* var_out, double* sumsq_out, int k_span, cudaStream_t s, int nprod = 3, int jtiles = -1) {
-  const int n_jt = (jtiles > 0 && jtiles < Npad / TC_BN) ? jtiles : Npad / TC_BN;   // a prefix of the trial tiles: an upper bound on the variance
+  // a prefix of the trial tiles (`jtiles` counts 256-column tiles): an upper bound on the variance
+  const int n_jt = (jtiles > 0 && 2 * jtiles < Npad / TC_BN) ? 2 * jtiles : Npad / TC_BN;
   if (nprod != 3 && !h->tc_pair) KBO_FAIL(h, KBO_ERR_STATE, "tc_variance: the one-product ranking pass needs the cluster kernel (kbo_set_tc_pair)");
-  if (rows % TC_BM != 0 || Npad % TC_BN != 0) KBO_FAIL(h, KBO_ERR_INVALID, "tc_variance: rows %% 128 and Npad %% 256 must be 0");
-  // TMEM accumulation rounds toward zero (one-sided error ≈ 5e-9·k_span relative on Σv², profiles/README.md): 128 puts the
-  // truncation at the level of the fp16×3 split error (≈ 5e-7) and costs 8 % of tensor time against never draining.
+  if (rows % TC_BM != 0 || Npad % 256 != 0) KBO_FAIL(h, KBO_ERR_INVALID, "tc_variance: rows %% 128 and Npad %% 256 must be 0");
+  // Long tensor-core accumulation chains lose low-order bits; adding the accumulator into fp32 registers every 128 trials keeps
+  // that error below the fp16×3 split error (≈ 5e-7).
   if (k_span <= 0) k_span = 128;
   int span_chunks = k_span / TC_BK;
   if (span_chunks < 1) span_chunks = 1;
   CUtensorMap tmAh, tmAl, tmBh, tmBl;
-  KBO_TRY(encode_map(h, &tmAh, Ksh, (uint64_t)Npad, (uint64_t)rows, TC_BM));
-  KBO_TRY(encode_map(h, &tmAl, Ksl, (uint64_t)Npad, (uint64_t)rows, TC_BM));
+  const uint32_t a_box = h->tc_pair ? TC_BM / 2 : TC_BM;   // the cluster variant loads (and multicasts) 64-row halves
+  KBO_TRY(encode_map(h, &tmAh, Ksh, (uint64_t)Npad, (uint64_t)rows, a_box));
+  KBO_TRY(encode_map(h, &tmAl, Ksl ? Ksl : Ksh, (uint64_t)Npad, (uint64_t)rows, a_box));
   KBO_TRY(encode_map(h, &tmBh, Wh, (uint64_t)Npad, (uint64_t)Npad, TC_BN));
-  KBO_TRY(encode_map(h, &tmBl, Wl, (uint64_t)Npad, (uint64_t)Npad, TC_BN));
+  KBO_TRY(encode_map(h, &tmBl, Wl ? Wl : Wh, (uint64_t)Npad, (uint64_t)Npad, TC_BN));
   if (!h->attr_tc) {
-    KBO_CUDA(h, cudaFuncSetAttribute(tc_variance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
-    KBO_CUDA(h, cudaFuncSetAttribute(tc_variance_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
+    KBO_CUDA(h, cudaFuncSetAttribute(tc_variance_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
+    KBO_CUDA(h, cudaFuncSetAttribute(tc_variance_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
     h->attr_tc = true;
   }
-  // default: the 2-CTA cluster / TMA-multicast kernel (half the K* panel re-reads); kbo_set_tc_pair(h, 0) selects the single-CTA one
+  // default: the 2-CTA cluster / TMA-multicast variant (half the K* panel re-reads); kbo_set_tc_pair(h, 0) selects the single-CTA one
   if (h->tc_pair) {
-    CUtensorMap tmAh64, tmAl64;
-    KBO_TRY(encode_map(h, &tmAh64, Ksh, (uint64_t)Npad, (uint64_t)rows, 64));
-    KBO_TRY(encode_map(h, &tmAl64, Ksl, (uint64_t)Npad, (uint64_t)rows, 64));
     KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * 2 * (size_t)rows));
-    tc_variance_pair_kernel<<<(unsigned)(2 * (rows / TC_BM)), TC_THREADS, TC_SMEM_BYTES, s>>>(tmAh64, tmAl64, tmBh, tmBl, n_jt, span_chunks,
-                                                                                             (double*)h->part.p, rows, nprod);
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3((unsigned)(2 * (rows / TC_BM)));
+    cfg.blockDim = dim3(TC_THREADS);
+    cfg.dynamicSmemBytes = TC_SMEM_BYTES;
+    cfg.stream = s;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    KBO_CUDA(h, cudaLaunchKernelEx(&cfg, tc_variance_kernel<true>, tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, nprod, w_scale_dev, amp, var_out,
+                                   sumsq_out, (double*)h->part.p, rows));
     KBO_LAUNCH_CHECK(h);
     tc_pair_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>((const double*)h->part.p, rows, w_scale_dev, amp, var_out, sumsq_out);
     KBO_LAUNCH_CHECK(h);
     return KBO_OK;
   }
-  tc_variance_kernel<<<(unsigned)(rows / TC_BM), TC_THREADS, TC_SMEM_BYTES, s>>>(tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, w_scale_dev,
-                                                                                amp, var_out, sumsq_out);
+  tc_variance_kernel<false><<<(unsigned)(rows / TC_BM), TC_THREADS, TC_SMEM_BYTES, s>>>(tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, nprod, w_scale_dev,
+                                                                                       amp, var_out, sumsq_out, nullptr, rows);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }

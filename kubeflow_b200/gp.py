@@ -1,4 +1,4 @@
-"""Host-side GP engine: fixed-θ tell (fit) / ask (sweep + argmax) on one B200 through libkbo's C ABI.
+"""Host-side GP engine: fixed-θ tell (fit) / ask (sweep + argmax) on one H100 through libkbo's C ABI.
 
 Mirrors what Katib's skopt service does per request at fixed θ (SURVEY.md §3.1):
 ``skopt.Optimizer.tell`` -> ``GaussianProcessRegressor.fit`` ($SK/_gpr.py:233-368) and
@@ -37,7 +37,7 @@ class GPEngine:
         if var_mode not in L.VAR_MODES:
             raise ValueError(f"var_mode must be one of {sorted(L.VAR_MODES)}, got {var_mode!r}")
         if not torch.cuda.is_available():
-            raise RuntimeError("kubeflow_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.lib = L.load()
         self.device = int(device)
         self._h = C.c_void_p()
@@ -182,7 +182,7 @@ class GPEngine:
         return float(out.value)
 
     def rank_pass(self, Xc, mode: int, want_plane: bool = False):
-        """Test hook: the ranking pass alone (mode 0: FP64 K* + one-product cluster kernel, 1: tensor-core K* + cta_group::2
+        """Test hook: the ranking pass alone (mode 0: FP64 K* + one-product cluster kernel, 1: tensor-core K* + wgmma
         kernel) -> normalised mean, normalised variance (float32 CUDA tensors) and optionally the fp16 K* hi plane."""
         dev = f"cuda:{self.device}"
         if not isinstance(Xc, torch.Tensor):

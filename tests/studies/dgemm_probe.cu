@@ -1,5 +1,5 @@
 // Throughput of the FP64 tensor-core GEMM building block (csrc/dgemm.cuh) on the shapes the Cholesky uses.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o /tmp/dgemm_probe tests/studies/dgemm_probe.cu && /tmp/dgemm_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o /tmp/dgemm_probe tests/studies/dgemm_probe.cu && /tmp/dgemm_probe
 #include <cstdio>
 #include <vector>
 #include <cuda_runtime.h>

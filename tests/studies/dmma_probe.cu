@@ -1,5 +1,5 @@
 // Peak FP64 tensor-core rate by mma shape (register-resident operands, independent accumulators).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/dmma_probe tests/studies/dmma_probe.cu && /tmp/dmma_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/dmma_probe tests/studies/dmma_probe.cu && /tmp/dmma_probe
 #include <cstdio>
 #include <cuda_runtime.h>
 

@@ -1,5 +1,5 @@
 // Phase timings (SM clocks) of the Cholesky's diagonal-block kernel, one launch on a 64×64 SPD block.
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o /tmp/potf2_probe tests/studies/potf2_probe.cu && /tmp/potf2_probe
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o /tmp/potf2_probe tests/studies/potf2_probe.cu && /tmp/potf2_probe
 #include <cstdio>
 #include <cmath>
 #include <vector>

@@ -2,7 +2,7 @@
 
 CPU emulation of the one-product pass — K* and W = L⁻¹ rounded to fp16 (W scaled as split_w_kernel does), exact accumulation —
 against the fp64 Σv², for a few fits of the workload of record: max |dσ²| over the first 18 944 candidates (what calib_kernel
-sees on a B200: one wave of 148 CTAs × 128 rows) versus the maximum over the whole grid.  Uses the oracle, hence lives under
+sees: one wave of sm_count CTAs × 128 rows) versus the maximum over the whole grid.  Uses the oracle, hence lives under
 tests/.  Output of the run recorded in DESIGN.md (2 min on 8 cores):
 
     N=2048 D=32 matern52: calibration rows 1.024e-03, all 160000 rows 1.141e-03, ratio 1.11

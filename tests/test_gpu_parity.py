@@ -170,7 +170,7 @@ def test_cfg3_full_size_history_candidate_subsample():
 @pytest.mark.parametrize("k_span", [32, 256, 1024, 1 << 20])
 @pytest.mark.parametrize("rows,Npad", [(128, 256), (256, 1024), (384, 2048), (128, 768)])
 def test_tc_variance_kernel_raw(rows, Npad, k_span, pair):
-    """The tcgen05 kernel alone: fp16 hi/lo planes in, Σ_j (Σ_{k<=j} A[m,k]·B[j,k])² out, vs fp64 NumPy on the same planes."""
+    """The wgmma kernel alone: fp16 hi/lo planes in, Σ_j (Σ_{k<=j} A[m,k]·B[j,k])² out, vs fp64 NumPy on the same planes."""
     import ctypes as C
     from kubeflow_b200 import _lib as Lb
     lib = Lb.load()
@@ -626,11 +626,11 @@ def test_rebase_then_append_across_a_256_boundary_in_tc_mode():
     eng.close(); ref.close()
 
 
-# ---- round 2: tensor-core K* generation + cta_group::2 ranking kernel --------------------------------------------------------
+# ---- round 2: tensor-core K* generation + wgmma ranking kernel --------------------------------------------------------
 @pytest.mark.parametrize("N,M,D,kind", [(1000, 700, 7, "matern52"), (2048, 1500, 32, "matern52"), (777, 300, 5, "rbf"), (1300, 513, 100, "matern52"),
                                         (300, 256, 40, "rbf")])
 def test_tensor_core_kstar_plane_and_mean_against_fp64_kernel(N, M, D, kind):
-    """tc_kstar.cu: K̃* from tcgen05 dot products + fp32 kernel evaluation vs the FP64 K* kernel of the same fit.  The fp16 hi
+    """tc_kstar.cu: K̃* from wgmma dot products + fp32 kernel evaluation vs the FP64 K* kernel of the same fit.  The fp16 hi
     planes may differ by one fp16 ulp where the fp32 value falls on the other side of a rounding boundary, nowhere by more;
     padding columns are zero; the on-the-fly mean agrees to the fp32 evaluation error times |alpha|."""
     X, y, Xc = O.synthetic(N, M, D)
@@ -667,7 +667,7 @@ def test_tensor_core_kstar_plane_and_mean_against_fp64_kernel(N, M, D, kind):
 @pytest.mark.parametrize("N,M,D,kind,acq", [(1024, 50000, 8, "rbf", "ei"), (2048, 30000, 32, "matern52", "ei"), (1500, 20000, 6, "matern52", "lcb"),
                                             (1200, 20000, 5, "rbf", "pi"), (1100, 9000, 70, "matern52", "ei")])
 def test_tensor_core_ranking_pass_returns_the_fp64_suggestion(N, M, D, kind, acq):
-    """The product path (prefix-bound pruning pass, tensor-core K*, cta_group::2 ranking kernel, stratified calibration with a
+    """The product path (prefix-bound pruning pass, tensor-core K*, wgmma ranking kernel, stratified calibration with a
     mean bound, FP64 decision) returns the same suggestion as the same path without the pruning pass, the round-1 ranking pass
     (FP64 K*), the three-product sweep and the FP64 engine."""
     X, y, Xc = O.synthetic(N, M, D)

@@ -1,5 +1,5 @@
-"""CPU: the built libkbo.so really contains the sm_100a instructions DESIGN.md claims, kernel by kernel (cuobjdump -sass; no GPU needed).
-A refactor that silently falls back to mma.sync / plain loads, or drops the cta_group::2 path, fails here."""
+"""CPU: the built libkbo.so really contains the sm_90a instructions DESIGN.md claims, kernel by kernel (cuobjdump -sass; no GPU needed).
+A refactor that silently falls back to mma.sync / plain loads, or drops the TMA multicast path, fails here."""
 import re
 import shutil
 import subprocess
@@ -34,24 +34,22 @@ def _ops(sass, needle):
     return [o for ops in hits for o in ops]
 
 
-def test_ranking_kernel_is_cta_group_2_tcgen05_with_tma(sass):
+def test_ranking_kernel_is_wgmma_with_tma(sass):
     ops = _ops(sass, "tc_rank_kernel")
-    assert any(o.startswith("UTCHMMA.2CTA") for o in ops)                 # tcgen05.mma.cta_group::2
-    assert any(o.startswith("UTMALDG") and "2CTA" in o for o in ops)      # cp.async.bulk.tensor ... cta_group::2
-    assert any(o.startswith("UTCBAR") and "MULTICAST" in o for o in ops)  # tcgen05.commit ... multicast::cluster
-    assert any(o.startswith("LDTM") for o in ops)                         # tcgen05.ld
+    assert any(o.startswith("HGMMA.64x256x16.F32") for o in ops)         # wgmma.mma_async m64n256k16, fp32 accumulate
+    assert any(o.startswith("UTMALDG") for o in ops)                      # cp.async.bulk.tensor
+    assert any(o.startswith("SYNCS.PHASECHK") for o in ops)               # mbarrier.try_wait
 
 
-def test_kstar_kernel_is_tcgen05_plus_two_mufu_per_pair(sass):
+def test_kstar_kernel_is_wgmma_plus_two_mufu_per_pair(sass):
     ops = _ops(sass, "tc_kstar_kernelILi1")
-    assert any(o.startswith("UTCHMMA") for o in ops) and any(o.startswith("UTMALDG") for o in ops) and any(o.startswith("LDTM") for o in ops)
+    assert any(o.startswith("HGMMA") for o in ops) and any(o.startswith("UTMALDG") for o in ops)
     assert ops.count("MUFU.SQRT") >= 64 and ops.count("MUFU.EX2") >= 64 and "MUFU.RSQ" not in ops
-    assert any(o.startswith("STG.E.ENL2.256") for o in ops)               # one 32-byte store per thread per 16 columns
 
 
 def test_three_product_kernel_uses_tma_multicast(sass):
-    ops = _ops(sass, "tc_variance_pair_kernel")
-    assert any(o.startswith("UTCHMMA") for o in ops) and any("MULTICAST" in o for o in ops if o.startswith("UTMALDG"))
+    ops = _ops(sass, "tc_variance_kernelILb1")
+    assert any(o.startswith("HGMMA") for o in ops) and any("MULTICAST" in o for o in ops if o.startswith("UTMALDG"))
 
 
 def test_fp64_gemm_runs_on_the_fp64_tensor_cores(sass):

@@ -1,5 +1,5 @@
-"""ncu report -> 'metric,value,unit' summary (one kernel launch) for profiles/, and launch-list shares.
-   python tools/ncu_summary.py rep  gpurun_out/x.ncu-rep  profiles/rN_x_summary.csv
+"""ncu report -> 'metric,value,unit' summary (one kernel launch), and launch-list shares.
+   python tools/ncu_summary.py rep  x.ncu-rep  x_summary.csv
    python tools/ncu_summary.py list gpurun_out/launches.csv            # per-kernel share of the captured launches"""
 import csv, subprocess, sys, collections, io, re
 

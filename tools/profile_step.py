@@ -1,5 +1,4 @@
-"""One warm-up + N timed suggestions at cfg3 through kbo_suggest_host — the command profiled under ncu
-(see profiles/README.md).  Prints the library's own CUDA-event phase timings for the last step."""
+"""One warm-up + N timed suggestions at cfg3 through kbo_suggest_host — the command to run under a profiler.  Prints the library's own CUDA-event phase timings for the last step."""
 import argparse, json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np

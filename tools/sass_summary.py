@@ -1,13 +1,13 @@
-"""cuobjdump -sass of libkbo.so -> per-kernel counts of the tensor-core / TMA / TMEM / FP64-tensor / SFU mnemonics (profiles/rN_sass_summary.txt).
-   python tools/sass_summary.py > profiles/r11_sass_summary.txt"""
+"""cuobjdump -sass of libkbo.so -> per-kernel counts of the tensor-core / TMA / mbarrier / FP64-tensor / SFU mnemonics.
+   python tools/sass_summary.py > sass_summary.txt"""
 import collections, os, re, subprocess, sys
 
 LIB = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "kubeflow_b200", "libkbo.so")
-KEEP = re.compile(r"^(UTC|UTMA|LDTM|STTM|DMMA|DFMA|MUFU|F2FP|STG\.E\.ENL2|SYNCS|UCGABAR|REDUX|SHFL|BAR|LDGSTS|ATOM|RED\.)")
+KEEP = re.compile(r"^(HGMMA|WARPGROUP|UTMA|DMMA|DFMA|MUFU|F2FP|STG\.E\.ENL2|SYNCS|UCGABAR|REDUX|SHFL|BAR|LDGSTS|ATOM|RED\.)")
 txt = subprocess.run(["cuobjdump", "-sass", LIB], capture_output=True, text=True, check=True).stdout
-print("cuobjdump -sass kubeflow_b200/libkbo.so (sm_100a) — instruction counts per kernel, tensor-core / TMA / TMEM / FP64-tensor mnemonics")
-print("(UTCHMMA = tcgen05.mma kind::f16, .2CTA = cta_group::2; UTMALDG = cp.async.bulk.tensor; LDTM = tcgen05.ld; UTCBAR = tcgen05.commit;")
-print(" UTCATOMSWS = tcgen05.alloc/dealloc; DMMA = mma.sync f64; MUFU = SFU)\n")
+print("cuobjdump -sass kubeflow_b200/libkbo.so (sm_90a) — instruction counts per kernel, tensor-core / TMA / mbarrier / FP64-tensor mnemonics")
+print("(HGMMA = wgmma.mma_async; WARPGROUP.ARRIVE / DEPBAR = wgmma.fence / wait_group; UTMALDG = cp.async.bulk.tensor; SYNCS = mbarrier;")
+print(" DMMA = mma.sync f64; MUFU = SFU)\n")
 name, counts, total = None, None, 0
 def flush():
     if name and any(k for k in counts if k.startswith(("UTC", "UTMA", "LDTM", "DMMA", "MUFU", "DFMA"))):
