@@ -3,6 +3,7 @@
 #include <stdlib.h>
 
 #include "kbo_internal.cuh"
+#include "dgemm_sm90.cuh"
 
 static const char* kNoHandle = "kbo: null handle";
 
@@ -356,23 +357,36 @@ int kbo_acq_argmax(kbo_handle* h, const float* mu_n, const float* var_n, int64_t
                               (cudaStream_t)stream);
 }
 
-// Test hook (not in kbo.h): the FP64 tensor-core rate of this GPU — DMMA m8n8k4 on register-resident operands, 8 independent
-// accumulator tiles per warp, 8 warps per CTA, one CTA per SM — the denominator bench.py's fit roofline uses (there is no FP64 entry
-// in MEASURED_PEAKS.json).  Same loop as tests/studies/dmma_probe.cu.
+}  // extern "C"
+
+// Test hook (not in kbo.h): the FP64 tensor-core rate of this GPU — DMMA on register-resident operands, 8 independent accumulator
+// tiles per warp, 8 warps per CTA, one CTA per SM — the denominator bench.py's fit roofline uses (there is no FP64 entry in
+// MEASURED_PEAKS.json).  Both shapes the FP64 GEMMs issue are timed and the faster is reported: on an H100 m8n8k4 reaches half the
+// rate of m16n8k8, which the fit's GEMMs (dgemm_sm90.cuh) use.  Same loops as tests/studies/dmma_probe.cu.
+template <bool K8>
 __global__ void __launch_bounds__(256) fp64_peak_kernel(double* out, int iters) {
-  double a = threadIdx.x * 1e-3, b = threadIdx.x * 1e-4 + 1.0, c[8][2];
+  double a[4], b[2], c[8][4];
 #pragma unroll
-  for (int j = 0; j < 8; j++) c[j][0] = c[j][1] = 0.0;
+  for (int i = 0; i < 4; i++) a[i] = threadIdx.x * 1e-3 + i;
+#pragma unroll
+  for (int i = 0; i < 2; i++) b[i] = threadIdx.x * 1e-4 + 1.0 + i;
+#pragma unroll
+  for (int j = 0; j < 8; j++) c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.0;
   for (int it = 0; it < iters; it++) {
 #pragma unroll
-    for (int j = 0; j < 8; j++)
-      asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c[j][0]), "+d"(c[j][1]) : "d"(a), "d"(b));
+    for (int j = 0; j < 8; j++) {
+      if (K8)
+        dmma_m16n8k8(c[j], a, b);
+      else
+        asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c[j][0]), "+d"(c[j][1]) : "d"(a[0]), "d"(b[0]));
+    }
   }
   double s = 0.0;
 #pragma unroll
-  for (int j = 0; j < 8; j++) s += c[j][0] + c[j][1];
+  for (int j = 0; j < 8; j++) s += c[j][0] + c[j][1] + c[j][2] + c[j][3];
   out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
+extern "C" {
 int kbo_debug_fp64_peak(kbo_handle* h, double* tflops_out) {
   if (!h || !tflops_out) return KBO_ERR_INVALID;
   cudaSetDevice(h->device);
@@ -382,21 +396,47 @@ int kbo_debug_fp64_peak(kbo_handle* h, double* tflops_out) {
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
-  float best = 1e30f;
-  for (int rep = 0; rep < 4; rep++) {
-    cudaEventRecord(e0, 0);
-    fp64_peak_kernel<<<ctas, 256>>>(out, iters);
-    cudaEventRecord(e1, 0);
-    cudaEventSynchronize(e1);
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    if (rep > 0 && ms < best) best = ms;
+  double peak = 0.0;
+  for (int k8 = 0; k8 < 2; k8++) {
+    const int its = k8 ? iters / 2 : iters;   // one m16n8k8 is four m8n8k4s of work: half the iterations, twice the time at twice the rate
+    float best = 1e30f;
+    for (int rep = 0; rep < 4; rep++) {
+      cudaEventRecord(e0, 0);
+      if (k8)
+        fp64_peak_kernel<true><<<ctas, 256>>>(out, its);
+      else
+        fp64_peak_kernel<false><<<ctas, 256>>>(out, its);
+      cudaEventRecord(e1, 0);
+      cudaEventSynchronize(e1);
+      float ms = 0.f;
+      cudaEventElapsedTime(&ms, e0, e1);
+      if (rep > 0 && ms < best) best = ms;
+    }
+    const double flop_per_mma = k8 ? 2.0 * 16 * 8 * 8 : 2.0 * 8 * 8 * 4;
+    peak = fmax(peak, flop_per_mma * 8.0 * its * 8 * ctas / (best * 1e-3) * 1e-12);
   }
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   cudaFree(out);
   KBO_CUDA(h, cudaGetLastError());
-  *tflops_out = 2.0 * 8 * 8 * 4 * 8.0 * iters * 8 * ctas / (best * 1e-3) * 1e-12;
+  *tflops_out = peak;
+  return KBO_OK;
+}
+
+// Test hook (not in kbo.h): one dgemm_sm90_kernel launch on caller-owned device buffers (row-major; transb = 1: B is N×K, C = A·Bᵀ;
+// 0: B is K×N), on the given stream.  For the tests that check the fit's FP64 GEMM against a host product.
+int kbo_debug_dgemm_sm90(kbo_handle* h, int32_t transb, int32_t M, int32_t N, int32_t K, const double* A, int32_t lda, const double* B, int32_t ldb,
+                         double* C, int32_t ldc, double alpha, double beta, int32_t kmode, int32_t kbegin, int32_t tileskip, void* stream) {
+  if (!h) return KBO_ERR_INVALID;
+  if (!A || !B || !C || M < 1 || N < 1 || K < 0 || lda < K || ldb < (transb ? K : N) || ldc < N || kmode < KM_FULL || kmode > KM_FROM_M ||
+      (tileskip != TS_NONE && tileskip != TS_LOWER))
+    KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_dgemm_sm90: bad argument");
+  cudaSetDevice(h->device);
+  if (transb)
+    dgemm_sm90_launch<true>((cudaStream_t)stream, M, N, K, A, lda, B, ldb, C, ldc, alpha, beta, kmode, kbegin, tileskip);
+  else
+    dgemm_sm90_launch<false>((cudaStream_t)stream, M, N, K, A, lda, B, ldb, C, ldc, alpha, beta, kmode, kbegin, tileskip);
+  KBO_CUDA(h, cudaGetLastError());
   return KBO_OK;
 }
 

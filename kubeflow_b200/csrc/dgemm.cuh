@@ -1,7 +1,7 @@
 // FP64 GEMM building block on the FP64 tensor cores (DMMA m8n8k4).
 // C[M×N] = alpha · A[M×K] · op(B) + beta · C, with per-tile K-range clipping for triangular operands.
-// Used by the blocked Cholesky (syrk trailing update), the triangular inverse and the FP64
-// (checker-precision) variance contraction.
+// Used by the FP64 (checker-precision) variance contraction, the LML gradient and CMA-ES; the fit's GEMMs use the m16n8k8 kernel
+// of dgemm_sm90.cuh, which shares this file's tile constants and K-range modes.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -27,8 +27,8 @@ enum { TS_NONE = 0, TS_LOWER = 1 };
 
 // FP64 tensor-core MMA (DMMA), warp-level: D(8×8) += A(8×4)·B(4×8).  Fragments (lane = 4g + t): a = A[g][t], b = B[t][g],
 // c/d = C[g][2t], C[g][2t+1].  DMMA and plain DFMA peak rates: tests/studies/dmma_probe.cu; the point of
-// the tensor form is that one fragment load feeds 256 FMAs, so the FP64 GEMM-shaped work (potrf / trtri updates, FP64 variance
-// contraction, CMA-ES products) is not bound by shared-memory loads.
+// the tensor form is that one fragment load feeds 256 FMAs, so the FP64 GEMM-shaped work (FP64 variance contraction, LML
+// gradient, CMA-ES products) is not bound by shared-memory loads.
 __device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
 }

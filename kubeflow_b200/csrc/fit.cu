@@ -7,7 +7,7 @@
 #include <stdlib.h>
 
 #include "kbo_internal.cuh"
-#include "dgemm.cuh"
+#include "dgemm_sm90.cuh"
 #include "ktab.cuh"
 
 // ------------------------------------------------------------------------------------------------
@@ -249,7 +249,7 @@ static int potrf_impl(kbo_handle* h, double* A, int N, int lda, int* info_dev, c
         const int cin = K0 + W - (k + jb);  // columns of the outer panel still to be factorised
         if (cin > 0) {
           double* C = A + (size_t)(k + jb) * lda + (k + jb);
-          dgemm64_launch<true, EPI_STORE>(s, rows, cin, jb, P, lda, P, lda, C, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
+          dgemm_sm90_launch<true>(s, rows, cin, jb, P, lda, P, lda, C, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
           KBO_LAUNCH_CHECK(h);
         }
       }
@@ -259,7 +259,7 @@ static int potrf_impl(kbo_handle* h, double* A, int N, int lda, int* info_dev, c
     if (rows_t > 0) {
       const double* Pp = A + (size_t)(K0 + W) * lda + K0;  // rows below the panel × the panel's W columns
       double* C = A + (size_t)(K0 + W) * lda + (K0 + W);
-      dgemm64_launch<true, EPI_STORE>(s, rows_t, rows_t, W, Pp, lda, Pp, lda, C, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
+      dgemm_sm90_launch<true>(s, rows_t, rows_t, W, Pp, lda, Pp, lda, C, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
       KBO_LAUNCH_CHECK(h);
     }
   }
@@ -284,12 +284,12 @@ int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int l
     const long long sL = 2 * b * (long long)ldl + 2 * b, sW = 2 * b * (long long)ldw + 2 * b;
     if (full > 0) {
       // T21 = L21 · W11   (W11 lower-triangular: k >= n)
-      dgemm64_launch<false, EPI_STORE>(s, (int)b, (int)b, (int)b, L + b * ldl, ldl, W, ldw, T + b * ldw, ldw, 1.0, 0.0, KM_FROM_N, 0,
-                                       TS_NONE, full, sL, sW, sW);
+      dgemm_sm90_launch<false>(s, (int)b, (int)b, (int)b, L + b * ldl, ldl, W, ldw, T + b * ldw, ldw, 1.0, 0.0, KM_FROM_N, 0,
+                               TS_NONE, full, sL, sW, sW);
       KBO_LAUNCH_CHECK(h);
       // W21 = −W22 · T21  (W22 lower-triangular: k <= m)
-      dgemm64_launch<false, EPI_STORE>(s, (int)b, (int)b, (int)b, W + b * ldw + b, ldw, T + b * ldw, ldw, W + b * ldw, ldw, -1.0, 0.0,
-                                       KM_UPTO_M, 0, TS_NONE, full, sW, sW, sW);
+      dgemm_sm90_launch<false>(s, (int)b, (int)b, (int)b, W + b * ldw + b, ldw, T + b * ldw, ldw, W + b * ldw, ldw, -1.0, 0.0,
+                               KM_UPTO_M, 0, TS_NONE, full, sW, sW, sW);
       KBO_LAUNCH_CHECK(h);
     }
     const long long r0 = (long long)full * 2 * b;
@@ -300,9 +300,9 @@ int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int l
       double* T21 = T + (r0 + b) * ldw + r0;
       double* W21 = W + (r0 + b) * ldw + r0;
       const double* W22 = W + (r0 + b) * ldw + (r0 + b);
-      dgemm64_launch<false, EPI_STORE>(s, rows2, (int)b, (int)b, L21, ldl, W11, ldw, T21, ldw, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
+      dgemm_sm90_launch<false>(s, rows2, (int)b, (int)b, L21, ldl, W11, ldw, T21, ldw, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
       KBO_LAUNCH_CHECK(h);
-      dgemm64_launch<false, EPI_STORE>(s, rows2, (int)b, rows2, W22, ldw, T21, ldw, W21, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+      dgemm_sm90_launch<false>(s, rows2, (int)b, rows2, W22, ldw, T21, ldw, W21, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
       KBO_LAUNCH_CHECK(h);
     }
   }
@@ -404,8 +404,8 @@ static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double
           double* Pn = A + (size_t)(k + jb) * lda + k;
           trsm_panel_kernel<<<(rows_in + 63) / 64, 256, smem, shi>>>(Pn, lda, rows_in, jb, Linv, info_dev);
           KBO_LAUNCH_CHECK(h);
-          dgemm64_launch<true, EPI_STORE>(shi, rows_in, rows_in, jb, Pn, lda, Pn, lda, A + (size_t)(k + jb) * lda + (k + jb), lda, -1.0, 1.0, KM_FULL, 0,
-                                          TS_LOWER);
+          dgemm_sm90_launch<true>(shi, rows_in, rows_in, jb, Pn, lda, Pn, lda, A + (size_t)(k + jb) * lda + (k + jb), lda, -1.0, 1.0, KM_FULL, 0,
+                                  TS_LOWER);
           KBO_LAUNCH_CHECK(h);
         }
       }
@@ -418,11 +418,11 @@ static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double
         for (int r0 = 0; r0 + b < Wd; r0 += 2 * b) {
           const int rows2 = min(b, Wd - (r0 + b));
           double* T21 = T + (size_t)(K0 + r0 + b) * ldw + K0 + r0;
-          dgemm64_launch<false, EPI_STORE>(shi, rows2, b, b, Lpp + (size_t)(r0 + b) * lda + r0, lda, Wpp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
-                                           KM_FROM_N, 0, TS_NONE);
+          dgemm_sm90_launch<false>(shi, rows2, b, b, Lpp + (size_t)(r0 + b) * lda + r0, lda, Wpp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
+                                   KM_FROM_N, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
-          dgemm64_launch<false, EPI_STORE>(shi, rows2, b, rows2, Wpp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
-                                           Wpp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+          dgemm_sm90_launch<false>(shi, rows2, b, rows2, Wpp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
+                                   Wpp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
         }
       mark();
@@ -430,7 +430,7 @@ static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double
       const int rows_t = N - (K0 + Wd);
       if (rows_t > 0) {
         double* Pp = A + (size_t)(K0 + Wd) * lda + K0;
-        dgemm64_launch<true, EPI_STORE>(shi, rows_t, Wd, Wd, Pp, lda, Wpp, ldw, T2, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
+        dgemm_sm90_launch<true>(shi, rows_t, Wd, Wd, Pp, lda, Wpp, ldw, T2, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
         KBO_LAUNCH_CHECK(h);
         KBO_CUDA(h, cudaMemcpy2DAsync(Pp, sizeof(double) * lda, T2, sizeof(double) * OW, sizeof(double) * Wd, rows_t, cudaMemcpyDeviceToDevice, shi));
       }
@@ -441,14 +441,14 @@ static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double
         KBO_CUDA(h, cudaStreamWaitEvent(supd, ev_solve[P], 0));
         const double* Pp = A + (size_t)(K0 + Wd) * lda + K0;
         const int nb = min(OW, rows_t);
-        dgemm64_launch<true, EPI_STORE>(supd, rows_t, nb, Wd, Pp, lda, Pp, lda, A + (size_t)(K0 + Wd) * lda + (K0 + Wd), lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
+        dgemm_sm90_launch<true>(supd, rows_t, nb, Wd, Pp, lda, Pp, lda, A + (size_t)(K0 + Wd) * lda + (K0 + Wd), lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
         KBO_LAUNCH_CHECK(h);
         KBO_CUDA(h, cudaEventRecord(ev_col[P + 1], supd));
         const int rows_r = rows_t - nb;
         if (rows_r > 0) {
           const double* Pr = Pp + (size_t)nb * lda;
-          dgemm64_launch<true, EPI_STORE>(supd, rows_r, rows_r, Wd, Pr, lda, Pr, lda, A + (size_t)(K0 + Wd + nb) * lda + (K0 + Wd + nb), lda, -1.0, 1.0,
-                                          KM_FULL, 0, TS_LOWER);
+          dgemm_sm90_launch<true>(supd, rows_r, rows_r, Wd, Pr, lda, Pr, lda, A + (size_t)(K0 + Wd + nb) * lda + (K0 + Wd + nb), lda, -1.0, 1.0,
+                                  KM_FULL, 0, TS_LOWER);
           KBO_LAUNCH_CHECK(h);
         }
       }
@@ -464,18 +464,18 @@ static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double
           for (int r0 = 0; r0 + b < Pw; r0 += 2 * b) {
             const int rows2 = min(b, Pw - (r0 + b));
             double* T21 = T + (size_t)(P0 + r0 + b) * ldw + P0 + r0;
-            dgemm64_launch<false, EPI_STORE>(sinv, rows2, b, b, Lrp + (size_t)(r0 + b) * lda + r0, lda, Wrp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
-                                             KM_FROM_N, 0, TS_NONE);
+            dgemm_sm90_launch<false>(sinv, rows2, b, b, Lrp + (size_t)(r0 + b) * lda + r0, lda, Wrp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
+                                     KM_FROM_N, 0, TS_NONE);
             KBO_LAUNCH_CHECK(h);
-            dgemm64_launch<false, EPI_STORE>(sinv, rows2, b, rows2, Wrp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
-                                             Wrp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+            dgemm_sm90_launch<false>(sinv, rows2, b, rows2, Wrp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
+                                     Wrp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
             KBO_LAUNCH_CHECK(h);
           }
         if (P0 > 0) {
           double* Trow = T + (size_t)P0 * ldw;
-          dgemm64_launch<false, EPI_STORE>(sinv, Pw, P0, P0, A + (size_t)P0 * lda, lda, W, ldw, Trow, ldw, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
+          dgemm_sm90_launch<false>(sinv, Pw, P0, P0, A + (size_t)P0 * lda, lda, W, ldw, Trow, ldw, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
-          dgemm64_launch<false, EPI_STORE>(sinv, Pw, P0, Pw, Wrp, ldw, Trow, ldw, W + (size_t)P0 * ldw, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+          dgemm_sm90_launch<false>(sinv, Pw, P0, Pw, Wrp, ldw, Trow, ldw, W + (size_t)P0 * ldw, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
         }
       }
@@ -761,8 +761,8 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           trsm_panel_kernel<<<(rows_in + 63) / 64, 256, smem, sc>>>(Pn, lda, rows_in, jb, Li, info_dev);
           KBO_LAUNCH_CHECK(h);
           KBO_CUDA(h, cudaEventRecord(ev_tr[b], sc));
-          dgemm64_launch<true, EPI_STORE>(sc, rows_in, rows_in, jb, Pn, lda, Pn, lda, A + (size_t)(k + jb) * lda + (k + jb), lda, -1.0, 1.0, KM_FULL, 0,
-                                          TS_LOWER);
+          dgemm_sm90_launch<true>(sc, rows_in, rows_in, jb, Pn, lda, Pn, lda, A + (size_t)(k + jb) * lda + (k + jb), lda, -1.0, 1.0, KM_FULL, 0,
+                                  TS_LOWER);
           KBO_LAUNCH_CHECK(h);
         }
       }
@@ -778,11 +778,11 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           if (r0 + bsz >= Wd) return KBO_OK;
           const int rows2 = min(bsz, Wd - (r0 + bsz));
           double* T21 = T + (size_t)(K0 + r0 + bsz) * ldw + K0 + r0;
-          dgemm64_launch<false, EPI_STORE>(sw, rows2, bsz, bsz, Lpp + (size_t)(r0 + bsz) * lda + r0, lda, Wpp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
-                                           KM_FROM_N, 0, TS_NONE);
+          dgemm_sm90_launch<false>(sw, rows2, bsz, bsz, Lpp + (size_t)(r0 + bsz) * lda + r0, lda, Wpp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
+                                   KM_FROM_N, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
-          dgemm64_launch<false, EPI_STORE>(sw, rows2, bsz, rows2, Wpp + (size_t)(r0 + bsz) * ldw + r0 + bsz, ldw, T21, ldw,
-                                           Wpp + (size_t)(r0 + bsz) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+          dgemm_sm90_launch<false>(sw, rows2, bsz, rows2, Wpp + (size_t)(r0 + bsz) * ldw + r0 + bsz, ldw, T21, ldw,
+                                   Wpp + (size_t)(r0 + bsz) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
           return KBO_OK;
         };
@@ -816,7 +816,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
             const int ncols = K0 + Wd - (k + jb);   // the panel's columns right of this block
             if (ncols > 0) {
               KBO_CUDA(h, cudaStreamWaitEvent(st, ev_tr[b], 0));   // L of the diagonal block's rows in this column block (the chain's trsm)
-              dgemm64_launch<true, EPI_STORE>(st, nrows, ncols, jb, Xb, lda, A + (size_t)(k + jb) * lda + k, lda, Xb + jb, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
+              dgemm_sm90_launch<true>(st, nrows, ncols, jb, Xb, lda, A + (size_t)(k + jb) * lda + k, lda, Xb + jb, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
               KBO_LAUNCH_CHECK(h);
             }
           }
@@ -838,7 +838,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
         if (P == 0 && e_early) KBO_CUDA(h, cudaStreamWaitEvent(sn, e_start, 0));   // that block is not in the first column block
         if (cudaEvent_t pe = midmode ? (P > 0 ? ev_t2[P - 1] : nullptr) : pred1) KBO_CUDA(h, cudaStreamWaitEvent(sn, pe, 0));
         const double* Ln = A + (size_t)rn * lda + K0;
-        dgemm64_launch<true, EPI_STORE>(sn, n_near, n_near, Wd, Ln, lda, Ln, lda, A + (size_t)rn * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
+        dgemm_sm90_launch<true>(sn, n_near, n_near, Wd, Ln, lda, Ln, lda, A + (size_t)rn * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
         KBO_LAUNCH_CHECK(h);
         KBO_CUDA(h, cudaEventRecord(ev_near[P + 1], sn));
         tmark(sn, "next diagonal block updated", P);
@@ -848,17 +848,17 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           double* T2m = T2 + (size_t)(N - OW) * OW;   // the far GEMM uses at most the first N − 3·256 rows of T2
           if (P > 0) KBO_CUDA(h, cudaStreamWaitEvent(sm, ev_col[P], 0));
           KBO_CUDA(h, cudaStreamWaitEvent(sm, ev_wpp[P], 0));
-          dgemm64_launch<true, EPI_STORE>(sm, n_mid, Wd, Wd, Lm, lda, W + (size_t)K0 * ldw + K0, ldw, T2m, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
+          dgemm_sm90_launch<true>(sm, n_mid, Wd, Wd, Lm, lda, W + (size_t)K0 * ldw + K0, ldw, T2m, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
           KBO_CUDA(h, cudaMemcpy2DAsync((double*)Lm, sizeof(double) * lda, T2m, sizeof(double) * OW, sizeof(double) * Wd, n_mid, cudaMemcpyDeviceToDevice, sm));
           KBO_CUDA(h, cudaEventRecord(ev_mid[P], sm));
           KBO_CUDA(h, cudaStreamWaitEvent(sm, ev_nsolve[P], 0));
           if (pred1) KBO_CUDA(h, cudaStreamWaitEvent(sm, pred1, 0));
-          dgemm64_launch<true, EPI_STORE>(sm, n_mid, n_near, Wd, Lm, lda, Ln, lda, A + (size_t)rm * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
+          dgemm_sm90_launch<true>(sm, n_mid, n_near, Wd, Lm, lda, Ln, lda, A + (size_t)rm * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
           KBO_CUDA(h, cudaEventRecord(ev_t1[P], sm));
           if (cudaEvent_t pe = pred_of(2)) KBO_CUDA(h, cudaStreamWaitEvent(sm, pe, 0));
-          dgemm64_launch<true, EPI_STORE>(sm, n_mid, n_mid, Wd, Lm, lda, Lm, lda, A + (size_t)rm * lda + rm, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
+          dgemm_sm90_launch<true>(sm, n_mid, n_mid, Wd, Lm, lda, Lm, lda, A + (size_t)rm * lda + rm, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
           KBO_LAUNCH_CHECK(h);
           KBO_CUDA(h, cudaEventRecord(ev_t2[P], sm));
           tmark(sm, "mid rows solved, their two updates done", P);
@@ -870,7 +870,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           if (P > 0) KBO_CUDA(h, cudaStreamWaitEvent(ss, ev_col[P], 0));
           KBO_CUDA(h, cudaStreamWaitEvent(ss, ev_wpp[P], 0));
           double* Pf = A + (size_t)rf * lda + K0;
-          dgemm64_launch<true, EPI_STORE>(ss, n_far, Wd, Wd, Pf, lda, W + (size_t)K0 * ldw + K0, ldw, T2, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
+          dgemm_sm90_launch<true>(ss, n_far, Wd, Wd, Pf, lda, W + (size_t)K0 * ldw + K0, ldw, T2, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
           KBO_CUDA(h, cudaMemcpy2DAsync(Pf, sizeof(double) * lda, T2, sizeof(double) * OW, sizeof(double) * Wd, n_far, cudaMemcpyDeviceToDevice, ss));
           KBO_CUDA(h, cudaEventRecord(ev_solve[P], ss));
@@ -880,7 +880,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           KBO_CUDA(h, cudaStreamWaitEvent(su, ev_nsolve[P], 0));
           if (pred1) KBO_CUDA(h, cudaStreamWaitEvent(su, pred1, 0));
           const double* Lf = A + (size_t)rf * lda + K0;
-          dgemm64_launch<true, EPI_STORE>(su, n_far, n_near, Wd, Lf, lda, Ln, lda, A + (size_t)rf * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
+          dgemm_sm90_launch<true>(su, n_far, n_near, Wd, Lf, lda, Ln, lda, A + (size_t)rf * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
           KBO_CUDA(h, cudaEventRecord(ev_col[P + 1], su));
           tmark(su, "distance-1 update done", P);
@@ -889,7 +889,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
             KBO_CUDA(h, cudaStreamWaitEvent(st, ev_solve[P], 0));
             KBO_CUDA(h, cudaStreamWaitEvent(st, ev_mid[P], 0));
             if (cudaEvent_t pe = pred_of(2)) KBO_CUDA(h, cudaStreamWaitEvent(st, pe, 0));
-            dgemm64_launch<true, EPI_STORE>(st, n_far, n_mid, Wd, Lf, lda, Lm, lda, A + (size_t)rf * lda + rm, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
+            dgemm_sm90_launch<true>(st, n_far, n_mid, Wd, Lf, lda, Lm, lda, A + (size_t)rf * lda + rm, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
             KBO_LAUNCH_CHECK(h);
             KBO_CUDA(h, cudaEventRecord(ev_cb[(size_t)(P + 2) * CBW + 2], st));
             tmark(st, "distance-2 update done", P);
@@ -903,7 +903,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
             KBO_CUDA(h, cudaStreamWaitEvent(st, ev_solve[P], 0));
             if (cudaEvent_t pe = pred_of(k)) KBO_CUDA(h, cudaStreamWaitEvent(st, pe, 0));
             const double* Lc = A + (size_t)c0 * lda + K0;
-            dgemm64_launch<true, EPI_STORE>(st, N - c0, min(OW, N - c0), Wd, Lc, lda, Lc, lda, A + (size_t)c0 * lda + c0, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
+            dgemm_sm90_launch<true>(st, N - c0, min(OW, N - c0), Wd, Lc, lda, Lc, lda, A + (size_t)c0 * lda + c0, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
             KBO_LAUNCH_CHECK(h);
             KBO_CUDA(h, cudaEventRecord(ev_cb[(size_t)j * CBW + k], st));
             tmark(st, k == 2 ? "distance-2 update done" : k == 3 ? "distance-3 update done" : "distance-4+ update done", P);
@@ -915,7 +915,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
             if (cB < N) {
               KBO_CUDA(h, cudaStreamWaitEvent(sb, ev_solve[P], 0));
               const double* Lb = A + (size_t)cB * lda + (size_t)Pb * OW;
-              dgemm64_launch<true, EPI_STORE>(sb, N - cB, N - cB, Kb, Lb, lda, Lb, lda, A + (size_t)cB * lda + cB, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
+              dgemm_sm90_launch<true>(sb, N - cB, N - cB, Kb, Lb, lda, Lb, lda, A + (size_t)cB * lda + cB, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
               KBO_LAUNCH_CHECK(h);
               KBO_CUDA(h, cudaEventRecord(ev_rest[P], sb));
               tmark(sb, "bulk update done", P);
@@ -947,18 +947,18 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           for (int r0 = 0; r0 + b < Pw; r0 += 2 * b) {
             const int rows2 = min(b, Pw - (r0 + b));
             double* T21 = T + (size_t)(P0 + r0 + b) * ldw + P0 + r0;
-            dgemm64_launch<false, EPI_STORE>(si, rows2, b, b, Lrp + (size_t)(r0 + b) * lda + r0, lda, Wrp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
-                                             KM_FROM_N, 0, TS_NONE);
+            dgemm_sm90_launch<false>(si, rows2, b, b, Lrp + (size_t)(r0 + b) * lda + r0, lda, Wrp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
+                                     KM_FROM_N, 0, TS_NONE);
             KBO_LAUNCH_CHECK(h);
-            dgemm64_launch<false, EPI_STORE>(si, rows2, b, rows2, Wrp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
-                                             Wrp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+            dgemm_sm90_launch<false>(si, rows2, b, rows2, Wrp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
+                                     Wrp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
             KBO_LAUNCH_CHECK(h);
           }
         if (P0 > 0) {
           double* Trow = T + (size_t)P0 * ldw;
-          dgemm64_launch<false, EPI_STORE>(si, Pw, P0, P0, A + (size_t)P0 * lda, lda, W, ldw, Trow, ldw, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
+          dgemm_sm90_launch<false>(si, Pw, P0, P0, A + (size_t)P0 * lda, lda, W, ldw, Trow, ldw, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
-          dgemm64_launch<false, EPI_STORE>(si, Pw, P0, Pw, Wrp, ldw, Trow, ldw, W + (size_t)P0 * ldw, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+          dgemm_sm90_launch<false>(si, Pw, P0, Pw, Wrp, ldw, Trow, ldw, W + (size_t)P0 * ldw, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
           KBO_LAUNCH_CHECK(h);
         }
       }
@@ -1322,18 +1322,18 @@ int kbo_i_ensure_w(kbo_handle* h, cudaStream_t s) {
       for (int r0 = 0; r0 + b < Pw; r0 += 2 * b) {
         const int rows2 = min(b, Pw - (r0 + b));
         double* T21 = T + (size_t)(P0 + r0 + b) * ld + P0 + r0;
-        dgemm64_launch<false, EPI_STORE>(s, rows2, b, b, Lrp + (size_t)(r0 + b) * ld + r0, ld, Wrp + (size_t)r0 * ld + r0, ld, T21, ld, 1.0, 0.0, KM_FROM_N, 0,
-                                         TS_NONE);
+        dgemm_sm90_launch<false>(s, rows2, b, b, Lrp + (size_t)(r0 + b) * ld + r0, ld, Wrp + (size_t)r0 * ld + r0, ld, T21, ld, 1.0, 0.0, KM_FROM_N, 0,
+                                 TS_NONE);
         KBO_LAUNCH_CHECK(h);
-        dgemm64_launch<false, EPI_STORE>(s, rows2, b, rows2, Wrp + (size_t)(r0 + b) * ld + r0 + b, ld, T21, ld, Wrp + (size_t)(r0 + b) * ld + r0, ld, -1.0,
-                                         0.0, KM_UPTO_M, 0, TS_NONE);
+        dgemm_sm90_launch<false>(s, rows2, b, rows2, Wrp + (size_t)(r0 + b) * ld + r0 + b, ld, T21, ld, Wrp + (size_t)(r0 + b) * ld + r0, ld, -1.0,
+                                 0.0, KM_UPTO_M, 0, TS_NONE);
         KBO_LAUNCH_CHECK(h);
       }
     if (P0 > 0) {
       double* Trow = T + (size_t)P0 * ld;
-      dgemm64_launch<false, EPI_STORE>(s, Pw, P0, P0, A + (size_t)P0 * ld, ld, W, ld, Trow, ld, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
+      dgemm_sm90_launch<false>(s, Pw, P0, P0, A + (size_t)P0 * ld, ld, W, ld, Trow, ld, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
       KBO_LAUNCH_CHECK(h);
-      dgemm64_launch<false, EPI_STORE>(s, Pw, P0, Pw, Wrp, ld, Trow, ld, W + (size_t)P0 * ld, ld, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
+      dgemm_sm90_launch<false>(s, Pw, P0, Pw, Wrp, ld, Trow, ld, W + (size_t)P0 * ld, ld, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
       KBO_LAUNCH_CHECK(h);
     }
   }
