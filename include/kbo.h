@@ -231,7 +231,8 @@ int kbo_last_timings(kbo_handle* h, kbo_timings* out);
  *            (reuses its inverted diagonal blocks).
  * kbo_acq_argmax: standalone acquisition + argmax pass over (mu, var) in the NORMALISED y scale:
  *            mu_n, var_n fp32 (8 B/candidate read) -> optional acq fp32 (4 B write) + best. The HBM-bound kernel
- *            whose GB/s the headline metric asks for. */
+ *            whose GB/s the headline metric asks for.  y_std must be finite and > 0 (KBO_ERR_INVALID otherwise):
+ *            the values are ranked in units of y_std. */
 int kbo_gram(kbo_handle* h, const double* Xs, int32_t N, int32_t D, int32_t kernel, double amplitude, double noise,
              double* K, int32_t ldk, void* stream);
 int kbo_potrf(kbo_handle* h, double* A, int32_t N, int32_t lda, int32_t* info_dev, void* stream);

@@ -353,6 +353,7 @@ int kbo_acq_argmax(kbo_handle* h, const float* mu_n, const float* var_n, int64_t
   if (!h) return KBO_ERR_INVALID;
   if (!mu_n || !var_n || !best_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_acq_argmax: null argument");
   if (acq < KBO_ACQ_EI || acq > KBO_ACQ_PI) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_acq_argmax: unknown acquisition %d", acq);
+  if (!(y_std > 0.0) || !(y_std < INFINITY)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_acq_argmax: y_std must be finite and > 0 (got %g)", y_std);
   return kbo_i_acq_argmax_f32(h, mu_n, var_n, M, global_offset, acq, y_mean, y_std, y_opt, xi, kappa, 1.0, acq_out, best_dev,
                               (cudaStream_t)stream);
 }

@@ -223,7 +223,7 @@ __device__ __forceinline__ T acq_value(T mun, T varn, int acq, T ymean, T ystd, 
   *mu_o = mu;
   *sd_o = sd;
   if (acq == KBO_ACQ_LCB) return -(mu - kappa * sd);
-  if (!(sd > (T)0)) return (T)0;
+  if (!(sd > (T)0)) return sd == sd ? (T)0 : sd;   // σ = 0: no improvement possible; a NaN σ (NaN y statistics) stays NaN
   const T imp = yopt - xi - mu;
   const T z = imp / sd;
   const T cdf = (T)0.5 * erfc(-z * (T)0.70710678118654752440);
@@ -260,14 +260,33 @@ __device__ __forceinline__ float kbo_erfc_nonneg_f32(float x) {
   p = fmaf(p, t, -1.26551223f);
   return t * kbo_ex2_ftz(1.44269504088896340736f * fmaf(-x, x, p));
 }
+// The fp32 acquisition is evaluated in NORMALISED units, never at the raw y scale: an fp32 μ = y_mean + y_std·μ_n rounds at
+// the scale of y_mean (half an ulp is 1e-3 at |y_mean| = 2e4 — a Katib metric in µs), which is above every slack of the
+// bounds below.  c_n = (y_opt − ξ − y_mean)/y_std is formed once in FP64 and carried as an fp32 hi/lo pair, so the
+// improvement c_n − μ_n is as accurate as μ_n itself.  The values returned are
+//   EI: imp_n·Φ(z) + σ_n·φ(z) = EI / y_std     PI: Φ(z) = PI     LCB: κσ_n − μ_n = (LCB value + y_mean) / y_std
+// — increasing maps of the raw value (y_std > 0), so they rank the same; acq_raw() undoes the map where a raw value is wanted.
+struct AcqFrame {
+  float chi, clo, kp;
+};
+__device__ __forceinline__ AcqFrame acq_frame(double ymean, double ystd, double yopt, double xi, double kappa) {
+  const double c = (yopt - xi - ymean) / ystd;
+  AcqFrame f;
+  f.chi = (float)c;
+  f.clo = (float)(c - (double)f.chi);
+  f.kp = (float)kappa;
+  return f;
+}
+__device__ __forceinline__ double acq_raw(int acq, double a, double ymean, double ystd) {
+  return acq == KBO_ACQ_PI ? a : acq == KBO_ACQ_LCB ? fma(ystd, a, -ymean) : ystd * a;
+}
 template <int ACQ>
-__device__ __forceinline__ float acq_value_f32(float mun, float varn, float ymean, float ystd, float yopt, float xi, float kappa) {
+__device__ __forceinline__ float acq_value_f32(float mun, float varn, const AcqFrame& f) {
   const float var = fmaxf(varn, 0.f);
-  const float mu = fmaf(ystd, mun, ymean);
-  const float sd = var > 0.f ? var * rsqrtf(var) * ystd : 0.f;
-  if (ACQ == KBO_ACQ_LCB) return kappa * sd - mu;
+  const float sd = var > 0.f ? var * rsqrtf(var) : 0.f;
+  if (ACQ == KBO_ACQ_LCB) return fmaf(f.kp, sd, -mun);
   if (!(sd > 0.f)) return 0.f;
-  const float imp = yopt - xi - mu;
+  const float imp = (f.chi - mun) + f.clo;
   const float z = __fdividef(imp, sd);   // MUFU.RCP + FMUL (2 ulp), no IEEE-division subroutine
   const float q = 0.5f * kbo_erfc_nonneg_f32(0.70710678118654752440f * fabsf(z));   // tail beyond |z|
   const float cdf = z <= 0.f ? q : 1.f - q;
@@ -291,7 +310,11 @@ acq_kernel(const T* __restrict__ mun, const T* __restrict__ varn, int64_t M, int
   }
   double bv = -INFINITY;
   long long bi = 0x7fffffffffffffffLL;
-  const T ym = (T)ymean, ys = (T)ystd, yo = (T)yopt, x = (T)xi, kp = (T)kappa;
+  const AcqFrame fr = acq_frame(ymean, ystd, yopt, xi, kappa);
+  constexpr int FA = FAST_ACQ >= 0 ? FAST_ACQ : 0;
+  // fp32 specialisation: ranking values are normalised (acq_value_f32); what leaves the kernel is the raw value
+  const float ysf = (float)ystd, ymf = (float)ymean;
+  auto raw32 = [&](float a) { return FA == KBO_ACQ_PI ? a : FA == KBO_ACQ_LCB ? fmaf(ysf, a, -ymf) : ysf * a; };
   const int64_t stride = (int64_t)gridDim.x * 256 * 4;
   auto load4 = [&](int64_t base, T (&m4)[4], T (&v4)[4]) {
     if (base + 3 < M) {
@@ -314,11 +337,14 @@ acq_kernel(const T* __restrict__ mun, const T* __restrict__ varn, int64_t M, int
       }
     }
   };
-  // Per-thread running best is kept in the value type T with a strict '>' (indices only grow inside a thread, so the
+  // Per-thread running best is kept in the value type VT with a strict '>' (indices only grow inside a thread, so the
   // first maximum wins without an index compare); it is widened to (double, int64) once, before the cross-thread reduce.
-  T tbest = -(T)INFINITY;
-  int64_t tidx = 0x7fffffffffffffffLL;
+  // The generic path evaluates in FP64 also for fp32 inputs (the arrays of a tensor-core sweep): an fp32 μ = y_mean + y_std·μ_n
+  // would round at the scale of y_mean.
   constexpr bool fast32 = FAST_ACQ >= 0;
+  using VT = typename std::conditional<fast32, T, double>::type;
+  VT tbest = -(VT)INFINITY;
+  int64_t tidx = 0x7fffffffffffffffLL;
   auto process4 = [&](int64_t base, const T (&m4)[4], const T (&v4)[4]) {
     if (base >= M) return;
     const bool full = base + 3 < M;
@@ -328,17 +354,17 @@ acq_kernel(const T* __restrict__ mun, const T* __restrict__ varn, int64_t M, int
       float a4[4];
 #pragma unroll
       for (int q = 0; q < 4; q++)
-        a4[q] = acq_value_f32<(FAST_ACQ >= 0 ? FAST_ACQ : 0)>((float)m4[q], (float)v4[q], (float)ym, (float)ys, (float)yo, (float)x, (float)kp);
-      if (acq_out32) __stcs(reinterpret_cast<float4*>(acq_out32 + base), make_float4(a4[0], a4[1], a4[2], a4[3]));
+        a4[q] = acq_value_f32<FA>((float)m4[q], (float)v4[q], fr);
+      if (acq_out32) __stcs(reinterpret_cast<float4*>(acq_out32 + base), make_float4(raw32(a4[0]), raw32(a4[1]), raw32(a4[2]), raw32(a4[3])));
       if (acq_out) {
 #pragma unroll
-        for (int q = 0; q < 4; q++) acq_out[base + q] = (double)a4[q];
+        for (int q = 0; q < 4; q++) acq_out[base + q] = acq_raw(FA, (double)a4[q], ymean, ystd);
       }
       const float gm = fmaxf(fmaxf(a4[0], a4[1]), fmaxf(a4[2], a4[3]));   // fmaxf ignores NaN operands
-      if ((T)gm > tbest || tidx == 0x7fffffffffffffffLL) {
+      if ((VT)gm > tbest || tidx == 0x7fffffffffffffffLL) {
         const int q = a4[0] == gm ? 0 : a4[1] == gm ? 1 : a4[2] == gm ? 2 : a4[3] == gm ? 3 : -1;   // −1: all four are NaN
         if (q >= 0) {
-          tbest = (T)gm;
+          tbest = (VT)gm;
           tidx = base + q;
         }
       }
@@ -347,21 +373,22 @@ acq_kernel(const T* __restrict__ mun, const T* __restrict__ varn, int64_t M, int
     float o4[4];
 #pragma unroll
     for (int q = 0; q < 4; q++) {
-      T mu = (T)0, sd = (T)0;
-      T a;
+      double mu = 0.0, sd = 0.0;
+      VT a;
       if (fast32) {
         const float fm = (float)m4[q], fv = (float)v4[q];
-        a = (T)acq_value_f32<(FAST_ACQ >= 0 ? FAST_ACQ : 0)>(fm, fv, (float)ym, (float)ys, (float)yo, (float)x, (float)kp);
+        a = (VT)acq_value_f32<FA>(fm, fv, fr);
+        o4[q] = raw32((float)a);
       } else {
-        a = acq_value<T>(m4[q], v4[q], acq, ym, ys, yo, x, kp, &mu, &sd);
+        a = (VT)acq_value<double>((double)m4[q], (double)v4[q], acq, ymean, ystd, yopt, xi, kappa, &mu, &sd);
+        o4[q] = (float)a;
       }
-      o4[q] = (float)a;
       if (full || base + q < M) {
         if (!fast32) {
           if (mu_out) mu_out[base + q] = (double)mu;
           if (std_out) std_out[base + q] = (double)sd;
         }
-        if (acq_out) acq_out[base + q] = (double)a;
+        if (acq_out) acq_out[base + q] = fast32 ? acq_raw(FA, (double)a, ymean, ystd) : (double)a;
         if (a > tbest || (tidx == 0x7fffffffffffffffLL && a == a)) {  // NaN never wins; −inf can (all-hopeless grids)
           tbest = a;
           tidx = base + q;
@@ -463,7 +490,7 @@ acq_kernel(const T* __restrict__ mun, const T* __restrict__ varn, int64_t M, int
         bv = sv[w];
         bi = si[w];
       }
-    best->value = bv;
+    best->value = fast32 && bv > -INFINITY ? acq_raw(FA, bv, ymean, ystd) : bv;   // no pick: −inf, whatever the y statistics
     best->index = bi;
     const int64_t l = bi - goff;
     if (l >= 0 && l < M) {
@@ -488,13 +515,19 @@ acq_kernel(const T* __restrict__ mun, const T* __restrict__ varn, int64_t M, int
 __global__ void __launch_bounds__(256)
 contender_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int64_t M, int acq, const double* __restrict__ scal, double xi,
                  double kappa, const kbo_best* __restrict__ best, int64_t goff, double delta, int* __restrict__ list, int* __restrict__ count) {
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
-  const float thr = (float)(best->value - delta);
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
+  auto value = [&](int64_t i) {
+    return acq == KBO_ACQ_EI    ? acq_value_f32<KBO_ACQ_EI>(mun[i], varn[i], f)
+           : acq == KBO_ACQ_LCB ? acq_value_f32<KBO_ACQ_LCB>(mun[i], varn[i], f)
+                                : acq_value_f32<KBO_ACQ_PI>(mun[i], varn[i], f);
+  };
+  // the window is centred on the pick's own normalised fp32 value (delta is in normalised units: delta·y_std raw); a pick
+  // that is not the fp32 maximum only widens it.  No pick (every value NaN: the index is the sentinel): no window.
+  const int64_t l = best->index - goff;
+  const float thr = (l >= 0 && l < M) ? value(l) - (float)delta : INFINITY;
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < M; i += (int64_t)gridDim.x * 256) {
-    const float a = acq == KBO_ACQ_EI    ? acq_value_f32<KBO_ACQ_EI>(mun[i], varn[i], ym, ys, yo, x, kp)
-                    : acq == KBO_ACQ_LCB ? acq_value_f32<KBO_ACQ_LCB>(mun[i], varn[i], ym, ys, yo, x, kp)
-                                         : acq_value_f32<KBO_ACQ_PI>(mun[i], varn[i], ym, ys, yo, x, kp);
-    if (a >= thr) {
+    const float a = value(i);
+    if (a >= thr || (l >= 0 && l < M && !(mun[i] == mun[i] && varn[i] == varn[i]))) {   // a NaN mean or variance is never pruned
       const int slot = atomicAdd(count, 1);
       if (slot < KBO_REFINE_CAP) list[slot] = (int)i;
     }
@@ -560,6 +593,12 @@ refine_best_kernel(const double* __restrict__ mun, const double* __restrict__ va
       }
     }
     __syncthreads();
+  }
+  if (threadIdx.x == 0 && sp[0] == 0x7fffffff) {   // every FP64 value NaN: what acq_kernel reports when nothing is picked
+    best->value = -INFINITY;
+    best->index = 0x7fffffffffffffffLL;
+    best->mu = 0.0;
+    best->std = 0.0;
   }
   if (threadIdx.x == 0 && sp[0] != 0x7fffffff) {
     const int p = sp[0];
@@ -754,8 +793,9 @@ static int refine_suggestion(kbo_handle* h, const void* Xc, int xc_dtype, int64_
   KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
   int* list = (int*)h->refine.p;
   int* count = list + KBO_REFINE_CAP;
-  // contenders: within delta of the fp32 maximum.  2e-4 is ≥ 10× the tensor-core mode's acquisition error bound; when more
-  // than the cap lie inside it (a flat landscape, or a late-stage experiment whose best EI is itself below 2e-4) the window is
+  // contenders: within delta of the fp32 maximum, in normalised units (2e-4·y_std on the raw scale; for LCB the raw value is
+  // ≈ −y_mean, whose fp32 ulp alone can exceed any absolute window).  2e-4 is ≥ 10× the tensor-core mode's acquisition error
+  // bound; when more than the cap lie inside it (a flat landscape, or a late-stage experiment whose best EI is itself below 2e-4·y_std) the window is
   // narrowed until the cap holds and the FP64 decision is taken among the best by fp32 value (last_unrefined = 1); only
   // exact fp32 ties beyond the cap — e.g. thousands of identical candidates — keep the tensor-core pick (last_unrefined = 2),
   // which is then the lowest index among them, as the reference's argmin is.
@@ -833,16 +873,19 @@ static int refine_evaluate(kbo_handle* h, const void* Xc, int xc_dtype, int n, i
 // and LCB grow with σ, PI is monotone either way, so the two ends bound the value over the interval.  Survivors (typically a
 // handful: EI is sharply peaked) go through the FP64 refinement; more than 4096 of them and the sweep is redone with the
 // three-product kernel.
-__device__ __forceinline__ float acq_any_f32(int acq, float mu, float var, float ym, float ys, float yo, float x, float kp) {
-  return acq == KBO_ACQ_EI    ? acq_value_f32<KBO_ACQ_EI>(mu, var, ym, ys, yo, x, kp)
-         : acq == KBO_ACQ_LCB ? acq_value_f32<KBO_ACQ_LCB>(mu, var, ym, ys, yo, x, kp)
-                              : acq_value_f32<KBO_ACQ_PI>(mu, var, ym, ys, yo, x, kp);
+__device__ __forceinline__ float acq_any_f32(int acq, float mu, float var, const AcqFrame& f) {
+  return acq == KBO_ACQ_EI    ? acq_value_f32<KBO_ACQ_EI>(mu, var, f)
+         : acq == KBO_ACQ_LCB ? acq_value_f32<KBO_ACQ_LCB>(mu, var, f)
+                              : acq_value_f32<KBO_ACQ_PI>(mu, var, f);
 }
 __device__ __forceinline__ unsigned ordered_bits(float v) {   // monotone float -> uint
   const unsigned b = __float_as_uint(v);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 __device__ __forceinline__ float from_ordered_bits(unsigned u) { return __uint_as_float((u & 0x80000000u) ? (u & 0x7fffffffu) : ~u); }
+// the calibration maxima propagate NaN (fmaxf drops it): a NaN error must not leave a tight bound behind.  A NaN E or Eμ makes
+// every bound NaN, so no lower bound is found, nothing is pruned and the sweep falls back to three products / the FP64 path.
+__device__ __forceinline__ float max_nan(float a, float b) { return (a != a || a > b) ? a : b; }
 
 // Calibration of the ranking pass on STRATIFIED rows: row i·M/n of the grid, i < n (n = one wave of the variance kernel, or all
 // rows of a small grid), so a sorted / clustered / blocked candidate order is sampled across its whole extent.  Those rows went
@@ -859,16 +902,16 @@ __global__ void __launch_bounds__(1024) calib_kernel(const float* __restrict__ v
   float m = 0.f, mm = 0.f;
   for (int i = threadIdx.x; i < n; i += 1024) {
     const int g = list[i];
-    m = fmaxf(m, fabsf(v1[g] - v3[i]));
-    mm = fmaxf(mm, fabsf(mu1[g] - mu3[i]));
+    m = max_nan(m, fabsf(v1[g] - v3[i]));
+    mm = max_nan(mm, fabsf(mu1[g] - mu3[i]));
   }
   red[threadIdx.x] = m;
   redm[threadIdx.x] = mm;
   __syncthreads();
   for (int o = 512; o > 0; o >>= 1) {
     if (threadIdx.x < o) {
-      red[threadIdx.x] = fmaxf(red[threadIdx.x], red[threadIdx.x + o]);
-      redm[threadIdx.x] = fmaxf(redm[threadIdx.x], redm[threadIdx.x + o]);
+      red[threadIdx.x] = max_nan(red[threadIdx.x], red[threadIdx.x + o]);
+      redm[threadIdx.x] = max_nan(redm[threadIdx.x], redm[threadIdx.x + o]);
     }
     __syncthreads();
   }
@@ -882,23 +925,29 @@ __global__ void __launch_bounds__(1024) calib_kernel(const float* __restrict__ v
 }
 // Bounds of the acquisition value over the box (μ ± Eμ) × (σ² ± E): all three kinds fall with μ; EI and LCB grow with σ, PI is
 // monotone in σ either way — so the corners bound the value.
-__device__ __forceinline__ void acq_bounds_f32(int acq, float mu, float var, float E, float Em, float ym, float ys, float yo, float x, float kp,
+// A NaN mean, variance, E or Eμ gives NaN bounds (the clamps and maxima below would drop it and bound at σ = 0): a NaN upper
+// bound survives every interval test, a NaN lower bound never enters the maximum.
+__device__ __forceinline__ void acq_bounds_f32(int acq, float mu, float var, float E, float Em, const AcqFrame& f,
                                                float* lb, float* ub) {
+  if (!(mu == mu && var == var && E == E && Em == Em)) {
+    *lb = *ub = __int_as_float(0x7fc00000);
+    return;
+  }
   const float vlo = fmaxf(var - E, 0.f), vhi = var + E;
-  const float u0 = acq_any_f32(acq, mu - Em, vlo, ym, ys, yo, x, kp), u1 = acq_any_f32(acq, mu - Em, vhi, ym, ys, yo, x, kp);
-  const float l0 = acq_any_f32(acq, mu + Em, vlo, ym, ys, yo, x, kp), l1 = acq_any_f32(acq, mu + Em, vhi, ym, ys, yo, x, kp);
+  const float u0 = acq_any_f32(acq, mu - Em, vlo, f), u1 = acq_any_f32(acq, mu - Em, vhi, f);
+  const float l0 = acq_any_f32(acq, mu + Em, vlo, f), l1 = acq_any_f32(acq, mu + Em, vhi, f);
   *ub = fmaxf(u0, u1);
   *lb = fminf(l0, l1);
 }
 __global__ void __launch_bounds__(256)
 bound_max_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int64_t M, int acq, const double* __restrict__ scal, double xi,
                  double kappa, float* __restrict__ fs) {
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   const float E = fs[0], Em = fs[3];
   float best = -INFINITY;
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < M; i += (int64_t)gridDim.x * 256) {
     float lb, ub;
-    acq_bounds_f32(acq, mun[i], varn[i], E, Em, ym, ys, yo, x, kp, &lb, &ub);
+    acq_bounds_f32(acq, mun[i], varn[i], E, Em, f, &lb, &ub);
     if (lb > best) best = lb;   // NaN never enters
   }
 #pragma unroll
@@ -908,14 +957,14 @@ bound_max_kernel(const float* __restrict__ mun, const float* __restrict__ varn, 
 __global__ void __launch_bounds__(256)
 survivor_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int64_t M, int acq, const double* __restrict__ scal, double xi,
                 double kappa, const float* __restrict__ fs, int* __restrict__ list, int* __restrict__ count) {
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   const float E = fs[0], Em = fs[3];
   const float lbmax = from_ordered_bits(((const unsigned*)fs)[1]);
   const float thr = lbmax - 1e-5f * fmaxf(1.f, fabsf(lbmax));   // fp32 evaluation and fp32 storage of μ
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < M; i += (int64_t)gridDim.x * 256) {
     float lb, ub;
-    acq_bounds_f32(acq, mun[i], varn[i], E, Em, ym, ys, yo, x, kp, &lb, &ub);
-    if (ub >= thr) {
+    acq_bounds_f32(acq, mun[i], varn[i], E, Em, f, &lb, &ub);
+    if (!(ub < thr)) {   // NaN survives
       const int slot = atomicAdd(count, 1);
       if (slot < KBO_REFINE_CAP) list[slot] = (int)i;
     }
@@ -935,12 +984,12 @@ __global__ void __launch_bounds__(1024)
 calib_lb_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_ex, const float* __restrict__ mu_rk, const float* __restrict__ mu_ex, int n,
                 int acq, const double* __restrict__ scal, double xi, double kappa, float* __restrict__ fs) {
   __shared__ float red[1024], redm[1024], redl[1024];
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   float m = 0.f, mm = 0.f, lb = -INFINITY;
   for (int i = threadIdx.x; i < n; i += 1024) {
-    m = fmaxf(m, fabsf(v_rk[i] - v_ex[i]));
-    mm = fmaxf(mm, fabsf(mu_rk[i] - mu_ex[i]));
-    const float a = acq_any_f32(acq, mu_ex[i], v_ex[i], ym, ys, yo, x, kp);   // three-product value: |error| ~ 1e-6
+    m = max_nan(m, fabsf(v_rk[i] - v_ex[i]));
+    mm = max_nan(mm, fabsf(mu_rk[i] - mu_ex[i]));
+    const float a = acq_any_f32(acq, mu_ex[i], v_ex[i], f);   // three-product value: |error| ~ 1e-6
     if (a > lb) lb = a;
   }
   red[threadIdx.x] = m;
@@ -949,8 +998,8 @@ calib_lb_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_ex, 
   __syncthreads();
   for (int o = 512; o > 0; o >>= 1) {
     if (threadIdx.x < o) {
-      red[threadIdx.x] = fmaxf(red[threadIdx.x], red[threadIdx.x + o]);
-      redm[threadIdx.x] = fmaxf(redm[threadIdx.x], redm[threadIdx.x + o]);
+      red[threadIdx.x] = max_nan(red[threadIdx.x], red[threadIdx.x + o]);
+      redm[threadIdx.x] = max_nan(redm[threadIdx.x], redm[threadIdx.x + o]);
       redl[threadIdx.x] = fmaxf(redl[threadIdx.x], redl[threadIdx.x + o]);
     }
     __syncthreads();
@@ -965,22 +1014,24 @@ calib_lb_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_ex, 
   }
 }
 // supremum of the acquisition value over mu in [mu ± Em], sigma² in (0, var_ub]
-__device__ __forceinline__ float acq_prefix_ub_f32(int acq, float mu, float var_ub, float Em, float ym, float ys, float yo, float x, float kp) {
+__device__ __forceinline__ float acq_prefix_ub_f32(int acq, float mu, float var_ub, float Em, const AcqFrame& f) {
+  if (!(mu == mu && var_ub == var_ub && Em == Em)) return __int_as_float(0x7fc00000);   // NaN: survives
   if (acq == KBO_ACQ_PI) {   // Φ(imp/σ): falls with σ where imp > 0 — its supremum there is 1
-    const float imp = yo - x - fmaf(ys, mu - Em, ym);
+    const float imp = (f.chi - (mu - Em)) + f.clo;
     if (imp > 0.f) return 1.f;
   }
-  return acq_any_f32(acq, mu - Em, var_ub, ym, ys, yo, x, kp);
+  return acq_any_f32(acq, mu - Em, var_ub, f);
 }
 __global__ void __launch_bounds__(256)
 prefix_survivor_kernel(const float* __restrict__ mun, const float* __restrict__ var_ub, int64_t M, int acq, const double* __restrict__ scal, double xi,
                        double kappa, const float* __restrict__ fs, int* __restrict__ list, int* __restrict__ count, int cap) {
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   const float E = fs[0], Em = fs[3];
   const float lb = from_ordered_bits(((const unsigned*)fs)[1]);
   const float thr = lb - 1e-5f * fmaxf(1.f, fabsf(lb));
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < M; i += (int64_t)gridDim.x * 256) {
-    const float ub = acq_prefix_ub_f32(acq, mun[i], fmaxf(var_ub[i], 0.f) + E, Em, ym, ys, yo, x, kp);
+    const float v = var_ub[i];
+    const float ub = acq_prefix_ub_f32(acq, mun[i], v == v ? fmaxf(v, 0.f) + E : v, Em, f);
     if (!(ub < thr)) {   // NaN survives
       const int slot = atomicAdd(count, 1);
       if (slot < cap) list[slot] = (int)i;
@@ -991,12 +1042,12 @@ prefix_survivor_kernel(const float* __restrict__ mun, const float* __restrict__ 
 __global__ void __launch_bounds__(256)
 survivor_lb_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int n, int acq, const double* __restrict__ scal, double xi, double kappa,
                    float* __restrict__ fs) {
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   const float E = fs[0], Em = fs[3];
   float best = -INFINITY;
   for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
     float lb, ub;
-    acq_bounds_f32(acq, mun[i], varn[i], E, Em, ym, ys, yo, x, kp, &lb, &ub);
+    acq_bounds_f32(acq, mun[i], varn[i], E, Em, f, &lb, &ub);
     if (lb > best) best = lb;
   }
 #pragma unroll
@@ -1006,13 +1057,13 @@ survivor_lb_kernel(const float* __restrict__ mun, const float* __restrict__ varn
 __global__ void __launch_bounds__(256)
 survivor_final_kernel(const float* __restrict__ mun, const float* __restrict__ varn, const int* __restrict__ src, int n, int acq,
                       const double* __restrict__ scal, double xi, double kappa, const float* __restrict__ fs, int* __restrict__ list, int* __restrict__ count) {
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   const float E = fs[0], Em = fs[3];
   const float lbmax = from_ordered_bits(((const unsigned*)fs)[1]);
   const float thr = lbmax - 1e-5f * fmaxf(1.f, fabsf(lbmax));
   for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
     float lb, ub;
-    acq_bounds_f32(acq, mun[i], varn[i], E, Em, ym, ys, yo, x, kp, &lb, &ub);
+    acq_bounds_f32(acq, mun[i], varn[i], E, Em, f, &lb, &ub);
     if (!(ub < thr)) {
       const int slot = atomicAdd(count, 1);
       if (slot < KBO_REFINE_CAP) list[slot] = src[i];
@@ -1025,21 +1076,23 @@ static int calibration_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
 // lower bound of the acquisition value over sigma² in (0, var_ub] at mean mu_n (normalised): EI and LCB grow with sigma, so the
 // bound is their sigma -> 0 limit (max(improvement, 0) and −mu: no variance needed at all); PI falls with sigma where the
 // improvement is positive, so its bound there sits at var_ub
-__device__ __forceinline__ float acq_lower_f32(int acq, float mu_n, float var_ub, float ym, float ys, float yo, float x, float kp) {
-  const float mu = fmaf(ys, mu_n, ym);
-  if (acq == KBO_ACQ_LCB) return -mu;
-  const float imp = yo - x - mu;
+__device__ __forceinline__ float acq_lower_f32(int acq, float mu_n, float var_ub, const AcqFrame& f) {
+  if (acq == KBO_ACQ_LCB) return -mu_n;
+  const float imp = (f.chi - mu_n) + f.clo;
   if (acq == KBO_ACQ_EI) return fmaxf(imp, 0.f);
-  return imp > 0.f ? acq_any_f32(acq, mu_n, var_ub, ym, ys, yo, x, kp) : 0.f;
+  return imp > 0.f ? acq_any_f32(acq, mu_n, var_ub, f) : 0.f;
 }
 __global__ void __launch_bounds__(256)
 grid_lower_bound_kernel(const float* __restrict__ mun, const float* __restrict__ var_ub, int64_t M, int acq, const double* __restrict__ scal, double xi,
                         double kappa, float* __restrict__ fs) {
-  const float ym = (float)scal[S_YMEAN], ys = (float)scal[S_YSTD], yo = (float)scal[S_YOPT], x = (float)xi, kp = (float)kappa;
+  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   const float E = fs[0], Em = fs[3];
+  if (!(E == E && Em == Em)) return;   // no bound from a NaN calibration: the lower bound stays unset and nothing is pruned
   float best = -INFINITY;
   for (int64_t i = (int64_t)blockIdx.x * 256 + threadIdx.x; i < M; i += (int64_t)gridDim.x * 256) {
-    const float lb = acq_lower_f32(acq, mun[i] + Em, fmaxf(var_ub[i], 0.f) + E, ym, ys, yo, x, kp);
+    const float m = mun[i], v = var_ub[i];
+    if (!(m == m && v == v)) continue;
+    const float lb = acq_lower_f32(acq, m + Em, fmaxf(v, 0.f) + E, f);
     if (lb > best) best = lb;
   }
 #pragma unroll
@@ -1053,16 +1106,16 @@ calib_prefix_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_
   __shared__ float red[1024], redm[1024];
   float m = 0.f, mm = 0.f;
   for (int i = threadIdx.x; i < n; i += 1024) {
-    m = fmaxf(m, fabsf(v_rk[i] - v_ex[i]));
-    mm = fmaxf(mm, fabsf(mu_rk[i] - mu_ex[i]));
+    m = max_nan(m, fabsf(v_rk[i] - v_ex[i]));
+    mm = max_nan(mm, fabsf(mu_rk[i] - mu_ex[i]));
   }
   red[threadIdx.x] = m;
   redm[threadIdx.x] = mm;
   __syncthreads();
   for (int o = 512; o > 0; o >>= 1) {
     if (threadIdx.x < o) {
-      red[threadIdx.x] = fmaxf(red[threadIdx.x], red[threadIdx.x + o]);
-      redm[threadIdx.x] = fmaxf(redm[threadIdx.x], redm[threadIdx.x + o]);
+      red[threadIdx.x] = max_nan(red[threadIdx.x], red[threadIdx.x + o]);
+      redm[threadIdx.x] = max_nan(redm[threadIdx.x], redm[threadIdx.x + o]);
     }
     __syncthreads();
   }
@@ -1340,8 +1393,15 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
   if (h->D > 256) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep: D <= 256 supported (got %d)", h->D);
   const int N = h->N, D = h->D, ld = h->ld, Npad = h->Npad;
   if (N > Npad || N > ld) KBO_FAIL(h, KBO_ERR_STATE, "kbo_sweep: inconsistent fit state (N=%d, Npad=%d, ld=%d)", N, Npad, ld);
-  const bool tc = h->prm.var_mode == KBO_VAR_TC_F16X3 ||
-                  (h->prm.var_mode == KBO_VAR_AUTO && h->have_planes && (double)M * h->N * h->N > 2e11);
+  // The fp16 K* planes hold amplitude·k: above 1e4 the entries near the trials approach the fp16 range (65504) and the
+  // contraction overflows, so such fits take the FP64 path in every mode.  The tensor-core error grows with the amplitude
+  // (|dσ²| ∝ amplitude): `auto` keeps the 1e-5 bound on returned arrays by using the tensor cores for array sweeps up to
+  // amplitude 10 only (DESIGN.md §1).  Array-free sweeps are decided in FP64 whatever the amplitude.
+  const double amp = h->prm.amplitude;
+  const bool arrays = mu_out || std_out || acq_out;
+  const bool tc = amp <= 1e4 && (h->prm.var_mode == KBO_VAR_TC_F16X3 ||
+                                 (h->prm.var_mode == KBO_VAR_AUTO && (amp <= 10.0 || !arrays) && h->have_planes &&
+                                  (double)M * h->N * h->N > 2e11));
   const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
   const double* scal = (const double*)h->scal.p;
   // array-free tensor-core sweeps rank with one fp16 product and let the FP64 refinement decide (fast_pick above)
