@@ -199,6 +199,24 @@ int kbo_fit_state(kbo_handle* h, double* L_out, double* W_out, double* alpha_out
  * best_dev: device kbo_best written at the end of the stream work. */
 int kbo_sweep(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, int64_t global_offset, int xc_on_host,
               double* mu_out, double* std_out, double* acq_out, kbo_best* best_dev, void* stream);
+/* Several acquisitions over ONE candidate grid, as skopt's gp_hedge evaluates EI, LCB and PI on the same candidates.
+ * acqs: n_acq (1-3) distinct kbo_acq_kind values, host memory; best_dev: n_acq device kbo_best.  best_dev[i] is what kbo_sweep
+ * with acq = acqs[i] returns on the same fit and grid.  The posterior (calibration rows, K* planes, contractions, mean) is
+ * computed once per stage for every acquisition still undecided; each acquisition keeps its own bounds, survivor lists and FP64
+ * decision and finishes at the first stage where its own list fits — where its single sweep would have.  Array-free.
+ * The FP64 decisions a stage takes are one evaluation over the union of those kinds' survivors.
+ * Duplicate or unknown kinds: KBO_ERR_INVALID.  kbo_last_decisions reports each kind's decision; kbo_last_unrefined,
+ * kbo_last_contenders, kbo_last_prefix_survivors, kbo_last_rank_error and kbo_last_rank_mu_error keep reporting the last
+ * kbo_sweep. */
+int kbo_sweep_multi(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, int64_t global_offset, int xc_on_host, int32_t n_acq,
+                    const int32_t* acqs, kbo_best* best_dev, void* stream);
+/* Per acquisition of the last kbo_sweep (one) or kbo_sweep_multi (n_acq, in request order): what kbo_last_unrefined,
+ * kbo_last_contenders and kbo_last_prefix_survivors report for a single sweep.  Fills up to n entries of each non-NULL array;
+ * returns the number of acquisitions the last sweep decided. */
+int kbo_last_decisions(kbo_handle* h, int32_t n, int32_t* unrefined, int32_t* contenders, int32_t* prefix_survivors);
+/* FP64 posterior mean (raw y scale) at n points X (n×D, dtype x_dtype, device or host): K*·alpha as the sweep's FP64
+ * refinement forms it.  Needs alpha only — a lazy fit's inverse is not formed.  mu_out_host: n doubles.  Synchronises. */
+int kbo_predict_mean(kbo_handle* h, const void* X, int32_t x_dtype, int32_t n, int x_on_host, double* mu_out_host, void* stream);
 /* synchronises `stream`, copies *best_dev to host, and returns KBO_ERR_NOT_PD if the fit failed. */
 int kbo_best_to_host(kbo_handle* h, const kbo_best* best_dev, kbo_best* best_host, void* stream);
 

@@ -48,7 +48,7 @@ void kbo_destroy(kbo_handle* h) {
                     &h->blockbest, &h->best, &h->XsT, &h->refine, &h->refine_x, &h->yraw, &h->lrow, &h->var_cal,
                     &h->ks_center, &h->ks_Xh, &h->ks_Xl, &h->ks_nxal, &h->ks_Ch, &h->ks_Cl, &h->ks_nc, &h->rk_part, &h->cal_idx, &h->cal_x, &h->cal_mu,
                     &h->comm_buf, &h->T2, &h->Linv4, &h->mu_part, &h->sv_B, &h->sv_V, &h->sv_bar, &h->zf, &h->lml_yn, &h->lml_scal, &h->rk_sched[0].dev, &h->rk_sched[1].dev, &h->rk_sched[2].dev, &h->rk_sched[3].dev, &h->rk_sched[4].dev, &h->rk_sched[5].dev,
-                    &h->rk_sched[6].dev, &h->rk_sched[7].dev, &h->pr_list, &h->pr_x, &h->pr_mu, &h->pr_var, &h->cal_mu_rk, &h->cal_var_rk};
+                    &h->rk_sched[6].dev, &h->rk_sched[7].dev, &h->pr_list, &h->pr_x, &h->pr_mu, &h->pr_var, &h->cal_mu_rk, &h->cal_var_rk, &h->un_idx, &h->un_mv};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   for (auto& ev : h->ev)
@@ -235,6 +235,47 @@ int kbo_sweep(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, int64_
     Xc = h->stage_Xc.p;
   }
   return kbo_i_sweep(h, Xc, xc_dtype, M, global_offset, mu_out, std_out, acq_out, best_dev, s);
+}
+
+static int stage_rows(kbo_handle* h, const void** X, int32_t dtype, int64_t rows, cudaStream_t s) {
+  const size_t bytes = (size_t)rows * h->D * (dtype == KBO_F64 ? 8 : 4);
+  KBO_TRY(kbo_reserve(h, h->stage_Xc, bytes));
+  KBO_CUDA(h, cudaMemcpyAsync(h->stage_Xc.p, *X, bytes, cudaMemcpyHostToDevice, s));
+  *X = h->stage_Xc.p;
+  return KBO_OK;
+}
+
+int kbo_sweep_multi(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, int64_t global_offset, int xc_on_host, int32_t n_acq,
+                    const int32_t* acqs, kbo_best* best_dev, void* stream) {
+  if (!h) return KBO_ERR_INVALID;
+  if (!Xc || !acqs || !best_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep_multi: null argument");
+  if (M < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep_multi: M must be >= 1");
+  cudaStream_t s = (cudaStream_t)stream;
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  if (xc_on_host) KBO_TRY(stage_rows(h, &Xc, xc_dtype, M, s));
+  return kbo_i_sweep_multi(h, Xc, xc_dtype, M, global_offset, n_acq, acqs, best_dev, s);
+}
+
+int kbo_last_decisions(kbo_handle* h, int32_t n, int32_t* unrefined, int32_t* contenders, int32_t* prefix_survivors) {
+  if (!h) return KBO_ERR_INVALID;
+  if (n < 0) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_last_decisions: n must be >= 0");
+  for (int k = 0; k < n && k < h->dec_n; k++) {
+    if (unrefined) unrefined[k] = h->dec_unrefined[k];
+    if (contenders) contenders[k] = h->dec_contenders[k];
+    if (prefix_survivors) prefix_survivors[k] = h->dec_prefix_survivors[k];
+  }
+  return h->dec_n;
+}
+
+int kbo_predict_mean(kbo_handle* h, const void* X, int32_t x_dtype, int32_t n, int x_on_host, double* mu_out_host, void* stream) {
+  if (!h) return KBO_ERR_INVALID;
+  if (!X || !mu_out_host) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_predict_mean: null argument");
+  if (n < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_predict_mean: n must be >= 1");
+  if (!h->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_predict_mean: call kbo_fit first");
+  cudaStream_t s = (cudaStream_t)stream;
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  if (x_on_host) KBO_TRY(stage_rows(h, &X, x_dtype, n, s));
+  return kbo_i_predict_mean(h, X, x_dtype, n, mu_out_host, s);
 }
 
 int kbo_best_to_host(kbo_handle* h, const kbo_best* best_dev, kbo_best* best_host, void* stream) {

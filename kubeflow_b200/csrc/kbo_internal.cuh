@@ -84,6 +84,9 @@ struct kbo_handle {
   DevBuf cal_idx, cal_x, cal_mu;   // stratified calibration rows of the ranking pass: indices, gathered rows, FP64-path mean
   float last_rank_mu_err = 0.f;    // largest |μ̃ − μ| (normalised units) on the calibration rows of the last ranking sweep
   int last_unrefined = 0;          // 1: the last tensor-core sweep could not decide in FP64 (more near-ties than the cap)
+  int dec_n = 0;                   // acquisitions the last kbo_sweep / kbo_sweep_multi decided, and how (kbo_last_decisions)
+  int dec_unrefined[3] = {}, dec_contenders[3] = {}, dec_prefix_survivors[3] = {};
+  DevBuf un_idx, un_mv;            // FP64 decision over the union of several acquisitions' survivors: indices / positions, mean + variance
   // ---- fit: Cholesky chain on a high-priority stream, row-panel inverse on a second one (fit.cu) ----------------------
   cudaStream_t s_hi = nullptr, s_lo = nullptr, s_upd = nullptr, s_copy = nullptr;
   DevBuf T2;                        // N × 256 panel-solve scratch of the look-ahead factorisation (v2)
@@ -182,6 +185,9 @@ int kbo_i_zsolve_update(kbo_handle* h, int K0, int Wd, cudaStream_t s);
 // ---- sweep.cu ----------------------------------------------------------------------------------
 int kbo_i_sweep(kbo_handle* h, const void* Xc_dev, int xc_dtype, int64_t M, int64_t goff, double* mu_out, double* std_out,
                 double* acq_out, kbo_best* best_dev, cudaStream_t s);
+int kbo_i_sweep_multi(kbo_handle* h, const void* Xc_dev, int xc_dtype, int64_t M, int64_t goff, int n_acq, const int32_t* acqs, kbo_best* best_dev,
+                      cudaStream_t s);
+int kbo_i_predict_mean(kbo_handle* h, const void* X_dev, int x_dtype, int n, double* mu_host, cudaStream_t s);
 int kbo_i_debug_cross_planes(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, cudaStream_t s);   // FP64 K* → Ksh/Ksl, mun (test hook)
 int kbo_i_acq_argmax_f32(kbo_handle* h, const float* mu_n, const float* var_n, int64_t M, int64_t goff, int acq, double y_mean,
                          double y_std, double y_opt, double xi, double kappa, double amp, float* acq_out, kbo_best* best_dev,

@@ -3,6 +3,7 @@
 //   skopt.acquisition.gaussian_ei / gaussian_lcb / gaussian_pi ; Optimizer._tell: X_cand[np.argmin(values)]
 // Per candidate chunk:  cross_mean_kernel (FP64: K*, μ = K*·alpha)  →  variance contraction (FP64 SIMT GEMM with a
 // fused Σv² epilogue, or the wgmma kernel in tc_var.cu)  →  once per sweep: acquisition + argmax.
+#include <algorithm>
 #include <type_traits>
 
 #include "kbo_internal.cuh"
@@ -533,29 +534,6 @@ contender_kernel(const float* __restrict__ mun, const float* __restrict__ varn, 
     }
   }
 }
-// ascending sort of the contender indices (single CTA, bitonic, padded with INT_MAX) so "first maximum" = lowest index
-__global__ void __launch_bounds__(1024) sort_contenders_kernel(int* __restrict__ list, const int* __restrict__ count) {
-  __shared__ int v[KBO_REFINE_CAP];
-  const int n = min(*count, KBO_REFINE_CAP);
-  for (int i = threadIdx.x; i < KBO_REFINE_CAP; i += 1024) v[i] = i < n ? list[i] : 0x7fffffff;
-  __syncthreads();
-  for (int k = 2; k <= KBO_REFINE_CAP; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < KBO_REFINE_CAP; i += 1024) {
-        const int l = i ^ j;
-        if (l > i) {
-          const bool up = (i & k) == 0;
-          const int a = v[i], b = v[l];
-          if ((a > b) == up) {
-            v[i] = b;
-            v[l] = a;
-          }
-        }
-      }
-      __syncthreads();
-    }
-  for (int i = threadIdx.x; i < n; i += 1024) list[i] = v[i];
-}
 template <typename XT>
 __global__ void gather_rows_kernel(const XT* __restrict__ Xc, int D, const int* __restrict__ list, int n, double* __restrict__ Xg) {
   const int r = blockIdx.x;
@@ -563,18 +541,30 @@ __global__ void gather_rows_kernel(const XT* __restrict__ Xc, int D, const int* 
   const int64_t src = list[r];
   for (int d = threadIdx.x; d < D; d += blockDim.x) Xg[(size_t)r * D + d] = (double)Xc[src * D + d];
 }
-// fp64 acquisition over the n contenders (sorted by index): first maximum wins; writes the refined suggestion
+// The FP64 decision of up to three acquisitions over the UNION of their survivors: the union's rows (uidx, ascending) carry
+// FP64 mean / variance evaluated once; acquisition k takes the first-index argmax over its own survivors, pos[off_k .. off_k+n_k)
+// (ascending positions into the union).  One CTA per acquisition.
+struct UnionPick {
+  int nk;
+  int acq[3], off[3], n[3];
+  kbo_best* best[3];
+};
 __global__ void __launch_bounds__(1024)
-refine_best_kernel(const double* __restrict__ mun, const double* __restrict__ varn, const int* __restrict__ list, int n, int acq,
-                   const double* __restrict__ scal, double xi, double kappa, int64_t goff, kbo_best* __restrict__ best) {
+refine_best_union_kernel(const double* __restrict__ mun, const double* __restrict__ varn, const int* __restrict__ uidx, const int* __restrict__ pos,
+                         UnionPick up, const double* __restrict__ scal, double xi, double kappa, int64_t goff) {
   __shared__ double sv[1024];
   __shared__ int sp[1024];
+  const int k = blockIdx.x;   // selects, not a dynamic index: the parameter block stays out of local memory
+  const int acq = k == 0 ? up.acq[0] : k == 1 ? up.acq[1] : up.acq[2];
+  const int n = k == 0 ? up.n[0] : k == 1 ? up.n[1] : up.n[2];
+  const int* ps = pos + (k == 0 ? up.off[0] : k == 1 ? up.off[1] : up.off[2]);
+  kbo_best* best = k == 0 ? up.best[0] : k == 1 ? up.best[1] : up.best[2];
   const double ym = scal[S_YMEAN], ys = scal[S_YSTD], yo = scal[S_YOPT];
   double bv = -INFINITY;
   int bp = 0x7fffffff;
   for (int p = threadIdx.x; p < n; p += 1024) {
     double mu, sd;
-    const double a = acq_value<double>(mun[p], varn[p], acq, ym, ys, yo, xi, kappa, &mu, &sd);
+    const double a = acq_value<double>(mun[ps[p]], varn[ps[p]], acq, ym, ys, yo, xi, kappa, &mu, &sd);
     if (a > bv || (bp == 0x7fffffff && a == a)) {   // positions only grow inside a thread: first maximum kept
       bv = a;
       bp = p;
@@ -601,11 +591,11 @@ refine_best_kernel(const double* __restrict__ mun, const double* __restrict__ va
     best->std = 0.0;
   }
   if (threadIdx.x == 0 && sp[0] != 0x7fffffff) {
-    const int p = sp[0];
+    const int q = ps[sp[0]];
     double mu, sd;
-    const double a = acq_value<double>(mun[p], varn[p], acq, ym, ys, yo, xi, kappa, &mu, &sd);
+    const double a = acq_value<double>(mun[q], varn[q], acq, ym, ys, yo, xi, kappa, &mu, &sd);
     best->value = a;
-    best->index = goff + list[p];
+    best->index = goff + uidx[q];
     best->mu = mu;
     best->std = sd;
   }
@@ -784,11 +774,106 @@ static cudaEvent_t* ev_pair(kbo_handle* h, std::vector<std::pair<cudaEvent_t, cu
 #define KBO_TIME_END()                                 \
   if (_ev) cudaEventRecord((&_ev[0])[1], s);
 
-// FP64 evaluation of the n contenders in list (sorted here) and the first-index argmax over them -> best_dev
 #define KBO_SOLVE_CAP 256   // survivors a lazy fit evaluates by triangular solves with L before it forms the rest of L⁻¹ instead
-static int refine_evaluate(kbo_handle* h, const void* Xc, int xc_dtype, int n, int* list, int* count, int64_t goff, kbo_best* best_dev, cudaStream_t s);
 
-static int refine_suggestion(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, kbo_best* best_dev, cudaStream_t s) {
+// One acquisition's way through the stages of a sweep.  kbo_sweep decides one; kbo_sweep_multi several over one posterior, each
+// leaving at the first stage where its own survivor list fits its cap — the stage its single sweep would have decided at.
+struct AcqDecision {
+  int acq;
+  kbo_best* best;
+  bool done;
+  int unrefined, contenders, prefix_survivors;   // what kbo_last_unrefined / _contenders / _prefix_survivors report for it
+};
+
+// The survivors of the acquisitions a stage decides, collected on the host (each list is read back once its count is known,
+// before the next acquisition reuses the device list) and evaluated together by refine_union.
+struct StagePicks {
+  int nk = 0;
+  AcqDecision* d[3];
+  std::vector<int> list[3];
+};
+static int take_list(kbo_handle* h, StagePicks& sp, AcqDecision& d, const int* list_dev, int n, cudaStream_t s) {
+  std::vector<int>& l = sp.list[sp.nk];
+  l.resize(n);
+  KBO_CUDA(h, cudaMemcpyAsync(l.data(), list_dev, sizeof(int) * (size_t)n, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  sp.d[sp.nk++] = &d;
+  return KBO_OK;
+}
+
+// FP64 decision of every acquisition in sp over the UNION of their survivor lists: K*, mean and variance of each union row are
+// evaluated once (a candidate's FP64 values depend on neither its position nor the number of rows evaluated with it — see
+// refine_var_kernel and the panel solves), then each acquisition takes the first-index argmax over its own survivors.  A lazy
+// fit evaluates the variance by panel solves with L in groups, whatever the union's size: it never forms W here.
+#define KBO_UNION_BATCH 4096   // union rows per K* / variance batch
+static int refine_union(kbo_handle* h, const void* Xc, int xc_dtype, int64_t goff, StagePicks& sp, cudaStream_t s) {
+  if (sp.nk == 0) return KBO_OK;
+  const int N = h->N, D = h->D, ld = h->ld;
+  std::vector<int> U;
+  for (int k = 0; k < sp.nk; k++) {
+    std::sort(sp.list[k].begin(), sp.list[k].end());   // ascending indices: first maximum = lowest index
+    U.insert(U.end(), sp.list[k].begin(), sp.list[k].end());
+  }
+  std::sort(U.begin(), U.end());
+  U.erase(std::unique(U.begin(), U.end()), U.end());
+  const int nu = (int)U.size();
+  UnionPick up{};
+  up.nk = sp.nk;
+  std::vector<int> host(U);   // [union indices][positions of acquisition 0][... 1][... 2]
+  for (int k = 0; k < sp.nk; k++) {
+    up.acq[k] = sp.d[k]->acq;
+    up.best[k] = sp.d[k]->best;
+    up.off[k] = (int)host.size() - nu;
+    up.n[k] = (int)sp.list[k].size();
+    for (int idx : sp.list[k]) host.push_back((int)(std::lower_bound(U.begin(), U.end(), idx) - U.begin()));
+  }
+  KBO_TRY(kbo_reserve(h, h->un_idx, sizeof(int) * host.size()));
+  KBO_TRY(kbo_reserve(h, h->un_mv, sizeof(double) * 2 * (size_t)nu));
+  int* uidx = (int*)h->un_idx.p;
+  double* mun64 = (double*)h->un_mv.p;
+  double* varn64 = mun64 + nu;
+  KBO_CUDA(h, cudaMemcpyAsync(uidx, host.data(), sizeof(int) * host.size(), cudaMemcpyHostToDevice, s));
+  const int njt = (N + 7) / 8;   // row blocks of refine_var_kernel (8 rows of W per CTA)
+  for (int b0 = 0; b0 < nu; b0 += KBO_UNION_BATCH) {
+    const int m = nu - b0 < KBO_UNION_BATCH ? nu - b0 : KBO_UNION_BATCH;
+    KBO_TRY(kbo_reserve(h, h->refine_x, sizeof(double) * (size_t)m * D));
+    KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)m * ld));
+    KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * (size_t)m * njt));
+    double* Xg = (double*)h->refine_x.p;
+    if (xc_dtype == KBO_F64)
+      gather_rows_kernel<double><<<m, 64, 0, s>>>((const double*)Xc, D, uidx + b0, m, Xg);
+    else
+      gather_rows_kernel<float><<<m, 64, 0, s>>>((const float*)Xc, D, uidx + b0, m, Xg);
+    KBO_LAUNCH_CHECK(h);
+    refine_cross_kernel<<<dim3((N + 255) / 256, m), 256, 0, s>>>(Xg, D, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(), (const double*)h->XsT.p, ld, N,
+                                                                 h->prm.kernel, h->prm.amplitude, (double*)h->Ks64.p);
+    KBO_LAUNCH_CHECK(h);
+    refine_mu_kernel<<<m, 256, 0, s>>>((const double*)h->Ks64.p, ld, N, (const double*)h->alpha.p, mun64 + b0);
+    KBO_LAUNCH_CHECK(h);
+    if (!h->w_full) {
+      // lazy inverse: ‖L⁻¹k*‖² by panel solves with the factor itself (solve.cu) — no W
+      KBO_TRY(kbo_i_variance_by_solves(h, (const double*)h->Ks64.p, m, varn64 + b0, s));
+    } else {
+      if (m <= 2)   // the usual case: one contender — no point carrying eight accumulators through the triangle of W
+        refine_var_kernel<1><<<dim3(njt, m), 256, 0, s>>>((const double*)h->W.p, ld, N, (const double*)h->Ks64.p, m, (double*)h->part.p, njt);
+      else
+        refine_var_kernel<8><<<dim3(njt, (m + 7) / 8), 256, 0, s>>>((const double*)h->W.p, ld, N, (const double*)h->Ks64.p, m, (double*)h->part.p, njt);
+      KBO_LAUNCH_CHECK(h);
+      var_from_parts_kernel<<<(m + 255) / 256, 256, 0, s>>>((const double*)h->part.p, m, njt, h->prm.amplitude, varn64 + b0);
+      KBO_LAUNCH_CHECK(h);
+    }
+  }
+  refine_best_union_kernel<<<sp.nk, 1024, 0, s>>>(mun64, varn64, uidx, uidx + nu, up, (const double*)h->scal.p, h->prm.xi, h->prm.kappa, goff);
+  KBO_LAUNCH_CHECK(h);
+  // the host copies above must outlive the asynchronous H2D copy
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  for (int k = 0; k < sp.nk; k++) sp.d[k]->done = true;
+  sp.nk = 0;
+  return KBO_OK;
+}
+
+// contenders of the three-product sweep's window (see below) for one acquisition; a list that fits is handed to sp
+static int refine_suggestion(kbo_handle* h, int64_t M, int64_t goff, AcqDecision& d, StagePicks& sp, cudaStream_t s) {
   const double* scal = (const double*)h->scal.p;
   KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
   int* list = (int*)h->refine.p;
@@ -801,67 +886,26 @@ static int refine_suggestion(kbo_handle* h, const void* Xc, int xc_dtype, int64_
   // which is then the lowest index among them, as the reference's argmin is.
   double delta = 2e-4;
   int n = 0, first_n = 0;
-  h->last_unrefined = 0;
+  d.unrefined = 0;
   for (int round = 0; round < 24; round++) {
     KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
-    contender_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, h->prm.acq, scal, h->prm.xi, h->prm.kappa,
-                                                    best_dev, goff, delta, list, count);
+    contender_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa,
+                                                    d.best, goff, delta, list, count);
     KBO_LAUNCH_CHECK(h);
     KBO_CUDA(h, cudaMemcpyAsync(&n, count, sizeof(int), cudaMemcpyDeviceToHost, s));
     KBO_CUDA(h, cudaStreamSynchronize(s));
     if (round == 0) first_n = n;
     if (n <= KBO_REFINE_CAP) break;
-    h->last_unrefined = 1;
+    d.unrefined = 1;
     delta = round < 22 ? delta * 0.25 : 0.0;   // the last attempt: exact ties of the maximum only
   }
-  h->last_contenders = first_n;
+  d.contenders = first_n;
   if (n < 1 || n > KBO_REFINE_CAP) {
-    h->last_unrefined = 2;
+    d.unrefined = 2;
+    d.done = true;   // keeps the tensor-core pick
     return KBO_OK;
   }
-  return refine_evaluate(h, Xc, xc_dtype, n, list, count, goff, best_dev, s);
-}
-
-static int refine_evaluate(kbo_handle* h, const void* Xc, int xc_dtype, int n, int* list, int* count, int64_t goff, kbo_best* best_dev, cudaStream_t s) {
-  const int N = h->N, D = h->D, ld = h->ld;
-  const double* scal = (const double*)h->scal.p;
-  if (n > 1) {   // a single contender needs no ordering
-    sort_contenders_kernel<<<1, 1024, 0, s>>>(list, count);
-    KBO_LAUNCH_CHECK(h);
-  }
-  const int njt = (N + 7) / 8;   // row blocks of refine_var_kernel (8 rows of W per CTA)
-  KBO_TRY(kbo_reserve(h, h->refine_x, sizeof(double) * (size_t)n * D));
-  KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)n * ld));
-  KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * ((size_t)n * njt + 2 * (size_t)n)));
-  double* Xg = (double*)h->refine_x.p;
-  double* mun64 = (double*)h->part.p + (size_t)n * njt;
-  double* varn64 = mun64 + n;
-  if (xc_dtype == KBO_F64)
-    gather_rows_kernel<double><<<n, 64, 0, s>>>((const double*)Xc, D, list, n, Xg);
-  else
-    gather_rows_kernel<float><<<n, 64, 0, s>>>((const float*)Xc, D, list, n, Xg);
-  KBO_LAUNCH_CHECK(h);
-  refine_cross_kernel<<<dim3((N + 255) / 256, n), 256, 0, s>>>(Xg, D, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(), (const double*)h->XsT.p, ld, N,
-                                                               h->prm.kernel, h->prm.amplitude, (double*)h->Ks64.p);
-  KBO_LAUNCH_CHECK(h);
-  refine_mu_kernel<<<n, 256, 0, s>>>((const double*)h->Ks64.p, ld, N, (const double*)h->alpha.p, mun64);
-  KBO_LAUNCH_CHECK(h);
-  if (!h->w_full && n <= KBO_SOLVE_CAP) {
-    // lazy inverse: ‖L⁻¹k*‖² by panel solves with the factor itself (solve.cu) — no W
-    KBO_TRY(kbo_i_variance_by_solves(h, (const double*)h->Ks64.p, n, varn64, s));
-  } else {
-    KBO_TRY(kbo_i_ensure_w(h, s));
-    if (n <= 2)   // the usual case: one contender — no point carrying eight accumulators through the triangle of W
-      refine_var_kernel<1><<<dim3(njt, n), 256, 0, s>>>((const double*)h->W.p, ld, N, (const double*)h->Ks64.p, n, (double*)h->part.p, njt);
-    else
-      refine_var_kernel<8><<<dim3(njt, (n + 7) / 8), 256, 0, s>>>((const double*)h->W.p, ld, N, (const double*)h->Ks64.p, n, (double*)h->part.p, njt);
-    KBO_LAUNCH_CHECK(h);
-    var_from_parts_kernel<<<(n + 255) / 256, 256, 0, s>>>((const double*)h->part.p, n, njt, h->prm.amplitude, varn64);
-    KBO_LAUNCH_CHECK(h);
-  }
-  refine_best_kernel<<<1, 1024, 0, s>>>(mun64, varn64, list, n, h->prm.acq, scal, h->prm.xi, h->prm.kappa, goff, best_dev);
-  KBO_LAUNCH_CHECK(h);
-  return KBO_OK;
+  return take_list(h, sp, d, list, n, s);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1134,11 +1178,11 @@ calib_prefix_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_
 // tiles) against the ranking arithmetic over the same prefix -> E, Emu.  Lower bound on the maximum: the sigma -> 0 limit of
 // the acquisition function over the whole grid (for EI: the largest predicted improvement) — free.  Candidates whose prefix
 // upper bound reaches it (normally a handful) are evaluated EXACTLY in FP64 by panel solves with L and the first-index
-// argmax is taken over those values: no ranking pass, no interval test.  *pruned = 0 (more than 256 such candidates, or no
-// usable lower bound): the caller forms the rest of W and runs the sweep of a full fit.
-static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int64_t chunk, kbo_best* best_dev, int* pruned,
+// argmax is taken over those values: no ranking pass, no interval test.  An acquisition left undecided (more than 256 such
+// candidates, or no usable lower bound) goes on to the caller, which forms the rest of W and runs the sweep of a full fit.
+// The grid pass is shared by every acquisition in dec[]; the bound, the survivor list and the FP64 decision are per kind.
+static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int64_t chunk, AcqDecision* dec, int n_acq,
                             cudaStream_t s) {
-  *pruned = 0;
   const int D = h->D, Npad = h->Npad;
   const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
   const double* scal = (const double*)h->scal.p;
@@ -1183,38 +1227,41 @@ static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
     }
   }
   KBO_TIME_BEGIN(ev_acq, ev_acq_used);
-  KBO_CUDA(h, cudaMemsetAsync(pcount, 0, sizeof(int), s));
-  grid_lower_bound_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs);
-  KBO_LAUNCH_CHECK(h);
-  prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
-                                                       pcount, KBO_PRUNE_CAP);
-  KBO_LAUNCH_CHECK(h);
-  struct { int n; int pad[3]; float fs[8]; } host;
-  int n1 = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(&n1, pcount, sizeof(int), cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));
-  h->last_prefix_survivors = n1;
-  h->last_rank_err = host.fs[2];
-  h->last_rank_mu_err = host.fs[4];
-  if (n1 < 1 || n1 > KBO_SOLVE_CAP) {
-    KBO_TIME_END();
-    return KBO_OK;
+  StagePicks sp;
+  for (int k = 0; k < n_acq; k++) {
+    AcqDecision& d = dec[k];
+    if (d.done) continue;
+    KBO_CUDA(h, cudaMemsetAsync(pcount, 0, sizeof(int), s));
+    KBO_CUDA(h, cudaMemsetAsync(fs + 1, 0, sizeof(float), s));   // this kind's lower bound starts below every ordered value
+    grid_lower_bound_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+    KBO_LAUNCH_CHECK(h);
+    prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
+                                                         pcount, KBO_PRUNE_CAP);
+    KBO_LAUNCH_CHECK(h);
+    struct { int n; int pad[3]; float fs[8]; } host;
+    int n1 = 0;
+    KBO_CUDA(h, cudaMemcpyAsync(&n1, pcount, sizeof(int), cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, cudaStreamSynchronize(s));
+    d.prefix_survivors = n1;
+    h->last_rank_err = host.fs[2];
+    h->last_rank_mu_err = host.fs[4];
+    if (n1 < 1 || n1 > KBO_SOLVE_CAP) continue;
+    d.contenders = n1;
+    d.unrefined = 0;
+    KBO_TRY(take_list(h, sp, d, plist, n1, s));
   }
-  h->last_contenders = n1;
-  h->last_unrefined = 0;
-  KBO_TRY(refine_evaluate(h, Xc, xc_dtype, n1, plist, pcount, goff, best_dev, s));
+  KBO_TRY(refine_union(h, Xc, xc_dtype, goff, sp, s));   // panel solves with L: the lazy fit stays lazy
   KBO_TIME_END();
-  *pruned = 1;
   return KBO_OK;
 }
 
 
-// The pruning sweep.  *pruned = 1: best_dev holds the FP64-decided suggestion.  *pruned = 0: too many candidates survive the
-// prefix bound (or the interval test) — the caller runs the full ranking pass; the calibration buffers stay valid for it.
-static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int cal_n, int64_t chunk, kbo_best* best_dev, int* pruned,
+// The pruning sweep.  An acquisition whose survivors fit (prefix bound, then interval test) is decided here in FP64 (done);
+// one with too many survivors goes on to the caller's full ranking pass; the calibration buffers stay valid for it.  The
+// calibration rows' ranking arithmetic and the grid pass are shared by every acquisition in dec[].
+static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int cal_n, int64_t chunk, AcqDecision* dec, int n_acq,
                        cudaStream_t s) {
-  *pruned = 0;
   const int D = h->D, Npad = h->Npad;
   const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
   const double* scal = (const double*)h->scal.p;
@@ -1237,9 +1284,6 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     // the ranking arithmetic on the calibration rows (all tile pairs): what E and Emu are measured from
     KBO_TRY(kbo_i_tc_kstar(h, h->cal_x.p, KBO_F64, cal_n, (__half*)h->Ksh.p, (float*)h->cal_mu_rk.p, s));
     KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, cal_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->cal_var_rk.p, s));
-    calib_lb_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p, cal_n,
-                                       h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs);
-    KBO_LAUNCH_CHECK(h);
     KBO_TIME_END();
   }
   // pass 1 over the grid: mean over all trials, variance bound from the first P1 tile pairs
@@ -1261,59 +1305,62 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     }
   }
   KBO_TIME_BEGIN(ev_acq, ev_acq_used);
-  KBO_CUDA(h, cudaMemsetAsync(pcount, 0, sizeof(int), s));
-  prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
-                                                       pcount, KBO_PRUNE_CAP);
-  KBO_LAUNCH_CHECK(h);
-  struct { int n; int pad[3]; float fs[8]; } host;
-  int n1 = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(&n1, pcount, sizeof(int), cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));
-  h->last_prefix_survivors = n1;
-  h->last_rank_err = host.fs[2];
-  h->last_rank_mu_err = host.fs[4];
-  if (n1 < 1 || n1 > KBO_PRUNE_CAP) {
-    KBO_TIME_END();
-    return KBO_OK;
+  StagePicks sp;
+  for (int k = 0; k < n_acq; k++) {
+    AcqDecision& d = dec[k];
+    if (d.done) continue;
+    // E, Emu and this kind's lower bound on the maximum from the calibration rows (one CTA over one wave of rows)
+    calib_lb_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p, cal_n,
+                                       d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+    KBO_LAUNCH_CHECK(h);
+    KBO_CUDA(h, cudaMemsetAsync(pcount, 0, sizeof(int), s));
+    prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
+                                                         pcount, KBO_PRUNE_CAP);
+    KBO_LAUNCH_CHECK(h);
+    struct { int n; int pad[3]; float fs[8]; } host;
+    int n1 = 0;
+    KBO_CUDA(h, cudaMemcpyAsync(&n1, pcount, sizeof(int), cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, cudaStreamSynchronize(s));
+    d.prefix_survivors = n1;
+    h->last_rank_err = host.fs[2];
+    h->last_rank_mu_err = host.fs[4];
+    if (n1 < 1 || n1 > KBO_PRUNE_CAP) continue;
+    // pass 2: the survivors' rows through the whole ranking pass, then the interval test and the FP64 decision
+    const int64_t n1_pad = round_up64(n1, 256);
+    KBO_TRY(kbo_reserve(h, h->pr_x, sizeof(double) * (size_t)n1_pad * D));
+    KBO_TRY(kbo_reserve(h, h->pr_mu, sizeof(float) * (size_t)(n1_pad + 256)));
+    KBO_TRY(kbo_reserve(h, h->pr_var, sizeof(float) * (size_t)(n1_pad + 256)));
+    if (xc_dtype == KBO_F64)
+      gather_rows_kernel<double><<<n1, 64, 0, s>>>((const double*)Xc, D, plist, n1, (double*)h->pr_x.p);
+    else
+      gather_rows_kernel<float><<<n1, 64, 0, s>>>((const float*)Xc, D, plist, n1, (double*)h->pr_x.p);
+    KBO_LAUNCH_CHECK(h);
+    KBO_TRY(kbo_i_tc_kstar(h, h->pr_x.p, KBO_F64, n1, (__half*)h->Ksh.p, (float*)h->pr_mu.p, s));
+    KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, n1_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->pr_var.p, s));
+    KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
+    const int g2 = (n1 + 255) / 256;
+    survivor_lb_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+    KBO_LAUNCH_CHECK(h);
+    survivor_final_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, plist, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs, list,
+                                             count);
+    KBO_LAUNCH_CHECK(h);
+    int n2 = 0;
+    KBO_CUDA(h, cudaMemcpyAsync(&n2, count, sizeof(int), cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, cudaStreamSynchronize(s));
+    d.contenders = n2;
+    if (n2 < 1 || n2 > KBO_REFINE_CAP) continue;
+    d.unrefined = 0;
+    KBO_TRY(take_list(h, sp, d, list, n2, s));
   }
-  // pass 2: the survivors' rows through the whole ranking pass, then the interval test and the FP64 decision
-  const int64_t n1_pad = round_up64(n1, 256);
-  KBO_TRY(kbo_reserve(h, h->pr_x, sizeof(double) * (size_t)n1_pad * D));
-  KBO_TRY(kbo_reserve(h, h->pr_mu, sizeof(float) * (size_t)(n1_pad + 256)));
-  KBO_TRY(kbo_reserve(h, h->pr_var, sizeof(float) * (size_t)(n1_pad + 256)));
-  if (xc_dtype == KBO_F64)
-    gather_rows_kernel<double><<<n1, 64, 0, s>>>((const double*)Xc, D, plist, n1, (double*)h->pr_x.p);
-  else
-    gather_rows_kernel<float><<<n1, 64, 0, s>>>((const float*)Xc, D, plist, n1, (double*)h->pr_x.p);
-  KBO_LAUNCH_CHECK(h);
-  KBO_TRY(kbo_i_tc_kstar(h, h->pr_x.p, KBO_F64, n1, (__half*)h->Ksh.p, (float*)h->pr_mu.p, s));
-  KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, n1_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->pr_var.p, s));
-  KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
-  const int g2 = (n1 + 255) / 256;
-  survivor_lb_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, n1, h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs);
-  KBO_LAUNCH_CHECK(h);
-  survivor_final_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, plist, n1, h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs, list,
-                                           count);
-  KBO_LAUNCH_CHECK(h);
-  int n2 = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(&n2, count, sizeof(int), cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));
-  h->last_contenders = n2;
-  if (n2 < 1 || n2 > KBO_REFINE_CAP) {
-    KBO_TIME_END();
-    return KBO_OK;
-  }
-  h->last_unrefined = 0;
-  KBO_TRY(refine_evaluate(h, Xc, xc_dtype, n2, list, count, goff, best_dev, s));
+  KBO_TRY(refine_union(h, Xc, xc_dtype, goff, sp, s));
   KBO_TIME_END();
-  *pruned = 1;
   return KBO_OK;
 }
 
-// returns KBO_OK with *overflow = 1 when the survivors do not fit (the caller redoes the sweep with three products)
-static int fast_pick(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int cal_n, kbo_best* best_dev, int* overflow,
-                     cudaStream_t s) {
+// The interval test of the full ranking pass for one acquisition; survivors that fit go to sp.  Not handed over: they do not
+// fit (the caller redoes the sweep with three products).
+static int fast_pick(kbo_handle* h, int64_t M, int cal_n, AcqDecision& d, StagePicks& sp, cudaStream_t s) {
   const double* scal = (const double*)h->scal.p;
   KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
   int* list = (int*)h->refine.p;
@@ -1323,21 +1370,20 @@ static int fast_pick(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int
   calib_kernel<<<1, 1024, 0, s>>>((const float*)h->varn.p, (const float*)h->var_cal.p, (const float*)h->mun.p, (const float*)h->cal_mu.p,
                                   (const int*)h->cal_idx.p, cal_n, fs);
   KBO_LAUNCH_CHECK(h);
-  bound_max_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs);
+  bound_max_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
   KBO_LAUNCH_CHECK(h);
-  survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, h->prm.acq, scal, h->prm.xi, h->prm.kappa, fs,
+  survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs,
                                                  list, count);
   KBO_LAUNCH_CHECK(h);
   struct { int n; int pad[3]; float fs[8]; } host;
   KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
-  h->last_contenders = host.n;
+  d.contenders = host.n;
   h->last_rank_err = host.fs[2];
   h->last_rank_mu_err = host.fs[4];
-  *overflow = (host.n < 1 || host.n > KBO_REFINE_CAP) ? 1 : 0;
-  if (*overflow) return KBO_OK;
-  h->last_unrefined = 0;
-  return refine_evaluate(h, Xc, xc_dtype, host.n, list, count, goff, best_dev, s);
+  if (host.n < 1 || host.n > KBO_REFINE_CAP) return KBO_OK;
+  d.unrefined = 0;
+  return take_list(h, sp, d, list, host.n, s);
 }
 
 // The stratified calibration rows of a ranking sweep through the FP64 K* kernel and the three-product contraction:
@@ -1371,7 +1417,7 @@ static int calibration_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
 }
 
 static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, double* mu_out, double* std_out, double* acq_out,
-                      kbo_best* best_dev, cudaStream_t s, bool force_three);
+                      AcqDecision* dec, int n_acq, cudaStream_t s, bool force_three);
 
 int kbo_i_debug_cross_planes(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, cudaStream_t s) {
   const int64_t rows_pad = round_up64(M, 128);
@@ -1380,13 +1426,49 @@ int kbo_i_debug_cross_planes(kbo_handle* h, const void* Xc, int xc_dtype, int64_
   return launch_cross<float, float, 1>(h, (const float*)Xc, M, rows_pad, nullptr, 0, (__half*)h->Ksh.p, (__half*)h->Ksl.p, (float*)h->mun.p, s);
 }
 
-int kbo_i_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, double* mu_out, double* std_out, double* acq_out,
-                kbo_best* best_dev, cudaStream_t s) {
-  return sweep_impl(h, Xc, xc_dtype, M, goff, mu_out, std_out, acq_out, best_dev, s, false);
+static void record_decisions(kbo_handle* h, const AcqDecision* dec, int n_acq) {
+  h->dec_n = n_acq;
+  for (int k = 0; k < n_acq; k++) {
+    h->dec_unrefined[k] = dec[k].unrefined;
+    h->dec_contenders[k] = dec[k].contenders;
+    h->dec_prefix_survivors[k] = dec[k].prefix_survivors;
+  }
 }
 
+int kbo_i_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, double* mu_out, double* std_out, double* acq_out,
+                kbo_best* best_dev, cudaStream_t s) {
+  AcqDecision d{h->prm.acq, best_dev, false, h->last_unrefined, h->last_contenders, h->last_prefix_survivors};
+  const int r = sweep_impl(h, Xc, xc_dtype, M, goff, mu_out, std_out, acq_out, &d, 1, s, false);
+  h->last_unrefined = d.unrefined;
+  h->last_contenders = d.contenders;
+  h->last_prefix_survivors = d.prefix_survivors;
+  record_decisions(h, &d, 1);
+  return r;
+}
+
+int kbo_i_sweep_multi(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int n_acq, const int32_t* acqs, kbo_best* best_dev,
+                      cudaStream_t s) {
+  if (n_acq < 1 || n_acq > 3) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep_multi: n_acq must be 1, 2 or 3 (got %d)", n_acq);
+  AcqDecision dec[3];
+  for (int k = 0; k < n_acq; k++) {
+    if (acqs[k] < KBO_ACQ_EI || acqs[k] > KBO_ACQ_PI) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep_multi: unknown acquisition %d", acqs[k]);
+    for (int j = 0; j < k; j++)
+      if (acqs[j] == acqs[k]) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep_multi: acquisition %d requested twice", acqs[k]);
+    dec[k] = AcqDecision{acqs[k], best_dev + k, false, 0, 0, -1};
+  }
+  const float rank_err = h->last_rank_err, rank_mu_err = h->last_rank_mu_err;   // kbo_last_* keep reporting the last kbo_sweep
+  const int r = sweep_impl(h, Xc, xc_dtype, M, goff, nullptr, nullptr, nullptr, dec, n_acq, s, false);
+  h->last_rank_err = rank_err;
+  h->last_rank_mu_err = rank_mu_err;
+  record_decisions(h, dec, n_acq);
+  return r;
+}
+
+// Every acquisition in dec[] that is not done yet is decided over ONE posterior: the calibration rows, the K* planes, the
+// contractions and the mean are computed once per stage and shared; the bounds, survivor lists and FP64 decisions are per kind.
+// Each kind leaves at the first stage where its own list fits its cap — where kbo_sweep with that kind alone would have.
 static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, double* mu_out, double* std_out, double* acq_out,
-                      kbo_best* best_dev, cudaStream_t s, bool force_three) {
+                      AcqDecision* dec, int n_acq, cudaStream_t s, bool force_three) {
   if (!h->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_sweep: call kbo_fit first");
   if (M < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep: M must be >= 1 (got %lld)", (long long)M);
   if (xc_dtype != KBO_F64 && xc_dtype != KBO_F32) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sweep: xc_dtype must be KBO_F64 or KBO_F32");
@@ -1446,13 +1528,18 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
     KBO_TRY(kbo_reserve(h, h->varn, sizeof(double) * (size_t)M));
   }
   h->tim.chunks = 0;
-  if (!force_three) h->last_prefix_survivors = -1;   // (a three-product redo keeps what the failed ranking attempt recorded)
+  auto all_done = [&]() {
+    for (int k = 0; k < n_acq; k++)
+      if (!dec[k].done) return false;
+    return true;
+  };
+  for (int k = 0; k < n_acq; k++)
+    if (!force_three && !dec[k].done) dec[k].prefix_survivors = -1;   // (a three-product redo keeps what the failed ranking attempt recorded)
   if (!h->w_full) {
     // a lazy fit: try the sweep that needs the leading rows of W only; anything else forms the rest first
     if (tc && rank_tc && h->rank_prefix != 0) {
-      int pruned = 0;
-      KBO_TRY(prune_sweep_lead(h, Xc, xc_dtype, M, goff, chunk, best_dev, &pruned, s));
-      if (pruned) return KBO_OK;
+      KBO_TRY(prune_sweep_lead(h, Xc, xc_dtype, M, goff, chunk, dec, n_acq, s));
+      if (all_done()) return KBO_OK;
       h->tim.chunks = 0;
     }
     KBO_TRY(kbo_i_ensure_w(h, s));
@@ -1463,9 +1550,8 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
     KBO_TIME_END();
   }
   if (rank_tc && h->rank_prefix != 0) {
-    int pruned = 0;
-    KBO_TRY(prune_sweep(h, Xc, xc_dtype, M, goff, cal_n, chunk, best_dev, &pruned, s));
-    if (pruned) return KBO_OK;
+    KBO_TRY(prune_sweep(h, Xc, xc_dtype, M, goff, cal_n, chunk, dec, n_acq, s));
+    if (all_done()) return KBO_OK;
     h->tim.chunks = 0;   // not prunable: the full ranking pass below starts over
   }
   for (int64_t c0 = 0; c0 < M; c0 += chunk) {
@@ -1528,23 +1614,88 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
   {
     KBO_TIME_BEGIN(ev_acq, ev_acq_used);
     if (fast) {
-      int overflow = 0;
-      KBO_TRY(fast_pick(h, Xc, xc_dtype, M, goff, cal_n, best_dev, &overflow, s));
+      StagePicks sp;
+      for (int k = 0; k < n_acq; k++)
+        if (!dec[k].done) KBO_TRY(fast_pick(h, M, cal_n, dec[k], sp, s));
+      KBO_TRY(refine_union(h, Xc, xc_dtype, goff, sp, s));
       KBO_TIME_END();
-      if (overflow) return sweep_impl(h, Xc, xc_dtype, M, goff, mu_out, std_out, acq_out, best_dev, s, true);
+      // the kinds whose survivors overflowed: one three-product sweep for all of them
+      if (!all_done()) return sweep_impl(h, Xc, xc_dtype, M, goff, mu_out, std_out, acq_out, dec, n_acq, s, true);
       return KBO_OK;
     }
-    if (tc) {
-      KBO_TRY(launch_acq<float>(h, (const float*)h->mun.p, (const float*)h->varn.p, M, goff, h->prm.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
-                                h->prm.kappa, mu_out, std_out, acq_out, nullptr, best_dev, s));
-      h->last_unrefined = 2;
-      if (h->tc_refine && M < 0x7fffffff) KBO_TRY(refine_suggestion(h, Xc, xc_dtype, M, goff, best_dev, s));
-    } else {
-      h->last_unrefined = 0;
-      KBO_TRY(launch_acq<double>(h, (const double*)h->mun.p, (const double*)h->varn.p, M, goff, h->prm.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
-                                 h->prm.kappa, mu_out, std_out, acq_out, nullptr, best_dev, s));
+    StagePicks sp;
+    for (int k = 0; k < n_acq; k++) {
+      AcqDecision& d = dec[k];
+      if (d.done) continue;
+      if (tc) {
+        KBO_TRY(launch_acq<float>(h, (const float*)h->mun.p, (const float*)h->varn.p, M, goff, d.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
+                                  h->prm.kappa, mu_out, std_out, acq_out, nullptr, d.best, s));
+        d.unrefined = 2;
+        if (h->tc_refine && M < 0x7fffffff)
+          KBO_TRY(refine_suggestion(h, M, goff, d, sp, s));
+        else
+          d.done = true;
+      } else {
+        d.unrefined = 0;
+        KBO_TRY(launch_acq<double>(h, (const double*)h->mun.p, (const double*)h->varn.p, M, goff, d.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
+                                   h->prm.kappa, mu_out, std_out, acq_out, nullptr, d.best, s));
+        d.done = true;
+      }
     }
+    KBO_TRY(refine_union(h, Xc, xc_dtype, goff, sp, s));
     KBO_TIME_END();
   }
+  return KBO_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// FP64 posterior mean at a few points, raw y scale: the refinement's K* row and fixed-order mean (refine_cross_kernel,
+// refine_mu_kernel) — alpha only, never W, so a lazy fit stays lazy.  What gp_hedge's gains update reads at the last picks.
+template <typename XT>
+__global__ void rows_to_f64_kernel(const XT* __restrict__ X, int64_t n, int D, double* __restrict__ out) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e < n * D) out[e] = (double)X[e];
+}
+__global__ void raw_mean_kernel(const double* __restrict__ mun, int n, const double* __restrict__ scal, double* __restrict__ mu) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) mu[i] = scal[S_YSTD] * mun[i] + scal[S_YMEAN];   // as acq_value forms μ
+}
+
+int kbo_i_predict_mean(kbo_handle* h, const void* X, int x_dtype, int n, double* mu_host, cudaStream_t s) {
+  if (!h->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_predict_mean: call kbo_fit first");
+  if (x_dtype != KBO_F64 && x_dtype != KBO_F32) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_predict_mean: xc_dtype must be KBO_F64 or KBO_F32");
+  if (h->D > 256) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_predict_mean: D <= 256 supported (got %d)", h->D);
+  const int N = h->N, D = h->D, ld = h->ld;
+  const int B = n < 1024 ? n : 1024;   // rows per batch: K* scratch of B × ld doubles
+  KBO_TRY(kbo_reserve(h, h->refine_x, sizeof(double) * (size_t)B * D));
+  KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)B * ld));
+  KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * 2 * (size_t)B));
+  double* Xg = (double*)h->refine_x.p;
+  double* mun = (double*)h->part.p;
+  double* mu = mun + B;
+  const size_t esz = x_dtype == KBO_F64 ? 8 : 4;
+  for (int r0 = 0; r0 < n; r0 += B) {
+    const int m = n - r0 < B ? n - r0 : B;
+    const unsigned char* x = (const unsigned char*)X + (size_t)r0 * D * esz;
+    const unsigned g = (unsigned)(((int64_t)m * D + 255) / 256);
+    if (x_dtype == KBO_F64)
+      rows_to_f64_kernel<double><<<g, 256, 0, s>>>((const double*)x, m, D, Xg);
+    else
+      rows_to_f64_kernel<float><<<g, 256, 0, s>>>((const float*)x, m, D, Xg);
+    KBO_LAUNCH_CHECK(h);
+    refine_cross_kernel<<<dim3((N + 255) / 256, m), 256, 0, s>>>(Xg, D, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(), (const double*)h->XsT.p, ld, N,
+                                                                 h->prm.kernel, h->prm.amplitude, (double*)h->Ks64.p);
+    KBO_LAUNCH_CHECK(h);
+    refine_mu_kernel<<<m, 256, 0, s>>>((const double*)h->Ks64.p, ld, N, (const double*)h->alpha.p, mun);
+    KBO_LAUNCH_CHECK(h);
+    raw_mean_kernel<<<(m + 255) / 256, 256, 0, s>>>(mun, m, (const double*)h->scal.p, mu);
+    KBO_LAUNCH_CHECK(h);
+    KBO_CUDA(h, cudaMemcpyAsync(mu_host + r0, mu, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, cudaStreamSynchronize(s));
+  }
+  int inf = 0;
+  KBO_CUDA(h, cudaMemcpyAsync(&inf, h->info.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (inf != 0) KBO_FAIL(h, KBO_ERR_NOT_PD, "kernel matrix is not positive definite (pivot %d); increase `noise`", inf);
   return KBO_OK;
 }

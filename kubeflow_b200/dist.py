@@ -24,12 +24,17 @@ class RankFailure(RuntimeError):
     """A rank's local sweep failed; raised on EVERY rank after the exchange so nobody is left waiting in a collective."""
 
 
-def global_argmax(best: Best | None, group=None, device=None, failed: str | None = None) -> Best:
+def global_argmax(best: Best | list[Best] | None, group=None, device=None, failed: str | None = None, n: int | None = None):
     """Combine per-rank Bests into the global first-index argmax with ONE collective: an all-gather of 5 doubles per rank
     (value, index, mu, std, failed flag); every rank then takes the maximum value, lowest global index among equals —
     exactly ``np.argmin(-values)`` over the concatenated grid.  Indices up to 2^53 are exact in a double.
+    ``best`` may also be a list of Bests — one per acquisition of a multi-acquisition sweep, in the same order on every
+    rank — and a list of global Bests is returned, still from ONE all-gather (5 doubles per entry and rank).  ``n``: the
+    list's length, needed when this rank has no list to give (``failed``).
     ``failed``: a rank whose local sweep raised still JOINS the collective (with −inf and the flag set) and all ranks raise
     ``RankFailure`` together — a rank-local CUDA / not-PD error must not leave the others blocked in the all-gather."""
+    multi = isinstance(best, list) or n is not None
+    k = (len(best) if isinstance(best, list) else int(n)) if multi else 1
     if not dist.is_initialized() or dist.get_world_size(group) == 1:
         if failed:
             raise RankFailure(failed)
@@ -38,15 +43,21 @@ def global_argmax(best: Best | None, group=None, device=None, failed: str | None
     if device is None:
         device = torch.device("cuda", torch.cuda.current_device()) if dist.get_backend(group) == "nccl" else torch.device("cpu")
     if failed or best is None:
-        mine = torch.tensor([float("-inf"), float(2 ** 52), 0.0, 0.0, 1.0], dtype=torch.float64, device=device)
+        mine = torch.tensor([float("-inf"), float(2 ** 52), 0.0, 0.0, 1.0] * k, dtype=torch.float64, device=device)
     else:
-        v = best.value if best.value == best.value else float("-inf")   # NaN never wins
-        mine = torch.tensor([v, float(best.index), best.mu, best.std, 0.0], dtype=torch.float64, device=device)
-    allv = torch.empty(world * 5, dtype=torch.float64, device=device)
+        rows = []
+        for b in (best if multi else [best]):
+            v = b.value if b.value == b.value else float("-inf")   # NaN never wins
+            rows += [v, float(b.index), b.mu, b.std, 0.0]
+        mine = torch.tensor(rows, dtype=torch.float64, device=device)
+    allv = torch.empty(world * 5 * k, dtype=torch.float64, device=device)
     dist.all_gather_into_tensor(allv, mine, group=group)
-    rows = allv.view(world, 5).cpu().tolist()
-    bad = [r for r, row in enumerate(rows) if row[4] != 0.0]
+    table = allv.view(world, k, 5).cpu().tolist()
+    bad = [r for r, rk in enumerate(table) if any(row[4] != 0.0 for row in rk)]
     if bad:
         raise RankFailure(f"local sweep failed on rank(s) {bad}" + (f": {failed}" if failed else ""))
-    win = max(rows, key=lambda r: (r[0], -r[1]))
-    return Best(float(win[0]), int(win[1]), float(win[2]), float(win[3]))
+    out = []
+    for j in range(k):
+        win = max((table[r][j] for r in range(world)), key=lambda r: (r[0], -r[1]))
+        out.append(Best(float(win[0]), int(win[1]), float(win[2]), float(win[3])))
+    return out if multi else out[0]

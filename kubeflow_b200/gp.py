@@ -271,20 +271,7 @@ class GPEngine:
         """Sweep the candidate grid; returns Best (and mu/std/acq float64 CUDA tensors if asked).  ``allreduce``: combine the
         ranks' results into the global first-index argmax inside libkbo (kbo_allreduce_argmax; needs ``comm_init``)."""
         dev = f"cuda:{self.device}"
-        if isinstance(Xc, torch.Tensor):
-            if not Xc.is_cuda or Xc.dtype not in (torch.float64, torch.float32):
-                raise ValueError("candidate tensor must be a float64/float32 CUDA tensor")
-            Xc = Xc.contiguous()
-            M, D = Xc.shape
-            ptr, on_host = Xc.data_ptr(), 0
-            dt = L.KBO_F64 if Xc.dtype == torch.float64 else L.KBO_F32
-        else:
-            Xc = np.ascontiguousarray(Xc)
-            if Xc.dtype not in (np.float64, np.float32):
-                Xc = Xc.astype(np.float64)
-            M, D = Xc.shape
-            ptr, on_host = Xc.ctypes.data, 1
-            dt = L.KBO_F64 if Xc.dtype == np.float64 else L.KBO_F32
+        ptr, on_host, dt, M, D, Xc = self._rows(Xc)
         if self.N == 0:
             raise L.KboError(L.KBO_ERR_STATE, "ask() before tell(): call tell(X, y) first")
         if D != self.D:
@@ -307,6 +294,68 @@ class GPEngine:
             L.check(self.lib, self._h, rc)
         best = Best(b.value, int(b.index), b.mu, b.std)
         return (best, mu, std, acq) if return_arrays else best
+
+    def _rows(self, X):
+        """(pointer, on_host, dtype code, rows, keep-alive) of a candidate / point matrix: NumPy or a CUDA tensor."""
+        if isinstance(X, torch.Tensor):
+            if not X.is_cuda or X.dtype not in (torch.float64, torch.float32):
+                raise ValueError("candidate tensor must be a float64/float32 CUDA tensor")
+            X = X.contiguous()
+            M, D = X.shape
+            return X.data_ptr(), 0, L.KBO_F64 if X.dtype == torch.float64 else L.KBO_F32, M, D, X
+        X = np.ascontiguousarray(X)
+        if X.dtype not in (np.float64, np.float32):
+            X = X.astype(np.float64)
+        M, D = X.shape
+        return X.ctypes.data, 1, L.KBO_F64 if X.dtype == np.float64 else L.KBO_F32, M, D, X
+
+    def ask_multi(self, Xc, acqs, global_offset: int = 0):
+        """Sweep the candidate grid once for several acquisitions (kbo_sweep_multi): one Best per entry of ``acqs`` (1-3
+        distinct names of "ei", "lcb", "pi"), each what ``ask`` with that acquisition returns on the same fit and grid."""
+        ptr, on_host, dt, M, D, keep = self._rows(Xc)
+        if self.N == 0:
+            raise L.KboError(L.KBO_ERR_STATE, "ask_multi() before tell(): call tell(X, y) first")
+        if D != self.D:
+            raise ValueError(f"candidates have D={D}, fit had D={self.D}")
+        for a in acqs:
+            if a not in L.ACQS:
+                raise ValueError(f"acq must be one of {sorted(L.ACQS)}, got {a!r}")
+        n = len(acqs)
+        kinds = (C.c_int32 * max(n, 1))(*[L.ACQS[a] for a in acqs])
+        out = torch.empty(4 * max(n, 1), dtype=torch.float64, device=f"cuda:{self.device}")
+        with torch.cuda.device(self.device):
+            rc = self.lib.kbo_sweep_multi(self._h, ptr, dt, int(M), int(global_offset), on_host, int(n), kinds, out.data_ptr(), self._stream())
+            L.check(self.lib, self._h, rc)
+            bests = []
+            for i in range(n):
+                b = L.KboBest()
+                L.check(self.lib, self._h, self.lib.kbo_best_to_host(self._h, out.data_ptr() + 32 * i, C.byref(b), self._stream()))
+                bests.append(Best(b.value, int(b.index), b.mu, b.std))
+        del keep
+        return bests
+
+    def last_decisions(self):
+        """Per acquisition of the last ask / ask_multi: (unrefined, contenders, prefix survivors) as kbo_last_unrefined,
+        kbo_last_contenders and kbo_last_prefix_survivors report them for a single sweep."""
+        u, c, p = (C.c_int32 * 3)(), (C.c_int32 * 3)(), (C.c_int32 * 3)()
+        n = self.lib.kbo_last_decisions(self._h, 3, u, c, p)
+        if n < 0:
+            L.check(self.lib, self._h, n)
+        return [(int(u[i]), int(c[i]), int(p[i])) for i in range(n)]
+
+    def predict_mean(self, X) -> np.ndarray:
+        """FP64 posterior mean (raw y scale) at the rows of X (kbo_predict_mean; does not form a lazy fit's inverse)."""
+        ptr, on_host, dt, n, D, keep = self._rows(np.atleast_2d(X) if not isinstance(X, torch.Tensor) else X)
+        if self.N == 0:
+            raise L.KboError(L.KBO_ERR_STATE, "predict_mean() before tell(): call tell(X, y) first")
+        if D != self.D:
+            raise ValueError(f"points have D={D}, fit had D={self.D}")
+        mu = np.empty(n, dtype=np.float64)
+        with torch.cuda.device(self.device):
+            rc = self.lib.kbo_predict_mean(self._h, ptr, dt, int(n), on_host, mu.ctypes.data, self._stream())
+        L.check(self.lib, self._h, rc)
+        del keep
+        return mu
 
     # -- one call, host buffers (the end-to-end entry bench.py times) -------------------------------
     def suggest_host(self, X, y, Xc, global_offset: int = 0):

@@ -11,15 +11,36 @@ requested assignment).  Differences, stated once:
   with SciPy's L-BFGS-B exactly as sklearn does ($SK/_gpr.py:658-667), every objective/gradient evaluation being one
   device fit + ``kbo_lml_grad`` (SURVEY.md §8(f)1).
 * ``acq_optimizer`` is "sampling" over ``n_points`` candidates (skopt default 10 000; here 65 536 by default and
-  millions are cheap) — ``lbfgs`` polishing and ``gp_hedge`` are accepted by ValidateAlgorithmSettings and mapped to
-  sampling / EI.
+  millions are cheap) — ``lbfgs`` polishing is accepted by ValidateAlgorithmSettings and mapped to sampling; ``EIps`` /
+  ``PIps`` (they need a second model of the trial durations) are mapped to EI / PI.
 * ``ask(n_points=k)`` uses skopt's constant-liar "cl_min" strategy: k sequential asks with the lie y = min(y).
+
+``acq_func="gp_hedge"`` (Katib's and skopt's default) is skopt's portfolio: every model-based ask sweeps ONE candidate set
+for EI, LCB and PI together (``GPEngine.ask_multi``: one posterior, three first-index argmaxes), keeps the three picks, and
+draws which one to suggest from softmax(η·gains), η = 1.  When the history has changed, the next model-based ask first
+subtracts the new model's posterior mean (raw y scale, ``GPEngine.predict_mean``) at the previous three picks from the
+gains — skopt's ``gains_ -= est.predict(vstack(next_xs_))``, a pick that turned out well predicted low gaining most.
+Here ``tell`` is lazy and the work happens in ``ask``, so:
+
+* the gains advance once per change of the told history: on the first model-based ask after new trials, with the picks
+  of the last sweep on the told history; an ask with no new trials leaves them alone;
+* during the ``n_initial_points`` random phase there are no gains updates and no picks;
+* in ``ask(n_points=k)`` the first point is the told-history step; points 2..k come from the lie-extended histories with a
+  scratch copy of the gains that advances once per lie, as the copy skopt's ``ask`` works on does — the real gains never
+  see a lie;
+* the draw uses ``self.rng`` (a NumPy Generator), so every rank of a sharded optimizer draws the same.
+
+Against skopt's gp_hedge, besides the fixed θ and the candidate count above: the draw comes from a NumPy Generator, not
+a RandomState, and the first point of a batch is the told-history step's draw, where skopt redraws it on its copy.
 """
 from __future__ import annotations
 
 import numpy as np
 
 from .space import Space
+
+
+HEDGE_ACQS = ("ei", "lcb", "pi")   # skopt's cand_acq_funcs_ = ["EI", "LCB", "PI"]
 
 
 class Optimizer:
@@ -35,6 +56,15 @@ class Optimizer:
         self.acq = {"EI": "ei", "LCB": "lcb", "PI": "pi", "gp_hedge": "ei", "EIps": "ei", "PIps": "pi"}.get(acq)
         if self.acq is None:
             raise ValueError(f"unknown acq_func {acq_func!r}")
+        # gp_hedge portfolio state (host-only: constructing a hedge optimizer touches no device)
+        self.hedge = acq == "gp_hedge"
+        self.eta = 1.0
+        self.gains = np.zeros(len(HEDGE_ACQS)) if self.hedge else None
+        self.next_xs = None           # transformed rows of the last told-history sweep's EI / LCB / PI picks
+        self._hedge_hist = None       # (Xt, y) those picks were made on
+        self._lie_gains = self._lie_next_xs = None   # scratch state of the lies of one ask(n_points=k)
+        self._last_gp = False         # the last _ask_one was model-based
+        self.last_hedge = None        # (Bests of EI / LCB / PI, probabilities, index drawn) of the last hedge ask
         if acq_optimizer not in ("auto", "sampling", "lbfgs"):
             raise ValueError(f"unknown acq_optimizer {acq_optimizer!r}")
         self.rng = np.random.default_rng(random_state)
@@ -150,9 +180,23 @@ class Optimizer:
     def _default_ls(self):
         return 0.3 * np.sqrt(self.space.transformed_n_dims) if self.length_scale is None else self.length_scale
 
+    def _hedge_gains(self, eng, Xt, ya, lie):
+        """The gains the draw of this ask uses, advanced where skopt's tell would advance them.  Nothing is stored here:
+        _hedge_pick commits them together with the new picks once the sweep has succeeded, so an ask that fails cannot
+        subtract the same picks twice."""
+        if lie:
+            prev, base = self._lie_next_xs, self._lie_gains
+        else:
+            h = self._hedge_hist
+            changed = h is None or h[0].shape != Xt.shape or not (np.array_equal(h[0], Xt) and np.array_equal(h[1], ya))
+            prev, base = (self.next_xs if changed else None), self.gains
+        return base if prev is None else base - eng.predict_mean(prev)
+
     def _ask_one(self, X, y):
         if len(y) < max(self.n_initial_points, 1):
+            self._last_gp = False
             return self.space.inverse_transform(self.space.rvs_transformed(1, self.rng, np.float64))[0]
+        self._last_gp = True
         n_told = len(self._Xt)
         Xt = self._Xt
         if len(X) > n_told:          # constant-liar rows appended by ask(n_points=k)
@@ -212,6 +256,7 @@ class Optimizer:
             eng.length_scale, eng.noise = np.exp(res.x[:-1]), float(np.exp(res.x[-1]))
             self.last_theta = dict(length_scale=eng.length_scale.copy(), noise=eng.noise, lml=-float(res.fun), nfev=int(res.nfev))
         self._tell_engine(eng, Xt, ya)
+        lie = len(X) > n_told
         rank, world = self._world() if self.shard else (0, 1)
         from .dist import global_argmax, shard_rows
         if world > 1 and self.n_points < world:     # identical on every rank, before any collective: all raise together
@@ -229,6 +274,8 @@ class Optimizer:
             if self._crng is None:
                 self._crng = self.rng if world == 1 else np.random.default_rng([int(self._seed), rank])
             cand = self.space.rvs_transformed(hi - lo, self._crng, np.float32)
+        if self.hedge:
+            return self._hedge_pick(eng, cand, lo, rank, world, lie, Xt, ya)
         failed = None
         try:
             best = self._sweep(eng, cand, lo)
@@ -259,12 +306,64 @@ class Optimizer:
         self.last_best = best
         return self.space.inverse_transform(row)[0]
 
+    def _hedge_pick(self, eng, cand, lo, rank, world, lie, Xt, ya):
+        """One sweep for EI, LCB and PI over the candidate set, the draw among the three picks, and the picks kept for the next
+        gains update.  Sharded: one all-gather for the three winners, one all-reduce that gives every rank all three rows."""
+        from .dist import global_argmax, shard_rows
+        failed = None
+        try:
+            gains = self._hedge_gains(eng, Xt, ya, lie)
+            local = eng.ask_multi(cand, list(HEDGE_ACQS), global_offset=lo)
+        except Exception as e:  # noqa: BLE001
+            self._fit_state = None      # e.g. an appended row made K singular: the next ask must refit from the history
+            if world == 1:
+                raise
+            local, failed = None, f"{type(e).__name__}: {e}"   # still join the exchange: every rank raises there, none hangs
+        self.last_local_best = local
+        Dt = self.space.transformed_n_dims
+        if world > 1:
+            import torch
+            import torch.distributed as dist
+            cdev = torch.device("cuda", self.device) if dist.get_backend() == "nccl" else torch.device("cpu")
+            bests = global_argmax(local, device=cdev, failed=failed, n=len(HEDGE_ACQS))
+            rows = torch.zeros((len(HEDGE_ACQS), Dt), dtype=torch.float64, device=cdev)
+            hi = shard_rows(self.n_points, rank, world)[1]
+            for j, b in enumerate(bests):   # each winner's owner fills its row; the sum hands every rank all three
+                if lo <= b.index < hi:
+                    src = cand[b.index - lo]
+                    rows[j].copy_((src if isinstance(src, torch.Tensor) else torch.from_numpy(np.asarray(src))).to(torch.float64))
+            dist.all_reduce(rows)
+            picks = rows.cpu().numpy()
+        else:
+            bests = local
+            li = [b.index - lo for b in bests]
+            if self.candidate_backend == "torch":
+                import torch
+                picks = cand[torch.tensor(li, device=cand.device)].to(torch.float64).cpu().numpy()
+            else:
+                picks = np.asarray(cand[li], dtype=np.float64)
+        logits = gains - np.max(gains)
+        probs = np.exp(self.eta * logits)
+        probs /= probs.sum()
+        j = int(np.argmax(self.rng.multinomial(1, probs)))
+        if lie:
+            self._lie_gains, self._lie_next_xs = gains, picks
+        else:
+            self.gains, self.next_xs = gains, picks
+            self._hedge_hist = (np.array(Xt, dtype=np.float64, copy=True), np.array(ya, dtype=np.float64, copy=True))
+        self.last_hedge = (bests, probs, j)
+        self.last_best = bests[j]
+        return self.space.inverse_transform(picks[j:j + 1])[0]
+
     def ask(self, n_points=None):
         if n_points is None:
             return self._ask_one(self.Xi, self.yi)
         X, y, out = list(self.Xi), list(self.yi), []
-        for _ in range(int(n_points)):
+        for i in range(int(n_points)):
             x = self._ask_one(X, y)
+            if i == 0 and self.hedge:   # the lies work on a copy of the gains, starting from this step's picks
+                self._lie_gains = self.gains.copy()
+                self._lie_next_xs = self.next_xs if self._last_gp else None
             out.append(x)
             if y:                      # constant liar, "cl_min"
                 X.append(x)
