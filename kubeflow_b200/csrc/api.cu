@@ -512,4 +512,16 @@ int kbo_debug_rank_pass(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t
   return KBO_OK;
 }
 
+// Test hook (not in kbo.h): the tensor-core K* kernel alone over M candidates (device pointer), writing straight into caller-owned
+// DEVICE buffers: mun_out (rows_pad floats) and plane_out (rows_pad × Npad fp16), rows_pad = M rounded up to 256.  store_cols < 0
+// stores every column; otherwise only the 128-column tiles covering the first store_cols, and the rest of plane_out is not written.
+int kbo_debug_kstar(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, int32_t store_cols, float* mun_out, void* plane_out, void* stream) {
+  if (!h) return KBO_ERR_INVALID;
+  if (!Xc || !mun_out || !plane_out || M < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_kstar: bad argument");
+  if (!h->fitted || !h->ks_ready) KBO_FAIL(h, KBO_ERR_STATE, "kbo_debug_kstar: needs a fit with tensor-core K* operands (D <= 128)");
+  cudaSetDevice(h->device);
+  KBO_TRY(kbo_i_tc_kstar(h, Xc, xc_dtype, M, (__half*)plane_out, mun_out, (cudaStream_t)stream, store_cols));
+  return KBO_OK;
+}
+
 }  // extern "C"

@@ -70,6 +70,22 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                "l"(map), "r"(bar), "r"(c0), "r"(c1)
                : "memory");
 }
+// plain bulk copy (no tensor map): `bytes` contiguous bytes, 16-byte aligned at both ends, counted on `bar` like a TMA tile
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes),
+               "r"(bar)
+               : "memory");
+}
+// LDS.128: the dynamic shared-memory base is realigned through an integer, so plain dereferences would compile to generic loads.
+// Volatile keeps it after the barrier waits (also volatile asm); no memory clobber, so global stores may move around it.
+__device__ __forceinline__ float4 lds128(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+// named barriers 1..15 (0 is __syncthreads): `n` threads in all, a multiple of 32, each either syncing (waits) or arriving (does not)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t n) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 __device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, uint16_t mask) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;" ::"r"(dst),

@@ -9,16 +9,18 @@
 // products are accumulated in fp32 (small ones first), so c·x carries ~1e-7 relative error — the kernel value is then
 // evaluated in fp32 (MUFU sqrt / ex2) per element by the epilogue warps, written ONCE as the fp16 hi plane the ranking kernel
 // consumes (no lo plane, no FP64), and the normalised mean μ̃ = Σ_n K̃*[m,n]·alpha[n] is accumulated on the fly (four fp32 FMA
-// chains of four trials, summed and added in FP64 once per 16 trials).  Both μ̃ and the variance built from this plane are only used to RANK: their error
+// chains, two per row, summed and added in FP64 once per 128-trial tile).  Both μ̃ and the variance built from this plane are only used to RANK: their error
 // is measured per sweep on stratified calibration rows against the FP64 path and every candidate that could still be the
 // maximum is re-evaluated in FP64 (sweep.cu).
 //
 // CTA = 128 candidate rows; it walks all 128-trial tiles.  Candidate planes (128 × Dp, hi and lo) stay in shared memory; trial
-// planes stream through a 4-stage TMA ring one 32-feature slab at a time (SWIZZLE_64B);
+// planes stream through a 4-stage TMA ring one 32-feature slab at a time (SWIZZLE_64B), and each tile's (|x̂|², alpha) pairs (1 KB)
+// arrive on the same barrier as its first slab, in a ring of their own, so the epilogue reads them with LDS;
 //   warps 0-7  two consumer warpgroups (rows 64·wg …): per (tile, slab) 2 k-steps × 4 products of wgmma m64n128k16 into 64 fp32
 //              registers, then the epilogue on those registers: d² → kernel → fp16 K* plane; μ̃ partials
 //   warp 8     TMA producer
-// The epilogue (~12 instructions and 2 MUFU per element) is the limiter; the MMAs take a fraction of that.
+// The epilogue (~12 instructions and 2 MUFU per element) is the limiter; the MMAs take a fraction of that.  Tiles a pruning pass
+// does not store run a body without the conversions, addresses and stores.
 #include "kbo_internal.cuh"
 #include <type_traits>
 
@@ -34,6 +36,7 @@
 #define KS_B_PLANE_BYTES (KS_BN * KS_BK * 2)    // 8 KB
 #define KS_STAGE_BYTES (2 * KS_B_PLANE_BYTES)   // hi + lo
 #define KS_MAX_SLABS 4                          // D <= 128
+#define KS_NX_BYTES (KS_BN * 8)                 // 1 KB: one tile's (|x̂|², alpha) pairs, loaded with its first slab
 
 namespace {
 using namespace tcx;
@@ -44,7 +47,9 @@ struct KsSmem {
   uint64_t a_full;
 };
 
-static size_t ks_smem_bytes(int ns) { return 1024 + (size_t)ns * 2 * KS_A_PLANE_BYTES + (size_t)KS_STAGES * KS_STAGE_BYTES + 256; }
+static size_t ks_smem_bytes(int ns) {
+  return 1024 + (size_t)ns * 2 * KS_A_PLANE_BYTES + (size_t)KS_STAGES * (KS_STAGE_BYTES + KS_NX_BYTES) + 256;
+}
 
 __device__ __forceinline__ float ex2_ftz(float x) {
   float r;
@@ -74,13 +79,14 @@ template <int KIND>
 __global__ void __launch_bounds__(KS_THREADS, 1)
 tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant__ CUtensorMap tmCl, const __grid_constant__ CUtensorMap tmXh,
                 const __grid_constant__ CUtensorMap tmXl, int ns, int ntiles, int N, const float* __restrict__ ncand,
-                const float4* __restrict__ nxal4 /* (|x̂_n|², alpha_n) pairs, two trials per float4 */, float log2amp,
-                __half* __restrict__ Ksh, int Npad, float* __restrict__ mun, int store_tiles /* trial tiles whose K* columns are written */) {
+                const float4* __restrict__ nxal4 /* (|x̂_n|², alpha_n) pairs, two trials per float4 */, int nx_tiles /* tiles that have pairs */,
+                float log2amp, __half* __restrict__ Ksh, int Npad, float* __restrict__ mun, int store_tiles /* trial tiles whose K* columns are written */) {
   extern __shared__ unsigned char ks_smem_raw[];
   unsigned char* base = (unsigned char*)(((uintptr_t)ks_smem_raw + 1023) & ~(uintptr_t)1023);
   unsigned char* smA = base;                                            // [ns][hi 8 KB | lo 8 KB]
   unsigned char* ring = smA + (size_t)ns * 2 * KS_A_PLANE_BYTES;        // [KS_STAGES][hi 8 KB | lo 8 KB]
-  KsSmem* S = (KsSmem*)(ring + KS_STAGES * KS_STAGE_BYTES);
+  unsigned char* nxs = ring + KS_STAGES * KS_STAGE_BYTES;               // [KS_STAGES][1 KB of pairs], entry t % KS_STAGES
+  KsSmem* S = (KsSmem*)(nxs + KS_STAGES * KS_NX_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m0 = blockIdx.x * KS_BM;
 
@@ -113,18 +119,27 @@ tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant_
           const uint32_t st = c % KS_STAGES, use = c / KS_STAGES;
           mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1);
           const uint32_t bar = smem_u32(&S->full[st]);
-          mbar_expect_tx(bar, KS_STAGE_BYTES);
+          const bool pairs = sl == 0 && t < nx_tiles;   // tiles past the trials' extent have no pairs: the EDGE body masks them
+          mbar_expect_tx(bar, KS_STAGE_BYTES + (pairs ? KS_NX_BYTES : 0));
           const uint32_t dst = smem_u32(ring + (size_t)st * KS_STAGE_BYTES);
           tma_load_2d(dst, &tmXh, bar, sl * KS_BK, t * KS_BN);
           tma_load_2d(dst + KS_B_PLANE_BYTES, &tmXl, bar, sl * KS_BK, t * KS_BN);
+          if (pairs) bulk_load(smem_u32(nxs + (size_t)(t % KS_STAGES) * KS_NX_BYTES), nxal4 + (size_t)t * (KS_BN / 2), KS_NX_BYTES, bar);
         }
     }
     __syncwarp();
   } else {
     // ===================================== consumer warpgroups ====================================
+    // Both warpgroups run their MMAs and then their epilogues at the same time.  Alternating them (one warpgroup's MMAs under the
+    // other's epilogue, by named turn barriers) was slower on an H100: tests/studies/kstar_probe.cu, and DESIGN.md §3.
     const int wg = threadIdx.x >> 7, wl = (threadIdx.x >> 5) & 3, q = lane & 3;
     const int r0 = m0 + wg * 64 + wl * 16 + (lane >> 2), r1 = r0 + 8;
     const bool signal = (threadIdx.x & 127) == 0;
+    // Each tile's (|x̂|², alpha) pairs sit in ring entry t % KS_STAGES until the producer refills it for tile t + KS_STAGES.  With
+    // one slab per tile that refill waits on this tile's own stage, so the stage is released only after the whole warpgroup has
+    // read the pairs (warpgroup barrier 1 + wg).  With more slabs it waits on a slab of tile t + 2 or later, released after that
+    // same barrier of tile t.
+    const bool hold = ns == 1;
     const float nc0 = ncand[r0], nc1 = ncand[r1];
     __half* out0 = Ksh + (size_t)r0 * Npad;
     __half* out1 = Ksh + (size_t)r1 * Npad;
@@ -156,18 +171,19 @@ tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant_
       }
       wgmma_wait<0>();
       acc_fence(acc);
-      if (signal) mbar_arrive(smem_u32(&S->empty[pending]));   // everything this warpgroup needs is in registers
+      if (!hold && signal) mbar_arrive(smem_u32(&S->empty[pending]));   // the accumulator is in registers; the pairs have their own ring
+      const uint32_t nx = smem_u32(nxs + (size_t)(t % KS_STAGES) * KS_NX_BYTES) + q * 16;
       const int n_base = t * KS_BN;
-      const bool store = t < store_tiles;   // a pruning pass contracts a prefix of the trials only: the mean needs every column, the plane does not
-      // EDGE: only the last tile(s) mask trials >= N.  Two instantiations behind one warp-uniform branch keep the mask out of the
-      // per-element code of every other tile.
-      auto tile_body = [&](auto edge_tag) {
-        constexpr bool EDGE = decltype(edge_tag)::value;
+      // EDGE: only the last tile(s) mask trials >= N.  STORE: a pruning pass contracts a prefix of the trials only, so tiles past
+      // store_tiles feed the mean and write no K* columns.  Instantiations behind warp-uniform branches keep the mask, and the
+      // conversions, addresses and stores, out of the per-element code of the tiles that do not need them.
+      auto tile_body = [&](auto edge_tag, auto store_tag) {
+        constexpr bool EDGE = decltype(edge_tag)::value, STORE = decltype(store_tag)::value;
         float ma0 = 0.f, mb0 = 0.f, ma1 = 0.f, mb1 = 0.f;   // two fp32 chains per row, added in FP64 once per tile
 #pragma unroll
         for (int i = 0; i < KS_BN / 8; i++) {
           const int n = n_base + 8 * i + 2 * q;
-          const float4 na = (EDGE && n >= N) ? make_float4(0.f, 0.f, 0.f, 0.f) : __ldg(nxal4 + (n >> 1));
+          const float4 na = (EDGE && n >= N) ? make_float4(0.f, 0.f, 0.f, 0.f) : lds128(nx + i * 64);
           float k00 = ks_kernel_value<KIND>(acc[4 * i], nc0 + na.x, log2amp);
           float k01 = ks_kernel_value<KIND>(acc[4 * i + 1], nc0 + na.z, log2amp);
           float k10 = ks_kernel_value<KIND>(acc[4 * i + 2], nc1 + na.x, log2amp);
@@ -182,7 +198,7 @@ tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant_
           mb0 = fmaf(k01, na.w, mb0);
           ma1 = fmaf(k10, na.y, ma1);
           mb1 = fmaf(k11, na.w, mb1);
-          if (store) {
+          if (STORE) {
             *reinterpret_cast<__half2*>(out0 + n) = __floats2half2_rn(k00, k01);
             *reinterpret_cast<__half2*>(out1 + n) = __floats2half2_rn(k10, k11);
           }
@@ -190,10 +206,20 @@ tc_kstar_kernel(const __grid_constant__ CUtensorMap tmCh, const __grid_constant_
         mu0 += (double)(ma0 + mb0);
         mu1 += (double)(ma1 + mb1);
       };
-      if (n_base + KS_BN > N)
-        tile_body(std::true_type{});
-      else
-        tile_body(std::false_type{});
+      const bool edge = n_base + KS_BN > N;
+      if (t < store_tiles) {
+        if (edge)
+          tile_body(std::true_type{}, std::true_type{});
+        else
+          tile_body(std::false_type{}, std::true_type{});
+      } else {
+        if (edge)
+          tile_body(std::true_type{}, std::false_type{});
+        else
+          tile_body(std::false_type{}, std::false_type{});
+      }
+      named_bar_sync(1 + wg, 128);   // every warp of this warpgroup is done with the tile's pairs
+      if (hold && signal) mbar_arrive(smem_u32(&S->empty[pending]));
     }
     // the four lanes of a quad hold the same two rows: fixed-order butterfly
     mu0 += __shfl_xor_sync(0xffffffffu, mu0, 1);
@@ -318,11 +344,11 @@ int kbo_i_tc_kstar(kbo_handle* h, const void* Xc, int xc_dtype, int64_t rows, __
   if (h->prm.kernel == KBO_KERNEL_RBF) {
     KBO_CUDA(h, cudaFuncSetAttribute(tc_kstar_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     tc_kstar_kernel<0><<<(unsigned)(rows_pad / KS_BM), KS_THREADS, smem, s>>>(tmCh, tmCl, tmXh, tmXl, ns, ntiles, N, (const float*)h->ks_nc.p,
-                                                                            (const float4*)h->ks_nxal.p, log2amp, Ksh, h->Npad, mun, store_tiles);
+                                                                            (const float4*)h->ks_nxal.p, Np / KS_BN, log2amp, Ksh, h->Npad, mun, store_tiles);
   } else {
     KBO_CUDA(h, cudaFuncSetAttribute(tc_kstar_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     tc_kstar_kernel<1><<<(unsigned)(rows_pad / KS_BM), KS_THREADS, smem, s>>>(tmCh, tmCl, tmXh, tmXl, ns, ntiles, N, (const float*)h->ks_nc.p,
-                                                                            (const float4*)h->ks_nxal.p, log2amp, Ksh, h->Npad, mun, store_tiles);
+                                                                            (const float4*)h->ks_nxal.p, Np / KS_BN, log2amp, Ksh, h->Npad, mun, store_tiles);
   }
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;

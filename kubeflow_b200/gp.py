@@ -201,6 +201,27 @@ class GPEngine:
             torch.cuda.current_stream(self.device).synchronize()
         return mu, var, plane
 
+    def kstar_pass(self, Xc, store_cols: int = -1, plane=None):
+        """Test hook: the tensor-core K* kernel alone -> (normalised mean of the M candidates, fp16 K* plane of rows_pad × Npad,
+        rows_pad = M rounded up to 256).  With store_cols >= 0 only the 128-column tiles covering the first store_cols columns are
+        written; pass ``plane`` to see what the kernel leaves alone."""
+        dev = f"cuda:{self.device}"
+        if not isinstance(Xc, torch.Tensor):
+            Xc = torch.as_tensor(np.ascontiguousarray(Xc), device=dev)
+        Xc = Xc.contiguous()
+        dt = L.KBO_F64 if Xc.dtype == torch.float64 else L.KBO_F32
+        M = Xc.shape[0]
+        rows_pad, npad = (M + 255) // 256 * 256, (self.N + 255) // 256 * 256
+        mu = torch.empty(rows_pad, dtype=torch.float32, device=dev)
+        if plane is None:
+            plane = torch.empty((rows_pad, npad), dtype=torch.float16, device=dev)
+        assert plane.shape == (rows_pad, npad) and plane.dtype == torch.float16 and plane.is_contiguous()
+        with torch.cuda.device(self.device):
+            rc = self.lib.kbo_debug_kstar(self._h, Xc.data_ptr(), dt, int(M), int(store_cols), mu.data_ptr(), plane.data_ptr(), self._stream())
+            L.check(self.lib, self._h, rc)
+            torch.cuda.current_stream(self.device).synchronize()
+        return mu[:M], plane
+
     def lml_grad(self):
         """(lml, grad) of the last tell; grad w.r.t. (log amplitude, log noise, log ℓ_1..ℓ_P) as a NumPy array."""
         info = self.fit_info()
