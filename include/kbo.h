@@ -169,14 +169,19 @@ int kbo_fit_append(kbo_handle* h, const double* x, double y, int x_on_host, void
 int kbo_fit_room(kbo_handle* h);
 /* Keep the first n_keep trials of the fitted history, optionally with new targets y[0..n_keep) (NULL: unchanged).  The
  * leading blocks of L and L^-1 are the factors of the shorter history and y enters only through yn / alpha / LML, so this is
- * O(N^2): it drops constant-liar rows before the real trials are appended and replaces a lie by the observed value. */
+ * O(N^2): it drops constant-liar rows before the real trials are appended and replaces a lie by the observed value.
+ * After a non-positive pivot p (kbo_fit_info's info) the rebase recovers only if every kept row was factored: after a failed
+ * kbo_fit_append, n_keep <= p - 1; after a failed kbo_fit, n_keep <= 64*floor((p - 1)/64), because the fit stops at the
+ * failing 64-row block as a whole.  A rebase into that block keeps reporting KBO_ERR_NOT_PD: the shorter history needs a
+ * kbo_fit. */
 int kbo_fit_rebase(kbo_handle* h, int32_t n_keep, const double* y, int y_on_host, void* stream);
 
 /* synchronises; any out pointer may be NULL.  info = 0 or 1-based index of the failed pivot. */
 int kbo_fit_info(kbo_handle* h, double* lml, double* y_mean, double* y_std, double* y_opt, int32_t* info,
                  void* stream);
 /* Gradient of the log-marginal likelihood of the last kbo_fit w.r.t. θ = (log amplitude, log noise, log ℓ_1..ℓ_P), P =
- * n_length_scale of that fit ($SK/_gpr.py:621-653).  grad_host: n_out = 2 + P doubles.  Synchronises. */
+ * n_length_scale of that fit ($SK/_gpr.py:621-653).  grad_host: n_out = 2 + P doubles.  Synchronises.  KBO_ERR_NOT_PD
+ * (grad_host then holds no gradient) if that fit met a non-positive pivot. */
 int kbo_lml_grad(kbo_handle* h, double* grad_host, int32_t n_out, void* stream);
 /* Log-marginal likelihood of G hyper-parameter settings over ONE history (X, y as for kbo_fit), for theta search: what sklearn's
  * optimiser evaluates one theta after another ($SK/_gpr.py:299-339, :604-618, :658-667).  The G factorisations run on G streams

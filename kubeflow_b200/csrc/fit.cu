@@ -383,7 +383,7 @@ static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double
   KBO_CUDA(h, cudaStreamWaitEvent(shi, e_start, 0));
   KBO_CUDA(h, cudaStreamWaitEvent(supd, e_start, 0));
   KBO_CUDA(h, cudaStreamWaitEvent(sinv, e_start, 0));
-  KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, sizeof(int), shi));
+  KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, 2 * sizeof(int), shi));   // h->info: the pivot and who set it
   KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, shi));
   const int RW = 512;
   int rp0 = 0;
@@ -726,7 +726,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
     cudaEventRecord(tr[0], s);
   }
   if (!e_early) {
-    KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, sizeof(int), s));
+    KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, 2 * sizeof(int), s));   // h->info: the pivot and who set it
     KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, s));   // on the caller's stream: all SMs, not the chain's 8
   }
   // a lazy fit takes alpha from triangular solves: the forward one (z = L⁻¹·yn) is carried along, one panel behind (solve.cu)
@@ -1251,7 +1251,7 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
   const bool early = early_env && !serial && !v2_env && N >= 1024;   // v3 starts on the first column block of the Gram matrix
   if (early) {
     KBO_TRY(fit_streams(h, 8));
-    KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, sizeof(int), s));
+    KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, 2 * sizeof(int), s));
     KBO_CUDA(h, cudaMemsetAsync(h->W.p, 0, sizeof(double) * (size_t)N * ld, s));
     if (!h->ev_gram) KBO_CUDA(h, cudaEventCreateWithFlags(&h->ev_gram, cudaEventDisableTiming));
     KBO_TRY(gram_two_parts(h, (const double*)h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, (double*)h->K.p, ld, 8, h->ev_gram, s));
@@ -1262,6 +1262,7 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
   h->w_full = true;
   h->w_lead = N;
   if (serial) {
+    KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, 2 * sizeof(int), s));   // kbo_i_potrf resets only the pivot
     KBO_TRY(kbo_i_potrf(h, (double*)h->K.p, N, ld, (int*)h->info.p, s));
     if (trace) cudaEventRecord(te[2], s);
     KBO_TRY(kbo_i_trtri(h, (const double*)h->K.p, N, ld, (double*)h->W.p, ld, s));
@@ -1547,7 +1548,10 @@ __global__ void __launch_bounds__(1024) append_diag_kernel(const double* __restr
   for (int j = t; j < ld; j += 1024) Lrow[j] = j < row ? l[j] : (j == row ? d : 0.0);
   if (t == 0) {
     *dinv = 1.0 / d;
-    if (!ok && *info == 0) *info = row + 1;
+    if (!ok && info[0] == 0) {
+      info[0] = row + 1;
+      info[1] = 1;   // the rows above are intact: a rebase below this row recovers (kbo_i_fit_rebase)
+    }
   }
 }
 // W row ← (−(Wᵀl)/d, 1/d, 0…)
@@ -1604,8 +1608,13 @@ int kbo_i_fit_append(kbo_handle* h, const double* x_dev, double y, cudaStream_t 
 // kbo_fit_rebase: keep the first n_keep trials of the fitted history (the leading blocks of L and W = L⁻¹ ARE the factors of
 // the shorter history), optionally with new y values — y enters only through yn/alpha/LML.  Drops constant-liar rows before
 // the real trials are appended, and replaces a lie by the observed value when the trial finishes.
+// A failure is cleared only if every kept row was factored: a failed append leaves just its own row unwritten, a failed fit its
+// whole failing 64-block (potf2_inv_kernel returns before writing the block back, and the rows below it are never solved).
 __global__ void clear_info_above_kernel(int* info, int n_keep) {
-  if (*info > n_keep) *info = 0;
+  const int bad = info[0];
+  if (bad == 0) return;
+  const int factored = info[1] ? bad - 1 : (bad - 1) / KBO_NB * KBO_NB;
+  if (n_keep <= factored) info[0] = info[1] = 0;
 }
 int kbo_i_fit_rebase(kbo_handle* h, int n_keep, const double* y_dev, cudaStream_t s) {
   if (!h->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_fit_rebase: call kbo_fit first");

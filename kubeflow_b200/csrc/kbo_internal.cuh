@@ -37,7 +37,8 @@ struct kbo_handle {
   DevBuf yraw, lrow;   // raw y (re-normalised on append) and the append's work vectors
   DevBuf Wh, Wl;        // fp16 planes Npad×Npad (TC mode)
   DevBuf scal;          // device scalars, see ScalIdx
-  DevBuf info;          // int32: potrf info
+  DevBuf info;          // int32: [0] potrf info; [1] 1 if an append set it (only that row is unfactored), 0 after a fit (its whole
+                        // failing 64-block is)
   DevBuf stage_X, stage_y, stage_Xc;  // H2D staging for host-pointer entry points
   // ---- sweep workspace ---------------------------------------------------------------------
   DevBuf Ks64;          // chunk × ldks fp64 (F64 mode)

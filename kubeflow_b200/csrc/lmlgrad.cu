@@ -161,7 +161,11 @@ extern "C" int kbo_lml_grad(kbo_handle* h, double* grad_host, int32_t n_out, voi
   KBO_LAUNCH_CHECK(h);
   lml_grad_reduce_kernel<<<(ncomp + 63) / 64, 64, 0, s>>>((const double*)h->part.p, nb, nb, ncomp, h->prm.noise, grad_dev);
   KBO_LAUNCH_CHECK(h);
+  int inf = 0;
   KBO_CUDA(h, cudaMemcpyAsync(grad_host, grad_dev, sizeof(double) * ncomp, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaMemcpyAsync(&inf, h->info.p, sizeof(int), cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
+  // a failed fit leaves L (and so K⁻¹) partly unfactored: the gradient built from it is meaningless
+  if (inf != 0) KBO_FAIL(h, KBO_ERR_NOT_PD, "kernel matrix is not positive definite (pivot %d); increase `noise`", inf);
   return KBO_OK;
 }

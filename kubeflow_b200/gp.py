@@ -230,10 +230,11 @@ class GPEngine:
         L.check(self.lib, self._h, rc)
         return info["lml"], g
 
-    def lml_batch(self, X, y, thetas):
+    def lml_batch(self, X, y, thetas, return_info: bool = False):
         """Log-marginal likelihood of several θ over one history in one call (kbo_lml_batch: the factorisations run concurrently).
         ``thetas``: list of dicts with any of length_scale / noise / amplitude (the engine's own values where absent).
-        Returns a float64 NumPy array, −inf where the Gram matrix is not positive definite.  The fitted state is untouched."""
+        Returns a float64 NumPy array, −inf where the Gram matrix is not positive definite (with ``return_info``, also each θ's
+        1-based failed pivot, 0 if none).  The fitted state is untouched."""
         X, y = self._as_host_f64(X), self._as_host_f64(y).reshape(-1)
         N, D = X.shape
         G = len(thetas)
@@ -253,7 +254,7 @@ class GPEngine:
             rc = self.lib.kbo_lml_batch(self._h, X.ctypes.data, y.ctypes.data, int(N), int(D), int(G), arr, 1,
                                         out.ctypes.data_as(C.POINTER(C.c_double)), info, self._stream())
         L.check(self.lib, self._h, rc)
-        return out
+        return (out, np.array(info[:], dtype=np.int32)) if return_info else out
 
     def state(self):
         """Copies of L (lower), W = L^-1 and alpha as float64 CUDA tensors (parity tests)."""

@@ -174,26 +174,53 @@ def theta_of_record(D):
     return dict(length_scale=0.3 * np.sqrt(D), amplitude=1.0, noise=1e-3, xi=0.01, kappa=1.96)
 
 
-def lml_and_grad(X, y, *, kind=KERNEL_MATERN52, length_scale=1.0, amplitude=1.0, noise=1e-10, normalize_y=True):
+def lml_and_grad(X, y, *, kind=KERNEL_MATERN52, length_scale=1.0, amplitude=1.0, noise=1e-10, normalize_y=True, chunk=64):
     """Log-marginal likelihood and its gradient w.r.t. θ = (log amplitude, log noise, log ℓ_1..ℓ_P) at fixed data
     ($SK/_gpr.py:541-655: ``0.5·einsum((ααᵀ − K⁻¹), ∂K/∂θ)``; kernel gradients $SK/kernels.py:1571-1591 (RBF),
-    :1731-1745 (Matérn ν=2.5), :1296 (Constant), :1421 (White)).  P = 1 (isotropic) or D."""
+    :1731-1745 (Matérn ν=2.5), :1296 (Constant), :1421 (White)).  P = 1 (isotropic) or D.
+
+    The (n, n, D) tensor of squared differences is formed ``chunk`` rows at a time (O(chunk·n·D) memory instead of 17 GB at
+    n = 8192, D = 32); ``chunk >= n`` is the one-shot computation.  Only the summation order depends on ``chunk``."""
     fit = gp_fit(X, y, kind=kind, length_scale=length_scale, amplitude=amplitude, noise=noise, normalize_y=normalize_y)
     Xs = fit["X"] / fit["length_scale"]
-    n = len(fit["yn"])
+    n, D = Xs.shape
     Kinv = cho_solve((fit["L"], True), np.eye(n), check_finite=False)
-    G = np.outer(fit["alpha"], fit["alpha"]) - Kinv
-    diff2 = (Xs[:, None, :] - Xs[None, :, :]) ** 2          # (n, n, D) scaled squared differences
-    r2 = diff2.sum(-1)
-    if kind == KERNEL_RBF:
-        k = np.exp(-0.5 * r2)
-        q = k                                              # ∂k/∂log ℓ_d = k · Δ_d²
-    else:
-        s = np.sqrt(5.0 * r2)
-        k = (1 + s + s * s / 3) * np.exp(-s)
-        q = (5.0 / 3.0) * (1 + s) * np.exp(-s)             # ∂k/∂log ℓ_d = (5/3)(1+s)e^{-s} · Δ_d²
-    g_amp = 0.5 * np.sum(G * (amplitude * k))
-    g_noise = 0.5 * noise * np.trace(G)
-    per_dim = 0.5 * amplitude * np.einsum("ij,ij,ijd->d", G, q, diff2)
+    g_amp, per_dim = 0.0, np.zeros(D)
+    for s0 in range(0, n, chunk):
+        G = np.outer(fit["alpha"][s0:s0 + chunk], fit["alpha"]) - Kinv[s0:s0 + chunk]
+        diff2 = (Xs[s0:s0 + chunk, None, :] - Xs[None, :, :]) ** 2     # (chunk, n, D) scaled squared differences
+        r2 = diff2.sum(-1)
+        if kind == KERNEL_RBF:
+            k = np.exp(-0.5 * r2)
+            q = k                                              # ∂k/∂log ℓ_d = k · Δ_d²
+        else:
+            s = np.sqrt(5.0 * r2)
+            k = (1 + s + s * s / 3) * np.exp(-s)
+            q = (5.0 / 3.0) * (1 + s) * np.exp(-s)             # ∂k/∂log ℓ_d = (5/3)(1+s)e^{-s} · Δ_d²
+        g_amp += 0.5 * np.sum(G * (amplitude * k))
+        per_dim += 0.5 * amplitude * np.einsum("ij,ij,ijd->d", G, q, diff2)
+    g_noise = 0.5 * noise * (np.sum(fit["alpha"] ** 2) - np.trace(Kinv))
     g_ls = per_dim if np.ndim(length_scale) and len(np.atleast_1d(length_scale)) > 1 else np.array([per_dim.sum()])
     return fit["lml"], np.concatenate([[g_amp, g_noise], g_ls])
+
+
+def not_pd_at(N, p, *, isolated=None):
+    """A history (X, y) in D = 4 whose RBF Gram matrix (amplitude 1, ℓ = 1, noise 0) has its first non-positive Cholesky pivot
+    EXACTLY at the 1-based index p (2 <= p <= N), in any summation order:
+      * the rows form part of the integer lattice {0, 2, …, 16}⁴ (spacing 2ℓ): a Kronecker product of 1-D factors whose smallest
+        eigenvalue is ≈ 1 − 2e⁻² ≈ 0.73, so every principal submatrix has λ_min ≳ 0.28 even without noise;
+      * row ``isolated`` (default (p − 1)//2) sits ≥ 64ℓ from every lattice point: exp(−d²/2) is exactly 0 in FP64 (and flushes to
+        0 on the device), so its pivot is k(0) = 1 exactly, and its column of L is 1 on the diagonal, 0 elsewhere;
+      * row p − 1 duplicates it: its pivot is 1 − 1·1 = 0 exactly.
+    Integer coordinates make every squared distance exact."""
+    assert 2 <= p <= N
+    i = (p - 1) // 2 if isolated is None else isolated
+    assert 0 <= i < p - 1
+    g = np.arange(0, 18, 2, dtype=np.float64)
+    lattice = np.stack(np.meshgrid(g, g, g, g, indexing="ij"), -1).reshape(-1, 4)
+    lattice = lattice[np.random.default_rng(N * 7919 + p).permutation(len(lattice))]
+    assert N - 2 <= len(lattice), f"N <= {len(lattice) + 2}"
+    far = np.full(4, 1000.0)
+    X = np.concatenate([lattice[:i], far[None], lattice[i:p - 2], far[None], lattice[p - 2:N - 2]])
+    y = np.sin(X.sum(axis=1) / 8.0)
+    return X, y

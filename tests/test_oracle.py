@@ -94,7 +94,40 @@ def test_lml_gradient_matches_sklearn_golden():
     assert len(names) == 4
     for n in names:
         ls = z[f"{n}__ls"]
-        lml, g = O.lml_and_grad(z[f"{n}__X"], z[f"{n}__y"], kind=str(z[f"{n}__kind"]), length_scale=ls if len(ls) > 1 else float(ls[0]),
-                                amplitude=float(z[f"{n}__amp"]), noise=float(z[f"{n}__noise"]))
-        assert abs(lml - float(z[f"{n}__lml"])) < 1e-9
-        np.testing.assert_allclose(g, z[f"{n}__grad"], rtol=0, atol=1e-9)
+        for chunk in (1, 7, 64):
+            lml, g = O.lml_and_grad(z[f"{n}__X"], z[f"{n}__y"], kind=str(z[f"{n}__kind"]), length_scale=ls if len(ls) > 1 else float(ls[0]),
+                                    amplitude=float(z[f"{n}__amp"]), noise=float(z[f"{n}__noise"]), chunk=chunk)
+            assert abs(lml - float(z[f"{n}__lml"])) < 1e-9
+            np.testing.assert_allclose(g, z[f"{n}__grad"], rtol=0, atol=1e-9)
+
+
+@pytest.mark.parametrize("n,D,kind,ard", [(150, 3, "matern52", False), (97, 17, "rbf", True), (130, 33, "matern52", True), (1, 2, "rbf", False)])
+def test_lml_gradient_row_chunks_sum_to_the_one_shot_gradient(n, D, kind, ard):
+    """The row-chunked gradient (what makes N = 8192, D = 32 fit in memory) is the one-shot (n, n, D) computation up to the
+    summation order, whatever the chunk and however the last chunk is cut."""
+    r = np.random.default_rng(n * D)
+    X, y = r.random((n, D)), r.standard_normal(n)
+    ls = 0.3 * np.sqrt(D) * (np.linspace(0.7, 1.4, D) if ard else 1.0)
+    kw = dict(kind=kind, length_scale=ls, amplitude=1.3, noise=1e-3)
+    lml0, g0 = O.lml_and_grad(X, y, chunk=n, **kw)
+    for chunk in (1, 7, 64):
+        lml, g = O.lml_and_grad(X, y, chunk=chunk, **kw)
+        assert lml == lml0
+        np.testing.assert_allclose(g, g0, rtol=1e-12, atol=1e-12 * np.abs(g0).max())
+
+
+@pytest.mark.parametrize("N", [4096, 5800])
+def test_not_pd_constructions_fail_exactly_at_the_chosen_pivot_in_lapack(N):
+    """oracle.not_pd_at(N, p): LAPACK's dpotrf on the RBF Gram matrix (amplitude 1, ℓ = 1, noise 0) reports the first
+    non-positive pivot at exactly p — the histories the GPU tests use to pin the engine's `info`."""
+    from scipy.linalg import lapack
+    for p in (2, 64, 65, 256, 257, 2985, N):
+        X, _ = O.not_pd_at(N, p)
+        assert np.all(X == np.round(X))
+        K = O.kernel_matrix(X, X, 1.0, "rbf", 1.0)
+        _, info = lapack.dpotrf(K, lower=1, clean=0, overwrite_a=1)
+        assert info == p, (N, p, info)
+    X, _ = O.not_pd_at(N, 2985)
+    K = O.kernel_matrix(X[:2984], X[:2984], 1.0, "rbf", 1.0)
+    _, info = lapack.dpotrf(K, lower=1, clean=0, overwrite_a=1)
+    assert info == 0
