@@ -162,8 +162,10 @@ int kbo_fit(kbo_handle* h, const double* X, const double* y, int32_t N, int32_t 
 /* Append ONE trial (x: D doubles, y) to the fitted history at the same theta without refactorising: the bordered Cholesky
  * row l = W k, d = sqrt(amp + noise - l.l), the matching row of W = L^-1, then the y statistics, alpha, LML and the fp16
  * planes are brought up to date — O(N^2) instead of O(N^3) (SURVEY.md 8(f)2: skopt's constant-liar `ask(n_points=k)` tells
- * k-1 lies one after another, `Optimizer.tell` refits each time).  Works in place while the history fits its 64-row pitch:
- * kbo_fit_room() says how many more trials can be appended (0: call kbo_fit with the whole history).  Not positive definite
+ * k-1 lies one after another, `Optimizer.tell` refits each time).  Works in place up to the row pitch of the last kbo_fit
+ * (its N rounded up to 64).  kbo_fit_rebase keeps that pitch, so after a rebase to n_keep up to pitch - n_keep rows can be
+ * appended on the same factorisation, not just the rest of one 64-row block.  kbo_fit_room() says how many more trials can
+ * be appended (0: call kbo_fit with the whole history).  Not positive definite
  * is reported by kbo_fit_info like after a fit; the handle then needs a kbo_fit.  Results equal a refit's to ~1e-12. */
 int kbo_fit_append(kbo_handle* h, const double* x, double y, int x_on_host, void* stream);
 int kbo_fit_room(kbo_handle* h);

@@ -133,7 +133,8 @@ class Optimizer:
         the constant liar extends it one row at a time, so most calls differ from what the engine already holds only past a
         long common prefix of rows: the engine keeps that prefix (kbo_fit_rebase — the leading blocks of L and L⁻¹ are the
         factors of the shorter history; targets are replaced wholesale, so a lie that became an observation costs nothing) and
-        the few new rows are appended (kbo_fit_append, O(N²) each) while there is room in the 64-row pitch.  Anything else —
+        the few new rows are appended (kbo_fit_append, O(N²) each) while there is room in the last fit's row pitch (its N
+        rounded up to 64, kept by a rebase: eng.room()).  Anything else —
         a different θ, an edited early row, many new rows — refits (O(N³)) as skopt does on every tell."""
         key = (eng.kernel, tuple(np.atleast_1d(eng.length_scale).tolist()), eng.amplitude, eng.noise, eng.normalize_y, eng.var_mode,
                eng.acq, eng.xi, eng.kappa)

@@ -1,7 +1,8 @@
 """Measurements of test_gpu_fit_scale.py, importable and runnable in a fresh process (the KBO_FIT_* schedule switches are read
 once per process).  One fit of a history at production N, its factors checked on the GPU against an FP64 Gram matrix rebuilt
 here by exact differences (as oracle.kernel_matrix forms it) and against a LAPACK reference saved by the caller; only numbers
-come back: per-256×256-tile worst errors and where they are, the suggestion, a SHA-256 of L.
+come back: per-256×256-tile worst errors and where they are, the suggestion, a SHA-256 of L.  `current` runs the same checks
+on whatever an engine holds after kbo_fit_append / kbo_fit_rebase chains (test_gpu_append_scale.py).
 
     python tests/_fit_scale.py '<json spec>' out.json
 spec: {"fits": [[N, case, var_mode, ref_prefix], ...]}  or  {"pivots": [[N, p], ...], "var_mode": "f64"|"tc"}
@@ -101,31 +102,64 @@ def device_y_stats(y):
     return a[0] / len(y), float(np.min(y))
 
 
+def lapack(X, y, th):
+    """oracle.gp_fit of a history (scipy cholesky / cho_solve) with cond_lb, the bound the forward errors are scaled by."""
+    f = O.gp_fit(X, y, kind=th["kind"], length_scale=th["length_scale"], amplitude=th["amplitude"], noise=th["noise"])
+    d = np.diag(f["L"])
+    f["cond_lb"] = float((th["amplitude"] + th["noise"]) / d.min() ** 2)   # 1/λ_min >= 1/min pivot: a lower bound on cond(K)
+    return f
+
+
 def reference(N, case, prefix):
     """LAPACK factor of the history (oracle.gp_fit: scipy cholesky / cho_solve) -> prefix_L.npy, prefix_alpha.npy and the scalars."""
     X, y, _, th = history(N, case, M=1)
-    f = O.gp_fit(X, y, kind=th["kind"], length_scale=th["length_scale"], amplitude=th["amplitude"], noise=th["noise"])
+    f = lapack(X, y, th)
     np.save(prefix + "_L.npy", f["L"])
     np.save(prefix + "_alpha.npy", f["alpha"])
-    d = np.diag(f["L"])
-    return dict(lml=f["lml"], y_mean=f["y_mean"], y_std=f["y_std"],
-                cond_lb=float((th["amplitude"] + th["noise"]) / d.min() ** 2))   # 1/λ_min >= 1/min pivot: a lower bound on cond(K)
+    return dict(lml=f["lml"], y_mean=f["y_mean"], y_std=f["y_std"], cond_lb=f["cond_lb"])
 
 
-def _errors(K, Lm, Wm, al, yn, Lref, aref, tag=""):
+def _errors(K, Lm, Wm, al, yn, Lref, aref, tag="", first=None):
+    """`first`: also the worst entry in rows [first, N) of K − LLᵀ and WL − I — the rows kbo_fit_append bordered on."""
     r = {}
     kmax = float(K.diagonal().max())
-    r["backward" + tag], r["backward_tile" + tag] = tile_max(K - Lm @ Lm.T)
+    E = K - Lm @ Lm.T
+    r["backward" + tag], r["backward_tile" + tag] = tile_max(E)
     r["backward" + tag] /= kmax
+    if first is not None:
+        r["backward_app" + tag] = float(E[first:].abs().max()) / kmax
+    del E
     r["upper_L_nonzero" + tag] = int(torch.count_nonzero(torch.triu(Lm, 1)))
     r["alpha_res" + tag] = float(torch.linalg.vector_norm(K @ al - yn) / (torch.linalg.matrix_norm(K) * torch.linalg.vector_norm(al)))
     r["L_fwd" + tag] = float((Lm - Lref).abs().max() / Lref.abs().max())
     r["alpha_fwd" + tag] = float((al - aref).abs().max() / aref.abs().max())
     if Wm is not None:
         I = torch.eye(K.shape[0], dtype=torch.float64, device="cuda")
-        r["WL" + tag], r["WL_tile" + tag] = tile_max(Wm @ Lm - I)
+        E = Wm @ Lm - I
+        r["WL" + tag], r["WL_tile" + tag] = tile_max(E)
+        if first is not None:
+            r["WL_app" + tag] = float(E[first:].abs().max())
+        del E
         r["LW" + tag], r["LW_tile" + tag] = tile_max(Lm @ Wm - I)
         r["upper_W_nonzero" + tag] = int(torch.count_nonzero(torch.triu(Wm, 1)))
+    return r
+
+
+def current(e, X, y, th, ref, first=None):
+    """The checks of `measure` on whatever the engine holds now — after kbo_fit_append / kbo_fit_rebase chains too — against a
+    Gram matrix rebuilt from (X, y) and its LAPACK factor `ref` (`lapack`).  `first`: the first appended row, whose rows are
+    also reported on their own."""
+    fi = e.fit_info()
+    assert e.N == len(y), (e.N, len(y))
+    K = gram(X, th)
+    Lm, Wm, al = state(e)
+    yn = torch.tensor((y - fi["y_mean"]) / fi["y_std"], device="cuda")
+    Lref, aref = torch.tensor(ref["L"], device="cuda"), torch.tensor(ref["alpha"], device="cuda")
+    r = dict(N=e.N, info=fi["info"], lml=fi["lml"], y_mean=fi["y_mean"], y_std=fi["y_std"], y_opt=fi["y_opt"],
+             pivot_last=float(Lm[-1, -1]))
+    r.update(_errors(K, Lm, Wm, al, yn, Lref, aref, first=first))
+    del K, Lm, Wm, al, Lref, aref
+    torch.cuda.empty_cache()
     return r
 
 
