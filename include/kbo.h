@@ -294,8 +294,11 @@ uint64_t kbo_hash64(const void* bytes, uint64_t len);   /* the FNV-1a hash kbo_r
  * State (mean, sigma, C, evolution paths, eigenbasis) lives on the device.  One generation = ask + tell:
  *   kbo_cma_ask : X (lambda×D, device, fp64) = m + sigma·B·(d∘z); z from the built-in Philox stream (seed, generation) or,
  *                 for parity tests, from z_in_dev (lambda×D device, may be NULL).
- *   kbo_cma_tell: fitness (lambda, device, minimised, ties → lower sample index) for the X of the last ask → rank-μ/rank-1
- *                 covariance update, step-size control and a warm-started Jacobi eigendecomposition.
+ *   kbo_cma_tell: fitness (lambda, device, minimised) for the X of the last ask → rank-μ/rank-1 covariance update,
+ *                 step-size control and a warm-started Jacobi eigendecomposition C = B diag(d²) Bᵀ.
+ *                 Ranking is NumPy's sort order: -inf < finite < +inf < NaN, -0 == +0, every NaN equal (a diverged trial
+ *                 that reports nan ranks last, after inf); ties → lower sample index.
+ *                 d_j² is the eigenvalue λ_j itself (b_jᵀ C b_j); only λ_j ≤ 0 is replaced, by 1e-8.
  * Limits: 1 <= D <= 128, 4 <= lambda <= 8192.  kbo_cma_state copies to HOST buffers (any may be NULL) and synchronises.
  * kbo_cma_run_synthetic runs `generations` ask/fitness/tell rounds entirely on the device with a built-in fitness
  * (0 = sphere, 1 = Rastrigin) — the BASELINE.json config-4 benchmark. */

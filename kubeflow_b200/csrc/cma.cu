@@ -1,9 +1,10 @@
 // (μ/μ_w, λ)-CMA-ES generation on the device, FP64 — the sampler behind Katib's `cmaes` algorithm (goptuna; SURVEY.md §8(a) A9).
 // N. Hansen, "The CMA Evolution Strategy: A Tutorial" (arXiv:1604.00772), active-weights variant as in CyberAgent `cmaes`:
 //   ask : z ~ N(0,I) (Philox4x32-10 + Box–Muller, or caller-supplied), y = B·(d∘z), x = m + σ·y
-//   tell: rank by fitness (ties → lower sample index), y_w, m, p_σ, σ, h_σ, p_c, C ← a·C + c1·p_c p_cᵀ + cμ·Σ w°_i y_i y_iᵀ,
-//         then C = B diag(d²) Bᵀ by one-sided Jacobi warm-started from the previous basis (G = C·B_prev is already nearly
-//         column-orthogonal, so one or two sweeps suffice instead of ~8 from scratch).
+//   tell: rank by fitness (NumPy order, NaN last; ties → lower sample index), y_w, m, p_σ, σ, h_σ, p_c,
+//         C ← a·C + c1·p_c p_cᵀ + cμ·Σ w°_i y_i y_iᵀ, then C = B diag(d²) Bᵀ by one-sided Jacobi warm-started from the previous
+//         basis (G = C·B_prev), d_j² = b_jᵀ C b_j.  Over the cfg4 run (D = 128, λ = 4096, Rastrigin) the warm start still
+//         takes 6–7 sweeps, counting the last one that rotates nothing (10 at most), measured on an H100.
 // Everything is tiny (D ≤ 128, λ ≤ 8192: C is 128 KiB) — the generation is launch/latency bound, so each phase is one
 // kernel and the whole state lives in HBM/L2 between them; nothing returns to the host until the caller asks.
 #include "kbo_internal.cuh"
@@ -87,16 +88,16 @@ __global__ void cma_fitness_kernel(const double* __restrict__ X, int lambda, int
 }
 
 // ------------------------------------------------------------------------------------------------ rank
-// single-CTA bitonic sort of (fitness, index) in shared memory; NaN sorts last; ties → lower index first
+// single-CTA bitonic sort of (fitness, index) in shared memory, in NumPy's order (what the oracle's lexsort gives):
+// -inf < finite < +inf < NaN, -0 == +0, every NaN equal; ties → lower index first.  Padding rows are NaN with indices
+// past lambda, so they sort after every real sample.
 __global__ void __launch_bounds__(1024) cma_sort_kernel(const double* __restrict__ f, int lambda, int n2, int* __restrict__ order,
                                                         double* __restrict__ scal) {
   extern __shared__ unsigned char smc[];
   double* key = reinterpret_cast<double*>(smc);
   int* idx = reinterpret_cast<int*>(key + n2);
   for (int i = threadIdx.x; i < n2; i += 1024) {
-    double v = i < lambda ? f[i] : INFINITY;
-    if (v != v) v = INFINITY;
-    key[i] = v;
+    key[i] = i < lambda ? f[i] : NAN;
     idx[i] = i;
   }
   __syncthreads();
@@ -108,7 +109,8 @@ __global__ void __launch_bounds__(1024) cma_sort_kernel(const double* __restrict
           const bool up = (i & k) == 0;
           const double a = key[i], b = key[l];
           const int ia = idx[i], ib = idx[l];
-          const bool gt = a > b || (a == b && ia > ib);
+          const bool an = a != a, bn = b != b;
+          const bool gt = an != bn ? an : (a > b || (!(a < b) && ia > ib));
           if (gt == up) {
             key[i] = b; key[l] = a;
             idx[i] = ib; idx[l] = ia;
@@ -224,8 +226,8 @@ __global__ void cma_c_finalize_kernel(double* __restrict__ C, const double* __re
 // Rotations stop at |g_a·g_b| ≤ 1e-13·‖g_a‖‖g_b‖ (orthogonality of B to ~1e-13; the last quadratic sweep to 1e-16 buys nothing).
 // DT = compile-time D (128: fully unrolled 8-row loops, loads pipelined) or 0 = runtime D.
 template <int DT>
-__global__ void __launch_bounds__(1024) cma_jacobi_kernel(const double* __restrict__ G, int Drt, double* __restrict__ B, double* __restrict__ Dv,
-                                                          double* __restrict__ scal, int max_sweeps) {
+__global__ void __launch_bounds__(1024) cma_jacobi_kernel(const double* __restrict__ G, int Drt, double* __restrict__ B, double* __restrict__ scal,
+                                                          int max_sweeps) {
   const int D = DT > 0 ? DT : Drt;
   extern __shared__ double Gt[];  // [Dp][D+1], Dp = D rounded up to even
   __shared__ int s_rot;
@@ -292,7 +294,10 @@ __global__ void __launch_bounds__(1024) cma_jacobi_kernel(const double* __restri
     __syncthreads();
     if (!rotated) break;
   }
-  // column norms are the eigenvalues of C (SPD); normalised columns the eigenvectors
+  // normalised columns are the eigenvectors (up to sign: a column's norm is |λ_j|, so cma_eigval_kernel takes λ_j itself).
+  // Every nonzero column is written, a NaN one included (so a broken C shows in B instead of leaving it stale).  An exactly
+  // zero column was never rotated (pairs with a zero column are skipped), so its warm-start vector, left in place, is the
+  // eigenvector C annihilates; its d_j is the floor.
   for (int j0 = 0; j0 < D; j0 += 64) {
     const int j = j0 + pair;
     double n2 = 0.0;
@@ -300,13 +305,53 @@ __global__ void __launch_bounds__(1024) cma_jacobi_kernel(const double* __restri
       for (int i = q; i < D; i += 16) n2 = fma(Gt[j * ldg + i], Gt[j * ldg + i], n2);
 #pragma unroll
     for (int o = 8; o > 0; o >>= 1) n2 += __shfl_xor_sync(0xffffffffu, n2, o);
-    const double lam = sqrt(n2);
-    if (j < D && lam > 1e-300) {
-      for (int i = q; i < D; i += 16) B[(size_t)i * D + j] = Gt[j * ldg + i] / lam;
-      if (q == 0) Dv[j] = sqrt(lam < CMA_EPS ? CMA_EPS : lam);
+    if (j < D && n2 != 0.0) {
+      const double inv = 1.0 / sqrt(n2);
+      for (int i = q; i < D; i += 16) B[(size_t)i * D + j] = Gt[j * ldg + i] * inv;
     }
   }
   if (t == 0) scal[CS_SWEEPS] = (double)(sweep + 1);
+}
+// d_j = √λ_j with λ_j = b_jᵀ C b_j (the Rayleigh quotient keeps the sign a column norm loses); only λ_j ≤ 0 is floored,
+// at CMA_EPS, as the oracle does.  One CTA per eigenpair: thread (part, i) sums every 8th term of (C b_j)_i from column i
+// of C (= row i, C being symmetric, so the loads coalesce) with all 16 loads in flight; fixed-order reductions.
+__global__ void __launch_bounds__(1024) cma_eigval_kernel(const double* __restrict__ C, const double* __restrict__ B, int D,
+                                                          double* __restrict__ Dv) {
+  constexpr int PARTS = 1024 / CMA_MAXD;
+  __shared__ double b[CMA_MAXD], red[1024];
+  const int j = blockIdx.x, t = threadIdx.x, i = t % CMA_MAXD, part = t / CMA_MAXD;
+  if (t < D) b[t] = B[(size_t)t * D + j];
+  __syncthreads();
+  double s = 0.0;
+  if (i < D) {
+    double c[CMA_MAXD / PARTS];
+#pragma unroll
+    for (int u = 0; u < CMA_MAXD / PARTS; u++) {
+      const int k = part + u * PARTS;
+      c[u] = k < D ? C[(size_t)k * D + i] : 0.0;
+    }
+#pragma unroll
+    for (int u = 0; u < CMA_MAXD / PARTS; u++) {
+      const int k = part + u * PARTS;
+      if (k < D) s = fma(c[u], b[k], s);
+    }
+  }
+  red[t] = s;
+  __syncthreads();
+  if (t < CMA_MAXD) {
+    double a = 0.0;
+    for (int p = 0; p < PARTS; p++) a += red[p * CMA_MAXD + t];
+    red[t] = t < D ? a * b[t] : 0.0;
+  }
+  __syncthreads();
+  for (int o = CMA_MAXD / 2; o > 0; o >>= 1) {
+    if (t < o) red[t] += red[t + o];
+    __syncthreads();
+  }
+  if (t == 0) {
+    const double lam = red[0];
+    Dv[j] = sqrt(lam <= 0.0 ? CMA_EPS : lam);
+  }
 }
 
 __global__ void cma_init_kernel(double* __restrict__ C, double* __restrict__ B, double* __restrict__ Dv, double* __restrict__ ps,
@@ -351,9 +396,11 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
   KBO_LAUNCH_CHECK(h);
   const int Dp = (D + 1) & ~1;
   if (D == 128)
-    cma_jacobi_kernel<128><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>((const double*)c->G.p, D, (double*)c->B.p, (double*)c->Dv.p, (double*)c->scal.p, 30);
+    cma_jacobi_kernel<128><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>((const double*)c->G.p, D, (double*)c->B.p, (double*)c->scal.p, 30);
   else
-    cma_jacobi_kernel<0><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>((const double*)c->G.p, D, (double*)c->B.p, (double*)c->Dv.p, (double*)c->scal.p, 30);
+    cma_jacobi_kernel<0><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>((const double*)c->G.p, D, (double*)c->B.p, (double*)c->scal.p, 30);
+  KBO_LAUNCH_CHECK(h);
+  cma_eigval_kernel<<<D, 1024, 0, s>>>((const double*)c->C.p, (const double*)c->B.p, D, (double*)c->Dv.p);
   KBO_LAUNCH_CHECK(h);
   c->gen++;
   c->asked = false;

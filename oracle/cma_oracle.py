@@ -11,6 +11,9 @@ tutorial's default setting, w = 0.4563, 0.2708, 0.1622, 0.0852, 0.0255, μ_eff =
 this file's own arithmetic (tests/golden/cma_replay.npz, generator oracle/make_golden_cma.py) so that any drift shows, and
 property checks (rotation equivariance, convergence on the sphere, C stays SPD, tie-breaking).  No vector from goptuna /
 `cmaes` itself exists here: the judge's "partial" for this row stands until one does.
+
+One deliberate departure from `cmaes`: `eigen` floors eigenvalues that are exactly zero as well as negative ones (`cmaes`
+floors only D² < 0, so an exact zero there divides by zero in C^{-1/2} and turns the run into NaN).
 """
 from __future__ import annotations
 
@@ -56,10 +59,11 @@ class CmaState:
 
 
 def eigen(C):
-    """C = B diag(D²) Bᵀ, symmetrised, eigenvalues floored at EPS (as ``cmaes`` does before the square root)."""
+    """C = B diag(D²) Bᵀ, symmetrised.  Only non-positive eigenvalues are replaced, by EPS, before the square root; a positive
+    eigenvalue below EPS is kept as it is (``cmaes`` does the same for negative ones; see the module docstring for zero)."""
     C = (C + C.T) / 2
     D2, B = np.linalg.eigh(C)
-    D = np.sqrt(np.where(D2 < 0, EPS, D2))
+    D = np.sqrt(np.where(D2 <= 0, EPS, D2))
     return B, D
 
 
@@ -70,9 +74,11 @@ def ask(state: CmaState, z):
     return state.mean + state.sigma * Y, Y
 
 
-def tell(state: CmaState, Y, fitness, znorm2=None):
+def tell(state: CmaState, Y, fitness, znorm2=None, h_sigma=None):
     """One generation update from the steps Y = (X − m)/σ (λ×n, in the order they were sampled) and their fitness
-    (minimised; ties broken by sample index).  ``znorm2`` = ‖C^{-1/2} y_k‖² per sample (defaults to computing it)."""
+    (minimised, in NumPy's sort order: -inf < finite < +inf < NaN, -0 == +0; ties broken by sample index).
+    ``znorm2`` = ‖C^{-1/2} y_k‖² per sample (defaults to computing it).  ``h_sigma`` (0 or 1) overrides the stall test,
+    for comparing with an implementation whose ‖p_σ‖ lands on the other side of the threshold by rounding."""
     p, n = state.p, len(state.mean)
     order = np.lexsort((np.arange(len(fitness)), np.asarray(fitness)))
     Ys = np.asarray(Y, dtype=np.float64)[order]
@@ -84,7 +90,8 @@ def tell(state: CmaState, Y, fitness, znorm2=None):
     norm_ps = np.linalg.norm(state.p_sigma)
     sigma_new = state.sigma * np.exp((p.c_sigma / p.d_sigma) * (norm_ps / p.chi_n - 1))
     h_left = norm_ps / np.sqrt(1 - (1 - p.c_sigma) ** (2 * (state.g + 1)))
-    h_sigma = 1.0 if h_left < (1.4 + 2 / (n + 1)) * p.chi_n else 0.0
+    if h_sigma is None:
+        h_sigma = 1.0 if h_left < (1.4 + 2 / (n + 1)) * p.chi_n else 0.0
     state.pc = (1 - p.cc) * state.pc + h_sigma * np.sqrt(p.cc * (2 - p.cc) * p.mu_eff) * y_w
     if znorm2 is None:
         zn2 = ((Ys @ C_2.T) ** 2).sum(1)
@@ -106,3 +113,35 @@ def sphere(X):
 
 def rastrigin(X):
     return 10.0 * X.shape[1] + (X * X - 10.0 * np.cos(2 * np.pi * X)).sum(1)
+
+
+OBJECTIVES = ("sphere", "ellipsoid1e3", "ellipsoid1e6", "cigar", "discus", "rosenbrock")
+
+
+def objective(name: str, n: int, seed: int = 0):
+    """f(X) (rows of X are points) with its minimum f = 0 at x* inside the unit cube, in the coordinates of the service's
+    search (mean 0.5, σ = 1/6).  Returns (f, x*, H): H is the Hessian at x* (None for Rosenbrock, which is not quadratic).
+    The ellipsoids (condition 1e3, 1e6), the cigar (one axis of weight 1, n − 1 of weight 1e6) and the discus (one of 1e6,
+    n − 1 of 1) are rotated by a random orthogonal Q, so C has to learn a non-axis-aligned shape."""
+    r = np.random.default_rng(seed)
+    xs = r.uniform(0.2, 0.8, n)
+    if name == "rosenbrock":
+        def f(X):
+            Z = X - xs + 1.0
+            return (100.0 * (Z[:, 1:] - Z[:, :-1] ** 2) ** 2 + (1.0 - Z[:, :-1]) ** 2).sum(1)
+        return f, xs, None
+    Q = np.linalg.qr(r.standard_normal((n, n)))[0] if name != "sphere" else np.eye(n)
+    if name == "sphere":
+        s = np.ones(n)
+    elif name.startswith("ellipsoid"):
+        s = float(name[len("ellipsoid"):]) ** (np.arange(n) / max(n - 1, 1))
+    elif name == "cigar":
+        s = np.r_[1.0, np.full(n - 1, 1e6)]
+    elif name == "discus":
+        s = np.r_[1e6, np.ones(n - 1)]
+    else:
+        raise ValueError(name)
+
+    def f(X):
+        return (((X - xs) @ Q.T) ** 2 * s).sum(1)
+    return f, xs, 2.0 * (Q.T * s) @ Q

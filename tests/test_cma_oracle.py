@@ -86,3 +86,78 @@ def test_oracle_replays_its_committed_run_bit_for_bit():
             assert abs(st.sigma - z[f"{name}_sigma"][g]) <= 1e-13
             np.testing.assert_allclose(st.p_sigma, z[f"{name}_p_sigma"][g], rtol=0, atol=1e-13)
             np.testing.assert_allclose(st.pc, z[f"{name}_pc"][g], rtol=0, atol=1e-13)
+
+
+def test_eigen_floors_only_non_positive_eigenvalues():
+    """eigen keeps a positive eigenvalue below EPS as it is and replaces only zero or negative ones by EPS (checked against
+    eigh by hand); an exactly singular C gives a finite C^{-1/2}, where flooring only D² < 0 would divide by zero."""
+    r = np.random.default_rng(3)
+    lam = np.array([1.0, 1e-3, 1e-9, 0.0, -1e-12])
+    B, D = C.eigen(np.diag(lam))                                        # eigh is exact on a diagonal matrix
+    np.testing.assert_array_equal(np.sort(D), np.sqrt([C.EPS, C.EPS, 1e-9, 1e-3, 1.0])[[2, 0, 1, 3, 4]])
+    np.testing.assert_array_equal(np.abs(B), np.abs(B) @ np.eye(5))
+    Q = np.linalg.qr(r.standard_normal((5, 5)))[0]                     # rotated: the same rule on eigh's eigenvalues
+    A = Q @ np.diag(lam) @ Q.T
+    B, D = C.eigen(A)
+    ev = np.linalg.eigh((A + A.T) / 2)[0]
+    np.testing.assert_array_equal(D, np.sqrt(np.where(ev <= 0, C.EPS, ev)))
+    assert np.abs(D ** 2 - 1e-9).min() < 1e-14                          # kept, not raised to EPS
+    np.testing.assert_allclose(B.T @ B, np.eye(5), atol=1e-14)
+    # exact zero: diag(1, 0) has a zero eigenvalue that eigh returns exactly
+    B, D = C.eigen(np.diag([1.0, 0.0]))
+    assert np.all(np.isfinite(1.0 / D)) and sorted(D ** 2) == [C.EPS, 1.0]
+    s = C.CmaState(np.zeros(2), 0.5, 6)
+    s.C = np.diag([1.0, 0.0])
+    z = r.standard_normal((6, 2))
+    _, Y = C.ask(s, z)
+    C.tell(s, Y, C.sphere(Y))
+    assert np.all(np.isfinite(s.C)) and np.all(np.isfinite(s.p_sigma)) and np.isfinite(s.sigma)
+
+
+def test_tell_ranks_in_numpy_order():
+    """NaN ranks after +inf, -0 equals +0, ties go to the lower sample index: the same update as the finite values
+    listed in that order."""
+    z = np.random.default_rng(4).standard_normal((8, 3))
+    f = np.array([np.nan, np.inf, -0.0, -np.inf, 0.0, np.copysign(np.nan, -1.0), 1.0, 1.0])
+    order = [3, 2, 4, 6, 7, 1, 0, 5]
+    s1, s2 = C.CmaState(np.zeros(3), 1.0, 8), C.CmaState(np.zeros(3), 1.0, 8)
+    _, Y = C.ask(s1, z)
+    C.tell(s1, Y, f)
+    C.tell(s2, Y[order], np.arange(8.0))
+    np.testing.assert_array_equal(s1.mean, s2.mean)
+    np.testing.assert_array_equal(s1.C, s2.C)
+
+
+def test_tell_h_sigma_override():
+    s1, s2, s3 = (C.CmaState(np.zeros(4), 1.0, 8) for _ in range(3))
+    z = np.random.default_rng(5).standard_normal((8, 4))
+    _, Y = C.ask(s1, z)
+    f = C.sphere(Y)
+    C.tell(s1, Y, f)
+    C.tell(s2, Y, f, h_sigma=1.0)
+    C.tell(s3, Y, f, h_sigma=0.0)
+    assert np.array_equal(s1.pc, s2.pc) or np.array_equal(s1.pc, s3.pc)
+    assert np.array_equal(s3.pc, np.zeros(4)) and not np.array_equal(s2.pc, s3.pc)
+    assert s2.sigma == s3.sigma and np.array_equal(s2.p_sigma, s3.p_sigma)
+
+
+def test_objectives_have_their_minimum_inside_the_cube():
+    for n in (2, 4, 10, 32):
+        for name in C.OBJECTIVES:
+            f, xs, H = C.objective(name, n, seed=n)
+            assert np.all((0 < xs) & (xs < 1)) and f(xs[None])[0] == 0.0
+            X = np.random.default_rng(n).uniform(0, 1, (64, n))
+            assert np.all(f(X) > 0)
+            if H is None:
+                continue
+            # quadratic: f(x* + h) = ½ hᵀHh exactly (up to rounding), H has the advertised spectrum
+            h = X - xs
+            np.testing.assert_allclose(f(X), 0.5 * np.einsum("ki,ij,kj->k", h, H, h), rtol=1e-10)
+            ev = np.linalg.eigvalsh(H) / 2
+            cond = {"sphere": 1.0, "ellipsoid1e3": 1e3, "ellipsoid1e6": 1e6, "cigar": 1e6, "discus": 1e6}[name]
+            np.testing.assert_allclose(ev.max() / ev.min(), cond, rtol=1e-6)
+            if name in ("cigar", "discus"):
+                big = np.sum(ev > 1e3)
+                assert big == (n - 1 if name == "cigar" else 1)
+    f, xs, _ = C.objective("rosenbrock", 3)
+    assert f((xs + 1e-3)[None])[0] > 0
