@@ -759,7 +759,8 @@ def test_ranking_pass_on_a_flat_landscape_falls_back_and_still_decides_in_fp64()
 def test_cfg3_full_size_path_of_record():
     """BASELINE.json config 3 at full size through the path the bench times (array-free tensor-core sweep): N=8192, D=32,
     M=1,048,576, Matérn-5/2, EI.  The suggestion must be the FP64 engine's (same index, value to rounding) and the oracle's
-    value on the winner row and on a 4096-row sample must agree to 1e-5 with the winner dominating the sample."""
+    value on the winner row and on a 4096-row sample must agree to 1e-5 with the winner dominating the sample.  Every row of this
+    grid, every acquisition and gp_hedge against an FP64 posterior of the whole grid: test_gpu_grid_scale.py."""
     N, M, D = 8192, 1_048_576, 32
     X, y, _ = O.synthetic(N, 1, D)
     Xc = np.random.default_rng(4321).random((M, D)).astype(np.float32)
