@@ -115,7 +115,7 @@ int kbo_set_tc_refine(kbo_handle* h, int enabled);
 int kbo_last_contenders(kbo_handle* h);
 /* Tensor-core sweeps that return only the suggestion (no mu/std/acq arrays) rank the grid with ONE fp16 product per term —
  * a third of the MMAs — and keep every candidate that could still be the maximum given that pass's error on sigma²
- * (calibrated per sweep against the three-product kernel on the first wave of rows, x8 + 1e-6); the survivors are decided
+ * (calibrated per sweep against the three-product kernel on sm_count·64 rows stratified over the grid, x8 + 1e-6); the survivors are decided
  * by the FP64 refinement above, so the returned suggestion is unchanged.  More than 4096 survivors: the sweep is redone
  * with three products.  Default on; needs kbo_set_tc_refine and kbo_set_tc_pair on.  kbo_last_rank_error returns the
  * largest |sigma²(1 product) - sigma²(3 products)| seen on the calibration rows of the last such sweep. */

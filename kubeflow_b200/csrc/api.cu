@@ -524,4 +524,40 @@ int kbo_debug_kstar(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, 
   return KBO_OK;
 }
 
+// Test hook (not in kbo.h): the pruning pass's (tile_pairs >= 1) or the full ranking pass's (tile_pairs < 0) normalised mean and
+// variance of M candidate rows (device pointer) into caller-owned DEVICE float arrays.  Scratch is M × Npad fp16: callers slice
+// large grids (a row's values do not depend on the rows swept with it).
+int kbo_debug_rank_rows(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t M, int32_t tile_pairs, float* mun_out, float* varn_out, void* stream) {
+  if (!h) return KBO_ERR_INVALID;
+  if (!Xc || !mun_out || !varn_out || M < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_rank_rows: bad argument");
+  cudaSetDevice(h->device);
+  return kbo_i_debug_rank_rows(h, Xc, xc_dtype, M, tile_pairs, mun_out, varn_out, (cudaStream_t)stream);
+}
+
+// Test hooks (not in kbo.h): with recording on, each kbo_sweep / kbo_sweep_multi keeps, per stage it ran and per acquisition, the
+// bounds that stage pruned with and its survivor list (kbo_handle::StageRec); recording adds read-backs, never arithmetic.
+int kbo_debug_record_stages(kbo_handle* h, int32_t on) {
+  if (!h) return KBO_ERR_INVALID;
+  h->record_stages = on != 0;
+  h->stage_recs.clear();
+  return KBO_OK;
+}
+int kbo_debug_stage_count(kbo_handle* h) { return h ? (int)h->stage_recs.size() : KBO_ERR_INVALID; }
+// ints[4] = (stage, acquisition, calibration rows, survivors counted), floats[7] = (E, Eμ, raw max |dσ²|, raw max |dμ|, lower bound,
+// threshold, window delta); the first min(cap, list length) survivors go to list.  Returns the list length.
+int kbo_debug_stage(kbo_handle* h, int32_t i, int32_t* ints, float* floats, int32_t* list, int32_t cap) {
+  if (!h) return KBO_ERR_INVALID;
+  if (i < 0 || i >= (int)h->stage_recs.size() || !ints || !floats || cap < 0) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_stage: bad argument");
+  const kbo_handle::StageRec& r = h->stage_recs[i];
+  ints[0] = r.stage;
+  ints[1] = r.acq;
+  ints[2] = r.cal_n;
+  ints[3] = r.n;
+  for (int k = 0; k < 7; k++) floats[k] = r.f[k];
+  const int n = (int)r.list.size();
+  if (list)
+    for (int k = 0; k < n && k < cap; k++) list[k] = r.list[k];
+  return n;
+}
+
 }  // extern "C"

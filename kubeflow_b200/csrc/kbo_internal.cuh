@@ -88,6 +88,14 @@ struct kbo_handle {
   int dec_n = 0;                   // acquisitions the last kbo_sweep / kbo_sweep_multi decided, and how (kbo_last_decisions)
   int dec_unrefined[3] = {}, dec_contenders[3] = {}, dec_prefix_survivors[3] = {};
   DevBuf un_idx, un_mv;            // FP64 decision over the union of several acquisitions' survivors: indices / positions, mean + variance
+  // test hook (kbo_debug_record_stages): what each stage of the last kbo_sweep / kbo_sweep_multi kept, read back only when switched on
+  struct StageRec {
+    int stage, acq, cal_n, n;      // n: survivors counted; list holds the first min(n, the stage's cap) of them (grid-local indices)
+    float f[7];                    // E, Eμ, raw max |dσ²|, raw max |dμ|, lower bound on the maximum, threshold, window delta
+    std::vector<int> list;
+  };
+  bool record_stages = false;
+  std::vector<StageRec> stage_recs;
   // ---- fit: Cholesky chain on a high-priority stream, row-panel inverse on a second one (fit.cu) ----------------------
   cudaStream_t s_hi = nullptr, s_lo = nullptr, s_upd = nullptr, s_copy = nullptr;
   DevBuf T2;                        // N × 256 panel-solve scratch of the look-ahead factorisation (v2)
@@ -177,6 +185,7 @@ int kbo_i_lml_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int
 void kbo_i_lml_batch_free(kbo_handle* h);
 void kbo_i_fit_partition_free(kbo_handle* h);
 int kbo_i_ensure_w(kbo_handle* h, cudaStream_t s);   // form the rest of W and the full planes if the fit left them out
+int kbo_i_debug_rank_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int tile_pairs, float* mun_out, float* varn_out, cudaStream_t s);
 // ---- solve.cu ----------------------------------------------------------------------------------
 int kbo_i_alpha_by_solves(kbo_handle* h, cudaStream_t s);
 int kbo_i_variance_by_solves(kbo_handle* h, const double* Ks, int n, double* varn64, cudaStream_t s);

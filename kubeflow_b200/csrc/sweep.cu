@@ -4,6 +4,7 @@
 // Per candidate chunk:  cross_mean_kernel (FP64: K*, μ = K*·alpha)  →  variance contraction (FP64 SIMT GEMM with a
 // fused Σv² epilogue, or the wgmma kernel in tc_var.cu)  →  once per sweep: acquisition + argmax.
 #include <algorithm>
+#include <cstring>
 #include <type_traits>
 
 #include "kbo_internal.cuh"
@@ -872,6 +873,39 @@ static int refine_union(kbo_handle* h, const void* Xc, int xc_dtype, int64_t gof
   return KBO_OK;
 }
 
+// Test hook (kbo_debug_record_stages): one stage's bounds (fs[] as the stage's survivor kernel read it) and its survivor list.
+// Off by default; when off, nothing is read back and the sweep's launches and synchronisation are unchanged.
+enum { KBO_STAGE_LAZY_PRUNE = 0, KBO_STAGE_PRUNE = 1, KBO_STAGE_PRUNE_INTERVAL = 2, KBO_STAGE_INTERVAL = 3, KBO_STAGE_WINDOW = 4 };
+static int record_stage(kbo_handle* h, int stage, int acq, int cal_n, const float* fs_dev, const int* count_dev, const int* list_dev, int cap,
+                        float delta, cudaStream_t s) {
+  if (!h->record_stages) return KBO_OK;
+  kbo_handle::StageRec r{};
+  r.stage = stage;
+  r.acq = acq;
+  r.cal_n = cal_n;
+  float fs[5];
+  for (float& v : fs) v = NAN;
+  if (fs_dev) KBO_CUDA(h, cudaMemcpyAsync(fs, fs_dev, sizeof fs, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaMemcpyAsync(&r.n, count_dev, sizeof(int), cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  r.list.resize(r.n < cap ? r.n : cap);
+  if (!r.list.empty()) {
+    KBO_CUDA(h, cudaMemcpyAsync(r.list.data(), list_dev, sizeof(int) * r.list.size(), cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, cudaStreamSynchronize(s));
+  }
+  float lb = NAN;
+  if (fs_dev) {   // from_ordered_bits on the host; 0 (no bound set) decodes to NaN, as the survivor kernels read it
+    unsigned u;
+    memcpy(&u, &fs[1], sizeof u);
+    u = (u & 0x80000000u) ? (u & 0x7fffffffu) : ~u;
+    memcpy(&lb, &u, sizeof lb);
+  }
+  const float f[7] = {fs[0], fs[3], fs[2], fs[4], lb, lb - 1e-5f * fmaxf(1.f, fabsf(lb)), delta};
+  for (int k = 0; k < 7; k++) r.f[k] = f[k];
+  h->stage_recs.push_back(std::move(r));
+  return KBO_OK;
+}
+
 // contenders of the three-product sweep's window (see below) for one acquisition; a list that fits is handed to sp
 static int refine_suggestion(kbo_handle* h, int64_t M, int64_t goff, AcqDecision& d, StagePicks& sp, cudaStream_t s) {
   const double* scal = (const double*)h->scal.p;
@@ -900,6 +934,7 @@ static int refine_suggestion(kbo_handle* h, int64_t M, int64_t goff, AcqDecision
     delta = round < 22 ? delta * 0.25 : 0.0;   // the last attempt: exact ties of the maximum only
   }
   d.contenders = first_n;
+  KBO_TRY(record_stage(h, KBO_STAGE_WINDOW, d.acq, 0, nullptr, count, list, KBO_REFINE_CAP, (float)delta, s));
   if (n < 1 || n > KBO_REFINE_CAP) {
     d.unrefined = 2;
     d.done = true;   // keeps the tensor-core pick
@@ -982,6 +1017,9 @@ __device__ __forceinline__ void acq_bounds_f32(int acq, float mu, float var, flo
   const float l0 = acq_any_f32(acq, mu + Em, vlo, f), l1 = acq_any_f32(acq, mu + Em, vhi, f);
   *ub = fmaxf(u0, u1);
   *lb = fminf(l0, l1);
+  // PI where the box reaches σ = 0: acq_value_f32 gives 0 there, but Φ(imp/σ) → 1 as σ → 0 with a positive improvement — that
+  // supremum (as in acq_prefix_ub_f32), or a saturated PI near a trial would be pruned below a maximum of 1
+  if (acq == KBO_ACQ_PI && !(vlo > 0.f) && (f.chi - (mu - Em)) + f.clo > 0.f) *ub = 1.f;
 }
 __global__ void __launch_bounds__(256)
 bound_max_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int64_t M, int acq, const double* __restrict__ scal, double xi,
@@ -1246,6 +1284,7 @@ static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
     d.prefix_survivors = n1;
     h->last_rank_err = host.fs[2];
     h->last_rank_mu_err = host.fs[4];
+    KBO_TRY(record_stage(h, KBO_STAGE_LAZY_PRUNE, d.acq, cal_n, fs, pcount, plist, KBO_PRUNE_CAP, NAN, s));
     if (n1 < 1 || n1 > KBO_SOLVE_CAP) continue;
     d.contenders = n1;
     d.unrefined = 0;
@@ -1325,6 +1364,7 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     d.prefix_survivors = n1;
     h->last_rank_err = host.fs[2];
     h->last_rank_mu_err = host.fs[4];
+    KBO_TRY(record_stage(h, KBO_STAGE_PRUNE, d.acq, cal_n, fs, pcount, plist, KBO_PRUNE_CAP, NAN, s));
     if (n1 < 1 || n1 > KBO_PRUNE_CAP) continue;
     // pass 2: the survivors' rows through the whole ranking pass, then the interval test and the FP64 decision
     const int64_t n1_pad = round_up64(n1, 256);
@@ -1349,6 +1389,7 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     KBO_CUDA(h, cudaMemcpyAsync(&n2, count, sizeof(int), cudaMemcpyDeviceToHost, s));
     KBO_CUDA(h, cudaStreamSynchronize(s));
     d.contenders = n2;
+    KBO_TRY(record_stage(h, KBO_STAGE_PRUNE_INTERVAL, d.acq, cal_n, fs, count, list, KBO_REFINE_CAP, NAN, s));
     if (n2 < 1 || n2 > KBO_REFINE_CAP) continue;
     d.unrefined = 0;
     KBO_TRY(take_list(h, sp, d, list, n2, s));
@@ -1381,6 +1422,7 @@ static int fast_pick(kbo_handle* h, int64_t M, int cal_n, AcqDecision& d, StageP
   d.contenders = host.n;
   h->last_rank_err = host.fs[2];
   h->last_rank_mu_err = host.fs[4];
+  KBO_TRY(record_stage(h, KBO_STAGE_INTERVAL, d.acq, cal_n, fs, count, list, KBO_REFINE_CAP, NAN, s));
   if (host.n < 1 || host.n > KBO_REFINE_CAP) return KBO_OK;
   d.unrefined = 0;
   return take_list(h, sp, d, list, host.n, s);
@@ -1426,6 +1468,27 @@ int kbo_i_debug_cross_planes(kbo_handle* h, const void* Xc, int xc_dtype, int64_
   return launch_cross<float, float, 1>(h, (const float*)Xc, M, rows_pad, nullptr, 0, (__half*)h->Ksh.p, (__half*)h->Ksl.p, (float*)h->mun.p, s);
 }
 
+// Test hook: the ranking arithmetic of M rows as the pruning pass (tile_pairs >= 1: the first tile_pairs pairs of trial tiles, only
+// their columns of K̃* stored) or the full ranking pass (tile_pairs < 0, or all pairs) computes it: tensor-core K* and mean, then
+// the wgmma contraction.  A lazy fit forms the rest of W first where the pairs reach past its leading rows.
+int kbo_i_debug_rank_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int tile_pairs, float* mun_out, float* varn_out, cudaStream_t s) {
+  if (!h->fitted || !h->have_planes || !h->ks_ready)
+    KBO_FAIL(h, KBO_ERR_STATE, "kbo_debug_rank_rows: needs a fit with tensor-core planes and K* operands (D <= 128)");
+  const int Npad = h->Npad, n_pairs = (Npad / 256 + 1) / 2;
+  if (tile_pairs == 0) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_rank_rows: tile_pairs must be >= 1 or < 0");
+  const int P1 = (tile_pairs < 0 || tile_pairs > n_pairs) ? n_pairs : tile_pairs;
+  if (!h->w_full && (P1 == n_pairs || P1 * 512 > h->w_lead)) KBO_TRY(kbo_i_ensure_w(h, s));
+  const int64_t rows_pad = round_up64(M, 256);
+  KBO_TRY(kbo_reserve(h, h->Ksh, sizeof(__half) * (size_t)rows_pad * Npad));
+  KBO_TRY(kbo_reserve(h, h->mun, sizeof(float) * (size_t)(rows_pad + 256)));
+  KBO_TRY(kbo_reserve(h, h->varn, sizeof(float) * (size_t)(rows_pad + 256)));
+  KBO_TRY(kbo_i_tc_kstar(h, Xc, xc_dtype, M, (__half*)h->Ksh.p, (float*)h->mun.p, s, P1 < n_pairs ? P1 * 512 : -1));
+  KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, rows_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->varn.p, s, 0, P1));
+  KBO_CUDA(h, cudaMemcpyAsync(mun_out, h->mun.p, sizeof(float) * (size_t)M, cudaMemcpyDeviceToDevice, s));
+  KBO_CUDA(h, cudaMemcpyAsync(varn_out, h->varn.p, sizeof(float) * (size_t)M, cudaMemcpyDeviceToDevice, s));
+  return KBO_OK;
+}
+
 static void record_decisions(kbo_handle* h, const AcqDecision* dec, int n_acq) {
   h->dec_n = n_acq;
   for (int k = 0; k < n_acq; k++) {
@@ -1438,6 +1501,7 @@ static void record_decisions(kbo_handle* h, const AcqDecision* dec, int n_acq) {
 int kbo_i_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, double* mu_out, double* std_out, double* acq_out,
                 kbo_best* best_dev, cudaStream_t s) {
   AcqDecision d{h->prm.acq, best_dev, false, h->last_unrefined, h->last_contenders, h->last_prefix_survivors};
+  h->stage_recs.clear();
   const int r = sweep_impl(h, Xc, xc_dtype, M, goff, mu_out, std_out, acq_out, &d, 1, s, false);
   h->last_unrefined = d.unrefined;
   h->last_contenders = d.contenders;
@@ -1457,6 +1521,7 @@ int kbo_i_sweep_multi(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
     dec[k] = AcqDecision{acqs[k], best_dev + k, false, 0, 0, -1};
   }
   const float rank_err = h->last_rank_err, rank_mu_err = h->last_rank_mu_err;   // kbo_last_* keep reporting the last kbo_sweep
+  h->stage_recs.clear();
   const int r = sweep_impl(h, Xc, xc_dtype, M, goff, nullptr, nullptr, nullptr, dec, n_acq, s, false);
   h->last_rank_err = rank_err;
   h->last_rank_mu_err = rank_mu_err;

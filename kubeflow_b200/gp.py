@@ -222,6 +222,52 @@ class GPEngine:
             torch.cuda.current_stream(self.device).synchronize()
         return mu[:M], plane
 
+    def rank_rows(self, Xc, tile_pairs: int = -1, slice_rows: int = 131072):
+        """Test hook: the normalised mean and variance the pruning pass (``tile_pairs`` >= 1: the variance over the first
+        tile_pairs pairs of 256-trial tiles, an upper bound) or the full ranking pass (-1) computes for every row of the CUDA
+        tensor ``Xc``, as float32 CUDA tensors.  The grid goes through in slices of ``slice_rows`` (the hook's scratch is
+        slice_rows × N fp16)."""
+        if not (isinstance(Xc, torch.Tensor) and Xc.is_cuda):
+            raise ValueError("rank_rows takes a CUDA tensor")
+        Xc = Xc.contiguous()
+        dt = L.KBO_F64 if Xc.dtype == torch.float64 else L.KBO_F32
+        M = Xc.shape[0]
+        mu = torch.empty(M, dtype=torch.float32, device=Xc.device)
+        var = torch.empty(M, dtype=torch.float32, device=Xc.device)
+        with torch.cuda.device(self.device):
+            for r0 in range(0, M, slice_rows):
+                m = min(slice_rows, M - r0)
+                rc = self.lib.kbo_debug_rank_rows(self._h, Xc[r0:].data_ptr(), dt, int(m), int(tile_pairs), mu[r0:].data_ptr(),
+                                                  var[r0:].data_ptr(), self._stream())
+                L.check(self.lib, self._h, rc)
+            torch.cuda.current_stream(self.device).synchronize()
+        return mu, var
+
+    STAGES = ("lazy-prune", "prune", "prune-interval", "interval", "window")
+
+    def record_stages(self, on: bool = True):
+        """Test hook: keep, for every stage of each later ask / ask_multi and every acquisition, the bounds it pruned with and
+        its survivors (``stages()``).  Recording reads them back; it changes no arithmetic."""
+        L.check(self.lib, self._h, self.lib.kbo_debug_record_stages(self._h, int(bool(on))))
+        return self
+
+    def stages(self):
+        """The stages the last ask / ask_multi ran, in order: dicts of stage, acq, cal_n, n (survivors counted), E, E_mu,
+        dvar_raw / dmu_raw (the maxima E and E_mu came from), lb (lower bound on the maximum; NaN: none), thr (the survivor
+        threshold), delta (the three-product window) and survivors (grid-local indices, at most the stage's cap)."""
+        out = []
+        acq_names = {v: k for k, v in L.ACQS.items()}
+        for i in range(int(self.lib.kbo_debug_stage_count(self._h))):
+            ints, fl = (C.c_int32 * 4)(), (C.c_float * 7)()
+            n = self.lib.kbo_debug_stage(self._h, i, ints, fl, None, 0)
+            L.check(self.lib, self._h, min(n, 0))
+            lst = np.empty(max(n, 1), dtype=np.int32)
+            self.lib.kbo_debug_stage(self._h, i, ints, fl, lst.ctypes.data, n)
+            out.append(dict(stage=self.STAGES[ints[0]], acq=acq_names[ints[1]], cal_n=int(ints[2]), n=int(ints[3]),
+                            **dict(zip(("E", "E_mu", "dvar_raw", "dmu_raw", "lb", "thr", "delta"), (float(v) for v in fl))),
+                            survivors=np.sort(lst[:n].astype(np.int64))))
+        return out
+
     def lml_grad(self):
         """(lml, grad) of the last tell; grad w.r.t. (log amplitude, log noise, log ℓ_1..ℓ_P) as a NumPy array."""
         info = self.fit_info()

@@ -7,7 +7,8 @@ so that it can take a million candidates at N = 8192 on the GPU (device="cuda") 
   * X and Xc divided by ℓ (a scalar or one value per dimension), squared distances formed by exact differences summed over the
     dimensions (scipy cdist's arithmetic) — never as ‖a‖² + ‖b‖² − 2a·b, which cancels next to a trial point;
   * L = cholesky(amplitude·k(X, X) + noise·I), α = cholesky_solve(L, yn);
-  * per chunk of candidates: μ = K*·α, V = solve_triangular(L, K*ᵀ), σ² = amplitude − Σ V² clamped at 0, both un-normalised;
+  * per chunk of candidates: μ = K*·α, V = solve_triangular(L, K*ᵀ), σ² = amplitude − Σ V² clamped at 0, both un-normalised
+    (predict_normalised: μ_n, σ²_n unclamped and the prefix variances amplitude − Σ_{j<P} V_j², in normalised units);
   * EI / LCB / PI by oracle.acquisition on the host with y_opt = min(y).
 Float32 candidates are widened to float64 before anything else, as the engine widens them.  Temporaries stay under
 ``budget`` bytes (2 GiB by default), whatever the grid.
@@ -72,27 +73,53 @@ def fit(X, y, *, kind, length_scale, amplitude, noise, normalize_y=True, device=
                 amplitude=float(amplitude), lml=lml, budget=budget)
 
 
-def predict(f, Xc):
-    """oracle.gp_predict in torch: μ and σ of every row of Xc (host float64 arrays), in chunks whose K*, V and distance
-    temporaries fit the fit's budget."""
+def _chunks(f, Xc, prefixes=()):
+    """Per chunk of rows of Xc: (first row, μ_n = K*·α, σ²_n = amplitude − Σ V² unclamped, {P: amplitude − Σ_{j<P} V_j²}), all in
+    normalised units, as float64 tensors on the fit's device; chunks sized so that K*, V and the distance temporaries fit the
+    fit's budget."""
     dev = f["L"].device
     N, D = f["Xs"].shape
     M = Xc.shape[0]
     rows = max(1, f["budget"] // (4 * 8 * N))          # K*, V, and a quarter for the distance slabs and the row sums
-    mu = np.empty(M)
-    std = np.empty(M)
     for c0 in range(0, M, rows):
         A = _f64(Xc[c0:c0 + rows], dev) / f["ls"]
         Ks = kernel(A, f["Xs"], f["kind"], f["amplitude"], f["budget"] // 4)
         m = Ks @ f["alpha"]
         V = torch.linalg.solve_triangular(f["L"], Ks.T, upper=False)
         del Ks
-        var = f["amplitude"] - V.square_().sum(0)
+        V.square_()
+        var_p = {P: f["amplitude"] - V[:P].sum(0) for P in prefixes}
+        var = f["amplitude"] - V.sum(0)
         del V
+        yield c0, m, var, var_p
+
+
+def predict(f, Xc):
+    """oracle.gp_predict in torch: μ and σ of every row of Xc (host float64 arrays)."""
+    M = Xc.shape[0]
+    mu = np.empty(M)
+    std = np.empty(M)
+    for c0, m, var, _ in _chunks(f, Xc):
         var.clamp_(min=0.0)
-        mu[c0:c0 + rows] = (f["y_std"] * m + f["y_mean"]).cpu().numpy()
-        std[c0:c0 + rows] = torch.sqrt(var * f["y_std"] ** 2).cpu().numpy()
+        mu[c0:c0 + len(m)] = (f["y_std"] * m + f["y_mean"]).cpu().numpy()
+        std[c0:c0 + len(m)] = torch.sqrt(var * f["y_std"] ** 2).cpu().numpy()
     return mu, std
+
+
+def predict_normalised(f, Xc, prefixes=()):
+    """What the sweep's ranking arithmetic approximates, in normalised units (host float64 arrays): dict(mu_n = K*·α, var_n =
+    amplitude − Σ V² before any clamp, var_p = {P: amplitude − Σ_{j<P} V_j²}).  V = L⁻¹K*ᵀ, and its first P rows depend on
+    L[:P, :P] alone, so var_p[P] is the exact posterior variance given the first P trials: the upper bound a sweep forms from a
+    prefix of the trials.  It does not increase with P, and var_p[N] is var_n."""
+    M = Xc.shape[0]
+    out = dict(mu_n=np.empty(M), var_n=np.empty(M), var_p={P: np.empty(M) for P in prefixes})
+    for c0, m, var, var_p in _chunks(f, Xc, prefixes):
+        r = slice(c0, c0 + len(m))
+        out["mu_n"][r] = m.cpu().numpy()
+        out["var_n"][r] = var.cpu().numpy()
+        for P, v in var_p.items():
+            out["var_p"][P][r] = v.cpu().numpy()
+    return out
 
 
 def top2(a):

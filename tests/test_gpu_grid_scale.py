@@ -43,23 +43,15 @@ import torch
 
 from kubeflow_b200 import workload as W
 from oracle import gp_oracle as O
+from tests import _grid_cases as G
 from tests import _posterior_ref as R
 
 pytestmark = pytest.mark.gpu
 
 ACQS = R.ACQS
-M3 = 1_048_576
 
-# name -> history and grid (all at the θ of record unless stated): kernel, N, D, M, how the candidates reach the engine
-CASES = {
-    "cfg3": dict(kind="matern52", N=8192, D=32, M=M3, grid="cuda32"),
-    "cfg3-raw-y": dict(kind="matern52", N=8192, D=32, M=1_048_539, grid="host64", y=(2e4, 5.0)),
-    "cfg3-ard": dict(kind="matern52", N=8192, D=32, M=M3, grid="host32", ard=(0.5, 2.0)),
-    "n4097-rbf": dict(kind="rbf", N=4097, D=32, M=1_000_003, grid="cuda32"),
-    "cfg2": dict(kind="rbf", N=1024, D=8, M=65_536, grid="cuda32"),
-    "near-trials-1e-3": dict(kind="matern52", N=8192, D=32, M=M3, grid="host64", noise=1e-3, near=4096),
-    "near-trials-1e-6": dict(kind="matern52", N=8192, D=32, M=M3, grid="host64", noise=1e-6, near=4096),
-}
+# the cases of tests/_grid_cases.py this file runs
+SCALE_CASES = ("cfg3", "cfg3-raw-y", "cfg3-ard", "n4097-rbf", "cfg2", "near-trials-1e-3", "near-trials-1e-6")
 # (b): bounds on max |μ|, |σ| and |acquisition| of the FP64 engine against the reference, 4× the worst measured (header); the
 # acquisition bound is the ε of (c)-(f)
 BOUNDS = {"cfg3": (3.2e-12, 9.7e-14, 3.1e-12), "cfg3-raw-y": (6.0e-12, 1.4e-13, 1.2e-11), "cfg3-ard": (4.6e-12, 1.0e-13, 4.6e-12),
@@ -71,34 +63,10 @@ ORACLE_BOUND = {"cfg3": 1.7e-12, "cfg3-raw-y": 6.0e-12, "cfg3-ard": 2.5e-12, "n4
                 "near-trials-1e-6": 1.3e-10}
 
 
-def _case_data(name):
-    c = CASES[name]
-    N, D, M = c["N"], c["D"], c["M"]
-    X, y, _ = O.synthetic(N, 1, D)
-    if "y" in c:
-        y = c["y"][0] + c["y"][1] * y
-    th = O.theta_of_record(D)
-    if "ard" in c:
-        th["length_scale"] = th["length_scale"] * np.linspace(*c["ard"], D)
-    if "noise" in c:
-        th["noise"] = c["noise"]
-    Xc = W.candidates(M, D, dtype=np.float64 if c["grid"] == "host64" else np.float32)
-    near = None
-    if "near" in c:
-        r = np.random.default_rng(17)
-        n = c["near"]
-        near = r.choice(M, 2 * n, replace=False)
-        Xc[near[:n]] = X[r.choice(N, n, replace=False)]
-        Xc[near[n:]] = X[r.choice(N, n, replace=False)] + 1e-7 * (2 * r.random((n, D)) - 1)
-    if c["grid"] == "cuda32":
-        Xc = torch.tensor(Xc, device="cuda")
-    return dict(name=name, kind=c["kind"], X=X, y=y, Xc=Xc, M=M, theta=th, near=near, tc=name != "cfg2")
-
-
-@pytest.fixture(scope="module", params=list(CASES))
+@pytest.fixture(scope="module", params=SCALE_CASES)
 def case(request):
     """One case's data and its reference; pytest runs every check of a case before the next case is built."""
-    d = _case_data(request.param)
+    d = G.case_data(request.param)
     th = d["theta"]
     torch.cuda.synchronize()
     t0 = time.perf_counter()

@@ -110,3 +110,29 @@ def test_float32_candidates_are_widened():
     c = R.posterior(X, y, Xc32.astype(np.float64), **kw)
     for what in ("mu", "std"):
         assert np.array_equal(a[what], c[what]) and np.array_equal(b[what], c[what])
+
+
+@pytest.mark.parametrize("N,P", [(300, 128), (300, 1024), (2048, 1024)])
+def test_prefix_variance_against_the_oracle_inverse(N, P):
+    """predict_normalised: μ_n and σ²_n are the oracle's posterior in normalised units, σ²_P at P ≥ N is σ²_n, σ²_P never
+    increases with P, and σ²_P is amplitude − ‖(L⁻¹)[:P, :P] k*[:P]‖² with L the oracle's factor — the first P rows of L⁻¹ are
+    those of the inverse of L[:P, :P], so the prefix variance is the posterior given the first P trials."""
+    X, y, Xc = O.synthetic(N, 400, 6)
+    th = O.theta_of_record(6)
+    kw = dict(length_scale=th["length_scale"], amplitude=1.7, noise=1e-3)
+    f = R.fit(X, y, kind="matern52", device="cpu", **kw)
+    Ps = sorted({1, 64, P, N // 2, N})
+    r = R.predict_normalised(f, Xc, prefixes=Ps)
+    o = O.gp_fit(X, y, kind="matern52", **kw)
+    mu, sd = O.gp_predict(o, Xc)
+    np.testing.assert_allclose(r["mu_n"], (mu - o["y_mean"]) / o["y_std"], rtol=0, atol=1e-11)   # 2.4e-12 at N = 2048
+    np.testing.assert_allclose(np.maximum(r["var_n"], 0.0), (sd / o["y_std"]) ** 2, rtol=0, atol=1e-12)
+    assert np.array_equal(r["var_p"][N], r["var_n"])
+    for a, b in zip(Ps[:-1], Ps[1:]):
+        assert np.all(r["var_p"][b] <= r["var_p"][a] + 1e-14), (a, b)
+    p = min(P, N)
+    Ks = O.kernel_matrix(Xc, X[:p], kw["length_scale"], "matern52", kw["amplitude"])
+    Winv = np.linalg.inv(np.tril(o["L"][:p, :p]))
+    ref = kw["amplitude"] - ((Ks @ Winv.T) ** 2).sum(1)
+    np.testing.assert_allclose(r["var_p"][P], ref, rtol=0, atol=1e-11)
+    assert np.all(r["var_p"][P] >= r["var_n"] - 1e-14)
