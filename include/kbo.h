@@ -312,6 +312,42 @@ int kbo_cma_state(kbo_handle* h, kbo_cma* c, double* mean, double* sigma, double
 int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32_t generations, double* best_f_host,
                           float* elapsed_ms, double* jacobi_sweeps_last);
 
+/* ---- TPE (Katib algorithm `tpe`: hyperopt's tpe.suggest on a flat space; FP64 restatement oracle/tpe_oracle.py) -------
+ * Parameter kinds: UNIFORM = uniform(lo, hi); QUNIFORM = quniform(lo, hi, q), values rint(x/q)·q; CHOICE = choice over
+ * `levels` categories, observed and reported as the category index.
+ *   kbo_tpe_create: D parameters (HOST arrays kinds, lo, hi, q, levels; lo/hi/q are read for numeric kinds, levels for
+ *                   choices), gamma in (0, 1), prior_weight > 0, seed (random_state).
+ *   kbo_tpe_tell  : appends n_new trials in told order: X (n_new×D, parameter units) and losses (minimised; non-finite losses
+ *                   rank in NumPy's order, NaN last).  Device pointers, or host pointers with on_host = 1 (then synchronises).
+ *   kbo_tpe_ask   : k points, each with its own n_candidates draws per parameter from the below model (Philox4x32-10 keyed by
+ *                   (seed, ask counter, point, parameter, candidate)), or the caller's candidates cand_dev (k×D×n_candidates,
+ *                   device, fp64: numeric values before quantization, category indices for choices).  Each parameter takes
+ *                   the candidate at the first index of the maximum of log l(x) - log g(x); continuous parameters are scored
+ *                   in FP32 with an error bound and every candidate that can still be the maximum is decided in FP64;
+ *                   quantized and categorical parameters score each distinct value present once, in FP64.
+ *                   x_dev: k×D fp64 suggestions (device); optional device outputs: idx_dev (k×D winning candidate indices),
+ *                   cand_out_dev (k×D×n_candidates: the draws), score_out_dev (k×D×n_candidates×2 floats: FP32 score and
+ *                   its bound, continuous parameters only).  Synchronises.  1 <= n_candidates <= 2^24, k·D <= 65535.
+ *   kbo_tpe_state : the models of the current history (built on demand), HOST outputs, any may be NULL: for a numeric
+ *                   parameter the group's (0 below, 1 above) mixture weights, means, sigmas (first cap of ncomp components) and
+ *                   p_accept; for a choice the group's category probabilities (w, ncomp = categories).  Synchronises.
+ *   kbo_tpe_last_survivors: per (point, parameter) of the last ask, the candidates decided in FP64 (continuous) or the
+ *                   distinct values scored (quantized, categorical).  Returns k·D, fills up to n entries.
+ *   kbo_tpe_last_timings: milliseconds of the last ask's phases (models, FP32 score, FP64 decision, discrete parameters, final
+ *                   reduction), CUDA events on its stream.  Returns 5, fills up to n entries. */
+typedef enum kbo_tpe_kind { KBO_TPE_UNIFORM = 0, KBO_TPE_QUNIFORM = 1, KBO_TPE_CHOICE = 2 } kbo_tpe_kind;
+typedef struct kbo_tpe kbo_tpe;
+int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds, const double* lo, const double* hi, const double* q,
+                   const int32_t* levels, double gamma, double prior_weight, uint64_t seed);
+void kbo_tpe_destroy(kbo_tpe* t);
+int kbo_tpe_tell(kbo_handle* h, kbo_tpe* t, const double* X, const double* loss, int32_t n_new, int on_host, void* stream);
+int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t n_candidates, const double* cand_dev, double* x_dev, int64_t* idx_dev,
+                double* cand_out_dev, float* score_out_dev, void* stream);
+int kbo_tpe_state(kbo_handle* h, kbo_tpe* t, int32_t param, int32_t group, double* w, double* mu, double* sigma, int32_t cap,
+                  int32_t* ncomp, double* p_accept, int32_t* n_below, void* stream);
+int kbo_tpe_last_survivors(kbo_handle* h, kbo_tpe* t, int32_t* out, int32_t n);
+int kbo_tpe_last_timings(kbo_handle* h, kbo_tpe* t, float* ms, int32_t n);
+
 #ifdef __cplusplus
 }
 #endif

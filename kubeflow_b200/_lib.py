@@ -54,7 +54,8 @@ EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_se
            "kbo_comm_unique_id", "kbo_comm_init", "kbo_comm_destroy", "kbo_comm_size", "kbo_allreduce_argmax", "kbo_suggest_host", "kbo_last_timings",
            "kbo_gram", "kbo_potrf", "kbo_trtri", "kbo_acq_argmax",
            "kbo_req_open", "kbo_req_close", "kbo_req_header", "kbo_req_trials", "kbo_hash64",
-           "kbo_cma_create", "kbo_cma_destroy", "kbo_cma_ask", "kbo_cma_tell", "kbo_cma_state", "kbo_cma_run_synthetic"]
+           "kbo_cma_create", "kbo_cma_destroy", "kbo_cma_ask", "kbo_cma_tell", "kbo_cma_state", "kbo_cma_run_synthetic",
+           "kbo_tpe_create", "kbo_tpe_destroy", "kbo_tpe_tell", "kbo_tpe_ask", "kbo_tpe_state", "kbo_tpe_last_survivors", "kbo_tpe_last_timings"]
 
 _lib = None
 
@@ -143,6 +144,14 @@ def load() -> C.CDLL:
     lib.kbo_cma_tell.argtypes = [vp, vp, vp, vp]
     lib.kbo_cma_state.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i64), vp]
     lib.kbo_cma_run_synthetic.argtypes = [vp, vp, i32, i32, pd, C.POINTER(C.c_float), pd]
+    lib.kbo_tpe_create.argtypes = [vp, C.POINTER(vp), i32, vp, vp, vp, vp, vp, dbl, dbl, C.c_uint64]
+    lib.kbo_tpe_destroy.argtypes = [vp]
+    lib.kbo_tpe_destroy.restype = None
+    lib.kbo_tpe_tell.argtypes = [vp, vp, vp, vp, i32, C.c_int, vp]
+    lib.kbo_tpe_ask.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp, vp]
+    lib.kbo_tpe_state.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, vp, vp, vp, vp]
+    lib.kbo_tpe_last_survivors.argtypes = [vp, vp, vp, i32]
+    lib.kbo_tpe_last_timings.argtypes = [vp, vp, vp, i32]
     lib.kbo_tc_variance_raw.argtypes = [vp, vp, vp, i64, vp, vp, i32, vp, dbl, vp, vp, i32, vp]
     for name in EXPORTS + ["kbo_tc_variance_raw", "kbo_debug_rank_pass", "kbo_debug_kstar", "kbo_debug_rank_rows", "kbo_debug_record_stages",
                            "kbo_debug_stage_count", "kbo_debug_stage", "kbo_debug_fp64_peak", "kbo_debug_dgemm_sm90"]:

@@ -9,6 +9,7 @@
 // kernel and the whole state lives in HBM/L2 between them; nothing returns to the host until the caller asks.
 #include "kbo_internal.cuh"
 #include "dgemm.cuh"
+#include "kbo_rng.cuh"
 
 #define CMA_EPS 1e-8
 #define CMA_MAXD 128
@@ -25,19 +26,7 @@ struct kbo_cma {
 
 enum CmaScal { CS_SIGMA = 0, CS_ALPHA_C = 1, CS_BEST_F = 2, CS_SWEEPS = 3, CS_COUNT = 8 };
 
-// ------------------------------------------------------------------------------------------------ RNG
-__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1, uint32_t (&out)[4]) {
-#pragma unroll
-  for (int r = 0; r < 10; r++) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-    const uint32_t n0 = hi1 ^ c1 ^ k0, n1 = lo1, n2 = hi0 ^ c3 ^ k1, n3 = lo0;
-    c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-  out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
+// ------------------------------------------------------------------------------------------------ RNG (philox4x32_10: kbo_rng.cuh)
 // two standard normals per call from 128 random bits (53-bit uniforms, Box–Muller in FP64)
 __global__ void cma_normal_kernel(double* __restrict__ Z, int64_t n, uint64_t seed, uint64_t gen) {
   const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;  // pair index

@@ -65,6 +65,7 @@ def main():
     from .cmaes_service import CmaesService
     from .hyperband import HyperbandService
     from .service import DispatchService, RandomService, SkoptService, SobolService
+    from .tpe_service import TpeService
     ap = argparse.ArgumentParser()
     ap.add_argument("--port", type=int, default=DEFAULT_PORT)
     ap.add_argument("--device", type=int, default=0)
@@ -82,7 +83,7 @@ def main():
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
         inner = DispatchService([SkoptService({"device": local, "shard": True}), RandomService(), SobolService(),
-                                 CmaesService(), HyperbandService()])
+                                 CmaesService(), TpeService({"device": local}), HyperbandService()])
         spmd = SpmdServicer(inner)
         if dist.get_rank() == 0:
             server, port = serve(spmd, args.port)
@@ -95,7 +96,8 @@ def main():
             spmd.worker_loop()
         dist.destroy_process_group()
         return
-    server, port = serve(DispatchService([SkoptService({"device": args.device}), RandomService(), SobolService(), CmaesService(), HyperbandService()]), args.port)
+    server, port = serve(DispatchService([SkoptService({"device": args.device}), RandomService(), SobolService(), CmaesService(),
+                                         TpeService({"device": args.device}), HyperbandService()]), args.port)
     logging.info("api.v1.beta1.Suggestion listening on :%d", port)
     server.wait_for_termination()
 

@@ -81,6 +81,34 @@ def validate_skopt_settings(settings: dict) -> dict:
     return out
 
 
+def experiment_fingerprint(exp, search_space, settings: dict) -> tuple:
+    """What a cached per-experiment state depends on: goal, objective metric, the search space and the parsed settings."""
+    return (search_space.goal, exp.spec.objective.objective_metric_name,
+            tuple((p.name, p.type, p.min, p.max, tuple(p.list), p.step) for p in search_space.params),
+            tuple(sorted((k, repr(v)) for k, v in settings.items())))
+
+
+def cached_experiment(cache: dict, name: str, fingerprint, make, close, max_entries: int):
+    """The per-experiment state of ``name`` from ``cache`` (a dict kept in least-recently-used order), made by ``make()`` when
+    absent.  An experiment recreated under the same name, or whose search space / objective / settings changed, must not meet
+    the old state (old dimensions, old history, old settings): an entry is valid for one fingerprint only, and a stale one is
+    closed and replaced.  Each entry may own a libkbo handle (device memory), so past ``max_entries`` the least recently used
+    entries are closed and dropped.  Call with the service's lock held."""
+    entry = cache.get(name)
+    if entry is not None and entry.fingerprint != fingerprint:
+        close(cache.pop(name))
+        entry = None
+    if entry is None:
+        entry = make()
+        entry.fingerprint = fingerprint
+        cache[name] = entry
+        while len(cache) > max_entries:
+            close(cache.pop(next(iter(cache))))
+    else:
+        cache[name] = cache.pop(name)      # mark as most recently used
+    return entry
+
+
 def _reply_from(assignment_lists) -> "api.GetSuggestionsReply":
     reply = api.GetSuggestionsReply()
     for assignments in assignment_lists:
@@ -146,38 +174,35 @@ class SkoptService(_Base):
         settings = validate_skopt_settings(parse_settings(exp))
         from .ingest import LazyRequest
         lazy = request if isinstance(request, LazyRequest) and request.scanned else None
-        # an experiment recreated under the same name, or whose search space / objective / settings changed, must not meet the
-        # old optimizer (old dimensions, old history, old settings): the cache entry is valid for one fingerprint only
-        fingerprint = (search_space.goal, exp.spec.objective.objective_metric_name,
-                       tuple((p.name, p.type, p.min, p.max, tuple(p.list), p.step) for p in search_space.params),
-                       tuple(sorted((k, repr(v)) for k, v in settings.items())))
+        fingerprint = experiment_fingerprint(exp, search_space, settings)
         with self._lock:
-            svc = self._services.get(exp.name)
-            if svc is not None and svc.fingerprint != fingerprint:
-                eng = getattr(self._services.pop(exp.name).skopt_optimizer, "_engine", None)
-                if eng is not None:
-                    eng.close()
-                svc = None
-            if svc is None:
+            def make():
                 kw = dict(self.engine_defaults)
                 kw.update(settings)
                 from .base_service import BaseSkoptService
-                svc = BaseSkoptService(search_space=search_space, **kw)
-                svc.fingerprint = fingerprint
-                self._services[exp.name] = svc
-                while len(self._services) > self.max_experiments:       # evict the least recently used experiment's engine
-                    old_name = next(iter(self._services))
-                    old = self._services.pop(old_name)
-                    eng = getattr(old.skopt_optimizer, "_engine", None)
-                    if eng is not None:
-                        eng.close()
-            else:
-                self._services[exp.name] = self._services.pop(exp.name)  # mark as most recently used
+                return BaseSkoptService(search_space=search_space, **kw)
+
+            def close(old):
+                eng = getattr(old.skopt_optimizer, "_engine", None)
+                if eng is not None:
+                    eng.close()
+            svc = cached_experiment(self._services, exp.name, fingerprint, make, close, self.max_experiments)
             # the wire scan tells the new trials from flat arrays; it declines (False) whenever a trial needs the message walk
             self.last_ingest = "scan" if (lazy is not None and svc.ingest(lazy)) else "messages"
             trials = [] if self.last_ingest == "scan" else Trial.convert(request.trials, skip_names=svc.told_trials)
             lists = svc.getSuggestions(trials, max(int(request.current_request_number), 0))
         return _reply_from(lists)
+
+
+def prior_points(ss, rng, n: int) -> list:
+    """n uniform random points of the search space (integers uniform over [min, max], categories uniform), in parameter
+    values — the sampling of Katib's ``random`` algorithm, shared with ``tpe``'s start-up phase."""
+    from ..space import Categorical, Integer, Real, Space
+    from .internal import DOUBLE, INTEGER
+    dims = [Integer(int(p.min), int(p.max), p.name) if p.type == INTEGER else
+            Real(float(p.min), float(p.max), p.name) if p.type == DOUBLE else Categorical(list(p.list), p.name) for p in ss.params]
+    space = Space(dims)
+    return space.inverse_transform(space.rvs_transformed(n, rng, np.float64)) if n else []
 
 
 class RandomService(_Base):
@@ -202,9 +227,7 @@ class RandomService(_Base):
                 raise AlgorithmSettingsError(f"random_state should be great or equal than zero, got {v}")
 
     def get_suggestions(self, request):
-        from ..space import Categorical, Integer, Real, Space
         from .base_service import BaseSkoptService
-        from .internal import CATEGORICAL, DISCRETE, DOUBLE, INTEGER
         exp = request.experiment
         ss = HyperParameterSearchSpace.convert(exp)
         st = parse_settings(exp)
@@ -212,13 +235,7 @@ class RandomService(_Base):
             rng = self._rngs.get(exp.name)
             if rng is None:
                 rng = self._rngs[exp.name] = np.random.default_rng(int(st["random_state"]) if "random_state" in st else None)
-            dims = []
-            for p in ss.params:
-                dims.append(Integer(int(p.min), int(p.max), p.name) if p.type == INTEGER else
-                            Real(float(p.min), float(p.max), p.name) if p.type == DOUBLE else Categorical(list(p.list), p.name))
-            space = Space(dims)
-            n = max(int(request.current_request_number), 0)
-            pts = space.inverse_transform(space.rvs_transformed(n, rng, np.float64)) if n else []
+            pts = prior_points(ss, rng, max(int(request.current_request_number), 0))
         return _reply_from([BaseSkoptService.convert(ss, p) for p in pts])
 
 

@@ -1,0 +1,188 @@
+"""``tpe`` — Katib's hyperopt-backed Tree-structured Parzen Estimator (the second algorithm of the upstream hyperopt image) on
+the GPU engine ``kubeflow_b200.tpe`` (contract: oracle/tpe_oracle.py).
+
+* Space: DOUBLE → uniform(min, max) (``step`` ignored, as the other services here ignore it); INT → quniform(min, max, q), q =
+  ``step`` or 1, reported as integers; CATEGORICAL / DISCRETE → choice(list), observed as the category index.
+* History: the usable trials (``Trial.convert``), each told once by name, kept in the order first told; loss = objective value,
+  negated for MAXIMIZE.
+* While fewer than ``n_startup_jobs`` trials are told, points come from the prior — the sampling ``random`` uses — and no GPU
+  handle exists.  Then every request scores ``n_EI_candidates`` draws per parameter and point on the device.
+* Batches (``current_request_number`` = k > 1): every point gets its own independent draws against the same model, with no
+  lies in between.  [RECALL] hyperopt 0.2's ``tpe.suggest`` builds the posterior once per call and draws each new id's
+  candidates from it in turn, which is the same thing up to the random stream; Katib's hyperopt service passes
+  ``n_startup_jobs = current_request_number`` to it, where this service honours the ``n_startup_jobs`` setting.
+* Draws are keyed by (random_state, ask counter, point, parameter, candidate): the same request sequence gives the same
+  replies.
+"""
+from __future__ import annotations
+
+import threading
+
+import numpy as np
+
+from .internal import (DISCRETE, DOUBLE, INTEGER, MAX_GOAL, AlgorithmSettingsError, HyperParameterSearchSpace, Trial,
+                       parse_settings, Assignment)
+from .service import _Base, _reply_from, cached_experiment, experiment_fingerprint, prior_points
+
+MAX_EI_CANDIDATES = 1 << 24
+
+
+def validate_tpe_settings(settings: dict) -> dict:
+    """Parsed settings with defaults, or AlgorithmSettingsError naming the setting [RECALL: Katib's hyperopt validation]."""
+    out = dict(gamma=0.25, prior_weight=1.0, n_EI_candidates=24, n_startup_jobs=20)
+    for k, v in settings.items():
+        try:
+            if k == "gamma":
+                out[k] = float(v)
+                if not 0.0 < out[k] < 1.0:
+                    raise AlgorithmSettingsError(f"gamma should be in the range of (0, 1), got {v}")
+            elif k == "prior_weight":
+                out[k] = float(v)
+                if not (out[k] > 0.0 and np.isfinite(out[k])):
+                    raise AlgorithmSettingsError(f"prior_weight should be greater than zero, got {v}")
+            elif k == "n_EI_candidates":
+                out[k] = int(v)
+                if not 1 <= out[k] <= MAX_EI_CANDIDATES:
+                    raise AlgorithmSettingsError(f"n_EI_candidates should be in [1, 2^24], got {v}")
+            elif k == "n_startup_jobs":
+                out[k] = int(v)
+                if out[k] < 0:
+                    raise AlgorithmSettingsError(f"n_startup_jobs should be great or equal than zero, got {v}")
+            elif k == "random_state":
+                out[k] = int(v)
+                if out[k] < 0:
+                    raise AlgorithmSettingsError(f"random_state should be great or equal than zero, got {v}")
+            elif k == "device":
+                out[k] = int(v)
+                if out[k] < 0:
+                    raise AlgorithmSettingsError(f"device should be great or equal than zero, got {v}")
+            else:
+                raise AlgorithmSettingsError(f"unknown setting {k} for algorithm tpe")
+        except AlgorithmSettingsError:
+            raise
+        except (TypeError, ValueError):
+            raise AlgorithmSettingsError(f"failed to convert {v!r} for setting {k}")
+    return out
+
+
+def tpe_space(ss) -> list:
+    """The engine's parameter list for a Katib search space."""
+    out = []
+    for p in ss.params:
+        if p.type == DOUBLE:
+            out.append(("uniform", float(p.min), float(p.max)))
+        elif p.type == INTEGER:
+            q = float(p.step) if p.step else 1.0
+            if not q > 0:
+                raise AlgorithmSettingsError(f"parameter {p.name!r}: step must be > 0, got {p.step}")
+            out.append(("quniform", float(p.min), float(p.max), q))
+        else:
+            out.append(("choice", len(p.list)))
+    return out
+
+
+class _Experiment:
+    def __init__(self, ss, settings):
+        self.ss, self.settings = ss, settings
+        self.space = tpe_space(ss)
+        self.rows, self.losses, self.told = [], [], set()
+        self.rng = np.random.default_rng(settings.get("random_state"))       # start-up phase (None: fresh entropy)
+        self.seed = settings["random_state"] if "random_state" in settings else int(self.rng.integers(1 << 62))
+        self.engine = None       # kubeflow_b200.tpe.Tpe, created at the first model-based ask
+        self.n_engine = 0        # rows told to the engine
+
+    def close(self):
+        if self.engine is not None:
+            self.engine.close()
+            self.engine = None
+
+    def row(self, trial) -> list:
+        by_name = {a.name: a.value for a in trial.assignments}
+        row = []
+        for p in self.ss.params:
+            v = by_name.get(p.name)
+            if v is None:
+                raise ValueError(f"trial {trial.name!r} has no assignment for parameter {p.name!r}")
+            if p.type in (DOUBLE, INTEGER):
+                row.append(float(v))
+            elif v in p.list:
+                row.append(float(p.list.index(v)))
+            else:
+                hit = [i for i, c in enumerate(p.list) if p.type == DISCRETE and _same_number(c, v)]
+                if not hit:
+                    raise ValueError(f"trial {trial.name!r}: {v!r} is not in the feasible list of {p.name!r}")
+                row.append(float(hit[0]))
+        return row
+
+    def assignments(self, x) -> list:
+        out = []
+        for p, v in zip(self.ss.params, x):
+            if p.type == DOUBLE:
+                out.append(Assignment(p.name, repr(float(v))))
+            elif p.type == INTEGER:
+                out.append(Assignment(p.name, str(int(v))))
+            else:
+                out.append(Assignment(p.name, str(p.list[int(v)])))
+        return out
+
+
+def _same_number(a: str, b: str) -> bool:
+    try:
+        return float(a) == float(b)
+    except ValueError:
+        return False
+
+
+class TpeService(_Base):
+    algorithm_names = ("tpe",)
+
+    def __init__(self, engine_defaults: dict | None = None, max_experiments: int = 8):
+        self._lock = threading.Lock()
+        self._exps = {}                     # experiment name -> _Experiment, least-recently-used first
+        self.engine_defaults = dict(engine_defaults or {})
+        self.max_experiments = int(max_experiments)   # each experiment past its start-up phase owns a libkbo handle
+
+    def validate(self, experiment):
+        if experiment.spec.algorithm.algorithm_name != "tpe":
+            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        tpe_space(HyperParameterSearchSpace.convert(experiment))
+        validate_tpe_settings(parse_settings(experiment))
+
+    def get_suggestions(self, request):
+        exp = request.experiment
+        if exp.spec.algorithm.algorithm_name != "tpe":
+            raise AlgorithmSettingsError(f"unknown algorithm name {exp.spec.algorithm.algorithm_name}")
+        ss = HyperParameterSearchSpace.convert(exp)
+        tpe_space(ss)
+        raw = parse_settings(exp)
+        settings = validate_tpe_settings(raw)
+        settings.update({k: v for k, v in self.engine_defaults.items() if k not in raw})
+        k = max(int(request.current_request_number), 0)
+        with self._lock:
+            st = cached_experiment(self._exps, exp.name, experiment_fingerprint(exp, ss, settings), lambda: _Experiment(ss, settings),
+                                   lambda old: old.close(), self.max_experiments)
+            rows, losses, names = [], [], []
+            for t in Trial.convert(request.trials, skip_names=st.told):
+                if t.name in names:
+                    continue
+                loss = float(t.target_metric.value)
+                rows.append(st.row(t))
+                losses.append(-loss if ss.goal == MAX_GOAL else loss)
+                names.append(t.name)
+            st.rows += rows
+            st.losses += losses
+            st.told.update(names)        # only once every new trial converted: a bad one fails the request and is told later
+            if k == 0:
+                return _reply_from([])
+            if len(st.rows) < settings["n_startup_jobs"]:
+                from .base_service import BaseSkoptService
+                return _reply_from([BaseSkoptService.convert(ss, p) for p in prior_points(ss, st.rng, k)])
+            if st.engine is None:
+                from ..tpe import Tpe
+                st.engine = Tpe(st.space, gamma=settings["gamma"], prior_weight=settings["prior_weight"], seed=st.seed,
+                                device=int(settings.get("device", 0)))
+            if st.n_engine < len(st.rows):
+                st.engine.tell(np.asarray(st.rows[st.n_engine:]), np.asarray(st.losses[st.n_engine:]))
+                st.n_engine = len(st.rows)
+            X = st.engine.ask(k, settings["n_EI_candidates"])
+        return _reply_from([st.assignments(x) for x in X])

@@ -47,3 +47,9 @@ for N, M, D, mode in ((70, 300, 3, "f64"), (135, 515, 5, "tc"), (300, 700, 33, "
 es = CmaEs(np.zeros(9), 1.0, popsize=20, seed=1)
 print(es.run_synthetic("sphere", 3))
 es.close()
+from kubeflow_b200.tpe import Tpe                     # TPE: model build (radix + segmented sorts), draws, FP32 score + FP64 decision, levels
+_r = np.random.default_rng(3)
+tp = Tpe([("uniform", -1.0, 3.0), ("quniform", 3.0, 48.0, 5.0), ("choice", 5), ("quniform", 0.0, 1e6, 1.0)], seed=9)
+tp.tell(np.c_[_r.uniform(-1, 3, 300), 5.0 * _r.integers(1, 10, 300), _r.integers(0, 5, 300), _r.integers(0, 10 ** 6, 300)], _r.random(300))
+print(tp.ask(2, 3000).tolist(), tp.last_survivors().tolist(), tp.state()[0]["below"]["w"].shape)
+tp.close()
