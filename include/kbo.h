@@ -348,6 +348,45 @@ int kbo_tpe_state(kbo_handle* h, kbo_tpe* t, int32_t param, int32_t group, doubl
 int kbo_tpe_last_survivors(kbo_handle* h, kbo_tpe* t, int32_t* out, int32_t n);
 int kbo_tpe_last_timings(kbo_handle* h, kbo_tpe* t, float* ms, int32_t n);
 
+/* ---- multivariate TPE (Katib algorithm `multivariate-tpe`: Optuna's TPESampler(multivariate=True) on a flat space; FP64
+ * restatement oracle/mvtpe_oracle.py) ------------------------------------------------------------------------------------
+ * Parameter kinds: FLOAT on [lo, hi]; INT on the grid lo, lo + q, ... <= hi (q = step), values are grid points; CAT over
+ * `levels` categories, observed and reported as the category index.  Optuna's defaults are fixed: consider_prior,
+ * prior_weight = 1, consider_magic_clip, no endpoints.
+ *   kbo_mvtpe_create: D parameters (HOST arrays kinds, lo, hi, q, levels; lo/hi are read for FLOAT and INT, q for INT, levels
+ *                   for CAT), seed (random_state).  1 <= D <= 65535.
+ *   kbo_mvtpe_tell  : appends n_new trials in told order: X (n_new×D, parameter units) and losses (minimised; ±inf rank).
+ *                   Device pointers, or host pointers with on_host = 1.  A NaN loss, a float outside [lo, hi], an integer
+ *                   off its grid or an invalid category index fails the call and tells nothing.  Synchronises.
+ *   kbo_mvtpe_ask   : k points, each the best of its own n_candidates candidate vectors drawn from the below mixture
+ *                   (Philox4x32-10 keyed by (seed, ask counter, point, candidate, slot)), or of the caller's candidates
+ *                   cand_dev (k×D×n_candidates, device, fp64; integers are rounded to the grid and clipped, a float outside
+ *                   [lo, hi] or an invalid category index is an error).  The winner is the candidate at the first index of
+ *                   the maximum of log l(x) - log g(x): every candidate is scored in FP32 with an error bound and every one
+ *                   that can still be the maximum is decided in FP64.  x_dev: k×D fp64 suggestions (device); optional
+ *                   device outputs: idx_dev (k winning candidate indices), cand_out_dev (k×D×n_candidates: the candidates
+ *                   as scored), score_out_dev (k×n_candidates×2 floats: FP32 score and its bound).  Synchronises.
+ *                   1 <= k <= 65535, 1 <= n_candidates <= 2^24.
+ *   kbo_mvtpe_state : the models of the current history (built on demand) for group 0 (below) or 1 (above), HOST outputs, any
+ *                   may be NULL: w (the first cap of n_obs + 1 weights: observations in told order, then the prior), sigma
+ *                   (D; NaN for categoricals), mu (the first cap observations' values, cap×D), cat_rows (2×D: an observation
+ *                   row's entry at its own category and elsewhere; NaN for other kinds), n_obs, n_below.  Synchronises.
+ *   kbo_mvtpe_last_survivors: per point of the last ask, the candidates decided in FP64.  Returns k, fills up to n entries.
+ *   kbo_mvtpe_last_timings: milliseconds of the last ask's phases (models and draws, FP32 score, FP64 decision, final
+ *                   reduction), CUDA events on its stream.  Returns 4, fills up to n entries. */
+typedef enum kbo_mvtpe_kind { KBO_MVTPE_FLOAT = 0, KBO_MVTPE_INT = 1, KBO_MVTPE_CAT = 2 } kbo_mvtpe_kind;
+typedef struct kbo_mvtpe kbo_mvtpe;
+int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* kinds, const double* lo, const double* hi, const double* q,
+                     const int32_t* levels, uint64_t seed);
+void kbo_mvtpe_destroy(kbo_mvtpe* t);
+int kbo_mvtpe_tell(kbo_handle* h, kbo_mvtpe* t, const double* X, const double* loss, int32_t n_new, int on_host, void* stream);
+int kbo_mvtpe_ask(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t n_candidates, const double* cand_dev, double* x_dev, int64_t* idx_dev,
+                  double* cand_out_dev, float* score_out_dev, void* stream);
+int kbo_mvtpe_state(kbo_handle* h, kbo_mvtpe* t, int32_t group, double* w, double* sigma, double* mu, double* cat_rows, int32_t cap,
+                    int32_t* n_obs, int32_t* n_below, void* stream);
+int kbo_mvtpe_last_survivors(kbo_handle* h, kbo_mvtpe* t, int32_t* out, int32_t n);
+int kbo_mvtpe_last_timings(kbo_handle* h, kbo_mvtpe* t, float* ms, int32_t n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,8 +19,8 @@
 
 #include "kbo_internal.cuh"
 #include "kbo_rng.cuh"
+#include "kbo_tpe_common.cuh"
 
-#define TPE_LF 25          // hyperopt's DEFAULT_LF: linear forgetting, and the cap on n_below
 #define TPE_CB 32          // slots of a below mixture (<= 25 observations + the prior)
 #define TPE_CHUNK 1024     // components staged in shared memory at a time by the score kernel
 #define TPE_CPT 4          // candidates per thread in the score kernel (each staged component is read once for all four)
@@ -43,10 +43,6 @@ struct TpeHdr {  // one per (numeric parameter, group)
   int ncomp, pad;
   double p_acc;
   float A, B, C2max, C2abs;  // error-bound constants of the FP32 arithmetic: max r', max r'|mu'|, max c2, max |c2|
-};
-struct TpeBest {
-  double s;
-  long long i;  // -1: none
 };
 struct TpeModels {
   const TpeParam* prm;
@@ -76,85 +72,11 @@ struct kbo_tpe {
 };
 
 // ------------------------------------------------------------------------------------------------ device helpers
-__device__ __forceinline__ uint64_t tpe_ordered(double v) {  // doubles as unsigned keys in NumPy's order: -0 == +0, NaN last
-  if (v != v) return ~0ull;
-  if (v == 0.0) v = 0.0;
-  const uint64_t b = (uint64_t)__double_as_longlong(v);
-  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
-}
-__device__ __forceinline__ double tpe_unordered(uint64_t k) {
-  return __longlong_as_double((long long)((k >> 63) ? (k & 0x7FFFFFFFFFFFFFFFull) : ~k));
-}
-__device__ __forceinline__ unsigned tpe_fkey(float f) {  // floats as unsigned keys (0 is below every float)
-  const unsigned b = __float_as_uint(f);
-  return (b >> 31) ? ~b : (b | 0x80000000u);
-}
-__device__ __forceinline__ float tpe_funkey(unsigned k) { return __uint_as_float((k >> 31) ? (k & 0x7FFFFFFFu) : ~k); }
-__device__ __forceinline__ float tpe_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
 // hyperopt's normal_cdf: 0.5 * (1 + erf((x - mu) / max(sqrt(2) * sigma, 1e-12)))
 __device__ __forceinline__ double tpe_ncdf(double x, double mu, double sigma) {
   return 0.5 * (1.0 + erf((x - mu) / fmax(1.4142135623730951 * sigma, 1e-12)));
 }
-// hyperopt's linear_forgetting_weights(N, 25)[j]: ones for N <= 25, else linspace(1/N, 1, N - 25) then 25 ones
-__device__ __forceinline__ double tpe_lfw(int j, int N) {
-  if (N <= TPE_LF) return 1.0;
-  const int nr = N - TPE_LF;
-  if (j >= nr) return 1.0;
-  const double start = 1.0 / N;
-  if (nr == 1) return start;
-  if (j == nr - 1) return 1.0;
-  return (double)j * ((1.0 - start) / (double)(nr - 1)) + start;
-}
 __device__ __forceinline__ size_t tpe_moff(int slot, int g, int ms) { return (size_t)slot * ms + (g ? TPE_CB : 0); }
-// first index of the maximum, NaN above everything (np.argmax)
-__device__ __forceinline__ bool tpe_better(double s, long long i, const TpeBest& b) {
-  if (i < 0) return false;
-  if (b.i < 0) return true;
-  const bool an = s != s, bn = b.s != b.s;
-  if (an != bn) return an;
-  if (!an && s != b.s) return s > b.s;
-  return i < b.i;
-}
-__device__ __forceinline__ TpeBest tpe_block_best(TpeBest b) {
-  __shared__ double ss[32];
-  __shared__ long long si[32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double s = __shfl_xor_sync(0xffffffffu, b.s, o);
-    const long long i = __shfl_xor_sync(0xffffffffu, b.i, o);
-    if (tpe_better(s, i, b)) { b.s = s; b.i = i; }
-  }
-  if (lane == 0) { ss[warp] = b.s; si[warp] = b.i; }
-  __syncthreads();
-  if (threadIdx.x == 0)
-    for (int k = 1; k < (int)(blockDim.x >> 5); k++)
-      if (tpe_better(ss[k], si[k], b)) { b.s = ss[k]; b.i = si[k]; }
-  __syncthreads();
-  return b;  // valid in thread 0
-}
-template <bool MAX>
-__device__ __forceinline__ double tpe_block_reduce(double v) {
-  __shared__ double red[32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const double u = __shfl_xor_sync(0xffffffffu, v, o);
-    v = MAX ? fmax(v, u) : v + u;
-  }
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  if (threadIdx.x == 0)
-    for (int k = 1; k < (int)(blockDim.x >> 5); k++) v = MAX ? fmax(v, red[k]) : v + red[k];
-  if (threadIdx.x == 0) red[0] = v;
-  __syncthreads();
-  return red[0];
-}
 
 // one draw from the below model: choices from p_below; numeric parameters from the mixture truncated to [lo, hi) —
 // component k with probability ∝ w_k·mass_k (what hyperopt's rejection loop amounts to), then that component's truncated
@@ -162,8 +84,7 @@ __device__ __forceinline__ double tpe_block_reduce(double v) {
 __device__ double tpe_draw(const TpeModels& md, const TpeParam& P, uint64_t seed, uint32_t ask, int point, int d, int m) {
   uint32_t r[4];
   philox4x32_10((uint32_t)m, (uint32_t)d, (uint32_t)point, ask, (uint32_t)seed, (uint32_t)(seed >> 32), r);
-  const double u1 = (double)((((uint64_t)r[0]) << 21) ^ (uint64_t)(r[1] >> 11)) * (1.0 / 9007199254740992.0);          // [0,1)
-  const double u2 = ((double)((((uint64_t)r[2]) << 21) ^ (uint64_t)(r[3] >> 11)) + 0.5) * (1.0 / 9007199254740992.0);  // (0,1)
+  const double u1 = tpe_u01(r[0], r[1]), u2 = tpe_u01_open(r[2], r[3]);
   if (P.kind == KBO_TPE_CHOICE) {
     const double* cum = md.cat_cum + (size_t)P.slot * md.lcat;
     int c = 0;
@@ -174,20 +95,7 @@ __device__ double tpe_draw(const TpeModels& md, const TpeParam& P, uint64_t seed
   const int nc = md.hdr[2 * P.slot].ncomp;
   int k = 0;
   while (k < nc - 1 && !(u1 < md.cdf[o + k])) k++;
-  const double mu = md.mu[o + k], sg = md.sg[o + k];
-  const double a = (P.lo - mu) / sg, b = (P.hi - mu) / sg;
-  double z;
-  if (a + b > 0.0) {
-    const double pl = normcdf(-b), pu = normcdf(-a);
-    z = -normcdfinv(pl + u2 * (pu - pl));
-  } else {
-    const double pl = normcdf(a), pu = normcdf(b);
-    z = normcdfinv(pl + u2 * (pu - pl));
-  }
-  double x = fma(sg, z, mu);
-  if (!(x >= P.lo)) x = P.lo;
-  if (x >= P.hi) x = nextafter(P.hi, P.lo);
-  return x;
+  return tpe_truncnorm_draw(P.lo, P.hi, md.mu[o + k], md.sg[o + k], u2);
 }
 // every candidate of every (point, parameter), before quantization
 __global__ void tpe_draw_kernel(TpeModels md, int D, int M, uint64_t seed, uint32_t ask, double* __restrict__ X) {
@@ -263,38 +171,6 @@ __device__ __forceinline__ float tpe_lse_err(float m, float S, float L, const Tp
 }
 
 // ------------------------------------------------------------------------------------------------ model build
-__global__ void tpe_loss_keys_kernel(const double* __restrict__ loss, int n, uint64_t* __restrict__ key, int* __restrict__ idx) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) {
-    key[i] = tpe_ordered(loss[i]);
-    idx[i] = i;
-  }
-}
-// below trials in told order (the first n_below of the stable loss order, sorted by index)
-__global__ void tpe_split_kernel(const int* __restrict__ order, int nb, int* __restrict__ below) {
-  if (threadIdx.x != 0) return;
-  int b[TPE_LF];
-  for (int j = 0; j < nb; j++) {
-    int v = order[j], k = j;
-    while (k > 0 && b[k - 1] > v) { b[k] = b[k - 1]; k--; }
-    b[k] = v;
-  }
-  for (int j = 0; j < nb; j++) below[j] = b[j];
-}
-// group (0 below, 1 above) and position within the group in told order
-__global__ void tpe_group_kernel(const int* __restrict__ below, int nb, int n, int* __restrict__ grp, int* __restrict__ pos) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  int c = 0;
-  bool isb = false;
-  for (int j = 0; j < nb; j++) {
-    const int b = below[j];
-    c += b < i;
-    isb |= b == i;
-  }
-  grp[i] = isb ? 0 : 1;
-  pos[i] = isb ? c : i - c;
-}
 // segment (numeric parameter j, group g) holds that group's values of parameter j at [j·n + (g ? nb : 0), ...)
 __global__ void tpe_seg_fill_kernel(const double* __restrict__ vals, int n, int nb, int D, const int* __restrict__ num, const int* __restrict__ grp,
                                     const int* __restrict__ pos, uint64_t* __restrict__ key, int* __restrict__ val) {

@@ -1,0 +1,123 @@
+"""Multivariate TPE on the GPU (libkbo ``kbo_mvtpe_*``) — the engine behind Katib's ``multivariate-tpe`` algorithm (Optuna's
+``TPESampler(multivariate=True)`` on a flat space; FP64 restatement in oracle/mvtpe_oracle.py): ``tell()`` trials, ``ask()``
+points."""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+
+from . import _lib as L
+
+FLOAT, INT, CAT = 0, 1, 2
+
+
+class MvTpe:
+    """params: list of ``("float", lo, hi)``, ``("int", lo, hi, step)`` or ``("cat", n_categories)``.  Values are in parameter
+    units: integers are grid points lo + j·step <= hi, categoricals are observed and suggested as category indices."""
+
+    def __init__(self, params, seed: int = 0, device: int = 0):
+        if not torch.cuda.is_available():
+            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
+        self.params = [tuple(p) for p in params]
+        self.D = len(self.params)
+        kinds = np.zeros(self.D, np.int32)
+        lo, hi, q = np.zeros(self.D), np.ones(self.D), np.ones(self.D)
+        levels = np.zeros(self.D, np.int32)
+        for d, p in enumerate(self.params):
+            if p[0] == "float":
+                kinds[d], lo[d], hi[d] = FLOAT, p[1], p[2]
+            elif p[0] == "int":
+                kinds[d], lo[d], hi[d], q[d] = INT, p[1], p[2], p[3]
+            elif p[0] == "cat":
+                kinds[d], levels[d] = CAT, p[1]
+            else:
+                raise ValueError(f"unknown parameter kind {p[0]!r}")
+        self.kinds = kinds
+        self.device = int(device)
+        self.lib = L.load()
+        self._h, self._t = C.c_void_p(), C.c_void_p()
+        rc = self.lib.kbo_create(C.byref(self._h), self.device)
+        if rc != L.KBO_OK:
+            raise L.KboError(rc, "kbo_create failed")
+        L.check(self.lib, self._h, self.lib.kbo_mvtpe_create(self._h, C.byref(self._t), self.D, kinds.ctypes.data, lo.ctypes.data, hi.ctypes.data,
+                                                             q.ctypes.data, levels.ctypes.data, int(seed)))
+        self.n = 0
+
+    def close(self):
+        if getattr(self, "_t", None):
+            self.lib.kbo_mvtpe_destroy(self._t)
+            self._t = C.c_void_p()
+        if getattr(self, "_h", None):
+            self.lib.kbo_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def tell(self, X, losses):
+        """Append trials in told order: X (n × D, parameter units) and their losses (minimised; NaN is refused)."""
+        X = np.ascontiguousarray(np.asarray(X, dtype=np.float64).reshape(-1, self.D))
+        y = np.ascontiguousarray(np.asarray(losses, dtype=np.float64).reshape(-1))
+        if X.shape[0] != y.shape[0]:
+            raise ValueError("X and losses must have the same number of rows")
+        if X.shape[0]:
+            L.check(self.lib, self._h, self.lib.kbo_mvtpe_tell(self._h, self._t, X.ctypes.data, y.ctypes.data, X.shape[0], 1, self._stream()))
+            self.n += X.shape[0]
+
+    def ask(self, k: int = 1, n_candidates: int = 24, candidates: torch.Tensor | None = None, return_details: bool = False):
+        """k suggestions (k × D float64 NumPy array).  ``candidates``: optional k × D × n_candidates float64 CUDA tensor.
+        ``return_details``: also the winning indices, the candidates as scored (CUDA tensor, integers on their grid) and the
+        FP32 scores with their bounds (k × n_candidates × 2 CUDA tensor)."""
+        k, M = int(k), int(n_candidates)
+        dev = f"cuda:{self.device}"
+        cp = None
+        if candidates is not None:
+            if not (candidates.is_cuda and candidates.dtype == torch.float64 and tuple(candidates.shape) == (k, self.D, M)):
+                raise ValueError("candidates must be a float64 CUDA tensor of shape (k, D, n_candidates)")
+            candidates = candidates.contiguous()
+            cp = candidates.data_ptr()
+        x = torch.empty(k, self.D, dtype=torch.float64, device=dev)
+        idx = torch.empty(k, dtype=torch.int64, device=dev) if return_details else None
+        cout = torch.empty(k, self.D, M, dtype=torch.float64, device=dev) if return_details else None
+        sc = torch.empty(k, M, 2, dtype=torch.float32, device=dev) if return_details else None
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        L.check(self.lib, self._h, self.lib.kbo_mvtpe_ask(self._h, self._t, k, M, cp, x.data_ptr(), ptr(idx), ptr(cout), ptr(sc), self._stream()))
+        out = x.cpu().numpy()
+        if not return_details:
+            return out
+        return dict(x=out, index=idx.cpu().numpy(), candidates=cout, scores=sc, survivors=self.last_survivors())
+
+    def state(self) -> dict:
+        """{"below": ..., "above": ..., "n_below"}; each group is dict(w, sigma, mu, cat_rows): the weights of its observations
+        in told order followed by the prior's, sigma per parameter (NaN for categoricals), the observations' values (m × D) and,
+        per categorical, an observation row's entry at its own category and elsewhere (NaN for other kinds)."""
+        out = {}
+        for g, name in ((0, "below"), (1, "above")):
+            m, nb = C.c_int32(), C.c_int32()
+            L.check(self.lib, self._h, self.lib.kbo_mvtpe_state(self._h, self._t, g, None, None, None, None, 0, C.byref(m), C.byref(nb), self._stream()))
+            w, sg, mu, cr = np.empty(m.value + 1), np.empty(self.D), np.empty((m.value, self.D)), np.empty((self.D, 2))
+            L.check(self.lib, self._h, self.lib.kbo_mvtpe_state(self._h, self._t, g, w.ctypes.data, sg.ctypes.data, mu.ctypes.data, cr.ctypes.data,
+                                                                m.value + 1, None, None, self._stream()))
+            out[name] = dict(w=w, sigma=sg, mu=mu, cat_rows=cr)
+            out["n_below"] = nb.value
+        return out
+
+    def last_survivors(self) -> np.ndarray:
+        n = self.lib.kbo_mvtpe_last_survivors(self._h, self._t, None, 0)
+        out = np.zeros(max(n, 0), np.int32)
+        if n > 0:
+            self.lib.kbo_mvtpe_last_survivors(self._h, self._t, out.ctypes.data, n)
+        return out
+
+    def last_timings(self) -> dict:
+        ms = np.zeros(4, np.float32)
+        self.lib.kbo_mvtpe_last_timings(self._h, self._t, ms.ctypes.data, 4)
+        return dict(zip(("models_and_draws_ms", "score_fp32_ms", "decide_fp64_ms", "final_ms"), ms.tolist()))

@@ -114,6 +114,39 @@ class _Experiment:
                 row.append(float(hit[0]))
         return row
 
+    def ingest(self, trials, goal, skip_nan: bool = False):
+        """Take the request's new usable trials (each name once) into the history, in the order first seen; loss = objective,
+        negated for MAXIMIZE.  ``skip_nan``: a NaN objective is marked as seen but never told.  Nothing is taken unless every new
+        trial converts: a bad one fails the request."""
+        rows, losses, names = [], [], set()
+        for t in Trial.convert(trials, skip_names=self.told):
+            if t.name in names:
+                continue
+            names.add(t.name)
+            loss = float(t.target_metric.value)
+            if skip_nan and np.isnan(loss):
+                continue
+            rows.append(self.row(t))
+            losses.append(-loss if goal == MAX_GOAL else loss)
+        self.rows += rows
+        self.losses += losses
+        self.told.update(names)
+
+    def points(self, k: int, n_startup: int, n_candidates: int, make_engine) -> list:
+        """k assignment lists: start-up points from the prior (no engine) while fewer than ``n_startup`` trials are told, else
+        the engine's (made by ``make_engine()`` on first use), told every trial it has not seen."""
+        if k == 0:
+            return []
+        if len(self.rows) < n_startup:
+            from .base_service import BaseSkoptService
+            return [BaseSkoptService.convert(self.ss, p) for p in prior_points(self.ss, self.rng, k)]
+        if self.engine is None:
+            self.engine = make_engine()
+        if self.n_engine < len(self.rows):
+            self.engine.tell(np.asarray(self.rows[self.n_engine:]), np.asarray(self.losses[self.n_engine:]))
+            self.n_engine = len(self.rows)
+        return [self.assignments(x) for x in self.engine.ask(k, n_candidates)]
+
     def assignments(self, x) -> list:
         out = []
         for p, v in zip(self.ss.params, x):
@@ -161,28 +194,10 @@ class TpeService(_Base):
         with self._lock:
             st = cached_experiment(self._exps, exp.name, experiment_fingerprint(exp, ss, settings), lambda: _Experiment(ss, settings),
                                    lambda old: old.close(), self.max_experiments)
-            rows, losses, names = [], [], []
-            for t in Trial.convert(request.trials, skip_names=st.told):
-                if t.name in names:
-                    continue
-                loss = float(t.target_metric.value)
-                rows.append(st.row(t))
-                losses.append(-loss if ss.goal == MAX_GOAL else loss)
-                names.append(t.name)
-            st.rows += rows
-            st.losses += losses
-            st.told.update(names)        # only once every new trial converted: a bad one fails the request and is told later
-            if k == 0:
-                return _reply_from([])
-            if len(st.rows) < settings["n_startup_jobs"]:
-                from .base_service import BaseSkoptService
-                return _reply_from([BaseSkoptService.convert(ss, p) for p in prior_points(ss, st.rng, k)])
-            if st.engine is None:
+            st.ingest(request.trials, ss.goal)
+
+            def make_engine():
                 from ..tpe import Tpe
-                st.engine = Tpe(st.space, gamma=settings["gamma"], prior_weight=settings["prior_weight"], seed=st.seed,
-                                device=int(settings.get("device", 0)))
-            if st.n_engine < len(st.rows):
-                st.engine.tell(np.asarray(st.rows[st.n_engine:]), np.asarray(st.losses[st.n_engine:]))
-                st.n_engine = len(st.rows)
-            X = st.engine.ask(k, settings["n_EI_candidates"])
-        return _reply_from([st.assignments(x) for x in X])
+                return Tpe(st.space, gamma=settings["gamma"], prior_weight=settings["prior_weight"], seed=st.seed,
+                           device=int(settings.get("device", 0)))
+            return _reply_from(st.points(k, settings["n_startup_jobs"], settings["n_EI_candidates"], make_engine))

@@ -53,3 +53,14 @@ tp = Tpe([("uniform", -1.0, 3.0), ("quniform", 3.0, 48.0, 5.0), ("choice", 5), (
 tp.tell(np.c_[_r.uniform(-1, 3, 300), 5.0 * _r.integers(1, 10, 300), _r.integers(0, 5, 300), _r.integers(0, 10 ** 6, 300)], _r.random(300))
 print(tp.ask(2, 3000).tolist(), tp.last_survivors().tolist(), tp.state()[0]["below"]["w"].shape)
 tp.close()
+from kubeflow_b200.mvtpe import MvTpe                 # multivariate TPE: model build, tables, draws, prep, FP32 score + FP64 decision
+mv = MvTpe([("float", -1.0, 3.0), ("int", 3, 48, 5), ("cat", 5), ("int", 0, 10 ** 6, 1), ("float", 0.0, 1.0)], seed=9)
+mv.tell(np.c_[_r.uniform(-1, 3, 300), 3.0 + 5.0 * _r.integers(0, 10, 300), _r.integers(0, 5, 300), _r.integers(0, 10 ** 6, 300), _r.random(300)],
+        _r.random(300))
+print(mv.ask(2, 300).tolist(), mv.last_survivors().tolist(), mv.state()["below"]["w"].shape)
+mv.close()
+_wide = [("float", 0.0, 1.0)] * 40 + [("int", 0, 19, 1), ("cat", 3)] * 10     # two float slabs, two discrete slabs in the score kernel
+mv = MvTpe(_wide, seed=3)
+mv.tell(np.c_[_r.random((300, 40)), np.column_stack([_r.integers(0, 20 if i % 2 == 0 else 3, 300) for i in range(20)])], _r.random(300))
+print(mv.ask(2, 300).shape, mv.last_survivors().tolist())
+mv.close()
