@@ -387,6 +387,45 @@ int kbo_mvtpe_state(kbo_handle* h, kbo_mvtpe* t, int32_t group, double* w, doubl
 int kbo_mvtpe_last_survivors(kbo_handle* h, kbo_mvtpe* t, int32_t* out, int32_t n);
 int kbo_mvtpe_last_timings(kbo_handle* h, kbo_mvtpe* t, float* ms, int32_t n);
 
+/* ---- tree forests (Katib algorithm `bayesianoptimization` with base_estimator RF / ET: skopt's RandomForestRegressor /
+ * ExtraTreesRegressor surrogates; FP64 restatement oracle/forest_oracle.py) --------------------------------------------------
+ * Trees follow scikit-learn 1.9.0's DecisionTreeRegressor(min_samples_leaf) with the squared-error criterion and every feature
+ * considered at every node: X is float32, y and every statistic FP64; node ids are breadth-first (children of node k are the next
+ * two ids, left first); ties between splits go to the lowest feature, then the lowest threshold.
+ *   kbo_forest_create: kind RF (bootstrap; best split over the sorted values) or ET (no bootstrap; one uniform threshold per feature
+ *                   per node), n_trees (1..1024), min_samples_leaf (>= 1), seed.  Random draws are Philox4x32-10 keyed by seed:
+ *                   RF bootstrap draw d of tree t is sample (u32·N) >> 32, u32 = word 0 of counter (d, t, 0, 0); the ET threshold
+ *                   of (tree t, node k, feature f) is (max - min)·u + min (min where it equals max), u = the 53-bit uniform of
+ *                   words 0 and 1 of counter (k, t, f, 1), NumPy's (a >> 5, b >> 6) construction.
+ *   kbo_forest_fit  : X (N×D fp32), y (N fp64), device pointers.  counts (RF only, may be NULL): T×N int32 device bootstrap counts
+ *                   that replace the drawn ones.  NaN or infinite X or y: KBO_ERR_INVALID.  Synchronises.
+ *                   1 <= N <= 65536, 1 <= D <= 1024.
+ *   kbo_forest_sweep: skopt's forest predict with return_std (mean over trees of the leaf values; sigma² = mean over trees of
+ *                   max(impurity, 0) + value², minus mean², negatives to 0), then n_acq (0-3, distinct kbo_acq_kind, HOST acqs)
+ *                   acquisitions on the raw mean and sigma (EI / PI with y_opt and xi, LCB with kappa; EI = PI = 0 where sigma = 0)
+ *                   over M fp32 candidates Xc (M×D, device).  best_dev: n_acq device kbo_best, the first-index argmax of each, with
+ *                   global_offset added to the index.  mu_out / sigma_out: optional device fp64 arrays of M.  Asynchronous.
+ *   kbo_forest_predict: mean and sigma as above at n points (device, or host with x_on_host = 1) into HOST arrays.  Synchronises.
+ *   kbo_forest_export: one tree's arrays into HOST buffers (any may be NULL), sklearn's tree_ conventions: feature (-2 at leaves),
+ *                   threshold (-2 at leaves), left / right (-1 at leaves), value, impurity, n_node_samples (distinct samples),
+ *                   weighted_n (bootstrap weight).  et_draws (ET only): n_nodes×D, the threshold drawn for each feature of each
+ *                   internal node, NaN where the feature is constant in the node and on leaves.  counts (may be NULL): N int32, the
+ *                   tree's bootstrap counts (all 1 for ET).  n_nodes receives the tree's node count; with cap < n_nodes only n_nodes
+ *                   and counts are written.  Synchronises.
+ *   kbo_forest_last_timings: milliseconds of the last fit and the last sweep, CUDA events on their streams.  Returns 2. */
+typedef enum kbo_forest_kind { KBO_FOREST_RF = 0, KBO_FOREST_ET = 1 } kbo_forest_kind;
+typedef struct kbo_forest kbo_forest;
+int kbo_forest_create(kbo_handle* h, kbo_forest** out, int32_t kind, int32_t n_trees, int32_t min_samples_leaf, uint64_t seed);
+void kbo_forest_destroy(kbo_forest* f);
+int kbo_forest_fit(kbo_handle* h, kbo_forest* f, const float* X, const double* y, int32_t N, int32_t D, const int32_t* counts, void* stream);
+int kbo_forest_sweep(kbo_handle* h, kbo_forest* f, const float* Xc, int64_t M, int64_t global_offset, int32_t n_acq, const int32_t* acqs, double y_opt,
+                     double xi, double kappa, kbo_best* best_dev, double* mu_out, double* sigma_out, void* stream);
+int kbo_forest_predict(kbo_handle* h, kbo_forest* f, const float* X, int32_t n, int x_on_host, double* mu_host, double* sigma_host, void* stream);
+int kbo_forest_export(kbo_handle* h, kbo_forest* f, int32_t tree, int32_t* feature, double* threshold, int32_t* left, int32_t* right, double* value,
+                      double* impurity, int32_t* n_node_samples, double* weighted_n, double* et_draws, int32_t cap, int32_t* n_nodes, int32_t* counts,
+                      void* stream);
+int kbo_forest_last_timings(kbo_handle* h, kbo_forest* f, float* ms, int32_t n);
+
 #ifdef __cplusplus
 }
 #endif

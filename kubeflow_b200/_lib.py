@@ -57,7 +57,9 @@ EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_se
            "kbo_cma_create", "kbo_cma_destroy", "kbo_cma_ask", "kbo_cma_tell", "kbo_cma_state", "kbo_cma_run_synthetic",
            "kbo_tpe_create", "kbo_tpe_destroy", "kbo_tpe_tell", "kbo_tpe_ask", "kbo_tpe_state", "kbo_tpe_last_survivors", "kbo_tpe_last_timings",
            "kbo_mvtpe_create", "kbo_mvtpe_destroy", "kbo_mvtpe_tell", "kbo_mvtpe_ask", "kbo_mvtpe_state", "kbo_mvtpe_last_survivors",
-           "kbo_mvtpe_last_timings"]
+           "kbo_mvtpe_last_timings",
+           "kbo_forest_create", "kbo_forest_destroy", "kbo_forest_fit", "kbo_forest_sweep", "kbo_forest_predict", "kbo_forest_export",
+           "kbo_forest_last_timings"]
 
 _lib = None
 
@@ -162,6 +164,14 @@ def load() -> C.CDLL:
     lib.kbo_mvtpe_state.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp, vp, vp]
     lib.kbo_mvtpe_last_survivors.argtypes = [vp, vp, vp, i32]
     lib.kbo_mvtpe_last_timings.argtypes = [vp, vp, vp, i32]
+    lib.kbo_forest_create.argtypes = [vp, C.POINTER(vp), i32, i32, i32, C.c_uint64]
+    lib.kbo_forest_destroy.argtypes = [vp]
+    lib.kbo_forest_destroy.restype = None
+    lib.kbo_forest_fit.argtypes = [vp, vp, vp, vp, i32, i32, vp, vp]
+    lib.kbo_forest_sweep.argtypes = [vp, vp, vp, i64, i64, i32, vp, dbl, dbl, dbl, vp, vp, vp, vp]
+    lib.kbo_forest_predict.argtypes = [vp, vp, vp, i32, C.c_int, vp, vp, vp]
+    lib.kbo_forest_export.argtypes = [vp, vp, i32] + [vp] * 9 + [i32, vp, vp, vp]
+    lib.kbo_forest_last_timings.argtypes = [vp, vp, vp, i32]
     lib.kbo_tc_variance_raw.argtypes = [vp, vp, vp, i64, vp, vp, i32, vp, dbl, vp, vp, i32, vp]
     for name in EXPORTS + ["kbo_tc_variance_raw", "kbo_debug_rank_pass", "kbo_debug_kstar", "kbo_debug_rank_rows", "kbo_debug_record_stages",
                            "kbo_debug_stage_count", "kbo_debug_stage", "kbo_debug_fp64_peak", "kbo_debug_dgemm_sm90"]:

@@ -10,6 +10,7 @@
 #include "kbo_internal.cuh"
 #include "dgemm.cuh"
 #include "ktab.cuh"
+#include "kbo_acq.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // K* kernel.  A CTA owns 128 candidates and walks all 64-trial tiles (so μ = K*·alpha needs no atomics).
@@ -215,24 +216,6 @@ struct BlockBest {
   double v;
   long long i;
 };
-__device__ __forceinline__ bool better(double v, long long i, double bv, long long bi) { return v > bv || (v == bv && i < bi); }
-
-template <typename T>
-__device__ __forceinline__ T acq_value(T mun, T varn, int acq, T ymean, T ystd, T yopt, T xi, T kappa, T* mu_o, T* sd_o) {
-  const T var = varn > (T)0 ? varn : (T)0;  // $SK/_gpr.py:485-491
-  const T mu = ystd * mun + ymean;          // :450
-  const T sd = sqrt(var * ystd * ystd);     // :494,:500
-  *mu_o = mu;
-  *sd_o = sd;
-  if (acq == KBO_ACQ_LCB) return -(mu - kappa * sd);
-  if (!(sd > (T)0)) return sd == sd ? (T)0 : sd;   // σ = 0: no improvement possible; a NaN σ (NaN y statistics) stays NaN
-  const T imp = yopt - xi - mu;
-  const T z = imp / sd;
-  const T cdf = (T)0.5 * erfc(-z * (T)0.70710678118654752440);
-  if (acq == KBO_ACQ_PI) return cdf;
-  const T pdf = exp((T)-0.5 * z * z) * (T)0.39894228040143267794;
-  return imp * cdf + sd * pdf;
-}
 
 // One pass: 8 B/candidate in (μ_n, σ²_n as fp32), optional 4 B out.  Persistent-style grid (≤ 2 CTAs per SM, 256 threads),
 // each thread streams groups of 4 candidates with TWO groups (4×16 B loads) in flight before any math, so a 12 MB pass is

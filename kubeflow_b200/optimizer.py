@@ -14,6 +14,9 @@ requested assignment).  Differences, stated once:
   millions are cheap) — ``lbfgs`` polishing is accepted by ValidateAlgorithmSettings and mapped to sampling; ``EIps`` /
   ``PIps`` (they need a second model of the trial durations) are mapped to EI / PI.
 * ``ask(n_points=k)`` uses skopt's constant-liar "cl_min" strategy: k sequential asks with the lie y = min(y).
+* ``base_estimator`` "RF" / "ET" use skopt's forests (``kubeflow_b200.forest.ForestEngine``: fit and sweep on the GPU, raw y, no
+  θ), refit whenever the history changes — every lie included — and swept over the same candidates, shards, gp_hedge and
+  constant liar as the GP.  Their seed is fixed when the engine is made.  GBRT is not served.
 
 ``acq_func="gp_hedge"`` (Katib's and skopt's default) is skopt's portfolio: every model-based ask sweeps ONE candidate set
 for EI, LCB and PI together (``GPEngine.ask_multi``: one posterior, three first-index argmaxes), keeps the three picks, and
@@ -41,6 +44,7 @@ from .space import Space
 
 
 HEDGE_ACQS = ("ei", "lcb", "pi")   # skopt's cand_acq_funcs_ = ["EI", "LCB", "PI"]
+FOREST_ESTIMATORS = ("RF", "ET")   # skopt's cook_estimator forests, kubeflow_b200.forest.ForestEngine
 
 
 class Optimizer:
@@ -48,8 +52,13 @@ class Optimizer:
                  random_state=None, *, n_points=65536, kernel="matern52", length_scale=None, amplitude=1.0, noise=1e-3, xi=0.01,
                  kappa=1.96, var_mode="auto", theta_grid=1, theta_search=0, theta_fit=None, theta_fit_maxiter=25, ard=False, device=0, engine=None,
                  candidate_backend="torch", incremental=True, shard=False):
-        if str(base_estimator).upper() != "GP":
-            raise ValueError("base_estimator must be GP (RF/ET/GBRT are not part of the GPU path)")
+        self.base_estimator = str(base_estimator).upper()
+        if self.base_estimator not in ("GP",) + FOREST_ESTIMATORS:
+            raise ValueError("base_estimator must be GP, RF or ET (GBRT is not part of the GPU path)")
+        self.forest = self.base_estimator in FOREST_ESTIMATORS
+        if self.forest and acq_optimizer == "lbfgs":
+            name = "RandomForestRegressor" if self.base_estimator == "RF" else "ExtraTreesRegressor"
+            raise ValueError(f"The regressor {name} should run with acq_optimizer='sampling'.")
         self.space = dimensions if isinstance(dimensions, Space) else Space(dimensions)
         self.n_initial_points = int(n_initial_points)
         acq = str(acq_func)
@@ -193,6 +202,14 @@ class Optimizer:
             prev, base = (self.next_xs if changed else None), self.gains
         return base if prev is None else base - eng.predict_mean(prev)
 
+    def _get_forest(self):
+        """The RF / ET engine, made on first use with a seed fixed for its lifetime: the same history gives the same forest."""
+        from .forest import ForestEngine
+        if self._engine is None:
+            seed = int(self._seed) if self._seed is not None else int(self.rng.integers(0, 2 ** 31))
+            self._engine = ForestEngine(self.device, kind=self.base_estimator, seed=seed, acq=self.acq, xi=self.xi, kappa=self.kappa)
+        return self._engine
+
     def _ask_one(self, X, y):
         if len(y) < max(self.n_initial_points, 1):
             self._last_gp = False
@@ -203,6 +220,11 @@ class Optimizer:
         if len(X) > n_told:          # constant-liar rows appended by ask(n_points=k)
             Xt = np.concatenate([Xt, self.space.transform(X[n_told:])])
         ya = np.asarray(y, dtype=np.float64)
+        if self.forest:              # refit on a changed history (every lie included), as skopt's tell does; raw y, no θ
+            eng = self._get_forest()
+            eng.tell(Xt, ya)
+            self.last_fit = eng.last_fit
+            return self._pick(eng, Xt, ya, len(X) > n_told)
         base = np.atleast_1d(np.asarray(self._default_ls(), dtype=np.float64))
         eng = self._get_engine(base)
         if self.theta_grid > 1 or self.theta_search > 0:   # choose θ by the GPU log-marginal likelihood
@@ -257,7 +279,10 @@ class Optimizer:
             eng.length_scale, eng.noise = np.exp(res.x[:-1]), float(np.exp(res.x[-1]))
             self.last_theta = dict(length_scale=eng.length_scale.copy(), noise=eng.noise, lml=-float(res.fun), nfev=int(res.nfev))
         self._tell_engine(eng, Xt, ya)
-        lie = len(X) > n_told
+        return self._pick(eng, Xt, ya, len(X) > n_told)
+
+    def _pick(self, eng, Xt, ya, lie):
+        """Sample the candidates (this rank's share when sharded), sweep them with the fitted engine, and return the point."""
         rank, world = self._world() if self.shard else (0, 1)
         from .dist import global_argmax, shard_rows
         if world > 1 and self.n_points < world:     # identical on every rank, before any collective: all raise together

@@ -1,9 +1,10 @@
 """``api.v1.beta1.Suggestion`` servicers.
 
 * ``SkoptService``  — algorithm ``bayesianoptimization`` (kubeflow/katib pkg/suggestion/v1beta1/skopt/service.py):
-  GetSuggestions → BaseSkoptService → kubeflow_b200.Optimizer → libkbo (GPU).  ValidateAlgorithmSettings accepts the
-  upstream settings (base_estimator, n_initial_points, acq_func, acq_optimizer, random_state) plus engine knobs as
-  EXTRA settings, so an unchanged Experiment works and an extended one can opt in (SURVEY.md §5 "config").
+  GetSuggestions → BaseSkoptService → kubeflow_b200.Optimizer → libkbo (GPU), with base_estimator GP, RF or ET (GBRT is
+  refused).  ValidateAlgorithmSettings accepts the upstream settings (base_estimator, n_initial_points, acq_func,
+  acq_optimizer, random_state) plus engine knobs as EXTRA settings, so an unchanged Experiment works and an extended one
+  can opt in (SURVEY.md §5 "config"); the GP-only knobs are refused with a tree estimator.
 * ``RandomService`` — algorithm ``random`` (upstream: the hyperopt service's random search): BASELINE.json config 1,
   gRPC plumbing on CPU, no GPU involved.
 Errors: bad settings → INVALID_ARGUMENT; anything else → INTERNAL (SURVEY.md §8(b)).
@@ -25,6 +26,10 @@ SKOPT_SETTINGS = ("base_estimator", "n_initial_points", "acq_func", "acq_optimiz
 ENGINE_SETTINGS = {"n_points": int, "kernel": str, "length_scale": float, "amplitude": float, "noise": float, "xi": float,
                    "kappa": float, "var_mode": str, "theta_grid": int, "theta_search": int, "theta_fit": str, "theta_fit_maxiter": int, "ard": int, "device": int, "candidate_backend": str}
 
+TREE_ESTIMATORS = {"RF": "RandomForestRegressor", "ET": "ExtraTreesRegressor"}   # skopt's cook_estimator names
+GP_ONLY_SETTINGS = ("kernel", "length_scale", "amplitude", "noise", "var_mode", "theta_grid", "theta_search", "theta_fit",
+                    "theta_fit_maxiter", "ard")
+
 
 def validate_skopt_settings(settings: dict) -> dict:
     """Returns the parsed keyword arguments or raises AlgorithmSettingsError (mirrors upstream OptimizerConfiguration)."""
@@ -34,7 +39,7 @@ def validate_skopt_settings(settings: dict) -> dict:
             if name == "base_estimator":
                 if value not in ("GP", "RF", "ET", "GBRT"):
                     raise AlgorithmSettingsError(f"base_estimator {value} is not supported in Bayesian optimization")
-                if value != "GP":
+                if value == "GBRT":
                     raise AlgorithmSettingsError(f"base_estimator {value}: only GP runs on the GPU engine")
                 out[name] = value
             elif name == "n_initial_points":
@@ -78,6 +83,13 @@ def validate_skopt_settings(settings: dict) -> dict:
             raise
         except (TypeError, ValueError):
             raise AlgorithmSettingsError(f"failed to convert {value!r} for setting {name}")
+    if out.get("base_estimator") in TREE_ESTIMATORS:
+        est = out["base_estimator"]
+        if out.get("acq_optimizer") == "lbfgs":      # skopt's Optimizer refuses it: trees have no gradients
+            raise AlgorithmSettingsError(f"The regressor {TREE_ESTIMATORS[est]} should run with acq_optimizer='sampling'.")
+        for name in GP_ONLY_SETTINGS:
+            if name in out:
+                raise AlgorithmSettingsError(f"setting {name} applies to base_estimator GP only, not {est}")
     return out
 
 

@@ -64,3 +64,10 @@ mv = MvTpe(_wide, seed=3)
 mv.tell(np.c_[_r.random((300, 40)), np.column_stack([_r.integers(0, 20 if i % 2 == 0 else 3, 300) for i in range(20)])], _r.random(300))
 print(mv.ask(2, 300).shape, mv.last_survivors().tolist())
 mv.close()
+from kubeflow_b200.forest import ForestEngine       # RF / ET: bootstrap, presort, per-tree fit, packing, staged sweep, export draws
+for _kind in ("RF", "ET"):
+    fe = ForestEngine(kind=_kind, n_trees=8, seed=4)
+    fe.tell(_r.random((300, 5)), _r.random(300))
+    print(fe.ask_multi(_r.random((5000, 5)), ["ei", "lcb", "pi"])[0], fe.predict(_r.random((3, 5)))[0].tolist(),
+          len(fe.export(0, with_draws=_kind == "ET")["left"]))
+    fe.close()
