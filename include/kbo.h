@@ -299,7 +299,22 @@ uint64_t kbo_hash64(const void* bytes, uint64_t len);   /* the FNV-1a hash kbo_r
  *                 Ranking is NumPy's sort order: -inf < finite < +inf < NaN, -0 == +0, every NaN equal (a diverged trial
  *                 that reports nan ranks last, after inf); ties → lower sample index.
  *                 d_j² is the eigenvalue λ_j itself (b_jᵀ C b_j); only λ_j ≤ 0 is replaced, by 1e-8.
- * Limits: 1 <= D <= 128, 4 <= lambda <= 8192.  kbo_cma_state copies to HOST buffers (any may be NULL) and synchronises.
+ *                 Every tell ends with the termination test of CyberAgent `cmaes` (should_stop) on the updated state, on the
+ *                 device: the generation's best and worst fitness go to slot 2·(g mod term) of a history ring of 2·term
+ *                 doubles (term = 10 + ⌈30·D/lambda⌉, g = strategy generation after the tell), and six criteria set bits:
+ *                 TOLFUN=1 (g > term and max−min of the history < 1e-12), TOLX=2 (all σ·C_ii and σ·p_c,i < 1e-12·σ0),
+ *                 TOLXUP=4 (σ·max d > 1e4), NOEFFECTCOORD=8 (some m_i == m_i + 0.2σ·√C_ii), NOEFFECTAXIS=16
+ *                 (m == m + 0.1σ·d_i·b_i, i = g mod D, b_i column i of this library's Jacobi basis), CONDITIONCOV=32
+ *                 (max d / min d > 1e14).  NaN anywhere in a criterion's operands makes it false, as in NumPy.
+ * The built-in Philox stream is keyed by a draw counter that advances once per tell and is never reset (without a
+ * restart it equals the generation), so the draws of a restarted run never repeat earlier ones.
+ * Limits: 1 <= D <= 128, 4 <= lambda <= 8192.  kbo_cma_state copies to HOST buffers (any may be NULL) and synchronises;
+ * its `generation` is the strategy generation of the current run.
+ * kbo_cma_stop_flags copies the flags word (0 before the first tell of a run) and, if funhist_host is given, the 2·term
+ * history, writes term, and synchronises.
+ * kbo_cma_restart starts a new run in place (IPOP / BIPOP restarts): population lambda (buffers grow as needed, weights
+ * and constants are recomputed), mean0_host, sigma0, C = B = I, d = 1, zero paths, history and flags, strategy generation
+ * 0.  Same limits and error codes as kbo_cma_create; after a failed restart the instance may only be destroyed.
  * kbo_cma_run_synthetic runs `generations` ask/fitness/tell rounds entirely on the device with a built-in fitness
  * (0 = sphere, 1 = Rastrigin) — the BASELINE.json config-4 benchmark. */
 typedef struct kbo_cma kbo_cma;
@@ -309,6 +324,8 @@ int kbo_cma_ask(kbo_handle* h, kbo_cma* c, double* X_dev, const double* z_in_dev
 int kbo_cma_tell(kbo_handle* h, kbo_cma* c, const double* fitness_dev, void* stream);
 int kbo_cma_state(kbo_handle* h, kbo_cma* c, double* mean, double* sigma, double* C, double* p_sigma, double* p_c, double* B,
                   double* d, double* Y_last, int64_t* generation, void* stream);
+int kbo_cma_stop_flags(kbo_handle* h, kbo_cma* c, uint32_t* flags_host, double* funhist_host, int32_t* term_host, void* stream);
+int kbo_cma_restart(kbo_handle* h, kbo_cma* c, int32_t lambda, const double* mean0_host, double sigma0);
 int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32_t generations, double* best_f_host,
                           float* elapsed_ms, double* jacobi_sweeps_last);
 

@@ -78,6 +78,28 @@ class CmaEs:
             out["Y"] = Y
         return out
 
+    def stop_flags(self):
+        """(flags, funhist, term) of the termination test run at the end of the last tell: the bit mask (TOLFUN=1, TOLX=2,
+        TOLXUP=4, NOEFFECTCOORD=8, NOEFFECTAXIS=16, CONDITIONCOV=32; 0 before a run's first tell), the history ring of
+        each generation's best and worst fitness (2·term values) and term."""
+        flags, term = C.c_uint32(), C.c_int32()
+        hist = np.zeros(2 * (10 + -(-30 * self.D // 4)))     # room for the largest ring (λ = 4)
+        L.check(self.lib, self._h, self.lib.kbo_cma_stop_flags(self._h, self._c, C.byref(flags), hist.ctypes.data, C.byref(term),
+                                                               self._stream()))
+        return flags.value, hist[:2 * term.value].copy(), term.value
+
+    def restart(self, popsize: int, mean, sigma: float):
+        """Start a new run in place (IPOP / BIPOP): population `popsize`, C = I, zero paths, strategy generation 0.  The
+        built-in sampler's stream continues, so no earlier draw repeats."""
+        mean = np.ascontiguousarray(np.asarray(mean, dtype=np.float64))
+        if mean.shape != (self.D,):
+            raise ValueError(f"mean must have {self.D} entries")
+        L.check(self.lib, self._h, self.lib.kbo_cma_restart(self._h, self._c, int(popsize), mean.ctypes.data_as(C.POINTER(C.c_double)),
+                                                            float(sigma)))
+        if int(popsize) != self.popsize:
+            self.popsize = int(popsize)
+            self._X = torch.empty(self.popsize, self.D, dtype=torch.float64, device=f"cuda:{self.device}")
+
     def run_synthetic(self, fitness: str, generations: int):
         """BASELINE config 4: `generations` full generations on the device with a built-in fitness."""
         kind = {"sphere": 0, "rastrigin": 1}[fitness]

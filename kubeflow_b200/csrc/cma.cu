@@ -17,10 +17,14 @@
 struct kbo_cma {
   int D = 0, lambda = 0, mu = 0, lam_pow2 = 0, lam_pad = 0;  // lam_pad: λ rounded up to the 256-wide split-K slices
   uint64_t seed = 0;
-  long long gen = 0;
+  long long gen = 0;    // strategy generation: back to 0 at every restart (h_σ and the termination test read it)
+  long long draws = 0;  // Philox counter of the built-in sampler: one per tell, never reset, so no restart repeats a draw
   // strategy parameters (host copies)
   double mu_eff, c1, cmu, cm, c_sigma, d_sigma, cc, chi_n, wsum;
-  DevBuf mean, C, B, Dv, ps, pc, weights, Z, Zs, Y, Ys, YwT, zn2, order, R, G, scal, yw;
+  // termination test (`cmaes`' should_stop): constants of the current run, fitness history ring of 2·term doubles
+  int term = 0;
+  double tolx = 0.0;
+  DevBuf mean, C, B, Dv, ps, pc, weights, Z, Zs, Y, Ys, YwT, zn2, order, R, G, scal, yw, hist, flags;
   bool asked = false;
 };
 
@@ -357,6 +361,126 @@ __global__ void cma_init_kernel(double* __restrict__ C, double* __restrict__ B, 
   }
 }
 
+// ------------------------------------------------------------------------------------------------ termination test
+// Criteria 4 and 5 are exact equality tests, so every rounding is the one `cmaes` makes in NumPy: products by __dmul_rn and
+// sums by __dadd_rn (never contracted into a DFMA), and √c and max(d)/min(d) correctly rounded by the integer routines
+// below (the library's FP64 sqrt and division are DFMA Newton sequences; these give the same IEEE results without one).
+#define CMA_TOLXUP 1e4
+#define CMA_TOLFUN 1e-12
+#define CMA_TOLCONDCOV 1e14
+enum CmaStop { STOP_TOLFUN = 1, STOP_TOLX = 2, STOP_TOLXUP = 4, STOP_NOEFFECTCOORD = 8, STOP_NOEFFECTAXIS = 16, STOP_CONDITIONCOV = 32 };
+
+// RN(√x): digit-by-digit root of the 53-bit significand scaled to a 54-bit root, rounded to nearest-even by the remainder
+__device__ double cma_sqrt_rn(double x) {
+  if (x != x || x < 0.0) return __longlong_as_double(0x7ff8000000000000LL);
+  if (x == 0.0 || x > 1.7976931348623157e308) return x;
+  const unsigned long long bits = (unsigned long long)__double_as_longlong(x);
+  int e = (int)(bits >> 52);
+  unsigned long long m = bits & 0xfffffffffffffULL;
+  if (e == 0) {                                   // subnormal: normalise the significand
+    e = 1;
+    while (!(m & (1ULL << 52))) { m <<= 1; e--; }
+  } else {
+    m |= 1ULL << 52;
+  }
+  int E = e - 1075;                               // x = m·2^E
+  if (E & 1) { m <<= 1; E--; }                    // m < 2^54, E even
+  unsigned long long r = 0, rem = 0;              // √(m·2^54) = r + rem-fraction, r < 2^54
+  for (int i = 53; i >= 0; i--) {
+    const unsigned long long pair = i >= 27 ? (m >> (2 * (i - 27))) & 3ULL : 0ULL;
+    rem = (rem << 2) | pair;
+    const unsigned long long trial = (r << 2) | 1ULL;
+    if (rem >= trial) { rem -= trial; r = (r << 1) | 1ULL; } else { r <<= 1; }
+  }
+  unsigned long long q = r >> 1;                  // 53 bits; r's last bit is the guard, rem != 0 the sticky bit
+  if ((r & 1ULL) && (rem != 0 || (q & 1ULL))) q++;
+  const int k = (E - 54) / 2 + 1;                 // √x = q·2^k
+  return __longlong_as_double((long long)((((unsigned long long)(k + 1074)) << 52) + q));
+}
+// RN(a/b) for positive normal a, b with a ≥ b (max(d)/min(d)): long division of the significands to 54 quotient bits
+__device__ double cma_div_rn(double a, double b) {
+  const unsigned long long ba = (unsigned long long)__double_as_longlong(a), bb = (unsigned long long)__double_as_longlong(b);
+  unsigned long long ma = (ba & 0xfffffffffffffULL) | (1ULL << 52), mb = (bb & 0xfffffffffffffULL) | (1ULL << 52);
+  int k = (int)(ba >> 52) - (int)(bb >> 52) - 52;  // a/b = (ma/mb)·2^(k+52)
+  if (ma < mb) { ma <<= 1; k--; }
+  unsigned long long Q = 0, rem = ma;
+  for (int i = 0; i < 54; i++) {
+    Q <<= 1;
+    if (rem >= mb) { rem -= mb; Q |= 1ULL; }
+    rem <<= 1;
+  }
+  unsigned long long q = Q >> 1;                  // a/b ≈ q·2^k, q in [2^52, 2^53)
+  if ((Q & 1ULL) && (rem != 0 || (q & 1ULL))) q++;
+  if (k + 1075 > 2046) return __longlong_as_double(0x7ff0000000000000LL);
+  return __longlong_as_double((long long)((((unsigned long long)(k + 1074)) << 52) + q));   // q = 2^53 carries into the exponent
+}
+
+// One CTA of CMA_MAXD threads, after the tell on the tell's stream: records this generation's best and worst fitness
+// (NumPy order, so the worst is NaN when any sample is) in slot 2·(g mod term) of the ring, then evaluates all six criteria
+// on the updated state (g = strategy generation after the increment, i = g mod D for the axis test).
+__global__ void __launch_bounds__(CMA_MAXD) cma_stop_kernel(const double* __restrict__ f, const int* __restrict__ order, int lambda, int D,
+                                                            const double* __restrict__ mean, const double* __restrict__ C,
+                                                            const double* __restrict__ B, const double* __restrict__ Dv,
+                                                            const double* __restrict__ pc, const double* __restrict__ scal, double* hist,
+                                                            int term, long long g, double tolx, unsigned* __restrict__ flags) {
+  __shared__ double s_hi[CMA_MAXD / 32], s_lo[CMA_MAXD / 32], s_dhi[CMA_MAXD / 32], s_dlo[CMA_MAXD / 32];
+  __shared__ int s_nan[CMA_MAXD / 32], s_dnan[CMA_MAXD / 32];
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int slot = (int)(2 * (g % term));
+  if (t == 0) hist[slot] = f[order[0]];
+  if (t == 1) hist[slot + 1] = f[order[lambda - 1]];
+  __syncthreads();
+  // max / min of the history and of d, with NumPy's NaN propagation kept as a separate flag
+  int hnan = 0, dnan = 0;
+  double hi = -INFINITY, lo = INFINITY, dhi = -INFINITY, dlo = INFINITY;
+  for (int i = t; i < 2 * term; i += CMA_MAXD) {
+    const double v = hist[i];
+    hnan |= v != v;
+    hi = fmax(hi, v);
+    lo = fmin(lo, v);
+  }
+  const double sigma = scal[CS_SIGMA];
+  bool tolx_all = true, coord_any = false, axis_all = true;
+  if (t < D) {
+    const double c = C[(size_t)t * D + t], m = mean[t], d = Dv[t];
+    dnan = d != d;
+    dhi = d;
+    dlo = d;
+    tolx_all = __dmul_rn(sigma, c) < tolx && __dmul_rn(sigma, pc[t]) < tolx;
+    coord_any = m == __dadd_rn(m, __dmul_rn(__dmul_rn(0.2, sigma), cma_sqrt_rn(c)));
+    const int ax = (int)(g % D);
+    axis_all = m == __dadd_rn(m, __dmul_rn(__dmul_rn(__dmul_rn(0.1, sigma), Dv[ax]), B[(size_t)t * D + ax]));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    hnan |= __shfl_xor_sync(0xffffffffu, hnan, o);
+    dnan |= __shfl_xor_sync(0xffffffffu, dnan, o);
+    hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    dhi = fmax(dhi, __shfl_xor_sync(0xffffffffu, dhi, o));
+    dlo = fmin(dlo, __shfl_xor_sync(0xffffffffu, dlo, o));
+  }
+  if (lane == 0) { s_hi[w] = hi; s_lo[w] = lo; s_dhi[w] = dhi; s_dlo[w] = dlo; s_nan[w] = hnan; s_dnan[w] = dnan; }
+  tolx_all = __syncthreads_and(tolx_all);
+  coord_any = __syncthreads_or(coord_any);
+  axis_all = __syncthreads_and(axis_all);
+  if (t == 0) {
+    for (int i = 1; i < CMA_MAXD / 32; i++) {
+      hi = fmax(hi, s_hi[i]); lo = fmin(lo, s_lo[i]); dhi = fmax(dhi, s_dhi[i]); dlo = fmin(dlo, s_dlo[i]);
+      hnan |= s_nan[i]; dnan |= s_dnan[i];
+    }
+    unsigned fl = 0;
+    if (g > term && !hnan && __dadd_rn(hi, -lo) < CMA_TOLFUN) fl |= STOP_TOLFUN;   // inf − inf is NaN: false
+    if (tolx_all) fl |= STOP_TOLX;
+    if (!dnan && __dmul_rn(sigma, dhi) > CMA_TOLXUP) fl |= STOP_TOLXUP;
+    if (coord_any) fl |= STOP_NOEFFECTCOORD;
+    if (axis_all) fl |= STOP_NOEFFECTAXIS;
+    if (!dnan && (dhi > 1.7976931348623157e308 ? dlo <= 1.7976931348623157e308 : cma_div_rn(dhi, dlo) > CMA_TOLCONDCOV))
+      fl |= STOP_CONDITIONCOV;                                                    // inf/finite = inf, inf/inf = NaN
+    *flags = fl;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness, cudaStream_t s) {
   const int D = c->D, lam = c->lambda;
@@ -391,7 +515,12 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
   KBO_LAUNCH_CHECK(h);
   cma_eigval_kernel<<<D, 1024, 0, s>>>((const double*)c->C.p, (const double*)c->B.p, D, (double*)c->Dv.p);
   KBO_LAUNCH_CHECK(h);
+  cma_stop_kernel<<<1, CMA_MAXD, 0, s>>>(fitness, (const int*)c->order.p, lam, D, (const double*)c->mean.p, (const double*)c->C.p,
+                                         (const double*)c->B.p, (const double*)c->Dv.p, (const double*)c->pc.p, (const double*)c->scal.p,
+                                         (double*)c->hist.p, c->term, c->gen + 1, c->tolx, (unsigned*)c->flags.p);
+  KBO_LAUNCH_CHECK(h);
   c->gen++;
+  c->draws++;
   c->asked = false;
   return KBO_OK;
 }
@@ -401,7 +530,7 @@ static int cma_generation_ask(kbo_handle* h, kbo_cma* c, double* X, const double
   const int64_t n = (int64_t)lam * D;
   const double* Z = z_in;
   if (!Z) {
-    cma_normal_kernel<<<(unsigned)((n / 2 + 1 + 255) / 256), 256, 0, s>>>((double*)c->Z.p, n, c->seed, (uint64_t)c->gen);
+    cma_normal_kernel<<<(unsigned)((n / 2 + 1 + 255) / 256), 256, 0, s>>>((double*)c->Z.p, n, c->seed, (uint64_t)c->draws);
     KBO_LAUNCH_CHECK(h);
     Z = (const double*)c->Z.p;
   }
@@ -416,26 +545,16 @@ static int cma_generation_ask(kbo_handle* h, kbo_cma* c, double* X, const double
   return KBO_OK;
 }
 
-extern "C" {
-
-int kbo_cma_create(kbo_handle* h, kbo_cma** out, int32_t D, int32_t lambda, const double* mean0, double sigma0, uint64_t seed) {
-  if (!h || !out) return KBO_ERR_INVALID;
-  *out = nullptr;
-  if (D < 1 || D > CMA_MAXD) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: 1 <= D <= %d supported (got %d)", CMA_MAXD, D);
-  if (lambda < 4 || lambda > 8192) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: 4 <= lambda <= 8192 supported (got %d)", lambda);
-  if (!mean0 || !(sigma0 > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: mean0 must be given and sigma0 > 0");
-  KBO_CUDA(h, cudaSetDevice(h->device));
-  kbo_cma* c = new (std::nothrow) kbo_cma();
-  if (!c) return KBO_ERR_NOMEM;
-  c->D = D;
+// Strategy parameters for population λ (tutorial Table 1; active weights as in `cmaes`), the buffers they size, and the
+// termination constants of a run starting at σ0.  Shared by create and restart; uploads the weights (synchronous copy).
+static int cma_configure(kbo_handle* h, kbo_cma* c, int lambda, double sigma0) {
+  const int D = c->D;
   c->lambda = lambda;
   c->mu = lambda / 2;
-  c->seed = seed;
   int p2 = 1;
   while (p2 < lambda) p2 <<= 1;
   c->lam_pow2 = p2;
   c->lam_pad = round_up(lambda, 256);
-  // strategy parameters (tutorial Table 1; active weights as in `cmaes`)
   std::vector<double> w(lambda);
   const int mu = c->mu, n = D;
   double s1 = 0, s2 = 0, m1 = 0, m2 = 0;
@@ -463,31 +582,83 @@ int kbo_cma_create(kbo_handle* h, kbo_cma** out, int32_t D, int32_t lambda, cons
   c->d_sigma = 1 + 2 * (t > 0 ? t : 0) + c->c_sigma;
   c->cc = (4 + mu_eff / n) / (n + 4 + 2 * mu_eff / n);
   c->chi_n = sqrt((double)n) * (1.0 - 1.0 / (4.0 * n) + 1.0 / (21.0 * n * n));
+  c->term = 10 + (30 * n + lambda - 1) / lambda;   // 10 + ⌈30·n/λ⌉
+  c->tolx = 1e-12 * sigma0;
   const size_t LD = (size_t)lambda * D, LPD = (size_t)c->lam_pad * D;
   int r = KBO_OK;
   auto R_ = [&](DevBuf& b, size_t bytes) { if (r == KBO_OK) r = kbo_reserve(h, b, bytes); };
   R_(c->mean, 8 * D); R_(c->C, 8 * (size_t)D * D); R_(c->B, 8 * (size_t)D * D); R_(c->Dv, 8 * D); R_(c->ps, 8 * D); R_(c->pc, 8 * D);
   R_(c->weights, 8 * lambda); R_(c->Z, 8 * (LD + 2)); R_(c->Zs, 8 * LD); R_(c->Y, 8 * LD); R_(c->Ys, 8 * LPD); R_(c->YwT, 8 * LPD);
   R_(c->zn2, 8 * lambda); R_(c->order, 4 * lambda); R_(c->R, 8 * (size_t)D * D * (c->lam_pad / 256)); R_(c->G, 8 * (size_t)D * D); R_(c->scal, 8 * CS_COUNT);
-  R_(c->yw, 8 * D);
-  if (r != KBO_OK) { delete c; return r; }
+  R_(c->yw, 8 * D); R_(c->hist, 8 * 2 * (size_t)c->term); R_(c->flags, 4);
+  if (r != KBO_OK) return r;
+  KBO_CUDA(h, cudaMemcpy(c->weights.p, w.data(), 8 * lambda, cudaMemcpyHostToDevice));
+  return KBO_OK;
+}
+
+// A run's starting state: mean0, σ0, C = B = I, d = 1, zero paths, history and flags, strategy generation 0.
+static int cma_start_run(kbo_handle* h, kbo_cma* c, const double* mean0, double sigma0) {
+  const int D = c->D;
   double sc[CS_COUNT] = {sigma0, 0, 0, 0, 0, 0, 0, 0};
   cudaMemcpy(c->mean.p, mean0, 8 * D, cudaMemcpyHostToDevice);
-  cudaMemcpy(c->weights.p, w.data(), 8 * lambda, cudaMemcpyHostToDevice);
   cudaMemcpy(c->scal.p, sc, sizeof sc, cudaMemcpyHostToDevice);
   cma_init_kernel<<<D, 128>>>((double*)c->C.p, (double*)c->B.p, (double*)c->Dv.p, (double*)c->ps.p, (double*)c->pc.p, D);
+  cudaMemset(c->hist.p, 0, 8 * 2 * (size_t)c->term);
+  cudaMemset(c->flags.p, 0, 4);
+  KBO_CUDA(h, cudaDeviceSynchronize());
+  c->gen = 0;
+  c->asked = false;
+  return KBO_OK;
+}
+
+extern "C" {
+
+int kbo_cma_create(kbo_handle* h, kbo_cma** out, int32_t D, int32_t lambda, const double* mean0, double sigma0, uint64_t seed) {
+  if (!h || !out) return KBO_ERR_INVALID;
+  *out = nullptr;
+  if (D < 1 || D > CMA_MAXD) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: 1 <= D <= %d supported (got %d)", CMA_MAXD, D);
+  if (lambda < 4 || lambda > 8192) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: 4 <= lambda <= 8192 supported (got %d)", lambda);
+  if (!mean0 || !(sigma0 > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: mean0 must be given and sigma0 > 0");
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  kbo_cma* c = new (std::nothrow) kbo_cma();
+  if (!c) return KBO_ERR_NOMEM;
+  c->D = D;
+  c->seed = seed;
+  int r = cma_configure(h, c, lambda, sigma0);
+  if (r != KBO_OK) { kbo_cma_destroy(c); return r; }
   cudaFuncSetAttribute(cma_jacobi_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * CMA_MAXD * (CMA_MAXD + 1)));
   cudaFuncSetAttribute(cma_jacobi_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * CMA_MAXD * (CMA_MAXD + 1)));
   cudaFuncSetAttribute(cma_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 12);
-  KBO_CUDA(h, cudaDeviceSynchronize());
+  r = cma_start_run(h, c, mean0, sigma0);
+  if (r != KBO_OK) { kbo_cma_destroy(c); return r; }
   *out = c;
+  return KBO_OK;
+}
+
+int kbo_cma_restart(kbo_handle* h, kbo_cma* c, int32_t lambda, const double* mean0, double sigma0) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (lambda < 4 || lambda > 8192) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_restart: 4 <= lambda <= 8192 supported (got %d)", lambda);
+  if (!mean0 || !(sigma0 > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_restart: mean0 must be given and sigma0 > 0");
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  KBO_CUDA(h, cudaDeviceSynchronize());            // the last tell may still be reading buffers that are about to grow
+  KBO_TRY(cma_configure(h, c, lambda, sigma0));
+  return cma_start_run(h, c, mean0, sigma0);
+}
+
+int kbo_cma_stop_flags(kbo_handle* h, kbo_cma* c, uint32_t* flags_host, double* funhist_host, int32_t* term_host, void* stream) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (flags_host) KBO_CUDA(h, cudaMemcpyAsync(flags_host, c->flags.p, 4, cudaMemcpyDeviceToHost, s));
+  if (funhist_host) KBO_CUDA(h, cudaMemcpyAsync(funhist_host, c->hist.p, 8 * 2 * (size_t)c->term, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (term_host) *term_host = c->term;
   return KBO_OK;
 }
 
 void kbo_cma_destroy(kbo_cma* c) {
   if (!c) return;
   DevBuf* bufs[] = {&c->mean, &c->C, &c->B, &c->Dv, &c->ps, &c->pc, &c->weights, &c->Z, &c->Zs, &c->Y, &c->Ys, &c->YwT, &c->zn2, &c->order,
-                    &c->R, &c->G, &c->scal, &c->yw};
+                    &c->R, &c->G, &c->scal, &c->yw, &c->hist, &c->flags};
   for (DevBuf* b : bufs)
     if (b->p) cudaFree(b->p);
   delete c;

@@ -9,7 +9,11 @@ whose trial ended without an objective (FAILED / KILLED / METRICSUNAVAILABLE) go
 handed out again — goptuna likewise keeps sampling the running generation until popsize trials are COMPLETE — so neither
 duplicates nor failures can stall the generation.  If the controller asks for more points than the generation has left,
 the extra points are independent draws from the current distribution (they do not enter the update), which is what
-goptuna's relative/independent sampling split amounts to.
+goptuna's relative/independent sampling split amounts to.  With ``restart_strategy`` ``ipop`` or ``bipop`` the
+termination test the sampler runs on the device after every tell is read after each complete generation; when any of
+its criteria holds, the run restarts in place on the schedule of ``cma_restart.py`` (IPOP: doubled population; BIPOP:
+interlaced large and small runs) with a fresh mean drawn in the cube.  Outstanding samples of the stopped run stay
+unmatched, like extra independent draws.
 """
 from __future__ import annotations
 
@@ -20,6 +24,7 @@ import numpy as np
 from . import api_pb as api
 from .internal import (CATEGORICAL, DISCRETE, DOUBLE, INTEGER, MAX_GOAL, AlgorithmSettingsError, Assignment,
                        HyperParameterSearchSpace, Trial, parse_settings)
+from .cma_restart import STRATEGIES, Schedule
 from .service import _Base, _reply_from
 
 
@@ -45,6 +50,8 @@ def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
                 raise AlgorithmSettingsError(f"unknown setting {k} for algorithm cmaes")
         except ValueError:
             raise AlgorithmSettingsError(f"failed to convert {v!r} for setting {k}")
+    if out.get("restart_strategy", "none") not in STRATEGIES:
+        raise AlgorithmSettingsError(f"restart_strategy must be one of {', '.join(STRATEGIES)}, got {out['restart_strategy']!r}")
     if n_params < 2:
         raise AlgorithmSettingsError("cmaes only supports two or more dimensional continuous search space")   # goptuna's rule
     return out
@@ -61,6 +68,11 @@ class _Experiment:
         self.fitness = {}        # sample index -> value
         self.seen = set()        # trial names already accounted for (finished with or without an objective)
         self.extra_rng = np.random.default_rng(settings.get("random_state", 0) + 7919)
+        strategy = settings.get("restart_strategy", "none")
+        # IPOP / BIPOP: λ0, σ0, the restart draws and the BIPOP budgets live in the schedule; None = one run, no test read
+        self.schedule = None if strategy == "none" else Schedule(strategy, D, settings.get("popsize"), settings.get("sigma", 1.0 / 6.0),
+                                                                   settings.get("random_state", 0))
+        self.run_gens = 0        # generations told in the current run
 
 
 class CmaesService(_Base):
@@ -135,6 +147,11 @@ class CmaesService(_Base):
                     st.queue.insert(0, (i, st.assign[i]))
             if len(st.fitness) == st.es.popsize:
                 st.es.tell(np.array([st.fitness[i] for i in range(st.es.popsize)]))
+                st.run_gens += 1
+                if st.schedule is not None and st.es.stop_flags()[0]:
+                    lam, mean, sigma = st.schedule.next_run(st.es.popsize, st.run_gens)
+                    st.es.restart(lam, mean, sigma)
+                    st.run_gens = 0
                 self._new_generation(st, ss)
             lists = []
             for _ in range(max(int(request.current_request_number), 0)):
