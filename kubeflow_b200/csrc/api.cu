@@ -57,9 +57,6 @@ void kbo_destroy(kbo_handle* h) {
   if (h->ev_gram) cudaEventDestroy(h->ev_gram);
   kbo_i_fit_partition_free(h);
   if (h->s_copy) cudaStreamDestroy(h->s_copy);
-  if (h->s_upd) cudaStreamDestroy(h->s_upd);
-  if (h->s_hi) cudaStreamDestroy(h->s_hi);
-  if (h->s_lo) cudaStreamDestroy(h->s_lo);
   for (auto* v : {&h->ev_var, &h->ev_cross, &h->ev_acq, &h->ev_cal})
     for (auto& p : *v) {
       cudaEventDestroy(p.first);

@@ -310,15 +310,9 @@ int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int l
 }
 
 // ------------------------------------------------------------------------------------------------
-// Streams and events of the multi-stream factorisations below.
-static int fit_streams(kbo_handle* h, int n_panels) {
-  if (!h->s_hi) {
-    int lo = 0, hi = 0;
-    KBO_CUDA(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    KBO_CUDA(h, cudaStreamCreateWithPriority(&h->s_hi, cudaStreamNonBlocking, hi));
-    KBO_CUDA(h, cudaStreamCreateWithPriority(&h->s_lo, cudaStreamNonBlocking, lo));
-  }
-  while ((int)h->ev_panel.size() < n_panels + 3) {
+// Events of the multi-stream factorisation below: the handle keeps at least n of them.
+static int fit_events(kbo_handle* h, int n) {
+  while ((int)h->ev_panel.size() < n) {
     cudaEvent_t e;
     KBO_CUDA(h, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     h->ev_panel.push_back(e);
@@ -327,204 +321,23 @@ static int fit_streams(kbo_handle* h, int n_panels) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// L = chol(K) and (rows of) W = L⁻¹ TOGETHER, version 2: LOOK-AHEAD on three streams (kept for A/B runs: KBO_FIT_V2=1; version 3
-// below is the default).  The Cholesky of N = 8192 is a chain of 128 single-CTA diagonal blocks with small panel kernels in
-// between — most of the GPU idles — and the inverse W_i,<i = −W_ii·(L_i,<i·W_<i,<i) of row panel i needs only the rows of L the
-// Cholesky has already finished, so it runs on another stream under the chain.  In potrf_impl every 64-block step touches all
-// N−k rows below it (panel solve + in-panel update: ~125 CTAs each), so when a trailing update runs beside the chain those kernels
-// queue for SM slots behind long GEMM blocks and the chain doubles in length.  Here the dependent chain
-// of a 256-column panel works on its 256×256 DIAGONAL block only — four single-CTA factorisations, ≤ 3-CTA solves, ≤ 9-CTA
-// updates — then inverts that block (needed for L⁻¹ anyway) and solves the whole panel below it with ONE GEMM against the
-// inverse.  The trailing update is issued on a second stream as [next column block | rest]: the next panel's chain starts as
-// soon as its own column block is up to date, while the rest of the update and the inverse's row panels (third stream) fill
-// the SMs the chain leaves idle.
-// `lead`: rows of the inverse to form (N: all of them).  The diagonal 256-blocks of W are formed for every panel either way.
-static int factor_and_invert_v2(kbo_handle* h, double* A, int N, int lda, double* W, int ldw, int* info_dev, cudaStream_t s, int lead) {
-  const int OW = 256, n_panels = (N + OW - 1) / OW;
-  KBO_TRY(fit_streams(h, 2 * n_panels + 8));
-  if (!h->s_upd) {
-    int lo = 0, hi = 0;
-    KBO_CUDA(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
-    KBO_CUDA(h, cudaStreamCreateWithPriority(&h->s_upd, cudaStreamNonBlocking, (lo + hi) / 2));
-  }
-  KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ldw));
-  KBO_TRY(kbo_reserve(h, h->T2, sizeof(double) * (size_t)N * OW));
-  KBO_TRY(kbo_reserve(h, h->Linv, sizeof(double) * KBO_NB * KBO_NB));
-  const int smem = 2 * KBO_NB * (KBO_NB + 1) * (int)sizeof(double);
-  if (!h->attr_fit) {
-    KBO_CUDA(h, cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    KBO_CUDA(h, cudaFuncSetAttribute(trsm_panel_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    KBO_CUDA(h, cudaFuncSetAttribute(diag_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    h->attr_fit = true;
-  }
-  double* T = (double*)h->T.p;
-  double* T2 = (double*)h->T2.p;
-  double* Linv = (double*)h->Linv.p;
-  cudaStream_t shi = h->s_hi, supd = h->s_upd, sinv = h->s_lo;
-  cudaEvent_t* ev_solve = h->ev_panel.data();                  // [n_panels]
-  cudaEvent_t* ev_col = h->ev_panel.data() + n_panels;         // [n_panels + 1]
-  cudaEvent_t e_start = h->ev_panel[2 * n_panels + 2], e_hi = h->ev_panel[2 * n_panels + 3], e_upd = h->ev_panel[2 * n_panels + 4],
-              e_inv = h->ev_panel[2 * n_panels + 5];
-  static const bool trace = getenv("KBO_FIT_TRACE") != nullptr;
-  cudaEvent_t tr[4] = {nullptr, nullptr, nullptr, nullptr};
-  std::vector<cudaEvent_t> tp;   // KBO_FIT_TRACE: per panel, on the chain stream: [enqueued | column block ready | diagonal block done | W_PP done | panel solved]
-  auto mark = [&]() {
-    if (!trace) return;
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    cudaEventRecord(e, h->s_hi);
-    tp.push_back(e);
-  };
-  if (trace) {
-    for (auto& e : tr) cudaEventCreate(&e);
-    cudaEventRecord(tr[0], s);
-  }
-  KBO_CUDA(h, cudaEventRecord(e_start, s));
-  KBO_CUDA(h, cudaStreamWaitEvent(shi, e_start, 0));
-  KBO_CUDA(h, cudaStreamWaitEvent(supd, e_start, 0));
-  KBO_CUDA(h, cudaStreamWaitEvent(sinv, e_start, 0));
-  KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, 2 * sizeof(int), shi));   // h->info: the pivot and who set it
-  KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, shi));
-  const int RW = 512;
-  int rp0 = 0;
-  int rc = KBO_OK;
-  auto body = [&]() -> int {
-    for (int K0 = 0, P = 0; K0 < N; K0 += OW, P++) {
-      const int Wd = min(OW, N - K0);
-      mark();
-      if (P > 0) KBO_CUDA(h, cudaStreamWaitEvent(shi, ev_col[P], 0));   // this panel's column block carries every earlier panel's update
-      mark();
-      // ---- the chain: the diagonal block only -------------------------------------------------------------------------
-      for (int k = K0; k < K0 + Wd; k += KBO_NB) {
-        const int jb = min(KBO_NB, N - k);
-        potf2_inv_kernel<<<1, POTF2_THREADS, smem, shi>>>(A + (size_t)k * lda + k, lda, jb, k, Linv, info_dev, W + (size_t)k * ldw + k, ldw);
-        KBO_LAUNCH_CHECK(h);
-        const int rows_in = K0 + Wd - (k + jb);
-        if (rows_in > 0) {
-          double* Pn = A + (size_t)(k + jb) * lda + k;
-          trsm_panel_kernel<<<(rows_in + 63) / 64, 256, smem, shi>>>(Pn, lda, rows_in, jb, Linv, info_dev);
-          KBO_LAUNCH_CHECK(h);
-          dgemm_sm90_launch<true>(shi, rows_in, rows_in, jb, Pn, lda, Pn, lda, A + (size_t)(k + jb) * lda + (k + jb), lda, -1.0, 1.0, KM_FULL, 0,
-                                  TS_LOWER);
-          KBO_LAUNCH_CHECK(h);
-        }
-      }
-      mark();
-      // ---- W_PP = L_PP⁻¹ (64-block inverses, recursive doubling inside the panel) -----------------------------------------
-      double* Wpp = W + (size_t)K0 * ldw + K0;
-      const double* Lpp = A + (size_t)K0 * lda + K0;
-      // (the 64-blocks' inverses were written into W's diagonal by potf2_inv_kernel)
-      for (int b = KBO_NB; b < Wd; b *= 2)
-        for (int r0 = 0; r0 + b < Wd; r0 += 2 * b) {
-          const int rows2 = min(b, Wd - (r0 + b));
-          double* T21 = T + (size_t)(K0 + r0 + b) * ldw + K0 + r0;
-          dgemm_sm90_launch<false>(shi, rows2, b, b, Lpp + (size_t)(r0 + b) * lda + r0, lda, Wpp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
-                                   KM_FROM_N, 0, TS_NONE);
-          KBO_LAUNCH_CHECK(h);
-          dgemm_sm90_launch<false>(shi, rows2, b, rows2, Wpp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
-                                   Wpp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
-          KBO_LAUNCH_CHECK(h);
-        }
-      mark();
-      // ---- the panel below the diagonal block: L_>P,P = A_>P,P · W_PPᵀ, one GEMM (W_PP lower triangular: k <= n) ------------------
-      const int rows_t = N - (K0 + Wd);
-      if (rows_t > 0) {
-        double* Pp = A + (size_t)(K0 + Wd) * lda + K0;
-        dgemm_sm90_launch<true>(shi, rows_t, Wd, Wd, Pp, lda, Wpp, ldw, T2, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
-        KBO_LAUNCH_CHECK(h);
-        KBO_CUDA(h, cudaMemcpy2DAsync(Pp, sizeof(double) * lda, T2, sizeof(double) * OW, sizeof(double) * Wd, rows_t, cudaMemcpyDeviceToDevice, shi));
-      }
-      mark();
-      KBO_CUDA(h, cudaEventRecord(ev_solve[P], shi));
-      // ---- trailing update, second stream: next column block first (look-ahead), then the rest ---------------------------------
-      if (rows_t > 0) {
-        KBO_CUDA(h, cudaStreamWaitEvent(supd, ev_solve[P], 0));
-        const double* Pp = A + (size_t)(K0 + Wd) * lda + K0;
-        const int nb = min(OW, rows_t);
-        dgemm_sm90_launch<true>(supd, rows_t, nb, Wd, Pp, lda, Pp, lda, A + (size_t)(K0 + Wd) * lda + (K0 + Wd), lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
-        KBO_LAUNCH_CHECK(h);
-        KBO_CUDA(h, cudaEventRecord(ev_col[P + 1], supd));
-        const int rows_r = rows_t - nb;
-        if (rows_r > 0) {
-          const double* Pr = Pp + (size_t)nb * lda;
-          dgemm_sm90_launch<true>(supd, rows_r, rows_r, Wd, Pr, lda, Pr, lda, A + (size_t)(K0 + Wd + nb) * lda + (K0 + Wd + nb), lda, -1.0, 1.0,
-                                  KM_FULL, 0, TS_LOWER);
-          KBO_LAUNCH_CHECK(h);
-        }
-      }
-      // ---- the inverse's row panel (512 rows = two panels), third stream ------------------------------------------------------
-      const int done = K0 + Wd;
-      if (rp0 < lead && (done - rp0 >= RW || done >= N)) {
-        const int P0 = rp0, Pw = done - rp0;
-        rp0 = done;
-        KBO_CUDA(h, cudaStreamWaitEvent(sinv, ev_solve[P], 0));
-        double* Wrp = W + (size_t)P0 * ldw + P0;
-        const double* Lrp = A + (size_t)P0 * lda + P0;
-        for (int b = OW; b < Pw; b *= 2)      // levels above the 256-panel inside the row panel
-          for (int r0 = 0; r0 + b < Pw; r0 += 2 * b) {
-            const int rows2 = min(b, Pw - (r0 + b));
-            double* T21 = T + (size_t)(P0 + r0 + b) * ldw + P0 + r0;
-            dgemm_sm90_launch<false>(sinv, rows2, b, b, Lrp + (size_t)(r0 + b) * lda + r0, lda, Wrp + (size_t)r0 * ldw + r0, ldw, T21, ldw, 1.0, 0.0,
-                                     KM_FROM_N, 0, TS_NONE);
-            KBO_LAUNCH_CHECK(h);
-            dgemm_sm90_launch<false>(sinv, rows2, b, rows2, Wrp + (size_t)(r0 + b) * ldw + r0 + b, ldw, T21, ldw,
-                                     Wrp + (size_t)(r0 + b) * ldw + r0, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
-            KBO_LAUNCH_CHECK(h);
-          }
-        if (P0 > 0) {
-          double* Trow = T + (size_t)P0 * ldw;
-          dgemm_sm90_launch<false>(sinv, Pw, P0, P0, A + (size_t)P0 * lda, lda, W, ldw, Trow, ldw, 1.0, 0.0, KM_FROM_N, 0, TS_NONE);
-          KBO_LAUNCH_CHECK(h);
-          dgemm_sm90_launch<false>(sinv, Pw, P0, Pw, Wrp, ldw, Trow, ldw, W + (size_t)P0 * ldw, ldw, -1.0, 0.0, KM_UPTO_M, 0, TS_NONE);
-          KBO_LAUNCH_CHECK(h);
-        }
-      }
-    }
-    return KBO_OK;
-  };
-  rc = body();
-  cudaEventRecord(e_hi, shi);
-  cudaEventRecord(e_upd, supd);
-  cudaEventRecord(e_inv, sinv);
-  cudaStreamWaitEvent(s, e_hi, 0);
-  cudaStreamWaitEvent(s, e_upd, 0);
-  cudaStreamWaitEvent(s, e_inv, 0);
-  if (tr[0]) {
-    cudaEventRecord(tr[1], shi);
-    cudaEventRecord(tr[2], supd);
-    cudaEventRecord(tr[3], sinv);
-    cudaStreamSynchronize(shi); cudaStreamSynchronize(supd); cudaStreamSynchronize(sinv);
-    float a = 0.f, b = 0.f, c = 0.f;
-    cudaEventElapsedTime(&a, tr[0], tr[1]); cudaEventElapsedTime(&b, tr[0], tr[2]); cudaEventElapsedTime(&c, tr[0], tr[3]);
-    fprintf(stderr, "[kbo fit v2 N=%d] chain stream done at %.3f ms, update stream at %.3f ms, inverse stream at %.3f ms\n", N, a, b, c);
-    double sum[4] = {0, 0, 0, 0};
-    for (size_t i = 0; i + 4 < tp.size() + 0 && i + 4 <= tp.size() - 1; i += 5) {
-      float w, d, iv, so;
-      cudaEventElapsedTime(&w, tp[i], tp[i + 1]);
-      cudaEventElapsedTime(&d, tp[i + 1], tp[i + 2]);
-      cudaEventElapsedTime(&iv, tp[i + 2], tp[i + 3]);
-      cudaEventElapsedTime(&so, tp[i + 3], tp[i + 4]);
-      sum[0] += w; sum[1] += d; sum[2] += iv; sum[3] += so;
-      if ((i / 5) % 8 == 0) fprintf(stderr, "   panel %2d: wait for column block %.3f | diagonal block %.3f | W_PP %.3f | panel solve %.3f ms\n", (int)(i / 5), w, d, iv, so);
-    }
-    fprintf(stderr, "   chain totals: waiting %.3f | diagonal blocks %.3f | W_PP %.3f | panel solves %.3f ms\n", sum[0], sum[1], sum[2], sum[3]);
-    for (auto& e : tp) cudaEventDestroy(e);
-    for (auto& e : tr) cudaEventDestroy(e);
-  }
-  return rc;
-}
-
-// ------------------------------------------------------------------------------------------------
-// Version 3: the chain on its OWN SMs, the panel below it solved in its shadow.
-// What v2's chain-stream trace showed (KBO_FIT_TRACE, N = 8192): the four single-CTA factorisations of a panel take more
-// than twice as long while trailing updates run as on an idle GPU — the update GEMMs hold two 128-register CTAs per SM, i.e. the
-// whole register file, so a chain kernel waits until an SM drains (stream priority orders pending CTAs; it does not preempt) —
-// and W_PP plus the one-GEMM panel solve add dependent launches per panel.  Here
+// L = chol(K) and (rows of) W = L⁻¹ TOGETHER: the chain on its OWN SMs, the panel below it solved in its shadow.
+// The Cholesky of N = 8192 is a chain of 128 single-CTA diagonal blocks with small panel kernels in between — most of the GPU
+// idles — and the inverse W_i,<i = −W_ii·(L_i,<i·W_<i,<i) of row panel i needs only the rows of L the Cholesky has already
+// finished, so it runs on another stream under the chain.  The dependent chain of a 256-column panel works on its 256×256
+// DIAGONAL block only (four single-CTA factorisations, ≤ 3-CTA solves, ≤ 9-CTA updates), and the trailing update LOOKS AHEAD:
+// the next column blocks are updated first, so the next panel's chain starts as soon as its own column block is up to date,
+// while the rest of the update and the inverse's row panels fill the SMs the chain leaves idle.
+// On SMs shared with the updates that chain is slow (KBO_FIT_TRACE, N = 8192): the four single-CTA factorisations of a panel take
+// more than twice as long while trailing updates run as on an idle GPU — the update GEMMs hold two 128-register CTAs per SM, i.e.
+// the whole register file, so a chain kernel waits until an SM drains (stream priority orders pending CTAs; it does not preempt) —
+// and inverting the diagonal block and solving the panel below it with one GEMM against that inverse, on the chain's stream, add
+// dependent launches per panel.  Here
 //  * a GREEN CONTEXT (CUDA 12.4+) gives the chain stream 8 SMs of its own; everything else runs on the rest.  If the
 //    driver cannot split the device the same streams are created unpartitioned and only the second point applies;
 //  * the rows below the diagonal block are solved column block by column block on a second stream AS the chain produces the
 //    64×64 inverses (four buffers): after the last factorisation only one 64-column solve remains before the trailing update
-//    can start.  W_PP (for L⁻¹ and the triangular solves) moves to the inverse stream, off the critical path.
+//    can start.  W_PP (for L⁻¹ and the triangular solves) is formed on a stream of its own, off the critical path.
 // Driver entry points come from cudaGetDriverEntryPoint: libkbo links the runtime only.
 #include <cuda.h>
 namespace {
@@ -576,16 +389,16 @@ static bool profiler_attached() {
 
 // The streams of the v3 factorisation (roles: kbo_internal.cuh).  partitioned = true asks for the green-context set (created once;
 // falls back to the plain set if the driver cannot split the device).
-#define FIT_NSTREAMS 13
+#define FIT_NSTREAMS 10
 static int fit_partition(kbo_handle* h, bool partitioned, cudaStream_t (&out)[FIT_NSTREAMS]) {
   int lo = 0, hi = 0;
   KBO_CUDA(h, cudaDeviceGetStreamPriorityRange(&lo, &hi));
   int prio[FIT_NSTREAMS];   // numerically lower = more urgent
   prio[0] = prio[1] = prio[2] = prio[3] = hi;
-  for (int k = 2; k <= 6; k++) prio[2 + k] = min(lo, hi + (k - 1));
-  prio[9] = max(hi, lo - 1);
-  prio[10] = lo;
-  prio[11] = prio[12] = hi;
+  for (int k = 2; k <= 4; k++) prio[2 + k] = min(lo, hi + (k - 1));
+  prio[7] = max(hi, lo - 1);
+  prio[8] = lo;
+  prio[9] = hi;
   static const bool off = getenv("KBO_FIT_NO_PARTITION") != nullptr;
   const DrvApi& d = drv();
   if (partitioned && !h->part_tried && !off && d.ok && !profiler_attached()) {
@@ -601,7 +414,7 @@ static int fit_partition(kbo_handle* h, bool partitioned, cudaStream_t (&out)[FI
               d.GreenCtxCreate(&gc, dc, dev, CU_GREEN_CTX_DEFAULT_STREAM) == CUDA_SUCCESS;
     ok = ok && d.GreenCtxCreate(&gr, dr, dev, CU_GREEN_CTX_DEFAULT_STREAM) == CUDA_SUCCESS;
     for (int i = 0; ok && i < FIT_NSTREAMS; i++)
-      ok = d.GreenCtxStreamCreate((CUstream*)&h->s3g[i], (i < 2 || i >= 11) ? gc : gr, CU_STREAM_NON_BLOCKING, prio[i]) == CUDA_SUCCESS;
+      ok = d.GreenCtxStreamCreate((CUstream*)&h->s3g[i], (i < 2 || i == 9) ? gc : gr, CU_STREAM_NON_BLOCKING, prio[i]) == CUDA_SUCCESS;
     if (ok) {
       h->gctx_chain = gc;
       h->gctx_rest = gr;
@@ -644,20 +457,17 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
                                 cudaEvent_t e_early = nullptr) {
   // e_early (optional): the first column block of A is complete and info / W are zeroed (the caller did both); the rest of A follows
   // on s.  The chain-side streams then start on e_early; everything that touches other column blocks waits for the whole matrix.
-  // panel width: 256 (four 64-blocks per panel), or KBO_FIT_OW=512 (eight): wider panels make the trailing updates K = 512 GEMMs
-  static const int ow_env = getenv("KBO_FIT_OW") ? atoi(getenv("KBO_FIT_OW")) : 0;
-  const int OW = ow_env == 512 ? 512 : 256, NB = KBO_NB, n_panels = (N + OW - 1) / OW;
-  // look-ahead depth: column blocks at distance 1..depth from the panel get their own GEMM (and stream) per panel, the bulk of the
-  // trailing update covers the rest — the chain can run `depth` − 1 panels ahead of the bulk (KBO_FIT_DEPTH=1: [next block | rest])
-  static const int depth_env = getenv("KBO_FIT_DEPTH") ? atoi(getenv("KBO_FIT_DEPTH")) : 0;
-  const int Dn = OW == 256 ? (depth_env >= 1 && depth_env <= 6 ? depth_env : 3) : 1;
+  // panel width 256: four 64-blocks per panel
+  const int OW = 256, NB = KBO_NB, n_panels = (N + OW - 1) / OW;
+  // look-ahead depth: column blocks at distance 1..Dn from the panel get their own GEMM (and stream) per panel, the bulk of the
+  // trailing update covers the rest — the chain can run Dn − 1 panels ahead of the bulk
+  const int Dn = 3;
   // merged bulks: the bulk updates of panels (P, P+1), P even, run as ONE K = 512 GEMM after panel P+1 (a faster GEMM shape, half
   // the passes over the trailing matrix); the even panel covers the column block the merged region misses with one more distance GEMM
-  static const bool pair_env = !(getenv("KBO_FIT_PAIR") && atoi(getenv("KBO_FIT_PAIR")) == 0);
-  const bool pairs = pair_env && OW == 256 && Dn >= 2 && Dn <= 5;
-  auto kmax_of = [&](int P) { return pairs && (P % 2 == 0) ? Dn + 1 : Dn; };
+  auto kmax_of = [&](int P) { return P % 2 == 0 ? Dn + 1 : Dn; };
   const int CBW = Dn + 2;   // events per column block: distances 1..Dn+1
-  KBO_TRY(fit_streams(h, (12 + Dn) * n_panels + 8 * CBW + 80));
+  // the event layout below: six per panel (+ 2), CBW per column block, 32 singles, and W_PP's per panel
+  KBO_TRY(fit_events(h, 6 * n_panels + 2 + (n_panels + 8) * CBW + 32 + n_panels));
   // the SM partition pays when trailing updates big enough to fill the GPU run beside the chain; small factorisations (and any
   // process a profiler is attached to) use plain priority streams
   cudaStream_t st5[FIT_NSTREAMS];
@@ -665,7 +475,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   const bool partitioned = st5[0] == h->s3g[0] && h->part_ok;
   KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ldw));
   KBO_TRY(kbo_reserve(h, h->T2, sizeof(double) * (size_t)N * OW));
-  KBO_TRY(kbo_reserve(h, h->Linv4, sizeof(double) * 2 * 8 * NB * NB));
+  KBO_TRY(kbo_reserve(h, h->Linv4, sizeof(double) * 2 * 4 * NB * NB));
   const int smem = 2 * NB * (NB + 1) * (int)sizeof(double);
   if (!h->attr_fit) {
     KBO_CUDA(h, cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -679,7 +489,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   // the far shadow of panel P may still be reading its set (it is done before the chain of panel P+2 can start: that one waits for
   // the near shadow of P+1, which waits for the distance-1 update of P, which waits for the far shadow of P)
   double* Linv_sets = (double*)h->Linv4.p;
-  cudaStream_t sc = st5[0], sn = st5[1], ss = st5[2], su = st5[3], sb = st5[9], si = st5[10], sw = st5[11], sm = st5[12];
+  cudaStream_t sc = st5[0], sn = st5[1], ss = st5[2], su = st5[3], sb = st5[7], si = st5[8], sw = st5[9];
   cudaStream_t* colS = st5 + 2;   // colS[k]: column-block updates at distance k (colS[1] == su)
   cudaEvent_t* ev_solve = h->ev_panel.data();                     // [n_panels]     the FAR rows below the diagonal block (past the next block) are L
   cudaEvent_t* ev_col = h->ev_panel.data() + n_panels;            // [n_panels + 1] column block P, rows below its diagonal block, carries every earlier update
@@ -687,19 +497,12 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   cudaEvent_t* ev_near = h->ev_panel.data() + 3 * n_panels + 1;   // [n_panels + 1] diagonal block P carries every earlier update: the chain may start
   cudaEvent_t* ev_nsolve = h->ev_panel.data() + 4 * n_panels + 2; // [n_panels]     the NEAR rows (the next diagonal block's rows) of panel P are L
   cudaEvent_t* ev_rest = h->ev_panel.data() + 5 * n_panels + 2;   // [n_panels]     trailing update of panel P done
-  cudaEvent_t* ev_cb = h->ev_panel.data() + 6 * n_panels + 2;     // [(n_panels + 8) × (Dn + 1)] column block j updated through distance k
+  cudaEvent_t* ev_cb = h->ev_panel.data() + 6 * n_panels + 2;     // [(n_panels + 8) × CBW] column block j updated through distance k
   cudaEvent_t* ev_x = ev_cb + (size_t)(n_panels + 8) * CBW;  // pf[8], tr[8], start, joins
   cudaEvent_t *ev_pf = ev_x, *ev_tr = ev_x + 8, e_start = ev_x[16], *e_join = ev_x + 17;
-  std::vector<cudaStream_t> all_streams = {sc, sn, ss, sb, si, sw, sm};
+  std::vector<cudaStream_t> all_streams = {sc, sn, ss, sb, si, sw};
   cudaEvent_t* ev_wpp = ev_x + 32;   // [n_panels] W_PP complete
-  cudaEvent_t *ev_mid = ev_wpp + n_panels, *ev_t1 = ev_mid + n_panels, *ev_t2 = ev_t1 + n_panels;   // MID rows solved; their two 256×256 updates done
-  // MID rows (KBO_FIT_MID=1, off by default) = the second block below the diagonal block, solved against W_PP on the chain's partition
-  // together with their updates of blocks (P+2,P+1) and (P+2,P+2), so that the next panel's near shadow and the chain two panels on
-  // do not wait for the FAR shadow and the distance-1 update.  The dependency moves (KBO_FIT_TRACE=2), but the big partition is
-  // saturated by the updates, so the far GEMMs are slow whichever chain waits for them.  Kept as a tested variant.
-  static const bool mid_env = getenv("KBO_FIT_MID") && atoi(getenv("KBO_FIT_MID")) != 0;
-  const bool midmode = mid_env && OW == 256 && Dn >= 2;
-  for (int k = 1; k <= (pairs ? Dn + 1 : Dn); k++) all_streams.push_back(colS[k]);
+  for (int k = 1; k <= Dn + 1; k++) all_streams.push_back(colS[k]);
   static const bool trace = getenv("KBO_FIT_TRACE") != nullptr;
   cudaEvent_t tr[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   std::vector<cudaEvent_t> tp;   // per panel on the chain stream: enqueued | column block ready | diagonal block done
@@ -730,7 +533,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
     KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, s));   // on the caller's stream: all SMs, not the chain's 8
   }
   // a lazy fit takes alpha from triangular solves: the forward one (z = L⁻¹·yn) is carried along, one panel behind (solve.cu)
-  const bool zsolve = lead < N && OW == 256 && A == (double*)h->K.p && W == (double*)h->W.p && N == h->N && lda == h->ld;
+  const bool zsolve = lead < N && A == (double*)h->K.p && W == (double*)h->W.p && N == h->N && lda == h->ld;
   if (zsolve) KBO_TRY(kbo_i_zsolve_begin(h, s));
   KBO_CUDA(h, cudaEventRecord(e_start, s));
   for (cudaStream_t st : all_streams) {
@@ -743,7 +546,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
     for (int K0 = 0, P = 0; K0 < N; K0 += OW, P++) {
       const int Wd = min(OW, N - K0), rows_t = N - (K0 + Wd);
       const int nblk = (Wd + NB - 1) / NB;
-      double* Linv4 = Linv_sets + (size_t)(P & 1) * 8 * NB * NB;
+      double* Linv4 = Linv_sets + (size_t)(P & 1) * 4 * NB * NB;
       mark();
       if (P > 0) KBO_CUDA(h, cudaStreamWaitEvent(sc, ev_near[P], 0));
       mark();
@@ -786,7 +589,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           KBO_LAUNCH_CHECK(h);
           return KBO_OK;
         };
-        if (OW == 256 && nblk == 4) {
+        if (nblk == 4) {
           KBO_CUDA(h, cudaStreamWaitEvent(sw, ev_pf[1], 0));   // blocks 0, 1 factored (and L[1][0] solved before block 1 was)
           KBO_TRY(level(NB, 0));
           KBO_CUDA(h, cudaStreamWaitEvent(sw, ev_chain[P], 0));
@@ -804,7 +607,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
       // block (on the chain's SMs: 4-CTA kernels that must not queue behind GEMM blocks) — all the next panel's chain waits for is
       // their solve and the 256×256 update of its diagonal block; FAR = the rest, on the big partition ------------------------------
       if (rows_t > 0) {
-        const int n_near = min(OW, rows_t), n_mid = midmode ? min(OW, rows_t - n_near) : 0, n_far = rows_t - n_near - n_mid;
+        const int n_near = min(OW, rows_t), n_far = rows_t - n_near;
         auto shadow = [&](cudaStream_t st, int r0, int nrows, cudaEvent_t ready) -> int {
           if (ready) KBO_CUDA(h, cudaStreamWaitEvent(st, ready, 0));   // these rows of the column block carry the earlier updates too
           for (int b = 0; b < nblk; b++) {
@@ -822,9 +625,9 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           }
           return KBO_OK;
         };
-        const int rn = K0 + Wd, rm = rn + n_near, rf = rm + n_mid;
-        // block (P+1, P) got its last update from the previous panel's MID rows (or, without them, its distance-1 update)
-        KBO_TRY(shadow(sn, rn, n_near, P > 0 ? (midmode ? ev_t1[P - 1] : ev_col[P]) : nullptr));
+        const int rn = K0 + Wd, rf = rn + n_near;
+        // block (P+1, P) got its last update from the previous panel's distance-1 update
+        KBO_TRY(shadow(sn, rn, n_near, P > 0 ? ev_col[P] : nullptr));
         KBO_CUDA(h, cudaEventRecord(ev_nsolve[P], sn));
         tmark(sn, "near shadow done", P);
         // What was added to a column block last before this panel's distance-k update: panel P−1's update at distance k+1 if it made
@@ -834,35 +637,14 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           return k + 1 <= kmax_of(P - 1) ? ev_cb[(size_t)(P + k) * CBW + k + 1] : ev_rest[P - 1];
         };
         cudaEvent_t pred1 = pred_of(1);
-        // the next diagonal block's own update (after the previous panel's MID update of the same block, or the distance-2 update)
+        // the next diagonal block's own update (after the previous panel's distance-2 update of the same block)
         if (P == 0 && e_early) KBO_CUDA(h, cudaStreamWaitEvent(sn, e_start, 0));   // that block is not in the first column block
-        if (cudaEvent_t pe = midmode ? (P > 0 ? ev_t2[P - 1] : nullptr) : pred1) KBO_CUDA(h, cudaStreamWaitEvent(sn, pe, 0));
+        if (pred1) KBO_CUDA(h, cudaStreamWaitEvent(sn, pred1, 0));
         const double* Ln = A + (size_t)rn * lda + K0;
         dgemm_sm90_launch<true>(sn, n_near, n_near, Wd, Ln, lda, Ln, lda, A + (size_t)rn * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
         KBO_LAUNCH_CHECK(h);
         KBO_CUDA(h, cudaEventRecord(ev_near[P + 1], sn));
         tmark(sn, "next diagonal block updated", P);
-        const double* Lm = A + (size_t)rm * lda + K0;
-        if (n_mid > 0) {
-          // MID rows on the chain's partition (their own stream: W_PP of the next panel must not queue behind a wait of theirs): L_mid = A_mid·W_PPᵀ, then blocks (P+2,P+1) and (P+2,P+2)
-          double* T2m = T2 + (size_t)(N - OW) * OW;   // the far GEMM uses at most the first N − 3·256 rows of T2
-          if (P > 0) KBO_CUDA(h, cudaStreamWaitEvent(sm, ev_col[P], 0));
-          KBO_CUDA(h, cudaStreamWaitEvent(sm, ev_wpp[P], 0));
-          dgemm_sm90_launch<true>(sm, n_mid, Wd, Wd, Lm, lda, W + (size_t)K0 * ldw + K0, ldw, T2m, OW, 1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
-          KBO_LAUNCH_CHECK(h);
-          KBO_CUDA(h, cudaMemcpy2DAsync((double*)Lm, sizeof(double) * lda, T2m, sizeof(double) * OW, sizeof(double) * Wd, n_mid, cudaMemcpyDeviceToDevice, sm));
-          KBO_CUDA(h, cudaEventRecord(ev_mid[P], sm));
-          KBO_CUDA(h, cudaStreamWaitEvent(sm, ev_nsolve[P], 0));
-          if (pred1) KBO_CUDA(h, cudaStreamWaitEvent(sm, pred1, 0));
-          dgemm_sm90_launch<true>(sm, n_mid, n_near, Wd, Lm, lda, Ln, lda, A + (size_t)rm * lda + rn, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
-          KBO_LAUNCH_CHECK(h);
-          KBO_CUDA(h, cudaEventRecord(ev_t1[P], sm));
-          if (cudaEvent_t pe = pred_of(2)) KBO_CUDA(h, cudaStreamWaitEvent(sm, pe, 0));
-          dgemm_sm90_launch<true>(sm, n_mid, n_mid, Wd, Lm, lda, Lm, lda, A + (size_t)rm * lda + rm, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
-          KBO_LAUNCH_CHECK(h);
-          KBO_CUDA(h, cudaEventRecord(ev_t2[P], sm));
-          tmark(sm, "mid rows solved, their two updates done", P);
-        }
         if (n_far > 0) {
           // FAR rows: one GEMM against W_PP (L_far = A_far·W_PPᵀ, out of place + copy) instead of seven 64-column steps — under the bulk
           // updates every small kernel of the big partition waits for SM slots (KBO_FIT_TRACE=2 timeline: the seven steps queue,
@@ -875,7 +657,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           KBO_CUDA(h, cudaMemcpy2DAsync(Pf, sizeof(double) * lda, T2, sizeof(double) * OW, sizeof(double) * Wd, n_far, cudaMemcpyDeviceToDevice, ss));
           KBO_CUDA(h, cudaEventRecord(ev_solve[P], ss));
           tmark(ss, "far shadow done", P);
-          // ---- trailing update.  Distance 1: the next column block's FAR rows (the next panel's mid and far shadows wait for it)
+          // ---- trailing update.  Distance 1: the next column block's FAR rows (the next panel's far shadow waits for it)
           KBO_CUDA(h, cudaStreamWaitEvent(su, ev_solve[P], 0));
           KBO_CUDA(h, cudaStreamWaitEvent(su, ev_nsolve[P], 0));
           if (pred1) KBO_CUDA(h, cudaStreamWaitEvent(su, pred1, 0));
@@ -884,19 +666,9 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
           KBO_LAUNCH_CHECK(h);
           KBO_CUDA(h, cudaEventRecord(ev_col[P + 1], su));
           tmark(su, "distance-1 update done", P);
-          if (n_mid > 0) {   // distance 2, FAR rows: the diagonal block of that column block was the MID rows' second update
-            cudaStream_t st = colS[2];
-            KBO_CUDA(h, cudaStreamWaitEvent(st, ev_solve[P], 0));
-            KBO_CUDA(h, cudaStreamWaitEvent(st, ev_mid[P], 0));
-            if (cudaEvent_t pe = pred_of(2)) KBO_CUDA(h, cudaStreamWaitEvent(st, pe, 0));
-            dgemm_sm90_launch<true>(st, n_far, n_mid, Wd, Lf, lda, Lm, lda, A + (size_t)rf * lda + rm, lda, -1.0, 1.0, KM_FULL, 0, TS_NONE);
-            KBO_LAUNCH_CHECK(h);
-            KBO_CUDA(h, cudaEventRecord(ev_cb[(size_t)(P + 2) * CBW + 2], st));
-            tmark(st, "distance-2 update done", P);
-          }
-          // distances 2..Dn: column block j = P + k, rows from its diagonal block down; each after what was added to that block before
+          // distances 2..kmax_of(P): column block j = P + k, rows from its diagonal block down; each after what was added to that block before
           // (distance k + 1 of the previous panel, or — the farthest — the previous panel's bulk)
-          for (int k = n_mid > 0 ? 3 : 2; k <= kmax_of(P); k++) {
+          for (int k = 2; k <= kmax_of(P); k++) {
             const int j = P + k, c0 = j * OW;
             if (c0 >= N) break;
             cudaStream_t st = colS[k];
@@ -906,12 +678,12 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
             dgemm_sm90_launch<true>(st, N - c0, min(OW, N - c0), Wd, Lc, lda, Lc, lda, A + (size_t)c0 * lda + c0, lda, -1.0, 1.0, KM_FULL, 0, TS_LOWER);
             KBO_LAUNCH_CHECK(h);
             KBO_CUDA(h, cudaEventRecord(ev_cb[(size_t)j * CBW + k], st));
-            tmark(st, k == 2 ? "distance-2 update done" : k == 3 ? "distance-3 update done" : "distance-4+ update done", P);
+            tmark(st, k == 2 ? "distance-2 update done" : k == 3 ? "distance-3 update done" : "distance-4 update done", P);
           }
-          // the bulk: every column block farther than that — per panel, or (merged) for the pair (P−1, P) after the odd panel
-          if (!pairs || (P % 2 == 1)) {
-            const int Pb = pairs ? P - 1 : P;   // first panel of the bulk
-            const int cB = (Pb + kmax_of(Pb) + 1) * OW, Kb = pairs ? 2 * OW : Wd;
+          // the bulk: every column block farther than that, merged for the pair (P−1, P) after the odd panel
+          if (P % 2 == 1) {
+            const int Pb = P - 1;   // first panel of the bulk
+            const int cB = (Pb + kmax_of(Pb) + 1) * OW, Kb = 2 * OW;
             if (cB < N) {
               KBO_CUDA(h, cudaStreamWaitEvent(sb, ev_solve[P], 0));
               const double* Lb = A + (size_t)cB * lda + (size_t)Pb * OW;
@@ -927,8 +699,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
         KBO_TRY(kbo_i_zsolve_diag(h, K0, Wd, si));
         if (rows_t > 0) {
           KBO_CUDA(h, cudaStreamWaitEvent(si, ev_nsolve[P], 0));
-          if (midmode && rows_t > OW) KBO_CUDA(h, cudaStreamWaitEvent(si, ev_mid[P], 0));
-          if (rows_t > (midmode ? 2 : 1) * OW) KBO_CUDA(h, cudaStreamWaitEvent(si, ev_solve[P], 0));
+          if (rows_t > OW) KBO_CUDA(h, cudaStreamWaitEvent(si, ev_solve[P], 0));
           KBO_TRY(kbo_i_zsolve_update(h, K0, Wd, si));
         }
       }
@@ -939,7 +710,6 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
         if (P > 0) {   // rows [P0, done) of L left of this panel: the earlier panels' shadows
           KBO_CUDA(h, cudaStreamWaitEvent(si, ev_solve[P - 1], 0));
           KBO_CUDA(h, cudaStreamWaitEvent(si, ev_nsolve[P - 1], 0));
-          if (midmode) KBO_CUDA(h, cudaStreamWaitEvent(si, ev_mid[P - 1], 0));
         }
         double* Wrp = W + (size_t)P0 * ldw + P0;
         const double* Lrp = A + (size_t)P0 * lda + P0;
@@ -993,8 +763,8 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
       sum[1] += d;
       if ((i / 3) % 8 == 0) fprintf(stderr, "   panel %2d: wait for column block %.3f | diagonal block %.3f ms\n", (int)(i / 3), w, d);
     }
-    fprintf(stderr, "   chain totals: waiting %.3f | diagonal blocks %.3f ms; host enqueue of the whole factorisation %.3f ms (depth %d)\n", sum[0], sum[1],
-            host_ms, Dn);
+    fprintf(stderr, "   chain totals: waiting %.3f | diagonal blocks %.3f ms; host enqueue of the whole factorisation %.3f ms\n", sum[0], sum[1],
+            host_ms);
     if (!tl.empty()) {
       std::vector<std::pair<float, size_t>> order;
       for (size_t i = 0; i < tl.size(); i++) {
@@ -1251,12 +1021,10 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
   if (trace)
     for (auto& e : te) cudaEventCreate(&e);
   if (trace) cudaEventRecord(te[0], s);
-  static const bool serial = getenv("KBO_FIT_SERIAL") != nullptr;   // A/B: Cholesky, then recursive-doubling inverse, on one stream
-  static const bool v2_env = getenv("KBO_FIT_V2") != nullptr;
-  static const bool early_env = !(getenv("KBO_FIT_EARLY") && atoi(getenv("KBO_FIT_EARLY")) == 0);
-  const bool early = early_env && !serial && !v2_env && N >= 1024;   // v3 starts on the first column block of the Gram matrix
+  // the one-stream reference: Cholesky, then recursive-doubling inverse (kbo_potrf, kbo_trtri)
+  static const bool serial = getenv("KBO_FIT_SERIAL") != nullptr;
+  const bool early = !serial && N >= 1024;   // v3 starts on the first column block of the Gram matrix
   if (early) {
-    KBO_TRY(fit_streams(h, 8));
     KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, 2 * sizeof(int), s));
     KBO_CUDA(h, cudaMemsetAsync(h->W.p, 0, sizeof(double) * (size_t)N * ld, s));
     if (!h->ev_gram) KBO_CUDA(h, cudaEventCreateWithFlags(&h->ev_gram, cudaEventDisableTiming));
@@ -1283,11 +1051,7 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
         const int P1 = h->rank_prefix < 0 ? (n_pairs + 7) / 8 : h->rank_prefix;
         if (P1 >= 1 && P1 < n_pairs && P1 * 512 + 512 <= N) lead = round_up(P1 * 512, 512);
       }
-      static const bool v2 = getenv("KBO_FIT_V2") != nullptr;   // A/B: look-ahead without the SM partition and the shadow solve
-      if (v2)
-        KBO_TRY(factor_and_invert_v2(h, (double*)h->K.p, N, ld, (double*)h->W.p, ld, (int*)h->info.p, s, lead));
-      else
-        KBO_TRY(factor_and_invert_v3(h, (double*)h->K.p, N, ld, (double*)h->W.p, ld, (int*)h->info.p, s, lead, early ? h->ev_gram : nullptr));
+      KBO_TRY(factor_and_invert_v3(h, (double*)h->K.p, N, ld, (double*)h->W.p, ld, (int*)h->info.p, s, lead, early ? h->ev_gram : nullptr));
       h->w_lead = lead < N ? lead : N;
       h->w_full = lead >= N;
     }

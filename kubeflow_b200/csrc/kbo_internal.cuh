@@ -96,16 +96,15 @@ struct kbo_handle {
   };
   bool record_stages = false;
   std::vector<StageRec> stage_recs;
-  // ---- fit: Cholesky chain on a high-priority stream, row-panel inverse on a second one (fit.cu) ----------------------
-  cudaStream_t s_hi = nullptr, s_lo = nullptr, s_upd = nullptr, s_copy = nullptr;
-  DevBuf T2;                        // N × 256 panel-solve scratch of the look-ahead factorisation (v2)
-  // v3: the chain runs on its own SM partition (green contexts); shadow panel solve / trailing update / inverse share the rest
+  cudaStream_t s_copy = nullptr;   // the candidate grid's host-to-device copy, beside the fit (api.cu)
+  // ---- fit: the chain runs on its own SM partition (green contexts); shadow panel solve / trailing update / inverse share the rest (fit.cu)
+  DevBuf T2;                        // N × 256 scratch of the far rows' panel solve
   bool part_tried = false, part_ok = false;
   void *gctx_chain = nullptr, *gctx_rest = nullptr;   // CUgreenCtx
-  // stream roles: 0 chain, 1 near shadow (both on the chain's partition), 2 far shadow, 3..8 column-block updates at distance 1..6,
-  // 9 bulk trailing update, 10 inverse, 11 W_PP and 12 MID rows (both on the chain's partition)
-  cudaStream_t s3g[13] = {};       // green-context set
-  cudaStream_t s3p[13] = {};       // the same roles as plain priority streams (small N, profilers, no green contexts)
+  // stream roles: 0 chain, 1 near shadow (both on the chain's partition), 2 far shadow, 3..6 column-block updates at distance 1..4,
+  // 7 bulk trailing update, 8 inverse, 9 W_PP (on the chain's partition)
+  cudaStream_t s3g[10] = {};       // green-context set
+  cudaStream_t s3p[10] = {};       // the same roles as plain priority streams (small N, profilers, no green contexts)
   DevBuf Linv4;                     // the four 64×64 block inverses of the current panel
   std::vector<cudaEvent_t> ev_panel;
   cudaEvent_t ev_gram = nullptr;   // the first column block of the Gram matrix is complete (the factorisation starts on it)

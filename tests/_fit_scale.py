@@ -5,7 +5,8 @@ come back: per-256×256-tile worst errors and where they are, the suggestion, a 
 on whatever an engine holds after kbo_fit_append / kbo_fit_rebase chains (test_gpu_append_scale.py).
 
     python tests/_fit_scale.py '<json spec>' out.json
-spec: {"fits": [[N, case, var_mode, ref_prefix], ...]}  or  {"pivots": [[N, p], ...], "var_mode": "f64"|"tc"}
+spec: {"fits": [[N, case, var_mode, ref_prefix], ...]}  or  {"digests": [[N, var_mode], ...]}
+      or  {"pivots": [[N, p], ...], "var_mode": "f64"|"tc"}
 """
 import ctypes as C
 import hashlib
@@ -192,6 +193,33 @@ def measure(N, case, var_mode, prefix):
     return r
 
 
+def _sha(*arrays):
+    h = hashlib.sha256()
+    for a in arrays:
+        h.update(np.ascontiguousarray(a).tobytes())
+    return h.hexdigest()
+
+
+def digests(N, var_mode, case="m32"):
+    """SHA-256 of everything one fit and one suggestion produce, bit for bit: tril(L) and alpha (a tensor-core fit's before the
+    rest of W is formed), the LML and y statistics, the suggestion over M_CAND candidates, and W for an FP64 fit."""
+    X, y, Xc, th = history(N, case)
+    e = engine(th, var_mode)
+    e.tell(X, y)
+    Lm, _, al = state(e, with_w=False)
+    r = dict(L=_sha(torch.tril(Lm).cpu().numpy()), alpha=_sha(al.cpu().numpy()))
+    del Lm, al
+    fi = e.fit_info()
+    r["fit"] = _sha(np.array([fi["lml"], fi["y_mean"], fi["y_std"], fi["y_opt"]], dtype=np.float64))
+    b = e.ask(Xc)
+    r["ask"] = _sha(np.array([b.index], dtype=np.int64), np.array([b.value, b.mu, b.std], dtype=np.float64))
+    if var_mode == "f64":
+        r["W"] = _sha(torch.tril(state(e)[1]).cpu().numpy())
+    e.close()
+    torch.cuda.empty_cache()
+    return r
+
+
 def pivot_engine(var_mode):
     """RBF, amplitude 1, ℓ = 1, noise 0: the θ under which oracle.not_pd_at's histories fail at exactly the chosen pivot."""
     return GPEngine(0, kernel="rbf", acq="ei", var_mode=var_mode, length_scale=1.0, amplitude=1.0, noise=0.0)
@@ -231,6 +259,8 @@ if __name__ == "__main__":
     spec, out = json.loads(sys.argv[1]), sys.argv[2]
     if "fits" in spec:
         res = [measure(N, case, vm, prefix) for N, case, vm, prefix in spec["fits"]]
+    elif "digests" in spec:
+        res = [digests(N, vm) for N, vm in spec["digests"]]
     else:
         res = pivots(spec["pivots"], spec["var_mode"])
     with open(out, "w") as f:
