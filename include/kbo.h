@@ -443,6 +443,42 @@ int kbo_forest_export(kbo_handle* h, kbo_forest* f, int32_t tree, int32_t* featu
                       void* stream);
 int kbo_forest_last_timings(kbo_handle* h, kbo_forest* f, float* ms, int32_t n);
 
+/* ---- ENAS controller (Katib algorithm `enas`: the macro-search LSTM controller of ENAS and its REINFORCE training; FP64
+ * restatement oracle/enas_oracle.py) -----------------------------------------------------------------------------------------
+ * Parameters, in this order in every flat buffer (FP32, row-major): w_lstm (2H × 4H; gates i, f, o, g), g_emb (H), w_emb
+ * (n_ops × H), w_soft (H × n_ops), w_attn_1 (H × H), w_attn_2 (H × H), v_attn (H).  An arc holds L(L+1)/2 decisions: per layer l,
+ * its op, then skip_0 .. skip_{l-1}.
+ *   kbo_enas_settings: temperature / tanh_const <= 0 mean None (the factor is skipped); entropy_weight and skip_weight are >= 0
+ *                   (None is 0); baseline_decay in [0, 1]; learning_rate in (0, 1]; skip_target in (0, 1).
+ *   kbo_enas_create: 1 <= L <= 64, 1 <= H <= 128, 1 <= n_ops <= 4096.  Parameters start U(-0.1, 0.1) (Philox4x32-10 keyed by
+ *                   seed, counter (element lo, hi, 2^32 - 1, 2^32 - 1)); moments, baseline, step and draw counter start at 0.
+ *   kbo_enas_train  : `steps` (0..10000) REINFORCE steps on a fixed reward in ONE launch: sample an arc (draw counter + step),
+ *                   forward, backward, TF Adam (β1 = 0, β2 = 0.999, ε̂ = 1e-3, lr_t = lr·sqrt(1 - β2^t), t over the controller's
+ *                   life).  arcs (device, steps × L(L+1)/2 int32, may be NULL): imposed arcs (teacher forcing).  stats (device,
+ *                   may be NULL): steps × 6 floats nll, ent, mean kl, loss, baseline, skip rate.  Advances the draw counter by
+ *                   `steps`.  Synchronises.
+ *   kbo_enas_sample : k (1..1024) arcs into arcs (device, k × L(L+1)/2 int32); decision d of arc a draws u = (word 0 >> 8)·2^-24
+ *                   of counter (draw counter lo, hi, a, d) unless uniforms (device, k × L(L+1)/2 floats) are imposed; a
+ *                   decision is the first bin whose prefix sum of exp(s - max) exceeds u·total.  Optional device outputs:
+ *                   op_probs (k × L × n_ops), skip_probs (k × L(L-1)/2, P(skip = 1)).  Advances the draw counter by 1.
+ *                   Synchronises.
+ *   kbo_enas_state  : HOST copies (any may be NULL) of the parameters, Adam moments m and v (flat, as above), baseline, Adam
+ *                   step count and draw counter.  Synchronises.
+ *   kbo_enas_set_params: HOST parameters, optional moments (NULL: zero), baseline and step; the draw counter is kept.
+ *   kbo_enas_last_timings: milliseconds of the last train and the last sample call, CUDA events on their streams.  Returns 2. */
+typedef struct kbo_enas_settings {
+  double temperature, tanh_const, entropy_weight, baseline_decay, learning_rate, skip_target, skip_weight;
+} kbo_enas_settings;
+typedef struct kbo_enas kbo_enas;
+int kbo_enas_create(kbo_handle* h, kbo_enas** out, int32_t L, int32_t H, int32_t n_ops, const kbo_enas_settings* settings, uint64_t seed);
+void kbo_enas_destroy(kbo_enas* e);
+int kbo_enas_train(kbo_handle* h, kbo_enas* e, double reward, int32_t steps, const int32_t* arcs, float* stats, void* stream);
+int kbo_enas_sample(kbo_handle* h, kbo_enas* e, int32_t k, int32_t* arcs, const float* uniforms, float* op_probs, float* skip_probs, void* stream);
+int kbo_enas_state(kbo_handle* h, kbo_enas* e, float* params, float* m, float* v, float* baseline, int64_t* step, int64_t* draws, void* stream);
+int kbo_enas_set_params(kbo_handle* h, kbo_enas* e, const float* params, const float* m, const float* v, float baseline, int64_t step,
+                        void* stream);
+int kbo_enas_last_timings(kbo_handle* h, kbo_enas* e, float* ms, int32_t n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -60,7 +60,15 @@ EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_se
            "kbo_mvtpe_create", "kbo_mvtpe_destroy", "kbo_mvtpe_tell", "kbo_mvtpe_ask", "kbo_mvtpe_state", "kbo_mvtpe_last_survivors",
            "kbo_mvtpe_last_timings",
            "kbo_forest_create", "kbo_forest_destroy", "kbo_forest_fit", "kbo_forest_sweep", "kbo_forest_predict", "kbo_forest_export",
-           "kbo_forest_last_timings"]
+           "kbo_forest_last_timings",
+           "kbo_enas_create", "kbo_enas_destroy", "kbo_enas_train", "kbo_enas_sample", "kbo_enas_state", "kbo_enas_set_params",
+           "kbo_enas_last_timings"]
+
+
+class KboEnasSettings(C.Structure):
+    _fields_ = [("temperature", C.c_double), ("tanh_const", C.c_double), ("entropy_weight", C.c_double), ("baseline_decay", C.c_double),
+                ("learning_rate", C.c_double), ("skip_target", C.c_double), ("skip_weight", C.c_double)]
+
 
 _lib = None
 
@@ -175,6 +183,14 @@ def load() -> C.CDLL:
     lib.kbo_forest_predict.argtypes = [vp, vp, vp, i32, C.c_int, vp, vp, vp]
     lib.kbo_forest_export.argtypes = [vp, vp, i32] + [vp] * 9 + [i32, vp, vp, vp]
     lib.kbo_forest_last_timings.argtypes = [vp, vp, vp, i32]
+    lib.kbo_enas_create.argtypes = [vp, C.POINTER(vp), i32, i32, i32, C.POINTER(KboEnasSettings), C.c_uint64]
+    lib.kbo_enas_destroy.argtypes = [vp]
+    lib.kbo_enas_destroy.restype = None
+    lib.kbo_enas_train.argtypes = [vp, vp, dbl, i32, vp, vp, vp]
+    lib.kbo_enas_sample.argtypes = [vp, vp, i32, vp, vp, vp, vp, vp]
+    lib.kbo_enas_state.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.kbo_enas_set_params.argtypes = [vp, vp, vp, vp, vp, C.c_float, i64, vp]
+    lib.kbo_enas_last_timings.argtypes = [vp, vp, vp, i32]
     lib.kbo_tc_variance_raw.argtypes = [vp, vp, vp, i64, vp, vp, i32, vp, dbl, vp, vp, i32, vp]
     for name in EXPORTS + ["kbo_tc_variance_raw", "kbo_debug_rank_pass", "kbo_debug_kstar", "kbo_debug_rank_rows", "kbo_debug_record_stages",
                            "kbo_debug_stage_count", "kbo_debug_stage", "kbo_debug_fp64_peak", "kbo_debug_dgemm_sm90"]:

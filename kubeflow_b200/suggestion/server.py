@@ -63,6 +63,7 @@ class SuggestionStub:
 
 def main():
     from .cmaes_service import CmaesService
+    from .enas_service import EnasService
     from .hyperband import HyperbandService
     from .mvtpe_service import MultivariateTpeService
     from .service import DispatchService, RandomService, SkoptService, SobolService
@@ -84,7 +85,8 @@ def main():
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
         inner = DispatchService([SkoptService({"device": local, "shard": True}), RandomService(), SobolService(),
-                                 CmaesService(), TpeService({"device": local}), MultivariateTpeService({"device": local}), HyperbandService()])
+                                 CmaesService(), TpeService({"device": local}), MultivariateTpeService({"device": local}), EnasService({"device": local}),
+                                 HyperbandService()])
         spmd = SpmdServicer(inner)
         if dist.get_rank() == 0:
             server, port = serve(spmd, args.port)
@@ -99,7 +101,7 @@ def main():
         return
     server, port = serve(DispatchService([SkoptService({"device": args.device}), RandomService(), SobolService(), CmaesService(),
                                          TpeService({"device": args.device}), MultivariateTpeService({"device": args.device}),
-                                         HyperbandService()]), args.port)
+                                         EnasService({"device": args.device}), HyperbandService()]), args.port)
     logging.info("api.v1.beta1.Suggestion listening on :%d", port)
     server.wait_for_termination()
 

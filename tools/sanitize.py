@@ -71,3 +71,8 @@ for _kind in ("RF", "ET"):
     print(fe.ask_multi(_r.random((5000, 5)), ["ei", "lcb", "pi"])[0], fe.predict(_r.random((3, 5)))[0].tolist(),
           len(fe.export(0, with_draws=_kind == "ET")["left"]))
     fe.close()
+from kubeflow_b200.enas import EnasController        # ENAS: init, the one-CTA train chain (drawn and imposed arcs), batched draws
+en = EnasController(5, 12, 9, seed=2)
+print(en.sample(6).tolist(), en.train(0.5, 3)[:, 0].tolist())
+print(en.train(0.7, 2, arcs=en.sample(2)).shape, en.sample(5, uniforms=_r.random((5, 15)), return_probs=True)[0].tolist())
+en.close()
