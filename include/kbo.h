@@ -103,21 +103,16 @@ const char* kbo_last_error(const kbo_handle* h);
 /* cap (bytes) on the per-sweep K* scratch; default 4 GiB.  Determines the candidate chunk size (rounded down to a
  * multiple of sm_count*128 rows so every launch is a whole number of waves). */
 int kbo_set_scratch_limit(kbo_handle* h, uint64_t bytes);
-/* tensor-core variance kernel variant: 1 (default) = 2-CTA cluster per 128-row panel with TMA multicast of the K* chunks,
- * 0 = one CTA per panel.  Same arithmetic, same results to the last bit per j-tile; the default halves the DRAM re-reads.
- * The environment variable KBO_TC_PAIR sets the initial value for new handles. */
-int kbo_set_tc_pair(kbo_handle* h, int enabled);
-/* Tensor-core mode only: re-evaluate on the FP64 path every candidate whose fp32 acquisition value is within 2e-4 of the
- * maximum (at most 4096 of them) and take the first-index argmax over those FP64 values, so the returned suggestion (index,
- * value, mu, std) has FP64 accuracy.  Default on; costs one extra pass over (mu, sigma²) and one stream synchronisation.
+/* Tensor-core mode re-evaluates on the FP64 path every candidate whose fp32 acquisition value is within 2e-4 of the maximum
+ * (at most 4096 of them) and takes the first-index argmax over those FP64 values, so the returned suggestion (index, value,
+ * mu, std) has FP64 accuracy; this costs one extra pass over (mu, sigma²) and one stream synchronisation.
  * kbo_last_contenders returns how many candidates the last sweep refined (> 4096: refinement skipped). */
-int kbo_set_tc_refine(kbo_handle* h, int enabled);
 int kbo_last_contenders(kbo_handle* h);
 /* Tensor-core sweeps that return only the suggestion (no mu/std/acq arrays) rank the grid with ONE fp16 product per term —
  * a third of the MMAs — and keep every candidate that could still be the maximum given that pass's error on sigma²
  * (calibrated per sweep against the three-product kernel on sm_count·64 rows stratified over the grid, x8 + 1e-6); the survivors are decided
  * by the FP64 refinement above, so the returned suggestion is unchanged.  More than 4096 survivors: the sweep is redone
- * with three products.  Default on; needs kbo_set_tc_refine and kbo_set_tc_pair on.  kbo_last_rank_error returns the
+ * with three products.  Default on.  kbo_last_rank_error returns the
  * largest |sigma²(1 product) - sigma²(3 products)| seen on the calibration rows of the last such sweep. */
 int kbo_set_tc_fast(kbo_handle* h, int enabled);
 double kbo_last_rank_error(kbo_handle* h);
@@ -126,7 +121,7 @@ double kbo_last_rank_error(kbo_handle* h);
  * kernel + single-CTA-MMA cluster kernel of round 1 for that pass.  Default 1 (needs D <= 128; wider spaces use the FP64
  * kernel).  Either way the calibration rows are STRATIFIED over the grid (row i*M/n) and go through the FP64 K* kernel and
  * the three-product contraction; kbo_last_rank_mu_error is the largest |mean(ranking) - mean(FP64)| seen on them, in
- * normalised-y units (0 with the FP64 K* kernel).  The environment variable KBO_RANK_TC sets the initial value. */
+ * normalised-y units (0 with the FP64 K* kernel). */
 int kbo_set_rank_tc(kbo_handle* h, int enabled);
 double kbo_last_rank_mu_error(kbo_handle* h);
 /* Pruning pass in front of the ranking pass (needs kbo_set_rank_tc).  sigma² = amp - sum_j v_j² with every term >= 0, so the sum
@@ -135,8 +130,7 @@ double kbo_last_rank_mu_error(kbo_handle* h);
  * of the MMAs.  The calibration rows' (near-exact) values give a lower bound on the maximum for free.  Candidates whose upper
  * bound stays below it are out; the rest (at most 16384, else the full ranking pass runs as before) get the full contraction,
  * the interval test and the FP64 decision.  tile_pairs: 512-trial tile pairs in the prefix; -1 (default) = an eighth of them,
- * 0 = no pruning pass.  kbo_last_prefix_survivors: how many candidates the last pruning pass kept (-1: it did not run).
- * The environment variable KBO_RANK_PREFIX sets the initial value. */
+ * 0 = no pruning pass.  kbo_last_prefix_survivors: how many candidates the last pruning pass kept (-1: it did not run). */
 int kbo_set_rank_prefix(kbo_handle* h, int tile_pairs);
 /* Lazy inverse (default on).  A tensor-core fit whose sweeps will prune forms only the rows of W = L^-1 the pruning pass reads
  * (the first 512·tile_pairs; plus the 256×256 diagonal blocks of every panel, which the look-ahead factorisation needs anyway):
@@ -149,7 +143,7 @@ int kbo_set_lazy_inverse(kbo_handle* h, int enabled);
 int kbo_last_prefix_survivors(kbo_handle* h);
 /* How the last tensor-core sweep decided its suggestion: 0 = FP64 evaluation of every candidate that could still be the
  * maximum; 1 = more such candidates than the cap (4096), FP64 decision among the best 4096 by fp32 value; 2 = not refined
- * (exact fp32 ties beyond the cap, or refinement switched off): the suggestion carries the mode's own accuracy. */
+ * (exact fp32 ties beyond the cap, or a grid of 2^31 or more rows): the suggestion carries the mode's own accuracy. */
 int kbo_last_unrefined(kbo_handle* h);
 
 /* ---- tell: GaussianProcessRegressor.fit at fixed θ ($SK/_gpr.py:275-280, 349-368) ---------------

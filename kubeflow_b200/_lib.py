@@ -49,7 +49,7 @@ class KboNotPositiveDefinite(KboError):
 
 
 # every symbol include/kbo.h declares (tests/test_abi.py checks the .so exports exactly these)
-EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_set_scratch_limit", "kbo_set_tc_pair", "kbo_set_tc_refine", "kbo_last_contenders", "kbo_set_tc_fast", "kbo_last_rank_error", "kbo_set_rank_tc", "kbo_last_rank_mu_error", "kbo_last_unrefined", "kbo_set_rank_prefix", "kbo_last_prefix_survivors", "kbo_set_lazy_inverse", "kbo_fit", "kbo_fit_append", "kbo_fit_room", "kbo_fit_rebase",
+EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_set_scratch_limit", "kbo_last_contenders", "kbo_set_tc_fast", "kbo_last_rank_error", "kbo_set_rank_tc", "kbo_last_rank_mu_error", "kbo_last_unrefined", "kbo_set_rank_prefix", "kbo_last_prefix_survivors", "kbo_set_lazy_inverse", "kbo_fit", "kbo_fit_append", "kbo_fit_room", "kbo_fit_rebase",
            "kbo_fit_info", "kbo_lml_grad", "kbo_lml_batch", "kbo_fit_state", "kbo_sweep", "kbo_sweep_multi", "kbo_last_decisions", "kbo_predict_mean", "kbo_best_to_host",
            "kbo_comm_unique_id", "kbo_comm_init", "kbo_comm_destroy", "kbo_comm_size", "kbo_allreduce_argmax", "kbo_suggest_host", "kbo_last_timings",
            "kbo_gram", "kbo_potrf", "kbo_trtri", "kbo_acq_argmax",
@@ -97,8 +97,6 @@ def load() -> C.CDLL:
     lib.kbo_last_error.argtypes = [vp]
     lib.kbo_last_error.restype = C.c_char_p
     lib.kbo_set_scratch_limit.argtypes = [vp, C.c_uint64]
-    lib.kbo_set_tc_pair.argtypes = [vp, C.c_int]
-    lib.kbo_set_tc_refine.argtypes = [vp, C.c_int]
     lib.kbo_fit_append.argtypes = [vp, vp, C.c_double, C.c_int, vp]
     lib.kbo_fit_room.argtypes = [vp]
     lib.kbo_req_open.argtypes = [vp, C.c_uint64, C.POINTER(vp)]

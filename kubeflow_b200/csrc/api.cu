@@ -1,7 +1,5 @@
 // extern "C" surface of libkbo.so (include/kbo.h).  No exceptions cross this boundary; every failure is a
 // negative kbo_status plus kbo_last_error() text.  There is no CPU path: without a device kbo_create fails.
-#include <stdlib.h>
-
 #include "kbo_internal.cuh"
 #include "dgemm_sm90.cuh"
 
@@ -24,10 +22,6 @@ int kbo_create(kbo_handle** out, int device) {
   if (!h) return KBO_ERR_NOMEM;
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
-  if (const char* e = getenv("KBO_TC_PAIR")) h->tc_pair = atoi(e) != 0;
-  if (const char* e = getenv("KBO_RANK_TC")) h->rank_tc = atoi(e) != 0;
-  if (const char* e = getenv("KBO_RANK_PREFIX")) h->rank_prefix = atoi(e);
-  if (const char* e = getenv("KBO_LAZY_W")) h->lazy_w = atoi(e) != 0;
   if (prop.major != 9) {
     // sm_90a cubin only: refuse politely instead of failing at the first launch
     h->err = "libkbo is built for sm_90a (H100) only";
@@ -74,12 +68,6 @@ int kbo_set_scratch_limit(kbo_handle* h, uint64_t bytes) {
   return KBO_OK;
 }
 
-int kbo_set_tc_refine(kbo_handle* h, int enabled) {
-  if (!h) return KBO_ERR_INVALID;
-  h->tc_refine = enabled != 0;
-  return KBO_OK;
-}
-
 int kbo_set_tc_fast(kbo_handle* h, int enabled) {
   if (!h) return KBO_ERR_INVALID;
   h->tc_fast = enabled != 0;
@@ -113,12 +101,6 @@ int kbo_set_rank_tc(kbo_handle* h, int enabled) {
 }
 
 int kbo_last_contenders(kbo_handle* h) { return h ? h->last_contenders : KBO_ERR_INVALID; }
-
-int kbo_set_tc_pair(kbo_handle* h, int enabled) {
-  if (!h) return KBO_ERR_INVALID;
-  h->tc_pair = enabled != 0;
-  return KBO_OK;
-}
 
 int kbo_fit(kbo_handle* h, const double* X, const double* y, int32_t N, int32_t D, const kbo_params* p, int x_on_host, void* stream) {
   if (!h) return KBO_ERR_INVALID;

@@ -1046,10 +1046,9 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
       // contracts with — the first 512·P1 — and leaves the rest to kbo_i_ensure_w, which runs if something asks for all of W.
       int lead = N;
       const bool planes = p->var_mode == KBO_VAR_TC_F16X3 || (p->var_mode == KBO_VAR_AUTO && N > 1024);
-      if (h->lazy_w && planes && h->rank_tc && h->rank_prefix != 0 && h->tc_fast && h->tc_refine && h->tc_pair && D <= 128) {
-        const int n_pairs = (h->Npad / 256 + 1) / 2;
-        const int P1 = h->rank_prefix < 0 ? (n_pairs + 7) / 8 : h->rank_prefix;
-        if (P1 >= 1 && P1 < n_pairs && P1 * 512 + 512 <= N) lead = round_up(P1 * 512, 512);
+      if (h->lazy_w && planes && h->rank_tc && h->rank_prefix != 0 && h->tc_fast && D <= 128) {
+        const int P1 = kbo_prefix_pairs(h);
+        if (P1 >= 1 && P1 < kbo_tile_pairs(h->Npad) && P1 * 512 + 512 <= N) lead = round_up(P1 * 512, 512);
       }
       KBO_TRY(factor_and_invert_v3(h, (double*)h->K.p, N, ld, (double*)h->W.p, ld, (int*)h->info.p, s, lead, early ? h->ev_gram : nullptr));
       h->w_lead = lead < N ? lead : N;

@@ -51,7 +51,6 @@ struct kbo_handle {
   DevBuf refine, refine_x;  // contender list / gathered rows of the FP64 refinement (tensor-core mode)
   int last_contenders = 0;
   float last_rank_err = 0.f;   // largest |σ²(1 product) − σ²(3 products)| over the calibration rows of the last fast sweep
-  bool tc_refine = true;
   bool tc_fast = true;      // array-free tensor-core sweeps rank with ONE fp16 product and let the FP64 refinement decide
   DevBuf var_cal;           // three-product variance of the calibration rows
   kbo_timings tim{};
@@ -60,8 +59,7 @@ struct kbo_handle {
   size_t ev_var_used = 0, ev_cross_used = 0, ev_acq_used = 0, ev_cal_used = 0;
   int launches = 0;
   bool time_kernels = false;
-  bool attr_fit = false, attr_tc = false;
-  int tc_pair = 1;  // variance kernel variant (kbo_set_tc_pair)  // cudaFuncSetAttribute done for this handle's device
+  bool attr_fit = false, attr_tc = false;   // cudaFuncSetAttribute done for this handle's device
   // ---- tensor-core K* generation (tc_kstar.cu) and wgmma ranking kernel (tc_rank.cu) ---------------------------
   bool rank_tc = true;        // kbo_set_rank_tc: the ranking pass builds K̃* on the tensor cores and contracts with wgmma MMAs
   bool ks_ready = false;      // trial-side operands below match the current fit
@@ -169,6 +167,10 @@ static inline int kbo_reserve(kbo_handle* h, DevBuf& b, size_t bytes) {
 
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 static inline int64_t round_up64(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
+// Pairs of 256-trial tiles the ranking pass contracts over, and the pairs the pruning pass takes by default (an eighth of them;
+// kbo_set_rank_prefix sets another count, 0 turns the pass off).  Callers check the range they need themselves.
+static inline int kbo_tile_pairs(int Npad) { return (Npad / 256 + 1) / 2; }
+static inline int kbo_prefix_pairs(const kbo_handle* h) { return h->rank_prefix < 0 ? (kbo_tile_pairs(h->Npad) + 7) / 8 : h->rank_prefix; }
 
 // ---- fit.cu ------------------------------------------------------------------------------------
 int kbo_i_gram(kbo_handle* h, const double* Xs, int N, int D, int kernel, double amp, double noise, double* K, int ldk,

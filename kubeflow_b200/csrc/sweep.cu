@@ -951,29 +951,39 @@ __device__ __forceinline__ float max_nan(float a, float b) { return (a != a || a
 
 // Calibration of the ranking pass on STRATIFIED rows: row i·M/n of the grid, i < n (n = one wave of the variance kernel, or all
 // rows of a small grid), so a sorted / clustered / blocked candidate order is sampled across its whole extent.  Those rows went
-// through the FP64 K* kernel and the three-product contraction (var3, mu3); v1 / mu1 are the ranking pass's values of the whole grid.
-// fs[0] = E (bound on |σ̃² − σ²|), fs[1] (as uint) = ordered bits of the best lower bound (reset here), fs[2] = raw max |dσ²|,
-// fs[3] = Eμ (bound on |μ̃ − μ|, normalised units), fs[4] = raw max |dμ|.
+// through the FP64 K* kernel and the three-product contraction (v_ex, mu_ex); v_rk / mu_rk are the ranking arithmetic's values,
+// of the whole grid (row idx[i] goes with calibration row i) or, idx = nullptr, of the calibration rows themselves.
+// fs[0] = E (bound on |σ̃² − σ²|), fs[1] (as uint) = ordered bits of the best lower bound, fs[2] = raw max |dσ²|,
+// fs[3] = Eμ (bound on |μ̃ − μ|, normalised units), fs[4] = raw max |dμ|.  acq < 0: the lower bound is reset below every ordered
+// value; otherwise it is the best value of that acquisition on the calibration rows, less their own error.
 __global__ void cal_index_kernel(int* __restrict__ list, int n, int64_t M) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) list[i] = (int)(((int64_t)i * M) / n);
 }
-__global__ void __launch_bounds__(1024) calib_kernel(const float* __restrict__ v1, const float* __restrict__ v3, const float* __restrict__ mu1,
-                                                     const float* __restrict__ mu3, const int* __restrict__ list, int n, float* __restrict__ fs) {
-  __shared__ float red[1024], redm[1024];
-  float m = 0.f, mm = 0.f;
+__global__ void __launch_bounds__(1024)
+calib_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_ex, const float* __restrict__ mu_rk, const float* __restrict__ mu_ex,
+             const int* __restrict__ idx, int n, int acq, const double* __restrict__ scal, double xi, double kappa, float* __restrict__ fs) {
+  __shared__ float red[1024], redm[1024], redl[1024];
+  const AcqFrame f = acq >= 0 ? acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa) : AcqFrame{};
+  float m = 0.f, mm = 0.f, lb = -INFINITY;
   for (int i = threadIdx.x; i < n; i += 1024) {
-    const int g = list[i];
-    m = max_nan(m, fabsf(v1[g] - v3[i]));
-    mm = max_nan(mm, fabsf(mu1[g] - mu3[i]));
+    const int g = idx ? idx[i] : i;
+    m = max_nan(m, fabsf(v_rk[g] - v_ex[i]));
+    mm = max_nan(mm, fabsf(mu_rk[g] - mu_ex[i]));
+    if (acq >= 0) {
+      const float a = acq_any_f32(acq, mu_ex[i], v_ex[i], f);   // three-product value: |error| ~ 1e-6
+      if (a > lb) lb = a;
+    }
   }
   red[threadIdx.x] = m;
   redm[threadIdx.x] = mm;
+  redl[threadIdx.x] = lb;
   __syncthreads();
   for (int o = 512; o > 0; o >>= 1) {
     if (threadIdx.x < o) {
       red[threadIdx.x] = max_nan(red[threadIdx.x], red[threadIdx.x + o]);
       redm[threadIdx.x] = max_nan(redm[threadIdx.x], redm[threadIdx.x + o]);
+      redl[threadIdx.x] = fmaxf(redl[threadIdx.x], redl[threadIdx.x + o]);
     }
     __syncthreads();
   }
@@ -982,7 +992,8 @@ __global__ void __launch_bounds__(1024) calib_kernel(const float* __restrict__ v
     fs[2] = red[0];
     fs[3] = 8.f * redm[0] + 1e-7f;
     fs[4] = redm[0];
-    ((unsigned*)fs)[1] = 0u;   // below every ordered value
+    const float l = redl[0] - 2e-5f * fmaxf(1.f, fabsf(redl[0]));   // the calibration values' own error, generously
+    ((unsigned*)fs)[1] = acq >= 0 && l > -INFINITY ? ordered_bits(l) : 0u;   // 0: below every ordered value
   }
 }
 // Bounds of the acquisition value over the box (μ ± Eμ) × (σ² ± E): all three kinds fall with μ; EI and LCB grow with σ, PI is
@@ -1004,6 +1015,8 @@ __device__ __forceinline__ void acq_bounds_f32(int acq, float mu, float var, flo
   // supremum (as in acq_prefix_ub_f32), or a saturated PI near a trial would be pruned below a maximum of 1
   if (acq == KBO_ACQ_PI && !(vlo > 0.f) && (f.chi - (mu - Em)) + f.clo > 0.f) *ub = 1.f;
 }
+// The interval test: the best lower bound over the M rows (the whole grid, or the pruning pass's survivors), then the rows whose
+// upper bound can still reach it — src[i] is row i's index in the grid (nullptr: i itself)
 __global__ void __launch_bounds__(256)
 bound_max_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int64_t M, int acq, const double* __restrict__ scal, double xi,
                  double kappa, float* __restrict__ fs) {
@@ -1020,8 +1033,8 @@ bound_max_kernel(const float* __restrict__ mun, const float* __restrict__ varn, 
   if ((threadIdx.x & 31) == 0 && best > -INFINITY) atomicMax((unsigned*)fs + 1, ordered_bits(best));
 }
 __global__ void __launch_bounds__(256)
-survivor_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int64_t M, int acq, const double* __restrict__ scal, double xi,
-                double kappa, const float* __restrict__ fs, int* __restrict__ list, int* __restrict__ count) {
+survivor_kernel(const float* __restrict__ mun, const float* __restrict__ varn, const int* __restrict__ src, int64_t M, int acq,
+                const double* __restrict__ scal, double xi, double kappa, const float* __restrict__ fs, int* __restrict__ list, int* __restrict__ count) {
   const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
   const float E = fs[0], Em = fs[3];
   const float lbmax = from_ordered_bits(((const unsigned*)fs)[1]);
@@ -1031,7 +1044,7 @@ survivor_kernel(const float* __restrict__ mun, const float* __restrict__ varn, i
     acq_bounds_f32(acq, mun[i], varn[i], E, Em, f, &lb, &ub);
     if (!(ub < thr)) {   // NaN survives
       const int slot = atomicAdd(count, 1);
-      if (slot < KBO_REFINE_CAP) list[slot] = (int)i;
+      if (slot < KBO_REFINE_CAP) list[slot] = src ? src[i] : (int)i;
     }
   }
 }
@@ -1045,39 +1058,6 @@ survivor_kernel(const float* __restrict__ mun, const float* __restrict__ varn, i
 // far more than by sigma) get the full contraction, the interval test of the ranking pass and the FP64 decision, exactly as
 // before.  A landscape too flat to prune this way falls back to the full ranking pass over the grid.
 //   fs[0] = E, fs[1] = ordered bits of the lower bound on the maximum, fs[2] = raw max |d sigma²|, fs[3] = Emu, fs[4] = raw max |d mu|
-__global__ void __launch_bounds__(1024)
-calib_lb_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_ex, const float* __restrict__ mu_rk, const float* __restrict__ mu_ex, int n,
-                int acq, const double* __restrict__ scal, double xi, double kappa, float* __restrict__ fs) {
-  __shared__ float red[1024], redm[1024], redl[1024];
-  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
-  float m = 0.f, mm = 0.f, lb = -INFINITY;
-  for (int i = threadIdx.x; i < n; i += 1024) {
-    m = max_nan(m, fabsf(v_rk[i] - v_ex[i]));
-    mm = max_nan(mm, fabsf(mu_rk[i] - mu_ex[i]));
-    const float a = acq_any_f32(acq, mu_ex[i], v_ex[i], f);   // three-product value: |error| ~ 1e-6
-    if (a > lb) lb = a;
-  }
-  red[threadIdx.x] = m;
-  redm[threadIdx.x] = mm;
-  redl[threadIdx.x] = lb;
-  __syncthreads();
-  for (int o = 512; o > 0; o >>= 1) {
-    if (threadIdx.x < o) {
-      red[threadIdx.x] = max_nan(red[threadIdx.x], red[threadIdx.x + o]);
-      redm[threadIdx.x] = max_nan(redm[threadIdx.x], redm[threadIdx.x + o]);
-      redl[threadIdx.x] = fmaxf(redl[threadIdx.x], redl[threadIdx.x + o]);
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    fs[0] = 8.f * red[0] + 1e-6f;
-    fs[2] = red[0];
-    fs[3] = 8.f * redm[0] + 1e-7f;
-    fs[4] = redm[0];
-    const float l = redl[0] - 2e-5f * fmaxf(1.f, fabsf(redl[0]));   // the calibration values' own error, generously
-    ((unsigned*)fs)[1] = l > -INFINITY ? ordered_bits(l) : 0u;
-  }
-}
 // supremum of the acquisition value over mu in [mu ± Em], sigma² in (0, var_ub]
 __device__ __forceinline__ float acq_prefix_ub_f32(int acq, float mu, float var_ub, float Em, const AcqFrame& f) {
   if (!(mu == mu && var_ub == var_ub && Em == Em)) return __int_as_float(0x7fc00000);   // NaN: survives
@@ -1100,38 +1080,6 @@ prefix_survivor_kernel(const float* __restrict__ mun, const float* __restrict__ 
     if (!(ub < thr)) {   // NaN survives
       const int slot = atomicAdd(count, 1);
       if (slot < cap) list[slot] = (int)i;
-    }
-  }
-}
-// interval test among the n prefix survivors (contiguous ranking-pass values): best lower bound, then who can still reach it
-__global__ void __launch_bounds__(256)
-survivor_lb_kernel(const float* __restrict__ mun, const float* __restrict__ varn, int n, int acq, const double* __restrict__ scal, double xi, double kappa,
-                   float* __restrict__ fs) {
-  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
-  const float E = fs[0], Em = fs[3];
-  float best = -INFINITY;
-  for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
-    float lb, ub;
-    acq_bounds_f32(acq, mun[i], varn[i], E, Em, f, &lb, &ub);
-    if (lb > best) best = lb;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, o));
-  if ((threadIdx.x & 31) == 0 && best > -INFINITY) atomicMax((unsigned*)fs + 1, ordered_bits(best));
-}
-__global__ void __launch_bounds__(256)
-survivor_final_kernel(const float* __restrict__ mun, const float* __restrict__ varn, const int* __restrict__ src, int n, int acq,
-                      const double* __restrict__ scal, double xi, double kappa, const float* __restrict__ fs, int* __restrict__ list, int* __restrict__ count) {
-  const AcqFrame f = acq_frame(scal[S_YMEAN], scal[S_YSTD], scal[S_YOPT], xi, kappa);
-  const float E = fs[0], Em = fs[3];
-  const float lbmax = from_ordered_bits(((const unsigned*)fs)[1]);
-  const float thr = lbmax - 1e-5f * fmaxf(1.f, fabsf(lbmax));
-  for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
-    float lb, ub;
-    acq_bounds_f32(acq, mun[i], varn[i], E, Em, f, &lb, &ub);
-    if (!(ub < thr)) {
-      const int slot = atomicAdd(count, 1);
-      if (slot < KBO_REFINE_CAP) list[slot] = src[i];
     }
   }
 }
@@ -1164,36 +1112,43 @@ grid_lower_bound_kernel(const float* __restrict__ mun, const float* __restrict__
   for (int o = 16; o > 0; o >>= 1) best = fmaxf(best, __shfl_xor_sync(0xffffffffu, best, o));
   if ((threadIdx.x & 31) == 0 && best > -INFINITY) atomicMax((unsigned*)fs + 1, ordered_bits(best - 1e-5f * fmaxf(1.f, fabsf(best))));
 }
-// E, Emu from the calibration rows (ranking arithmetic vs exact, both over the same prefix of the trial tiles); lower bound reset
-__global__ void __launch_bounds__(1024)
-calib_prefix_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_ex, const float* __restrict__ mu_rk, const float* __restrict__ mu_ex, int n,
-                    float* __restrict__ fs) {
-  __shared__ float red[1024], redm[1024];
-  float m = 0.f, mm = 0.f;
-  for (int i = threadIdx.x; i < n; i += 1024) {
-    m = max_nan(m, fabsf(v_rk[i] - v_ex[i]));
-    mm = max_nan(mm, fabsf(mu_rk[i] - mu_ex[i]));
-  }
-  red[threadIdx.x] = m;
-  redm[threadIdx.x] = mm;
-  __syncthreads();
-  for (int o = 512; o > 0; o >>= 1) {
-    if (threadIdx.x < o) {
-      red[threadIdx.x] = max_nan(red[threadIdx.x], red[threadIdx.x + o]);
-      redm[threadIdx.x] = max_nan(redm[threadIdx.x], redm[threadIdx.x + o]);
-    }
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) {
-    fs[0] = 8.f * red[0] + 1e-6f;
-    fs[2] = red[0];
-    fs[3] = 8.f * redm[0] + 1e-7f;
-    fs[4] = redm[0];
-    ((unsigned*)fs)[1] = 0u;
-  }
-}
 
 #define KBO_PRUNE_CAP 16384
+// The grid pass of the pruning sweeps: per chunk, the mean over all trials and the variance bound from the first P1 tile pairs
+// (only their 512·P1 columns of K̃* are stored).
+static int prefix_grid_pass(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t chunk, int P1, cudaStream_t s) {
+  const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
+  for (int64_t c0 = 0; c0 < M; c0 += chunk) {
+    const int64_t rows = (M - c0 < chunk) ? (M - c0) : chunk;
+    const unsigned char* xc = (const unsigned char*)Xc + (size_t)c0 * h->D * esz;
+    h->tim.chunks++;
+    {
+      KBO_TIME_BEGIN(ev_cross, ev_cross_used);
+      KBO_TRY(kbo_i_tc_kstar(h, xc, xc_dtype, rows, (__half*)h->Ksh.p, (float*)h->mun.p + c0, s, P1 * 512));
+      KBO_TIME_END();
+    }
+    {
+      KBO_TIME_BEGIN(ev_var, ev_var_used);
+      KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, round_up64(rows, 256), (const __half*)h->Wh.p, h->Npad, h->prm.amplitude,
+                            (float*)h->varn.p + c0, s, 0, P1));
+      KBO_TIME_END();
+    }
+  }
+  return KBO_OK;
+}
+
+// Reads back the survivor count at `count` (into *n, if given) together with the bounds that follow it (fs = count + 4) and
+// reports the raw calibration maxima (kbo_last_rank_error, kbo_last_rank_mu_error).
+static int read_bounds(kbo_handle* h, const int* count, int* n, cudaStream_t s) {
+  struct { int n; int pad[3]; float fs[8]; } host;
+  KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (n) *n = host.n;
+  h->last_rank_err = host.fs[2];
+  h->last_rank_mu_err = host.fs[4];
+  return KBO_OK;
+}
+
 // The pruning sweep of a LAZY fit (only the leading rows of W exist): everything it touches is the factor L, alpha, and the
 // leading block of W.  Calibration: exact mean (FP64 K* kernel) and exact PREFIX variance (three products over the prefix's
 // tiles) against the ranking arithmetic over the same prefix -> E, Emu.  Lower bound on the maximum: the sigma -> 0 limit of
@@ -1204,13 +1159,10 @@ calib_prefix_kernel(const float* __restrict__ v_rk, const float* __restrict__ v_
 // The grid pass is shared by every acquisition in dec[]; the bound, the survivor list and the FP64 decision are per kind.
 static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int64_t chunk, AcqDecision* dec, int n_acq,
                             cudaStream_t s) {
-  const int D = h->D, Npad = h->Npad;
-  const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
+  const int Npad = h->Npad;
   const double* scal = (const double*)h->scal.p;
-  const int n_pairs = (Npad / 256 + 1) / 2;
-  int P1 = h->rank_prefix < 0 ? (n_pairs + 7) / 8 : h->rank_prefix;
-  if (P1 < 1 || P1 >= n_pairs || P1 * 512 > h->w_lead) return KBO_OK;
-  const int prefix_cols = P1 * 512;
+  const int P1 = kbo_prefix_pairs(h);
+  if (P1 < 1 || P1 >= kbo_tile_pairs(Npad) || P1 * 512 > h->w_lead) return KBO_OK;
   KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
   int* count = (int*)h->refine.p + KBO_REFINE_CAP;
   float* fs = (float*)(count + 4);
@@ -1224,29 +1176,14 @@ static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
     const int64_t cal_pad = round_up64(cal_n, 256);
     KBO_TRY(kbo_reserve(h, h->cal_mu_rk, sizeof(float) * (size_t)(cal_pad + 256)));
     KBO_TRY(kbo_reserve(h, h->cal_var_rk, sizeof(float) * (size_t)(cal_pad + 256)));
-    KBO_TRY(kbo_i_tc_kstar(h, h->cal_x.p, KBO_F64, cal_n, (__half*)h->Ksh.p, (float*)h->cal_mu_rk.p, s, prefix_cols));
+    KBO_TRY(kbo_i_tc_kstar(h, h->cal_x.p, KBO_F64, cal_n, (__half*)h->Ksh.p, (float*)h->cal_mu_rk.p, s, P1 * 512));
     KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, cal_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->cal_var_rk.p, s, 0, P1));
-    calib_prefix_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p,
-                                           cal_n, fs);
+    calib_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p,
+                                    nullptr, cal_n, -1, nullptr, 0.0, 0.0, fs);
     KBO_LAUNCH_CHECK(h);
     KBO_TIME_END();
   }
-  for (int64_t c0 = 0; c0 < M; c0 += chunk) {
-    const int64_t rows = (M - c0 < chunk) ? (M - c0) : chunk;
-    const unsigned char* xc = (const unsigned char*)Xc + (size_t)c0 * D * esz;
-    h->tim.chunks++;
-    {
-      KBO_TIME_BEGIN(ev_cross, ev_cross_used);
-      KBO_TRY(kbo_i_tc_kstar(h, xc, xc_dtype, rows, (__half*)h->Ksh.p, (float*)h->mun.p + c0, s, prefix_cols));
-      KBO_TIME_END();
-    }
-    {
-      KBO_TIME_BEGIN(ev_var, ev_var_used);
-      KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, round_up64(rows, 256), (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->varn.p + c0, s, 0,
-                            P1));
-      KBO_TIME_END();
-    }
-  }
+  KBO_TRY(prefix_grid_pass(h, Xc, xc_dtype, M, chunk, P1, s));
   KBO_TIME_BEGIN(ev_acq, ev_acq_used);
   StagePicks sp;
   for (int k = 0; k < n_acq; k++) {
@@ -1259,14 +1196,10 @@ static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
     prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
                                                          pcount, KBO_PRUNE_CAP);
     KBO_LAUNCH_CHECK(h);
-    struct { int n; int pad[3]; float fs[8]; } host;
     int n1 = 0;
     KBO_CUDA(h, cudaMemcpyAsync(&n1, pcount, sizeof(int), cudaMemcpyDeviceToHost, s));
-    KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
-    KBO_CUDA(h, cudaStreamSynchronize(s));
+    KBO_TRY(read_bounds(h, count, nullptr, s));
     d.prefix_survivors = n1;
-    h->last_rank_err = host.fs[2];
-    h->last_rank_mu_err = host.fs[4];
     KBO_TRY(record_stage(h, KBO_STAGE_LAZY_PRUNE, d.acq, cal_n, fs, pcount, plist, KBO_PRUNE_CAP, NAN, s));
     if (n1 < 1 || n1 > KBO_SOLVE_CAP) continue;
     d.contenders = n1;
@@ -1285,12 +1218,10 @@ static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
 static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int cal_n, int64_t chunk, AcqDecision* dec, int n_acq,
                        cudaStream_t s) {
   const int D = h->D, Npad = h->Npad;
-  const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
   const double* scal = (const double*)h->scal.p;
-  const int n_pairs = (Npad / 256 + 1) / 2;
-  int P1 = h->rank_prefix < 0 ? (n_pairs + 7) / 8 : h->rank_prefix;
+  int P1 = kbo_prefix_pairs(h);
   if (P1 < 1) P1 = 1;
-  if (P1 >= n_pairs) return KBO_OK;   // nothing to save: the caller's full pass is the prefix
+  if (P1 >= kbo_tile_pairs(Npad)) return KBO_OK;   // nothing to save: the caller's full pass is the prefix
   KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
   int* list = (int*)h->refine.p;
   int* count = list + KBO_REFINE_CAP;
@@ -1309,44 +1240,24 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     KBO_TIME_END();
   }
   // pass 1 over the grid: mean over all trials, variance bound from the first P1 tile pairs
-  const int prefix_cols = P1 * 512 < Npad ? P1 * 512 : Npad;
-  for (int64_t c0 = 0; c0 < M; c0 += chunk) {
-    const int64_t rows = (M - c0 < chunk) ? (M - c0) : chunk;
-    const unsigned char* xc = (const unsigned char*)Xc + (size_t)c0 * D * esz;
-    h->tim.chunks++;
-    {
-      KBO_TIME_BEGIN(ev_cross, ev_cross_used);
-      KBO_TRY(kbo_i_tc_kstar(h, xc, xc_dtype, rows, (__half*)h->Ksh.p, (float*)h->mun.p + c0, s, prefix_cols));
-      KBO_TIME_END();
-    }
-    {
-      KBO_TIME_BEGIN(ev_var, ev_var_used);
-      KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, round_up64(rows, 256), (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->varn.p + c0, s, 0,
-                            P1));
-      KBO_TIME_END();
-    }
-  }
+  KBO_TRY(prefix_grid_pass(h, Xc, xc_dtype, M, chunk, P1, s));
   KBO_TIME_BEGIN(ev_acq, ev_acq_used);
   StagePicks sp;
   for (int k = 0; k < n_acq; k++) {
     AcqDecision& d = dec[k];
     if (d.done) continue;
     // E, Emu and this kind's lower bound on the maximum from the calibration rows (one CTA over one wave of rows)
-    calib_lb_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p, cal_n,
-                                       d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+    calib_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p,
+                                    nullptr, cal_n, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
     KBO_LAUNCH_CHECK(h);
     KBO_CUDA(h, cudaMemsetAsync(pcount, 0, sizeof(int), s));
     prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
                                                          pcount, KBO_PRUNE_CAP);
     KBO_LAUNCH_CHECK(h);
-    struct { int n; int pad[3]; float fs[8]; } host;
     int n1 = 0;
     KBO_CUDA(h, cudaMemcpyAsync(&n1, pcount, sizeof(int), cudaMemcpyDeviceToHost, s));
-    KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
-    KBO_CUDA(h, cudaStreamSynchronize(s));
+    KBO_TRY(read_bounds(h, count, nullptr, s));
     d.prefix_survivors = n1;
-    h->last_rank_err = host.fs[2];
-    h->last_rank_mu_err = host.fs[4];
     KBO_TRY(record_stage(h, KBO_STAGE_PRUNE, d.acq, cal_n, fs, pcount, plist, KBO_PRUNE_CAP, NAN, s));
     if (n1 < 1 || n1 > KBO_PRUNE_CAP) continue;
     // pass 2: the survivors' rows through the whole ranking pass, then the interval test and the FP64 decision
@@ -1363,10 +1274,10 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, n1_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->pr_var.p, s));
     KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
     const int g2 = (n1 + 255) / 256;
-    survivor_lb_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+    bound_max_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
     KBO_LAUNCH_CHECK(h);
-    survivor_final_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, plist, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs, list,
-                                             count);
+    survivor_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, plist, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs, list,
+                                       count);
     KBO_LAUNCH_CHECK(h);
     int n2 = 0;
     KBO_CUDA(h, cudaMemcpyAsync(&n2, count, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -1392,23 +1303,20 @@ static int fast_pick(kbo_handle* h, int64_t M, int cal_n, AcqDecision& d, StageP
   float* fs = (float*)(count + 4);
   KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
   calib_kernel<<<1, 1024, 0, s>>>((const float*)h->varn.p, (const float*)h->var_cal.p, (const float*)h->mun.p, (const float*)h->cal_mu.p,
-                                  (const int*)h->cal_idx.p, cal_n, fs);
+                                  (const int*)h->cal_idx.p, cal_n, -1, nullptr, 0.0, 0.0, fs);
   KBO_LAUNCH_CHECK(h);
   bound_max_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
   KBO_LAUNCH_CHECK(h);
-  survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs,
+  survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, nullptr, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs,
                                                  list, count);
   KBO_LAUNCH_CHECK(h);
-  struct { int n; int pad[3]; float fs[8]; } host;
-  KBO_CUDA(h, cudaMemcpyAsync(&host, count, sizeof host, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));
-  d.contenders = host.n;
-  h->last_rank_err = host.fs[2];
-  h->last_rank_mu_err = host.fs[4];
+  int n = 0;
+  KBO_TRY(read_bounds(h, count, &n, s));
+  d.contenders = n;
   KBO_TRY(record_stage(h, KBO_STAGE_INTERVAL, d.acq, cal_n, fs, count, list, KBO_REFINE_CAP, NAN, s));
-  if (host.n < 1 || host.n > KBO_REFINE_CAP) return KBO_OK;
+  if (n < 1 || n > KBO_REFINE_CAP) return KBO_OK;
   d.unrefined = 0;
-  return take_list(h, sp, d, list, host.n, s);
+  return take_list(h, sp, d, list, n, s);
 }
 
 // The stratified calibration rows of a ranking sweep through the FP64 K* kernel and the three-product contraction:
@@ -1457,7 +1365,7 @@ int kbo_i_debug_cross_planes(kbo_handle* h, const void* Xc, int xc_dtype, int64_
 int kbo_i_debug_rank_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int tile_pairs, float* mun_out, float* varn_out, cudaStream_t s) {
   if (!h->fitted || !h->have_planes || !h->ks_ready)
     KBO_FAIL(h, KBO_ERR_STATE, "kbo_debug_rank_rows: needs a fit with tensor-core planes and K* operands (D <= 128)");
-  const int Npad = h->Npad, n_pairs = (Npad / 256 + 1) / 2;
+  const int Npad = h->Npad, n_pairs = kbo_tile_pairs(Npad);
   if (tile_pairs == 0) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_rank_rows: tile_pairs must be >= 1 or < 0");
   const int P1 = (tile_pairs < 0 || tile_pairs > n_pairs) ? n_pairs : tile_pairs;
   if (!h->w_full && (P1 == n_pairs || P1 * 512 > h->w_lead)) KBO_TRY(kbo_i_ensure_w(h, s));
@@ -1535,7 +1443,7 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
   const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
   const double* scal = (const double*)h->scal.p;
   // array-free tensor-core sweeps rank with one fp16 product and let the FP64 refinement decide (fast_pick above)
-  const bool fast = tc && !force_three && h->tc_fast && h->tc_refine && h->tc_pair && !mu_out && !std_out && !acq_out && M < 0x7fffffff;
+  const bool fast = tc && !force_three && h->tc_fast && !mu_out && !std_out && !acq_out && M < 0x7fffffff;
   // ... and, by default, build that pass's K̃* on the tensor cores and contract it with wgmma MMAs (tc_kstar.cu, tc_rank.cu)
   const bool rank_tc = fast && h->rank_tc && h->ks_ready;
   int cal_n = 0;
@@ -1679,7 +1587,7 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
         KBO_TRY(launch_acq<float>(h, (const float*)h->mun.p, (const float*)h->varn.p, M, goff, d.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
                                   h->prm.kappa, mu_out, std_out, acq_out, nullptr, d.best, s));
         d.unrefined = 2;
-        if (h->tc_refine && M < 0x7fffffff)
+        if (M < 0x7fffffff)
           KBO_TRY(refine_suggestion(h, M, goff, d, sp, s));
         else
           d.done = true;

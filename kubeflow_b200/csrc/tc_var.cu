@@ -7,8 +7,7 @@
 // fp32 accumulator: bf16/fp16 single-pass moves σ² by 1e-2 and bf16×3 by 1e-5..1e-4 (DESIGN.md §numerics) — fp16×3
 // stays at ~3e-7.
 //
-// One kernel template, two launch shapes: tc_variance_kernel<false> (one CTA per 128-row panel, all j-tiles) and the default
-// tc_variance_kernel<true> (a 2-CTA cluster per panel, j-tiles split by parity, K* chunks TMA-multicast to both CTAs).
+// A 2-CTA cluster per 128-row panel, j-tiles split by parity, K* chunks TMA-multicast to both CTAs.
 // CTA = 128 candidate rows × its j-tiles of 128 trial columns, walked in order; for j-tile t only k < 128(t+1) is issued (W is
 // lower triangular).  K is consumed in 32-wide chunks through a 6-stage TMA→smem ring:
 //   warps 0-7  two consumer warpgroups (rows 64·wg …): wgmma m64n128k16 into 64 fp32 registers per thread.  Every `k_span`
@@ -41,29 +40,25 @@ struct TcSmem {
   uint64_t empty[TC_STAGES];
 };
 
-// PAIR: the cluster variant.  The j-tiles are split by parity (CTA r owns tiles 2p + r) and both CTAs walk the K chunks of a
-// tile pair in lockstep, so every A (K*) chunk is fetched ONCE and TMA-multicast into both CTAs' shared memory (each CTA
-// issues the load for its 64-row half with ctaMask = 0b11); B (W) chunks stay private.  That halves the K* panel re-reads.
+// The j-tiles are split by parity (CTA r owns tiles 2p + r) and both CTAs walk the K chunks of a tile pair in lockstep, so
+// every A (K*) chunk is fetched ONCE and TMA-multicast into both CTAs' shared memory (each CTA issues the load for its 64-row
+// half with ctaMask = 0b11); B (W) chunks stay private.  That halves the K* panel re-reads.
 //   full[st]  (per CTA): 1 arrival (own producer's expect_tx) + A bytes from both multicast halves + own B bytes
 //   empty[st] (per CTA): one arrival per consumer warpgroup of BOTH CTAs, so a stage is refilled only when both CTAs are done
-// Per-row Σv² of the two CTAs' tile sets goes to part[rank][row]; tc_pair_finish_kernel adds them in a fixed order.
-// nprod 3: Al·Bh + Ah·Bl + Ah·Bh; 1: Ah·Bh only (ranking pass, lo planes never loaded; cluster variant only).
-template <bool PAIR>
+// Per-row Σv² of the two CTAs' tile sets goes to part[rank][row]; tc_variance_finish_kernel adds them in a fixed order.
+// nprod 3: Al·Bh + Ah·Bl + Ah·Bh; 1: Ah·Bh only (ranking pass, lo planes never loaded).
 __global__ void __launch_bounds__(TC_THREADS, 1)
 tc_variance_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
                    const __grid_constant__ CUtensorMap tmBh, const __grid_constant__ CUtensorMap tmBl, int n_jtiles,
-                   int span_chunks, int nprod, const double* __restrict__ w_scale /* [0]=2^s, [1]=2^-s */, double amp,
-                   float* __restrict__ var_out, double* __restrict__ sumsq_out /* optional raw Σv² (tests) */,
-                   double* __restrict__ part /* PAIR: [2][rows] raw Σv² (scaled units) */, int64_t rows) {
+                   int span_chunks, int nprod, double* __restrict__ part /* [2][rows] raw Σv² (scaled units) */, int64_t rows) {
   extern __shared__ unsigned char tc_smem_raw[];
   // SWIZZLE_64B tiles need 512 B alignment of each plane; keep the whole ring 1024 B aligned.
   unsigned char* ring = (unsigned char*)(((uintptr_t)tc_smem_raw + 1023) & ~(uintptr_t)1023);
   TcSmem* S = (TcSmem*)(ring + TC_STAGES * TC_STAGE_BYTES);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0;
-  const int m0 = (PAIR ? (blockIdx.x >> 1) : blockIdx.x) * TC_BM;
-  constexpr int STRIDE = PAIR ? 2 : 1;
-  const int n_groups = (n_jtiles + STRIDE - 1) / STRIDE;
+  const uint32_t rank = cluster_ctarank();
+  const int m0 = (blockIdx.x >> 1) * TC_BM;
+  const int n_groups = (n_jtiles + 1) / 2;
   const uint32_t planes = nprod == 3 ? 2u : 1u;
 
   if (threadIdx.x == TC_CONSUMERS) {
@@ -73,39 +68,31 @@ tc_variance_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     prefetch_tmap(&tmBl);
     for (int i = 0; i < TC_STAGES; i++) {
       mbar_init(smem_u32(&S->full[i]), 1);
-      mbar_init(smem_u32(&S->empty[i]), 2 * STRIDE);
+      mbar_init(smem_u32(&S->empty[i]), 4);   // two consumer warpgroups in each of the two CTAs
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (PAIR) cluster_sync_all();  // the peer's barriers exist before anything is multicast into them
+  cluster_sync_all();  // the peer's barriers exist before anything is multicast into them
 
   if (warp == TC_CONSUMERS / 32) {
     // ===================================== TMA producer ===========================================
     if (lane == 0) {
       uint32_t c = 0;
       for (int p = 0; p < n_groups; p++) {
-        const int my_tile = STRIDE * p + (int)rank;
+        const int my_tile = 2 * p + (int)rank;
         const int my_nch = my_tile < n_jtiles ? (my_tile + 1) * TC_CPT : 0;
-        const int nch = PAIR ? min(2 * p + 2, n_jtiles) * TC_CPT : my_nch;  // a pair streams the longer of its two K ranges
+        const int nch = min(2 * p + 2, n_jtiles) * TC_CPT;  // a pair streams the longer of its two K ranges
         for (int ch = 0; ch < nch; ch++, c++) {
           const uint32_t st = c % TC_STAGES, use = c / TC_STAGES;
-          if (PAIR)
-            mbar_wait_cluster(smem_u32(&S->empty[st]), (use & 1) ^ 1);
-          else
-            mbar_wait(smem_u32(&S->empty[st]), (use & 1) ^ 1);
+          mbar_wait_cluster(smem_u32(&S->empty[st]), (use & 1) ^ 1);
           const uint32_t bar = smem_u32(&S->full[st]);
           mbar_expect_tx(bar, planes * TC_A_BYTES + (ch < my_nch ? planes * TC_B_BYTES : 0));
           const uint32_t base = smem_u32(ring + st * TC_STAGE_BYTES);
           const int k0 = ch * TC_BK;
-          if (PAIR) {
-            const uint32_t half_off = rank * (TC_A_BYTES / 2);  // rows 64·rank … of the 128-row A tile
-            tma_load_2d_mc(base + half_off, &tmAh, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
-            if (nprod == 3) tma_load_2d_mc(base + TC_A_BYTES + half_off, &tmAl, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
-          } else {
-            tma_load_2d(base, &tmAh, bar, k0, m0);
-            if (nprod == 3) tma_load_2d(base + TC_A_BYTES, &tmAl, bar, k0, m0);
-          }
+          const uint32_t half_off = rank * (TC_A_BYTES / 2);  // rows 64·rank … of the 128-row A tile
+          tma_load_2d_mc(base + half_off, &tmAh, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
+          if (nprod == 3) tma_load_2d_mc(base + TC_A_BYTES + half_off, &tmAl, bar, k0, m0 + 64 * (int)rank, (uint16_t)3);
           if (ch < my_nch) {
             tma_load_2d(base + 2 * TC_A_BYTES, &tmBh, bar, k0, my_tile * TC_BN);
             if (nprod == 3) tma_load_2d(base + 2 * TC_A_BYTES + TC_B_BYTES, &tmBl, bar, k0, my_tile * TC_BN);
@@ -122,7 +109,7 @@ tc_variance_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     auto release = [&](uint32_t st) {
       if (!signal) return;
       mbar_arrive(smem_u32(&S->empty[st]));
-      if (PAIR) mbar_arrive_remote(smem_u32(&S->empty[st]), rank ^ 1u);
+      mbar_arrive_remote(smem_u32(&S->empty[st]), rank ^ 1u);
     };
     float acc[64], sum[64];
 #pragma unroll
@@ -130,9 +117,9 @@ tc_variance_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     double rowacc0 = 0.0, rowacc1 = 0.0;
     uint32_t c = 0;
     for (int p = 0; p < n_groups; p++) {
-      const int my_tile = STRIDE * p + (int)rank;
+      const int my_tile = 2 * p + (int)rank;
       const int my_nch = my_tile < n_jtiles ? (my_tile + 1) * TC_CPT : 0;
-      const int nch = PAIR ? min(2 * p + 2, n_jtiles) * TC_CPT : my_nch;
+      const int nch = min(2 * p + 2, n_jtiles) * TC_CPT;
       for (int ch0 = 0; ch0 < nch; ch0 += span_chunks) {
         const int che = min(nch, ch0 + span_chunks);
         int pending = -1;   // stage whose MMAs are committed but not yet known complete
@@ -196,26 +183,15 @@ tc_variance_kernel(const __grid_constant__ CUtensorMap tmAh, const __grid_consta
     rowacc0 += __shfl_xor_sync(0xffffffffu, rowacc0, 2);
     rowacc1 += __shfl_xor_sync(0xffffffffu, rowacc1, 2);
     if ((lane & 3) == 0) {
-      if (PAIR) {
-        part[(size_t)rank * rows + m0 + row0] = rowacc0;
-        part[(size_t)rank * rows + m0 + row0 + 8] = rowacc1;
-      } else {
-        const double sc = w_scale[1];
-        const double t0 = rowacc0 * sc * sc, t1 = rowacc1 * sc * sc;
-        var_out[m0 + row0] = (float)(amp - t0);
-        var_out[m0 + row0 + 8] = (float)(amp - t1);
-        if (sumsq_out) {
-          sumsq_out[m0 + row0] = t0;
-          sumsq_out[m0 + row0 + 8] = t1;
-        }
-      }
+      part[(size_t)rank * rows + m0 + row0] = rowacc0;
+      part[(size_t)rank * rows + m0 + row0 + 8] = rowacc1;
     }
   }
 
-  if (PAIR) cluster_sync_all();  // no CTA leaves while its peer may still multicast into it or arrive on its barriers
+  cluster_sync_all();  // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
-__global__ void tc_pair_finish_kernel(const double* __restrict__ part, int64_t rows, const double* __restrict__ w_scale, double amp,
+__global__ void tc_variance_finish_kernel(const double* __restrict__ part, int64_t rows, const double* __restrict__ w_scale, double amp,
                                       float* __restrict__ var_out, double* __restrict__ sumsq_out) {
   const int64_t m = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (m >= rows) return;
@@ -233,7 +209,6 @@ int tc_launch(kbo_handle* h, const __half* Ksh, const __half* Ksl, int64_t rows,
               const double* w_scale_dev, double amp, float* var_out, double* sumsq_out, int k_span, cudaStream_t s, int nprod = 3, int jtiles = -1) {
   // a prefix of the trial tiles (`jtiles` counts 256-column tiles): an upper bound on the variance
   const int n_jt = (jtiles > 0 && 2 * jtiles < Npad / TC_BN) ? 2 * jtiles : Npad / TC_BN;
-  if (nprod != 3 && !h->tc_pair) KBO_FAIL(h, KBO_ERR_STATE, "tc_variance: the one-product ranking pass needs the cluster kernel (kbo_set_tc_pair)");
   if (rows % TC_BM != 0 || Npad % 256 != 0) KBO_FAIL(h, KBO_ERR_INVALID, "tc_variance: rows %% 128 and Npad %% 256 must be 0");
   // Long tensor-core accumulation chains lose low-order bits; adding the accumulator into fp32 registers every 128 trials keeps
   // that error below the fp16×3 split error (≈ 5e-7).
@@ -241,40 +216,32 @@ int tc_launch(kbo_handle* h, const __half* Ksh, const __half* Ksl, int64_t rows,
   int span_chunks = k_span / TC_BK;
   if (span_chunks < 1) span_chunks = 1;
   CUtensorMap tmAh, tmAl, tmBh, tmBl;
-  const uint32_t a_box = h->tc_pair ? TC_BM / 2 : TC_BM;   // the cluster variant loads (and multicasts) 64-row halves
-  KBO_TRY(encode_map(h, &tmAh, Ksh, (uint64_t)Npad, (uint64_t)rows, a_box));
-  KBO_TRY(encode_map(h, &tmAl, Ksl ? Ksl : Ksh, (uint64_t)Npad, (uint64_t)rows, a_box));
+  // each CTA of a cluster loads (and multicasts) one 64-row half of the A tile
+  KBO_TRY(encode_map(h, &tmAh, Ksh, (uint64_t)Npad, (uint64_t)rows, TC_BM / 2));
+  KBO_TRY(encode_map(h, &tmAl, Ksl ? Ksl : Ksh, (uint64_t)Npad, (uint64_t)rows, TC_BM / 2));
   KBO_TRY(encode_map(h, &tmBh, Wh, (uint64_t)Npad, (uint64_t)Npad, TC_BN));
   KBO_TRY(encode_map(h, &tmBl, Wl ? Wl : Wh, (uint64_t)Npad, (uint64_t)Npad, TC_BN));
   if (!h->attr_tc) {
-    KBO_CUDA(h, cudaFuncSetAttribute(tc_variance_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
-    KBO_CUDA(h, cudaFuncSetAttribute(tc_variance_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
+    KBO_CUDA(h, cudaFuncSetAttribute(tc_variance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES));
     h->attr_tc = true;
   }
-  // default: the 2-CTA cluster / TMA-multicast variant (half the K* panel re-reads); kbo_set_tc_pair(h, 0) selects the single-CTA one
-  if (h->tc_pair) {
-    KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * 2 * (size_t)rows));
-    cudaLaunchConfig_t cfg = {};
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.gridDim = dim3((unsigned)(2 * (rows / TC_BM)));
-    cfg.blockDim = dim3(TC_THREADS);
-    cfg.dynamicSmemBytes = TC_SMEM_BYTES;
-    cfg.stream = s;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    KBO_CUDA(h, cudaLaunchKernelEx(&cfg, tc_variance_kernel<true>, tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, nprod, w_scale_dev, amp, var_out,
-                                   sumsq_out, (double*)h->part.p, rows));
-    KBO_LAUNCH_CHECK(h);
-    tc_pair_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>((const double*)h->part.p, rows, w_scale_dev, amp, var_out, sumsq_out);
-    KBO_LAUNCH_CHECK(h);
-    return KBO_OK;
-  }
-  tc_variance_kernel<false><<<(unsigned)(rows / TC_BM), TC_THREADS, TC_SMEM_BYTES, s>>>(tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, nprod, w_scale_dev,
-                                                                                       amp, var_out, sumsq_out, nullptr, rows);
+  // a 2-CTA cluster per 128-row panel: each K* chunk is read once for both CTAs (half the K* panel re-reads)
+  KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * 2 * (size_t)rows));
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.gridDim = dim3((unsigned)(2 * (rows / TC_BM)));
+  cfg.blockDim = dim3(TC_THREADS);
+  cfg.dynamicSmemBytes = TC_SMEM_BYTES;
+  cfg.stream = s;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  KBO_CUDA(h, cudaLaunchKernelEx(&cfg, tc_variance_kernel, tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, nprod, (double*)h->part.p, rows));
+  KBO_LAUNCH_CHECK(h);
+  tc_variance_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>((const double*)h->part.p, rows, w_scale_dev, amp, var_out, sumsq_out);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }

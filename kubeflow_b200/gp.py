@@ -28,8 +28,8 @@ class GPEngine:
     def __init__(self, device: int = 0, *, kernel: str = "matern52", length_scale=1.0, amplitude: float = 1.0,
                  noise: float = 1e-10, acq: str = "ei", xi: float = 0.01, kappa: float = 1.96,
                  normalize_y: bool = True, var_mode: str = "auto", tc_k_span: int = 0, scratch_limit: int | None = None,
-                 tc_pair: bool | None = None, tc_refine: bool | None = None, tc_fast: bool | None = None,
-                 rank_tc: bool | None = None, rank_prefix: int | None = None, lazy_inverse: bool | None = None):
+                 tc_fast: bool | None = None, rank_tc: bool | None = None, rank_prefix: int | None = None,
+                 lazy_inverse: bool | None = None):
         if kernel not in L.KERNELS:
             raise ValueError(f"kernel must be one of {sorted(L.KERNELS)}, got {kernel!r}")
         if acq not in L.ACQS:
@@ -51,10 +51,6 @@ class GPEngine:
         self.N = self.D = 0
         if scratch_limit is not None:
             L.check(self.lib, self._h, self.lib.kbo_set_scratch_limit(self._h, int(scratch_limit)))
-        if tc_pair is not None:
-            L.check(self.lib, self._h, self.lib.kbo_set_tc_pair(self._h, int(bool(tc_pair))))
-        if tc_refine is not None:
-            L.check(self.lib, self._h, self.lib.kbo_set_tc_refine(self._h, int(bool(tc_refine))))
         if tc_fast is not None:
             L.check(self.lib, self._h, self.lib.kbo_set_tc_fast(self._h, int(bool(tc_fast))))
         if rank_tc is not None:
@@ -155,7 +151,7 @@ class GPEngine:
         return dict(lml=lml.value, y_mean=ym.value, y_std=ys.value, y_opt=yo.value, info=info.value)
 
     def last_contenders(self) -> int:
-        """How many candidates the last tensor-core sweep re-evaluated in FP64 (kbo_set_tc_refine)."""
+        """How many candidates the last tensor-core sweep re-evaluated in FP64."""
         return int(self.lib.kbo_last_contenders(self._h))
 
     def last_rank_error(self) -> float:
@@ -172,7 +168,8 @@ class GPEngine:
 
     def last_unrefined(self) -> int:
         """0: the last tensor-core suggestion was decided in FP64 among every candidate that could be the maximum;
-        1: among the best 4096 by fp32 value (window overflow); 2: not refined (exact ties beyond the cap / refinement off)."""
+        1: among the best 4096 by fp32 value (window overflow); 2: not refined (exact ties beyond the cap, or a grid of 2^31 or
+        more rows)."""
         return int(self.lib.kbo_last_unrefined(self._h))
 
     def fp64_peak_tflops(self) -> float:

@@ -48,7 +48,7 @@ def test_kstar_kernel_is_wgmma_plus_two_mufu_per_pair(sass):
 
 
 def test_three_product_kernel_uses_tma_multicast(sass):
-    ops = _ops(sass, "tc_variance_kernelILb1")
+    ops = _ops(sass, "tc_variance_kernel")
     assert any(o.startswith("HGMMA") for o in ops) and any("MULTICAST" in o for o in ops if o.startswith("UTMALDG"))
 
 
