@@ -66,6 +66,7 @@ def main():
     from .enas_service import EnasService
     from .hyperband import HyperbandService
     from .mvtpe_service import MultivariateTpeService
+    from .pbt_service import PbtService
     from .service import DispatchService, RandomService, SkoptService, SobolService
     from .tpe_service import TpeService
     ap = argparse.ArgumentParser()
@@ -86,7 +87,7 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
         inner = DispatchService([SkoptService({"device": local, "shard": True}), RandomService(), SobolService(),
                                  CmaesService(), TpeService({"device": local}), MultivariateTpeService({"device": local}), EnasService({"device": local}),
-                                 HyperbandService()])
+                                 HyperbandService(), PbtService()])
         spmd = SpmdServicer(inner)
         if dist.get_rank() == 0:
             server, port = serve(spmd, args.port)
@@ -101,7 +102,7 @@ def main():
         return
     server, port = serve(DispatchService([SkoptService({"device": args.device}), RandomService(), SobolService(), CmaesService(),
                                          TpeService({"device": args.device}), MultivariateTpeService({"device": args.device}),
-                                         EnasService({"device": args.device}), HyperbandService()]), args.port)
+                                         EnasService({"device": args.device}), HyperbandService(), PbtService()]), args.port)
     logging.info("api.v1.beta1.Suggestion listening on :%d", port)
     server.wait_for_termination()
 

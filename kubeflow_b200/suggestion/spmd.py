@@ -43,7 +43,7 @@ class SpmdServicer:
 
     def GetSuggestions(self, request, context):
         if request.experiment.spec.algorithm.algorithm_name not in self.sharded_algorithms:
-            return self.inner.GetSuggestions(request, context)      # nothing to shard (random, sobol, cmaes, tpe, multivariate-tpe, enas, hyperband): rank 0 alone
+            return self.inner.GetSuggestions(request, context)      # nothing to shard (random, sobol, cmaes, tpe, multivariate-tpe, enas, hyperband, pbt): rank 0 alone
         data = request._data if isinstance(request, LazyRequest) else request.SerializeToString()
         with self._lock:
             self._bcast(("GetSuggestions", data))
