@@ -101,7 +101,8 @@ int kbo_create(kbo_handle** out, int device);
 void kbo_destroy(kbo_handle* h);
 const char* kbo_last_error(const kbo_handle* h);
 /* cap (bytes) on the per-sweep K* scratch; default 4 GiB.  Determines the candidate chunk size (rounded down to a
- * multiple of sm_count*128 rows so every launch is a whole number of waves). */
+ * multiple of sm_count*128 rows so every launch is a whole number of waves).  Also caps the lane memory of one
+ * kbo_lml_grad_batch call. */
 int kbo_set_scratch_limit(kbo_handle* h, uint64_t bytes);
 /* Tensor-core mode re-evaluates on the FP64 path every candidate whose fp32 acquisition value is within 2e-4 of the maximum
  * (at most 4096 of them) and takes the first-index argmax over those FP64 values, so the returned suggestion (index, value,
@@ -188,6 +189,18 @@ int kbo_lml_grad(kbo_handle* h, double* grad_host, int32_t n_out, void* stream);
  * pivots (0 = ok).  Synchronises.  1 <= G <= 64. */
 int kbo_lml_batch(kbo_handle* h, const double* X, const double* y, int32_t N, int32_t D, int32_t G, const kbo_params* params,
                   int x_on_host, double* lml_host, int32_t* info_host, void* stream);
+/* Log-marginal likelihood AND its gradient for G hyper-parameter settings over ONE history, for gradient-based theta fitting
+ * with several starts in lockstep: what sklearn's L-BFGS-B asks of log_marginal_likelihood(theta, eval_gradient=True) once
+ * per start and iteration ($SK/_gpr.py:541-655).  Arguments as kbo_lml_batch; every entry must have the same n_length_scale P.
+ * Per theta, on its own stream: Gram, Cholesky, W = L^-1, alpha = W^T W yn, the LML, K^-1 = W^T W and the kbo_lml_grad
+ * gradient.  grad_host: G x (2 + P) doubles, row g in kbo_lml_grad's order (log amplitude, log noise, log l_1..l_P).  A theta
+ * whose Gram matrix is not positive definite gets lml = -inf, a zero gradient and its pivot in info_host; the others are
+ * unaffected.  Each theta's (lml, gradient) is bit-identical whatever batch or position it is computed in.  Memory: about
+ * 3 * 8 * ld^2 bytes per theta (ld = N rounded up to 64; 1.5 GiB at N = 8192), kept by the handle for the next call; a batch
+ * needing more than kbo_set_scratch_limit fails with KBO_ERR_INVALID (naming the bytes needed) before any work.  Does not
+ * touch the handle's fitted state.  Synchronises.  1 <= G <= 64, 1 <= D <= 512, N <= 25600. */
+int kbo_lml_grad_batch(kbo_handle* h, const double* X, const double* y, int32_t N, int32_t D, int32_t G, const kbo_params* params,
+                       int x_on_host, double* lml_host, double* grad_host, int32_t* info_host, void* stream);
 /* copies the fit state into caller-owned DEVICE buffers (any may be NULL): L_out, W_out are N×N row-major
  * (L: lower Cholesky factor, strict upper part zeroed; W = L^-1), alpha_out has N entries. For parity tests. */
 int kbo_fit_state(kbo_handle* h, double* L_out, double* W_out, double* alpha_out, void* stream);

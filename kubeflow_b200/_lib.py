@@ -50,7 +50,7 @@ class KboNotPositiveDefinite(KboError):
 
 # every symbol include/kbo.h declares (tests/test_abi.py checks the .so exports exactly these)
 EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_set_scratch_limit", "kbo_last_contenders", "kbo_set_tc_fast", "kbo_last_rank_error", "kbo_set_rank_tc", "kbo_last_rank_mu_error", "kbo_last_unrefined", "kbo_set_rank_prefix", "kbo_last_prefix_survivors", "kbo_set_lazy_inverse", "kbo_fit", "kbo_fit_append", "kbo_fit_room", "kbo_fit_rebase",
-           "kbo_fit_info", "kbo_lml_grad", "kbo_lml_batch", "kbo_fit_state", "kbo_sweep", "kbo_sweep_multi", "kbo_last_decisions", "kbo_predict_mean", "kbo_best_to_host",
+           "kbo_fit_info", "kbo_lml_grad", "kbo_lml_batch", "kbo_lml_grad_batch", "kbo_fit_state", "kbo_sweep", "kbo_sweep_multi", "kbo_last_decisions", "kbo_predict_mean", "kbo_best_to_host",
            "kbo_comm_unique_id", "kbo_comm_init", "kbo_comm_destroy", "kbo_comm_size", "kbo_allreduce_argmax", "kbo_suggest_host", "kbo_last_timings",
            "kbo_gram", "kbo_potrf", "kbo_trtri", "kbo_acq_argmax",
            "kbo_req_open", "kbo_req_close", "kbo_req_header", "kbo_req_trials", "kbo_hash64",
@@ -136,6 +136,7 @@ def load() -> C.CDLL:
     lib.kbo_fit_state.argtypes = [vp, vp, vp, vp, vp]
     lib.kbo_lml_grad.argtypes = [vp, pd, i32, vp]
     lib.kbo_lml_batch.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(KboParams), C.c_int, pd, C.POINTER(i32), vp]
+    lib.kbo_lml_grad_batch.argtypes = [vp, vp, vp, i32, i32, i32, C.POINTER(KboParams), C.c_int, pd, pd, C.POINTER(i32), vp]
     lib.kbo_sweep.argtypes = [vp, vp, i32, i64, i64, C.c_int, vp, vp, vp, vp, vp]
     lib.kbo_sweep_multi.argtypes = [vp, vp, i32, i64, i64, C.c_int, i32, vp, vp, vp]
     lib.kbo_last_decisions.argtypes = [vp, i32, vp, vp, vp]

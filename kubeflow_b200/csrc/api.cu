@@ -137,6 +137,24 @@ int kbo_lml_batch(kbo_handle* h, const double* X, const double* y, int32_t N, in
   return kbo_i_lml_batch(h, X, y, N, D, G, params, lml_host, info_host, s);
 }
 
+int kbo_lml_grad_batch(kbo_handle* h, const double* X, const double* y, int32_t N, int32_t D, int32_t G, const kbo_params* params, int x_on_host,
+                       double* lml_host, double* grad_host, int32_t* info_host, void* stream) {
+  if (!h) return KBO_ERR_INVALID;
+  if (!X || !y || !params || !lml_host || !grad_host) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_grad_batch: null argument");
+  if (N < 1 || D < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_grad_batch: need N >= 1 and D >= 1");
+  cudaStream_t s = (cudaStream_t)stream;
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  if (x_on_host) {
+    KBO_TRY(kbo_reserve(h, h->stage_X, sizeof(double) * (size_t)N * D));
+    KBO_TRY(kbo_reserve(h, h->stage_y, sizeof(double) * (size_t)N));
+    KBO_CUDA(h, cudaMemcpyAsync(h->stage_X.p, X, sizeof(double) * (size_t)N * D, cudaMemcpyHostToDevice, s));
+    KBO_CUDA(h, cudaMemcpyAsync(h->stage_y.p, y, sizeof(double) * (size_t)N, cudaMemcpyHostToDevice, s));
+    X = (const double*)h->stage_X.p;
+    y = (const double*)h->stage_y.p;
+  }
+  return kbo_i_lml_grad_batch(h, X, y, N, D, G, params, lml_host, grad_host, info_host, s);
+}
+
 int kbo_fit_append(kbo_handle* h, const double* x, double y, int x_on_host, void* stream) {
   if (!h) return KBO_ERR_INVALID;
   if (!x) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_fit_append: null argument");

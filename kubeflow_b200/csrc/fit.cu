@@ -271,11 +271,14 @@ int kbo_i_potrf(kbo_handle* h, double* A, int N, int lda, int* info_dev, cudaStr
 }
 
 // W = L^-1 by recursive doubling: [[W11,0],[−W22·L21·W11, W22]] — log2(N/64) levels of two batched GEMMs.
-int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int ldw, cudaStream_t s) {
+// T: N × ldw scratch (nullptr: the handle's)
+int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int ldw, cudaStream_t s, double* T) {
   const int smem = 2 * KBO_NB * (KBO_NB + 1) * (int)sizeof(double);
   KBO_CUDA(h, cudaFuncSetAttribute(diag_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-  KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ldw));
-  double* T = (double*)h->T.p;
+  if (!T) {
+    KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ldw));
+    T = (double*)h->T.p;
+  }
   KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, s));
   diag_inv_kernel<<<(N + KBO_NB - 1) / KBO_NB, 1024, smem, s>>>(L, N, ldl, W, ldw);
   KBO_LAUNCH_CHECK(h);
@@ -1182,21 +1185,22 @@ trsv_lml_kernel(const double* __restrict__ L, int N, int ldl, const double* __re
 struct LmlLane {
   cudaStream_t s = nullptr;
   DevBuf K, Xs, XsT, nx, inv_ls, Linv, info, out;
+  DevBuf W, T, z, alpha, part;   // kbo_lml_grad_batch only: W = L⁻¹, the trtri / transpose scratch, alpha, gradient partials
 };
 
-int kbo_i_lml_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int N, int D, int G, const kbo_params* params, double* lml_host,
-                    int32_t* info_host, cudaStream_t s) {
-  if (N < 1 || D < 1 || D > 512 || G < 1 || G > 64) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_batch: need N >= 1, 1 <= D <= 512, 1 <= G <= 64");
-  const int ld = round_up(N, 64);
+// Checks shared by kbo_lml_batch and kbo_lml_grad_batch; makes G lanes and the kernels' shared-memory opt-ins.
+static int lml_lanes_prepare(kbo_handle* h, const char* name, int N, int D, int G, const kbo_params* params, std::vector<LmlLane>*& lanes) {
+  if (N < 1 || D < 1 || D > 512 || G < 1 || G > 64) KBO_FAIL(h, KBO_ERR_INVALID, "%s: need N >= 1, 1 <= D <= 512, 1 <= G <= 64", name);
   for (int g = 0; g < G; g++) {
     const kbo_params* p = params + g;
-    if (!p->length_scale || (p->n_length_scale != 1 && p->n_length_scale != D)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_batch: theta %d: n_length_scale must be 1 or D", g);
-    if (!(p->noise >= 0.0) || !(p->amplitude > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_batch: theta %d: amplitude must be > 0 and noise >= 0", g);
-    if (p->kernel != KBO_KERNEL_RBF && p->kernel != KBO_KERNEL_MATERN52) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_batch: theta %d: unknown kernel", g);
+    if (!p->length_scale || (p->n_length_scale != 1 && p->n_length_scale != D)) KBO_FAIL(h, KBO_ERR_INVALID, "%s: theta %d: n_length_scale must be 1 or D", name, g);
+    if (!(p->noise >= 0.0) || !(p->amplitude > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "%s: theta %d: amplitude must be > 0 and noise >= 0", name, g);
+    if (p->kernel != KBO_KERNEL_RBF && p->kernel != KBO_KERNEL_MATERN52) KBO_FAIL(h, KBO_ERR_INVALID, "%s: theta %d: unknown kernel", name, g);
     for (int d = 0; d < p->n_length_scale; d++)
-      if (!(p->length_scale[d] > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_batch: theta %d: length_scale[%d] must be > 0", g, d);
+      if (!(p->length_scale[d] > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "%s: theta %d: length_scale[%d] must be > 0", name, g, d);
   }
-  auto* lanes = (std::vector<LmlLane>*)h->lml_lanes;
+  if ((int)sizeof(double) * N > 200 * 1024) KBO_FAIL(h, KBO_ERR_INVALID, "%s: N <= 25600 supported (got %d)", name, N);
+  lanes = (std::vector<LmlLane>*)h->lml_lanes;
   if (!lanes) h->lml_lanes = lanes = new std::vector<LmlLane>();
   if ((int)lanes->size() < G) lanes->resize(G);
   const int smem_pf = 2 * KBO_NB * (KBO_NB + 1) * (int)sizeof(double);
@@ -1206,37 +1210,54 @@ int kbo_i_lml_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int
     KBO_CUDA(h, cudaFuncSetAttribute(diag_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_pf));
     h->attr_fit = true;
   }
-  const int zs_bytes = (int)sizeof(double) * N;
-  if (zs_bytes > 200 * 1024) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_batch: N <= 25600 supported (got %d)", N);
-  KBO_CUDA(h, cudaFuncSetAttribute(trsv_lml_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, zs_bytes));
-  // y statistics are θ-independent: normalise once on the caller's stream
+  return KBO_OK;
+}
+
+// y statistics are θ-independent: normalise once on the caller's stream, which every lane then waits for
+static int lml_lanes_prep_y(kbo_handle* h, const double* y_dev, int N, int ld, int normalize_y, cudaStream_t s) {
   KBO_TRY(kbo_reserve(h, h->lml_yn, sizeof(double) * ld));
   KBO_TRY(kbo_reserve(h, h->lml_scal, sizeof(double) * 16));
-  prep_y_kernel<<<1, 1024, 0, s>>>(y_dev, N, params[0].normalize_y, (double*)h->lml_yn.p, (double*)h->lml_scal.p);
+  prep_y_kernel<<<1, 1024, 0, s>>>(y_dev, N, normalize_y, (double*)h->lml_yn.p, (double*)h->lml_scal.p);
   KBO_LAUNCH_CHECK(h);
   if (!h->lml_ev) KBO_CUDA(h, cudaEventCreateWithFlags(&h->lml_ev, cudaEventDisableTiming));
   KBO_CUDA(h, cudaEventRecord(h->lml_ev, s));
+  return KBO_OK;
+}
+
+// One θ on its lane: X/ℓ, Gram, Cholesky in L.K (pivot in L.info).
+static int lml_lane_factor(kbo_handle* h, LmlLane& L, const double* X_dev, int N, int D, int ld, const kbo_params* p, std::vector<double>& inv) {
+  if (!L.s) KBO_CUDA(h, cudaStreamCreateWithFlags(&L.s, cudaStreamNonBlocking));
+  KBO_TRY(kbo_reserve(h, L.K, sizeof(double) * (size_t)ld * ld));
+  KBO_TRY(kbo_reserve(h, L.Xs, sizeof(double) * (size_t)ld * D));
+  KBO_TRY(kbo_reserve(h, L.XsT, sizeof(double) * (size_t)D * ld));
+  KBO_TRY(kbo_reserve(h, L.nx, sizeof(double) * ld));
+  KBO_TRY(kbo_reserve(h, L.inv_ls, sizeof(double) * 512));
+  KBO_TRY(kbo_reserve(h, L.Linv, sizeof(double) * KBO_NB * KBO_NB));
+  KBO_TRY(kbo_reserve(h, L.info, sizeof(int) * 4));
+  KBO_TRY(kbo_reserve(h, L.out, sizeof(double) * 2));
+  KBO_CUDA(h, cudaStreamWaitEvent(L.s, h->lml_ev, 0));
+  for (int d = 0; d < p->n_length_scale; d++) inv[d] = 1.0 / p->length_scale[d];
+  KBO_CUDA(h, cudaMemcpyAsync(L.inv_ls.p, inv.data(), sizeof(double) * p->n_length_scale, cudaMemcpyHostToDevice, L.s));   // pageable: staged before return
+  prep_x_kernel<<<(N + 127) / 128, 128, 0, L.s>>>(X_dev, N, D, (const double*)L.inv_ls.p, p->n_length_scale, (double*)L.Xs.p, (double*)L.XsT.p, ld,
+                                                 (double*)L.nx.p);
+  KBO_LAUNCH_CHECK(h);
+  KBO_TRY(kbo_i_gram(h, (const double*)L.Xs.p, N, D, p->kernel, p->amplitude, p->noise, (double*)L.K.p, ld, L.s));
+  KBO_TRY(potrf_impl(h, (double*)L.K.p, N, ld, (int*)L.info.p, L.s, [](int, int) { return (int)KBO_OK; }, (double*)L.Linv.p));
+  return KBO_OK;
+}
+
+int kbo_i_lml_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int N, int D, int G, const kbo_params* params, double* lml_host,
+                    int32_t* info_host, cudaStream_t s) {
+  std::vector<LmlLane>* lanes = nullptr;
+  KBO_TRY(lml_lanes_prepare(h, "kbo_lml_batch", N, D, G, params, lanes));
+  const int ld = round_up(N, 64);
+  const int zs_bytes = (int)sizeof(double) * N;
+  KBO_CUDA(h, cudaFuncSetAttribute(trsv_lml_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, zs_bytes));
+  KBO_TRY(lml_lanes_prep_y(h, y_dev, N, ld, params[0].normalize_y, s));
   std::vector<double> inv(512);
   for (int g = 0; g < G; g++) {
     LmlLane& L = (*lanes)[g];
-    const kbo_params* p = params + g;
-    if (!L.s) KBO_CUDA(h, cudaStreamCreateWithFlags(&L.s, cudaStreamNonBlocking));
-    KBO_TRY(kbo_reserve(h, L.K, sizeof(double) * (size_t)ld * ld));
-    KBO_TRY(kbo_reserve(h, L.Xs, sizeof(double) * (size_t)ld * D));
-    KBO_TRY(kbo_reserve(h, L.XsT, sizeof(double) * (size_t)D * ld));
-    KBO_TRY(kbo_reserve(h, L.nx, sizeof(double) * ld));
-    KBO_TRY(kbo_reserve(h, L.inv_ls, sizeof(double) * 512));
-    KBO_TRY(kbo_reserve(h, L.Linv, sizeof(double) * KBO_NB * KBO_NB));
-    KBO_TRY(kbo_reserve(h, L.info, sizeof(int) * 4));
-    KBO_TRY(kbo_reserve(h, L.out, sizeof(double) * 2));
-    KBO_CUDA(h, cudaStreamWaitEvent(L.s, h->lml_ev, 0));
-    for (int d = 0; d < p->n_length_scale; d++) inv[d] = 1.0 / p->length_scale[d];
-    KBO_CUDA(h, cudaMemcpyAsync(L.inv_ls.p, inv.data(), sizeof(double) * p->n_length_scale, cudaMemcpyHostToDevice, L.s));   // pageable: staged before return
-    prep_x_kernel<<<(N + 127) / 128, 128, 0, L.s>>>(X_dev, N, D, (const double*)L.inv_ls.p, p->n_length_scale, (double*)L.Xs.p, (double*)L.XsT.p, ld,
-                                                   (double*)L.nx.p);
-    KBO_LAUNCH_CHECK(h);
-    KBO_TRY(kbo_i_gram(h, (const double*)L.Xs.p, N, D, p->kernel, p->amplitude, p->noise, (double*)L.K.p, ld, L.s));
-    KBO_TRY(potrf_impl(h, (double*)L.K.p, N, ld, (int*)L.info.p, L.s, [](int, int) { return (int)KBO_OK; }, (double*)L.Linv.p));
+    KBO_TRY(lml_lane_factor(h, L, X_dev, N, D, ld, params + g, inv));
     trsv_lml_kernel<<<1, 256, zs_bytes, L.s>>>((const double*)L.K.p, N, ld, (const double*)h->lml_yn.p, (const int*)L.info.p, (double*)L.out.p);
     KBO_LAUNCH_CHECK(h);
   }
@@ -1251,11 +1272,80 @@ int kbo_i_lml_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int
   return KBO_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// kbo_lml_grad_batch: LML and ∂LML/∂θ of G settings over one history — what sklearn's L-BFGS-B asks of
+// log_marginal_likelihood(theta, eval_gradient=True) once per start and iteration ($SK/_gpr.py:541-655), for the starts of a
+// restart search in lockstep.  Per θ on its lane stream: Gram, Cholesky (as kbo_lml_batch), W = L⁻¹ (kbo_i_trtri with the
+// lane's scratch), alpha = Wᵀ(W·yn) and the LML (the fit's kernels), then K⁻¹ and the gradient (kbo_i_lml_grad_from_w, the
+// kernels kbo_lml_grad runs).  Every reduction has a fixed order and nothing is shared between lanes, so a θ's result does not
+// depend on the batch it is in.  Lane memory: L / K⁻¹, W and the scratch plane, 3·ld² doubles, plus the small vectors.
+size_t kbo_i_lml_grad_lane_bytes(int N, int D, int P) {
+  const size_t ld = (size_t)round_up(N, 64), nb = (size_t)(N + 63) / 64;
+  return sizeof(double) * (3 * ld * ld + 2 * ld * D + 3 * ld + nb * nb * (2 + P) + (2 + P) + KBO_NB * KBO_NB + 512 + 16) + sizeof(int) * 4;
+}
+
+int kbo_i_lml_grad_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int N, int D, int G, const kbo_params* params, double* lml_host,
+                         double* grad_host, int32_t* info_host, cudaStream_t s) {
+  std::vector<LmlLane>* lanes = nullptr;
+  KBO_TRY(lml_lanes_prepare(h, "kbo_lml_grad_batch", N, D, G, params, lanes));
+  const int P = params[0].n_length_scale;
+  for (int g = 1; g < G; g++)
+    if (params[g].n_length_scale != P) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_grad_batch: theta %d: every theta needs the same n_length_scale", g);
+  const size_t need = (size_t)G * kbo_i_lml_grad_lane_bytes(N, D, P);   // checked before anything is allocated or launched
+  if (need > h->scratch_limit)
+    KBO_FAIL(h, KBO_ERR_INVALID, "kbo_lml_grad_batch: %d thetas at N = %d, D = %d need %zu bytes of lane memory, over the scratch limit of %llu bytes",
+             G, N, D, need, (unsigned long long)h->scratch_limit);
+  const int ld = round_up(N, 64), nb = (N + 63) / 64, ncomp = 2 + P, nslab = (N + 255) / 256;
+  KBO_TRY(lml_lanes_prep_y(h, y_dev, N, ld, params[0].normalize_y, s));
+  std::vector<double> inv(512);
+  for (int g = 0; g < G; g++) {
+    LmlLane& L = (*lanes)[g];
+    const kbo_params* p = params + g;
+    KBO_TRY(kbo_reserve(h, L.W, sizeof(double) * (size_t)ld * ld));
+    KBO_TRY(kbo_reserve(h, L.T, sizeof(double) * (size_t)ld * ld));
+    KBO_TRY(kbo_reserve(h, L.z, sizeof(double) * ld));
+    KBO_TRY(kbo_reserve(h, L.alpha, sizeof(double) * ld));
+    KBO_TRY(kbo_reserve(h, L.part, sizeof(double) * ((size_t)nb * nb * ncomp + ncomp)));
+    KBO_TRY(kbo_reserve(h, L.out, sizeof(double) * 16));   // the LML kernel writes S_QUAD, S_LOGDET, S_LML
+    KBO_TRY(lml_lane_factor(h, L, X_dev, N, D, ld, p, inv));
+    double *K = (double*)L.K.p, *W = (double*)L.W.p, *T = (double*)L.T.p, *alpha = (double*)L.alpha.p, *out = (double*)L.out.p;
+    KBO_TRY(kbo_i_trtri(h, K, N, ld, W, ld, L.s, T));
+    trmv_lower_kernel<<<(N + 7) / 8, 256, 0, L.s>>>(W, N, ld, (const double*)h->lml_yn.p, (double*)L.z.p);
+    KBO_LAUNCH_CHECK(h);
+    trmv_lower_t_kernel<<<dim3((N + 127) / 128, nslab), 128, 0, L.s>>>(W, N, ld, (const double*)L.z.p, T);   // slab partials in the scratch plane
+    KBO_LAUNCH_CHECK(h);
+    trmv_t_reduce_kernel<<<(N + 127) / 128, 128, 0, L.s>>>(T, N, nslab, alpha);
+    KBO_LAUNCH_CHECK(h);
+    lml_kernel<<<1, 1024, 0, L.s>>>(K, N, ld, (const double*)h->lml_yn.p, alpha, out);   // LML in out[S_LML]; L is not read after this
+    KBO_LAUNCH_CHECK(h);
+    double* part = (double*)L.part.p;
+    KBO_TRY(kbo_i_lml_grad_from_w(h, (const double*)L.Xs.p, N, D, p->kernel, p->amplitude, p->noise, alpha, W, T, K, ld, P, part,
+                                  part + (size_t)nb * nb * ncomp, L.s));
+  }
+  for (int g = 0; g < G; g++) {
+    LmlLane& L = (*lanes)[g];
+    int inf = 0;
+    double lml = 0.0;
+    double* gh = grad_host + (size_t)g * ncomp;
+    KBO_CUDA(h, cudaMemcpyAsync(&lml, (double*)L.out.p + S_LML, sizeof(double), cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, cudaMemcpyAsync(gh, (double*)L.part.p + (size_t)nb * nb * ncomp, sizeof(double) * ncomp, cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, cudaMemcpyAsync(&inf, L.info.p, sizeof(int), cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, cudaStreamSynchronize(L.s));
+    if (inf != 0) {   // the lane ran on a partly factored L: nothing it computed after the pivot means anything
+      lml = -INFINITY;
+      for (int c = 0; c < ncomp; c++) gh[c] = 0.0;
+    }
+    lml_host[g] = lml;
+    if (info_host) info_host[g] = inf;
+  }
+  return KBO_OK;
+}
+
 void kbo_i_lml_batch_free(kbo_handle* h) {
   auto* lanes = (std::vector<LmlLane>*)h->lml_lanes;
   if (!lanes) return;
   for (auto& L : *lanes) {
-    for (DevBuf* b : {&L.K, &L.Xs, &L.XsT, &L.nx, &L.inv_ls, &L.Linv, &L.info, &L.out})
+    for (DevBuf* b : {&L.K, &L.Xs, &L.XsT, &L.nx, &L.inv_ls, &L.Linv, &L.info, &L.out, &L.W, &L.T, &L.z, &L.alpha, &L.part})
       if (b->p) cudaFree(b->p);
     if (L.s) cudaStreamDestroy(L.s);
   }

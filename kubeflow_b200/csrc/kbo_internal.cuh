@@ -178,15 +178,21 @@ int kbo_i_gram(kbo_handle* h, const double* Xs, int N, int D, int kernel, double
 int kbo_i_potrf(kbo_handle* h, double* A, int N, int lda, int* info_dev, cudaStream_t s);
 int kbo_i_fit_append(kbo_handle* h, const double* x_dev, double y, cudaStream_t s);
 int kbo_i_fit_rebase(kbo_handle* h, int n_keep, const double* y_dev, cudaStream_t s);
-int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int ldw, cudaStream_t s);
+int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int ldw, cudaStream_t s, double* T = nullptr);
 int kbo_i_zero_upper(kbo_handle* h, double* A, int N, int lda, cudaStream_t s);
 int kbo_i_fit(kbo_handle* h, const double* X_dev, const double* y_dev, int N, int D, const kbo_params* p, cudaStream_t s);
 int kbo_i_lml_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int N, int D, int G, const kbo_params* params, double* lml_host,
                     int32_t* info_host, cudaStream_t s);
+int kbo_i_lml_grad_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int N, int D, int G, const kbo_params* params, double* lml_host,
+                         double* grad_host, int32_t* info_host, cudaStream_t s);
+size_t kbo_i_lml_grad_lane_bytes(int N, int D, int P);   // device memory one θ of kbo_lml_grad_batch takes
 void kbo_i_lml_batch_free(kbo_handle* h);
 void kbo_i_fit_partition_free(kbo_handle* h);
 int kbo_i_ensure_w(kbo_handle* h, cudaStream_t s);   // form the rest of W and the full planes if the fit left them out
 int kbo_i_debug_rank_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int tile_pairs, float* mun_out, float* varn_out, cudaStream_t s);
+// ---- lmlgrad.cu ---------------------------------------------------------------------------------
+int kbo_i_lml_grad_from_w(kbo_handle* h, const double* Xs, int N, int D, int kind, double amp, double noise, const double* alpha,
+                          const double* W, double* Wt, double* Kinv, int ld, int P, double* part, double* grad_dev, cudaStream_t s);
 // ---- solve.cu ----------------------------------------------------------------------------------
 int kbo_i_alpha_by_solves(kbo_handle* h, cudaStream_t s);
 int kbo_i_variance_by_solves(kbo_handle* h, const double* Ks, int n, double* varn64, cudaStream_t s);

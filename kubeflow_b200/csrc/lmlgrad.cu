@@ -3,7 +3,8 @@
 //   ∂K/∂log a = a·k ; ∂K/∂log σ² = σ²·I ; ∂K/∂log ℓ_d = a·q(r)·Δ_d²,  q = k (RBF), (5/3)(1+s)e^{−s} (Matérn-5/2, s = √5 r)
 // K⁻¹ = WᵀW is formed as the lower triangle of Wt·Wtᵀ (Wt = Wᵀ, FP64 GEMM with the triangular K-range cut: N³/3 flop);
 // one fused pass over the lower-triangular 64×64 pair tiles then accumulates every component (off-diagonal pairs count
-// twice), per-block partials are reduced in a fixed order.  Everything FP64; called after kbo_fit at the same θ.
+// twice), per-block partials are reduced in a fixed order.  Everything FP64; kbo_lml_grad runs it after kbo_fit at the same θ,
+// kbo_lml_grad_batch (fit.cu) on each θ's lane.
 #include "kbo_internal.cuh"
 #include "dgemm.cuh"
 #include "ktab.cuh"
@@ -135,6 +136,24 @@ __global__ void lml_grad_reduce_kernel(const double* __restrict__ partial, int n
   grad[cidx] = cidx == 1 ? 0.5 * noise * s : 0.5 * s;
 }
 
+// K⁻¹ (lower triangle of Wt·Wtᵀ, Wt = Wᵀ) into Kinv, then the 2 + P gradient components into grad_dev.  Every operand is the
+// caller's: kbo_lml_grad passes the handle's fit state, kbo_lml_grad_batch each lane's own planes.  part: nb²·(2 + P) doubles.
+int kbo_i_lml_grad_from_w(kbo_handle* h, const double* Xs, int N, int D, int kind, double amp, double noise, const double* alpha,
+                          const double* W, double* Wt, double* Kinv, int ld, int P, double* part, double* grad_dev, cudaStream_t s) {
+  const int ncomp = 2 + P, nb = (N + 63) / 64;
+  dim3 tg((N + 31) / 32, (N + 31) / 32), tb(32, 8);
+  transpose_kernel<<<tg, tb, 0, s>>>(W, N, ld, Wt, ld);
+  KBO_LAUNCH_CHECK(h);
+  dgemm64_launch<true, EPI_STORE>(s, N, N, N, Wt, ld, Wt, ld, Kinv, ld, 1.0, 0.0, KM_FROM_M, 0, TS_LOWER);
+  KBO_LAUNCH_CHECK(h);
+  dim3 g(nb, nb);
+  lml_grad_kernel<<<g, 256, 0, s>>>(Xs, N, D, kind, amp, alpha, Kinv, ld, P, part, ncomp);
+  KBO_LAUNCH_CHECK(h);
+  lml_grad_reduce_kernel<<<(ncomp + 63) / 64, 64, 0, s>>>(part, nb, nb, ncomp, noise, grad_dev);
+  KBO_LAUNCH_CHECK(h);
+  return KBO_OK;
+}
+
 extern "C" int kbo_lml_grad(kbo_handle* h, double* grad_host, int32_t n_out, void* stream) {
   if (!h) return KBO_ERR_INVALID;
   if (!h->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_lml_grad: call kbo_fit first");
@@ -146,21 +165,11 @@ extern "C" int kbo_lml_grad(kbo_handle* h, double* grad_host, int32_t n_out, voi
   // Wt = Wᵀ into the trtri scratch, K⁻¹ (lower) into the K* fp64 scratch
   KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ld));
   KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)N * ld));
-  dim3 tg((N + 31) / 32, (N + 31) / 32), tb(32, 8);
-  transpose_kernel<<<tg, tb, 0, s>>>((const double*)h->W.p, N, ld, (double*)h->T.p, ld);
-  KBO_LAUNCH_CHECK(h);
-  dgemm64_launch<true, EPI_STORE>(s, N, N, N, (const double*)h->T.p, ld, (const double*)h->T.p, ld, (double*)h->Ks64.p, ld, 1.0, 0.0, KM_FROM_M, 0,
-                                  TS_LOWER);
-  KBO_LAUNCH_CHECK(h);
   const int nb = (N + 63) / 64;
   KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * ((size_t)nb * nb * ncomp + ncomp)));
   double* grad_dev = (double*)h->part.p + (size_t)nb * nb * ncomp;
-  dim3 g(nb, nb);
-  lml_grad_kernel<<<g, 256, 0, s>>>((const double*)h->Xs.p, N, D, h->prm.kernel, h->prm.amplitude, (const double*)h->alpha.p, (const double*)h->Ks64.p, ld,
-                                    P, (double*)h->part.p, ncomp);
-  KBO_LAUNCH_CHECK(h);
-  lml_grad_reduce_kernel<<<(ncomp + 63) / 64, 64, 0, s>>>((const double*)h->part.p, nb, nb, ncomp, h->prm.noise, grad_dev);
-  KBO_LAUNCH_CHECK(h);
+  KBO_TRY(kbo_i_lml_grad_from_w(h, (const double*)h->Xs.p, N, D, h->prm.kernel, h->prm.amplitude, h->prm.noise, (const double*)h->alpha.p,
+                                (const double*)h->W.p, (double*)h->T.p, (double*)h->Ks64.p, ld, P, (double*)h->part.p, grad_dev, s));
   int inf = 0;
   KBO_CUDA(h, cudaMemcpyAsync(grad_host, grad_dev, sizeof(double) * ncomp, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaMemcpyAsync(&inf, h->info.p, sizeof(int), cudaMemcpyDeviceToHost, s));

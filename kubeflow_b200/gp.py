@@ -49,6 +49,7 @@ class GPEngine:
         self.amplitude, self.noise, self.xi, self.kappa = float(amplitude), float(noise), float(xi), float(kappa)
         self.normalize_y, self.tc_k_span = bool(normalize_y), int(tc_k_span)
         self.N = self.D = 0
+        self.scratch_limit = 4 << 30 if scratch_limit is None else int(scratch_limit)   # libkbo's default
         if scratch_limit is not None:
             L.check(self.lib, self._h, self.lib.kbo_set_scratch_limit(self._h, int(scratch_limit)))
         if tc_fast is not None:
@@ -273,15 +274,10 @@ class GPEngine:
         L.check(self.lib, self._h, rc)
         return info["lml"], g
 
-    def lml_batch(self, X, y, thetas, return_info: bool = False):
-        """Log-marginal likelihood of several θ over one history in one call (kbo_lml_batch: the factorisations run concurrently).
-        ``thetas``: list of dicts with any of length_scale / noise / amplitude (the engine's own values where absent).
-        Returns a float64 NumPy array, −inf where the Gram matrix is not positive definite (with ``return_info``, also each θ's
-        1-based failed pivot, 0 if none).  The fitted state is untouched."""
-        X, y = self._as_host_f64(X), self._as_host_f64(y).reshape(-1)
-        N, D = X.shape
-        G = len(thetas)
-        arr = (L.KboParams * G)()
+    def _theta_params(self, thetas):
+        """KboParams array for a list of θ dicts (length_scale / noise / amplitude; the engine's own values where absent), and
+        the length-scale buffers it points to."""
+        arr = (L.KboParams * len(thetas))()
         keep = []
         for g, th in enumerate(thetas):
             ls = np.atleast_1d(np.asarray(th.get("length_scale", self.length_scale), dtype=np.float64))
@@ -291,6 +287,17 @@ class GPEngine:
                                  var_mode=L.VAR_MODES[self.var_mode], amplitude=float(th.get("amplitude", self.amplitude)),
                                  noise=float(th.get("noise", self.noise)), xi=self.xi, kappa=self.kappa, length_scale=buf,
                                  n_length_scale=len(ls), tc_k_span=self.tc_k_span)
+        return arr, keep
+
+    def lml_batch(self, X, y, thetas, return_info: bool = False):
+        """Log-marginal likelihood of several θ over one history in one call (kbo_lml_batch: the factorisations run concurrently).
+        ``thetas``: list of dicts with any of length_scale / noise / amplitude (the engine's own values where absent).
+        Returns a float64 NumPy array, −inf where the Gram matrix is not positive definite (with ``return_info``, also each θ's
+        1-based failed pivot, 0 if none).  The fitted state is untouched."""
+        X, y = self._as_host_f64(X), self._as_host_f64(y).reshape(-1)
+        N, D = X.shape
+        G = len(thetas)
+        arr, keep = self._theta_params(thetas)
         out = np.empty(G, dtype=np.float64)
         info = (C.c_int32 * G)()
         with torch.cuda.device(self.device):
@@ -298,6 +305,34 @@ class GPEngine:
                                         out.ctypes.data_as(C.POINTER(C.c_double)), info, self._stream())
         L.check(self.lib, self._h, rc)
         return (out, np.array(info[:], dtype=np.int32)) if return_info else out
+
+    def lml_grad_batch(self, X, y, thetas, return_info: bool = False):
+        """Log-marginal likelihood and its gradient for several θ over one history in one call (kbo_lml_grad_batch: each θ on
+        its own stream, results independent of the batch).  ``thetas`` as for ``lml_batch``; every θ needs the same number of
+        length scales P.  Returns (lml[G], grad[G, 2 + P]) as float64 NumPy arrays, grad in ``lml_grad``'s order (log amplitude,
+        log noise, log ℓ_1..ℓ_P); a θ whose Gram matrix is not positive definite has lml −inf and a zero gradient (with
+        ``return_info``, also each θ's 1-based failed pivot, 0 if none).  The fitted state is untouched."""
+        X, y = self._as_host_f64(X), self._as_host_f64(y).reshape(-1)
+        N, D = X.shape
+        G = len(thetas)
+        arr, keep = self._theta_params(thetas)
+        P = arr[0].n_length_scale if G else 1
+        lml = np.empty(G, dtype=np.float64)
+        grad = np.empty((G, 2 + P), dtype=np.float64)
+        info = (C.c_int32 * max(G, 1))()
+        with torch.cuda.device(self.device):
+            rc = self.lib.kbo_lml_grad_batch(self._h, X.ctypes.data, y.ctypes.data, int(N), int(D), int(G), arr, 1,
+                                             lml.ctypes.data_as(C.POINTER(C.c_double)), grad.ctypes.data_as(C.POINTER(C.c_double)),
+                                             info, self._stream())
+        L.check(self.lib, self._h, rc)
+        return (lml, grad, np.array(info[:G], dtype=np.int32)) if return_info else (lml, grad)
+
+    @staticmethod
+    def lml_grad_lane_bytes(N: int, D: int, P: int) -> int:
+        """Device memory one θ of ``lml_grad_batch`` takes (kbo_i_lml_grad_lane_bytes in fit.cu); a batch needs G times this
+        within the engine's scratch limit."""
+        ld, nb = (N + 63) // 64 * 64, (N + 63) // 64
+        return 8 * (3 * ld * ld + 2 * ld * D + 3 * ld + nb * nb * (2 + P) + (2 + P) + 64 * 64 + 512 + 16) + 4 * 4
 
     def state(self):
         """Copies of L (lower), W = L^-1 and alpha as float64 CUDA tensors (parity tests)."""

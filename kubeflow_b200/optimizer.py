@@ -2,9 +2,14 @@
 (upstream kubeflow/katib pkg/suggestion/v1beta1/skopt/base_service.py: ``tell(X, y)`` then ``ask()`` per
 requested assignment).  Differences, stated once:
 
-* θ is FIXED per request (length scales, amplitude, noise are settings), where skopt refits them by L-BFGS on the
-  log-marginal likelihood ($SK/_gpr.py:299-339) — bit-reproducing that optimiser is outside the 1e-5 contract
-  (SURVEY.md §7).  Two GPU-side substitutes, both maximising the device-computed LML (one FP64 fit per candidate θ):
+* θ is FIXED per request by default (length scales, amplitude, noise are settings), where skopt refits them by L-BFGS on the
+  log-marginal likelihood ($SK/_gpr.py:299-339).  ``theta_fit="skopt"`` fits θ as skopt does (``kubeflow_b200.thetafit``):
+  amplitude, ARD length scales and noise over skopt's bounds, by SciPy's L-BFGS-B from 1 + ``theta_restarts`` (default 2)
+  starts drawn as sklearn draws them, run in lockstep with one ``GPEngine.lml_grad_batch`` call per round; the engine is then
+  fitted at the winner.  θ is refitted once per change of the told history; constant-liar lies reuse it and take the append
+  path, where skopt refits θ on each lie's copy.  ``kernel="rbf"`` is allowed there, and an all-categorical space keeps
+  Matérn on its one-hot columns where skopt would switch to a HammingKernel.  Older GPU-side substitutes, both maximising
+  the device-computed LML (one FP64 fit per candidate θ):
   ``theta_grid`` = G > 1 tries G multiples of the length scale (geometric, 0.25×…4×); ``theta_search`` = K > 0 additionally
   draws K random (length-scale multiple, noise) pairs log-uniformly from [0.2, 5] × [1e-6, 1e-1] (seeded) — the gradient-free
   analogue of skopt's restarts; ``theta_fit="lbfgs"`` then polishes (log ℓ — per dimension with ``ard=True`` —, log noise)
@@ -50,8 +55,8 @@ FOREST_ESTIMATORS = ("RF", "ET")   # skopt's cook_estimator forests, kubeflow_b2
 class Optimizer:
     def __init__(self, dimensions, base_estimator="GP", n_initial_points=10, acq_func="EI", acq_optimizer="sampling",
                  random_state=None, *, n_points=65536, kernel="matern52", length_scale=None, amplitude=1.0, noise=1e-3, xi=0.01,
-                 kappa=1.96, var_mode="auto", theta_grid=1, theta_search=0, theta_fit=None, theta_fit_maxiter=25, ard=False, device=0, engine=None,
-                 candidate_backend="torch", incremental=True, shard=False):
+                 kappa=1.96, var_mode="auto", theta_grid=1, theta_search=0, theta_fit=None, theta_fit_maxiter=None, theta_restarts=None, ard=False,
+                 device=0, engine=None, candidate_backend="torch", incremental=True, shard=False):
         self.base_estimator = str(base_estimator).upper()
         if self.base_estimator not in ("GP",) + FOREST_ESTIMATORS:
             raise ValueError("base_estimator must be GP, RF or ET (GBRT is not part of the GPU path)")
@@ -81,9 +86,22 @@ class Optimizer:
         self.kernel, self.amplitude, self.noise, self.xi, self.kappa = kernel, amplitude, noise, xi, kappa
         self.length_scale = length_scale
         self.var_mode, self.theta_grid, self.theta_search, self.device = var_mode, int(theta_grid), int(theta_search), device
-        if theta_fit not in (None, "lbfgs"):
-            raise ValueError("theta_fit must be None or 'lbfgs'")
-        self.theta_fit, self.theta_fit_maxiter, self.ard = theta_fit, int(theta_fit_maxiter), bool(ard)
+        if theta_fit not in (None, "lbfgs", "skopt"):
+            raise ValueError("theta_fit must be None, 'lbfgs' or 'skopt'")
+        if theta_restarts is not None and theta_fit != "skopt":
+            raise ValueError("theta_restarts applies to theta_fit='skopt' only")
+        if theta_fit == "skopt":      # the start and the fit are skopt's: nothing may set or search θ beside it
+            for name, given in (("theta_grid", int(theta_grid) > 1), ("theta_search", int(theta_search) > 0), ("ard", bool(ard)),
+                                ("length_scale", length_scale is not None), ("amplitude", amplitude != 1.0), ("noise", noise != 1e-3)):
+                if given:
+                    raise ValueError(f"{name} cannot be combined with theta_fit='skopt': skopt's start and bounds are used")
+            if theta_restarts is not None and int(theta_restarts) < 0:
+                raise ValueError(f"theta_restarts must be >= 0, got {theta_restarts}")
+        self.theta_fit, self.ard = theta_fit, bool(ard)
+        self.theta_fit_maxiter = None if theta_fit_maxiter is None else int(theta_fit_maxiter)
+        self.theta_restarts = 2 if theta_restarts is None else int(theta_restarts)   # skopt's n_restarts_optimizer
+        self._skopt_fit = None        # (told rows, told y, FitResult) of the last theta_fit="skopt" refit
+        self.theta_refits = 0         # theta_fit="skopt" refits so far (diagnostics, tests)
         self.last_theta = None
         if candidate_backend not in ("torch", "numpy"):
             raise ValueError("candidate_backend must be 'torch' (sampled on the device) or 'numpy'")
@@ -107,6 +125,10 @@ class Optimizer:
             random_state = box[0]
             self._seed = random_state
             self.rng = np.random.default_rng(random_state)
+        self._est_seed = None
+        if theta_fit == "skopt":      # skopt cooks its GP once, with a seed drawn from the optimizer's random_state
+            from .thetafit import estimator_seed
+            self._est_seed = estimator_seed(random_state)
         self._fit_state = None        # (θ key, rows in the engine, digest of those rows): lets a request that only adds trials append
         self.last_fit = None          # "fit" | "append" | "reuse": what the last ask did to the engine (diagnostics, tests)
         self.last_best = None
@@ -257,6 +279,8 @@ class Optimizer:
                         best_lml, best_t = lml, (m, nz)
             eng.length_scale, eng.noise = base * best_t[0], best_t[1]
             self.last_theta = dict(length_scale=eng.length_scale.copy(), noise=eng.noise, lml=best_lml)
+        if self.theta_fit == "skopt":
+            self._skopt_theta(eng, self._Xt, ya[:n_told])
         if self.theta_fit == "lbfgs":
             from scipy.optimize import minimize
             Dt = self.space.transformed_n_dims
@@ -275,11 +299,30 @@ class Optimizer:
                     return 1e25, np.zeros_like(t)
                 return -lml, -np.concatenate([g[2:], g[1:2]])
 
-            res = minimize(negative_lml, x0, jac=True, method="L-BFGS-B", bounds=bounds, options=dict(maxiter=self.theta_fit_maxiter))
+            maxiter = 25 if self.theta_fit_maxiter is None else self.theta_fit_maxiter
+            res = minimize(negative_lml, x0, jac=True, method="L-BFGS-B", bounds=bounds, options=dict(maxiter=maxiter))
             eng.length_scale, eng.noise = np.exp(res.x[:-1]), float(np.exp(res.x[-1]))
             self.last_theta = dict(length_scale=eng.length_scale.copy(), noise=eng.noise, lml=-float(res.fun), nfev=int(res.nfev))
         self._tell_engine(eng, Xt, ya)
         return self._pick(eng, Xt, ya, len(X) > n_told)
+
+    def _skopt_theta(self, eng, Xt, yt):
+        """θ as skopt fits it, on the told history (Xt, yt): refitted when that history changed since the last fit, else
+        reused.  Leaves the engine at the winner's θ (its noise plus sklearn's alpha on the diagonal)."""
+        from . import thetafit
+        st = self._skopt_fit
+        if st is None or st[0].shape != Xt.shape or not (np.array_equal(st[0], Xt) and np.array_equal(st[1], yt)):
+            res = thetafit.fit(thetafit.engine_batch_fn(eng, Xt, yt), Xt.shape[1], self._est_seed, self.theta_restarts,
+                               self.theta_fit_maxiter)
+            self._skopt_fit = st = (np.array(Xt, dtype=np.float64, copy=True), np.array(yt, dtype=np.float64, copy=True), res)
+            self.theta_refits += 1
+        res = st[2]
+        th = thetafit.theta_dict(res.theta)
+        eng.amplitude, eng.length_scale, eng.noise = th["amplitude"], th["length_scale"], th["noise"]
+        self.last_theta = dict(amplitude=th["amplitude"], length_scale=th["length_scale"].copy(), noise=float(np.exp(res.theta[-1])),
+                               lml=res.lml, winner=res.winner, batch_calls=res.batch_calls,
+                               starts=[dict(theta0=p.theta0.copy(), theta=p.theta.copy(), neg_lml=p.fun, nit=p.nit, nfev=p.nfev,
+                                            status=p.status, message=p.message) for p in res.starts])
 
     def _pick(self, eng, Xt, ya, lie):
         """Sample the candidates (this rank's share when sharded), sweep them with the fitted engine, and return the point."""

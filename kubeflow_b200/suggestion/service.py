@@ -24,11 +24,14 @@ logger = logging.getLogger(__name__)
 
 SKOPT_SETTINGS = ("base_estimator", "n_initial_points", "acq_func", "acq_optimizer", "random_state")
 ENGINE_SETTINGS = {"n_points": int, "kernel": str, "length_scale": float, "amplitude": float, "noise": float, "xi": float,
-                   "kappa": float, "var_mode": str, "theta_grid": int, "theta_search": int, "theta_fit": str, "theta_fit_maxiter": int, "ard": int, "device": int, "candidate_backend": str}
+                   "kappa": float, "var_mode": str, "theta_grid": int, "theta_search": int, "theta_fit": str, "theta_fit_maxiter": int, "theta_restarts": int, "ard": int, "device": int,
+                   "candidate_backend": str}
 
 TREE_ESTIMATORS = {"RF": "RandomForestRegressor", "ET": "ExtraTreesRegressor"}   # skopt's cook_estimator names
 GP_ONLY_SETTINGS = ("kernel", "length_scale", "amplitude", "noise", "var_mode", "theta_grid", "theta_search", "theta_fit",
-                    "theta_fit_maxiter", "ard")
+                    "theta_fit_maxiter", "theta_restarts", "ard")
+# what theta_fit: skopt takes from skopt itself (its start, its bounds, its search): an Experiment may not set them beside it
+SKOPT_THETA_EXCLUSIVE = ("theta_grid", "theta_search", "ard", "length_scale", "amplitude", "noise")
 
 
 def validate_skopt_settings(settings: dict) -> dict:
@@ -66,10 +69,10 @@ def validate_skopt_settings(settings: dict) -> dict:
                     raise AlgorithmSettingsError(f"var_mode {v} must be tc, f64 or auto")
                 if name == "candidate_backend" and v not in ("torch", "numpy"):
                     raise AlgorithmSettingsError(f"candidate_backend {v} must be torch or numpy")
-                if name == "theta_fit" and v != "lbfgs":
-                    raise AlgorithmSettingsError(f"theta_fit {v} must be lbfgs")
-                if name == "theta_search" and v < 0:
-                    raise AlgorithmSettingsError(f"theta_search must be >= 0, got {value}")
+                if name == "theta_fit" and v not in ("lbfgs", "skopt"):
+                    raise AlgorithmSettingsError(f"theta_fit {v} must be lbfgs or skopt")
+                if name in ("theta_search", "theta_restarts") and v < 0:
+                    raise AlgorithmSettingsError(f"{name} must be >= 0, got {value}")
                 if name in ("n_points", "theta_grid") and v < 1:
                     raise AlgorithmSettingsError(f"{name} must be >= 1, got {value}")
                 if name in ("length_scale", "amplitude") and not v > 0:
@@ -90,6 +93,12 @@ def validate_skopt_settings(settings: dict) -> dict:
         for name in GP_ONLY_SETTINGS:
             if name in out:
                 raise AlgorithmSettingsError(f"setting {name} applies to base_estimator GP only, not {est}")
+    if out.get("theta_fit") == "skopt":
+        for name in SKOPT_THETA_EXCLUSIVE:
+            if name in out and not (name == "theta_grid" and out[name] == 1) and not (name in ("theta_search", "ard") and out[name] == 0):
+                raise AlgorithmSettingsError(f"setting {name} cannot be combined with theta_fit skopt, which uses skopt's own start and bounds")
+    elif "theta_restarts" in out:
+        raise AlgorithmSettingsError("setting theta_restarts applies to theta_fit skopt only")
     return out
 
 

@@ -35,8 +35,9 @@ for N, M, D, mode in ((70, 300, 3, "f64"), (135, 515, 5, "tc"), (300, 700, 33, "
     b4 = e.ask(Xc)
     g = e.lml_grad()[1]
     lm = e.lml_batch(X, y, [dict(noise=1e-3), dict(noise=1e-2, length_scale=th["length_scale"] * 2)])
+    lg = e.lml_grad_batch(X, y, [dict(noise=1e-3), dict(noise=0.0, amplitude=2.0)])      # lanes with W, K⁻¹ and the gradient
     b5, _, _, _ = e.ask(Xc, return_arrays=True)      # three-product / FP64 array path
-    print(N, M, D, mode, b.index, b2.index, b3.index, b4.index, b5.index, e.last_contenders(), e.last_prefix_survivors(), float(g[0]), lm.tolist())
+    print(N, M, D, mode, b.index, b2.index, b3.index, b4.index, b5.index, e.last_contenders(), e.last_prefix_survivors(), float(g[0]), lm.tolist(), lg[0].tolist())
     e.close()
     if mode == "tc":                                  # the ranking pass without pruning, and the round-1 ranking pass
         for kw in (dict(rank_prefix=0), dict(rank_tc=False)):
