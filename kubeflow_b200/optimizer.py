@@ -7,8 +7,13 @@ requested assignment).  Differences, stated once:
   amplitude, ARD length scales and noise over skopt's bounds, by SciPy's L-BFGS-B from 1 + ``theta_restarts`` (default 2)
   starts drawn as sklearn draws them, run in lockstep with one ``GPEngine.lml_grad_batch`` call per round; the engine is then
   fitted at the winner.  θ is refitted once per change of the told history; constant-liar lies reuse it and take the append
-  path, where skopt refits θ on each lie's copy.  ``kernel="rbf"`` is allowed there, and an all-categorical space keeps
-  Matérn on its one-hot columns where skopt would switch to a HammingKernel.  Older GPU-side substitutes, both maximising
+  path, where skopt refits θ on each lie's copy.  ``kernel="rbf"`` is allowed there.  An all-categorical space keeps
+  Matérn on its one-hot columns by default, where skopt switches to a HammingKernel; ``kernel="hamming"`` gives skopt's
+  model there (``kubeflow_b200.hamming``): θ holds the per-dimension weights l_j (``length_scale`` is the isotropic l, 1.0 by
+  default; ``theta_fit="skopt"`` fits one l_j per dimension over (1e-5, 1e5)), mapped to RBF length scales of the one-hot
+  columns in one place, so the fit, append, rebase, sweep and LML gradient are the engine's own.  It is refused, before any
+  device is touched, unless every dimension is Categorical, and beside ``theta_grid``, ``theta_search`` or
+  ``theta_fit="lbfgs"``, which search one-hot length scales.  Older GPU-side substitutes, both maximising
   the device-computed LML (one FP64 fit per candidate θ):
   ``theta_grid`` = G > 1 tries G multiples of the length scale (geometric, 0.25×…4×); ``theta_search`` = K > 0 additionally
   draws K random (length-scale multiple, noise) pairs log-uniformly from [0.2, 5] × [1e-6, 1e-1] (seeded) — the gradient-free
@@ -97,6 +102,14 @@ class Optimizer:
                     raise ValueError(f"{name} cannot be combined with theta_fit='skopt': skopt's start and bounds are used")
             if theta_restarts is not None and int(theta_restarts) < 0:
                 raise ValueError(f"theta_restarts must be >= 0, got {theta_restarts}")
+        self._hmap = None             # kernel="hamming": the map from Hamming weights to the one-hot columns' RBF θ
+        if kernel == "hamming":
+            from .hamming import HammingMap
+            self._hmap = HammingMap(self.space)
+            for name, given in (("theta_grid", int(theta_grid) > 1), ("theta_search", int(theta_search) > 0),
+                                ("theta_fit='lbfgs'", theta_fit == "lbfgs")):
+                if given:
+                    raise ValueError(f"{name} cannot be combined with kernel='hamming': it searches one-hot length scales")
         self.theta_fit, self.ard = theta_fit, bool(ard)
         self.theta_fit_maxiter = None if theta_fit_maxiter is None else int(theta_fit_maxiter)
         self.theta_restarts = 2 if theta_restarts is None else int(theta_restarts)   # skopt's n_restarts_optimizer
@@ -151,13 +164,24 @@ class Optimizer:
 
     def _get_engine(self, ls):
         from .gp import GPEngine
+        kernel = "rbf" if self._hmap is not None else self.kernel
         if self._engine is None:
-            self._engine = GPEngine(self.device, kernel=self.kernel, length_scale=ls, amplitude=self.amplitude, noise=self.noise,
+            self._engine = GPEngine(self.device, kernel=kernel, amplitude=self.amplitude, noise=self.noise,
                                     acq=self.acq, xi=self.xi, kappa=self.kappa, var_mode=self.var_mode)
         e = self._engine
-        e.kernel, e.acq, e.amplitude, e.noise, e.xi, e.kappa = self.kernel, self.acq, self.amplitude, self.noise, self.xi, self.kappa
-        e.length_scale = np.atleast_1d(np.asarray(ls, dtype=np.float64))
+        e.kernel, e.acq, e.amplitude, e.noise, e.xi, e.kappa = kernel, self.acq, self.amplitude, self.noise, self.xi, self.kappa
+        self._set_length_scale(e, ls)
         return e
+
+    def _set_length_scale(self, e, ls):
+        """Every length scale the engine is fitted at passes here.  With kernel="hamming", ``ls`` are the Hamming weights l_j,
+        mapped to the one-hot columns' RBF length scales, and "auto" sweeps at those θ take the path HammingMap.var_mode
+        chooses."""
+        if self._hmap is None:
+            e.length_scale = np.atleast_1d(np.asarray(ls, dtype=np.float64))
+            return
+        e.length_scale = self._hmap.length_scale(ls)
+        e.var_mode = self._hmap.var_mode(ls, self.var_mode)
 
     def _tell_engine(self, eng, Xt, ya, max_append=16):
         """Bring the engine to the history (Xt, ya) at its current θ.  Katib resends the whole history on every request and
@@ -210,6 +234,8 @@ class Optimizer:
             raise
 
     def _default_ls(self):
+        if self._hmap is not None:    # skopt's HammingKernel(length_scale=1.0) start
+            return 1.0 if self.length_scale is None else self.length_scale
         return 0.3 * np.sqrt(self.space.transformed_n_dims) if self.length_scale is None else self.length_scale
 
     def _hedge_gains(self, eng, Xt, ya, lie):
@@ -312,13 +338,19 @@ class Optimizer:
         from . import thetafit
         st = self._skopt_fit
         if st is None or st[0].shape != Xt.shape or not (np.array_equal(st[0], Xt) and np.array_equal(st[1], yt)):
-            res = thetafit.fit(thetafit.engine_batch_fn(eng, Xt, yt), Xt.shape[1], self._est_seed, self.theta_restarts,
-                               self.theta_fit_maxiter)
+            if self._hmap is None:
+                res = thetafit.fit(thetafit.engine_batch_fn(eng, Xt, yt), Xt.shape[1], self._est_seed, self.theta_restarts,
+                                   self.theta_fit_maxiter)
+            else:
+                from .hamming import LS_BOUNDS
+                res = thetafit.fit(thetafit.engine_batch_fn(eng, Xt, yt, hamming=self._hmap), self._hmap.n_dims, self._est_seed,
+                                   self.theta_restarts, self.theta_fit_maxiter, ls_bounds=LS_BOUNDS)
             self._skopt_fit = st = (np.array(Xt, dtype=np.float64, copy=True), np.array(yt, dtype=np.float64, copy=True), res)
             self.theta_refits += 1
         res = st[2]
         th = thetafit.theta_dict(res.theta)
-        eng.amplitude, eng.length_scale, eng.noise = th["amplitude"], th["length_scale"], th["noise"]
+        eng.amplitude, eng.noise = th["amplitude"], th["noise"]
+        self._set_length_scale(eng, th["length_scale"])
         self.last_theta = dict(amplitude=th["amplitude"], length_scale=th["length_scale"].copy(), noise=float(np.exp(res.theta[-1])),
                                lml=res.lml, winner=res.winner, batch_calls=res.batch_calls,
                                starts=[dict(theta0=p.theta0.copy(), theta=p.theta.copy(), neg_lml=p.fun, nit=p.nit, nfev=p.nfev,
@@ -343,6 +375,8 @@ class Optimizer:
             if self._crng is None:
                 self._crng = self.rng if world == 1 else np.random.default_rng([int(self._seed), rank])
             cand = self.space.rvs_transformed(hi - lo, self._crng, np.float32)
+        if self._hmap is not None:
+            cand = self._hmap.candidates(cand)
         if self.hedge:
             return self._hedge_pick(eng, cand, lo, rank, world, lie, Xt, ya)
         failed = None

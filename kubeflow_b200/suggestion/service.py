@@ -63,8 +63,8 @@ def validate_skopt_settings(settings: dict) -> dict:
                 out[name] = int(value)
             elif name in ENGINE_SETTINGS:
                 v = ENGINE_SETTINGS[name](value)
-                if name == "kernel" and v not in ("rbf", "matern52"):
-                    raise AlgorithmSettingsError(f"kernel {v} must be rbf or matern52")
+                if name == "kernel" and v not in ("rbf", "matern52", "hamming"):
+                    raise AlgorithmSettingsError(f"kernel {v} must be rbf, matern52 or hamming")
                 if name == "var_mode" and v not in ("tc", "f64", "auto"):
                     raise AlgorithmSettingsError(f"var_mode {v} must be tc, f64 or auto")
                 if name == "candidate_backend" and v not in ("torch", "numpy"):
@@ -99,7 +99,23 @@ def validate_skopt_settings(settings: dict) -> dict:
                 raise AlgorithmSettingsError(f"setting {name} cannot be combined with theta_fit skopt, which uses skopt's own start and bounds")
     elif "theta_restarts" in out:
         raise AlgorithmSettingsError("setting theta_restarts applies to theta_fit skopt only")
+    if out.get("kernel") == "hamming":   # these search the one-hot columns' length scales, which Hamming weights replace
+        for name, given in (("theta_grid", out.get("theta_grid", 1) > 1), ("theta_search", out.get("theta_search", 0) > 0),
+                            ("theta_fit", out.get("theta_fit") == "lbfgs")):
+            if given:
+                raise AlgorithmSettingsError(f"setting {name} {out[name]} cannot be combined with kernel hamming")
     return out
+
+
+def check_kernel_space(settings: dict, search_space):
+    """skopt's HammingKernel is its model of all-categorical spaces only: ``kernel: hamming`` beside a ``double`` or ``int``
+    parameter is refused, naming it."""
+    if settings.get("kernel") != "hamming":
+        return
+    from .internal import CATEGORICAL, DISCRETE
+    for p in search_space.params:
+        if p.type not in (CATEGORICAL, DISCRETE):
+            raise AlgorithmSettingsError(f"kernel hamming needs every parameter categorical or discrete: parameter {p.name} is {p.type}")
 
 
 def experiment_fingerprint(exp, search_space, settings: dict) -> tuple:
@@ -184,8 +200,8 @@ class SkoptService(_Base):
         name = experiment.spec.algorithm.algorithm_name
         if name != "bayesianoptimization":
             raise AlgorithmSettingsError(f"unknown algorithm name {name}")
-        HyperParameterSearchSpace.convert(experiment)
-        validate_skopt_settings(parse_settings(experiment))
+        search_space = HyperParameterSearchSpace.convert(experiment)
+        check_kernel_space(validate_skopt_settings(parse_settings(experiment)), search_space)
 
     def get_suggestions(self, request):
         exp = request.experiment
@@ -193,6 +209,7 @@ class SkoptService(_Base):
             raise AlgorithmSettingsError(f"unknown algorithm name {exp.spec.algorithm.algorithm_name}")
         search_space = HyperParameterSearchSpace.convert(exp)
         settings = validate_skopt_settings(parse_settings(exp))
+        check_kernel_space(settings, search_space)
         from .ingest import LazyRequest
         lazy = request if isinstance(request, LazyRequest) and request.scanned else None
         fingerprint = experiment_fingerprint(exp, search_space, settings)

@@ -25,9 +25,10 @@ LS_BOUNDS = (0.01, 100.0)             # Matern(length_scale_bounds=[(0.01, 100)]
 NOISE_BOUNDS = (1e-5, 1e5)            # WhiteKernel's default noise_level_bounds [RECALL]
 
 
-def bounds(n_dims: int) -> np.ndarray:
-    """(2 + n_dims, 2) log bounds in sklearn's θ order: log amp, log ℓ_1..n_dims, log noise."""
-    rows = [AMP_BOUNDS] + [LS_BOUNDS] * n_dims + [NOISE_BOUNDS]
+def bounds(n_dims: int, ls_bounds=LS_BOUNDS) -> np.ndarray:
+    """(2 + n_dims, 2) log bounds in sklearn's θ order: log amp, log ℓ_1..n_dims, log noise.  ``ls_bounds``: the length scales'
+    bounds (Matérn's by default; ``hamming.LS_BOUNDS`` for the HammingKernel's weights)."""
+    rows = [AMP_BOUNDS] + [ls_bounds] * n_dims + [NOISE_BOUNDS]
     return np.log(np.asarray(rows, dtype=np.float64))
 
 
@@ -37,11 +38,11 @@ def estimator_seed(random_state) -> int:
     return int(np.random.RandomState(random_state).randint(0, np.iinfo(np.int32).max))
 
 
-def starts(n_dims: int, est_seed: int, n_restarts: int) -> np.ndarray:
+def starts(n_dims: int, est_seed: int, n_restarts: int, ls_bounds=LS_BOUNDS) -> np.ndarray:
     """The initial θ of each L-BFGS-B run: the kernel's own θ = log(1, …, 1), then ``n_restarts`` draws of
     ``RandomState(est_seed).uniform(lo, hi)``, in order, as sklearn's fit draws them (it re-seeds on every fit, so a refit
     starts from the same points)."""
-    b = bounds(n_dims)
+    b = bounds(n_dims, ls_bounds)
     rng = np.random.RandomState(est_seed)
     return np.stack([np.zeros(len(b))] + [rng.uniform(b[:, 0], b[:, 1]) for _ in range(n_restarts)])
 
@@ -141,12 +142,13 @@ def _minimize(fun, x0, b, maxiter):
     return minimize(fun, x0, method="L-BFGS-B", jac=True, bounds=b, options=options)
 
 
-def fit(batch_fn, n_dims: int, est_seed: int, n_restarts: int = 2, maxiter: int | None = None, lockstep: bool = True) -> FitResult:
+def fit(batch_fn, n_dims: int, est_seed: int, n_restarts: int = 2, maxiter: int | None = None, lockstep: bool = True,
+        ls_bounds=LS_BOUNDS) -> FitResult:
     """sklearn's restart search over skopt's bounds.  ``batch_fn(list of θ) -> list of (−LML, −gradient)`` in sklearn's order
     (see ``to_objective``).  ``lockstep=False`` runs the starts one after another, one θ per call (the reference the lockstep
     must equal).  ``maxiter``: L-BFGS-B's iteration limit (None: SciPy's default)."""
-    x0s = starts(n_dims, est_seed, n_restarts)
-    b = bounds(n_dims)
+    x0s = starts(n_dims, est_seed, n_restarts, ls_bounds)
+    b = bounds(n_dims, ls_bounds)
     res = [None] * len(x0s)
     calls = 0
     if lockstep:
@@ -181,9 +183,10 @@ def fit(batch_fn, n_dims: int, est_seed: int, n_restarts: int = 2, maxiter: int 
     return FitResult(theta=per[w].theta, lml=-per[w].fun, winner=w, starts=per, batch_calls=calls)
 
 
-def engine_batch_fn(eng, X, y, scratch_limit: int | None = None):
+def engine_batch_fn(eng, X, y, scratch_limit: int | None = None, hamming=None):
     """``batch_fn`` over a GPEngine: one ``lml_grad_batch`` per round, split into calls of as many θ as the engine's scratch
-    limit holds (a θ's result does not depend on the split)."""
+    limit holds (a θ's result does not depend on the split).  ``hamming``: a ``hamming.HammingMap``; θ's length scales are then
+    the Hamming weights l_j, evaluated as RBF length scales of the one-hot columns, and the gradient is returned per l_j."""
     X = np.ascontiguousarray(X, dtype=np.float64)
     y = np.ascontiguousarray(y, dtype=np.float64).reshape(-1)
     N, D = X.shape
@@ -194,7 +197,13 @@ def engine_batch_fn(eng, X, y, scratch_limit: int | None = None):
         out = []
         for i in range(0, len(thetas), per_call):
             part = thetas[i:i + per_call]
-            lml, grad = eng.lml_grad_batch(X, y, [theta_dict(t) for t in part])
+            ths = [theta_dict(t) for t in part]
+            if hamming is not None:
+                for th in ths:
+                    th["length_scale"] = hamming.length_scale(th["length_scale"])
+            lml, grad = eng.lml_grad_batch(X, y, ths)
+            if hamming is not None:
+                grad = [np.concatenate([g[:2], hamming.grad(g[2:])]) for g in grad]
             out += [to_objective(v, g, float(np.exp(t[-1]))) for v, g, t in zip(lml, grad, part)]
         return out
     return batch_fn
