@@ -18,7 +18,7 @@ int kbo_create(kbo_handle** out, int device) {
   if (cudaSetDevice(device) != cudaSuccess) return KBO_ERR_CUDA;
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return KBO_ERR_CUDA;
-  kbo_handle* h = new (std::nothrow) kbo_handle();
+  std::unique_ptr<kbo_handle> h(new (std::nothrow) kbo_handle());
   if (!h) return KBO_ERR_NOMEM;
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
@@ -26,27 +26,19 @@ int kbo_create(kbo_handle** out, int device) {
     // sm_90a cubin only: refuse politely instead of failing at the first launch
     h->err = "libkbo is built for sm_90a (H100) only";
   }
-  for (auto& ev : h->ev) cudaEventCreate(&ev);
-  *out = h;
+  KBO_TRY(h->ev.create());
+  *out = h.release();
   return KBO_OK;
 }
 
+// Device memory and the fixed events go with `delete h`; what has to be torn down in order (the communicator, streams,
+// green contexts and the events the fit and sweep create on demand) is released here first.
 void kbo_destroy(kbo_handle* h) {
   if (!h) return;
   cudaSetDevice(h->device);
   kbo_comm_destroy(h);
   kbo_i_lml_batch_free(h);
   if (h->lml_ev) cudaEventDestroy(h->lml_ev);
-  DevBuf* bufs[] = {&h->d_inv_ls, &h->Xs, &h->nx, &h->yn, &h->K, &h->W, &h->Linv, &h->T, &h->alpha, &h->z, &h->Wh, &h->Wl,
-                    &h->scal, &h->info, &h->stage_X, &h->stage_y, &h->stage_Xc, &h->Ks64, &h->Ksh, &h->Ksl, &h->mun, &h->part, &h->varn,
-                    &h->blockbest, &h->best, &h->XsT, &h->refine, &h->refine_x, &h->yraw, &h->lrow, &h->var_cal,
-                    &h->ks_center, &h->ks_Xh, &h->ks_Xl, &h->ks_nxal, &h->ks_Ch, &h->ks_Cl, &h->ks_nc, &h->rk_part, &h->cal_idx, &h->cal_x, &h->cal_mu,
-                    &h->comm_buf, &h->T2, &h->Linv4, &h->mu_part, &h->sv_B, &h->sv_V, &h->sv_bar, &h->zf, &h->lml_yn, &h->lml_scal, &h->rk_sched[0].dev, &h->rk_sched[1].dev, &h->rk_sched[2].dev, &h->rk_sched[3].dev, &h->rk_sched[4].dev, &h->rk_sched[5].dev,
-                    &h->rk_sched[6].dev, &h->rk_sched[7].dev, &h->pr_list, &h->pr_x, &h->pr_mu, &h->pr_var, &h->cal_mu_rk, &h->cal_var_rk, &h->un_idx, &h->un_mv};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  for (auto& ev : h->ev)
-    if (ev) cudaEventDestroy(ev);
   for (auto& e : h->ev_panel) cudaEventDestroy(e);
   if (h->ev_gram) cudaEventDestroy(h->ev_gram);
   kbo_i_fit_partition_free(h);
@@ -430,8 +422,9 @@ int kbo_debug_fp64_peak(kbo_handle* h, double* tflops_out) {
   if (!h || !tflops_out) return KBO_ERR_INVALID;
   cudaSetDevice(h->device);
   const int iters = 20000, ctas = h->sm_count;
-  double* out = nullptr;
-  KBO_CUDA(h, cudaMalloc(&out, sizeof(double) * (size_t)ctas * 256));
+  DevBuf buf;
+  KBO_TRY(kbo_reserve(h, buf, sizeof(double) * (size_t)ctas * 256));
+  double* out = (double*)buf.p;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
@@ -456,7 +449,6 @@ int kbo_debug_fp64_peak(kbo_handle* h, double* tflops_out) {
   }
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
-  cudaFree(out);
   KBO_CUDA(h, cudaGetLastError());
   *tflops_out = peak;
   return KBO_OK;

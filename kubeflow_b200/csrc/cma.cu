@@ -585,13 +585,26 @@ static int cma_configure(kbo_handle* h, kbo_cma* c, int lambda, double sigma0) {
   c->term = 10 + (30 * n + lambda - 1) / lambda;   // 10 + ⌈30·n/λ⌉
   c->tolx = 1e-12 * sigma0;
   const size_t LD = (size_t)lambda * D, LPD = (size_t)c->lam_pad * D;
-  int r = KBO_OK;
-  auto R_ = [&](DevBuf& b, size_t bytes) { if (r == KBO_OK) r = kbo_reserve(h, b, bytes); };
-  R_(c->mean, 8 * D); R_(c->C, 8 * (size_t)D * D); R_(c->B, 8 * (size_t)D * D); R_(c->Dv, 8 * D); R_(c->ps, 8 * D); R_(c->pc, 8 * D);
-  R_(c->weights, 8 * lambda); R_(c->Z, 8 * (LD + 2)); R_(c->Zs, 8 * LD); R_(c->Y, 8 * LD); R_(c->Ys, 8 * LPD); R_(c->YwT, 8 * LPD);
-  R_(c->zn2, 8 * lambda); R_(c->order, 4 * lambda); R_(c->R, 8 * (size_t)D * D * (c->lam_pad / 256)); R_(c->G, 8 * (size_t)D * D); R_(c->scal, 8 * CS_COUNT);
-  R_(c->yw, 8 * D); R_(c->hist, 8 * 2 * (size_t)c->term); R_(c->flags, 4);
-  if (r != KBO_OK) return r;
+  KBO_TRY(kbo_reserve(h, c->mean, 8 * D));
+  KBO_TRY(kbo_reserve(h, c->C, 8 * (size_t)D * D));
+  KBO_TRY(kbo_reserve(h, c->B, 8 * (size_t)D * D));
+  KBO_TRY(kbo_reserve(h, c->Dv, 8 * D));
+  KBO_TRY(kbo_reserve(h, c->ps, 8 * D));
+  KBO_TRY(kbo_reserve(h, c->pc, 8 * D));
+  KBO_TRY(kbo_reserve(h, c->weights, 8 * lambda));
+  KBO_TRY(kbo_reserve(h, c->Z, 8 * (LD + 2)));
+  KBO_TRY(kbo_reserve(h, c->Zs, 8 * LD));
+  KBO_TRY(kbo_reserve(h, c->Y, 8 * LD));
+  KBO_TRY(kbo_reserve(h, c->Ys, 8 * LPD));
+  KBO_TRY(kbo_reserve(h, c->YwT, 8 * LPD));
+  KBO_TRY(kbo_reserve(h, c->zn2, 8 * lambda));
+  KBO_TRY(kbo_reserve(h, c->order, 4 * lambda));
+  KBO_TRY(kbo_reserve(h, c->R, 8 * (size_t)D * D * (c->lam_pad / 256)));
+  KBO_TRY(kbo_reserve(h, c->G, 8 * (size_t)D * D));
+  KBO_TRY(kbo_reserve(h, c->scal, 8 * CS_COUNT));
+  KBO_TRY(kbo_reserve(h, c->yw, 8 * D));
+  KBO_TRY(kbo_reserve(h, c->hist, 8 * 2 * (size_t)c->term));
+  KBO_TRY(kbo_reserve(h, c->flags, 4));
   KBO_CUDA(h, cudaMemcpy(c->weights.p, w.data(), 8 * lambda, cudaMemcpyHostToDevice));
   return KBO_OK;
 }
@@ -620,18 +633,16 @@ int kbo_cma_create(kbo_handle* h, kbo_cma** out, int32_t D, int32_t lambda, cons
   if (lambda < 4 || lambda > 8192) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: 4 <= lambda <= 8192 supported (got %d)", lambda);
   if (!mean0 || !(sigma0 > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_create: mean0 must be given and sigma0 > 0");
   KBO_CUDA(h, cudaSetDevice(h->device));
-  kbo_cma* c = new (std::nothrow) kbo_cma();
+  std::unique_ptr<kbo_cma> c(new (std::nothrow) kbo_cma());
   if (!c) return KBO_ERR_NOMEM;
   c->D = D;
   c->seed = seed;
-  int r = cma_configure(h, c, lambda, sigma0);
-  if (r != KBO_OK) { kbo_cma_destroy(c); return r; }
+  KBO_TRY(cma_configure(h, c.get(), lambda, sigma0));
   cudaFuncSetAttribute(cma_jacobi_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * CMA_MAXD * (CMA_MAXD + 1)));
   cudaFuncSetAttribute(cma_jacobi_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(sizeof(double) * CMA_MAXD * (CMA_MAXD + 1)));
   cudaFuncSetAttribute(cma_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 12);
-  r = cma_start_run(h, c, mean0, sigma0);
-  if (r != KBO_OK) { kbo_cma_destroy(c); return r; }
-  *out = c;
+  KBO_TRY(cma_start_run(h, c.get(), mean0, sigma0));
+  *out = c.release();
   return KBO_OK;
 }
 
@@ -656,12 +667,7 @@ int kbo_cma_stop_flags(kbo_handle* h, kbo_cma* c, uint32_t* flags_host, double* 
 }
 
 void kbo_cma_destroy(kbo_cma* c) {
-  if (!c) return;
-  DevBuf* bufs[] = {&c->mean, &c->C, &c->B, &c->Dv, &c->ps, &c->pc, &c->weights, &c->Z, &c->Zs, &c->Y, &c->Ys, &c->YwT, &c->zn2, &c->order,
-                    &c->R, &c->G, &c->scal, &c->yw, &c->hist, &c->flags};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  delete c;
+  if (c) delete c;
 }
 
 int kbo_cma_ask(kbo_handle* h, kbo_cma* c, double* X_dev, const double* z_in_dev, void* stream) {
@@ -700,7 +706,7 @@ int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32
   if (!h || !c) return KBO_ERR_INVALID;
   if (fitness_kind < 0 || fitness_kind > 1 || generations < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_run_synthetic: bad argument");
   cudaStream_t s = 0;
-  DevBuf X{}, f{};
+  DevBuf X, f;
   KBO_TRY(kbo_reserve(h, X, 8 * (size_t)c->lambda * c->D));
   KBO_TRY(kbo_reserve(h, f, 8 * (size_t)c->lambda));
   cudaEventRecord(h->ev[5], s);
@@ -716,8 +722,6 @@ int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32
   double sc[CS_COUNT];
   cudaMemcpyAsync(sc, c->scal.p, sizeof sc, cudaMemcpyDeviceToHost, s);
   cudaError_t e = cudaStreamSynchronize(s);
-  cudaFree(X.p);
-  cudaFree(f.p);
   if (r != KBO_OK) return r;
   if (e != cudaSuccess) KBO_FAIL(h, KBO_ERR_CUDA, "kbo_cma_run_synthetic: %s", cudaGetErrorString(e));
   if (best_f_host) *best_f_host = sc[CS_BEST_F];

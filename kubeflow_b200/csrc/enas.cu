@@ -665,7 +665,7 @@ struct kbo_enas {
   EnCfg cf{};
   DevBuf par, mom, var, dev, scr, sscr;
   EnBufs bf{};
-  cudaEvent_t ev[4] = {};
+  EventSet<4> ev;
   float last_ms[2] = {};
   long long step = 0;                   // host copy of the Adam step count (the kernel's β2^t starts from it)
 };
@@ -693,6 +693,24 @@ static int en_carve_scratch(kbo_handle* h, kbo_enas* e, cudaStream_t s) {
   return KBO_OK;
 }
 
+// The controller's buffers, events and initial parameters (uniform in [-0.1, 0.1)), with the work queued on cs.
+static int en_setup(kbo_handle* h, kbo_enas* e, cudaStream_t cs) {
+  const long long o = e->cf.n_par;
+  KBO_TRY(kbo_reserve(h, e->par, 4 * (size_t)o));
+  KBO_TRY(kbo_reserve(h, e->mom, 4 * (size_t)o));
+  KBO_TRY(kbo_reserve(h, e->var, 4 * (size_t)o));
+  KBO_TRY(kbo_reserve(h, e->dev, sizeof(EnDev)));
+  KBO_TRY(en_carve_scratch(h, e, cs));
+  KBO_TRY(e->ev.create());
+  const EnDev d0{0.f, 0, 0, 0};
+  KBO_CUDA(h, cudaMemsetAsync(e->mom.p, 0, 4 * (size_t)o, cs));
+  KBO_CUDA(h, cudaMemsetAsync(e->var.p, 0, 4 * (size_t)o, cs));
+  KBO_CUDA(h, cudaMemcpyAsync(e->dev.p, &d0, sizeof d0, cudaMemcpyHostToDevice, cs));
+  enas_init_kernel<<<(int)std::min<long long>((o + 255) / 256, 1024), 256, 0, cs>>>((float*)e->par.p, o, e->cf.k0, e->cf.k1);
+  KBO_CUDA(h, cudaGetLastError());
+  return KBO_OK;
+}
+
 extern "C" {
 
 int kbo_enas_create(kbo_handle* h, kbo_enas** out, int32_t L, int32_t H, int32_t n_ops, const kbo_enas_settings* s, uint64_t seed) {
@@ -707,7 +725,7 @@ int kbo_enas_create(kbo_handle* h, kbo_enas** out, int32_t L, int32_t H, int32_t
   if (!(s->entropy_weight >= 0.0) || !(s->skip_weight >= 0.0) || !std::isfinite(s->temperature) || !std::isfinite(s->tanh_const))
     KBO_FAIL(h, KBO_ERR_INVALID, "kbo_enas_create: entropy_weight and skip_weight must be >= 0, temperature and tanh_const finite");
   KBO_CUDA(h, cudaSetDevice(h->device));
-  kbo_enas* e = new (std::nothrow) kbo_enas();
+  std::unique_ptr<kbo_enas> e(new (std::nothrow) kbo_enas());
   if (!e) return KBO_ERR_NOMEM;
   EnCfg& c = e->cf;
   c.L = L;
@@ -737,22 +755,7 @@ int kbo_enas_create(kbo_handle* h, kbo_enas** out, int32_t L, int32_t H, int32_t
   // set-up work runs on a private non-blocking stream, so creating a controller never waits on (or stalls) other work
   // on the device
   cudaStream_t cs = nullptr;
-  int r = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess ? KBO_OK : KBO_ERR_CUDA;
-  if (r == KBO_OK) r = kbo_reserve(h, e->par, 4 * (size_t)o);
-  if (r == KBO_OK) r = kbo_reserve(h, e->mom, 4 * (size_t)o);
-  if (r == KBO_OK) r = kbo_reserve(h, e->var, 4 * (size_t)o);
-  if (r == KBO_OK) r = kbo_reserve(h, e->dev, sizeof(EnDev));
-  if (r == KBO_OK) r = en_carve_scratch(h, e, cs);
-  for (auto& ev : e->ev)
-    if (r == KBO_OK && cudaEventCreate(&ev) != cudaSuccess) r = KBO_ERR_CUDA;
-  const EnDev d0{0.f, 0, 0, 0};
-  if (r == KBO_OK && (cudaMemsetAsync(e->mom.p, 0, 4 * (size_t)o, cs) != cudaSuccess || cudaMemsetAsync(e->var.p, 0, 4 * (size_t)o, cs) != cudaSuccess ||
-                      cudaMemcpyAsync(e->dev.p, &d0, sizeof d0, cudaMemcpyHostToDevice, cs) != cudaSuccess))
-    r = KBO_ERR_CUDA;
-  if (r == KBO_OK) {
-    enas_init_kernel<<<(int)std::min<long long>((o + 255) / 256, 1024), 256, 0, cs>>>((float*)e->par.p, o, c.k0, c.k1);
-    if (cudaGetLastError() != cudaSuccess) r = KBO_ERR_CUDA;
-  }
+  int r = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking) == cudaSuccess ? en_setup(h, e.get(), cs) : KBO_ERR_CUDA;
   if (cs) {
     if (cudaStreamSynchronize(cs) != cudaSuccess && r == KBO_OK) r = KBO_ERR_CUDA;
     cudaStreamDestroy(cs);
@@ -765,23 +768,14 @@ int kbo_enas_create(kbo_handle* h, kbo_enas** out, int32_t L, int32_t H, int32_t
                       cudaFuncSetAttribute(enas_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                            (int)en_smem_bytes(EN_SB, EN_MAXL, EN_MAXH, EN_MAXOPS)) != cudaSuccess))
     r = KBO_ERR_CUDA;
-  if (r != KBO_OK) {
-    kbo_enas_destroy(e);
-    if (r == KBO_ERR_CUDA) KBO_FAIL(h, r, "kbo_enas_create: CUDA setup failed");
-    return r;
-  }
-  *out = e;
+  if (r == KBO_ERR_CUDA) KBO_FAIL(h, r, "kbo_enas_create: CUDA setup failed");
+  KBO_TRY(r);
+  *out = e.release();
   return KBO_OK;
 }
 
 void kbo_enas_destroy(kbo_enas* e) {
-  if (!e) return;
-  DevBuf* bufs[] = {&e->par, &e->mom, &e->var, &e->dev, &e->scr, &e->sscr};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  for (auto& ev : e->ev)
-    if (ev) cudaEventDestroy(ev);
-  delete e;
+  if (e) delete e;
 }
 
 int kbo_enas_train(kbo_handle* h, kbo_enas* e, double reward, int32_t steps, const int32_t* arcs, float* stats, void* stream) {

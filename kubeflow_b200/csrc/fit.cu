@@ -1344,11 +1344,8 @@ int kbo_i_lml_grad_batch(kbo_handle* h, const double* X_dev, const double* y_dev
 void kbo_i_lml_batch_free(kbo_handle* h) {
   auto* lanes = (std::vector<LmlLane>*)h->lml_lanes;
   if (!lanes) return;
-  for (auto& L : *lanes) {
-    for (DevBuf* b : {&L.K, &L.Xs, &L.XsT, &L.nx, &L.inv_ls, &L.Linv, &L.info, &L.out, &L.W, &L.T, &L.z, &L.alpha, &L.part})
-      if (b->p) cudaFree(b->p);
+  for (auto& L : *lanes)
     if (L.s) cudaStreamDestroy(L.s);
-  }
   delete lanes;
   h->lml_lanes = nullptr;
 }

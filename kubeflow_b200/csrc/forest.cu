@@ -53,7 +53,7 @@ struct kbo_forest {
   std::vector<long long> h_off;
   size_t max_tree_bytes = 0;
   float last_ms[2] = {0.f, 0.f};     // fit, sweep
-  cudaEvent_t ev[4] = {};
+  EventSet<4> ev;
 };
 
 struct ForestPart {
@@ -679,27 +679,19 @@ int kbo_forest_create(kbo_handle* h, kbo_forest** out, int32_t kind, int32_t n_t
   if (n_trees < 1 || n_trees > FOREST_MAX_T) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_create: 1 <= n_trees <= %d (got %d)", FOREST_MAX_T, n_trees);
   if (min_samples_leaf < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_create: min_samples_leaf must be >= 1 (got %d)", min_samples_leaf);
   KBO_CUDA(h, cudaSetDevice(h->device));
-  kbo_forest* f = new (std::nothrow) kbo_forest();
+  std::unique_ptr<kbo_forest> f(new (std::nothrow) kbo_forest());
   if (!f) return KBO_ERR_NOMEM;
   f->kind = kind;
   f->T = n_trees;
   f->msl = min_samples_leaf;
   f->seed = seed;
-  for (auto& e : f->ev) cudaEventCreate(&e);
-  *out = f;
+  KBO_TRY(f->ev.create());
+  *out = f.release();
   return KBO_OK;
 }
 
 void kbo_forest_destroy(kbo_forest* f) {
-  if (!f) return;
-  DevBuf* bufs[] = {&f->X, &f->y, &f->cnt, &f->keys, &f->keys2, &f->order, &f->order_in, &f->seg, &f->sort_tmp, &f->cols, &f->tmp, &f->side,
-                    &f->nstart, &f->nend, &f->flag, &f->feat, &f->thr, &f->left, &f->right, &f->value, &f->imp, &f->nns, &f->wn,
-                    &f->nnodes, &f->nleaves, &f->blob, &f->tree_off, &f->part, &f->ex_mn, &f->ex_mx};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  for (auto& e : f->ev)
-    if (e) cudaEventDestroy(e);
-  delete f;
+  if (f) delete f;
 }
 
 int kbo_forest_fit(kbo_handle* h, kbo_forest* f, const float* X, const double* y, int32_t N, int32_t D, const int32_t* counts, void* stream) {

@@ -6,6 +6,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -13,9 +14,49 @@
 
 #define KBO_NB 64  // Cholesky / trtri block size (one diagonal block = one CTA in shared memory)
 
+// A device allocation owned by its holder: freed when the holder is destroyed, grown only by kbo_reserve.
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf& operator=(DevBuf&& o) noexcept {
+    if (this != &o) {
+      if (p) cudaFree(p);
+      p = o.p;
+      cap = o.cap;
+      o.p = nullptr;
+      o.cap = 0;
+    }
+    return *this;
+  }
+  ~DevBuf() {
+    if (p) cudaFree(p);
+  }
+};
+
+// The fixed timing events of one object: create() makes all of them, the destructor destroys them.
+template <int N>
+struct EventSet {
+  cudaEvent_t e[N] = {};
+  EventSet() = default;
+  EventSet(const EventSet&) = delete;
+  EventSet& operator=(const EventSet&) = delete;
+  ~EventSet() {
+    for (cudaEvent_t x : e)
+      if (x) cudaEventDestroy(x);
+  }
+  int create() {
+    for (cudaEvent_t& x : e)
+      if (cudaEventCreate(&x) != cudaSuccess) {
+        x = nullptr;
+        return KBO_ERR_CUDA;
+      }
+    return KBO_OK;
+  }
+  cudaEvent_t operator[](int i) const { return e[i]; }
 };
 
 struct kbo_handle {
@@ -54,7 +95,7 @@ struct kbo_handle {
   bool tc_fast = true;      // array-free tensor-core sweeps rank with ONE fp16 product and let the FP64 refinement decide
   DevBuf var_cal;           // three-product variance of the calibration rows
   kbo_timings tim{};
-  cudaEvent_t ev[8] = {};
+  EventSet<8> ev;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_var, ev_cross, ev_acq, ev_cal;
   size_t ev_var_used = 0, ev_cross_used = 0, ev_acq_used = 0, ev_cal_used = 0;
   int launches = 0;
@@ -164,6 +205,12 @@ static inline int kbo_reserve(kbo_handle* h, DevBuf& b, size_t bytes) {
     int _r = (expr);           \
     if (_r != KBO_OK) return _r; \
   } while (0)
+// bytes of host data into b (at least 4 bytes reserved, so an empty list still has a device pointer)
+static inline int kbo_upload(kbo_handle* h, DevBuf& b, const void* host, size_t bytes) {
+  KBO_TRY(kbo_reserve(h, b, bytes > 4 ? bytes : 4));
+  if (bytes) KBO_CUDA(h, cudaMemcpy(b.p, host, bytes, cudaMemcpyHostToDevice));
+  return KBO_OK;
+}
 
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 static inline int64_t round_up64(int64_t x, int64_t m) { return (x + m - 1) / m * m; }

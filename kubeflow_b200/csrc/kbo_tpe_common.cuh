@@ -1,8 +1,11 @@
-// Device code shared by the Parzen-estimator samplers: tpe.cu (hyperopt's tpe.suggest) and mvtpe.cu (Optuna's multivariate
+// Code shared by the Parzen-estimator samplers: tpe.cu (hyperopt's tpe.suggest) and mvtpe.cu (Optuna's multivariate
 // TPESampler).  Loss keys in NumPy's order and the below / above split, the truncated-normal inverse-CDF draw, first-index
-// argmax bookkeeping, block reductions and the MUFU exponential.
+// argmax bookkeeping, block reductions and the MUFU exponential; on the host, the told history's append.
 #pragma once
 #include <stdint.h>
+#include <algorithm>
+
+#include "kbo_internal.cuh"
 
 #define TPE_LF 25  // hyperopt's DEFAULT_LF and Optuna's ramp length: linear forgetting, and the cap on n_below
 
@@ -145,4 +148,30 @@ static __global__ void tpe_group_kernel(const int* __restrict__ below, int nb, i
   }
   grp[i] = isb ? 0 : 1;
   pos[i] = isb ? c : i - c;
+}
+
+// ---- the told history (host) -----------------------------------------------------------------------------------------
+// Queues the copy of n_new trials (D values and one loss each) into rows t->n .. t->n + n_new - 1 of t->vals / t->loss on s,
+// growing both by doubling first.  Rows already told survive a failed growth; t->n is left for the caller to advance.
+template <class Sampler>
+static int tpe_history_append(kbo_handle* h, Sampler* t, const double* X, const double* loss, int n_new, int on_host, cudaStream_t s) {
+  const size_t D = t->D;
+  if (t->n + n_new > t->cap) {
+    const int cap = std::max({2 * t->cap, t->n + n_new, 64});
+    DevBuf v, l;
+    KBO_TRY(kbo_reserve(h, v, 8 * D * cap));
+    KBO_TRY(kbo_reserve(h, l, 8 * (size_t)cap));
+    if (t->n) {
+      KBO_CUDA(h, cudaMemcpyAsync(v.p, t->vals.p, 8 * D * t->n, cudaMemcpyDeviceToDevice, s));
+      KBO_CUDA(h, cudaMemcpyAsync(l.p, t->loss.p, 8 * (size_t)t->n, cudaMemcpyDeviceToDevice, s));
+      KBO_CUDA(h, cudaStreamSynchronize(s));
+    }
+    t->vals = std::move(v);
+    t->loss = std::move(l);
+    t->cap = cap;
+  }
+  const cudaMemcpyKind kind = on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+  KBO_CUDA(h, cudaMemcpyAsync((double*)t->vals.p + D * t->n, X, 8 * D * n_new, kind, s));
+  KBO_CUDA(h, cudaMemcpyAsync((double*)t->loss.p + t->n, loss, 8 * (size_t)n_new, kind, s));
+  return KBO_OK;
 }

@@ -78,7 +78,7 @@ struct kbo_mvtpe {
   DevBuf idx, w, c64, c2, mu32, dv, sg, fs, tab32, tab64, hdr;
   DevBuf draws, prior, sc, lb, surv, bb;
   std::vector<int> last_surv;
-  cudaEvent_t ev[5] = {};
+  EventSet<5> ev;
   float last_ms[4] = {};
 };
 
@@ -698,12 +698,6 @@ static int mv_build(kbo_handle* h, kbo_mvtpe* t, cudaStream_t s) {
   return KBO_OK;
 }
 
-static int mv_upload(kbo_handle* h, DevBuf& b, const void* v, size_t bytes) {
-  KBO_TRY(kbo_reserve(h, b, std::max<size_t>(bytes, 4)));
-  if (bytes) KBO_CUDA(h, cudaMemcpy(b.p, v, bytes, cudaMemcpyHostToDevice));
-  return KBO_OK;
-}
-
 extern "C" {
 
 int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* kinds, const double* lo, const double* hi, const double* q,
@@ -713,7 +707,7 @@ int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* k
   if (D < 1 || D > MV_MAXD) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: 1 <= D <= %d supported (got %d)", MV_MAXD, D);
   if (!kinds) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: null kinds");
   KBO_CUDA(h, cudaSetDevice(h->device));
-  kbo_mvtpe* t = new (std::nothrow) kbo_mvtpe();
+  std::unique_ptr<kbo_mvtpe> t(new (std::nothrow) kbo_mvtpe());
   if (!t) return KBO_ERR_NOMEM;
   t->D = D;
   t->seed = seed;
@@ -725,7 +719,7 @@ int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* k
     P.kind = kinds[d];
     P.tab = -1;
     if (P.kind == KBO_MVTPE_CAT) {
-      if (!levels || levels[d] < 1) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: a categorical needs >= 1 categories", d); }
+      if (!levels || levels[d] < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: a categorical needs >= 1 categories", d);
       P.levels = levels[d];
       P.slot = t->Dd++;
       t->dsc.push_back(d);
@@ -734,20 +728,18 @@ int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* k
       P.b = std::log(a + 1.0) - std::log(a);
       continue;
     }
-    if (P.kind != KBO_MVTPE_FLOAT && P.kind != KBO_MVTPE_INT) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: unknown kind %d", d, kinds[d]); }
-    if (!lo || !hi || !std::isfinite(lo[d]) || !std::isfinite(hi[d]) || !(lo[d] <= hi[d]) || (P.kind == KBO_MVTPE_FLOAT && !(lo[d] < hi[d]))) {
-      delete t;
+    if (P.kind != KBO_MVTPE_FLOAT && P.kind != KBO_MVTPE_INT) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: unknown kind %d", d, kinds[d]);
+    if (!lo || !hi || !std::isfinite(lo[d]) || !std::isfinite(hi[d]) || !(lo[d] <= hi[d]) || (P.kind == KBO_MVTPE_FLOAT && !(lo[d] < hi[d])))
       KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: need finite lo < hi (lo <= hi for an integer)", d);
-    }
     P.lo = lo[d];
     P.hi = hi[d];
     P.lo2 = P.lo;
     P.hi2 = P.hi;
     if (P.kind == KBO_MVTPE_INT) {
-      if (!q || !(q[d] > 0.0) || !std::isfinite(q[d])) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: step must be > 0", d); }
+      if (!q || !(q[d] > 0.0) || !std::isfinite(q[d])) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: step must be > 0", d);
       P.q = q[d];
       const double L = std::floor((P.hi - P.lo) / P.q) + 1.0;
-      if (!(L >= 1.0 && L < 2147483647.0)) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: too many levels", d); }
+      if (!(L >= 1.0 && L < 2147483647.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_create: parameter %d: too many levels", d);
       P.levels = (int)L;
       P.hi = P.lo + (double)(P.levels - 1) * P.q;
       P.lo2 = P.lo - 0.5 * P.q;
@@ -768,31 +760,18 @@ int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* k
     P.ps = P.hi2 - P.lo2;
     P.lpm = lpm;
   }
-  int r = mv_upload(h, t->d_prm, t->prm.data(), sizeof(MvParam) * D);
-  if (r == KBO_OK) r = mv_upload(h, t->d_flt, t->flt.data(), 4 * t->flt.size());
-  if (r == KBO_OK) r = mv_upload(h, t->d_dsc, t->dsc.data(), 4 * t->dsc.size());
-  if (r == KBO_OK) r = mv_upload(h, t->d_tabd, t->tabd.data(), 4 * t->tabd.size());
-  if (r == KBO_OK) r = kbo_reserve(h, t->err, 4);
-  for (auto& e : t->ev)
-    if (r == KBO_OK && cudaEventCreate(&e) != cudaSuccess) r = KBO_ERR_CUDA;
-  if (r != KBO_OK) {
-    kbo_mvtpe_destroy(t);
-    return r;
-  }
-  *out = t;
+  KBO_TRY(kbo_upload(h, t->d_prm, t->prm.data(), sizeof(MvParam) * D));
+  KBO_TRY(kbo_upload(h, t->d_flt, t->flt.data(), 4 * t->flt.size()));
+  KBO_TRY(kbo_upload(h, t->d_dsc, t->dsc.data(), 4 * t->dsc.size()));
+  KBO_TRY(kbo_upload(h, t->d_tabd, t->tabd.data(), 4 * t->tabd.size()));
+  KBO_TRY(kbo_reserve(h, t->err, 4));
+  KBO_TRY(t->ev.create());
+  *out = t.release();
   return KBO_OK;
 }
 
 void kbo_mvtpe_destroy(kbo_mvtpe* t) {
-  if (!t) return;
-  DevBuf* bufs[] = {&t->d_prm, &t->d_flt, &t->d_dsc, &t->d_tabd, &t->vals, &t->loss, &t->err, &t->lkey, &t->lkey2, &t->lidx, &t->lidx2,
-                    &t->below, &t->grp, &t->pos, &t->tmp, &t->idx, &t->w, &t->c64, &t->c2, &t->mu32, &t->dv, &t->sg, &t->fs, &t->tab32,
-                    &t->tab64, &t->hdr, &t->draws, &t->prior, &t->sc, &t->lb, &t->surv, &t->bb};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  for (auto& e : t->ev)
-    if (e) cudaEventDestroy(e);
-  delete t;
+  if (t) delete t;
 }
 
 int kbo_mvtpe_tell(kbo_handle* h, kbo_mvtpe* t, const double* X, const double* loss, int32_t n_new, int on_host, void* stream) {
@@ -803,29 +782,9 @@ int kbo_mvtpe_tell(kbo_handle* h, kbo_mvtpe* t, const double* X, const double* l
   if ((int64_t)t->n + n_new > (1 << 24)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_tell: at most 2^24 trials supported");
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
-  const size_t D = t->D;
-  if (t->n + n_new > t->cap) {   // grow (doubling), keeping the rows already told
-    const int cap = std::max({2 * t->cap, t->n + n_new, 64});
-    DevBuf v{}, l{};
-    KBO_TRY(kbo_reserve(h, v, 8 * D * cap));
-    int r = kbo_reserve(h, l, 8 * (size_t)cap);
-    if (r != KBO_OK) { cudaFree(v.p); return r; }
-    if (t->n) {
-      cudaMemcpyAsync(v.p, t->vals.p, 8 * D * t->n, cudaMemcpyDeviceToDevice, s);
-      cudaMemcpyAsync(l.p, t->loss.p, 8 * (size_t)t->n, cudaMemcpyDeviceToDevice, s);
-      cudaStreamSynchronize(s);
-    }
-    if (t->vals.p) cudaFree(t->vals.p);
-    if (t->loss.p) cudaFree(t->loss.p);
-    t->vals = v;
-    t->loss = l;
-    t->cap = cap;
-  }
-  const cudaMemcpyKind kind = on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-  double* Xn = (double*)t->vals.p + D * t->n;
-  double* Ln = (double*)t->loss.p + t->n;
-  KBO_CUDA(h, cudaMemcpyAsync(Xn, X, 8 * D * n_new, kind, s));
-  KBO_CUDA(h, cudaMemcpyAsync(Ln, loss, 8 * (size_t)n_new, kind, s));
+  KBO_TRY(tpe_history_append(h, t, X, loss, n_new, on_host, s));
+  const double* Xn = (const double*)t->vals.p + (size_t)t->D * t->n;   // the new rows: checked before n counts them
+  const double* Ln = (const double*)t->loss.p + t->n;
   KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, 4, s));
   mvtpe_check_kernel<<<(n_new + 255) / 256, 256, 0, s>>>((const MvParam*)t->d_prm.p, t->D, Xn, Ln, n_new, (int*)t->err.p);
   KBO_LAUNCH_CHECK(h);

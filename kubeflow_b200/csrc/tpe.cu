@@ -67,7 +67,7 @@ struct kbo_tpe {
   DevBuf w, mu, sg, lc, f4, cdf, hdr, cat_p, cat_sc, cat_cum;
   DevBuf draws, sc, lb, surv, bb, first, err;
   std::vector<int> last_surv;
-  cudaEvent_t ev[6] = {};
+  EventSet<6> ev;
   float last_ms[5] = {};
 };
 
@@ -624,12 +624,6 @@ static int tpe_build(kbo_handle* h, kbo_tpe* t, cudaStream_t s) {
   return KBO_OK;
 }
 
-static int upload_list(kbo_handle* h, DevBuf& b, const std::vector<int>& v) {
-  KBO_TRY(kbo_reserve(h, b, 4 * std::max<size_t>(v.size(), 1)));
-  if (!v.empty()) KBO_CUDA(h, cudaMemcpy(b.p, v.data(), 4 * v.size(), cudaMemcpyHostToDevice));
-  return KBO_OK;
-}
-
 extern "C" {
 
 int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds, const double* lo, const double* hi, const double* q,
@@ -641,7 +635,7 @@ int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds
   if (!(gamma > 0.0 && gamma < 1.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: gamma must be in (0, 1) (got %g)", gamma);
   if (!(prior_weight > 0.0) || !std::isfinite(prior_weight)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: prior_weight must be > 0 (got %g)", prior_weight);
   KBO_CUDA(h, cudaSetDevice(h->device));
-  kbo_tpe* t = new (std::nothrow) kbo_tpe();
+  std::unique_ptr<kbo_tpe> t(new (std::nothrow) kbo_tpe());
   if (!t) return KBO_ERR_NOMEM;
   t->D = D;
   t->gamma = gamma;
@@ -653,7 +647,7 @@ int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds
     memset(&P, 0, sizeof P);
     P.kind = kinds[d];
     if (P.kind == KBO_TPE_CHOICE) {
-      if (!levels || levels[d] < 1) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: a choice needs >= 1 categories", d); }
+      if (!levels || levels[d] < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: a choice needs >= 1 categories", d);
       P.levels = levels[d];
       P.slot = t->Dcat++;
       t->cat.push_back(d);
@@ -662,11 +656,9 @@ int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds
       if (P.levels <= TPE_LCAP) t->lt = std::max(t->lt, P.levels);
       continue;
     }
-    if (P.kind != KBO_TPE_UNIFORM && P.kind != KBO_TPE_QUNIFORM) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: unknown kind %d", d, kinds[d]); }
-    if (!lo || !hi || !std::isfinite(lo[d]) || !std::isfinite(hi[d]) || !(lo[d] < hi[d])) {
-      delete t;
+    if (P.kind != KBO_TPE_UNIFORM && P.kind != KBO_TPE_QUNIFORM) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: unknown kind %d", d, kinds[d]);
+    if (!lo || !hi || !std::isfinite(lo[d]) || !std::isfinite(hi[d]) || !(lo[d] < hi[d]))
       KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: need finite lo < hi", d);
-    }
     P.lo = lo[d];
     P.hi = hi[d];
     P.pm = 0.5 * (P.hi + P.lo);
@@ -674,11 +666,11 @@ int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds
     P.slot = t->Dnum++;
     t->num.push_back(d);
     if (P.kind == KBO_TPE_QUNIFORM) {
-      if (!q || !(q[d] > 0.0) || !std::isfinite(q[d])) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: q must be > 0", d); }
+      if (!q || !(q[d] > 0.0) || !std::isfinite(q[d])) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: q must be > 0", d);
       P.q = q[d];
       P.base = std::nearbyint(P.lo / P.q);
       const double L = std::nearbyint(P.hi / P.q) - P.base + 1.0;
-      if (!(L >= 1.0 && L < 2147483647.0)) { delete t; KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: too many levels", d); }
+      if (!(L >= 1.0 && L < 2147483647.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_create: parameter %d: too many levels", d);
       P.levels = (int)L;
       t->disc.push_back(d);
       if (P.levels <= TPE_LCAP) t->lt = std::max(t->lt, P.levels);
@@ -688,33 +680,18 @@ int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds
   }
   t->Dc = (int)t->cont.size();
   t->Dd = (int)t->disc.size();
-  int r = kbo_reserve(h, t->d_prm, sizeof(TpeParam) * D);
-  if (r == KBO_OK && cudaMemcpy(t->d_prm.p, t->prm.data(), sizeof(TpeParam) * D, cudaMemcpyHostToDevice) != cudaSuccess) r = KBO_ERR_CUDA;
-  if (r == KBO_OK) r = upload_list(h, t->d_cont, t->cont);
-  if (r == KBO_OK) r = upload_list(h, t->d_disc, t->disc);
-  if (r == KBO_OK) r = upload_list(h, t->d_num, t->num);
-  if (r == KBO_OK) r = upload_list(h, t->d_cat, t->cat);
-  for (auto& e : t->ev)
-    if (r == KBO_OK && cudaEventCreate(&e) != cudaSuccess) r = KBO_ERR_CUDA;
-  if (r != KBO_OK) {
-    kbo_tpe_destroy(t);
-    return r;
-  }
-  *out = t;
+  KBO_TRY(kbo_upload(h, t->d_prm, t->prm.data(), sizeof(TpeParam) * D));
+  KBO_TRY(kbo_upload(h, t->d_cont, t->cont.data(), 4 * t->cont.size()));
+  KBO_TRY(kbo_upload(h, t->d_disc, t->disc.data(), 4 * t->disc.size()));
+  KBO_TRY(kbo_upload(h, t->d_num, t->num.data(), 4 * t->num.size()));
+  KBO_TRY(kbo_upload(h, t->d_cat, t->cat.data(), 4 * t->cat.size()));
+  KBO_TRY(t->ev.create());
+  *out = t.release();
   return KBO_OK;
 }
 
 void kbo_tpe_destroy(kbo_tpe* t) {
-  if (!t) return;
-  DevBuf* bufs[] = {&t->d_prm, &t->d_cont, &t->d_disc, &t->d_num, &t->d_cat, &t->vals, &t->loss, &t->lkey, &t->lkey2, &t->lidx, &t->lidx2,
-                    &t->below, &t->grp, &t->pos, &t->skey, &t->skey2, &t->sval, &t->sval2, &t->segb, &t->sege, &t->tmp, &t->w, &t->mu,
-                    &t->sg, &t->lc, &t->f4, &t->cdf, &t->hdr, &t->cat_p, &t->cat_sc, &t->cat_cum, &t->draws, &t->sc, &t->lb, &t->surv, &t->bb,
-                    &t->first, &t->err};
-  for (DevBuf* b : bufs)
-    if (b->p) cudaFree(b->p);
-  for (auto& e : t->ev)
-    if (e) cudaEventDestroy(e);
-  delete t;
+  if (t) delete t;
 }
 
 int kbo_tpe_tell(kbo_handle* h, kbo_tpe* t, const double* X, const double* loss, int32_t n_new, int on_host, void* stream) {
@@ -725,27 +702,7 @@ int kbo_tpe_tell(kbo_handle* h, kbo_tpe* t, const double* X, const double* loss,
   if ((int64_t)t->n + n_new > (1 << 24)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_tell: at most 2^24 trials supported");
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
-  const size_t D = t->D;
-  if (t->n + n_new > t->cap) {   // grow (doubling), keeping the rows already told
-    const int cap = std::max({2 * t->cap, t->n + n_new, 64});
-    DevBuf v{}, l{};
-    KBO_TRY(kbo_reserve(h, v, 8 * D * cap));
-    int r = kbo_reserve(h, l, 8 * (size_t)cap);
-    if (r != KBO_OK) { cudaFree(v.p); return r; }
-    if (t->n) {
-      cudaMemcpyAsync(v.p, t->vals.p, 8 * D * t->n, cudaMemcpyDeviceToDevice, s);
-      cudaMemcpyAsync(l.p, t->loss.p, 8 * (size_t)t->n, cudaMemcpyDeviceToDevice, s);
-      cudaStreamSynchronize(s);
-    }
-    if (t->vals.p) cudaFree(t->vals.p);
-    if (t->loss.p) cudaFree(t->loss.p);
-    t->vals = v;
-    t->loss = l;
-    t->cap = cap;
-  }
-  const cudaMemcpyKind kind = on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-  KBO_CUDA(h, cudaMemcpyAsync((double*)t->vals.p + D * t->n, X, 8 * D * n_new, kind, s));
-  KBO_CUDA(h, cudaMemcpyAsync((double*)t->loss.p + t->n, loss, 8 * (size_t)n_new, kind, s));
+  KBO_TRY(tpe_history_append(h, t, X, loss, n_new, on_host, s));
   if (on_host) KBO_CUDA(h, cudaStreamSynchronize(s));   // the caller may free its host arrays on return
   t->n += n_new;
   return KBO_OK;

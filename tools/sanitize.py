@@ -77,3 +77,29 @@ en = EnasController(5, 12, 9, seed=2)
 print(en.sample(6).tolist(), en.train(0.5, 3)[:, 0].tolist())
 print(en.train(0.7, 2, arcs=en.sample(2)).shape, en.sample(5, uniforms=_r.random((5, 15)), return_probs=True)[0].tolist())
 en.close()
+
+
+def refused(call):                                   # a call that fails after it has allocated: nothing may leak
+    try:
+        call()
+    except ValueError as ex:
+        return str(ex).splitlines()[0][:60]
+    raise AssertionError("the call was expected to be refused")
+
+
+tp = Tpe([("uniform", -1.0, 3.0), ("choice", 5)], seed=1)    # history grown twice (64 -> 128 -> 256 rows), the told rows kept
+for n in (40, 40, 100):
+    tp.tell(np.c_[_r.uniform(-1, 3, n), _r.integers(0, 5, n)], _r.random(n))
+bad = torch.zeros(1, 2, 64, dtype=torch.float64, device="cuda:0")
+bad[0, 1, 7] = 9.0                                    # category 9 of 5
+print(tp.ask(1, 64).tolist(), refused(lambda: tp.ask(1, 64, candidates=bad)))
+tp.close()
+mv = MvTpe([("float", 0.0, 1.0), ("cat", 3)], seed=1)
+mv.tell(np.c_[_r.random(20), _r.integers(0, 3, 20)], _r.random(20))
+print(refused(lambda: mv.tell([[0.5, 1.0]], [float("nan")])), mv.ask(1, 64).tolist())
+mv.close()
+fe = ForestEngine(kind="RF", n_trees=4, seed=1)
+Xn = _r.random((50, 3))
+Xn[7, 1] = np.nan
+print(refused(lambda: fe.tell(Xn, _r.random(50))))
+fe.close()
