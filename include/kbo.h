@@ -323,7 +323,17 @@ uint64_t kbo_hash64(const void* bytes, uint64_t len);   /* the FNV-1a hash kbo_r
  * and constants are recomputed), mean0_host, sigma0, C = B = I, d = 1, zero paths, history and flags, strategy generation
  * 0.  Same limits and error codes as kbo_cma_create; after a failed restart the instance may only be destroyed.
  * kbo_cma_run_synthetic runs `generations` ask/fitness/tell rounds entirely on the device with a built-in fitness
- * (0 = sphere, 1 = Rastrigin) — the BASELINE.json config-4 benchmark. */
+ * (0 = sphere, 1 = Rastrigin) — the BASELINE.json config-4 benchmark.
+ * kbo_cma_set_margin turns on CMA-ES with Margin (CMAwM, Hamano et al. GECCO 2022, as in CyberAgent `cmaes`) for
+ * n_discrete dimensions dims[] (increasing).  Dimension dims[i] has the sorted levels levels[level_offsets[i],
+ * level_offsets[i+1]) (2 or more, increasing; level_offsets has n_discrete + 1 entries from 0) or, when that range is
+ * empty, the arithmetic levels first + k·step, k < count, from arith[3i .. 3i+2] = (first, step, count).  alpha is the
+ * margin α in (0, 1), or 0 for 1/(D·lambda), recomputed at every restart.  Then kbo_cma_ask returns x = m + σ·(A∘y) with
+ * each discrete coordinate encoded to its level (the interval (ℓ_{k−1}, ℓ_k] of thresholds ℓ_k = (v_k + v_{k+1})/2 that
+ * holds it); the tell's mean step is m + c_m·σ·A∘y_w, and after the eigendecomposition a one-CTA kernel corrects m_j and
+ * A_j of each discrete dimension (oracle/cma_margin_oracle.py).  A starts at 1 and a restart resets it.  n_discrete = 0
+ * turns the margin off: every kernel is then the margin-free one.  Not between an ask and its tell (KBO_ERR_STATE).
+ * kbo_cma_margin_state copies A, the mean before the last correction and α to HOST (any may be NULL) and synchronises. */
 typedef struct kbo_cma kbo_cma;
 int kbo_cma_create(kbo_handle* h, kbo_cma** out, int32_t D, int32_t lambda, const double* mean0_host, double sigma0, uint64_t seed);
 void kbo_cma_destroy(kbo_cma* c);
@@ -335,6 +345,9 @@ int kbo_cma_stop_flags(kbo_handle* h, kbo_cma* c, uint32_t* flags_host, double* 
 int kbo_cma_restart(kbo_handle* h, kbo_cma* c, int32_t lambda, const double* mean0_host, double sigma0);
 int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32_t generations, double* best_f_host,
                           float* elapsed_ms, double* jacobi_sweeps_last);
+int kbo_cma_set_margin(kbo_handle* h, kbo_cma* c, int32_t n_discrete, const int32_t* dims, const int64_t* level_offsets,
+                       const double* levels, const double* arith, double alpha);
+int kbo_cma_margin_state(kbo_handle* h, kbo_cma* c, double* A_host, double* mean_before_host, double* alpha_host, void* stream);
 
 /* ---- TPE (Katib algorithm `tpe`: hyperopt's tpe.suggest on a flat space; FP64 restatement oracle/tpe_oracle.py) -------
  * Parameter kinds: UNIFORM = uniform(lo, hi); QUNIFORM = quniform(lo, hi, q), values rint(x/q)·q; CHOICE = choice over

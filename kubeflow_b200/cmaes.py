@@ -100,6 +100,36 @@ class CmaEs:
             self.popsize = int(popsize)
             self._X = torch.empty(self.popsize, self.D, dtype=torch.float64, device=f"cuda:{self.device}")
 
+    def set_margin(self, dims: dict, alpha: float | None = None):
+        """CMA-ES with Margin on the discrete dimensions ``dims``: {index: sorted cube levels (1-D array, 2 or more) or an
+        arithmetic range (first, step, count)}.  ``alpha`` is the margin (default 1/(D·λ), recomputed at restarts).  From
+        the next ask on, samples carry each discrete coordinate encoded to its level, and A starts at ones.  An empty
+        ``dims`` turns the margin off.  Not between an ask and its tell."""
+        idx = sorted(int(i) for i in dims)
+        offs, lev, arith = [0], [], []
+        for i in idx:
+            v = dims[i]
+            if isinstance(v, tuple):
+                arith += [float(v[0]), float(v[1]), float(v[2])]
+            else:
+                lev.append(np.asarray(v, dtype=np.float64).ravel())
+                arith += [0.0, 0.0, 0.0]
+            offs.append(offs[-1] + (0 if isinstance(v, tuple) else len(lev[-1])))
+        d = np.array(idx, dtype=np.int32)
+        o = np.array(offs, dtype=np.int64)
+        lv = np.ascontiguousarray(np.concatenate(lev) if lev else np.zeros(1))
+        ar = np.array(arith if arith else [0.0], dtype=np.float64)
+        L.check(self.lib, self._h, self.lib.kbo_cma_set_margin(self._h, self._c, len(idx), d.ctypes.data, o.ctypes.data, lv.ctypes.data,
+                                                               ar.ctypes.data, float(alpha or 0.0)))
+        self.margin_dims = idx
+
+    def margin_state(self) -> dict:
+        """A, the mean after the last tell's update and before its margin correction, and α (needs set_margin)."""
+        A, mb, alpha = np.empty(self.D), np.empty(self.D), C.c_double()
+        L.check(self.lib, self._h, self.lib.kbo_cma_margin_state(self._h, self._c, A.ctypes.data, mb.ctypes.data, C.byref(alpha),
+                                                                 self._stream()))
+        return dict(A=A, mean_before=mb, alpha=alpha.value)
+
     def run_synthetic(self, fitness: str, generations: int):
         """BASELINE config 4: `generations` full generations on the device with a built-in fitness."""
         kind = {"sphere": 0, "rastrigin": 1}[fitness]

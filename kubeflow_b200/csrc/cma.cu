@@ -7,6 +7,8 @@
 //         takes 6–7 sweeps, counting the last one that rotates nothing (10 at most), measured on an H100.
 // Everything is tiny (D ≤ 128, λ ≤ 8192: C is 128 KiB) — the generation is launch/latency bound, so each phase is one
 // kernel and the whole state lives in HBM/L2 between them; nothing returns to the host until the caller asks.
+#include <cmath>
+
 #include "kbo_internal.cuh"
 #include "dgemm.cuh"
 #include "kbo_rng.cuh"
@@ -26,6 +28,18 @@ struct kbo_cma {
   double tolx = 0.0;
   DevBuf mean, C, B, Dv, ps, pc, weights, Z, Zs, Y, Ys, YwT, zn2, order, R, G, scal, yw, hist, flags;
   bool asked = false;
+  // CMA-ES with Margin (kbo_cma_set_margin): off while n_disc == 0, and then no margin buffer is touched
+  int n_disc = 0;
+  double alpha = 0.0, alpha_set = 0.0;  // alpha_set: the caller's α, or 0 for the default 1/(D·λ) recomputed at restarts
+  DevBuf A, mdim, mlev, mprev, mpre;    // A; per-dimension level descriptors; level tables; (m, σ) before the tell; m before the correction
+};
+
+// A discrete dimension's sorted levels in cube coordinates: levels[off, off + count) of the table, or, for ranges too long
+// for a table (kind 2), level k = first + k·step.  Continuous dimensions have kind 0.
+struct CmaMarginDim {
+  double first, step;
+  long long count, off;
+  int kind;
 };
 
 enum CmaScal { CS_SIGMA = 0, CS_ALPHA_C = 1, CS_BEST_F = 2, CS_SWEEPS = 3, CS_COUNT = 8 };
@@ -481,6 +495,85 @@ __global__ void __launch_bounds__(CMA_MAXD) cma_stop_kernel(const double* __rest
   }
 }
 
+// ------------------------------------------------------------------------------------------------ margin (CMAwM)
+// CMA-ES with Margin (Hamano et al., GECCO 2022) as in CyberAgent `cmaes`: oracle/cma_margin_oracle.py states each rule.
+// Levels and thresholds ℓ_k = (v_k + v_{k+1})/2 round as NumPy does (DMUL / DADD, never a contracted DFMA), so a sample
+// encodes to the same level on both sides of a threshold.
+__device__ __forceinline__ double cma_level(const CmaMarginDim& m, const double* __restrict__ lev, long long k) {
+  return m.kind == 1 ? lev[m.off + k] : __dadd_rn(m.first, __dmul_rn((double)k, m.step));
+}
+__device__ __forceinline__ double cma_threshold(const CmaMarginDim& m, const double* __restrict__ lev, long long k) {
+  return __dmul_rn(__dadd_rn(cma_level(m, lev, k), cma_level(m, lev, k + 1)), 0.5);
+}
+// number of thresholds ℓ_k (k < count − 1) with ℓ_k < x (below = false) or ℓ_k ≤ x (below = true), by binary search
+__device__ __forceinline__ long long cma_rank(const CmaMarginDim& m, const double* __restrict__ lev, double x, bool below) {
+  long long lo = 0, hi = m.count - 1;
+  while (lo < hi) {
+    const long long mid = lo + ((hi - lo) >> 1);
+    const double l = cma_threshold(m, lev, mid);
+    if (below ? l <= x : l < x) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+
+// x = m + σ·(A∘y); a discrete coordinate encodes to the level whose interval (ℓ_{k−1}, ℓ_k] holds x (margin-free: cma_x_kernel)
+__global__ void cma_x_margin_kernel(const double* __restrict__ Y, const double* __restrict__ mean, const double* __restrict__ scal,
+                                    const double* __restrict__ A, const CmaMarginDim* __restrict__ md, const double* __restrict__ lev,
+                                    int64_t n, int D, double* __restrict__ X) {
+  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n) return;
+  const int d = (int)(e % D);
+  const double x = fma(scal[CS_SIGMA], A[d] * Y[e], mean[d]);
+  const CmaMarginDim m = md[d];
+  X[e] = m.kind == 0 ? x : cma_level(m, lev, cma_rank(m, lev, x, false));
+}
+
+// One CTA of CMA_MAXD threads, one per dimension, after cma_eigval_kernel.  The mean step of cma_update_kernel is redone
+// with A from the (m, σ) it started from — m ← m + c_m·σ·A∘y_w, the same DFMA, so A_j = 1 reproduces it bit for bit —
+// then each discrete dimension gets the margin correction of m_j and A_j at the updated σ and C.
+__global__ void __launch_bounds__(CMA_MAXD) cma_margin_kernel(const double* __restrict__ mprev, const double* __restrict__ yw, double cm,
+                                                              const double* __restrict__ scal, const double* __restrict__ C,
+                                                              const CmaMarginDim* __restrict__ md, const double* __restrict__ lev, int D,
+                                                              double alpha, double* __restrict__ mean, double* __restrict__ A,
+                                                              double* __restrict__ mpre) {
+  const int t = threadIdx.x;
+  if (t >= D) return;
+  const double a = A[t];
+  double m = fma(cm * mprev[D], a * yw[t], mprev[t]);
+  mpre[t] = m;
+  const CmaMarginDim dm = md[t];
+  if (dm.kind != 0) {
+    const long long r = cma_rank(dm, lev, m, true);
+    const double l_lo = cma_threshold(dm, lev, r == 0 ? 0 : r - 1);
+    const double l_up = cma_threshold(dm, lev, r == dm.count - 1 ? r - 1 : r);
+    const double sc = sqrt(C[(size_t)t * D + t]);
+    const double s = __dmul_rn(__dmul_rn(scal[CS_SIGMA], a), sc);
+    const double p_lo = normcdf(__dadd_rn(l_lo, -m) / s);
+    const double p_up = normcdf(__dadd_rn(m, -l_up) / s);
+    const double p_mid = __dadd_rn(__dadd_rn(1.0, -p_lo), -p_up);
+    if (fmax(p_lo, p_up) > 0.5) {
+      if (fmin(p_lo, p_up) < alpha) {
+        const double sg = m > l_up ? 1.0 : (m < l_up ? -1.0 : 0.0);
+        m = __dadd_rn(l_up, __dmul_rn(sg, __dmul_rn(s, -normcdfinv(alpha))));
+      }
+    } else {
+      const double h = 0.5 * alpha;
+      const double lo = fmax(p_lo, h), up = fmax(p_up, h);
+      const double over = __dadd_rn(__dadd_rn(__dadd_rn(1.0, -lo), -up), -p_mid);
+      const double den = __dadd_rn(__dadd_rn(__dadd_rn(lo, p_mid), up), -3.0 * h);
+      double q_lo = __dadd_rn(lo, __dmul_rn(over, __dadd_rn(lo, -h)) / den);
+      double q_up = __dadd_rn(up, __dmul_rn(over, __dadd_rn(up, -h)) / den);
+      q_lo = fmin(fmax(q_lo, 1e-10), 0.5 - 1e-10);
+      q_up = fmin(fmax(q_up, 1e-10), 0.5 - 1e-10);
+      const double chi_lo = -normcdfinv(q_lo), chi_up = -normcdfinv(q_up);
+      const double chi = __dadd_rn(chi_lo, chi_up);
+      A[t] = __dadd_rn(l_up, -l_lo) / __dmul_rn(__dmul_rn(chi, scal[CS_SIGMA]), sc);
+      m = __dadd_rn(__dmul_rn(l_lo, chi_up), __dmul_rn(l_up, chi_lo)) / chi;
+    }
+  }
+  mean[t] = m;
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness, cudaStream_t s) {
   const int D = c->D, lam = c->lambda;
@@ -491,6 +584,10 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
                                                c->lam_pad, D, (double*)c->Ys.p, (double*)c->YwT.p);
   KBO_LAUNCH_CHECK(h);
   CmaConst k{c->mu_eff, c->c1, c->cmu, c->cm, c->c_sigma, c->d_sigma, c->cc, c->chi_n, c->wsum, c->mu, c->gen};
+  if (c->n_disc) {   // (m, σ) the update starts from, for the margin kernel's A-scaled mean step
+    KBO_CUDA(h, cudaMemcpyAsync(c->mprev.p, c->mean.p, 8 * (size_t)D, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, cudaMemcpyAsync((double*)c->mprev.p + D, c->scal.p, 8, cudaMemcpyDeviceToDevice, s));
+  }
   cma_update_kernel<<<1, 1024, 0, s>>>((const double*)c->Ys.p, (const double*)c->weights.p, D, k, (double*)c->mean.p, (const double*)c->B.p,
                                        (const double*)c->Dv.p, (double*)c->ps.p, (double*)c->pc.p, (double*)c->scal.p, (double*)c->yw.p);
   KBO_LAUNCH_CHECK(h);
@@ -515,6 +612,12 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
   KBO_LAUNCH_CHECK(h);
   cma_eigval_kernel<<<D, 1024, 0, s>>>((const double*)c->C.p, (const double*)c->B.p, D, (double*)c->Dv.p);
   KBO_LAUNCH_CHECK(h);
+  if (c->n_disc) {
+    cma_margin_kernel<<<1, CMA_MAXD, 0, s>>>((const double*)c->mprev.p, (const double*)c->yw.p, c->cm, (const double*)c->scal.p,
+                                             (const double*)c->C.p, (const CmaMarginDim*)c->mdim.p, (const double*)c->mlev.p, D, c->alpha,
+                                             (double*)c->mean.p, (double*)c->A.p, (double*)c->mpre.p);
+    KBO_LAUNCH_CHECK(h);
+  }
   cma_stop_kernel<<<1, CMA_MAXD, 0, s>>>(fitness, (const int*)c->order.p, lam, D, (const double*)c->mean.p, (const double*)c->C.p,
                                          (const double*)c->B.p, (const double*)c->Dv.p, (const double*)c->pc.p, (const double*)c->scal.p,
                                          (double*)c->hist.p, c->term, c->gen + 1, c->tolx, (unsigned*)c->flags.p);
@@ -539,7 +642,12 @@ static int cma_generation_ask(kbo_handle* h, kbo_cma* c, double* X, const double
   // Y[k,i] = Σ_j Zs[k,j]·B[i,j]
   dgemm64_launch<true, EPI_STORE>(s, lam, D, D, (const double*)c->Zs.p, D, (const double*)c->B.p, D, (double*)c->Y.p, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
   KBO_LAUNCH_CHECK(h);
-  cma_x_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const double*)c->Y.p, (const double*)c->mean.p, (const double*)c->scal.p, n, D, X);
+  if (c->n_disc)
+    cma_x_margin_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const double*)c->Y.p, (const double*)c->mean.p, (const double*)c->scal.p,
+                                                                     (const double*)c->A.p, (const CmaMarginDim*)c->mdim.p,
+                                                                     (const double*)c->mlev.p, n, D, X);
+  else
+    cma_x_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const double*)c->Y.p, (const double*)c->mean.p, (const double*)c->scal.p, n, D, X);
   KBO_LAUNCH_CHECK(h);
   c->asked = true;
   return KBO_OK;
@@ -624,7 +732,73 @@ static int cma_start_run(kbo_handle* h, kbo_cma* c, const double* mean0, double 
   return KBO_OK;
 }
 
+// A run's margin state: A = 1, and α = the caller's or the default 1/(D·λ) of the current λ (synchronous)
+static int cma_margin_reset(kbo_handle* h, kbo_cma* c) {
+  if (!c->n_disc) return KBO_OK;
+  c->alpha = c->alpha_set > 0.0 ? c->alpha_set : 1.0 / ((double)c->D * c->lambda);
+  const std::vector<double> ones(c->D, 1.0);
+  KBO_CUDA(h, cudaMemcpy(c->A.p, ones.data(), 8 * (size_t)c->D, cudaMemcpyHostToDevice));
+  return KBO_OK;
+}
+
 extern "C" {
+
+int kbo_cma_set_margin(kbo_handle* h, kbo_cma* c, int32_t n_discrete, const int32_t* dims, const int64_t* level_offsets,
+                       const double* levels, const double* arith, double alpha) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (c->asked) KBO_FAIL(h, KBO_ERR_STATE, "kbo_cma_set_margin: the last ask has not been told");
+  if (n_discrete < 0 || n_discrete > c->D) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: 0 <= n_discrete <= D required (got %d)", n_discrete);
+  if (!(alpha == 0.0 || (alpha > 0.0 && alpha < 1.0))) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: alpha must be in (0, 1), or 0 for 1/(D*lambda)");
+  if (n_discrete && (!dims || !level_offsets)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: dims and level_offsets must be given");
+  const int D = c->D;
+  std::vector<CmaMarginDim> md(D, CmaMarginDim{0.0, 0.0, 0, 0, 0});
+  const int64_t n_lev = n_discrete ? level_offsets[n_discrete] : 0;
+  if (level_offsets && (level_offsets[0] != 0 || n_lev < 0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: level_offsets must start at 0");
+  if (n_lev && !levels) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: null levels");
+  for (int i = 0; i < n_discrete; i++) {
+    const int d = dims[i];
+    if (d < 0 || d >= D || (i && d <= dims[i - 1])) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: dims must be increasing in [0, D)");
+    const int64_t off = level_offsets[i], k = level_offsets[i + 1] - off;
+    if (k < 0 || level_offsets[i + 1] > n_lev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: level_offsets must be non-decreasing");
+    if (k) {
+      for (int64_t j = 0; j < k; j++)
+        if (!std::isfinite(levels[off + j]) || (j && !(levels[off + j] > levels[off + j - 1])))
+          KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: dimension %d: levels must be finite and increasing", d);
+      if (k < 2) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: dimension %d: a discrete dimension needs 2 or more levels", d);
+      md[d] = CmaMarginDim{0.0, 0.0, (long long)k, (long long)off, 1};
+    } else {
+      if (!arith) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: dimension %d has no level table and arith is null", d);
+      const double first = arith[3 * i], step = arith[3 * i + 1], cnt = arith[3 * i + 2];
+      if (!std::isfinite(first) || !(step > 0.0) || !std::isfinite(step) || !(cnt >= 2.0 && cnt <= 9007199254740992.0) || cnt != std::floor(cnt))
+        KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: dimension %d: arithmetic levels need finite first, step > 0 and an integer count >= 2", d);
+      md[d] = CmaMarginDim{first, step, (long long)cnt, 0, 2};
+    }
+  }
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  KBO_CUDA(h, cudaDeviceSynchronize());            // a tell in flight may still read the tables about to be replaced
+  c->n_disc = 0;
+  if (!n_discrete) return KBO_OK;
+  KBO_TRY(kbo_reserve(h, c->A, 8 * (size_t)D));
+  KBO_TRY(kbo_reserve(h, c->mprev, 8 * (size_t)(D + 1)));
+  KBO_TRY(kbo_reserve(h, c->mpre, 8 * (size_t)D));
+  KBO_TRY(kbo_upload(h, c->mdim, md.data(), sizeof(CmaMarginDim) * D));
+  KBO_TRY(kbo_upload(h, c->mlev, levels, 8 * (size_t)n_lev));
+  KBO_CUDA(h, cudaMemcpy(c->mpre.p, c->mean.p, 8 * (size_t)D, cudaMemcpyDeviceToDevice));
+  c->n_disc = n_discrete;
+  c->alpha_set = alpha;
+  return cma_margin_reset(h, c);
+}
+
+int kbo_cma_margin_state(kbo_handle* h, kbo_cma* c, double* A_host, double* mean_before_host, double* alpha_host, void* stream) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (!c->n_disc) KBO_FAIL(h, KBO_ERR_STATE, "kbo_cma_margin_state: no margin is set");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (A_host) KBO_CUDA(h, cudaMemcpyAsync(A_host, c->A.p, 8 * (size_t)c->D, cudaMemcpyDeviceToHost, s));
+  if (mean_before_host) KBO_CUDA(h, cudaMemcpyAsync(mean_before_host, c->mpre.p, 8 * (size_t)c->D, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (alpha_host) *alpha_host = c->alpha;
+  return KBO_OK;
+}
 
 int kbo_cma_create(kbo_handle* h, kbo_cma** out, int32_t D, int32_t lambda, const double* mean0, double sigma0, uint64_t seed) {
   if (!h || !out) return KBO_ERR_INVALID;
@@ -653,6 +827,7 @@ int kbo_cma_restart(kbo_handle* h, kbo_cma* c, int32_t lambda, const double* mea
   KBO_CUDA(h, cudaSetDevice(h->device));
   KBO_CUDA(h, cudaDeviceSynchronize());            // the last tell may still be reading buffers that are about to grow
   KBO_TRY(cma_configure(h, c, lambda, sigma0));
+  KBO_TRY(cma_margin_reset(h, c));
   return cma_start_run(h, c, mean0, sigma0);
 }
 

@@ -13,7 +13,10 @@ goptuna's relative/independent sampling split amounts to.  With ``restart_strate
 termination test the sampler runs on the device after every tell is read after each complete generation; when any of
 its criteria holds, the run restarts in place on the schedule of ``cma_restart.py`` (IPOP: doubled population; BIPOP:
 interlaced large and small runs) with a fresh mean drawn in the cube.  Outstanding samples of the stopped run stay
-unmatched, like extra independent draws.
+unmatched, like extra independent draws.  With ``with_margin: true`` the sampler runs CMA-ES with Margin (Optuna's
+``CmaEsSampler(with_margin=True)``): ``int`` and numeric ``discrete`` parameters become discrete dimensions whose levels
+(``cma_margin.py``) the sampler encodes on the device, and the margin α (``margin``, default 1/(D·λ)) keeps a
+coordinate from freezing on one level once σ is small.  Trials get the encoded level's value; a restart resets the margin.
 """
 from __future__ import annotations
 
@@ -24,6 +27,7 @@ import numpy as np
 from . import api_pb as api
 from .internal import (CATEGORICAL, DISCRETE, DOUBLE, INTEGER, MAX_GOAL, AlgorithmSettingsError, Assignment,
                        HyperParameterSearchSpace, Trial, parse_settings)
+from .cma_margin import discrete_dims, encode, parse_with_margin
 from .cma_restart import STRATEGIES, Schedule
 from .service import _Base, _reply_from
 
@@ -46,10 +50,18 @@ def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
                     raise AlgorithmSettingsError(f"popsize must be in [4, 8192], got {v}")
             elif k in ("restart_strategy", "device"):
                 out[k] = v
+            elif k == "with_margin":
+                out[k] = parse_with_margin(v)
+            elif k == "margin":
+                out[k] = float(v)
+                if not 0.0 < out[k] < 1.0:
+                    raise AlgorithmSettingsError(f"margin must be in (0, 1), got {v}")
             else:
                 raise AlgorithmSettingsError(f"unknown setting {k} for algorithm cmaes")
         except ValueError:
             raise AlgorithmSettingsError(f"failed to convert {v!r} for setting {k}")
+    if "margin" in out and not out.get("with_margin", False):
+        raise AlgorithmSettingsError("margin needs with_margin: true")
     if out.get("restart_strategy", "none") not in STRATEGIES:
         raise AlgorithmSettingsError(f"restart_strategy must be one of {', '.join(STRATEGIES)}, got {out['restart_strategy']!r}")
     if n_params < 2:
@@ -73,6 +85,10 @@ class _Experiment:
         self.schedule = None if strategy == "none" else Schedule(strategy, D, settings.get("popsize"), settings.get("sigma", 1.0 / 6.0),
                                                                    settings.get("random_state", 0))
         self.run_gens = 0        # generations told in the current run
+        # with_margin: {parameter index: Levels} of the discrete dimensions, encoded by the sampler
+        self.levels = discrete_dims(space.params) if settings.get("with_margin", False) else {}
+        if self.levels:
+            self.es.set_margin({j: L.cube for j, L in self.levels.items()}, settings.get("margin"))
 
 
 class CmaesService(_Base):
@@ -85,8 +101,10 @@ class CmaesService(_Base):
     @staticmethod
     def _space(experiment):
         ss = HyperParameterSearchSpace.convert(experiment)
+        margin = any(s.name == "with_margin" and str(s.value).strip().lower() == "true"
+                     for s in experiment.spec.algorithm.algorithm_settings)
         for p in ss.params:
-            if p.type in (CATEGORICAL, DISCRETE):
+            if p.type == CATEGORICAL or (p.type == DISCRETE and not margin):
                 raise AlgorithmSettingsError(f"cmaes does not support categorical/discrete parameter {p.name!r}")
         return ss
 
@@ -94,12 +112,16 @@ class CmaesService(_Base):
         if experiment.spec.algorithm.algorithm_name != "cmaes":
             raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
         ss = self._space(experiment)
-        validate_cmaes_settings(parse_settings(experiment), len(ss.params))
+        if validate_cmaes_settings(parse_settings(experiment), len(ss.params)).get("with_margin", False):
+            discrete_dims(ss.params)
 
     @staticmethod
-    def _to_assignments(ss, u):
+    def _to_assignments(ss, u, levels=None):
         out = []
-        for p, v in zip(ss.params, np.clip(u, 0.0, 1.0)):
+        for j, (p, v) in enumerate(zip(ss.params, np.clip(u, 0.0, 1.0))):
+            if levels and j in levels:
+                out.append(Assignment(p.name, levels[j].value(float(u[j]))))
+                continue
             lo, hi = float(p.min), float(p.max)
             x = lo + float(v) * (hi - lo)
             out.append(Assignment(p.name, str(int(round(x))) if p.type == INTEGER else repr(x)))
@@ -111,7 +133,7 @@ class CmaesService(_Base):
 
     def _new_generation(self, st, ss):
         X = st.es.ask().cpu().numpy()
-        st.queue = [(i, self._to_assignments(ss, X[i])) for i in range(X.shape[0])]
+        st.queue = [(i, self._to_assignments(ss, X[i], st.levels)) for i in range(X.shape[0])]
         st.assign = {i: a for i, a in st.queue}
         st.pending = {}
         st.fitness = {}
@@ -162,5 +184,9 @@ class CmaesService(_Base):
                 else:   # generation exhausted but not finished: independent draw from the current distribution
                     s = st.es.state()
                     z = st.extra_rng.standard_normal(st.es.D)
-                    lists.append(self._to_assignments(ss, s["mean"] + s["sigma"] * (s["B"] @ (s["d"] * z))))
+                    if st.levels:
+                        x = s["mean"] + s["sigma"] * (st.es.margin_state()["A"] * (s["B"] @ (s["d"] * z)))
+                        lists.append(self._to_assignments(ss, encode(st.levels, x), st.levels))
+                    else:
+                        lists.append(self._to_assignments(ss, s["mean"] + s["sigma"] * (s["B"] @ (s["d"] * z))))
         return _reply_from(lists)
