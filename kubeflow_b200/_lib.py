@@ -5,6 +5,9 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import numpy as np
+import torch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libkbo.so")
 
@@ -211,3 +214,63 @@ def check(lib, handle, code: int):
     if code == KBO_ERR_NOT_PD:
         raise KboNotPositiveDefinite(code, msg)
     raise KboError(code, msg)
+
+
+class Handle:
+    """Owner of one libkbo handle (``kbo_create`` on ``device``) and, given ``kind``, of one engine object made on it by
+    ``kbo_<kind>_create(handle, &object, *create_args)``.  ``close()`` destroys the object, then the handle; it is idempotent
+    and safe after an ``__init__`` that failed partway (a failed ``kbo_<kind>_create`` closes the handle before raising)."""
+
+    def __init__(self, device: int = 0, kind: str | None = None, *create_args):
+        if not torch.cuda.is_available():
+            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
+        self.lib = load()
+        self.device = int(device)
+        h = C.c_void_p()
+        rc = self.lib.kbo_create(C.byref(h), self.device)
+        if rc != KBO_OK:
+            raise KboError(rc, "kbo_create failed (no usable CUDA device?)")
+        self._h = h
+        if kind is not None:
+            self._kind, o = kind, C.c_void_p()
+            try:
+                self.check(getattr(self.lib, f"kbo_{kind}_create")(self._h, C.byref(o), *create_args))
+            except BaseException:
+                self.close()
+                raise
+            self._o = o
+
+    def close(self):
+        if getattr(self, "_o", None):
+            getattr(self.lib, f"kbo_{self._kind}_destroy")(self._o)
+            self._o = C.c_void_p()
+        if getattr(self, "_h", None):
+            self.lib.kbo_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def check(self, code: int):
+        check(self.lib, self._h, code)
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _last_survivors(self) -> np.ndarray:
+        """``kbo_<kind>_last_survivors``: the count (NULL buffer), then the int32 entries."""
+        fn = getattr(self.lib, f"kbo_{self._kind}_last_survivors")
+        n = fn(self._h, self._o, None, 0)
+        out = np.zeros(max(n, 0), np.int32)
+        if n > 0:
+            fn(self._h, self._o, out.ctypes.data, n)
+        return out
+
+    def _last_timings(self, names) -> dict:
+        """``kbo_<kind>_last_timings``: one float32 millisecond figure per name."""
+        ms = np.zeros(len(names), np.float32)
+        getattr(self.lib, f"kbo_{self._kind}_last_timings")(self._h, self._o, ms.ctypes.data, len(names))
+        return dict(zip(names, ms.tolist()))

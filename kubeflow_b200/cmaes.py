@@ -10,39 +10,13 @@ import torch
 from . import _lib as L
 
 
-class CmaEs:
+class CmaEs(L.Handle):
     def __init__(self, mean, sigma: float, popsize: int | None = None, seed: int = 0, device: int = 0):
-        if not torch.cuda.is_available():
-            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         mean = np.ascontiguousarray(np.asarray(mean, dtype=np.float64))
         self.D = int(mean.shape[0])
         self.popsize = int(popsize) if popsize else 4 + int(3 * np.log(self.D))
-        self.device = int(device)
-        self.lib = L.load()
-        self._h, self._c = C.c_void_p(), C.c_void_p()
-        rc = self.lib.kbo_create(C.byref(self._h), self.device)
-        if rc != L.KBO_OK:
-            raise L.KboError(rc, "kbo_create failed")
-        L.check(self.lib, self._h, self.lib.kbo_cma_create(self._h, C.byref(self._c), self.D, self.popsize,
-                                                           mean.ctypes.data_as(C.POINTER(C.c_double)), float(sigma), int(seed)))
+        super().__init__(device, "cma", self.D, self.popsize, mean.ctypes.data_as(C.POINTER(C.c_double)), float(sigma), int(seed))
         self._X = torch.empty(self.popsize, self.D, dtype=torch.float64, device=f"cuda:{self.device}")
-
-    def close(self):
-        if getattr(self, "_c", None):
-            self.lib.kbo_cma_destroy(self._c)
-            self._c = C.c_void_p()
-        if getattr(self, "_h", None):
-            self.lib.kbo_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def ask(self, z: torch.Tensor | None = None) -> torch.Tensor:
         """Population (popsize × D float64 CUDA tensor).  ``z``: optional popsize×D standard normals (CUDA float64)."""
@@ -52,7 +26,7 @@ class CmaEs:
                 raise ValueError("z must be a float64 CUDA tensor of shape (popsize, D)")
             z = z.contiguous()
             zp = z.data_ptr()
-        L.check(self.lib, self._h, self.lib.kbo_cma_ask(self._h, self._c, self._X.data_ptr(), zp, self._stream()))
+        self.check(self.lib.kbo_cma_ask(self._h, self._o, self._X.data_ptr(), zp, self._stream()))
         return self._X
 
     def tell(self, fitness):
@@ -60,7 +34,7 @@ class CmaEs:
         f = f.to(device=f"cuda:{self.device}", dtype=torch.float64).contiguous()
         if f.numel() != self.popsize:
             raise ValueError(f"fitness must have {self.popsize} entries")
-        L.check(self.lib, self._h, self.lib.kbo_cma_tell(self._h, self._c, f.data_ptr(), self._stream()))
+        self.check(self.lib.kbo_cma_tell(self._h, self._o, f.data_ptr(), self._stream()))
 
     def state(self, with_Y: bool = False) -> dict:
         D, lam = self.D, self.popsize
@@ -69,9 +43,9 @@ class CmaEs:
         Y = np.empty((lam, D)) if with_Y else None
         gen = C.c_int64()
         ptr = lambda a: a.ctypes.data if a is not None else None
-        L.check(self.lib, self._h, self.lib.kbo_cma_state(self._h, self._c, ptr(out["mean"]), ptr(out["sigma"]), ptr(out["C"]),
-                                                          ptr(out["p_sigma"]), ptr(out["pc"]), ptr(out["B"]), ptr(out["d"]), ptr(Y),
-                                                          C.byref(gen), self._stream()))
+        self.check(self.lib.kbo_cma_state(self._h, self._o, ptr(out["mean"]), ptr(out["sigma"]), ptr(out["C"]),
+                                          ptr(out["p_sigma"]), ptr(out["pc"]), ptr(out["B"]), ptr(out["d"]), ptr(Y),
+                                          C.byref(gen), self._stream()))
         out["sigma"] = float(out["sigma"][0])
         out["generation"] = gen.value
         if with_Y:
@@ -84,8 +58,8 @@ class CmaEs:
         each generation's best and worst fitness (2·term values) and term."""
         flags, term = C.c_uint32(), C.c_int32()
         hist = np.zeros(2 * (10 + -(-30 * self.D // 4)))     # room for the largest ring (λ = 4)
-        L.check(self.lib, self._h, self.lib.kbo_cma_stop_flags(self._h, self._c, C.byref(flags), hist.ctypes.data, C.byref(term),
-                                                               self._stream()))
+        self.check(self.lib.kbo_cma_stop_flags(self._h, self._o, C.byref(flags), hist.ctypes.data, C.byref(term),
+                                               self._stream()))
         return flags.value, hist[:2 * term.value].copy(), term.value
 
     def restart(self, popsize: int, mean, sigma: float):
@@ -94,8 +68,8 @@ class CmaEs:
         mean = np.ascontiguousarray(np.asarray(mean, dtype=np.float64))
         if mean.shape != (self.D,):
             raise ValueError(f"mean must have {self.D} entries")
-        L.check(self.lib, self._h, self.lib.kbo_cma_restart(self._h, self._c, int(popsize), mean.ctypes.data_as(C.POINTER(C.c_double)),
-                                                            float(sigma)))
+        self.check(self.lib.kbo_cma_restart(self._h, self._o, int(popsize), mean.ctypes.data_as(C.POINTER(C.c_double)),
+                                            float(sigma)))
         if int(popsize) != self.popsize:
             self.popsize = int(popsize)
             self._X = torch.empty(self.popsize, self.D, dtype=torch.float64, device=f"cuda:{self.device}")
@@ -119,21 +93,21 @@ class CmaEs:
         o = np.array(offs, dtype=np.int64)
         lv = np.ascontiguousarray(np.concatenate(lev) if lev else np.zeros(1))
         ar = np.array(arith if arith else [0.0], dtype=np.float64)
-        L.check(self.lib, self._h, self.lib.kbo_cma_set_margin(self._h, self._c, len(idx), d.ctypes.data, o.ctypes.data, lv.ctypes.data,
-                                                               ar.ctypes.data, float(alpha or 0.0)))
+        self.check(self.lib.kbo_cma_set_margin(self._h, self._o, len(idx), d.ctypes.data, o.ctypes.data, lv.ctypes.data,
+                                               ar.ctypes.data, float(alpha or 0.0)))
         self.margin_dims = idx
 
     def margin_state(self) -> dict:
         """A, the mean after the last tell's update and before its margin correction, and α (needs set_margin)."""
         A, mb, alpha = np.empty(self.D), np.empty(self.D), C.c_double()
-        L.check(self.lib, self._h, self.lib.kbo_cma_margin_state(self._h, self._c, A.ctypes.data, mb.ctypes.data, C.byref(alpha),
-                                                                 self._stream()))
+        self.check(self.lib.kbo_cma_margin_state(self._h, self._o, A.ctypes.data, mb.ctypes.data, C.byref(alpha),
+                                                 self._stream()))
         return dict(A=A, mean_before=mb, alpha=alpha.value)
 
     def run_synthetic(self, fitness: str, generations: int):
         """BASELINE config 4: `generations` full generations on the device with a built-in fitness."""
         kind = {"sphere": 0, "rastrigin": 1}[fitness]
         best, ms, sw = C.c_double(), C.c_float(), C.c_double()
-        L.check(self.lib, self._h, self.lib.kbo_cma_run_synthetic(self._h, self._c, kind, int(generations), C.byref(best), C.byref(ms),
-                                                                  C.byref(sw)))
+        self.check(self.lib.kbo_cma_run_synthetic(self._h, self._o, kind, int(generations), C.byref(best), C.byref(ms),
+                                                  C.byref(sw)))
         return dict(best_f=best.value, elapsed_ms=ms.value, generations_per_s=generations / (ms.value * 1e-3), jacobi_sweeps=sw.value)

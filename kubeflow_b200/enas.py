@@ -34,14 +34,12 @@ def unflatten(flat: np.ndarray, L_: int, H: int, n_ops: int) -> dict:
     return out
 
 
-class EnasController:
+class EnasController(L.Handle):
     """L layers, hidden size H, n_ops operations.  ``settings``: the keys of DEFAULT_SETTINGS; None for temperature,
     tanh_const, entropy_weight or skip_weight drops that term.  An arc is L(L+1)/2 integers: per layer its op, then one skip
     bit per earlier layer."""
 
     def __init__(self, num_layers: int, hidden: int, n_ops: int, settings: dict | None = None, seed: int = 0, device: int = 0):
-        if not torch.cuda.is_available():
-            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.L, self.H, self.n_ops = int(num_layers), int(hidden), int(n_ops)
         self.A = self.L * (self.L + 1) // 2
         st = dict(DEFAULT_SETTINGS)
@@ -52,31 +50,8 @@ class EnasController:
                                entropy_weight=0.0 if st["entropy_weight"] is None else float(st["entropy_weight"]),
                                baseline_decay=float(st["baseline_decay"]), learning_rate=float(st["learning_rate"]),
                                skip_target=float(st["skip_target"]), skip_weight=0.0 if st["skip_weight"] is None else float(st["skip_weight"]))
-        self.device = int(device)
-        self.lib = L.load()
-        self._h, self._e = C.c_void_p(), C.c_void_p()
-        rc = self.lib.kbo_create(C.byref(self._h), self.device)
-        if rc != L.KBO_OK:
-            raise L.KboError(rc, "kbo_create failed")
-        L.check(self.lib, self._h, self.lib.kbo_enas_create(self._h, C.byref(self._e), self.L, self.H, self.n_ops, C.byref(cs), int(seed)))
+        super().__init__(device, "enas", self.L, self.H, self.n_ops, C.byref(cs), int(seed))
         self.n_par = sum(a * b for a, b in param_shapes(self.L, self.H, self.n_ops).values())
-
-    def close(self):
-        if getattr(self, "_e", None):
-            self.lib.kbo_enas_destroy(self._e)
-            self._e = C.c_void_p()
-        if getattr(self, "_h", None):
-            self.lib.kbo_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def train(self, reward: float, steps: int, arcs=None) -> np.ndarray:
         """``steps`` REINFORCE steps on ``reward``; ``arcs`` (steps × L(L+1)/2) imposes the arcs.  Returns the per-step
@@ -88,7 +63,7 @@ class EnasController:
         if arcs is not None:
             a = torch.as_tensor(np.ascontiguousarray(np.asarray(arcs, dtype=np.int32).reshape(steps, self.A)), device=dev)
             ap = a.data_ptr()
-        L.check(self.lib, self._h, self.lib.kbo_enas_train(self._h, self._e, float(reward), steps, ap, stats.data_ptr(), self._stream()))
+        self.check(self.lib.kbo_enas_train(self._h, self._o, float(reward), steps, ap, stats.data_ptr(), self._stream()))
         return stats[:steps].cpu().numpy()
 
     def sample(self, k: int, uniforms=None, return_probs: bool = False):
@@ -104,7 +79,7 @@ class EnasController:
         opp = torch.empty(k, self.L, self.n_ops, dtype=torch.float32, device=dev) if return_probs else None
         skp = torch.empty(k, max(self.L * (self.L - 1) // 2, 1), dtype=torch.float32, device=dev) if return_probs else None
         ptr = lambda t: t.data_ptr() if t is not None else None
-        L.check(self.lib, self._h, self.lib.kbo_enas_sample(self._h, self._e, k, arcs.data_ptr(), up, ptr(opp), ptr(skp), self._stream()))
+        self.check(self.lib.kbo_enas_sample(self._h, self._o, k, arcs.data_ptr(), up, ptr(opp), ptr(skp), self._stream()))
         out = arcs.cpu().numpy()
         if not return_probs:
             return out
@@ -114,8 +89,8 @@ class EnasController:
         """Parameters (dict of float32 arrays), Adam moments m and v (same layout), baseline, step and draw counter."""
         p, m, v = (np.empty(self.n_par, np.float32) for _ in range(3))
         b, t, d = C.c_float(), C.c_int64(), C.c_int64()
-        L.check(self.lib, self._h, self.lib.kbo_enas_state(self._h, self._e, p.ctypes.data, m.ctypes.data, v.ctypes.data, C.byref(b), C.byref(t),
-                                                           C.byref(d), self._stream()))
+        self.check(self.lib.kbo_enas_state(self._h, self._o, p.ctypes.data, m.ctypes.data, v.ctypes.data, C.byref(b), C.byref(t),
+                                           C.byref(d), self._stream()))
         u = lambda f: unflatten(f, self.L, self.H, self.n_ops)
         return dict(params=u(p), m=u(m), v=u(v), baseline=b.value, step=t.value, draws=d.value)
 
@@ -125,10 +100,8 @@ class EnasController:
         mm = flatten(m) if m is not None else None
         vv = flatten(v) if v is not None else None
         ptr = lambda a: a.ctypes.data if a is not None else None
-        L.check(self.lib, self._h, self.lib.kbo_enas_set_params(self._h, self._e, p.ctypes.data, ptr(mm), ptr(vv), float(baseline), int(step),
-                                                                self._stream()))
+        self.check(self.lib.kbo_enas_set_params(self._h, self._o, p.ctypes.data, ptr(mm), ptr(vv), float(baseline), int(step),
+                                                self._stream()))
 
     def last_timings(self) -> dict:
-        ms = np.zeros(2, np.float32)
-        self.lib.kbo_enas_last_timings(self._h, self._e, ms.ctypes.data, 2)
-        return dict(train_ms=float(ms[0]), sample_ms=float(ms[1]))
+        return self._last_timings(("train_ms", "sample_ms"))

@@ -25,43 +25,18 @@ from .gp import Best
 KINDS = {"RF": 0, "ET": 1}
 
 
-class ForestEngine:
+class ForestEngine(L.Handle):
     def __init__(self, device: int = 0, *, kind: str = "RF", n_trees: int = 100, min_samples_leaf: int = 3, seed: int = 0,
                  acq: str = "ei", xi: float = 0.01, kappa: float = 1.96):
-        if not torch.cuda.is_available():
-            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         if kind not in KINDS:
             raise ValueError(f"kind must be RF or ET, got {kind!r}")
-        self.device, self.kind, self.n_trees = int(device), kind, int(n_trees)
+        self.kind, self.n_trees = kind, int(n_trees)
         self.acq, self.xi, self.kappa = acq, float(xi), float(kappa)
-        self.lib = L.load()
-        self._h, self._f = C.c_void_p(), C.c_void_p()
-        rc = self.lib.kbo_create(C.byref(self._h), self.device)
-        if rc != L.KBO_OK:
-            raise L.KboError(rc, "kbo_create failed")
-        L.check(self.lib, self._h, self.lib.kbo_forest_create(self._h, C.byref(self._f), KINDS[kind], self.n_trees, int(min_samples_leaf),
-                                                              int(seed) & (2 ** 64 - 1)))
+        super().__init__(device, "forest", KINDS[kind], self.n_trees, int(min_samples_leaf), int(seed) & (2 ** 64 - 1))
         self.N = self.D = 0
         self.y_opt = None
         self._hist = None          # (X, y) of the fitted forest
         self.last_fit = None       # "fit" | "reuse"
-
-    def close(self):
-        if getattr(self, "_f", None):
-            self.lib.kbo_forest_destroy(self._f)
-            self._f = C.c_void_p()
-        if getattr(self, "_h", None):
-            self.lib.kbo_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def _dev32(self, X) -> torch.Tensor:
         if isinstance(X, torch.Tensor):
@@ -87,8 +62,8 @@ class ForestEngine:
         if counts is not None:
             cd = torch.from_numpy(np.ascontiguousarray(counts, dtype=np.int32).reshape(self.n_trees, len(yh))).to(f"cuda:{self.device}")
         with torch.cuda.device(self.device):
-            L.check(self.lib, self._h, self.lib.kbo_forest_fit(self._h, self._f, Xd.data_ptr(), yd.data_ptr(), len(yh), Xh.shape[1],
-                                                               cd.data_ptr() if cd is not None else None, self._stream()))
+            self.check(self.lib.kbo_forest_fit(self._h, self._o, Xd.data_ptr(), yd.data_ptr(), len(yh), Xh.shape[1],
+                                               cd.data_ptr() if cd is not None else None, self._stream()))
         self.N, self.D = Xh.shape
         self.y_opt = float(np.min(yh))
         self._hist = (Xh.copy(), yh.copy()) if counts is None else None
@@ -115,10 +90,10 @@ class ForestEngine:
         mu = torch.empty(M, dtype=torch.float64, device=dev) if return_arrays else None
         sd = torch.empty(M, dtype=torch.float64, device=dev) if return_arrays else None
         with torch.cuda.device(self.device):
-            L.check(self.lib, self._h, self.lib.kbo_forest_sweep(self._h, self._f, Xd.data_ptr(), int(M), int(global_offset), n, kinds, self.y_opt,
-                                                                 self.xi, self.kappa, out.data_ptr() if n else None,
-                                                                 mu.data_ptr() if mu is not None else None,
-                                                                 sd.data_ptr() if sd is not None else None, self._stream()))
+            self.check(self.lib.kbo_forest_sweep(self._h, self._o, Xd.data_ptr(), int(M), int(global_offset), n, kinds, self.y_opt,
+                                                 self.xi, self.kappa, out.data_ptr() if n else None,
+                                                 mu.data_ptr() if mu is not None else None,
+                                                 sd.data_ptr() if sd is not None else None, self._stream()))
             raw = out.cpu().numpy()
         bests = [Best(float(raw[4 * i]), int(raw[4 * i + 1:4 * i + 2].view(np.int64)[0]), float(raw[4 * i + 2]), float(raw[4 * i + 3]))
                  for i in range(n)]
@@ -137,8 +112,8 @@ class ForestEngine:
         self._check(Xh.shape[1])
         mu, sd = np.empty(len(Xh)), np.empty(len(Xh))
         with torch.cuda.device(self.device):
-            L.check(self.lib, self._h, self.lib.kbo_forest_predict(self._h, self._f, Xh.ctypes.data, len(Xh), 1, mu.ctypes.data, sd.ctypes.data,
-                                                                   self._stream()))
+            self.check(self.lib.kbo_forest_predict(self._h, self._o, Xh.ctypes.data, len(Xh), 1, mu.ctypes.data, sd.ctypes.data,
+                                                   self._stream()))
         return mu, sd
 
     def predict_mean(self, X) -> np.ndarray:
@@ -149,14 +124,14 @@ class ForestEngine:
         n_nodes × D thresholds drawn at each internal node (NaN where the feature is constant there)."""
         n = C.c_int32()
         counts = np.zeros(self.N, np.int32)
-        L.check(self.lib, self._h, self.lib.kbo_forest_export(self._h, self._f, int(tree), *([None] * 9), 0, C.byref(n), counts.ctypes.data,
-                                                              self._stream()))
+        self.check(self.lib.kbo_forest_export(self._h, self._o, int(tree), *([None] * 9), 0, C.byref(n), counts.ctypes.data,
+                                              self._stream()))
         k = n.value
         out = dict(feature=np.empty(k, np.int32), threshold=np.empty(k), left=np.empty(k, np.int32), right=np.empty(k, np.int32),
                    value=np.empty(k), impurity=np.empty(k), n_node_samples=np.empty(k, np.int32), weighted_n_node_samples=np.empty(k))
         draws = np.empty((k, self.D)) if with_draws else None
-        L.check(self.lib, self._h, self.lib.kbo_forest_export(
-            self._h, self._f, int(tree), *[out[a].ctypes.data for a in ("feature", "threshold", "left", "right", "value", "impurity",
+        self.check(self.lib.kbo_forest_export(
+            self._h, self._o, int(tree), *[out[a].ctypes.data for a in ("feature", "threshold", "left", "right", "value", "impurity",
                                                                          "n_node_samples", "weighted_n_node_samples")],
             draws.ctypes.data if draws is not None else None, k, None, None, self._stream()))
         out["counts"] = counts
@@ -165,6 +140,4 @@ class ForestEngine:
         return out
 
     def last_timings(self) -> dict:
-        ms = np.zeros(2, np.float32)
-        self.lib.kbo_forest_last_timings(self._h, self._f, ms.ctypes.data, 2)
-        return dict(fit_ms=float(ms[0]), sweep_ms=float(ms[1]))
+        return self._last_timings(("fit_ms", "sweep_ms"))

@@ -24,7 +24,7 @@ class Best:
     std: float     # posterior std at that candidate (raw y scale)
 
 
-class GPEngine:
+class GPEngine(L.Handle):
     def __init__(self, device: int = 0, *, kernel: str = "matern52", length_scale=1.0, amplitude: float = 1.0,
                  noise: float = 1e-10, acq: str = "ei", xi: float = 0.01, kappa: float = 1.96,
                  normalize_y: bool = True, var_mode: str = "auto", tc_k_span: int = 0, scratch_limit: int | None = None,
@@ -36,14 +36,7 @@ class GPEngine:
             raise ValueError(f"acq must be one of {sorted(L.ACQS)}, got {acq!r}")
         if var_mode not in L.VAR_MODES:
             raise ValueError(f"var_mode must be one of {sorted(L.VAR_MODES)}, got {var_mode!r}")
-        if not torch.cuda.is_available():
-            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
-        self.lib = L.load()
-        self.device = int(device)
-        self._h = C.c_void_p()
-        rc = self.lib.kbo_create(C.byref(self._h), self.device)
-        if rc != L.KBO_OK:
-            raise L.KboError(rc, "kbo_create failed (no usable CUDA device?)")
+        super().__init__(device)
         self.kernel, self.acq, self.var_mode = kernel, acq, var_mode
         self.length_scale = np.atleast_1d(np.asarray(length_scale, dtype=np.float64)).copy()
         self.amplitude, self.noise, self.xi, self.kappa = float(amplitude), float(noise), float(xi), float(kappa)
@@ -51,38 +44,24 @@ class GPEngine:
         self.N = self.D = 0
         self.scratch_limit = 4 << 30 if scratch_limit is None else int(scratch_limit)   # libkbo's default
         if scratch_limit is not None:
-            L.check(self.lib, self._h, self.lib.kbo_set_scratch_limit(self._h, int(scratch_limit)))
+            self.check(self.lib.kbo_set_scratch_limit(self._h, int(scratch_limit)))
         if tc_fast is not None:
-            L.check(self.lib, self._h, self.lib.kbo_set_tc_fast(self._h, int(bool(tc_fast))))
+            self.check(self.lib.kbo_set_tc_fast(self._h, int(bool(tc_fast))))
         if rank_tc is not None:
-            L.check(self.lib, self._h, self.lib.kbo_set_rank_tc(self._h, int(bool(rank_tc))))
+            self.check(self.lib.kbo_set_rank_tc(self._h, int(bool(rank_tc))))
         if lazy_inverse is not None:
-            L.check(self.lib, self._h, self.lib.kbo_set_lazy_inverse(self._h, int(bool(lazy_inverse))))
+            self.check(self.lib.kbo_set_lazy_inverse(self._h, int(bool(lazy_inverse))))
         if rank_prefix is not None:
-            L.check(self.lib, self._h, self.lib.kbo_set_rank_prefix(self._h, int(rank_prefix)))
+            self.check(self.lib.kbo_set_rank_prefix(self._h, int(rank_prefix)))
         self._best_dev = torch.empty(4, dtype=torch.float64, device=f"cuda:{self.device}")
 
     # -- plumbing ----------------------------------------------------------------------------------
-    def close(self):
-        if getattr(self, "_h", None) is not None and self._h:
-            self.lib.kbo_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
     def _params(self):
         self._ls_arr = (C.c_double * len(self.length_scale))(*self.length_scale)
         return L.KboParams(kernel=L.KERNELS[self.kernel], acq=L.ACQS[self.acq], normalize_y=int(self.normalize_y),
                            var_mode=L.VAR_MODES[self.var_mode], amplitude=self.amplitude, noise=self.noise, xi=self.xi,
                            kappa=self.kappa, length_scale=self._ls_arr, n_length_scale=len(self.length_scale),
                            tc_k_span=self.tc_k_span)
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     @staticmethod
     def _as_host_f64(a):
@@ -108,7 +87,7 @@ class GPEngine:
             xp, yp, on_host = X.ctypes.data, y.ctypes.data, 1
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_fit(self._h, xp, yp, int(N), int(D), C.byref(p), on_host, self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         self.N, self.D = int(N), int(D)
         return self
 
@@ -126,7 +105,7 @@ class GPEngine:
             raise ValueError(f"x has {x.shape[0]} values, fit had D={self.D}")
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_fit_append(self._h, x.ctypes.data, float(y), 1, self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         self.N += 1
         return self
 
@@ -141,14 +120,14 @@ class GPEngine:
             yp = y.ctypes.data
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_fit_rebase(self._h, int(n_keep), yp, 1, self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         self.N = int(n_keep)
         return self
 
     def fit_info(self):
         lml, ym, ys, yo, info = C.c_double(), C.c_double(), C.c_double(), C.c_double(), C.c_int32()
         rc = self.lib.kbo_fit_info(self._h, C.byref(lml), C.byref(ym), C.byref(ys), C.byref(yo), C.byref(info), self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         return dict(lml=lml.value, y_mean=ym.value, y_std=ys.value, y_opt=yo.value, info=info.value)
 
     def last_contenders(self) -> int:
@@ -176,7 +155,7 @@ class GPEngine:
     def fp64_peak_tflops(self) -> float:
         """Test / bench hook: the FP64 tensor-core (DMMA) rate of this GPU, measured on register-resident operands."""
         out = C.c_double(0.0)
-        L.check(self.lib, self._h, self.lib.kbo_debug_fp64_peak(self._h, C.byref(out)))
+        self.check(self.lib.kbo_debug_fp64_peak(self._h, C.byref(out)))
         return float(out.value)
 
     def rank_pass(self, Xc, mode: int, want_plane: bool = False):
@@ -195,7 +174,7 @@ class GPEngine:
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_debug_rank_pass(self._h, Xc.data_ptr(), dt, int(M), int(mode), mu.data_ptr(), var.data_ptr(),
                                               plane.data_ptr() if want_plane else None, self._stream())
-            L.check(self.lib, self._h, rc)
+            self.check(rc)
             torch.cuda.current_stream(self.device).synchronize()
         return mu, var, plane
 
@@ -216,7 +195,7 @@ class GPEngine:
         assert plane.shape == (rows_pad, npad) and plane.dtype == torch.float16 and plane.is_contiguous()
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_debug_kstar(self._h, Xc.data_ptr(), dt, int(M), int(store_cols), mu.data_ptr(), plane.data_ptr(), self._stream())
-            L.check(self.lib, self._h, rc)
+            self.check(rc)
             torch.cuda.current_stream(self.device).synchronize()
         return mu[:M], plane
 
@@ -237,7 +216,7 @@ class GPEngine:
                 m = min(slice_rows, M - r0)
                 rc = self.lib.kbo_debug_rank_rows(self._h, Xc[r0:].data_ptr(), dt, int(m), int(tile_pairs), mu[r0:].data_ptr(),
                                                   var[r0:].data_ptr(), self._stream())
-                L.check(self.lib, self._h, rc)
+                self.check(rc)
             torch.cuda.current_stream(self.device).synchronize()
         return mu, var
 
@@ -246,7 +225,7 @@ class GPEngine:
     def record_stages(self, on: bool = True):
         """Test hook: keep, for every stage of each later ask / ask_multi and every acquisition, the bounds it pruned with and
         its survivors (``stages()``).  Recording reads them back; it changes no arithmetic."""
-        L.check(self.lib, self._h, self.lib.kbo_debug_record_stages(self._h, int(bool(on))))
+        self.check(self.lib.kbo_debug_record_stages(self._h, int(bool(on))))
         return self
 
     def stages(self):
@@ -258,7 +237,7 @@ class GPEngine:
         for i in range(int(self.lib.kbo_debug_stage_count(self._h))):
             ints, fl = (C.c_int32 * 4)(), (C.c_float * 7)()
             n = self.lib.kbo_debug_stage(self._h, i, ints, fl, None, 0)
-            L.check(self.lib, self._h, min(n, 0))
+            self.check(min(n, 0))
             lst = np.empty(max(n, 1), dtype=np.int32)
             self.lib.kbo_debug_stage(self._h, i, ints, fl, lst.ctypes.data, n)
             out.append(dict(stage=self.STAGES[ints[0]], acq=acq_names[ints[1]], cal_n=int(ints[2]), n=int(ints[3]),
@@ -271,7 +250,7 @@ class GPEngine:
         info = self.fit_info()
         g = np.empty(2 + len(self.length_scale), dtype=np.float64)
         rc = self.lib.kbo_lml_grad(self._h, g.ctypes.data_as(C.POINTER(C.c_double)), len(g), self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         return info["lml"], g
 
     def _theta_params(self, thetas):
@@ -303,7 +282,7 @@ class GPEngine:
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_lml_batch(self._h, X.ctypes.data, y.ctypes.data, int(N), int(D), int(G), arr, 1,
                                         out.ctypes.data_as(C.POINTER(C.c_double)), info, self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         return (out, np.array(info[:], dtype=np.int32)) if return_info else out
 
     def lml_grad_batch(self, X, y, thetas, return_info: bool = False):
@@ -324,7 +303,7 @@ class GPEngine:
             rc = self.lib.kbo_lml_grad_batch(self._h, X.ctypes.data, y.ctypes.data, int(N), int(D), int(G), arr, 1,
                                              lml.ctypes.data_as(C.POINTER(C.c_double)), grad.ctypes.data_as(C.POINTER(C.c_double)),
                                              info, self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         return (lml, grad, np.array(info[:G], dtype=np.int32)) if return_info else (lml, grad)
 
     @staticmethod
@@ -341,7 +320,7 @@ class GPEngine:
         Wm = torch.empty(N, N, dtype=torch.float64, device=dev)
         al = torch.empty(N, dtype=torch.float64, device=dev)
         rc = self.lib.kbo_fit_state(self._h, Lm.data_ptr(), Wm.data_ptr(), al.data_ptr(), self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         torch.cuda.current_stream(self.device).synchronize()
         return Lm, Wm, al
 
@@ -360,7 +339,7 @@ class GPEngine:
         if len(unique_id) != 128:
             raise ValueError("unique_id must be the 128 bytes of comm_unique_id()")
         with torch.cuda.device(self.device):
-            L.check(self.lib, self._h, self.lib.kbo_comm_init(self._h, int(n_ranks), int(rank), C.c_char_p(unique_id)))
+            self.check(self.lib.kbo_comm_init(self._h, int(n_ranks), int(rank), C.c_char_p(unique_id)))
         return self
 
     def comm_size(self) -> int:
@@ -386,12 +365,12 @@ class GPEngine:
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_sweep(self._h, ptr, dt, int(M), int(global_offset), on_host, mp, sp, ap,
                                     self._best_dev.data_ptr(), self._stream())
-            L.check(self.lib, self._h, rc)
+            self.check(rc)
             if allreduce:
-                L.check(self.lib, self._h, self.lib.kbo_allreduce_argmax(self._h, self._best_dev.data_ptr(), self._stream()))
+                self.check(self.lib.kbo_allreduce_argmax(self._h, self._best_dev.data_ptr(), self._stream()))
             b = L.KboBest()
             rc = self.lib.kbo_best_to_host(self._h, self._best_dev.data_ptr(), C.byref(b), self._stream())
-            L.check(self.lib, self._h, rc)
+            self.check(rc)
         best = Best(b.value, int(b.index), b.mu, b.std)
         return (best, mu, std, acq) if return_arrays else best
 
@@ -425,11 +404,11 @@ class GPEngine:
         out = torch.empty(4 * max(n, 1), dtype=torch.float64, device=f"cuda:{self.device}")
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_sweep_multi(self._h, ptr, dt, int(M), int(global_offset), on_host, int(n), kinds, out.data_ptr(), self._stream())
-            L.check(self.lib, self._h, rc)
+            self.check(rc)
             bests = []
             for i in range(n):
                 b = L.KboBest()
-                L.check(self.lib, self._h, self.lib.kbo_best_to_host(self._h, out.data_ptr() + 32 * i, C.byref(b), self._stream()))
+                self.check(self.lib.kbo_best_to_host(self._h, out.data_ptr() + 32 * i, C.byref(b), self._stream()))
                 bests.append(Best(b.value, int(b.index), b.mu, b.std))
         del keep
         return bests
@@ -440,7 +419,7 @@ class GPEngine:
         u, c, p = (C.c_int32 * 3)(), (C.c_int32 * 3)(), (C.c_int32 * 3)()
         n = self.lib.kbo_last_decisions(self._h, 3, u, c, p)
         if n < 0:
-            L.check(self.lib, self._h, n)
+            self.check(n)
         return [(int(u[i]), int(c[i]), int(p[i])) for i in range(n)]
 
     def predict_mean(self, X) -> np.ndarray:
@@ -453,7 +432,7 @@ class GPEngine:
         mu = np.empty(n, dtype=np.float64)
         with torch.cuda.device(self.device):
             rc = self.lib.kbo_predict_mean(self._h, ptr, dt, int(n), on_host, mu.ctypes.data, self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         del keep
         return mu
 
@@ -468,7 +447,7 @@ class GPEngine:
         b, t = L.KboBest(), L.KboTimings()
         rc = self.lib.kbo_suggest_host(self._h, X.ctypes.data, y.ctypes.data, X.shape[0], X.shape[1], Xc.ctypes.data, dt,
                                        Xc.shape[0], int(global_offset), C.byref(p), C.byref(b), C.byref(t))
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         self.N, self.D = X.shape
         return Best(b.value, int(b.index), b.mu, b.std), t.as_dict()
 
@@ -479,7 +458,7 @@ class GPEngine:
                                      L.ACQS[self.acq], y_mean, y_std, y_opt, self.xi, self.kappa,
                                      acq_out.data_ptr() if acq_out is not None else None, self._best_dev.data_ptr(),
                                      self._stream())
-        L.check(self.lib, self._h, rc)
+        self.check(rc)
         torch.cuda.current_stream(self.device).synchronize()
         v = self._best_dev.cpu()
         return Best(float(v[0]), int(v[1:2].view(torch.int64)[0]), float(v[2]), float(v[3]))

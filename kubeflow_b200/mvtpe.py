@@ -13,13 +13,11 @@ from . import _lib as L
 FLOAT, INT, CAT = 0, 1, 2
 
 
-class MvTpe:
+class MvTpe(L.Handle):
     """params: list of ``("float", lo, hi)``, ``("int", lo, hi, step)`` or ``("cat", n_categories)``.  Values are in parameter
     units: integers are grid points lo + j·step <= hi, categoricals are observed and suggested as category indices."""
 
     def __init__(self, params, seed: int = 0, device: int = 0):
-        if not torch.cuda.is_available():
-            raise RuntimeError("kubeflow_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         self.params = [tuple(p) for p in params]
         self.D = len(self.params)
         kinds = np.zeros(self.D, np.int32)
@@ -35,32 +33,9 @@ class MvTpe:
             else:
                 raise ValueError(f"unknown parameter kind {p[0]!r}")
         self.kinds = kinds
-        self.device = int(device)
-        self.lib = L.load()
-        self._h, self._t = C.c_void_p(), C.c_void_p()
-        rc = self.lib.kbo_create(C.byref(self._h), self.device)
-        if rc != L.KBO_OK:
-            raise L.KboError(rc, "kbo_create failed")
-        L.check(self.lib, self._h, self.lib.kbo_mvtpe_create(self._h, C.byref(self._t), self.D, kinds.ctypes.data, lo.ctypes.data, hi.ctypes.data,
-                                                             q.ctypes.data, levels.ctypes.data, int(seed)))
+        super().__init__(device, "mvtpe", self.D, kinds.ctypes.data, lo.ctypes.data, hi.ctypes.data, q.ctypes.data, levels.ctypes.data,
+                         int(seed))
         self.n = 0
-
-    def close(self):
-        if getattr(self, "_t", None):
-            self.lib.kbo_mvtpe_destroy(self._t)
-            self._t = C.c_void_p()
-        if getattr(self, "_h", None):
-            self.lib.kbo_destroy(self._h)
-            self._h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def tell(self, X, losses):
         """Append trials in told order: X (n × D, parameter units) and their losses (minimised; NaN is refused)."""
@@ -69,7 +44,7 @@ class MvTpe:
         if X.shape[0] != y.shape[0]:
             raise ValueError("X and losses must have the same number of rows")
         if X.shape[0]:
-            L.check(self.lib, self._h, self.lib.kbo_mvtpe_tell(self._h, self._t, X.ctypes.data, y.ctypes.data, X.shape[0], 1, self._stream()))
+            self.check(self.lib.kbo_mvtpe_tell(self._h, self._o, X.ctypes.data, y.ctypes.data, X.shape[0], 1, self._stream()))
             self.n += X.shape[0]
 
     def ask(self, k: int = 1, n_candidates: int = 24, candidates: torch.Tensor | None = None, return_details: bool = False):
@@ -89,7 +64,7 @@ class MvTpe:
         cout = torch.empty(k, self.D, M, dtype=torch.float64, device=dev) if return_details else None
         sc = torch.empty(k, M, 2, dtype=torch.float32, device=dev) if return_details else None
         ptr = lambda t: t.data_ptr() if t is not None else None
-        L.check(self.lib, self._h, self.lib.kbo_mvtpe_ask(self._h, self._t, k, M, cp, x.data_ptr(), ptr(idx), ptr(cout), ptr(sc), self._stream()))
+        self.check(self.lib.kbo_mvtpe_ask(self._h, self._o, k, M, cp, x.data_ptr(), ptr(idx), ptr(cout), ptr(sc), self._stream()))
         out = x.cpu().numpy()
         if not return_details:
             return out
@@ -102,22 +77,16 @@ class MvTpe:
         out = {}
         for g, name in ((0, "below"), (1, "above")):
             m, nb = C.c_int32(), C.c_int32()
-            L.check(self.lib, self._h, self.lib.kbo_mvtpe_state(self._h, self._t, g, None, None, None, None, 0, C.byref(m), C.byref(nb), self._stream()))
+            self.check(self.lib.kbo_mvtpe_state(self._h, self._o, g, None, None, None, None, 0, C.byref(m), C.byref(nb), self._stream()))
             w, sg, mu, cr = np.empty(m.value + 1), np.empty(self.D), np.empty((m.value, self.D)), np.empty((self.D, 2))
-            L.check(self.lib, self._h, self.lib.kbo_mvtpe_state(self._h, self._t, g, w.ctypes.data, sg.ctypes.data, mu.ctypes.data, cr.ctypes.data,
-                                                                m.value + 1, None, None, self._stream()))
+            self.check(self.lib.kbo_mvtpe_state(self._h, self._o, g, w.ctypes.data, sg.ctypes.data, mu.ctypes.data, cr.ctypes.data,
+                                                m.value + 1, None, None, self._stream()))
             out[name] = dict(w=w, sigma=sg, mu=mu, cat_rows=cr)
             out["n_below"] = nb.value
         return out
 
     def last_survivors(self) -> np.ndarray:
-        n = self.lib.kbo_mvtpe_last_survivors(self._h, self._t, None, 0)
-        out = np.zeros(max(n, 0), np.int32)
-        if n > 0:
-            self.lib.kbo_mvtpe_last_survivors(self._h, self._t, out.ctypes.data, n)
-        return out
+        return self._last_survivors()
 
     def last_timings(self) -> dict:
-        ms = np.zeros(4, np.float32)
-        self.lib.kbo_mvtpe_last_timings(self._h, self._t, ms.ctypes.data, 4)
-        return dict(zip(("models_and_draws_ms", "score_fp32_ms", "decide_fp64_ms", "final_ms"), ms.tolist()))
+        return self._last_timings(("models_and_draws_ms", "score_fp32_ms", "decide_fp64_ms", "final_ms"))

@@ -146,6 +146,13 @@ class Optimizer:
         self.last_fit = None          # "fit" | "append" | "reuse": what the last ask did to the engine (diagnostics, tests)
         self.last_best = None
 
+    def close(self):
+        """Release the GP or forest engine (its libkbo handle and device memory); a later ask makes a fresh one."""
+        if self._engine is not None:
+            self._engine.close()
+            self._engine = None
+        self._fit_state = None
+
     # ------------------------------------------------------------------------------------------------------
     def tell(self, x, y, xt=None):
         """``xt``: the rows already in the transformed space (the request scan computes them column-wise); must equal

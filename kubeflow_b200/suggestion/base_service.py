@@ -7,9 +7,16 @@ import logging
 
 from ..optimizer import Optimizer
 from ..space import Categorical, Integer, Real
-from .internal import CATEGORICAL, DISCRETE, DOUBLE, INTEGER, MAX_GOAL, Assignment
+from .internal import DOUBLE, INTEGER, MAX_GOAL, Assignment
 
 logger = logging.getLogger(__name__)
+
+
+def dimensions(search_space) -> list:
+    """The ``Space`` dimensions of a Katib search space: INT → Integer, DOUBLE → Real, CATEGORICAL / DISCRETE → Categorical."""
+    return [Integer(int(p.min), int(p.max), name=p.name) if p.type == INTEGER else
+            Real(float(p.min), float(p.max), name=p.name) if p.type == DOUBLE else Categorical(list(p.list), name=p.name)
+            for p in search_space.params]
 
 
 class BaseSkoptService:
@@ -25,17 +32,12 @@ class BaseSkoptService:
         self.create_optimizer()
 
     def create_optimizer(self):
-        dims = []
-        for p in self.search_space.params:
-            if p.type == INTEGER:
-                dims.append(Integer(int(p.min), int(p.max), name=p.name))
-            elif p.type == DOUBLE:
-                dims.append(Real(float(p.min), float(p.max), name=p.name))
-            elif p.type in (CATEGORICAL, DISCRETE):
-                dims.append(Categorical(list(p.list), name=p.name))
-        self.skopt_optimizer = Optimizer(dims, base_estimator=self.base_estimator, n_initial_points=self.n_initial_points,
+        self.skopt_optimizer = Optimizer(dimensions(self.search_space), base_estimator=self.base_estimator, n_initial_points=self.n_initial_points,
                                          acq_func=self.acq_func, acq_optimizer=self.acq_optimizer, random_state=self.random_state,
                                          **self.engine_settings)
+
+    def close(self):
+        self.skopt_optimizer.close()
 
     def getSuggestions(self, trials, current_request_number):
         """trials: internal.Trial list (all completed trials, resent every call); returns a list of Assignment lists."""

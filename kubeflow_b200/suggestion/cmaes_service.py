@@ -17,10 +17,14 @@ unmatched, like extra independent draws.  With ``with_margin: true`` the sampler
 ``CmaEsSampler(with_margin=True)``): ``int`` and numeric ``discrete`` parameters become discrete dimensions whose levels
 (``cma_margin.py``) the sampler encodes on the device, and the margin α (``margin``, default 1/(D·λ)) keeps a
 coordinate from freezing on one level once σ is small.  Trials get the encoded level's value; a restart resets the margin.
+
+Each experiment's sampler is kept for one fingerprint of its search space, objective and settings: an experiment recreated
+under the same name with a changed space or changed settings starts a new run, and the old sampler is closed.  At most
+``max_experiments`` (default 64) samplers live at once; past that the least recently used is closed.  A CMA-ES run is the
+sampler's device state and cannot be rebuilt from the trials Katib resends, so an evicted experiment that comes back starts
+a new run from the initial mean and σ.
 """
 from __future__ import annotations
-
-import threading
 
 import numpy as np
 
@@ -29,7 +33,7 @@ from .internal import (CATEGORICAL, DISCRETE, DOUBLE, INTEGER, MAX_GOAL, Algorit
                        HyperParameterSearchSpace, Trial, parse_settings)
 from .cma_margin import discrete_dims, encode, parse_with_margin
 from .cma_restart import STRATEGIES, Schedule
-from .service import _Base, _reply_from
+from .service import _Base, _reply_from, experiment_fingerprint
 
 
 def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
@@ -90,13 +94,13 @@ class _Experiment:
         if self.levels:
             self.es.set_margin({j: L.cube for j, L in self.levels.items()}, settings.get("margin"))
 
+    def close(self):
+        self.es.close()
+
 
 class CmaesService(_Base):
     algorithm_names = ("cmaes",)
-
-    def __init__(self):
-        self._lock = threading.Lock()
-        self._exps = {}
+    MAX_EXPERIMENTS = 64          # an evicted run cannot be rebuilt from the trials (module docstring)
 
     @staticmethod
     def _space(experiment):
@@ -109,8 +113,7 @@ class CmaesService(_Base):
         return ss
 
     def validate(self, experiment):
-        if experiment.spec.algorithm.algorithm_name != "cmaes":
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         ss = self._space(experiment)
         if validate_cmaes_settings(parse_settings(experiment), len(ss.params)).get("with_margin", False):
             discrete_dims(ss.params)
@@ -141,14 +144,16 @@ class CmaesService(_Base):
     def get_suggestions(self, request):
         exp = request.experiment
         ss = self._space(exp)
-        settings = validate_cmaes_settings(parse_settings(exp), len(ss.params))
+        raw = parse_settings(exp)
+        settings = self.with_defaults(raw, validate_cmaes_settings(raw, len(ss.params)))
         trials = Trial.convert(request.trials)
         sign = -1.0 if ss.goal == MAX_GOAL else 1.0
         with self._lock:
-            st = self._exps.get(exp.name)
-            if st is None:
-                st = self._exps[exp.name] = _Experiment(ss, len(ss.params), settings)
+            def make():
+                st = _Experiment(ss, len(ss.params), settings)
                 self._new_generation(st, ss)
+                return st
+            st = self.experiment(exp.name, experiment_fingerprint(exp, ss, settings), make)
             for t in trials:
                 if t.name in st.seen:
                     continue

@@ -21,13 +21,12 @@ from __future__ import annotations
 import itertools
 import json
 import logging
-import threading
 
 import numpy as np
 
 from . import api_pb as api
 from .internal import AlgorithmSettingsError, Assignment, parse_settings
-from .service import _Base, _reply_from, cached_experiment
+from .service import _Base, _reply_from
 
 logger = logging.getLogger(__name__)
 
@@ -208,15 +207,8 @@ class _EnasExperiment:
 class EnasService(_Base):
     algorithm_names = (NAME,)
 
-    def __init__(self, engine_defaults: dict | None = None, max_experiments: int = 8):
-        self._lock = threading.Lock()
-        self._exps = {}                     # experiment name -> _EnasExperiment, least-recently-used first
-        self.engine_defaults = dict(engine_defaults or {})
-        self.max_experiments = int(max_experiments)
-
     def _check(self, experiment) -> tuple:
-        if experiment.spec.algorithm.algorithm_name != NAME:
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         raw = parse_settings(experiment)
         settings = validate_enas_settings(raw)
         return raw, settings, parse_nas_config(experiment)
@@ -227,15 +219,14 @@ class EnasService(_Base):
     def get_suggestions(self, request):
         exp = request.experiment
         raw, settings, (L, ins, outs, ops) = self._check(exp)
-        settings.update({k: v for k, v in self.engine_defaults.items() if k not in raw})
+        settings = self.with_defaults(raw, settings)
         k = max(int(request.current_request_number), 0)
         if k > MAX_REQUEST:
             raise AlgorithmSettingsError(f"current_request_number = {k} exceeds this engine's limit of {MAX_REQUEST} arcs per call")
         if k == 0:
             return _reply_from([])
         with self._lock:
-            st = cached_experiment(self._exps, exp.name, _fingerprint(exp, settings), lambda: _EnasExperiment(L, ins, outs, ops, settings),
-                                   lambda old: old.close(), self.max_experiments)
+            st = self.experiment(exp.name, _fingerprint(exp, settings), lambda: _EnasExperiment(L, ins, outs, ops, settings))
             if st.engine is None:
                 from ..enas import EnasController
                 ctl = {k2[len("controller_"):]: settings[k2] for k2 in ("controller_temperature", "controller_tanh_const",

@@ -71,8 +71,7 @@ class HyperbandService(_Base):
         self._calls = {}
 
     def validate(self, experiment):
-        if experiment.spec.algorithm.algorithm_name != "hyperband":
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         ss = HyperParameterSearchSpace.convert(experiment)
         p = HyperBandParam(parse_settings(experiment))
         if p.resource_name not in [q.name for q in ss.params]:
@@ -83,9 +82,7 @@ class HyperbandService(_Base):
         return str(int(round(r))) if param_spec.type == "int" else repr(float(r))
 
     def get_suggestions(self, request):
-        from ..space import Categorical, Integer, Real, Space
-        from .base_service import BaseSkoptService
-        from .internal import DOUBLE, INTEGER, Assignment
+        from .internal import Assignment
         exp = request.experiment
         ss = HyperParameterSearchSpace.convert(exp)
         p = HyperBandParam(parse_settings(exp))
@@ -129,16 +126,13 @@ class HyperbandService(_Base):
         return self._reply(lists, p)
 
     def _master(self, ss, p, res_spec, exp_name):
-        from ..space import Categorical, Integer, Real, Space
-        from .base_service import BaseSkoptService
-        from .internal import DOUBLE, INTEGER
+        from ..space import Space
+        from .base_service import BaseSkoptService, dimensions
         with self._lock:
             k = self._calls.get(exp_name, 0)
             self._calls[exp_name] = k + 1
         rng = np.random.default_rng(None if p.random_state is None else [p.random_state, p.current_s, k])
-        dims = [Integer(int(q.min), int(q.max), q.name) if q.type == INTEGER else Real(float(q.min), float(q.max), q.name)
-                if q.type == DOUBLE else Categorical(list(q.list), q.name) for q in ss.params]
-        space = Space(dims)
+        space = Space(dimensions(ss))
         pts = space.inverse_transform(space.rvs_transformed(p.n, rng, np.float64))
         out = []
         for pt in pts:

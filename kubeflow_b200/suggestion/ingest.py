@@ -16,6 +16,7 @@ objective metric) and skopt/base_service.py ``getSuggestions`` (assignment looku
 from __future__ import annotations
 
 import ctypes as C
+import weakref
 from dataclasses import dataclass
 
 import numpy as np
@@ -59,11 +60,12 @@ class LazyRequest:
         self._exp = None
         self._h = C.c_void_p()
         self._lib = L.load()
-        rc = self._lib.kbo_req_open(self._data, len(self._data), C.byref(self._h))
-        if rc != L.KBO_OK:                         # malformed: let protobuf raise its own DecodeError, as before
-            self._h = C.c_void_p()
-            self._msg = api.GetSuggestionsRequest.FromString(self._data)
+        h = C.c_void_p()
+        if self._lib.kbo_req_open(self._data, len(self._data), C.byref(h)) != L.KBO_OK:
+            self._msg = api.GetSuggestionsRequest.FromString(self._data)    # malformed: let protobuf raise its own DecodeError
             return
+        self._h = h
+        weakref.finalize(self, self._lib.kbo_req_close, h)           # the scan's host buffers go with the request
         eo, el, cur, tot, nt = C.c_uint64(), C.c_uint64(), C.c_int32(), C.c_int32(), C.c_int32()
         self._lib.kbo_req_header(self._h, C.byref(eo), C.byref(el), C.byref(cur), C.byref(tot), C.byref(nt))
         self._exp_span = (eo.value, el.value)
@@ -72,13 +74,6 @@ class LazyRequest:
     @classmethod
     def FromString(cls, data: bytes) -> "LazyRequest":
         return cls(data)
-
-    def __del__(self):
-        try:
-            if self._h:
-                self._lib.kbo_req_close(self._h)
-        except Exception:
-            pass
 
     # -- protobuf view ------------------------------------------------------------------------------------------------
     @property

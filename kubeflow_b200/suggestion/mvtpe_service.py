@@ -15,12 +15,10 @@ Katib's Optuna service is unpinned).
 """
 from __future__ import annotations
 
-import threading
-
 import numpy as np
 
 from .internal import DOUBLE, INTEGER, AlgorithmSettingsError, HyperParameterSearchSpace, parse_settings
-from .service import _Base, _reply_from, cached_experiment, experiment_fingerprint
+from .service import _Base, _reply_from, experiment_fingerprint
 from .tpe_service import _Experiment
 
 NAME = "multivariate-tpe"
@@ -103,31 +101,21 @@ class _MvExperiment(_Experiment):
 class MultivariateTpeService(_Base):
     algorithm_names = (NAME,)
 
-    def __init__(self, engine_defaults: dict | None = None, max_experiments: int = 8):
-        self._lock = threading.Lock()
-        self._exps = {}                     # experiment name -> _MvExperiment, least-recently-used first
-        self.engine_defaults = dict(engine_defaults or {})
-        self.max_experiments = int(max_experiments)   # each experiment past its start-up phase owns a libkbo handle
-
     def validate(self, experiment):
-        if experiment.spec.algorithm.algorithm_name != NAME:
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         mvtpe_space(HyperParameterSearchSpace.convert(experiment))
         validate_mvtpe_settings(parse_settings(experiment))
 
     def get_suggestions(self, request):
         exp = request.experiment
-        if exp.spec.algorithm.algorithm_name != NAME:
-            raise AlgorithmSettingsError(f"unknown algorithm name {exp.spec.algorithm.algorithm_name}")
+        self.check_algorithm(exp)
         ss = HyperParameterSearchSpace.convert(exp)
         mvtpe_space(ss)
         raw = parse_settings(exp)
-        settings = validate_mvtpe_settings(raw)
-        settings.update({k: v for k, v in self.engine_defaults.items() if k not in raw})
+        settings = self.with_defaults(raw, validate_mvtpe_settings(raw))
         k = max(int(request.current_request_number), 0)
         with self._lock:
-            st = cached_experiment(self._exps, exp.name, experiment_fingerprint(exp, ss, settings), lambda: _MvExperiment(ss, settings),
-                                   lambda old: old.close(), self.max_experiments)
+            st = self.experiment(exp.name, experiment_fingerprint(exp, ss, settings), lambda: _MvExperiment(ss, settings))
             st.ingest(request.trials, ss.goal, skip_nan=True)      # a NaN objective is a failed trial in Optuna: never told
 
             def make_engine():

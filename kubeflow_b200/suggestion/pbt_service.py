@@ -65,7 +65,7 @@ import numpy as np
 from . import api_pb as api
 from .internal import (DOUBLE, INTEGER, MAX_GOAL, AlgorithmSettingsError, Assignment, HyperParameterSearchSpace, Trial,
                        parse_settings)
-from .service import _Base, _reply_from, cached_experiment, experiment_fingerprint
+from .service import _Base, _reply_from, experiment_fingerprint
 
 logger = logging.getLogger(__name__)
 
@@ -276,18 +276,16 @@ class _PbtExperiment:
     lock: threading.Lock = field(default_factory=threading.Lock)
     issued: dict = field(default_factory=dict)    # name -> PbtTrial handed out and not yet seen in request.trials
 
+    def close(self):
+        pass
+
 
 class PbtService(_Base):
     algorithm_names = (NAME,)
-
-    def __init__(self, max_experiments: int = 64):
-        self._lock = threading.Lock()
-        self._exps = {}                     # experiment name -> _PbtExperiment, least-recently-used first
-        self.max_experiments = int(max_experiments)
+    MAX_EXPERIMENTS = 64          # an entry is a few issued names, no device memory
 
     def _check(self, experiment) -> tuple:
-        if experiment.spec.algorithm.algorithm_name != NAME:
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         return HyperParameterSearchSpace.convert(experiment), validate_pbt_settings(parse_settings(experiment))
 
     def validate(self, experiment):
@@ -304,8 +302,7 @@ class PbtService(_Base):
         if not os.path.isdir(root):
             raise AlgorithmSettingsError(f"suggestion_trial_dir {root} is not a directory")
         with self._lock:
-            entry = cached_experiment(self._exps, exp.name, experiment_fingerprint(exp, ss, st), _PbtExperiment, lambda old: None,
-                                      self.max_experiments)
+            entry = self.experiment(exp.name, experiment_fingerprint(exp, ss, st), _PbtExperiment)
         with entry.lock:
             for t in trials:
                 entry.issued.pop(t.name, None)

@@ -85,9 +85,9 @@ def main():
         local = int(os.environ.get("LOCAL_RANK", "0"))
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-        inner = DispatchService([SkoptService({"device": local, "shard": True}), RandomService(), SobolService(),
-                                 CmaesService(), TpeService({"device": local}), MultivariateTpeService({"device": local}), EnasService({"device": local}),
-                                 HyperbandService(), PbtService()])
+        dev = {"device": local}
+        inner = DispatchService([SkoptService({**dev, "shard": True}), RandomService(), SobolService(), CmaesService(dev),
+                                 TpeService(dev), MultivariateTpeService(dev), EnasService(dev), HyperbandService(), PbtService()])
         spmd = SpmdServicer(inner)
         if dist.get_rank() == 0:
             server, port = serve(spmd, args.port)
@@ -100,9 +100,9 @@ def main():
             spmd.worker_loop()
         dist.destroy_process_group()
         return
-    server, port = serve(DispatchService([SkoptService({"device": args.device}), RandomService(), SobolService(), CmaesService(),
-                                         TpeService({"device": args.device}), MultivariateTpeService({"device": args.device}),
-                                         EnasService({"device": args.device}), HyperbandService(), PbtService()]), args.port)
+    dev = {"device": args.device}
+    server, port = serve(DispatchService([SkoptService(dev), RandomService(), SobolService(), CmaesService(dev), TpeService(dev),
+                                          MultivariateTpeService(dev), EnasService(dev), HyperbandService(), PbtService()]), args.port)
     logging.info("api.v1.beta1.Suggestion listening on :%d", port)
     server.wait_for_termination()
 

@@ -125,27 +125,6 @@ def experiment_fingerprint(exp, search_space, settings: dict) -> tuple:
             tuple(sorted((k, repr(v)) for k, v in settings.items())))
 
 
-def cached_experiment(cache: dict, name: str, fingerprint, make, close, max_entries: int):
-    """The per-experiment state of ``name`` from ``cache`` (a dict kept in least-recently-used order), made by ``make()`` when
-    absent.  An experiment recreated under the same name, or whose search space / objective / settings changed, must not meet
-    the old state (old dimensions, old history, old settings): an entry is valid for one fingerprint only, and a stale one is
-    closed and replaced.  Each entry may own a libkbo handle (device memory), so past ``max_entries`` the least recently used
-    entries are closed and dropped.  Call with the service's lock held."""
-    entry = cache.get(name)
-    if entry is not None and entry.fingerprint != fingerprint:
-        close(cache.pop(name))
-        entry = None
-    if entry is None:
-        entry = make()
-        entry.fingerprint = fingerprint
-        cache[name] = entry
-        while len(cache) > max_entries:
-            close(cache.pop(next(iter(cache))))
-    else:
-        cache[name] = cache.pop(name)      # mark as most recently used
-    return entry
-
-
 def _reply_from(assignment_lists) -> "api.GetSuggestionsReply":
     reply = api.GetSuggestionsReply()
     for assignments in assignment_lists:
@@ -157,7 +136,45 @@ def _reply_from(assignment_lists) -> "api.GetSuggestionsReply":
 
 
 class _Base:
+    """A servicer for ``algorithm_names``.  The services that keep per-experiment state hold it in ``_exps`` (experiment name ->
+    entry with ``close()``, least recently used first), reached through ``experiment()`` under ``_lock``; ``engine_defaults``
+    are settings (``device``, ...) an Experiment may override."""
     algorithm_names: tuple = ()
+    MAX_EXPERIMENTS = 8           # entries own libkbo handles (device memory): bound how many live at once
+
+    def __init__(self, engine_defaults: dict | None = None, max_experiments: int | None = None):
+        self._lock = threading.Lock()       # handlers may run concurrently (grpc thread pool): GPU work is serialised here
+        self._exps = {}
+        self.engine_defaults = dict(engine_defaults or {})
+        self.max_experiments = int(self.MAX_EXPERIMENTS if max_experiments is None else max_experiments)
+
+    def check_algorithm(self, experiment, allow_empty: bool = False):
+        name = experiment.spec.algorithm.algorithm_name
+        if name not in self.algorithm_names and not (allow_empty and name == ""):
+            raise AlgorithmSettingsError(f"unknown algorithm name {name}")
+
+    def with_defaults(self, raw: dict, settings: dict) -> dict:
+        """``settings`` (parsed from the Experiment's ``raw`` settings) plus the engine defaults it does not set."""
+        return {**settings, **{k: v for k, v in self.engine_defaults.items() if k not in raw}}
+
+    def experiment(self, name: str, fingerprint, make):
+        """The per-experiment state of ``name``, made by ``make()`` when absent.  An experiment recreated under the same name,
+        or whose search space / objective / settings changed, must not meet the old state (old dimensions, old history, old
+        settings): an entry is valid for one fingerprint only, and a stale one is closed and replaced.  Past
+        ``max_experiments`` the least recently used entries are closed and dropped.  Call with ``_lock`` held."""
+        entry = self._exps.get(name)
+        if entry is not None and entry.fingerprint != fingerprint:
+            self._exps.pop(name).close()
+            entry = None
+        if entry is None:
+            entry = make()
+            entry.fingerprint = fingerprint
+            self._exps[name] = entry
+            while len(self._exps) > self.max_experiments:
+                self._exps.pop(next(iter(self._exps))).close()
+        else:
+            self._exps[name] = self._exps.pop(name)      # mark as most recently used
+        return entry
 
     def _abort(self, context, code, msg):
         logger.warning("%s: %s", code, msg)
@@ -189,42 +206,34 @@ class _Base:
 class SkoptService(_Base):
     algorithm_names = ("bayesianoptimization",)
 
-    def __init__(self, engine_defaults: dict | None = None, max_experiments: int = 8):
-        self._lock = threading.Lock()       # handlers may run concurrently (grpc thread pool): GPU work is serialised here
-        self._services = {}                 # experiment name -> BaseSkoptService, least-recently-used first
-        self.engine_defaults = dict(engine_defaults or {})
+    def __init__(self, engine_defaults: dict | None = None, max_experiments: int | None = None):
+        super().__init__(engine_defaults, max_experiments)
         self.last_ingest = None             # "scan" | "messages": how the last request's trials reached the optimizer
-        self.max_experiments = int(max_experiments)   # each experiment owns a libkbo handle (K, W, scratch): bound the device memory
+
+    @property
+    def _services(self) -> dict:
+        """experiment name -> BaseSkoptService (the per-experiment cache under the name the benchmark and tests read)."""
+        return self._exps
 
     def validate(self, experiment):
-        name = experiment.spec.algorithm.algorithm_name
-        if name != "bayesianoptimization":
-            raise AlgorithmSettingsError(f"unknown algorithm name {name}")
+        self.check_algorithm(experiment)
         search_space = HyperParameterSearchSpace.convert(experiment)
         check_kernel_space(validate_skopt_settings(parse_settings(experiment)), search_space)
 
     def get_suggestions(self, request):
-        exp = request.experiment
-        if exp.spec.algorithm.algorithm_name not in ("", "bayesianoptimization"):
-            raise AlgorithmSettingsError(f"unknown algorithm name {exp.spec.algorithm.algorithm_name}")
-        search_space = HyperParameterSearchSpace.convert(exp)
-        settings = validate_skopt_settings(parse_settings(exp))
-        check_kernel_space(settings, search_space)
+        from .base_service import BaseSkoptService
         from .ingest import LazyRequest
+        exp = request.experiment
+        self.check_algorithm(exp, allow_empty=True)
+        search_space = HyperParameterSearchSpace.convert(exp)
+        raw = parse_settings(exp)
+        settings = validate_skopt_settings(raw)
+        check_kernel_space(settings, search_space)
         lazy = request if isinstance(request, LazyRequest) and request.scanned else None
         fingerprint = experiment_fingerprint(exp, search_space, settings)
         with self._lock:
-            def make():
-                kw = dict(self.engine_defaults)
-                kw.update(settings)
-                from .base_service import BaseSkoptService
-                return BaseSkoptService(search_space=search_space, **kw)
-
-            def close(old):
-                eng = getattr(old.skopt_optimizer, "_engine", None)
-                if eng is not None:
-                    eng.close()
-            svc = cached_experiment(self._services, exp.name, fingerprint, make, close, self.max_experiments)
+            svc = self.experiment(exp.name, fingerprint,
+                                  lambda: BaseSkoptService(search_space=search_space, **self.with_defaults(raw, settings)))
             # the wire scan tells the new trials from flat arrays; it declines (False) whenever a trial needs the message walk
             self.last_ingest = "scan" if (lazy is not None and svc.ingest(lazy)) else "messages"
             trials = [] if self.last_ingest == "scan" else Trial.convert(request.trials, skip_names=svc.told_trials)
@@ -235,11 +244,9 @@ class SkoptService(_Base):
 def prior_points(ss, rng, n: int) -> list:
     """n uniform random points of the search space (integers uniform over [min, max], categories uniform), in parameter
     values — the sampling of Katib's ``random`` algorithm, shared with ``tpe``'s start-up phase."""
-    from ..space import Categorical, Integer, Real, Space
-    from .internal import DOUBLE, INTEGER
-    dims = [Integer(int(p.min), int(p.max), p.name) if p.type == INTEGER else
-            Real(float(p.min), float(p.max), p.name) if p.type == DOUBLE else Categorical(list(p.list), p.name) for p in ss.params]
-    space = Space(dims)
+    from ..space import Space
+    from .base_service import dimensions
+    space = Space(dimensions(ss))
     return space.inverse_transform(space.rvs_transformed(n, rng, np.float64)) if n else []
 
 
@@ -252,8 +259,7 @@ class RandomService(_Base):
         self._lock = threading.Lock()
 
     def validate(self, experiment):
-        if experiment.spec.algorithm.algorithm_name != "random":
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         HyperParameterSearchSpace.convert(experiment)
         for k, v in parse_settings(experiment).items():
             if k != "random_state":
@@ -289,8 +295,7 @@ class SobolService(_Base):
         self._issued = {}
 
     def validate(self, experiment):
-        if experiment.spec.algorithm.algorithm_name != "sobol":
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         ss = HyperParameterSearchSpace.convert(experiment)
         for p in ss.params:
             if p.type in ("categorical", "discrete") and len(p.list) < 1:
@@ -306,9 +311,8 @@ class SobolService(_Base):
 
     def get_suggestions(self, request):
         from scipy.stats import qmc
-        from ..space import Categorical, Integer, Real, Space
-        from .base_service import BaseSkoptService
-        from .internal import DOUBLE, INTEGER
+        from ..space import Categorical, Integer
+        from .base_service import BaseSkoptService, dimensions
         exp = request.experiment
         ss = HyperParameterSearchSpace.convert(exp)
         st = parse_settings(exp)
@@ -322,8 +326,7 @@ class SobolService(_Base):
         if start:
             eng.fast_forward(start)
         U = eng.random(n)
-        dims = [Integer(int(p.min), int(p.max), p.name) if p.type == INTEGER else Real(float(p.min), float(p.max), p.name)
-                if p.type == DOUBLE else Categorical(list(p.list), p.name) for p in ss.params]
+        dims = dimensions(ss)
         pts = []
         for u in U:
             pt = []

@@ -16,13 +16,11 @@ the GPU engine ``kubeflow_b200.tpe`` (contract: oracle/tpe_oracle.py).
 """
 from __future__ import annotations
 
-import threading
-
 import numpy as np
 
 from .internal import (DISCRETE, DOUBLE, INTEGER, MAX_GOAL, AlgorithmSettingsError, HyperParameterSearchSpace, Trial,
                        parse_settings, Assignment)
-from .service import _Base, _reply_from, cached_experiment, experiment_fingerprint, prior_points
+from .service import _Base, _reply_from, experiment_fingerprint, prior_points
 
 MAX_EI_CANDIDATES = 1 << 24
 
@@ -169,31 +167,21 @@ def _same_number(a: str, b: str) -> bool:
 class TpeService(_Base):
     algorithm_names = ("tpe",)
 
-    def __init__(self, engine_defaults: dict | None = None, max_experiments: int = 8):
-        self._lock = threading.Lock()
-        self._exps = {}                     # experiment name -> _Experiment, least-recently-used first
-        self.engine_defaults = dict(engine_defaults or {})
-        self.max_experiments = int(max_experiments)   # each experiment past its start-up phase owns a libkbo handle
-
     def validate(self, experiment):
-        if experiment.spec.algorithm.algorithm_name != "tpe":
-            raise AlgorithmSettingsError(f"unknown algorithm name {experiment.spec.algorithm.algorithm_name}")
+        self.check_algorithm(experiment)
         tpe_space(HyperParameterSearchSpace.convert(experiment))
         validate_tpe_settings(parse_settings(experiment))
 
     def get_suggestions(self, request):
         exp = request.experiment
-        if exp.spec.algorithm.algorithm_name != "tpe":
-            raise AlgorithmSettingsError(f"unknown algorithm name {exp.spec.algorithm.algorithm_name}")
+        self.check_algorithm(exp)
         ss = HyperParameterSearchSpace.convert(exp)
         tpe_space(ss)
         raw = parse_settings(exp)
-        settings = validate_tpe_settings(raw)
-        settings.update({k: v for k, v in self.engine_defaults.items() if k not in raw})
+        settings = self.with_defaults(raw, validate_tpe_settings(raw))
         k = max(int(request.current_request_number), 0)
         with self._lock:
-            st = cached_experiment(self._exps, exp.name, experiment_fingerprint(exp, ss, settings), lambda: _Experiment(ss, settings),
-                                   lambda old: old.close(), self.max_experiments)
+            st = self.experiment(exp.name, experiment_fingerprint(exp, ss, settings), lambda: _Experiment(ss, settings))
             st.ingest(request.trials, ss.goal)
 
             def make_engine():

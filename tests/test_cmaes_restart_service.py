@@ -49,6 +49,9 @@ class _FlagEs:
     def state(self):
         return {"mean": np.full(self.D, 0.5), "sigma": 0.1, "B": np.eye(self.D), "d": np.ones(self.D)}
 
+    def close(self):
+        pass
+
 
 @pytest.fixture
 def fake(monkeypatch):

@@ -231,6 +231,9 @@ class _FakeEs:
     def state(self):
         return {"mean": np.full(self.D, 0.5), "sigma": 0.1, "B": np.eye(self.D), "d": np.ones(self.D)}
 
+    def close(self):
+        pass
+
 
 def test_cmaes_generation_survives_duplicate_assignments_and_failed_trials(monkeypatch):
     import kubeflow_b200.cmaes as cm
