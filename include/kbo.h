@@ -333,7 +333,16 @@ uint64_t kbo_hash64(const void* bytes, uint64_t len);   /* the FNV-1a hash kbo_r
  * holds it); the tell's mean step is m + c_m·σ·A∘y_w, and after the eigendecomposition a one-CTA kernel corrects m_j and
  * A_j of each discrete dimension (oracle/cma_margin_oracle.py).  A starts at 1 and a restart resets it.  n_discrete = 0
  * turns the margin off: every kernel is then the margin-free one.  Not between an ask and its tell (KBO_ERR_STATE).
- * kbo_cma_margin_state copies A, the mean before the last correction and α to HOST (any may be NULL) and synchronises. */
+ * kbo_cma_margin_state copies A, the mean before the last correction and α to HOST (any may be NULL) and synchronises.
+ * Margin dimensions are refused (KBO_ERR_INVALID) while learning-rate adaptation is on.
+ * kbo_cma_set_lr_adapt turns learning-rate adaptation on (on != 0) or off (LRA-CMA-ES, Nomura, Akimoto & Ono, GECCO 2023,
+ * as in CyberAgent `cmaes`; oracle/cma_lra_oracle.py).  Each tell then blends the plain update with the state it started
+ * from: m ← m + η_m·Δm, Σ ← σ²C + η_Σ·ΔΣ, with η_m and η_Σ in (0, 1] driven by the signal-to-noise ratios of moving
+ * averages of Δm and ΔΣ in the local coordinates Σ^{-1/2}; σ is taken from log det Σ so that det C = 1, then scaled by
+ * η_m(before)/η_m(after).  Turning it on or off resets E = V = 0 and η = 1, and so does every restart.  Not between an
+ * ask and its tell (KBO_ERR_STATE); refused with margin dimensions set (KBO_ERR_INVALID).  Off, no LRA work is done.
+ * kbo_cma_lra_state copies E_m (D), E_Σ (D×D), V = (V_m, V_Σ) and eta = (η_m, η_Σ) to HOST (any may be NULL) and
+ * synchronises; KBO_ERR_STATE while the adaptation is off. */
 typedef struct kbo_cma kbo_cma;
 int kbo_cma_create(kbo_handle* h, kbo_cma** out, int32_t D, int32_t lambda, const double* mean0_host, double sigma0, uint64_t seed);
 void kbo_cma_destroy(kbo_cma* c);
@@ -348,6 +357,9 @@ int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32
 int kbo_cma_set_margin(kbo_handle* h, kbo_cma* c, int32_t n_discrete, const int32_t* dims, const int64_t* level_offsets,
                        const double* levels, const double* arith, double alpha);
 int kbo_cma_margin_state(kbo_handle* h, kbo_cma* c, double* A_host, double* mean_before_host, double* alpha_host, void* stream);
+int kbo_cma_set_lr_adapt(kbo_handle* h, kbo_cma* c, int32_t on);
+int kbo_cma_lra_state(kbo_handle* h, kbo_cma* c, double* E_mean_host, double* E_Sigma_host, double* V_host, double* eta_host,
+                      void* stream);
 
 /* ---- TPE (Katib algorithm `tpe`: hyperopt's tpe.suggest on a flat space; FP64 restatement oracle/tpe_oracle.py) -------
  * Parameter kinds: UNIFORM = uniform(lo, hi); QUNIFORM = quniform(lo, hi, q), values rint(x/q)·q; CHOICE = choice over

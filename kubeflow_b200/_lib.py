@@ -58,7 +58,8 @@ EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_se
            "kbo_gram", "kbo_potrf", "kbo_trtri", "kbo_acq_argmax",
            "kbo_req_open", "kbo_req_close", "kbo_req_header", "kbo_req_trials", "kbo_hash64",
            "kbo_cma_create", "kbo_cma_destroy", "kbo_cma_ask", "kbo_cma_tell", "kbo_cma_state", "kbo_cma_run_synthetic",
-           "kbo_cma_stop_flags", "kbo_cma_restart", "kbo_cma_set_margin", "kbo_cma_margin_state",
+           "kbo_cma_stop_flags", "kbo_cma_restart", "kbo_cma_set_margin", "kbo_cma_margin_state", "kbo_cma_set_lr_adapt",
+           "kbo_cma_lra_state",
            "kbo_tpe_create", "kbo_tpe_destroy", "kbo_tpe_tell", "kbo_tpe_ask", "kbo_tpe_state", "kbo_tpe_last_survivors", "kbo_tpe_last_timings",
            "kbo_mvtpe_create", "kbo_mvtpe_destroy", "kbo_mvtpe_tell", "kbo_mvtpe_ask", "kbo_mvtpe_state", "kbo_mvtpe_last_survivors",
            "kbo_mvtpe_last_timings",
@@ -163,6 +164,8 @@ def load() -> C.CDLL:
     lib.kbo_cma_restart.argtypes = [vp, vp, i32, pd, dbl]
     lib.kbo_cma_set_margin.argtypes = [vp, vp, i32, vp, vp, vp, vp, dbl]
     lib.kbo_cma_margin_state.argtypes = [vp, vp, vp, vp, pd, vp]
+    lib.kbo_cma_set_lr_adapt.argtypes = [vp, vp, i32]
+    lib.kbo_cma_lra_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
     lib.kbo_tpe_create.argtypes = [vp, C.POINTER(vp), i32, vp, vp, vp, vp, vp, dbl, dbl, C.c_uint64]
     lib.kbo_tpe_destroy.argtypes = [vp]
     lib.kbo_tpe_destroy.restype = None

@@ -104,6 +104,20 @@ class CmaEs(L.Handle):
                                                  self._stream()))
         return dict(A=A, mean_before=mb, alpha=alpha.value)
 
+    def set_lr_adapt(self, on: bool):
+        """Learning-rate adaptation (LRA-CMA-ES, Optuna's ``CmaEsSampler(lr_adapt=True)``) on or off; either way the
+        adaptation's state starts afresh (E = V = 0, η = 1), as it does at every restart.  Not between an ask and its
+        tell, and not with a margin set."""
+        self.check(self.lib.kbo_cma_set_lr_adapt(self._h, self._o, 1 if on else 0))
+
+    def lr_state(self) -> dict:
+        """The adaptation's state after the last tell: E_mean (D), E_Sigma (D×D), V_mean, V_Sigma, eta_mean, eta_Sigma
+        (needs set_lr_adapt(True))."""
+        Em, ES, V, eta = np.empty(self.D), np.empty((self.D, self.D)), np.empty(2), np.empty(2)
+        self.check(self.lib.kbo_cma_lra_state(self._h, self._o, Em.ctypes.data, ES.ctypes.data, V.ctypes.data, eta.ctypes.data,
+                                              self._stream()))
+        return dict(E_mean=Em, E_Sigma=ES, V_mean=float(V[0]), V_Sigma=float(V[1]), eta_mean=float(eta[0]), eta_Sigma=float(eta[1]))
+
     def run_synthetic(self, fitness: str, generations: int):
         """BASELINE config 4: `generations` full generations on the device with a built-in fitness."""
         kind = {"sphere": 0, "rastrigin": 1}[fitness]

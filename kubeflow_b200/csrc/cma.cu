@@ -32,6 +32,11 @@ struct kbo_cma {
   int n_disc = 0;
   double alpha = 0.0, alpha_set = 0.0;  // alpha_set: the caller's α, or 0 for the default 1/(D·λ) recomputed at restarts
   DevBuf A, mdim, mlev, mprev, mpre;    // A; per-dimension level descriptors; level tables; (m, σ) before the tell; m before the correction
+  // learning-rate adaptation (kbo_cma_set_lr_adapt): off while !lra, and then no LRA buffer is touched
+  bool lra = false;
+  DevBuf lprev, lC0;                    // (m, σ) and C before the tell
+  DevBuf lW, lP, lS, lT, lL;            // B·diag(1/d); P₀ = C^{-1/2}; S = ΔΣ/σ′²; P₀·S; P₀·S·P₀ (all D×D)
+  DevBuf lE, lscal;                     // E_m (D) then E_Σ (D×D); V_m, V_Σ, η_m, η_Σ, η_m before the last tell
 };
 
 // A discrete dimension's sorted levels in cube coordinates: levels[off, off + count) of the table, or, for ranges too long
@@ -574,6 +579,141 @@ __global__ void __launch_bounds__(CMA_MAXD) cma_margin_kernel(const double* __re
   mean[t] = m;
 }
 
+// ------------------------------------------------------------------------------------------------ learning-rate adaptation (LRA)
+// LRA-CMA-ES (Nomura, Akimoto & Ono, GECCO 2023) as in CyberAgent `cmaes`: oracle/cma_lra_oracle.py states each rule.
+// The covariance side works in units of the plain update's σ′²: S = ΔΣ/σ′² = C′ − r²·C with r = σ/σ′, and the blended
+// Σ/σ′² = r²·C + η_Σ·S goes into C for the unchanged eigendecomposition, so no σ² is ever formed.
+#define LRA_ALPHA 1.4
+#define LRA_BETA_M 0.1
+#define LRA_BETA_S 0.03
+#define LRA_GAMMA 0.1
+#define LRA_SIGMA_MAX 1e32
+enum LraScal { LS_V_M = 0, LS_V_S = 1, LS_ETA_M = 2, LS_ETA_S = 3, LS_ETA_M_PREV = 4, LS_COUNT = 5 };
+
+// W = B·diag(1/d) of the basis from before the tell (P₀ = W·Bᵀ = C^{-1/2}), and S = C′ − r²·C_prev (exactly symmetric)
+__global__ void cma_lra_prep_kernel(const double* __restrict__ B, const double* __restrict__ Dv, const double* __restrict__ C,
+                                    const double* __restrict__ C0, const double* __restrict__ prev, const double* __restrict__ scal, int D,
+                                    double* __restrict__ W, double* __restrict__ S) {
+  const int i = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= D) return;
+  const double r = prev[D] / scal[CS_SIGMA];
+  const size_t e = (size_t)i * D + j;
+  W[e] = B[e] / Dv[j];
+  S[e] = C[e] - (r * r) * C0[e];
+}
+
+// The next η from one moving average's ‖E‖² and V; when V − ‖E‖² is not positive and finite, η stays (a stated departure)
+__device__ __forceinline__ double cma_lra_eta(double eta, double E2, double V, double beta) {
+  const double den = V - E2;
+  if (!(den > 0.0 && den < INFINITY)) return eta;
+  const double snr = (E2 - beta / (2.0 - beta) * V) / den;
+  const double rel = fmin(fmax(snr / LRA_ALPHA / eta - 1.0, -1.0), 1.0);
+  return fmin(eta * exp(fmin(LRA_GAMMA * eta, beta) * rel), 1.0);
+}
+
+// One CTA, after cma_c_finalize_kernel (mean = m′, σ′ in scal, C = C′) and the three products (L = P₀·S·P₀): local
+// differences Δ̃m = P₀·Δm/σ and Δ̃Σ = L/(r²·√2), the moving averages, both SNRs and η, then m ← m + η_m·Δm and
+// C ← r²·C_prev + η_Σ·S.  Per-thread sums in a fixed stride order, then a fixed tree: no atomics.
+__global__ void __launch_bounds__(1024) cma_lra_kernel(const double* __restrict__ prev, const double* __restrict__ C0,
+                                                       const double* __restrict__ P, const double* __restrict__ S,
+                                                       const double* __restrict__ L, const double* __restrict__ scal, int D,
+                                                       double* __restrict__ E, double* __restrict__ ls, double* __restrict__ mean,
+                                                       double* __restrict__ C) {
+  __shared__ double dm[CMA_MAXD], red[4][1024];
+  __shared__ double s_eta[2];
+  const int t = threadIdx.x;
+  const double s0 = prev[D], r = s0 / scal[CS_SIGMA];
+  const double cs = 0.7071067811865476 / (r * r);
+  if (t < D) dm[t] = mean[t] - prev[t];
+  __syncthreads();
+  double a = 0.0, b = 0.0, a2 = 0.0, b2 = 0.0;
+  if (t < D) {
+    double u = 0.0;
+    for (int j = 0; j < D; j++) u = fma(P[(size_t)t * D + j], dm[j], u);
+    const double x = u / s0;
+    const double e = (1.0 - LRA_BETA_M) * E[t] + LRA_BETA_M * x;
+    E[t] = e;
+    a = x * x;
+    b = e * e;
+  }
+  double* ES = E + D;
+  for (int k = t; k < D * D; k += 1024) {
+    const double x = cs * L[k];
+    const double e = (1.0 - LRA_BETA_S) * ES[k] + LRA_BETA_S * x;
+    ES[k] = e;
+    a2 = fma(x, x, a2);
+    b2 = fma(e, e, b2);
+  }
+  red[0][t] = a; red[1][t] = b; red[2][t] = a2; red[3][t] = b2;
+  __syncthreads();
+  for (int o = 512; o > 0; o >>= 1) {
+    if (t < o)
+      for (int q = 0; q < 4; q++) red[q][t] += red[q][t + o];
+    __syncthreads();
+  }
+  if (t == 0) {
+    const double vm = (1.0 - LRA_BETA_M) * ls[LS_V_M] + LRA_BETA_M * red[0][0];
+    const double vs = (1.0 - LRA_BETA_S) * ls[LS_V_S] + LRA_BETA_S * red[2][0];
+    const double em = ls[LS_ETA_M];
+    ls[LS_V_M] = vm;
+    ls[LS_V_S] = vs;
+    ls[LS_ETA_M_PREV] = em;
+    s_eta[0] = ls[LS_ETA_M] = cma_lra_eta(em, red[1][0], vm, LRA_BETA_M);
+    s_eta[1] = ls[LS_ETA_S] = cma_lra_eta(ls[LS_ETA_S], red[3][0], vs, LRA_BETA_S);
+  }
+  __syncthreads();
+  const double eta_m = s_eta[0], eta_s = s_eta[1], r2 = r * r;
+  if (t < D) mean[t] = fma(eta_m, dm[t], prev[t]);
+  for (int k = t; k < D * D; k += 1024) C[k] = fma(eta_s, S[k], r2 * C0[k]);
+}
+
+// One CTA, after cma_eigval_kernel on the blended C = Σ/σ′²: σ = σ′·exp(Σ_j log d_j / D) (= exp(log det Σ / 2D), d_j²
+// floored as cma_eigval_kernel floors), capped; C and d are divided by g = (σ/σ′)² and √g, so det C = 1; then the
+// step-size correction σ·η_m(before)/η_m(after).  Runs before cma_stop_kernel, which reads the final state.
+__global__ void __launch_bounds__(1024) cma_lra_finish_kernel(const double* __restrict__ ls, int D, double* __restrict__ Dv,
+                                                              double* __restrict__ C, double* __restrict__ scal) {
+  __shared__ double red[CMA_MAXD];
+  __shared__ double s_r;
+  const int t = threadIdx.x;
+  if (t < CMA_MAXD) red[t] = t < D ? log(Dv[t]) : 0.0;
+  __syncthreads();
+  for (int o = CMA_MAXD / 2; o > 0; o >>= 1) {
+    if (t < o) red[t] += red[t + o];
+    __syncthreads();
+  }
+  if (t == 0) {
+    const double s1 = scal[CS_SIGMA];
+    double sn = s1 * exp(red[0] / D);
+    if (sn > LRA_SIGMA_MAX) sn = LRA_SIGMA_MAX;
+    s_r = sn / s1;
+    scal[CS_SIGMA] = sn * ls[LS_ETA_M_PREV] / ls[LS_ETA_M];
+  }
+  __syncthreads();
+  const double rr = s_r, g = rr * rr;
+  if (t < D) Dv[t] = Dv[t] / rr;
+  for (int k = t; k < D * D; k += 1024) C[k] = C[k] / g;
+}
+
+// The LRA step between cma_c_finalize_kernel and the eigendecomposition: W and S, P₀ = W·Bᵀ, L = (P₀·S)·P₀, the blend
+static int cma_lra_blend(kbo_handle* h, kbo_cma* c, cudaStream_t s) {
+  const int D = c->D;
+  double *W = (double*)c->lW.p, *P = (double*)c->lP.p, *S = (double*)c->lS.p, *T = (double*)c->lT.p, *L = (double*)c->lL.p;
+  cma_lra_prep_kernel<<<dim3((D + 127) / 128, D), 128, 0, s>>>((const double*)c->B.p, (const double*)c->Dv.p, (const double*)c->C.p,
+                                                                (const double*)c->lC0.p, (const double*)c->lprev.p,
+                                                                (const double*)c->scal.p, D, W, S);
+  KBO_LAUNCH_CHECK(h);
+  dgemm64_launch<true, EPI_STORE>(s, D, D, D, W, D, (const double*)c->B.p, D, P, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
+  KBO_LAUNCH_CHECK(h);
+  dgemm64_launch<false, EPI_STORE>(s, D, D, D, P, D, S, D, T, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
+  KBO_LAUNCH_CHECK(h);
+  dgemm64_launch<false, EPI_STORE>(s, D, D, D, T, D, P, D, L, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
+  KBO_LAUNCH_CHECK(h);
+  cma_lra_kernel<<<1, 1024, 0, s>>>((const double*)c->lprev.p, (const double*)c->lC0.p, P, S, L, (const double*)c->scal.p, D,
+                                    (double*)c->lE.p, (double*)c->lscal.p, (double*)c->mean.p, (double*)c->C.p);
+  KBO_LAUNCH_CHECK(h);
+  return KBO_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness, cudaStream_t s) {
   const int D = c->D, lam = c->lambda;
@@ -588,6 +728,11 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
     KBO_CUDA(h, cudaMemcpyAsync(c->mprev.p, c->mean.p, 8 * (size_t)D, cudaMemcpyDeviceToDevice, s));
     KBO_CUDA(h, cudaMemcpyAsync((double*)c->mprev.p + D, c->scal.p, 8, cudaMemcpyDeviceToDevice, s));
   }
+  if (c->lra) {      // (m, σ) and C the update starts from, for the learning-rate adaptation after it
+    KBO_CUDA(h, cudaMemcpyAsync(c->lprev.p, c->mean.p, 8 * (size_t)D, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, cudaMemcpyAsync((double*)c->lprev.p + D, c->scal.p, 8, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, cudaMemcpyAsync(c->lC0.p, c->C.p, 8 * (size_t)D * D, cudaMemcpyDeviceToDevice, s));
+  }
   cma_update_kernel<<<1, 1024, 0, s>>>((const double*)c->Ys.p, (const double*)c->weights.p, D, k, (double*)c->mean.p, (const double*)c->B.p,
                                        (const double*)c->Dv.p, (double*)c->ps.p, (double*)c->pc.p, (double*)c->scal.p, (double*)c->yw.p);
   KBO_LAUNCH_CHECK(h);
@@ -601,6 +746,7 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
   cma_c_finalize_kernel<<<g, 128, 0, s>>>((double*)c->C.p, (const double*)c->R.p, nsl, (const double*)c->pc.p, (const double*)c->scal.p, D, c->c1,
                                           c->cmu);
   KBO_LAUNCH_CHECK(h);
+  if (c->lra) KBO_TRY(cma_lra_blend(h, c, s));   // B and Dv are still C_prev's here; C becomes the blended Σ/σ′²
   // G = C·B_prev, then Jacobi
   dgemm64_launch<false, EPI_STORE>(s, D, D, D, (const double*)c->C.p, D, (const double*)c->B.p, D, (double*)c->G.p, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
   KBO_LAUNCH_CHECK(h);
@@ -616,6 +762,10 @@ static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness,
     cma_margin_kernel<<<1, CMA_MAXD, 0, s>>>((const double*)c->mprev.p, (const double*)c->yw.p, c->cm, (const double*)c->scal.p,
                                              (const double*)c->C.p, (const CmaMarginDim*)c->mdim.p, (const double*)c->mlev.p, D, c->alpha,
                                              (double*)c->mean.p, (double*)c->A.p, (double*)c->mpre.p);
+    KBO_LAUNCH_CHECK(h);
+  }
+  if (c->lra) {
+    cma_lra_finish_kernel<<<1, 1024, 0, s>>>((const double*)c->lscal.p, D, (double*)c->Dv.p, (double*)c->C.p, (double*)c->scal.p);
     KBO_LAUNCH_CHECK(h);
   }
   cma_stop_kernel<<<1, CMA_MAXD, 0, s>>>(fitness, (const int*)c->order.p, lam, D, (const double*)c->mean.p, (const double*)c->C.p,
@@ -741,7 +891,53 @@ static int cma_margin_reset(kbo_handle* h, kbo_cma* c) {
   return KBO_OK;
 }
 
+// A run's LRA state: E = 0, V = 0, η = 1 (synchronous)
+static int cma_lra_reset(kbo_handle* h, kbo_cma* c) {
+  if (!c->lra) return KBO_OK;
+  const double ls[LS_COUNT] = {0.0, 0.0, 1.0, 1.0, 1.0};
+  KBO_CUDA(h, cudaMemset(c->lE.p, 0, 8 * (size_t)c->D * (c->D + 1)));
+  KBO_CUDA(h, cudaMemcpy(c->lscal.p, ls, sizeof ls, cudaMemcpyHostToDevice));
+  return KBO_OK;
+}
+
 extern "C" {
+
+int kbo_cma_set_lr_adapt(kbo_handle* h, kbo_cma* c, int32_t on) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (c->asked) KBO_FAIL(h, KBO_ERR_STATE, "kbo_cma_set_lr_adapt: the last ask has not been told");
+  if (on && c->n_disc) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_lr_adapt: learning-rate adaptation is not available with margin dimensions");
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  KBO_CUDA(h, cudaDeviceSynchronize());            // a tell in flight may still use the state about to be reset
+  c->lra = false;
+  if (!on) return KBO_OK;
+  const size_t D = c->D, DD = 8 * D * D;
+  KBO_TRY(kbo_reserve(h, c->lprev, 8 * (D + 1)));
+  KBO_TRY(kbo_reserve(h, c->lC0, DD));
+  KBO_TRY(kbo_reserve(h, c->lW, DD));
+  KBO_TRY(kbo_reserve(h, c->lP, DD));
+  KBO_TRY(kbo_reserve(h, c->lS, DD));
+  KBO_TRY(kbo_reserve(h, c->lT, DD));
+  KBO_TRY(kbo_reserve(h, c->lL, DD));
+  KBO_TRY(kbo_reserve(h, c->lE, 8 * D * (D + 1)));
+  KBO_TRY(kbo_reserve(h, c->lscal, 8 * LS_COUNT));
+  c->lra = true;
+  return cma_lra_reset(h, c);
+}
+
+int kbo_cma_lra_state(kbo_handle* h, kbo_cma* c, double* E_mean_host, double* E_Sigma_host, double* V_host, double* eta_host, void* stream) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (!c->lra) KBO_FAIL(h, KBO_ERR_STATE, "kbo_cma_lra_state: learning-rate adaptation is off");
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t D = c->D;
+  double ls[LS_COUNT];
+  if (E_mean_host) KBO_CUDA(h, cudaMemcpyAsync(E_mean_host, c->lE.p, 8 * D, cudaMemcpyDeviceToHost, s));
+  if (E_Sigma_host) KBO_CUDA(h, cudaMemcpyAsync(E_Sigma_host, (double*)c->lE.p + D, 8 * D * D, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaMemcpyAsync(ls, c->lscal.p, sizeof ls, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (V_host) { V_host[0] = ls[LS_V_M]; V_host[1] = ls[LS_V_S]; }
+  if (eta_host) { eta_host[0] = ls[LS_ETA_M]; eta_host[1] = ls[LS_ETA_S]; }
+  return KBO_OK;
+}
 
 int kbo_cma_set_margin(kbo_handle* h, kbo_cma* c, int32_t n_discrete, const int32_t* dims, const int64_t* level_offsets,
                        const double* levels, const double* arith, double alpha) {
@@ -749,6 +945,7 @@ int kbo_cma_set_margin(kbo_handle* h, kbo_cma* c, int32_t n_discrete, const int3
   if (c->asked) KBO_FAIL(h, KBO_ERR_STATE, "kbo_cma_set_margin: the last ask has not been told");
   if (n_discrete < 0 || n_discrete > c->D) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: 0 <= n_discrete <= D required (got %d)", n_discrete);
   if (!(alpha == 0.0 || (alpha > 0.0 && alpha < 1.0))) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: alpha must be in (0, 1), or 0 for 1/(D*lambda)");
+  if (n_discrete && c->lra) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: margin dimensions are not available with learning-rate adaptation");
   if (n_discrete && (!dims || !level_offsets)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_set_margin: dims and level_offsets must be given");
   const int D = c->D;
   std::vector<CmaMarginDim> md(D, CmaMarginDim{0.0, 0.0, 0, 0, 0});
@@ -828,6 +1025,7 @@ int kbo_cma_restart(kbo_handle* h, kbo_cma* c, int32_t lambda, const double* mea
   KBO_CUDA(h, cudaDeviceSynchronize());            // the last tell may still be reading buffers that are about to grow
   KBO_TRY(cma_configure(h, c, lambda, sigma0));
   KBO_TRY(cma_margin_reset(h, c));
+  KBO_TRY(cma_lra_reset(h, c));
   return cma_start_run(h, c, mean0, sigma0);
 }
 

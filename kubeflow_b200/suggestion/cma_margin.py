@@ -14,10 +14,11 @@ from .internal import DISCRETE, INTEGER, AlgorithmSettingsError
 TABLE_MAX = 4096
 
 
-def parse_with_margin(v) -> bool:
+def parse_with_margin(v, name: str = "with_margin") -> bool:
+    """A boolean setting (``true`` / ``false`` in any case): ``with_margin``, or the one ``name`` gives."""
     s = str(v).strip().lower()
     if s not in ("true", "false"):
-        raise AlgorithmSettingsError(f"with_margin must be true or false, got {v!r}")
+        raise AlgorithmSettingsError(f"{name} must be true or false, got {v!r}")
     return s == "true"
 
 

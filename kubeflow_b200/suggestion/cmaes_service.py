@@ -17,6 +17,11 @@ unmatched, like extra independent draws.  With ``with_margin: true`` the sampler
 ``CmaEsSampler(with_margin=True)``): ``int`` and numeric ``discrete`` parameters become discrete dimensions whose levels
 (``cma_margin.py``) the sampler encodes on the device, and the margin α (``margin``, default 1/(D·λ)) keeps a
 coordinate from freezing on one level once σ is small.  Trials get the encoded level's value; a restart resets the margin.
+With ``lr_adapt: true`` the sampler runs CMA-ES with learning-rate adaptation (Optuna's ``CmaEsSampler(lr_adapt=True)``,
+``oracle/cma_lra_oracle.py``): at the default population it lowers the learning rates of the mean and the covariance
+when the signal-to-noise ratio of their updates falls, as on a noisy or multimodal objective, instead of asking for a
+larger ``popsize``.  It works with ``popsize``, ``sigma`` and ``restart_strategy`` (each restart starts the adaptation
+afresh) and is refused beside ``with_margin: true``.
 
 Each experiment's sampler is kept for one fingerprint of its search space, objective and settings: an experiment recreated
 under the same name with a changed space or changed settings starts a new run, and the old sampler is closed.  At most
@@ -54,8 +59,8 @@ def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
                     raise AlgorithmSettingsError(f"popsize must be in [4, 8192], got {v}")
             elif k in ("restart_strategy", "device"):
                 out[k] = v
-            elif k == "with_margin":
-                out[k] = parse_with_margin(v)
+            elif k in ("with_margin", "lr_adapt"):
+                out[k] = parse_with_margin(v, k)
             elif k == "margin":
                 out[k] = float(v)
                 if not 0.0 < out[k] < 1.0:
@@ -66,6 +71,8 @@ def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
             raise AlgorithmSettingsError(f"failed to convert {v!r} for setting {k}")
     if "margin" in out and not out.get("with_margin", False):
         raise AlgorithmSettingsError("margin needs with_margin: true")
+    if out.get("lr_adapt", False) and out.get("with_margin", False):
+        raise AlgorithmSettingsError("lr_adapt: true cannot be combined with with_margin: true")
     if out.get("restart_strategy", "none") not in STRATEGIES:
         raise AlgorithmSettingsError(f"restart_strategy must be one of {', '.join(STRATEGIES)}, got {out['restart_strategy']!r}")
     if n_params < 2:
@@ -93,6 +100,8 @@ class _Experiment:
         self.levels = discrete_dims(space.params) if settings.get("with_margin", False) else {}
         if self.levels:
             self.es.set_margin({j: L.cube for j, L in self.levels.items()}, settings.get("margin"))
+        if settings.get("lr_adapt", False):
+            self.es.set_lr_adapt(True)
 
     def close(self):
         self.es.close()

@@ -47,6 +47,10 @@ for N, M, D, mode in ((70, 300, 3, "f64"), (135, 515, 5, "tc"), (300, 700, 33, "
             e.close()
 es = CmaEs(np.zeros(9), 1.0, popsize=20, seed=1)
 print(es.run_synthetic("sphere", 3))
+es.set_lr_adapt(True)                                # LRA tells: prep, three products, the blend, the finish
+print(es.run_synthetic("rastrigin", 3), es.lr_state()["eta_mean"])
+es.restart(40, np.full(9, 0.5), 0.3)                 # an LRA restart with a larger λ, then a tell of the new run
+print(es.run_synthetic("sphere", 2), es.lr_state()["eta_mean"])
 es.close()
 from kubeflow_b200.tpe import Tpe                     # TPE: model build (radix + segmented sorts), draws, FP32 score + FP64 decision, levels
 _r = np.random.default_rng(3)
