@@ -101,12 +101,12 @@ int kbo_fit(kbo_handle* h, const double* X, const double* y, int32_t N, int32_t 
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   if (x_on_host) {
-    KBO_TRY(kbo_reserve(h, h->stage_X, sizeof(double) * (size_t)N * D));
-    KBO_TRY(kbo_reserve(h, h->stage_y, sizeof(double) * (size_t)N));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_X.p, X, sizeof(double) * (size_t)N * D, cudaMemcpyHostToDevice, s));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_y.p, y, sizeof(double) * (size_t)N, cudaMemcpyHostToDevice, s));
-    X = (const double*)h->stage_X.p;
-    y = (const double*)h->stage_y.p;
+    KBO_TRY(kbo_reserve(h, h->stage_X, (size_t)N * D));
+    KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)N));
+    KBO_CUDA(h, kbo_copy(h->stage_X.p, X, (size_t)N * D, cudaMemcpyHostToDevice, s));
+    KBO_CUDA(h, kbo_copy(h->stage_y.p, y, (size_t)N, cudaMemcpyHostToDevice, s));
+    X = h->stage_X.p;
+    y = h->stage_y.p;
   }
   return kbo_i_fit(h, X, y, N, D, p, s);
 }
@@ -119,12 +119,12 @@ int kbo_lml_batch(kbo_handle* h, const double* X, const double* y, int32_t N, in
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   if (x_on_host) {
-    KBO_TRY(kbo_reserve(h, h->stage_X, sizeof(double) * (size_t)N * D));
-    KBO_TRY(kbo_reserve(h, h->stage_y, sizeof(double) * (size_t)N));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_X.p, X, sizeof(double) * (size_t)N * D, cudaMemcpyHostToDevice, s));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_y.p, y, sizeof(double) * (size_t)N, cudaMemcpyHostToDevice, s));
-    X = (const double*)h->stage_X.p;
-    y = (const double*)h->stage_y.p;
+    KBO_TRY(kbo_reserve(h, h->stage_X, (size_t)N * D));
+    KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)N));
+    KBO_CUDA(h, kbo_copy(h->stage_X.p, X, (size_t)N * D, cudaMemcpyHostToDevice, s));
+    KBO_CUDA(h, kbo_copy(h->stage_y.p, y, (size_t)N, cudaMemcpyHostToDevice, s));
+    X = h->stage_X.p;
+    y = h->stage_y.p;
   }
   return kbo_i_lml_batch(h, X, y, N, D, G, params, lml_host, info_host, s);
 }
@@ -137,12 +137,12 @@ int kbo_lml_grad_batch(kbo_handle* h, const double* X, const double* y, int32_t 
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   if (x_on_host) {
-    KBO_TRY(kbo_reserve(h, h->stage_X, sizeof(double) * (size_t)N * D));
-    KBO_TRY(kbo_reserve(h, h->stage_y, sizeof(double) * (size_t)N));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_X.p, X, sizeof(double) * (size_t)N * D, cudaMemcpyHostToDevice, s));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_y.p, y, sizeof(double) * (size_t)N, cudaMemcpyHostToDevice, s));
-    X = (const double*)h->stage_X.p;
-    y = (const double*)h->stage_y.p;
+    KBO_TRY(kbo_reserve(h, h->stage_X, (size_t)N * D));
+    KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)N));
+    KBO_CUDA(h, kbo_copy(h->stage_X.p, X, (size_t)N * D, cudaMemcpyHostToDevice, s));
+    KBO_CUDA(h, kbo_copy(h->stage_y.p, y, (size_t)N, cudaMemcpyHostToDevice, s));
+    X = h->stage_X.p;
+    y = h->stage_y.p;
   }
   return kbo_i_lml_grad_batch(h, X, y, N, D, G, params, lml_host, grad_host, info_host, s);
 }
@@ -154,9 +154,9 @@ int kbo_fit_append(kbo_handle* h, const double* x, double y, int x_on_host, void
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   if (x_on_host) {
-    KBO_TRY(kbo_reserve(h, h->stage_X, sizeof(double) * (size_t)h->D));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_X.p, x, sizeof(double) * (size_t)h->D, cudaMemcpyHostToDevice, s));
-    x = (const double*)h->stage_X.p;
+    KBO_TRY(kbo_reserve(h, h->stage_X, (size_t)h->D));
+    KBO_CUDA(h, kbo_copy(h->stage_X.p, x, (size_t)h->D, cudaMemcpyHostToDevice, s));
+    x = h->stage_X.p;
   }
   return kbo_i_fit_append(h, x, y, s);
 }
@@ -168,9 +168,9 @@ int kbo_fit_rebase(kbo_handle* h, int32_t n_keep, const double* y, int y_on_host
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   if (y && y_on_host) {
-    KBO_TRY(kbo_reserve(h, h->stage_y, sizeof(double) * (size_t)n_keep));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_y.p, y, sizeof(double) * (size_t)n_keep, cudaMemcpyHostToDevice, s));
-    y = (const double*)h->stage_y.p;
+    KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)n_keep));
+    KBO_CUDA(h, kbo_copy(h->stage_y.p, y, (size_t)n_keep, cudaMemcpyHostToDevice, s));
+    y = h->stage_y.p;
   }
   return kbo_i_fit_rebase(h, n_keep, y, s);
 }
@@ -183,8 +183,8 @@ int kbo_fit_info(kbo_handle* h, double* lml, double* y_mean, double* y_std, doub
   cudaStream_t s = (cudaStream_t)stream;
   double sc[S_COUNT];
   int inf = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(sc, h->scal.p, sizeof sc, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&inf, h->info.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(sc, h->scal.p, S_COUNT, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&inf, h->info.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (lml) *lml = sc[S_LML];
   if (y_mean) *y_mean = sc[S_YMEAN];
@@ -206,7 +206,7 @@ int kbo_fit_state(kbo_handle* h, double* L_out, double* W_out, double* alpha_out
     KBO_TRY(kbo_i_zero_upper(h, L_out, (int)N, (int)N, s));
   }
   if (W_out) KBO_CUDA(h, cudaMemcpy2DAsync(W_out, N * 8, h->W.p, ld * 8, N * 8, N, cudaMemcpyDeviceToDevice, s));
-  if (alpha_out) KBO_CUDA(h, cudaMemcpyAsync(alpha_out, h->alpha.p, N * 8, cudaMemcpyDeviceToDevice, s));
+  if (alpha_out) KBO_CUDA(h, kbo_copy(alpha_out, h->alpha.p, N, cudaMemcpyDeviceToDevice, s));
   return KBO_OK;
 }
 
@@ -273,7 +273,7 @@ int kbo_best_to_host(kbo_handle* h, const kbo_best* best_dev, kbo_best* best_hos
   cudaStream_t s = (cudaStream_t)stream;
   int inf = 0;
   KBO_CUDA(h, cudaMemcpyAsync(best_host, best_dev, sizeof(kbo_best), cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&inf, h->info.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&inf, h->info.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (inf != 0) KBO_FAIL(h, KBO_ERR_NOT_PD, "kernel matrix is not positive definite (pivot %d); increase `noise`", inf);
   return KBO_OK;
@@ -295,7 +295,7 @@ int kbo_suggest_host(kbo_handle* h, const double* X, const double* y, int32_t N,
   if (!X || !y || !Xc || !p || !best_host) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_suggest_host: null argument");
   cudaStream_t s = 0;
   KBO_CUDA(h, cudaSetDevice(h->device));
-  KBO_TRY(kbo_reserve(h, h->best, sizeof(kbo_best)));
+  KBO_TRY(kbo_reserve(h, h->best, 1));
   h->launches = 0;
   h->time_kernels = true;
   h->ev_var_used = h->ev_cross_used = h->ev_acq_used = h->ev_cal_used = 0;
@@ -328,10 +328,10 @@ int kbo_suggest_host(kbo_handle* h, const double* X, const double* y, int32_t N,
     }
   }
   cudaEventRecord(h->ev[2], s);
-  if (r == KBO_OK) r = kbo_i_sweep(h, h->stage_Xc.p, xc_dtype, M, global_offset, nullptr, nullptr, nullptr, (kbo_best*)h->best.p, s);
-  if (r == KBO_OK && h->comm) r = kbo_allreduce_argmax(h, (kbo_best*)h->best.p, s);   // sharded grid: the global first-index argmax
+  if (r == KBO_OK) r = kbo_i_sweep(h, h->stage_Xc.p, xc_dtype, M, global_offset, nullptr, nullptr, nullptr, h->best.p, s);
+  if (r == KBO_OK && h->comm) r = kbo_allreduce_argmax(h, h->best.p, s);   // sharded grid: the global first-index argmax
   cudaEventRecord(h->ev[3], s);
-  if (r == KBO_OK) r = kbo_best_to_host(h, (const kbo_best*)h->best.p, best_host, s);
+  if (r == KBO_OK) r = kbo_best_to_host(h, h->best.p, best_host, s);
   cudaEventRecord(h->ev[4], s);
   cudaEventSynchronize(h->ev[4]);
   h->time_kernels = false;
@@ -422,9 +422,9 @@ int kbo_debug_fp64_peak(kbo_handle* h, double* tflops_out) {
   if (!h || !tflops_out) return KBO_ERR_INVALID;
   cudaSetDevice(h->device);
   const int iters = 20000, ctas = h->sm_count;
-  DevBuf buf;
-  KBO_TRY(kbo_reserve(h, buf, sizeof(double) * (size_t)ctas * 256));
-  double* out = (double*)buf.p;
+  DevBuf<double> buf;
+  KBO_TRY(kbo_reserve(h, buf, (size_t)ctas * 256));
+  double* out = buf.p;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
@@ -481,23 +481,24 @@ int kbo_debug_rank_pass(kbo_handle* h, const void* Xc, int32_t xc_dtype, int64_t
   cudaStream_t s = (cudaStream_t)stream;
   const int Npad = h->Npad;
   const int64_t rows_pad = round_up64(M, 256);
-  KBO_TRY(kbo_reserve(h, h->Ksh, sizeof(__half) * (size_t)rows_pad * Npad));
-  KBO_TRY(kbo_reserve(h, h->Ksl, sizeof(__half) * (size_t)rows_pad * Npad));
-  KBO_TRY(kbo_reserve(h, h->mun, sizeof(float) * (size_t)(rows_pad + 256)));
-  KBO_TRY(kbo_reserve(h, h->varn, sizeof(float) * (size_t)(rows_pad + 256)));
+  KBO_TRY(kbo_reserve(h, h->Ksh, (size_t)rows_pad * Npad));
+  KBO_TRY(kbo_reserve(h, h->Ksl, (size_t)rows_pad * Npad));
+  const size_t bytes = sizeof(float) * (size_t)(rows_pad + 256);
+  KBO_TRY(kbo_reserve(h, h->mun, bytes));
+  KBO_TRY(kbo_reserve(h, h->varn, bytes));
   KBO_TRY(kbo_i_ensure_w(h, s));
   if (mode == 1) {
     if (!h->ks_ready) KBO_FAIL(h, KBO_ERR_STATE, "kbo_debug_rank_pass: tensor-core K* operands not available (D > 128?)");
-    KBO_TRY(kbo_i_tc_kstar(h, Xc, xc_dtype, M, (__half*)h->Ksh.p, (float*)h->mun.p, s));
-    KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, rows_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->varn.p, s));
+    KBO_TRY(kbo_i_tc_kstar(h, Xc, xc_dtype, M, h->Ksh.p, kbo_view<float>(h->mun), s));
+    KBO_TRY(kbo_i_tc_rank(h, h->Ksh.p, rows_pad, h->Wh.p, Npad, h->prm.amplitude, kbo_view<float>(h->varn), s));
   } else {
     KBO_TRY(kbo_i_debug_cross_planes(h, Xc, xc_dtype, M, s));
-    KBO_TRY(kbo_i_tc_variance(h, (const __half*)h->Ksh.p, (const __half*)h->Ksl.p, round_up64(M, 128), (const __half*)h->Wh.p, (const __half*)h->Wl.p,
-                              Npad, 0.0, h->prm.amplitude, (float*)h->varn.p, 1024, s, 1));
+    KBO_TRY(kbo_i_tc_variance(h, h->Ksh.p, h->Ksl.p, round_up64(M, 128), h->Wh.p, h->Wl.p,
+                              Npad, 0.0, h->prm.amplitude, kbo_view<float>(h->varn), 1024, s, 1));
   }
-  KBO_CUDA(h, cudaMemcpyAsync(mun_out, h->mun.p, sizeof(float) * (size_t)M, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, cudaMemcpyAsync(varn_out, h->varn.p, sizeof(float) * (size_t)M, cudaMemcpyDeviceToDevice, s));
-  if (plane_out) KBO_CUDA(h, cudaMemcpyAsync(plane_out, h->Ksh.p, sizeof(__half) * (size_t)M * Npad, cudaMemcpyDeviceToDevice, s));
+  KBO_CUDA(h, kbo_copy(mun_out, kbo_view<float>(h->mun), M, cudaMemcpyDeviceToDevice, s));
+  KBO_CUDA(h, kbo_copy(varn_out, kbo_view<float>(h->varn), M, cudaMemcpyDeviceToDevice, s));
+  if (plane_out) KBO_CUDA(h, kbo_copy(static_cast<__half*>(plane_out), h->Ksh.p, (size_t)M * Npad, cudaMemcpyDeviceToDevice, s));
   return KBO_OK;
 }
 

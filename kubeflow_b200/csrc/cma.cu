@@ -16,6 +16,8 @@
 #define CMA_EPS 1e-8
 #define CMA_MAXD 128
 
+struct CmaMarginDim;
+
 struct kbo_cma {
   int D = 0, lambda = 0, mu = 0, lam_pow2 = 0, lam_pad = 0;  // lam_pad: λ rounded up to the 256-wide split-K slices
   uint64_t seed = 0;
@@ -26,17 +28,21 @@ struct kbo_cma {
   // termination test (`cmaes`' should_stop): constants of the current run, fitness history ring of 2·term doubles
   int term = 0;
   double tolx = 0.0;
-  DevBuf mean, C, B, Dv, ps, pc, weights, Z, Zs, Y, Ys, YwT, zn2, order, R, G, scal, yw, hist, flags;
+  DevBuf<double> mean, C, B, Dv, ps, pc, weights, Z, Zs, Y, Ys, YwT, zn2, R, G, scal, yw, hist;
+  DevBuf<int> order;
+  DevBuf<unsigned> flags;
   bool asked = false;
   // CMA-ES with Margin (kbo_cma_set_margin): off while n_disc == 0, and then no margin buffer is touched
   int n_disc = 0;
   double alpha = 0.0, alpha_set = 0.0;  // alpha_set: the caller's α, or 0 for the default 1/(D·λ) recomputed at restarts
-  DevBuf A, mdim, mlev, mprev, mpre;    // A; per-dimension level descriptors; level tables; (m, σ) before the tell; m before the correction
+  DevBuf<double> A;                     // A
+  DevBuf<CmaMarginDim> mdim;            // per-dimension level descriptors
+  DevBuf<double> mlev, mprev, mpre;     // level tables; (m, σ) before the tell; m before the correction
   // learning-rate adaptation (kbo_cma_set_lr_adapt): off while !lra, and then no LRA buffer is touched
   bool lra = false;
-  DevBuf lprev, lC0;                    // (m, σ) and C before the tell
-  DevBuf lW, lP, lS, lT, lL;            // B·diag(1/d); P₀ = C^{-1/2}; S = ΔΣ/σ′²; P₀·S; P₀·S·P₀ (all D×D)
-  DevBuf lE, lscal;                     // E_m (D) then E_Σ (D×D); V_m, V_Σ, η_m, η_Σ, η_m before the last tell
+  DevBuf<double> lprev, lC0;                    // (m, σ) and C before the tell
+  DevBuf<double> lW, lP, lS, lT, lL;            // B·diag(1/d); P₀ = C^{-1/2}; S = ΔΣ/σ′²; P₀·S; P₀·S·P₀ (all D×D)
+  DevBuf<double> lE, lscal;                     // E_m (D) then E_Σ (D×D); V_m, V_Σ, η_m, η_Σ, η_m before the last tell
 };
 
 // A discrete dimension's sorted levels in cube coordinates: levels[off, off + count) of the table, or, for ranges too long
@@ -697,19 +703,19 @@ __global__ void __launch_bounds__(1024) cma_lra_finish_kernel(const double* __re
 // The LRA step between cma_c_finalize_kernel and the eigendecomposition: W and S, P₀ = W·Bᵀ, L = (P₀·S)·P₀, the blend
 static int cma_lra_blend(kbo_handle* h, kbo_cma* c, cudaStream_t s) {
   const int D = c->D;
-  double *W = (double*)c->lW.p, *P = (double*)c->lP.p, *S = (double*)c->lS.p, *T = (double*)c->lT.p, *L = (double*)c->lL.p;
-  cma_lra_prep_kernel<<<dim3((D + 127) / 128, D), 128, 0, s>>>((const double*)c->B.p, (const double*)c->Dv.p, (const double*)c->C.p,
-                                                                (const double*)c->lC0.p, (const double*)c->lprev.p,
-                                                                (const double*)c->scal.p, D, W, S);
+  double *W = c->lW.p, *P = c->lP.p, *S = c->lS.p, *T = c->lT.p, *L = c->lL.p;
+  cma_lra_prep_kernel<<<dim3((D + 127) / 128, D), 128, 0, s>>>(c->B.p, c->Dv.p, c->C.p,
+                                                                c->lC0.p, c->lprev.p,
+                                                                c->scal.p, D, W, S);
   KBO_LAUNCH_CHECK(h);
-  dgemm64_launch<true, EPI_STORE>(s, D, D, D, W, D, (const double*)c->B.p, D, P, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
+  dgemm64_launch<true, EPI_STORE>(s, D, D, D, W, D, c->B.p, D, P, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
   KBO_LAUNCH_CHECK(h);
   dgemm64_launch<false, EPI_STORE>(s, D, D, D, P, D, S, D, T, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
   KBO_LAUNCH_CHECK(h);
   dgemm64_launch<false, EPI_STORE>(s, D, D, D, T, D, P, D, L, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
   KBO_LAUNCH_CHECK(h);
-  cma_lra_kernel<<<1, 1024, 0, s>>>((const double*)c->lprev.p, (const double*)c->lC0.p, P, S, L, (const double*)c->scal.p, D,
-                                    (double*)c->lE.p, (double*)c->lscal.p, (double*)c->mean.p, (double*)c->C.p);
+  cma_lra_kernel<<<1, 1024, 0, s>>>(c->lprev.p, c->lC0.p, P, S, L, c->scal.p, D,
+                                    c->lE.p, c->lscal.p, c->mean.p, c->C.p);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }
@@ -718,59 +724,59 @@ static int cma_lra_blend(kbo_handle* h, kbo_cma* c, cudaStream_t s) {
 static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness, cudaStream_t s) {
   const int D = c->D, lam = c->lambda;
   const int smem_sort = c->lam_pow2 * 12;
-  cma_sort_kernel<<<1, 1024, smem_sort, s>>>(fitness, lam, c->lam_pow2, (int*)c->order.p, (double*)c->scal.p);
+  cma_sort_kernel<<<1, 1024, smem_sort, s>>>(fitness, lam, c->lam_pow2, c->order.p, c->scal.p);
   KBO_LAUNCH_CHECK(h);
-  cma_gather_kernel<<<c->lam_pad, 128, 0, s>>>((const double*)c->Y.p, (const int*)c->order.p, (const double*)c->weights.p, (const double*)c->zn2.p, lam,
-                                               c->lam_pad, D, (double*)c->Ys.p, (double*)c->YwT.p);
+  cma_gather_kernel<<<c->lam_pad, 128, 0, s>>>(c->Y.p, c->order.p, c->weights.p, c->zn2.p, lam,
+                                               c->lam_pad, D, c->Ys.p, c->YwT.p);
   KBO_LAUNCH_CHECK(h);
   CmaConst k{c->mu_eff, c->c1, c->cmu, c->cm, c->c_sigma, c->d_sigma, c->cc, c->chi_n, c->wsum, c->mu, c->gen};
   if (c->n_disc) {   // (m, σ) the update starts from, for the margin kernel's A-scaled mean step
-    KBO_CUDA(h, cudaMemcpyAsync(c->mprev.p, c->mean.p, 8 * (size_t)D, cudaMemcpyDeviceToDevice, s));
-    KBO_CUDA(h, cudaMemcpyAsync((double*)c->mprev.p + D, c->scal.p, 8, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, kbo_copy(c->mprev.p, c->mean.p, (size_t)D, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, kbo_copy(c->mprev.p + D, c->scal.p, 1, cudaMemcpyDeviceToDevice, s));
   }
   if (c->lra) {      // (m, σ) and C the update starts from, for the learning-rate adaptation after it
-    KBO_CUDA(h, cudaMemcpyAsync(c->lprev.p, c->mean.p, 8 * (size_t)D, cudaMemcpyDeviceToDevice, s));
-    KBO_CUDA(h, cudaMemcpyAsync((double*)c->lprev.p + D, c->scal.p, 8, cudaMemcpyDeviceToDevice, s));
-    KBO_CUDA(h, cudaMemcpyAsync(c->lC0.p, c->C.p, 8 * (size_t)D * D, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, kbo_copy(c->lprev.p, c->mean.p, (size_t)D, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, kbo_copy(c->lprev.p + D, c->scal.p, 1, cudaMemcpyDeviceToDevice, s));
+    KBO_CUDA(h, kbo_copy(c->lC0.p, c->C.p, (size_t)D * D, cudaMemcpyDeviceToDevice, s));
   }
-  cma_update_kernel<<<1, 1024, 0, s>>>((const double*)c->Ys.p, (const double*)c->weights.p, D, k, (double*)c->mean.p, (const double*)c->B.p,
-                                       (const double*)c->Dv.p, (double*)c->ps.p, (double*)c->pc.p, (double*)c->scal.p, (double*)c->yw.p);
+  cma_update_kernel<<<1, 1024, 0, s>>>(c->Ys.p, c->weights.p, D, k, c->mean.p, c->B.p,
+                                       c->Dv.p, c->ps.p, c->pc.p, c->scal.p, c->yw.p);
   KBO_LAUNCH_CHECK(h);
   // R = Σ w°_i y_i y_iᵀ  (D×D = YwT[D×λ]·Ys[λ×D]) as split-K over 256-sample slices: a 128×128 output is only two
   // tiles of the GEMM, so without the split a K = 4096 product ran on 2 CTAs; the slices fill 2·λ/256 CTAs
   const int nsl = c->lam_pad / 256;
-  dgemm64_launch<false, EPI_STORE>(s, D, D, 256, (const double*)c->YwT.p, c->lam_pad, (const double*)c->Ys.p, D, (double*)c->R.p, D, 1.0, 0.0, KM_FULL,
+  dgemm64_launch<false, EPI_STORE>(s, D, D, 256, c->YwT.p, c->lam_pad, c->Ys.p, D, c->R.p, D, 1.0, 0.0, KM_FULL,
                                    0, TS_NONE, nsl, 256, 256LL * D, (long long)D * D);
   KBO_LAUNCH_CHECK(h);
   dim3 g((D + 127) / 128, D);
-  cma_c_finalize_kernel<<<g, 128, 0, s>>>((double*)c->C.p, (const double*)c->R.p, nsl, (const double*)c->pc.p, (const double*)c->scal.p, D, c->c1,
+  cma_c_finalize_kernel<<<g, 128, 0, s>>>(c->C.p, c->R.p, nsl, c->pc.p, c->scal.p, D, c->c1,
                                           c->cmu);
   KBO_LAUNCH_CHECK(h);
   if (c->lra) KBO_TRY(cma_lra_blend(h, c, s));   // B and Dv are still C_prev's here; C becomes the blended Σ/σ′²
   // G = C·B_prev, then Jacobi
-  dgemm64_launch<false, EPI_STORE>(s, D, D, D, (const double*)c->C.p, D, (const double*)c->B.p, D, (double*)c->G.p, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
+  dgemm64_launch<false, EPI_STORE>(s, D, D, D, c->C.p, D, c->B.p, D, c->G.p, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
   KBO_LAUNCH_CHECK(h);
   const int Dp = (D + 1) & ~1;
   if (D == 128)
-    cma_jacobi_kernel<128><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>((const double*)c->G.p, D, (double*)c->B.p, (double*)c->scal.p, 30);
+    cma_jacobi_kernel<128><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>(c->G.p, D, c->B.p, c->scal.p, 30);
   else
-    cma_jacobi_kernel<0><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>((const double*)c->G.p, D, (double*)c->B.p, (double*)c->scal.p, 30);
+    cma_jacobi_kernel<0><<<1, 1024, sizeof(double) * Dp * (D + 1), s>>>(c->G.p, D, c->B.p, c->scal.p, 30);
   KBO_LAUNCH_CHECK(h);
-  cma_eigval_kernel<<<D, 1024, 0, s>>>((const double*)c->C.p, (const double*)c->B.p, D, (double*)c->Dv.p);
+  cma_eigval_kernel<<<D, 1024, 0, s>>>(c->C.p, c->B.p, D, c->Dv.p);
   KBO_LAUNCH_CHECK(h);
   if (c->n_disc) {
-    cma_margin_kernel<<<1, CMA_MAXD, 0, s>>>((const double*)c->mprev.p, (const double*)c->yw.p, c->cm, (const double*)c->scal.p,
-                                             (const double*)c->C.p, (const CmaMarginDim*)c->mdim.p, (const double*)c->mlev.p, D, c->alpha,
-                                             (double*)c->mean.p, (double*)c->A.p, (double*)c->mpre.p);
+    cma_margin_kernel<<<1, CMA_MAXD, 0, s>>>(c->mprev.p, c->yw.p, c->cm, c->scal.p,
+                                             c->C.p, c->mdim.p, c->mlev.p, D, c->alpha,
+                                             c->mean.p, c->A.p, c->mpre.p);
     KBO_LAUNCH_CHECK(h);
   }
   if (c->lra) {
-    cma_lra_finish_kernel<<<1, 1024, 0, s>>>((const double*)c->lscal.p, D, (double*)c->Dv.p, (double*)c->C.p, (double*)c->scal.p);
+    cma_lra_finish_kernel<<<1, 1024, 0, s>>>(c->lscal.p, D, c->Dv.p, c->C.p, c->scal.p);
     KBO_LAUNCH_CHECK(h);
   }
-  cma_stop_kernel<<<1, CMA_MAXD, 0, s>>>(fitness, (const int*)c->order.p, lam, D, (const double*)c->mean.p, (const double*)c->C.p,
-                                         (const double*)c->B.p, (const double*)c->Dv.p, (const double*)c->pc.p, (const double*)c->scal.p,
-                                         (double*)c->hist.p, c->term, c->gen + 1, c->tolx, (unsigned*)c->flags.p);
+  cma_stop_kernel<<<1, CMA_MAXD, 0, s>>>(fitness, c->order.p, lam, D, c->mean.p, c->C.p,
+                                         c->B.p, c->Dv.p, c->pc.p, c->scal.p,
+                                         c->hist.p, c->term, c->gen + 1, c->tolx, c->flags.p);
   KBO_LAUNCH_CHECK(h);
   c->gen++;
   c->draws++;
@@ -783,21 +789,21 @@ static int cma_generation_ask(kbo_handle* h, kbo_cma* c, double* X, const double
   const int64_t n = (int64_t)lam * D;
   const double* Z = z_in;
   if (!Z) {
-    cma_normal_kernel<<<(unsigned)((n / 2 + 1 + 255) / 256), 256, 0, s>>>((double*)c->Z.p, n, c->seed, (uint64_t)c->draws);
+    cma_normal_kernel<<<(unsigned)((n / 2 + 1 + 255) / 256), 256, 0, s>>>(c->Z.p, n, c->seed, (uint64_t)c->draws);
     KBO_LAUNCH_CHECK(h);
-    Z = (const double*)c->Z.p;
+    Z = c->Z.p;
   }
-  cma_scale_kernel<<<(lam + 7) / 8, 256, 0, s>>>(Z, (const double*)c->Dv.p, lam, D, (double*)c->Zs.p, (double*)c->zn2.p);
+  cma_scale_kernel<<<(lam + 7) / 8, 256, 0, s>>>(Z, c->Dv.p, lam, D, c->Zs.p, c->zn2.p);
   KBO_LAUNCH_CHECK(h);
   // Y[k,i] = Σ_j Zs[k,j]·B[i,j]
-  dgemm64_launch<true, EPI_STORE>(s, lam, D, D, (const double*)c->Zs.p, D, (const double*)c->B.p, D, (double*)c->Y.p, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
+  dgemm64_launch<true, EPI_STORE>(s, lam, D, D, c->Zs.p, D, c->B.p, D, c->Y.p, D, 1.0, 0.0, KM_FULL, 0, TS_NONE);
   KBO_LAUNCH_CHECK(h);
   if (c->n_disc)
-    cma_x_margin_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const double*)c->Y.p, (const double*)c->mean.p, (const double*)c->scal.p,
-                                                                     (const double*)c->A.p, (const CmaMarginDim*)c->mdim.p,
-                                                                     (const double*)c->mlev.p, n, D, X);
+    cma_x_margin_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c->Y.p, c->mean.p, c->scal.p,
+                                                                     c->A.p, c->mdim.p,
+                                                                     c->mlev.p, n, D, X);
   else
-    cma_x_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>((const double*)c->Y.p, (const double*)c->mean.p, (const double*)c->scal.p, n, D, X);
+    cma_x_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c->Y.p, c->mean.p, c->scal.p, n, D, X);
   KBO_LAUNCH_CHECK(h);
   c->asked = true;
   return KBO_OK;
@@ -843,27 +849,27 @@ static int cma_configure(kbo_handle* h, kbo_cma* c, int lambda, double sigma0) {
   c->term = 10 + (30 * n + lambda - 1) / lambda;   // 10 + ⌈30·n/λ⌉
   c->tolx = 1e-12 * sigma0;
   const size_t LD = (size_t)lambda * D, LPD = (size_t)c->lam_pad * D;
-  KBO_TRY(kbo_reserve(h, c->mean, 8 * D));
-  KBO_TRY(kbo_reserve(h, c->C, 8 * (size_t)D * D));
-  KBO_TRY(kbo_reserve(h, c->B, 8 * (size_t)D * D));
-  KBO_TRY(kbo_reserve(h, c->Dv, 8 * D));
-  KBO_TRY(kbo_reserve(h, c->ps, 8 * D));
-  KBO_TRY(kbo_reserve(h, c->pc, 8 * D));
-  KBO_TRY(kbo_reserve(h, c->weights, 8 * lambda));
-  KBO_TRY(kbo_reserve(h, c->Z, 8 * (LD + 2)));
-  KBO_TRY(kbo_reserve(h, c->Zs, 8 * LD));
-  KBO_TRY(kbo_reserve(h, c->Y, 8 * LD));
-  KBO_TRY(kbo_reserve(h, c->Ys, 8 * LPD));
-  KBO_TRY(kbo_reserve(h, c->YwT, 8 * LPD));
-  KBO_TRY(kbo_reserve(h, c->zn2, 8 * lambda));
-  KBO_TRY(kbo_reserve(h, c->order, 4 * lambda));
-  KBO_TRY(kbo_reserve(h, c->R, 8 * (size_t)D * D * (c->lam_pad / 256)));
-  KBO_TRY(kbo_reserve(h, c->G, 8 * (size_t)D * D));
-  KBO_TRY(kbo_reserve(h, c->scal, 8 * CS_COUNT));
-  KBO_TRY(kbo_reserve(h, c->yw, 8 * D));
-  KBO_TRY(kbo_reserve(h, c->hist, 8 * 2 * (size_t)c->term));
-  KBO_TRY(kbo_reserve(h, c->flags, 4));
-  KBO_CUDA(h, cudaMemcpy(c->weights.p, w.data(), 8 * lambda, cudaMemcpyHostToDevice));
+  KBO_TRY(kbo_reserve(h, c->mean, D));
+  KBO_TRY(kbo_reserve(h, c->C, (size_t)D * D));
+  KBO_TRY(kbo_reserve(h, c->B, (size_t)D * D));
+  KBO_TRY(kbo_reserve(h, c->Dv, D));
+  KBO_TRY(kbo_reserve(h, c->ps, D));
+  KBO_TRY(kbo_reserve(h, c->pc, D));
+  KBO_TRY(kbo_reserve(h, c->weights, lambda));
+  KBO_TRY(kbo_reserve(h, c->Z, LD + 2));
+  KBO_TRY(kbo_reserve(h, c->Zs, LD));
+  KBO_TRY(kbo_reserve(h, c->Y, LD));
+  KBO_TRY(kbo_reserve(h, c->Ys, LPD));
+  KBO_TRY(kbo_reserve(h, c->YwT, LPD));
+  KBO_TRY(kbo_reserve(h, c->zn2, lambda));
+  KBO_TRY(kbo_reserve(h, c->order, lambda));
+  KBO_TRY(kbo_reserve(h, c->R, (size_t)D * D * (c->lam_pad / 256)));
+  KBO_TRY(kbo_reserve(h, c->G, (size_t)D * D));
+  KBO_TRY(kbo_reserve(h, c->scal, CS_COUNT));
+  KBO_TRY(kbo_reserve(h, c->yw, D));
+  KBO_TRY(kbo_reserve(h, c->hist, (size_t)c->term * 2));
+  KBO_TRY(kbo_reserve(h, c->flags, 1));
+  KBO_TRY(kbo_upload(h, c->weights, w.data(), lambda));
   return KBO_OK;
 }
 
@@ -871,11 +877,11 @@ static int cma_configure(kbo_handle* h, kbo_cma* c, int lambda, double sigma0) {
 static int cma_start_run(kbo_handle* h, kbo_cma* c, const double* mean0, double sigma0) {
   const int D = c->D;
   double sc[CS_COUNT] = {sigma0, 0, 0, 0, 0, 0, 0, 0};
-  cudaMemcpy(c->mean.p, mean0, 8 * D, cudaMemcpyHostToDevice);
+  cudaMemcpy(c->mean.p, mean0, sizeof *c->mean.p * D, cudaMemcpyHostToDevice);
   cudaMemcpy(c->scal.p, sc, sizeof sc, cudaMemcpyHostToDevice);
-  cma_init_kernel<<<D, 128>>>((double*)c->C.p, (double*)c->B.p, (double*)c->Dv.p, (double*)c->ps.p, (double*)c->pc.p, D);
-  cudaMemset(c->hist.p, 0, 8 * 2 * (size_t)c->term);
-  cudaMemset(c->flags.p, 0, 4);
+  cma_init_kernel<<<D, 128>>>(c->C.p, c->B.p, c->Dv.p, c->ps.p, c->pc.p, D);
+  cudaMemset(c->hist.p, 0, sizeof *c->hist.p * 2 * (size_t)c->term);
+  cudaMemset(c->flags.p, 0, sizeof *c->flags.p);
   KBO_CUDA(h, cudaDeviceSynchronize());
   c->gen = 0;
   c->asked = false;
@@ -887,7 +893,7 @@ static int cma_margin_reset(kbo_handle* h, kbo_cma* c) {
   if (!c->n_disc) return KBO_OK;
   c->alpha = c->alpha_set > 0.0 ? c->alpha_set : 1.0 / ((double)c->D * c->lambda);
   const std::vector<double> ones(c->D, 1.0);
-  KBO_CUDA(h, cudaMemcpy(c->A.p, ones.data(), 8 * (size_t)c->D, cudaMemcpyHostToDevice));
+  KBO_TRY(kbo_upload(h, c->A, ones.data(), c->D));
   return KBO_OK;
 }
 
@@ -895,8 +901,8 @@ static int cma_margin_reset(kbo_handle* h, kbo_cma* c) {
 static int cma_lra_reset(kbo_handle* h, kbo_cma* c) {
   if (!c->lra) return KBO_OK;
   const double ls[LS_COUNT] = {0.0, 0.0, 1.0, 1.0, 1.0};
-  KBO_CUDA(h, cudaMemset(c->lE.p, 0, 8 * (size_t)c->D * (c->D + 1)));
-  KBO_CUDA(h, cudaMemcpy(c->lscal.p, ls, sizeof ls, cudaMemcpyHostToDevice));
+  KBO_CUDA(h, cudaMemset(c->lE.p, 0, sizeof *c->lE.p * (size_t)c->D * (c->D + 1)));
+  KBO_TRY(kbo_upload(h, c->lscal, ls, LS_COUNT));
   return KBO_OK;
 }
 
@@ -910,16 +916,16 @@ int kbo_cma_set_lr_adapt(kbo_handle* h, kbo_cma* c, int32_t on) {
   KBO_CUDA(h, cudaDeviceSynchronize());            // a tell in flight may still use the state about to be reset
   c->lra = false;
   if (!on) return KBO_OK;
-  const size_t D = c->D, DD = 8 * D * D;
-  KBO_TRY(kbo_reserve(h, c->lprev, 8 * (D + 1)));
+  const size_t D = c->D, DD = D * D;
+  KBO_TRY(kbo_reserve(h, c->lprev, D + 1));
   KBO_TRY(kbo_reserve(h, c->lC0, DD));
   KBO_TRY(kbo_reserve(h, c->lW, DD));
   KBO_TRY(kbo_reserve(h, c->lP, DD));
   KBO_TRY(kbo_reserve(h, c->lS, DD));
   KBO_TRY(kbo_reserve(h, c->lT, DD));
   KBO_TRY(kbo_reserve(h, c->lL, DD));
-  KBO_TRY(kbo_reserve(h, c->lE, 8 * D * (D + 1)));
-  KBO_TRY(kbo_reserve(h, c->lscal, 8 * LS_COUNT));
+  KBO_TRY(kbo_reserve(h, c->lE, D * (D + 1)));
+  KBO_TRY(kbo_reserve(h, c->lscal, LS_COUNT));
   c->lra = true;
   return cma_lra_reset(h, c);
 }
@@ -930,9 +936,9 @@ int kbo_cma_lra_state(kbo_handle* h, kbo_cma* c, double* E_mean_host, double* E_
   cudaStream_t s = (cudaStream_t)stream;
   const size_t D = c->D;
   double ls[LS_COUNT];
-  if (E_mean_host) KBO_CUDA(h, cudaMemcpyAsync(E_mean_host, c->lE.p, 8 * D, cudaMemcpyDeviceToHost, s));
-  if (E_Sigma_host) KBO_CUDA(h, cudaMemcpyAsync(E_Sigma_host, (double*)c->lE.p + D, 8 * D * D, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(ls, c->lscal.p, sizeof ls, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_d2h(E_mean_host, c->lE.p, D, s));
+  KBO_CUDA(h, kbo_d2h(E_Sigma_host, c->lE.p + D, D * D, s));
+  KBO_CUDA(h, kbo_copy(ls, c->lscal.p, LS_COUNT, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (V_host) { V_host[0] = ls[LS_V_M]; V_host[1] = ls[LS_V_S]; }
   if (eta_host) { eta_host[0] = ls[LS_ETA_M]; eta_host[1] = ls[LS_ETA_S]; }
@@ -975,12 +981,12 @@ int kbo_cma_set_margin(kbo_handle* h, kbo_cma* c, int32_t n_discrete, const int3
   KBO_CUDA(h, cudaDeviceSynchronize());            // a tell in flight may still read the tables about to be replaced
   c->n_disc = 0;
   if (!n_discrete) return KBO_OK;
-  KBO_TRY(kbo_reserve(h, c->A, 8 * (size_t)D));
-  KBO_TRY(kbo_reserve(h, c->mprev, 8 * (size_t)(D + 1)));
-  KBO_TRY(kbo_reserve(h, c->mpre, 8 * (size_t)D));
-  KBO_TRY(kbo_upload(h, c->mdim, md.data(), sizeof(CmaMarginDim) * D));
-  KBO_TRY(kbo_upload(h, c->mlev, levels, 8 * (size_t)n_lev));
-  KBO_CUDA(h, cudaMemcpy(c->mpre.p, c->mean.p, 8 * (size_t)D, cudaMemcpyDeviceToDevice));
+  KBO_TRY(kbo_reserve(h, c->A, (size_t)D));
+  KBO_TRY(kbo_reserve(h, c->mprev, (size_t)(D + 1)));
+  KBO_TRY(kbo_reserve(h, c->mpre, (size_t)D));
+  KBO_TRY(kbo_upload(h, c->mdim, md.data(), D));
+  KBO_TRY(kbo_upload(h, c->mlev, levels, (size_t)n_lev));
+  KBO_CUDA(h, cudaMemcpy(c->mpre.p, c->mean.p, sizeof *c->mpre.p * D, cudaMemcpyDeviceToDevice));
   c->n_disc = n_discrete;
   c->alpha_set = alpha;
   return cma_margin_reset(h, c);
@@ -990,8 +996,8 @@ int kbo_cma_margin_state(kbo_handle* h, kbo_cma* c, double* A_host, double* mean
   if (!h || !c) return KBO_ERR_INVALID;
   if (!c->n_disc) KBO_FAIL(h, KBO_ERR_STATE, "kbo_cma_margin_state: no margin is set");
   cudaStream_t s = (cudaStream_t)stream;
-  if (A_host) KBO_CUDA(h, cudaMemcpyAsync(A_host, c->A.p, 8 * (size_t)c->D, cudaMemcpyDeviceToHost, s));
-  if (mean_before_host) KBO_CUDA(h, cudaMemcpyAsync(mean_before_host, c->mpre.p, 8 * (size_t)c->D, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_d2h(A_host, c->A.p, (size_t)c->D, s));
+  KBO_CUDA(h, kbo_d2h(mean_before_host, c->mpre.p, (size_t)c->D, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (alpha_host) *alpha_host = c->alpha;
   return KBO_OK;
@@ -1032,8 +1038,8 @@ int kbo_cma_restart(kbo_handle* h, kbo_cma* c, int32_t lambda, const double* mea
 int kbo_cma_stop_flags(kbo_handle* h, kbo_cma* c, uint32_t* flags_host, double* funhist_host, int32_t* term_host, void* stream) {
   if (!h || !c) return KBO_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
-  if (flags_host) KBO_CUDA(h, cudaMemcpyAsync(flags_host, c->flags.p, 4, cudaMemcpyDeviceToHost, s));
-  if (funhist_host) KBO_CUDA(h, cudaMemcpyAsync(funhist_host, c->hist.p, 8 * 2 * (size_t)c->term, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_d2h(flags_host, c->flags.p, 1, s));
+  KBO_CUDA(h, kbo_d2h(funhist_host, c->hist.p, (size_t)c->term * 2, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (term_host) *term_host = c->term;
   return KBO_OK;
@@ -1061,14 +1067,14 @@ int kbo_cma_state(kbo_handle* h, kbo_cma* c, double* mean, double* sigma, double
   if (!h || !c) return KBO_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
   const size_t D = c->D;
-  if (mean) KBO_CUDA(h, cudaMemcpyAsync(mean, c->mean.p, 8 * D, cudaMemcpyDeviceToHost, s));
-  if (sigma) KBO_CUDA(h, cudaMemcpyAsync(sigma, c->scal.p, 8, cudaMemcpyDeviceToHost, s));
-  if (C) KBO_CUDA(h, cudaMemcpyAsync(C, c->C.p, 8 * D * D, cudaMemcpyDeviceToHost, s));
-  if (p_sigma) KBO_CUDA(h, cudaMemcpyAsync(p_sigma, c->ps.p, 8 * D, cudaMemcpyDeviceToHost, s));
-  if (p_c) KBO_CUDA(h, cudaMemcpyAsync(p_c, c->pc.p, 8 * D, cudaMemcpyDeviceToHost, s));
-  if (B) KBO_CUDA(h, cudaMemcpyAsync(B, c->B.p, 8 * D * D, cudaMemcpyDeviceToHost, s));
-  if (Dv) KBO_CUDA(h, cudaMemcpyAsync(Dv, c->Dv.p, 8 * D, cudaMemcpyDeviceToHost, s));
-  if (Y_last) KBO_CUDA(h, cudaMemcpyAsync(Y_last, c->Y.p, 8 * D * c->lambda, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_d2h(mean, c->mean.p, D, s));
+  KBO_CUDA(h, kbo_d2h(sigma, c->scal.p, 1, s));
+  KBO_CUDA(h, kbo_d2h(C, c->C.p, D * D, s));
+  KBO_CUDA(h, kbo_d2h(p_sigma, c->ps.p, D, s));
+  KBO_CUDA(h, kbo_d2h(p_c, c->pc.p, D, s));
+  KBO_CUDA(h, kbo_d2h(B, c->B.p, D * D, s));
+  KBO_CUDA(h, kbo_d2h(Dv, c->Dv.p, D, s));
+  KBO_CUDA(h, kbo_d2h(Y_last, c->Y.p, D * c->lambda, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (generation) *generation = c->gen;
   return KBO_OK;
@@ -1079,21 +1085,21 @@ int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32
   if (!h || !c) return KBO_ERR_INVALID;
   if (fitness_kind < 0 || fitness_kind > 1 || generations < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_cma_run_synthetic: bad argument");
   cudaStream_t s = 0;
-  DevBuf X, f;
-  KBO_TRY(kbo_reserve(h, X, 8 * (size_t)c->lambda * c->D));
-  KBO_TRY(kbo_reserve(h, f, 8 * (size_t)c->lambda));
+  DevBuf<double> X, f;
+  KBO_TRY(kbo_reserve(h, X, (size_t)c->lambda * c->D));
+  KBO_TRY(kbo_reserve(h, f, (size_t)c->lambda));
   cudaEventRecord(h->ev[5], s);
   int r = KBO_OK;
   for (int g = 0; g < generations && r == KBO_OK; g++) {
-    r = cma_generation_ask(h, c, (double*)X.p, nullptr, s);
+    r = cma_generation_ask(h, c, X.p, nullptr, s);
     if (r != KBO_OK) break;
-    cma_fitness_kernel<<<(c->lambda + 7) / 8, 256, 0, s>>>((const double*)X.p, c->lambda, c->D, fitness_kind, (double*)f.p);
+    cma_fitness_kernel<<<(c->lambda + 7) / 8, 256, 0, s>>>(X.p, c->lambda, c->D, fitness_kind, f.p);
     h->launches++;
-    r = cma_generation_tell(h, c, (const double*)f.p, s);
+    r = cma_generation_tell(h, c, f.p, s);
   }
   cudaEventRecord(h->ev[6], s);
   double sc[CS_COUNT];
-  cudaMemcpyAsync(sc, c->scal.p, sizeof sc, cudaMemcpyDeviceToHost, s);
+  kbo_copy(sc, c->scal.p, CS_COUNT, cudaMemcpyDeviceToHost, s);
   cudaError_t e = cudaStreamSynchronize(s);
   if (r != KBO_OK) return r;
   if (e != cudaSuccess) KBO_FAIL(h, KBO_ERR_CUDA, "kbo_cma_run_synthetic: %s", cudaGetErrorString(e));

@@ -92,7 +92,7 @@ int kbo_comm_init(kbo_handle* h, int32_t n_ranks, int32_t rank, const void* id) 
   h->comm = comm;
   h->comm_ranks = n_ranks;
   h->comm_rank = rank;
-  return kbo_reserve(h, h->comm_buf, sizeof(kbo_best) * (size_t)n_ranks);
+  return kbo_reserve(h, h->comm_buf, (size_t)n_ranks);
 }
 
 int kbo_comm_destroy(kbo_handle* h) {
@@ -119,7 +119,7 @@ int kbo_allreduce_argmax(kbo_handle* h, kbo_best* best_dev, void* stream) {
   NcclApi* a = nccl_api();
   const int r = a->all_gather(best_dev, h->comm_buf.p, sizeof(kbo_best) / sizeof(double), 8 /* ncclFloat64 */, h->comm, s);
   if (r != 0) KBO_FAIL(h, KBO_ERR_CUDA, "ncclAllGather failed: %s", a->get_error_string ? a->get_error_string(r) : "?");
-  argmax_reduce_kernel<<<1, 1, 0, s>>>((const kbo_best*)h->comm_buf.p, h->comm_ranks, best_dev);
+  argmax_reduce_kernel<<<1, 1, 0, s>>>(h->comm_buf.p, h->comm_ranks, best_dev);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }

@@ -663,7 +663,9 @@ __global__ void enas_init_kernel(float* P, long long n, uint32_t k0, uint32_t k1
 // ------------------------------------------------------------------------------------------------ host side
 struct kbo_enas {
   EnCfg cf{};
-  DevBuf par, mom, var, dev, scr, sscr;
+  DevBuf<float> par, mom, var, sscr;
+  DevBuf<float> scr;   // the training kernel's float arrays, then its int arrays OPS / SK / NSK (en_carve_scratch): both types
+  DevBuf<EnDev> dev;
   EnBufs bf{};
   EventSet<4> ev;
   float last_ms[2] = {};
@@ -677,16 +679,16 @@ static int en_carve_scratch(kbo_handle* h, kbo_enas* e, cudaStream_t s) {
   size_t total = 0;
   for (size_t f : nf) total += (f + 31) / 32 * 32;
   const size_t ints = L + np + L + 3;
-  KBO_TRY(kbo_reserve(h, e->scr, 4 * (total + ints)));
-  KBO_CUDA(h, cudaMemsetAsync(e->scr.p, 0, 4 * (total + ints), s));
-  float* p = (float*)e->scr.p;
+  KBO_TRY(kbo_reserve(h, e->scr, total + ints));
+  KBO_CUDA(h, cudaMemsetAsync(e->scr.p, 0, sizeof *e->scr.p * (total + ints), s));
+  float* p = e->scr.p;
   float** dst[] = {&e->bf.XH, &e->bf.CS, &e->bf.GT, &e->bf.DZS, &e->bf.Z, &e->bf.PR, &e->bf.ANC, &e->bf.AW1,
                    &e->bf.TA, &e->bf.Q, &e->bf.DQ, &e->bf.G, &e->bf.DU, &e->bf.DA, &e->bf.GW, &e->bf.GG};
   for (int i = 0; i < 16; i++) {
     *dst[i] = p;
     p += (nf[i] + 31) / 32 * 32;
   }
-  int* q = (int*)p;
+  int* q = reinterpret_cast<int*>(p);   // ints after the floats: same size, and every float array starts 128-byte aligned
   e->bf.OPS = q;
   e->bf.SK = q + L;
   e->bf.NSK = q + L + np + 1;
@@ -696,17 +698,17 @@ static int en_carve_scratch(kbo_handle* h, kbo_enas* e, cudaStream_t s) {
 // The controller's buffers, events and initial parameters (uniform in [-0.1, 0.1)), with the work queued on cs.
 static int en_setup(kbo_handle* h, kbo_enas* e, cudaStream_t cs) {
   const long long o = e->cf.n_par;
-  KBO_TRY(kbo_reserve(h, e->par, 4 * (size_t)o));
-  KBO_TRY(kbo_reserve(h, e->mom, 4 * (size_t)o));
-  KBO_TRY(kbo_reserve(h, e->var, 4 * (size_t)o));
-  KBO_TRY(kbo_reserve(h, e->dev, sizeof(EnDev)));
+  KBO_TRY(kbo_reserve(h, e->par, (size_t)o));
+  KBO_TRY(kbo_reserve(h, e->mom, (size_t)o));
+  KBO_TRY(kbo_reserve(h, e->var, (size_t)o));
+  KBO_TRY(kbo_reserve(h, e->dev, 1));
   KBO_TRY(en_carve_scratch(h, e, cs));
   KBO_TRY(e->ev.create());
   const EnDev d0{0.f, 0, 0, 0};
-  KBO_CUDA(h, cudaMemsetAsync(e->mom.p, 0, 4 * (size_t)o, cs));
-  KBO_CUDA(h, cudaMemsetAsync(e->var.p, 0, 4 * (size_t)o, cs));
-  KBO_CUDA(h, cudaMemcpyAsync(e->dev.p, &d0, sizeof d0, cudaMemcpyHostToDevice, cs));
-  enas_init_kernel<<<(int)std::min<long long>((o + 255) / 256, 1024), 256, 0, cs>>>((float*)e->par.p, o, e->cf.k0, e->cf.k1);
+  KBO_CUDA(h, cudaMemsetAsync(e->mom.p, 0, sizeof *e->mom.p * (size_t)o, cs));
+  KBO_CUDA(h, cudaMemsetAsync(e->var.p, 0, sizeof *e->var.p * (size_t)o, cs));
+  KBO_CUDA(h, kbo_copy(e->dev.p, &d0, 1, cudaMemcpyHostToDevice, cs));
+  enas_init_kernel<<<(int)std::min<long long>((o + 255) / 256, 1024), 256, 0, cs>>>(e->par.p, o, e->cf.k0, e->cf.k1);
   KBO_CUDA(h, cudaGetLastError());
   return KBO_OK;
 }
@@ -786,13 +788,13 @@ int kbo_enas_train(kbo_handle* h, kbo_enas* e, double reward, int32_t steps, con
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   cudaEventRecord(e->ev[0], s);
-  enas_train_kernel<<<1, EN_NT, en_smem_bytes(1, e->cf.L, e->cf.H, e->cf.n_ops), s>>>(e->cf, (float*)e->par.p, (float*)e->mom.p, (float*)e->var.p,
-                                                                                   (EnDev*)e->dev.p, (float)reward, steps, arcs, stats, e->bf,
+  enas_train_kernel<<<1, EN_NT, en_smem_bytes(1, e->cf.L, e->cf.H, e->cf.n_ops), s>>>(e->cf, e->par.p, e->mom.p, e->var.p,
+                                                                                   e->dev.p, (float)reward, steps, arcs, stats, e->bf,
                                                                                    std::pow(0.999, (double)e->step));
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(e->ev[1], s);
   int err = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(&err, (char*)e->dev.p + offsetof(EnDev, err), 4, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&err, &e->dev.p->err, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   cudaEventElapsedTime(&e->last_ms[0], e->ev[0], e->ev[1]);
   if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_enas_train: an imposed arc has an op outside [0, n_ops) or a skip other than 0 / 1 (nothing was trained)");
@@ -807,12 +809,12 @@ int kbo_enas_sample(kbo_handle* h, kbo_enas* e, int32_t k, int32_t* arcs, const 
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   const int blocks = (k + EN_SB - 1) / EN_SB;
-  KBO_TRY(kbo_reserve(h, e->sscr, 4 * (size_t)blocks * 2 * EN_SB * e->cf.L * e->cf.H));
+  KBO_TRY(kbo_reserve(h, e->sscr, (size_t)blocks * 2 * EN_SB * e->cf.L * e->cf.H));
   cudaEventRecord(e->ev[2], s);
-  enas_sample_kernel<<<blocks, EN_NT, en_smem_bytes(EN_SB, e->cf.L, e->cf.H, e->cf.n_ops), s>>>(e->cf, (const float*)e->par.p, (const EnDev*)e->dev.p, k,
-                                                                                              uniforms, arcs, op_probs, skip_probs, (float*)e->sscr.p);
+  enas_sample_kernel<<<blocks, EN_NT, en_smem_bytes(EN_SB, e->cf.L, e->cf.H, e->cf.n_ops), s>>>(e->cf, e->par.p, e->dev.p, k,
+                                                                                              uniforms, arcs, op_probs, skip_probs, e->sscr.p);
   KBO_LAUNCH_CHECK(h);
-  enas_bump_kernel<<<1, 1, 0, s>>>((EnDev*)e->dev.p);
+  enas_bump_kernel<<<1, 1, 0, s>>>(e->dev.p);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(e->ev[3], s);
   KBO_CUDA(h, cudaStreamSynchronize(s));
@@ -824,12 +826,12 @@ int kbo_enas_state(kbo_handle* h, kbo_enas* e, float* params, float* m, float* v
   if (!h || !e) return KBO_ERR_INVALID;
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
-  const size_t n = 4 * (size_t)e->cf.n_par;
+  const size_t n = e->cf.n_par;
   EnDev d{};
-  if (params) KBO_CUDA(h, cudaMemcpyAsync(params, e->par.p, n, cudaMemcpyDeviceToHost, s));
-  if (m) KBO_CUDA(h, cudaMemcpyAsync(m, e->mom.p, n, cudaMemcpyDeviceToHost, s));
-  if (v) KBO_CUDA(h, cudaMemcpyAsync(v, e->var.p, n, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&d, e->dev.p, sizeof d, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_d2h(params, e->par.p, n, s));
+  KBO_CUDA(h, kbo_d2h(m, e->mom.p, n, s));
+  KBO_CUDA(h, kbo_d2h(v, e->var.p, n, s));
+  KBO_CUDA(h, kbo_copy(&d, e->dev.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (baseline) *baseline = d.baseline;
   if (step) *step = d.step;
@@ -843,18 +845,18 @@ int kbo_enas_set_params(kbo_handle* h, kbo_enas* e, const float* params, const f
   if (step < 0) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_enas_set_params: step must be >= 0");
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
-  const size_t n = 4 * (size_t)e->cf.n_par;
+  const size_t n = e->cf.n_par;
   EnDev d{};
-  KBO_CUDA(h, cudaMemcpyAsync(&d, e->dev.p, sizeof d, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&d, e->dev.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   d.baseline = baseline;
   d.step = step;
-  KBO_CUDA(h, cudaMemcpyAsync(e->par.p, params, n, cudaMemcpyHostToDevice, s));
-  if (m) KBO_CUDA(h, cudaMemcpyAsync(e->mom.p, m, n, cudaMemcpyHostToDevice, s));
-  else KBO_CUDA(h, cudaMemsetAsync(e->mom.p, 0, n, s));
-  if (v) KBO_CUDA(h, cudaMemcpyAsync(e->var.p, v, n, cudaMemcpyHostToDevice, s));
-  else KBO_CUDA(h, cudaMemsetAsync(e->var.p, 0, n, s));
-  KBO_CUDA(h, cudaMemcpyAsync(e->dev.p, &d, sizeof d, cudaMemcpyHostToDevice, s));
+  KBO_CUDA(h, kbo_copy(e->par.p, params, n, cudaMemcpyHostToDevice, s));
+  if (m) KBO_CUDA(h, kbo_copy(e->mom.p, m, n, cudaMemcpyHostToDevice, s));
+  else KBO_CUDA(h, cudaMemsetAsync(e->mom.p, 0, sizeof *e->mom.p * n, s));
+  if (v) KBO_CUDA(h, kbo_copy(e->var.p, v, n, cudaMemcpyHostToDevice, s));
+  else KBO_CUDA(h, cudaMemsetAsync(e->var.p, 0, sizeof *e->var.p * n, s));
+  KBO_CUDA(h, kbo_copy(e->dev.p, &d, 1, cudaMemcpyHostToDevice, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   e->step = step;
   return KBO_OK;

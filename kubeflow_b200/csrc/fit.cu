@@ -219,7 +219,7 @@ __global__ void __launch_bounds__(256) trsm_panel_kernel(double* __restrict__ P,
 // trailing update of the rest is enqueued — with the number of finished columns; the fit uses it to interleave L⁻¹.
 template <typename Hook>
 static int potrf_impl(kbo_handle* h, double* A, int N, int lda, int* info_dev, cudaStream_t s, Hook panel_done, double* Linv_lane = nullptr) {
-  if (!Linv_lane) KBO_TRY(kbo_reserve(h, h->Linv, sizeof(double) * KBO_NB * KBO_NB));
+  if (!Linv_lane) KBO_TRY(kbo_reserve(h, h->Linv, KBO_NB * KBO_NB));
   const int smem = 2 * KBO_NB * (KBO_NB + 1) * (int)sizeof(double);
   if (!h->attr_fit) {
     KBO_CUDA(h, cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -228,7 +228,7 @@ static int potrf_impl(kbo_handle* h, double* A, int N, int lda, int* info_dev, c
     h->attr_fit = true;
   }
   KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, sizeof(int), s));
-  double* Linv = Linv_lane ? Linv_lane : (double*)h->Linv.p;   // inverted diagonal block of the current step (one per concurrent factorisation)
+  double* Linv = Linv_lane ? Linv_lane : h->Linv.p;   // inverted diagonal block of the current step (one per concurrent factorisation)
   // Two-level blocking: 64-wide diagonal blocks (one CTA each) inside 256-wide outer panels.  Inside a panel only the
   // panel's own remaining columns are updated after each 64-block (K = 64, ≤ 192 columns); the rest of the trailing
   // matrix sees ONE update per outer panel with K = 256 — 4× less read-modify-write traffic on the trailing matrix than
@@ -276,8 +276,8 @@ int kbo_i_trtri(kbo_handle* h, const double* L, int N, int ldl, double* W, int l
   const int smem = 2 * KBO_NB * (KBO_NB + 1) * (int)sizeof(double);
   KBO_CUDA(h, cudaFuncSetAttribute(diag_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   if (!T) {
-    KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ldw));
-    T = (double*)h->T.p;
+    KBO_TRY(kbo_reserve(h, h->T, (size_t)N * ldw));
+    T = h->T.p;
   }
   KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, s));
   diag_inv_kernel<<<(N + KBO_NB - 1) / KBO_NB, 1024, smem, s>>>(L, N, ldl, W, ldw);
@@ -476,9 +476,9 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   cudaStream_t st5[FIT_NSTREAMS];
   KBO_TRY(fit_partition(h, N >= 2048, st5));
   const bool partitioned = st5[0] == h->s3g[0] && h->part_ok;
-  KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ldw));
-  KBO_TRY(kbo_reserve(h, h->T2, sizeof(double) * (size_t)N * OW));
-  KBO_TRY(kbo_reserve(h, h->Linv4, sizeof(double) * 2 * 4 * NB * NB));
+  KBO_TRY(kbo_reserve(h, h->T, (size_t)N * ldw));
+  KBO_TRY(kbo_reserve(h, h->T2, (size_t)N * OW));
+  KBO_TRY(kbo_reserve(h, h->Linv4, (size_t)NB * NB * 4 * 2));   // two sets of the four block inverses
   const int smem = 2 * NB * (NB + 1) * (int)sizeof(double);
   if (!h->attr_fit) {
     KBO_CUDA(h, cudaFuncSetAttribute(potf2_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
@@ -486,12 +486,12 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
     KBO_CUDA(h, cudaFuncSetAttribute(diag_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     h->attr_fit = true;
   }
-  double* T = (double*)h->T.p;
-  double* T2 = (double*)h->T2.p;
+  double* T = h->T.p;
+  double* T2 = h->T2.p;
   // the 64×64 inverses of a panel's diagonal blocks, two sets: the chain of panel P+1 starts when the NEAR shadow of panel P is done,
   // the far shadow of panel P may still be reading its set (it is done before the chain of panel P+2 can start: that one waits for
   // the near shadow of P+1, which waits for the distance-1 update of P, which waits for the far shadow of P)
-  double* Linv_sets = (double*)h->Linv4.p;
+  double* Linv_sets = h->Linv4.p;
   cudaStream_t sc = st5[0], sn = st5[1], ss = st5[2], su = st5[3], sb = st5[7], si = st5[8], sw = st5[9];
   cudaStream_t* colS = st5 + 2;   // colS[k]: column-block updates at distance k (colS[1] == su)
   cudaEvent_t* ev_solve = h->ev_panel.data();                     // [n_panels]     the FAR rows below the diagonal block (past the next block) are L
@@ -536,7 +536,7 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
     KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, s));   // on the caller's stream: all SMs, not the chain's 8
   }
   // a lazy fit takes alpha from triangular solves: the forward one (z = L⁻¹·yn) is carried along, one panel behind (solve.cu)
-  const bool zsolve = lead < N && A == (double*)h->K.p && W == (double*)h->W.p && N == h->N && lda == h->ld;
+  const bool zsolve = lead < N && A == h->K.p && W == h->W.p && N == h->N && lda == h->ld;
   if (zsolve) KBO_TRY(kbo_i_zsolve_begin(h, s));
   KBO_CUDA(h, cudaEventRecord(e_start, s));
   for (cudaStream_t st : all_streams) {
@@ -919,35 +919,35 @@ static int fit_finish(kbo_handle* h, cudaStream_t s, bool new_center) {
   if (!h->w_full) {
     KBO_TRY(kbo_i_alpha_by_solves(h, s));   // alpha = L⁻ᵀ(L⁻¹ yn): two panel solves instead of Wᵀ(W yn)
   } else {
-  trmv_lower_kernel<<<(N + 7) / 8, 256, 0, s>>>((const double*)h->W.p, N, ld, (const double*)h->yn.p, (double*)h->z.p);
+  trmv_lower_kernel<<<(N + 7) / 8, 256, 0, s>>>(h->W.p, N, ld, h->yn.p, h->z.p);
   KBO_LAUNCH_CHECK(h);
   {
     const int nslab = (N + 255) / 256;
-    KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)nslab * N));  // the trtri scratch doubles as the slab partials
+    KBO_TRY(kbo_reserve(h, h->T, (size_t)nslab * N));  // the trtri scratch doubles as the slab partials
     dim3 g((N + 127) / 128, nslab);
-    trmv_lower_t_kernel<<<g, 128, 0, s>>>((const double*)h->W.p, N, ld, (const double*)h->z.p, (double*)h->T.p);
+    trmv_lower_t_kernel<<<g, 128, 0, s>>>(h->W.p, N, ld, h->z.p, h->T.p);
     KBO_LAUNCH_CHECK(h);
-    trmv_t_reduce_kernel<<<(N + 127) / 128, 128, 0, s>>>((const double*)h->T.p, N, nslab, (double*)h->alpha.p);
+    trmv_t_reduce_kernel<<<(N + 127) / 128, 128, 0, s>>>(h->T.p, N, nslab, h->alpha.p);
     KBO_LAUNCH_CHECK(h);
   }
   }
   if (trace) cudaEventRecord(fe[1], s);
-  lml_kernel<<<1, 1024, 0, s>>>((const double*)h->K.p, N, ld, (const double*)h->yn.p, (const double*)h->alpha.p, (double*)h->scal.p);
+  lml_kernel<<<1, 1024, 0, s>>>(h->K.p, N, ld, h->yn.p, h->alpha.p, h->scal.p);
   KBO_LAUNCH_CHECK(h);
   if (trace) cudaEventRecord(fe[2], s);
   if (p->var_mode == KBO_VAR_TC_F16X3 || (p->var_mode == KBO_VAR_AUTO && N > 1024)) {
     h->have_planes = true;
     const int Npad = h->Npad;
-    KBO_TRY(kbo_reserve(h, h->Wh, sizeof(__half) * (size_t)Npad * Npad));
-    KBO_TRY(kbo_reserve(h, h->Wl, sizeof(__half) * (size_t)Npad * Npad));
-    unsigned long long* amax = (unsigned long long*)((double*)h->scal.p + 8);
+    KBO_TRY(kbo_reserve(h, h->Wh, (size_t)Npad * Npad));
+    KBO_TRY(kbo_reserve(h, h->Wl, (size_t)Npad * Npad));
+    unsigned long long* amax = reinterpret_cast<unsigned long long*>(h->scal.p + S_WAMAX);  // a uint64 in a double slot (same size and alignment)
     KBO_CUDA(h, cudaMemsetAsync(amax, 0, sizeof(unsigned long long), s));
     // with a lazy inverse only the leading w_lead rows of W exist: planes (and their scale) cover those rows; kbo_i_ensure_w redoes both
     const int Nw = h->w_full ? N : h->w_lead;
-    absmax_kernel<<<h->sm_count * 4, 256, 0, s>>>((const double*)h->W.p, Nw, ld, amax);
+    absmax_kernel<<<h->sm_count * 4, 256, 0, s>>>(h->W.p, Nw, ld, amax);
     KBO_LAUNCH_CHECK(h);
     dim3 g((Npad + 255) / 256, h->w_full ? Npad : round_up(Nw, 256));
-    split_w_kernel<<<g, 256, 0, s>>>((const double*)h->W.p, Nw, ld, Npad, amax, (__half*)h->Wh.p, (__half*)h->Wl.p, (double*)h->scal.p + 6);
+    split_w_kernel<<<g, 256, 0, s>>>(h->W.p, Nw, ld, Npad, amax, h->Wh.p, h->Wl.p, h->scal.p + S_WSCALE);
     KBO_LAUNCH_CHECK(h);
     if (trace) cudaEventRecord(fe[3], s);
     // trial-side operands of the tensor-core K* kernel (alpha changes with every fit / append / rebase)
@@ -994,29 +994,29 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
   for (int d = 0; d < p->n_length_scale; d++) h->inv_ls[d] = 1.0 / p->length_scale[d];
   h->prm.length_scale = nullptr;
   const int ld = h->ld;
-  KBO_TRY(kbo_reserve(h, h->d_inv_ls, sizeof(double) * 512));
+  KBO_TRY(kbo_reserve(h, h->d_inv_ls, 512));
   // rows are reserved up to the pitch (ld = N rounded up to 64) so kbo_fit_append can add trials in place until the pitch is
   // full; past it the caller refits.  Only ld bounds how many appended rows stack on one factorisation: kbo_fit_rebase keeps ld
   // and lowers N, so after a rebase to n_keep another ld − n_keep rows (the dropped rows plus up to 63) can be appended, each
   // l = W·k formed with the W rows of the appends before it.  Measured on an H100 80GB HBM3 at 511 stacked rows and noise 1e-6,
   // their backward errors stay below a fresh fit's worst tile (tests/test_gpu_append_scale.py).
-  KBO_TRY(kbo_reserve(h, h->Xs, sizeof(double) * (size_t)ld * D));
-  KBO_TRY(kbo_reserve(h, h->XsT, sizeof(double) * (size_t)D * ld));
-  KBO_TRY(kbo_reserve(h, h->nx, sizeof(double) * ld));
-  KBO_TRY(kbo_reserve(h, h->yn, sizeof(double) * ld));
-  KBO_TRY(kbo_reserve(h, h->yraw, sizeof(double) * ld));
-  KBO_TRY(kbo_reserve(h, h->K, sizeof(double) * (size_t)ld * ld));
-  KBO_TRY(kbo_reserve(h, h->W, sizeof(double) * (size_t)ld * ld));
-  KBO_TRY(kbo_reserve(h, h->alpha, sizeof(double) * ld));
-  KBO_TRY(kbo_reserve(h, h->z, sizeof(double) * ld));
-  KBO_CUDA(h, cudaMemcpyAsync(h->yraw.p, y, sizeof(double) * N, cudaMemcpyDeviceToDevice, s));
-  KBO_TRY(kbo_reserve(h, h->scal, sizeof(double) * 16));
-  KBO_TRY(kbo_reserve(h, h->info, sizeof(int) * 4));
+  KBO_TRY(kbo_reserve(h, h->Xs, (size_t)ld * D));
+  KBO_TRY(kbo_reserve(h, h->XsT, (size_t)D * ld));
+  KBO_TRY(kbo_reserve(h, h->nx, ld));
+  KBO_TRY(kbo_reserve(h, h->yn, ld));
+  KBO_TRY(kbo_reserve(h, h->yraw, ld));
+  KBO_TRY(kbo_reserve(h, h->K, (size_t)ld * ld));
+  KBO_TRY(kbo_reserve(h, h->W, (size_t)ld * ld));
+  KBO_TRY(kbo_reserve(h, h->alpha, ld));
+  KBO_TRY(kbo_reserve(h, h->z, ld));
+  KBO_CUDA(h, kbo_copy(h->yraw.p, y, N, cudaMemcpyDeviceToDevice, s));
+  KBO_TRY(kbo_reserve(h, h->scal, 16));
+  KBO_TRY(kbo_reserve(h, h->info, 4));
   // inv_ls is tiny: stage through pageable memory is fine, but keep it async-safe by copying from the vector we own
-  KBO_CUDA(h, cudaMemcpyAsync(h->d_inv_ls.p, h->inv_ls.data(), sizeof(double) * h->inv_ls.size(), cudaMemcpyHostToDevice, s));
-  prep_x_kernel<<<(N + 127) / 128, 128, 0, s>>>(X, N, D, (const double*)h->d_inv_ls.p, p->n_length_scale, (double*)h->Xs.p, (double*)h->XsT.p, ld, (double*)h->nx.p);
+  KBO_CUDA(h, kbo_copy(h->d_inv_ls.p, h->inv_ls.data(), h->inv_ls.size(), cudaMemcpyHostToDevice, s));
+  prep_x_kernel<<<(N + 127) / 128, 128, 0, s>>>(X, N, D, h->d_inv_ls.p, p->n_length_scale, h->Xs.p, h->XsT.p, ld, h->nx.p);
   KBO_LAUNCH_CHECK(h);
-  prep_y_kernel<<<1, 1024, 0, s>>>(y, N, p->normalize_y, (double*)h->yn.p, (double*)h->scal.p);
+  prep_y_kernel<<<1, 1024, 0, s>>>(y, N, p->normalize_y, h->yn.p, h->scal.p);
   KBO_LAUNCH_CHECK(h);
   // KBO_FIT_TRACE=1: per-phase CUDA-event timings on stderr (debug aid; adds stream syncs)
   static const bool trace = getenv("KBO_FIT_TRACE") != nullptr;
@@ -1028,21 +1028,21 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
   static const bool serial = getenv("KBO_FIT_SERIAL") != nullptr;
   const bool early = !serial && N >= 1024;   // v3 starts on the first column block of the Gram matrix
   if (early) {
-    KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, 2 * sizeof(int), s));
-    KBO_CUDA(h, cudaMemsetAsync(h->W.p, 0, sizeof(double) * (size_t)N * ld, s));
+    KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, sizeof *h->info.p * 2, s));
+    KBO_CUDA(h, cudaMemsetAsync(h->W.p, 0, sizeof *h->W.p * N * ld, s));
     if (!h->ev_gram) KBO_CUDA(h, cudaEventCreateWithFlags(&h->ev_gram, cudaEventDisableTiming));
-    KBO_TRY(gram_two_parts(h, (const double*)h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, (double*)h->K.p, ld, 8, h->ev_gram, s));
+    KBO_TRY(gram_two_parts(h, h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, h->K.p, ld, 8, h->ev_gram, s));
   } else {
-    KBO_TRY(kbo_i_gram(h, (const double*)h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, (double*)h->K.p, ld, s));
+    KBO_TRY(kbo_i_gram(h, h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, h->K.p, ld, s));
   }
   if (trace) cudaEventRecord(te[1], s);
   h->w_full = true;
   h->w_lead = N;
   if (serial) {
-    KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, 2 * sizeof(int), s));   // kbo_i_potrf resets only the pivot
-    KBO_TRY(kbo_i_potrf(h, (double*)h->K.p, N, ld, (int*)h->info.p, s));
+    KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, sizeof *h->info.p * 2, s));   // kbo_i_potrf resets only the pivot
+    KBO_TRY(kbo_i_potrf(h, h->K.p, N, ld, h->info.p, s));
     if (trace) cudaEventRecord(te[2], s);
-    KBO_TRY(kbo_i_trtri(h, (const double*)h->K.p, N, ld, (double*)h->W.p, ld, s));
+    KBO_TRY(kbo_i_trtri(h, h->K.p, N, ld, h->W.p, ld, s));
   } else {
     {
       // Lazy inverse: a tensor-core fit whose sweeps will prune (kbo_set_rank_prefix) forms only the rows of W the pruning pass
@@ -1053,7 +1053,7 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
         const int P1 = kbo_prefix_pairs(h);
         if (P1 >= 1 && P1 < kbo_tile_pairs(h->Npad) && P1 * 512 + 512 <= N) lead = round_up(P1 * 512, 512);
       }
-      KBO_TRY(factor_and_invert_v3(h, (double*)h->K.p, N, ld, (double*)h->W.p, ld, (int*)h->info.p, s, lead, early ? h->ev_gram : nullptr));
+      KBO_TRY(factor_and_invert_v3(h, h->K.p, N, ld, h->W.p, ld, h->info.p, s, lead, early ? h->ev_gram : nullptr));
       h->w_lead = lead < N ? lead : N;
       h->w_full = lead >= N;
     }
@@ -1083,10 +1083,10 @@ int kbo_i_ensure_w(kbo_handle* h, cudaStream_t s) {
   if (!h->fitted && !h->w_lead) return KBO_OK;
   if (h->w_full) return KBO_OK;
   const int N = h->N, ld = h->ld, OW = 256, RW = 512;
-  double* A = (double*)h->K.p;
-  double* W = (double*)h->W.p;
-  KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ld));
-  double* T = (double*)h->T.p;
+  double* A = h->K.p;
+  double* W = h->W.p;
+  KBO_TRY(kbo_reserve(h, h->T, (size_t)N * ld));
+  double* T = h->T.p;
   for (int P0 = h->w_lead; P0 < N; P0 += RW) {
     const int Pw = min(RW, N - P0);
     double* Wrp = W + (size_t)P0 * ld + P0;
@@ -1114,12 +1114,12 @@ int kbo_i_ensure_w(kbo_handle* h, cudaStream_t s) {
   h->w_lead = N;
   if (h->have_planes) {
     const int Npad = h->Npad;
-    unsigned long long* amax = (unsigned long long*)((double*)h->scal.p + 8);
+    unsigned long long* amax = reinterpret_cast<unsigned long long*>(h->scal.p + S_WAMAX);  // a uint64 in a double slot (same size and alignment)
     KBO_CUDA(h, cudaMemsetAsync(amax, 0, sizeof(unsigned long long), s));
-    absmax_kernel<<<h->sm_count * 4, 256, 0, s>>>((const double*)h->W.p, N, ld, amax);
+    absmax_kernel<<<h->sm_count * 4, 256, 0, s>>>(h->W.p, N, ld, amax);
     KBO_LAUNCH_CHECK(h);
     dim3 g((Npad + 255) / 256, Npad);
-    split_w_kernel<<<g, 256, 0, s>>>((const double*)h->W.p, N, ld, Npad, amax, (__half*)h->Wh.p, (__half*)h->Wl.p, (double*)h->scal.p + 6);
+    split_w_kernel<<<g, 256, 0, s>>>(h->W.p, N, ld, Npad, amax, h->Wh.p, h->Wl.p, h->scal.p + S_WSCALE);
     KBO_LAUNCH_CHECK(h);
   }
   return KBO_OK;
@@ -1184,8 +1184,9 @@ trsv_lml_kernel(const double* __restrict__ L, int N, int ldl, const double* __re
 
 struct LmlLane {
   cudaStream_t s = nullptr;
-  DevBuf K, Xs, XsT, nx, inv_ls, Linv, info, out;
-  DevBuf W, T, z, alpha, part;   // kbo_lml_grad_batch only: W = L⁻¹, the trtri / transpose scratch, alpha, gradient partials
+  DevBuf<double> K, Xs, XsT, nx, inv_ls, Linv, out;
+  DevBuf<int> info;
+  DevBuf<double> W, T, z, alpha, part;   // kbo_lml_grad_batch only: W = L⁻¹, the trtri / transpose scratch, alpha, gradient partials
 };
 
 // Checks shared by kbo_lml_batch and kbo_lml_grad_batch; makes G lanes and the kernels' shared-memory opt-ins.
@@ -1215,9 +1216,9 @@ static int lml_lanes_prepare(kbo_handle* h, const char* name, int N, int D, int 
 
 // y statistics are θ-independent: normalise once on the caller's stream, which every lane then waits for
 static int lml_lanes_prep_y(kbo_handle* h, const double* y_dev, int N, int ld, int normalize_y, cudaStream_t s) {
-  KBO_TRY(kbo_reserve(h, h->lml_yn, sizeof(double) * ld));
-  KBO_TRY(kbo_reserve(h, h->lml_scal, sizeof(double) * 16));
-  prep_y_kernel<<<1, 1024, 0, s>>>(y_dev, N, normalize_y, (double*)h->lml_yn.p, (double*)h->lml_scal.p);
+  KBO_TRY(kbo_reserve(h, h->lml_yn, ld));
+  KBO_TRY(kbo_reserve(h, h->lml_scal, 16));
+  prep_y_kernel<<<1, 1024, 0, s>>>(y_dev, N, normalize_y, h->lml_yn.p, h->lml_scal.p);
   KBO_LAUNCH_CHECK(h);
   if (!h->lml_ev) KBO_CUDA(h, cudaEventCreateWithFlags(&h->lml_ev, cudaEventDisableTiming));
   KBO_CUDA(h, cudaEventRecord(h->lml_ev, s));
@@ -1227,22 +1228,22 @@ static int lml_lanes_prep_y(kbo_handle* h, const double* y_dev, int N, int ld, i
 // One θ on its lane: X/ℓ, Gram, Cholesky in L.K (pivot in L.info).
 static int lml_lane_factor(kbo_handle* h, LmlLane& L, const double* X_dev, int N, int D, int ld, const kbo_params* p, std::vector<double>& inv) {
   if (!L.s) KBO_CUDA(h, cudaStreamCreateWithFlags(&L.s, cudaStreamNonBlocking));
-  KBO_TRY(kbo_reserve(h, L.K, sizeof(double) * (size_t)ld * ld));
-  KBO_TRY(kbo_reserve(h, L.Xs, sizeof(double) * (size_t)ld * D));
-  KBO_TRY(kbo_reserve(h, L.XsT, sizeof(double) * (size_t)D * ld));
-  KBO_TRY(kbo_reserve(h, L.nx, sizeof(double) * ld));
-  KBO_TRY(kbo_reserve(h, L.inv_ls, sizeof(double) * 512));
-  KBO_TRY(kbo_reserve(h, L.Linv, sizeof(double) * KBO_NB * KBO_NB));
-  KBO_TRY(kbo_reserve(h, L.info, sizeof(int) * 4));
-  KBO_TRY(kbo_reserve(h, L.out, sizeof(double) * 2));
+  KBO_TRY(kbo_reserve(h, L.K, (size_t)ld * ld));
+  KBO_TRY(kbo_reserve(h, L.Xs, (size_t)ld * D));
+  KBO_TRY(kbo_reserve(h, L.XsT, (size_t)D * ld));
+  KBO_TRY(kbo_reserve(h, L.nx, ld));
+  KBO_TRY(kbo_reserve(h, L.inv_ls, 512));
+  KBO_TRY(kbo_reserve(h, L.Linv, KBO_NB * KBO_NB));
+  KBO_TRY(kbo_reserve(h, L.info, 4));
+  KBO_TRY(kbo_reserve(h, L.out, 2));
   KBO_CUDA(h, cudaStreamWaitEvent(L.s, h->lml_ev, 0));
   for (int d = 0; d < p->n_length_scale; d++) inv[d] = 1.0 / p->length_scale[d];
-  KBO_CUDA(h, cudaMemcpyAsync(L.inv_ls.p, inv.data(), sizeof(double) * p->n_length_scale, cudaMemcpyHostToDevice, L.s));   // pageable: staged before return
-  prep_x_kernel<<<(N + 127) / 128, 128, 0, L.s>>>(X_dev, N, D, (const double*)L.inv_ls.p, p->n_length_scale, (double*)L.Xs.p, (double*)L.XsT.p, ld,
-                                                 (double*)L.nx.p);
+  KBO_CUDA(h, kbo_copy(L.inv_ls.p, inv.data(), p->n_length_scale, cudaMemcpyHostToDevice, L.s));   // pageable: staged before return
+  prep_x_kernel<<<(N + 127) / 128, 128, 0, L.s>>>(X_dev, N, D, L.inv_ls.p, p->n_length_scale, L.Xs.p, L.XsT.p, ld,
+                                                 L.nx.p);
   KBO_LAUNCH_CHECK(h);
-  KBO_TRY(kbo_i_gram(h, (const double*)L.Xs.p, N, D, p->kernel, p->amplitude, p->noise, (double*)L.K.p, ld, L.s));
-  KBO_TRY(potrf_impl(h, (double*)L.K.p, N, ld, (int*)L.info.p, L.s, [](int, int) { return (int)KBO_OK; }, (double*)L.Linv.p));
+  KBO_TRY(kbo_i_gram(h, L.Xs.p, N, D, p->kernel, p->amplitude, p->noise, L.K.p, ld, L.s));
+  KBO_TRY(potrf_impl(h, L.K.p, N, ld, L.info.p, L.s, [](int, int) { return (int)KBO_OK; }, L.Linv.p));
   return KBO_OK;
 }
 
@@ -1258,14 +1259,14 @@ int kbo_i_lml_batch(kbo_handle* h, const double* X_dev, const double* y_dev, int
   for (int g = 0; g < G; g++) {
     LmlLane& L = (*lanes)[g];
     KBO_TRY(lml_lane_factor(h, L, X_dev, N, D, ld, params + g, inv));
-    trsv_lml_kernel<<<1, 256, zs_bytes, L.s>>>((const double*)L.K.p, N, ld, (const double*)h->lml_yn.p, (const int*)L.info.p, (double*)L.out.p);
+    trsv_lml_kernel<<<1, 256, zs_bytes, L.s>>>(L.K.p, N, ld, h->lml_yn.p, L.info.p, L.out.p);
     KBO_LAUNCH_CHECK(h);
   }
   for (int g = 0; g < G; g++) {
     LmlLane& L = (*lanes)[g];
     int inf = 0;
-    KBO_CUDA(h, cudaMemcpyAsync(lml_host + g, L.out.p, sizeof(double), cudaMemcpyDeviceToHost, L.s));
-    KBO_CUDA(h, cudaMemcpyAsync(&inf, L.info.p, sizeof(int), cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, kbo_copy(lml_host + g, L.out.p, 1, cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, kbo_copy(&inf, L.info.p, 1, cudaMemcpyDeviceToHost, L.s));
     KBO_CUDA(h, cudaStreamSynchronize(L.s));
     if (info_host) info_host[g] = inf;
   }
@@ -1301,25 +1302,25 @@ int kbo_i_lml_grad_batch(kbo_handle* h, const double* X_dev, const double* y_dev
   for (int g = 0; g < G; g++) {
     LmlLane& L = (*lanes)[g];
     const kbo_params* p = params + g;
-    KBO_TRY(kbo_reserve(h, L.W, sizeof(double) * (size_t)ld * ld));
-    KBO_TRY(kbo_reserve(h, L.T, sizeof(double) * (size_t)ld * ld));
-    KBO_TRY(kbo_reserve(h, L.z, sizeof(double) * ld));
-    KBO_TRY(kbo_reserve(h, L.alpha, sizeof(double) * ld));
-    KBO_TRY(kbo_reserve(h, L.part, sizeof(double) * ((size_t)nb * nb * ncomp + ncomp)));
-    KBO_TRY(kbo_reserve(h, L.out, sizeof(double) * 16));   // the LML kernel writes S_QUAD, S_LOGDET, S_LML
+    KBO_TRY(kbo_reserve(h, L.W, (size_t)ld * ld));
+    KBO_TRY(kbo_reserve(h, L.T, (size_t)ld * ld));
+    KBO_TRY(kbo_reserve(h, L.z, ld));
+    KBO_TRY(kbo_reserve(h, L.alpha, ld));
+    KBO_TRY(kbo_reserve(h, L.part, (size_t)nb * nb * ncomp + ncomp));
+    KBO_TRY(kbo_reserve(h, L.out, 16));   // the LML kernel writes S_QUAD, S_LOGDET, S_LML
     KBO_TRY(lml_lane_factor(h, L, X_dev, N, D, ld, p, inv));
-    double *K = (double*)L.K.p, *W = (double*)L.W.p, *T = (double*)L.T.p, *alpha = (double*)L.alpha.p, *out = (double*)L.out.p;
+    double *K = L.K.p, *W = L.W.p, *T = L.T.p, *alpha = L.alpha.p, *out = L.out.p;
     KBO_TRY(kbo_i_trtri(h, K, N, ld, W, ld, L.s, T));
-    trmv_lower_kernel<<<(N + 7) / 8, 256, 0, L.s>>>(W, N, ld, (const double*)h->lml_yn.p, (double*)L.z.p);
+    trmv_lower_kernel<<<(N + 7) / 8, 256, 0, L.s>>>(W, N, ld, h->lml_yn.p, L.z.p);
     KBO_LAUNCH_CHECK(h);
-    trmv_lower_t_kernel<<<dim3((N + 127) / 128, nslab), 128, 0, L.s>>>(W, N, ld, (const double*)L.z.p, T);   // slab partials in the scratch plane
+    trmv_lower_t_kernel<<<dim3((N + 127) / 128, nslab), 128, 0, L.s>>>(W, N, ld, L.z.p, T);   // slab partials in the scratch plane
     KBO_LAUNCH_CHECK(h);
     trmv_t_reduce_kernel<<<(N + 127) / 128, 128, 0, L.s>>>(T, N, nslab, alpha);
     KBO_LAUNCH_CHECK(h);
-    lml_kernel<<<1, 1024, 0, L.s>>>(K, N, ld, (const double*)h->lml_yn.p, alpha, out);   // LML in out[S_LML]; L is not read after this
+    lml_kernel<<<1, 1024, 0, L.s>>>(K, N, ld, h->lml_yn.p, alpha, out);   // LML in out[S_LML]; L is not read after this
     KBO_LAUNCH_CHECK(h);
-    double* part = (double*)L.part.p;
-    KBO_TRY(kbo_i_lml_grad_from_w(h, (const double*)L.Xs.p, N, D, p->kernel, p->amplitude, p->noise, alpha, W, T, K, ld, P, part,
+    double* part = L.part.p;
+    KBO_TRY(kbo_i_lml_grad_from_w(h, L.Xs.p, N, D, p->kernel, p->amplitude, p->noise, alpha, W, T, K, ld, P, part,
                                   part + (size_t)nb * nb * ncomp, L.s));
   }
   for (int g = 0; g < G; g++) {
@@ -1327,9 +1328,9 @@ int kbo_i_lml_grad_batch(kbo_handle* h, const double* X_dev, const double* y_dev
     int inf = 0;
     double lml = 0.0;
     double* gh = grad_host + (size_t)g * ncomp;
-    KBO_CUDA(h, cudaMemcpyAsync(&lml, (double*)L.out.p + S_LML, sizeof(double), cudaMemcpyDeviceToHost, L.s));
-    KBO_CUDA(h, cudaMemcpyAsync(gh, (double*)L.part.p + (size_t)nb * nb * ncomp, sizeof(double) * ncomp, cudaMemcpyDeviceToHost, L.s));
-    KBO_CUDA(h, cudaMemcpyAsync(&inf, L.info.p, sizeof(int), cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, kbo_copy(&lml, L.out.p + S_LML, 1, cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, kbo_copy(gh, L.part.p + (size_t)nb * nb * ncomp, ncomp, cudaMemcpyDeviceToHost, L.s));
+    KBO_CUDA(h, kbo_copy(&inf, L.info.p, 1, cudaMemcpyDeviceToHost, L.s));
     KBO_CUDA(h, cudaStreamSynchronize(L.s));
     if (inf != 0) {   // the lane ran on a partly factored L: nothing it computed after the pivot means anything
       lml = -INFINITY;
@@ -1423,31 +1424,31 @@ int kbo_i_fit_append(kbo_handle* h, const double* x_dev, double y, cudaStream_t 
   KBO_TRY(kbo_i_ensure_w(h, s));   // the bordered row is l = W·k
   const int row = h->N, ld = h->ld, D = h->D;
   if (row + 1 > ld) KBO_FAIL(h, KBO_ERR_STATE, "kbo_fit_append: no room (N=%d fills its %d-row pitch): call kbo_fit with the whole history", row, ld);
-  double* Krow = (double*)h->K.p + (size_t)row * ld;
-  double* Wrow = (double*)h->W.p + (size_t)row * ld;
-  KBO_TRY(kbo_reserve(h, h->lrow, sizeof(double) * (2 * (size_t)ld + 8)));
-  double* l = (double*)h->lrow.p;
+  double* Krow = h->K.p + (size_t)row * ld;
+  double* Wrow = h->W.p + (size_t)row * ld;
+  KBO_TRY(kbo_reserve(h, h->lrow, (size_t)ld * 2 + 8));
+  double* l = h->lrow.p;
   double* wtl = l + ld;
   double* dinv = wtl + ld;
-  append_x_kernel<<<1, 256, 0, s>>>(x_dev, D, (const double*)h->d_inv_ls.p, h->prm.n_length_scale, (double*)h->Xs.p, (double*)h->XsT.p, ld,
-                                    (double*)h->nx.p, row, y, (double*)h->yraw.p);
+  append_x_kernel<<<1, 256, 0, s>>>(x_dev, D, h->d_inv_ls.p, h->prm.n_length_scale, h->Xs.p, h->XsT.p, ld,
+                                    h->nx.p, row, y, h->yraw.p);
   KBO_LAUNCH_CHECK(h);
   if (row > 0) {
-    gram_row_kernel<<<(row + 127) / 128, 128, 0, s>>>((const double*)h->Xs.p, D, row, h->prm.kernel, h->prm.amplitude, Krow);
+    gram_row_kernel<<<(row + 127) / 128, 128, 0, s>>>(h->Xs.p, D, row, h->prm.kernel, h->prm.amplitude, Krow);
     KBO_LAUNCH_CHECK(h);
-    trmv_lower_kernel<<<(row + 7) / 8, 256, 0, s>>>((const double*)h->W.p, row, ld, Krow, l);
+    trmv_lower_kernel<<<(row + 7) / 8, 256, 0, s>>>(h->W.p, row, ld, Krow, l);
     KBO_LAUNCH_CHECK(h);
   }
-  append_diag_kernel<<<1, 1024, 0, s>>>(l, row, ld, h->prm.amplitude + h->prm.noise, Krow, dinv, (int*)h->info.p);
+  append_diag_kernel<<<1, 1024, 0, s>>>(l, row, ld, h->prm.amplitude + h->prm.noise, Krow, dinv, h->info.p);
   KBO_LAUNCH_CHECK(h);
   {
     const int nslab = (row + 255) / 256;
-    KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)(nslab + 1) * ld));
+    KBO_TRY(kbo_reserve(h, h->T, (size_t)(nslab + 1) * ld));
     if (row > 0) {
       dim3 g((row + 127) / 128, nslab);
-      trmv_lower_t_kernel<<<g, 128, 0, s>>>((const double*)h->W.p, row, ld, l, (double*)h->T.p);
+      trmv_lower_t_kernel<<<g, 128, 0, s>>>(h->W.p, row, ld, l, h->T.p);
       KBO_LAUNCH_CHECK(h);
-      trmv_t_reduce_kernel<<<(row + 127) / 128, 128, 0, s>>>((const double*)h->T.p, row, nslab, wtl);
+      trmv_t_reduce_kernel<<<(row + 127) / 128, 128, 0, s>>>(h->T.p, row, nslab, wtl);
       KBO_LAUNCH_CHECK(h);
     }
     append_wrow_kernel<<<(ld + 255) / 256, 256, 0, s>>>(wtl, row, ld, dinv, Wrow);
@@ -1455,7 +1456,7 @@ int kbo_i_fit_append(kbo_handle* h, const double* x_dev, double y, cudaStream_t 
   }
   h->N = row + 1;
   h->Npad = round_up(h->N, 256);   // a rebase may have shrunk it below the new N; the planes are rebuilt at this extent by fit_finish
-  prep_y_kernel<<<1, 1024, 0, s>>>((const double*)h->yraw.p, h->N, h->prm.normalize_y, (double*)h->yn.p, (double*)h->scal.p);
+  prep_y_kernel<<<1, 1024, 0, s>>>(h->yraw.p, h->N, h->prm.normalize_y, h->yn.p, h->scal.p);
   KBO_LAUNCH_CHECK(h);
   KBO_TRY(fit_finish(h, s, false));
   return KBO_OK;
@@ -1476,12 +1477,12 @@ int kbo_i_fit_rebase(kbo_handle* h, int n_keep, const double* y_dev, cudaStream_
   if (!h->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_fit_rebase: call kbo_fit first");
   if (n_keep < 1 || n_keep > h->N) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_fit_rebase: need 1 <= n_keep <= N=%d (got %d)", h->N, n_keep);
   KBO_TRY(kbo_i_ensure_w(h, s));   // keeps the bookkeeping simple: a rebased history carries all of W
-  if (y_dev) KBO_CUDA(h, cudaMemcpyAsync(h->yraw.p, y_dev, sizeof(double) * n_keep, cudaMemcpyDeviceToDevice, s));
+  if (y_dev) KBO_CUDA(h, kbo_copy(h->yraw.p, y_dev, n_keep, cudaMemcpyDeviceToDevice, s));
   h->N = n_keep;
   h->Npad = round_up(n_keep, 256);
-  clear_info_above_kernel<<<1, 1, 0, s>>>((int*)h->info.p, n_keep);
+  clear_info_above_kernel<<<1, 1, 0, s>>>(h->info.p, n_keep);
   KBO_LAUNCH_CHECK(h);
-  prep_y_kernel<<<1, 1024, 0, s>>>((const double*)h->yraw.p, h->N, h->prm.normalize_y, (double*)h->yn.p, (double*)h->scal.p);
+  prep_y_kernel<<<1, 1024, 0, s>>>(h->yraw.p, h->N, h->prm.normalize_y, h->yn.p, h->scal.p);
   KBO_LAUNCH_CHECK(h);
   KBO_TRY(fit_finish(h, s, false));
   return KBO_OK;

@@ -39,16 +39,26 @@
 #define FOREST_MAX_D 1024
 #define FOREST_MAX_T 1024
 
+struct ForestPart;
+
 struct kbo_forest {
   int kind = 0, T = 0, msl = 3;
   uint64_t seed = 0;
   int N = 0, D = 0, n_cap = 0;       // fitted history; node capacity per tree
   bool fitted = false;
-  DevBuf X, y, cnt, keys, keys2, order, order_in, seg, sort_tmp;
-  DevBuf cols, tmp, side, nstart, nend, flag;
-  DevBuf feat, thr, left, right, value, imp, nns, wn, nnodes, nleaves;
-  DevBuf blob, tree_off, part;
-  DevBuf ex_mn, ex_mx;
+  DevBuf<float> X;
+  DevBuf<double> y;
+  DevBuf<int> cnt, order, order_in, seg;
+  DevBuf<uint32_t> keys, keys2;
+  DevBuf<unsigned char> sort_tmp;
+  DevBuf<int> cols, tmp, nstart, nend, flag;
+  DevBuf<unsigned char> side;
+  DevBuf<int> feat, left, right, nns, nnodes, nleaves;
+  DevBuf<double> thr, value, imp, wn;
+  DevBuf<unsigned char> blob;
+  DevBuf<long long> tree_off;
+  DevBuf<ForestPart> part;
+  DevBuf<uint32_t> ex_mn, ex_mx;
   std::vector<int> h_nnodes, h_nleaves;
   std::vector<long long> h_off;
   size_t max_tree_bytes = 0;
@@ -648,9 +658,9 @@ static int forest_sweep_launch(kbo_handle* h, kbo_forest* f, const float* Xc, in
   const int cpt = (M + 1023) / 1024 >= 2 * h->sm_count ? 4 : 1;
   const int64_t ntiles = (M + 256 * cpt - 1) / (256 * cpt);
   const int nb = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * occ);
-  KBO_TRY(kbo_reserve(h, f->part, sizeof(ForestPart) * 3 * (size_t)nb));
-  SweepArgs a{(const unsigned char*)f->blob.p, (const long long*)f->tree_off.p, (const int*)f->nleaves.p, f->T, Xc, M, f->D, n_acq,
-              n_acq > 0 ? acqs[0] : 0, n_acq > 1 ? acqs[1] : 0, n_acq > 2 ? acqs[2] : 0, yopt, xi, kappa, mu_out, sd_out, (ForestPart*)f->part.p};
+  KBO_TRY(kbo_reserve(h, f->part, (size_t)nb * 3));
+  SweepArgs a{f->blob.p, f->tree_off.p, f->nleaves.p, f->T, Xc, M, f->D, n_acq,
+              n_acq > 0 ? acqs[0] : 0, n_acq > 1 ? acqs[1] : 0, n_acq > 2 ? acqs[2] : 0, yopt, xi, kappa, mu_out, sd_out, f->part.p};
   const size_t sm = staged ? smem : 0;
   if (staged) {
     if (cpt == 4) {
@@ -705,83 +715,83 @@ int kbo_forest_fit(kbo_handle* h, kbo_forest* f, const float* X, const double* y
   const int T = f->T;
   const bool rf = f->kind == KBO_FOREST_RF;
   const size_t ND = (size_t)N * D;
-  KBO_TRY(kbo_reserve(h, f->X, ND * 4));
-  KBO_TRY(kbo_reserve(h, f->y, (size_t)N * 8));
-  KBO_TRY(kbo_reserve(h, f->flag, 4));
+  KBO_TRY(kbo_reserve(h, f->X, ND));
+  KBO_TRY(kbo_reserve(h, f->y, (size_t)N));
+  KBO_TRY(kbo_reserve(h, f->flag, 1));
   KBO_CUDA(h, cudaEventRecord(f->ev[0], s));
-  KBO_CUDA(h, cudaMemcpyAsync(f->X.p, X, ND * 4, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, cudaMemcpyAsync(f->y.p, y, (size_t)N * 8, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, cudaMemsetAsync(f->flag.p, 0, 4, s));
-  forest_check_kernel<<<(unsigned)((ND + 255) / 256), 256, 0, s>>>((const float*)f->X.p, (const double*)f->y.p, N, D, (int*)f->flag.p);
+  KBO_CUDA(h, kbo_copy(f->X.p, X, ND, cudaMemcpyDeviceToDevice, s));
+  KBO_CUDA(h, kbo_copy(f->y.p, y, (size_t)N, cudaMemcpyDeviceToDevice, s));
+  KBO_CUDA(h, cudaMemsetAsync(f->flag.p, 0, sizeof *f->flag.p, s));
+  forest_check_kernel<<<(unsigned)((ND + 255) / 256), 256, 0, s>>>(f->X.p, f->y.p, N, D, f->flag.p);
   KBO_LAUNCH_CHECK(h);
   int bad = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(&bad, f->flag.p, 4, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&bad, f->flag.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (bad & 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_fit: y contains NaN or infinity");
   if (bad & 2) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_fit: X contains NaN or infinity");
   if (rf) {
-    KBO_TRY(kbo_reserve(h, f->cnt, (size_t)T * N * 4));
+    KBO_TRY(kbo_reserve(h, f->cnt, (size_t)T * N));
     if (counts) {
-      KBO_CUDA(h, cudaMemcpyAsync(f->cnt.p, counts, (size_t)T * N * 4, cudaMemcpyDeviceToDevice, s));
+      KBO_CUDA(h, kbo_copy(f->cnt.p, counts, (size_t)T * N, cudaMemcpyDeviceToDevice, s));
     } else {
-      KBO_CUDA(h, cudaMemsetAsync(f->cnt.p, 0, (size_t)T * N * 4, s));
-      forest_bootstrap_kernel<<<dim3((N + 255) / 256, T), 256, 0, s>>>((int*)f->cnt.p, N, f->seed);
+      KBO_CUDA(h, cudaMemsetAsync(f->cnt.p, 0, sizeof *f->cnt.p * T * N, s));
+      forest_bootstrap_kernel<<<dim3((N + 255) / 256, T), 256, 0, s>>>(f->cnt.p, N, f->seed);
       KBO_LAUNCH_CHECK(h);
     }
     // presort every column once: stable segmented radix sort of (order-preserving key, sample index)
-    KBO_TRY(kbo_reserve(h, f->keys, ND * 4));
-    KBO_TRY(kbo_reserve(h, f->keys2, ND * 4));
-    KBO_TRY(kbo_reserve(h, f->order_in, ND * 4));
-    KBO_TRY(kbo_reserve(h, f->order, ND * 4));
-    KBO_TRY(kbo_reserve(h, f->seg, (size_t)(D + 1) * 4));
-    forest_keys_kernel<<<(unsigned)((ND + 255) / 256), 256, 0, s>>>((const float*)f->X.p, N, D, (uint32_t*)f->keys.p, (int*)f->order_in.p);
+    KBO_TRY(kbo_reserve(h, f->keys, ND));
+    KBO_TRY(kbo_reserve(h, f->keys2, ND));
+    KBO_TRY(kbo_reserve(h, f->order_in, ND));
+    KBO_TRY(kbo_reserve(h, f->order, ND));
+    KBO_TRY(kbo_reserve(h, f->seg, (size_t)(D + 1)));
+    forest_keys_kernel<<<(unsigned)((ND + 255) / 256), 256, 0, s>>>(f->X.p, N, D, f->keys.p, f->order_in.p);
     KBO_LAUNCH_CHECK(h);
-    forest_seg_kernel<<<(D + 1 + 255) / 256, 256, 0, s>>>((int*)f->seg.p, N, D);
+    forest_seg_kernel<<<(D + 1 + 255) / 256, 256, 0, s>>>(f->seg.p, N, D);
     KBO_LAUNCH_CHECK(h);
     size_t tb = 0;
-    const int* seg = (const int*)f->seg.p;
-    KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, (const uint32_t*)f->keys.p, (uint32_t*)f->keys2.p, (const int*)f->order_in.p,
-                                                         (int*)f->order.p, (int)ND, D, seg, seg + 1, 0, 32, s));
+    const int* seg = f->seg.p;
+    KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, f->keys.p, f->keys2.p, f->order_in.p,
+                                                         f->order.p, (int)ND, D, seg, seg + 1, 0, 32, s));
     KBO_TRY(kbo_reserve(h, f->sort_tmp, std::max<size_t>(tb, 16)));
-    KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(f->sort_tmp.p, tb, (const uint32_t*)f->keys.p, (uint32_t*)f->keys2.p, (const int*)f->order_in.p,
-                                                         (int*)f->order.p, (int)ND, D, seg, seg + 1, 0, 32, s));
+    KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(f->sort_tmp.p, tb, f->keys.p, f->keys2.p, f->order_in.p,
+                                                         f->order.p, (int)ND, D, seg, seg + 1, 0, 32, s));
   }
   // node capacity: every leaf holds >= min_samples_leaf samples (or is the root)
   const int cap = 2 * std::max(1, N / f->msl) + 1;
   f->n_cap = cap;
   const size_t TC = (size_t)T * cap;
-  KBO_TRY(kbo_reserve(h, f->feat, TC * 4));
-  KBO_TRY(kbo_reserve(h, f->thr, TC * 8));
-  KBO_TRY(kbo_reserve(h, f->left, TC * 4));
-  KBO_TRY(kbo_reserve(h, f->right, TC * 4));
-  KBO_TRY(kbo_reserve(h, f->value, TC * 8));
-  KBO_TRY(kbo_reserve(h, f->imp, TC * 8));
-  KBO_TRY(kbo_reserve(h, f->nns, TC * 4));
-  KBO_TRY(kbo_reserve(h, f->wn, TC * 8));
-  KBO_TRY(kbo_reserve(h, f->nnodes, (size_t)T * 4));
-  KBO_TRY(kbo_reserve(h, f->nleaves, (size_t)T * 4));
+  KBO_TRY(kbo_reserve(h, f->feat, TC));
+  KBO_TRY(kbo_reserve(h, f->thr, TC));
+  KBO_TRY(kbo_reserve(h, f->left, TC));
+  KBO_TRY(kbo_reserve(h, f->right, TC));
+  KBO_TRY(kbo_reserve(h, f->value, TC));
+  KBO_TRY(kbo_reserve(h, f->imp, TC));
+  KBO_TRY(kbo_reserve(h, f->nns, TC));
+  KBO_TRY(kbo_reserve(h, f->wn, TC));
+  KBO_TRY(kbo_reserve(h, f->nnodes, (size_t)T));
+  KBO_TRY(kbo_reserve(h, f->nleaves, (size_t)T));
   // trees in batches whose column scratch stays within 2 GiB
-  const size_t per = (rf ? ND : (size_t)N) * 4;
-  const int batch = (int)std::max<size_t>(1, std::min<size_t>((size_t)T, (2ull << 30) / (2 * per + N + 8ull * cap)));
+  const size_t per = rf ? ND : (size_t)N;   // column scratch ints per tree
+  const int batch = (int)std::max<size_t>(1, std::min<size_t>((size_t)T, (2ull << 30) / (2 * sizeof(int) * per + N + 8ull * cap)));
   KBO_TRY(kbo_reserve(h, f->cols, per * batch));
   KBO_TRY(kbo_reserve(h, f->tmp, per * batch));
   KBO_TRY(kbo_reserve(h, f->side, (size_t)N * batch));
-  KBO_TRY(kbo_reserve(h, f->nstart, (size_t)cap * 4 * batch));
-  KBO_TRY(kbo_reserve(h, f->nend, (size_t)cap * 4 * batch));
+  KBO_TRY(kbo_reserve(h, f->nstart, (size_t)cap * batch));
+  KBO_TRY(kbo_reserve(h, f->nend, (size_t)cap * batch));
   for (int t0 = 0; t0 < T; t0 += batch) {
-    FitArgs a{(const float*)f->X.p, (const double*)f->y.p, rf ? (const int*)f->cnt.p : nullptr, rf ? (const int*)f->order.p : nullptr, N, D, f->msl,
-              f->kind, t0, cap, f->seed, (int*)f->cols.p, (int*)f->tmp.p, (unsigned char*)f->side.p, (int*)f->nstart.p, (int*)f->nend.p,
-              (int*)f->feat.p, (double*)f->thr.p, (int*)f->left.p, (int*)f->right.p, (double*)f->value.p, (double*)f->imp.p, (int*)f->nns.p,
-              (double*)f->wn.p, (int*)f->nnodes.p};
+    FitArgs a{f->X.p, f->y.p, rf ? f->cnt.p : nullptr, rf ? f->order.p : nullptr, N, D, f->msl,
+              f->kind, t0, cap, f->seed, f->cols.p, f->tmp.p, f->side.p, f->nstart.p, f->nend.p,
+              f->feat.p, f->thr.p, f->left.p, f->right.p, f->value.p, f->imp.p, f->nns.p,
+              f->wn.p, f->nnodes.p};
     forest_fit_kernel<<<std::min(batch, T - t0), FOREST_FIT_THREADS, 0, s>>>(a);
     KBO_LAUNCH_CHECK(h);
   }
-  forest_count_leaves_kernel<<<T, 256, 0, s>>>((const int*)f->left.p, (const int*)f->nnodes.p, cap, (int*)f->nleaves.p);
+  forest_count_leaves_kernel<<<T, 256, 0, s>>>(f->left.p, f->nnodes.p, cap, f->nleaves.p);
   KBO_LAUNCH_CHECK(h);
   f->h_nnodes.assign(T, 0);
   f->h_nleaves.assign(T, 0);
-  KBO_CUDA(h, cudaMemcpyAsync(f->h_nnodes.data(), f->nnodes.p, (size_t)T * 4, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(f->h_nleaves.data(), f->nleaves.p, (size_t)T * 4, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(f->h_nnodes.data(), f->nnodes.p, (size_t)T, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(f->h_nleaves.data(), f->nleaves.p, (size_t)T, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   f->h_off.assign(T + 1, 0);
   f->max_tree_bytes = 0;
@@ -791,12 +801,12 @@ int kbo_forest_fit(kbo_handle* h, kbo_forest* f, const float* X, const double* y
     f->max_tree_bytes = std::max(f->max_tree_bytes, bytes);
   }
   KBO_TRY(kbo_reserve(h, f->blob, (size_t)f->h_off[T]));
-  KBO_TRY(kbo_reserve(h, f->tree_off, (size_t)(T + 1) * 8));
-  KBO_CUDA(h, cudaMemcpyAsync(f->tree_off.p, f->h_off.data(), (size_t)(T + 1) * 8, cudaMemcpyHostToDevice, s));
+  KBO_TRY(kbo_reserve(h, f->tree_off, (size_t)(T + 1)));
+  KBO_CUDA(h, kbo_copy(f->tree_off.p, f->h_off.data(), (size_t)(T + 1), cudaMemcpyHostToDevice, s));
   KBO_CUDA(h, cudaMemsetAsync(f->blob.p, 0, (size_t)f->h_off[T], s));
-  forest_pack_kernel<<<T, 1024, 0, s>>>((const int*)f->feat.p, (const double*)f->thr.p, (const int*)f->left.p, (const double*)f->value.p,
-                                        (const double*)f->imp.p, (const int*)f->nnodes.p, (const int*)f->nleaves.p, cap,
-                                        (const long long*)f->tree_off.p, (unsigned char*)f->blob.p);
+  forest_pack_kernel<<<T, 1024, 0, s>>>(f->feat.p, f->thr.p, f->left.p, f->value.p,
+                                        f->imp.p, f->nnodes.p, f->nleaves.p, cap,
+                                        f->tree_off.p, f->blob.p);
   KBO_LAUNCH_CHECK(h);
   KBO_CUDA(h, cudaEventRecord(f->ev[1], s));
   KBO_CUDA(h, cudaStreamSynchronize(s));   // the host copy of tree_off must outlive its transfer
@@ -825,7 +835,7 @@ int kbo_forest_sweep(kbo_handle* h, kbo_forest* f, const float* Xc, int64_t M, i
   int nb = 0;
   KBO_TRY(forest_sweep_launch(h, f, Xc, M, n_acq, acqs, y_opt, xi, kappa, mu_out, sigma_out, &nb, s));
   if (n_acq > 0) {
-    forest_reduce_kernel<<<n_acq, 32, 0, s>>>((const ForestPart*)f->part.p, nb, n_acq, global_offset, best_dev);
+    forest_reduce_kernel<<<n_acq, 32, 0, s>>>(f->part.p, nb, n_acq, global_offset, best_dev);
     KBO_LAUNCH_CHECK(h);
   }
   KBO_CUDA(h, cudaEventRecord(f->ev[3], s));
@@ -839,16 +849,17 @@ int kbo_forest_predict(kbo_handle* h, kbo_forest* f, const float* X, int32_t n, 
   KBO_CUDA(h, cudaSetDevice(h->device));
   const float* Xd = X;
   if (x_on_host) {
-    KBO_TRY(kbo_reserve(h, h->stage_Xc, (size_t)n * f->D * 4));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_Xc.p, X, (size_t)n * f->D * 4, cudaMemcpyHostToDevice, s));
-    Xd = (const float*)h->stage_Xc.p;
+    const size_t bytes = (size_t)n * f->D * sizeof(float);
+    KBO_TRY(kbo_reserve(h, h->stage_Xc, bytes));
+    KBO_CUDA(h, cudaMemcpyAsync(h->stage_Xc.p, X, bytes, cudaMemcpyHostToDevice, s));
+    Xd = kbo_view<float>(h->stage_Xc);
   }
-  KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)n * 16));
-  double* mu = (double*)h->stage_y.p;
+  KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)n * 2));
+  double* mu = h->stage_y.p;
   int nb = 0;
   KBO_TRY(forest_sweep_launch(h, f, Xd, n, 0, nullptr, 0.0, 0.0, 0.0, mu, mu + n, &nb, s));
-  if (mu_host) KBO_CUDA(h, cudaMemcpyAsync(mu_host, mu, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
-  if (sigma_host) KBO_CUDA(h, cudaMemcpyAsync(sigma_host, mu + n, (size_t)n * 8, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_d2h(mu_host, mu, n, s));
+  KBO_CUDA(h, kbo_d2h(sigma_host, mu + n, n, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   return KBO_OK;
 }
@@ -866,7 +877,7 @@ int kbo_forest_export(kbo_handle* h, kbo_forest* f, int32_t tree, int32_t* featu
   if (n_nodes) *n_nodes = n;
   if (counts) {
     if (f->kind == KBO_FOREST_RF) {
-      KBO_CUDA(h, cudaMemcpyAsync(counts, (const int*)f->cnt.p + (size_t)tree * f->N, (size_t)f->N * 4, cudaMemcpyDeviceToHost, s));
+      KBO_CUDA(h, kbo_copy(counts, f->cnt.p + (size_t)tree * f->N, (size_t)f->N, cudaMemcpyDeviceToHost, s));
     } else {
       for (int i = 0; i < f->N; i++) counts[i] = 1;
     }
@@ -876,32 +887,28 @@ int kbo_forest_export(kbo_handle* h, kbo_forest* f, int32_t tree, int32_t* featu
     return KBO_OK;   // size query
   }
   const size_t ob = (size_t)tree * f->n_cap;
-  auto cp = [&](void* dst, const DevBuf& b, size_t esz) -> int {
-    if (dst) KBO_CUDA(h, cudaMemcpyAsync(dst, (const char*)b.p + ob * esz, (size_t)n * esz, cudaMemcpyDeviceToHost, s));
-    return KBO_OK;
-  };
-  KBO_TRY(cp(feature, f->feat, 4));
-  KBO_TRY(cp(threshold, f->thr, 8));
-  KBO_TRY(cp(left, f->left, 4));
-  KBO_TRY(cp(right, f->right, 4));
-  KBO_TRY(cp(value, f->value, 8));
-  KBO_TRY(cp(impurity, f->imp, 8));
-  KBO_TRY(cp(n_node_samples, f->nns, 4));
-  KBO_TRY(cp(weighted_n, f->wn, 8));
+  KBO_CUDA(h, kbo_d2h(feature, f->feat.p + ob, n, s));
+  KBO_CUDA(h, kbo_d2h(threshold, f->thr.p + ob, n, s));
+  KBO_CUDA(h, kbo_d2h(left, f->left.p + ob, n, s));
+  KBO_CUDA(h, kbo_d2h(right, f->right.p + ob, n, s));
+  KBO_CUDA(h, kbo_d2h(value, f->value.p + ob, n, s));
+  KBO_CUDA(h, kbo_d2h(impurity, f->imp.p + ob, n, s));
+  KBO_CUDA(h, kbo_d2h(n_node_samples, f->nns.p + ob, n, s));
+  KBO_CUDA(h, kbo_d2h(weighted_n, f->wn.p + ob, n, s));
   if (et_draws) {
     const size_t nd = (size_t)n * f->D;
-    KBO_TRY(kbo_reserve(h, f->ex_mn, nd * 4));
-    KBO_TRY(kbo_reserve(h, f->ex_mx, nd * 4));
-    KBO_TRY(kbo_reserve(h, h->stage_X, nd * 8));
-    KBO_CUDA(h, cudaMemsetAsync(f->ex_mn.p, 0xFF, nd * 4, s));
-    KBO_CUDA(h, cudaMemsetAsync(f->ex_mx.p, 0x00, nd * 4, s));
-    forest_route_minmax_kernel<<<f->N, 128, 0, s>>>((const float*)f->X.p, f->N, f->D, (const int*)f->feat.p + ob, (const double*)f->thr.p + ob,
-                                                    (const int*)f->left.p + ob, (uint32_t*)f->ex_mn.p, (uint32_t*)f->ex_mx.p);
+    KBO_TRY(kbo_reserve(h, f->ex_mn, nd));
+    KBO_TRY(kbo_reserve(h, f->ex_mx, nd));
+    KBO_TRY(kbo_reserve(h, h->stage_X, nd));
+    KBO_CUDA(h, cudaMemsetAsync(f->ex_mn.p, 0xFF, sizeof *f->ex_mn.p * nd, s));
+    KBO_CUDA(h, cudaMemsetAsync(f->ex_mx.p, 0x00, sizeof *f->ex_mx.p * nd, s));
+    forest_route_minmax_kernel<<<f->N, 128, 0, s>>>(f->X.p, f->N, f->D, f->feat.p + ob, f->thr.p + ob,
+                                                    f->left.p + ob, f->ex_mn.p, f->ex_mx.p);
     KBO_LAUNCH_CHECK(h);
-    forest_draws_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, s>>>((const uint32_t*)f->ex_mn.p, (const uint32_t*)f->ex_mx.p, (const int*)f->left.p + ob,
-                                                                     n, f->D, f->seed, tree, (double*)h->stage_X.p);
+    forest_draws_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, s>>>(f->ex_mn.p, f->ex_mx.p, f->left.p + ob,
+                                                                     n, f->D, f->seed, tree, h->stage_X.p);
     KBO_LAUNCH_CHECK(h);
-    KBO_CUDA(h, cudaMemcpyAsync(et_draws, h->stage_X.p, nd * 8, cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, kbo_copy(et_draws, h->stage_X.p, nd, cudaMemcpyDeviceToHost, s));
   }
   KBO_CUDA(h, cudaStreamSynchronize(s));
   return KBO_OK;

@@ -6,6 +6,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <algorithm>
 #include <memory>
 #include <string>
 #include <vector>
@@ -14,9 +15,10 @@
 
 #define KBO_NB 64  // Cholesky / trtri block size (one diagonal block = one CTA in shared memory)
 
-// A device allocation owned by its holder: freed when the holder is destroyed, grown only by kbo_reserve.
+// A device array of T owned by its holder: freed when the holder is destroyed, grown only by kbo_reserve.  cap counts elements.
+template <class T>
 struct DevBuf {
-  void* p = nullptr;
+  T* p = nullptr;
   size_t cap = 0;
   DevBuf() = default;
   DevBuf(const DevBuf&) = delete;
@@ -36,6 +38,11 @@ struct DevBuf {
     if (p) cudaFree(p);
   }
 };
+
+// A byte buffer holds data with no single element type (one of two dtypes, CUB temporary storage, packed tree nodes); this is
+// the one place it is read as U.
+template <class U>
+static inline U* kbo_view(const DevBuf<unsigned char>& b) { return reinterpret_cast<U*>(b.p); }
 
 // The fixed timing events of one object: create() makes all of them, the destructor destroys them.
 template <int N>
@@ -59,6 +66,8 @@ struct EventSet {
   cudaEvent_t operator[](int i) const { return e[i]; }
 };
 
+struct BlockBest;  // sweep.cu
+
 struct kbo_handle {
   int device = 0;
   int sm_count = 132;
@@ -72,28 +81,32 @@ struct kbo_handle {
   int Npad = 0;              // multiple of 256: extent of the fp16 W planes and of K* scratch rows
   kbo_params prm{};
   std::vector<double> inv_ls;  // 1/ℓ_d, host copy
-  DevBuf d_inv_ls;             // D doubles
-  DevBuf XsT;                  // Xs transposed: D × ld (coalesced trial-tile loads in the K* kernel)
-  DevBuf Xs, nx, yn, K, W, Linv, T, alpha, z;
-  DevBuf yraw, lrow;   // raw y (re-normalised on append) and the append's work vectors
-  DevBuf Wh, Wl;        // fp16 planes Npad×Npad (TC mode)
-  DevBuf scal;          // device scalars, see ScalIdx
-  DevBuf info;          // int32: [0] potrf info; [1] 1 if an append set it (only that row is unfactored), 0 after a fit (its whole
-                        // failing 64-block is)
-  DevBuf stage_X, stage_y, stage_Xc;  // H2D staging for host-pointer entry points
+  DevBuf<double> d_inv_ls;     // D doubles
+  DevBuf<double> XsT;          // Xs transposed: D × ld (coalesced trial-tile loads in the K* kernel)
+  DevBuf<double> Xs, nx, yn, K, W, Linv, T, alpha, z;
+  DevBuf<double> yraw, lrow;  // raw y (re-normalised on append) and the append's work vectors
+  DevBuf<__half> Wh, Wl;      // fp16 planes Npad×Npad (TC mode)
+  DevBuf<double> scal;        // device scalars, see ScalIdx
+  DevBuf<int> info;           // [0] potrf info; [1] 1 if an append set it (only that row is unfactored), 0 after a fit (its whole
+                              // failing 64-block is)
+  DevBuf<double> stage_X, stage_y;  // H2D staging for host-pointer entry points
+  DevBuf<unsigned char> stage_Xc;   // the same for candidates, fp64 or fp32 (xc_dtype)
   // ---- sweep workspace ---------------------------------------------------------------------
-  DevBuf Ks64;          // chunk × ldks fp64 (F64 mode)
-  DevBuf Ksh, Ksl;      // chunk × Npad fp16 planes (TC mode)
-  DevBuf mun;           // M (fp64 in F64 mode, fp32 in TC mode)
-  DevBuf part;          // chunk × n_jtiles partial Σv² (fp64) — F64 mode
-  DevBuf varn;          // M (same dtype as mun)
-  DevBuf blockbest;     // per-block argmax partials
-  DevBuf best;          // one kbo_best for suggest_host
-  DevBuf refine, refine_x;  // contender list / gathered rows of the FP64 refinement (tensor-core mode)
+  DevBuf<double> Ks64;         // chunk × ldks fp64 (F64 mode)
+  DevBuf<__half> Ksh, Ksl;     // chunk × Npad fp16 planes (TC mode)
+  DevBuf<unsigned char> mun;   // M (fp64 in F64 mode, fp32 in TC mode)
+  DevBuf<double> part;         // chunk × n_jtiles partial Σv² (fp64) — F64 mode
+  DevBuf<unsigned char> varn;  // M (same dtype as mun)
+  DevBuf<BlockBest> blockbest; // per-block argmax partials
+  DevBuf<kbo_best> best;       // one kbo_best for suggest_host
+  // contender list of the FP64 refinement (tensor-core mode); at KBO_REFINE_CAP the survivor count padded to 4 ints, then
+  // 8 floats of stage bounds (slot 1 holds ordered unsigned bits): both types, all 4 bytes wide and 4-byte aligned
+  DevBuf<int> refine;
+  DevBuf<double> refine_x;     // gathered rows of the FP64 refinement
   int last_contenders = 0;
   float last_rank_err = 0.f;   // largest |σ²(1 product) − σ²(3 products)| over the calibration rows of the last fast sweep
   bool tc_fast = true;      // array-free tensor-core sweeps rank with ONE fp16 product and let the FP64 refinement decide
-  DevBuf var_cal;           // three-product variance of the calibration rows
+  DevBuf<float> var_cal;    // three-product variance of the calibration rows
   kbo_timings tim{};
   EventSet<8> ev;
   std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_var, ev_cross, ev_acq, ev_cal;
@@ -104,29 +117,35 @@ struct kbo_handle {
   // ---- tensor-core K* generation (tc_kstar.cu) and wgmma ranking kernel (tc_rank.cu) ---------------------------
   bool rank_tc = true;        // kbo_set_rank_tc: the ranking pass builds K̃* on the tensor cores and contracts with wgmma MMAs
   bool ks_ready = false;      // trial-side operands below match the current fit
-  DevBuf ks_center;           // D doubles: centre subtracted from the scaled coordinates (any fixed vector is valid)
-  DevBuf ks_Xh, ks_Xl;        // trials, fp16 hi/lo planes, round_up(N,256) × round_up(D,32)
-  DevBuf ks_nxal;             // (|x̂_n|², alpha_n) float pairs
-  DevBuf ks_Ch, ks_Cl, ks_nc; // candidate planes / squared norms of the current chunk
-  DevBuf rk_part;             // [tile pairs][rows] partial Σ v² of the ranking kernel
+  DevBuf<double> ks_center;   // D doubles: centre subtracted from the scaled coordinates (any fixed vector is valid)
+  DevBuf<__half> ks_Xh, ks_Xl; // trials, fp16 hi/lo planes, round_up(N,256) × round_up(D,32)
+  DevBuf<float> ks_nxal;      // (|x̂_n|², alpha_n) float pairs
+  DevBuf<__half> ks_Ch, ks_Cl; // candidate planes of the current chunk
+  DevBuf<float> ks_nc;        // squared norms of the current chunk
+  DevBuf<float> rk_part;      // [tile pairs][rows] partial Σ v² of the ranking kernel
   struct RkSched {
     int key[5] = {-1, -1, -1, -1, -1};  // (row groups, j-tiles, CTAs, first tile pair, end tile pair)
-    DevBuf dev;
+    DevBuf<int> dev;
     std::vector<int> host;
   } rk_sched[8];
   int rk_sched_next = 0;
   bool attr_rank = false;
   int rank_prefix = -1;            // kbo_set_rank_prefix: tile pairs of the pruning pass (-1: an eighth of them, 0: no pruning pass)
   int last_prefix_survivors = -1;  // candidates whose prefix upper bound reached the calibration rows' best value (-1: pass not run)
-  DevBuf pr_list, pr_x, pr_mu, pr_var;   // pruning pass: survivor indices, their gathered rows, their ranking-pass mean / variance
-  DevBuf cal_mu_rk, cal_var_rk;          // the ranking arithmetic on the calibration rows
-  DevBuf mu_part;                  // FP64 K* kernel with the trial tiles split over blockIdx.y: partial means [split][row]
-  DevBuf cal_idx, cal_x, cal_mu;   // stratified calibration rows of the ranking pass: indices, gathered rows, FP64-path mean
+  DevBuf<int> pr_list;             // pruning pass: survivor indices
+  DevBuf<double> pr_x;             // their gathered rows
+  DevBuf<float> pr_mu, pr_var;     // their ranking-pass mean / variance
+  DevBuf<float> cal_mu_rk, cal_var_rk;  // the ranking arithmetic on the calibration rows
+  DevBuf<double> mu_part;          // FP64 K* kernel with the trial tiles split over blockIdx.y: partial means [split][row]
+  DevBuf<int> cal_idx;             // stratified calibration rows of the ranking pass: indices
+  DevBuf<double> cal_x;            // their gathered rows
+  DevBuf<float> cal_mu;            // their FP64-path mean
   float last_rank_mu_err = 0.f;    // largest |μ̃ − μ| (normalised units) on the calibration rows of the last ranking sweep
   int last_unrefined = 0;          // 1: the last tensor-core sweep could not decide in FP64 (more near-ties than the cap)
   int dec_n = 0;                   // acquisitions the last kbo_sweep / kbo_sweep_multi decided, and how (kbo_last_decisions)
   int dec_unrefined[3] = {}, dec_contenders[3] = {}, dec_prefix_survivors[3] = {};
-  DevBuf un_idx, un_mv;            // FP64 decision over the union of several acquisitions' survivors: indices / positions, mean + variance
+  DevBuf<int> un_idx;              // FP64 decision over the union of several acquisitions' survivors: indices / positions
+  DevBuf<double> un_mv;            // their mean + variance
   // test hook (kbo_debug_record_stages): what each stage of the last kbo_sweep / kbo_sweep_multi kept, read back only when switched on
   struct StageRec {
     int stage, acq, cal_n, n;      // n: survivors counted; list holds the first min(n, the stage's cap) of them (grid-local indices)
@@ -137,35 +156,37 @@ struct kbo_handle {
   std::vector<StageRec> stage_recs;
   cudaStream_t s_copy = nullptr;   // the candidate grid's host-to-device copy, beside the fit (api.cu)
   // ---- fit: the chain runs on its own SM partition (green contexts); shadow panel solve / trailing update / inverse share the rest (fit.cu)
-  DevBuf T2;                        // N × 256 scratch of the far rows' panel solve
+  DevBuf<double> T2;                // N × 256 scratch of the far rows' panel solve
   bool part_tried = false, part_ok = false;
   void *gctx_chain = nullptr, *gctx_rest = nullptr;   // CUgreenCtx
   // stream roles: 0 chain, 1 near shadow (both on the chain's partition), 2 far shadow, 3..6 column-block updates at distance 1..4,
   // 7 bulk trailing update, 8 inverse, 9 W_PP (on the chain's partition)
   cudaStream_t s3g[10] = {};       // green-context set
   cudaStream_t s3p[10] = {};       // the same roles as plain priority streams (small N, profilers, no green contexts)
-  DevBuf Linv4;                     // the four 64×64 block inverses of the current panel
+  DevBuf<double> Linv4;             // the four 64×64 block inverses of the current panel
   std::vector<cudaEvent_t> ev_panel;
   cudaEvent_t ev_gram = nullptr;   // the first column block of the Gram matrix is complete (the factorisation starts on it)
   // ---- lazy inverse (fit.cu, solve.cu): the product path never needs all of W = L⁻¹ -----------------------------------------
   bool lazy_w = true;              // kbo_set_lazy_inverse: tensor-core fits form only the leading rows of W the pruning pass reads
   bool w_full = true;              // all rows of W (and the full fp16 planes) exist
   int w_lead = 0;                  // rows of W formed so far (the diagonal 256-blocks exist for every panel)
-  DevBuf sv_B, sv_V;               // N × 8 right-hand sides / solutions of the panel solves
-  DevBuf sv_bar;                   // grid-barrier counter of the cooperative solve kernels
-  DevBuf zf;                       // b (consumed) and z = L⁻¹·yn of the forward substitution carried along by the factorisation
+  DevBuf<double> sv_B, sv_V;       // N × 8 right-hand sides / solutions of the panel solves
+  DevBuf<unsigned> sv_bar;         // grid-barrier counter of the cooperative solve kernels
+  DevBuf<double> zf;               // b (consumed) and z = L⁻¹·yn of the forward substitution carried along by the factorisation
   bool z_ready = false;            // zf holds z of the current factorisation
   // ---- kbo_lml_batch: concurrent factorisations for several θ (fit.cu) --------------------------------------------------
   void* lml_lanes = nullptr;       // std::vector<LmlLane>*
-  DevBuf lml_yn, lml_scal;
+  DevBuf<double> lml_yn, lml_scal;
   cudaEvent_t lml_ev = nullptr;
   // ---- multi-GPU exchange (comm.cu): NCCL communicator bound at run time ------------------------------------------------
   void* comm = nullptr;            // ncclComm_t
   int comm_ranks = 1, comm_rank = 0;
-  DevBuf comm_buf;                 // n_ranks kbo_best gathered
+  DevBuf<kbo_best> comm_buf;       // n_ranks kbo_best gathered
 };
 
-enum ScalIdx { S_YMEAN = 0, S_YSTD = 1, S_YOPT = 2, S_LML = 3, S_LOGDET = 4, S_QUAD = 5, S_COUNT = 8 };
+// h->scal holds 16 doubles.  The first S_COUNT are the fit's scalars; S_WSCALE and S_WSCALE + 1 hold 2^s and 2^-s of the fp16 W
+// planes, and S_WAMAX, past S_COUNT, holds max |W| as the bit pattern of a uint64 (the atomic max of absmax_kernel).
+enum ScalIdx { S_YMEAN = 0, S_YSTD = 1, S_YOPT = 2, S_LML = 3, S_LOGDET = 4, S_QUAD = 5, S_WSCALE = 6, S_COUNT = 8, S_WAMAX = 8 };
 
 #define KBO_FAIL(h, code, ...)                         \
   do {                                                 \
@@ -190,26 +211,40 @@ enum ScalIdx { S_YMEAN = 0, S_YSTD = 1, S_YOPT = 2, S_LML = 3, S_LOGDET = 4, S_Q
       KBO_FAIL(h, KBO_ERR_CUDA, "kernel launch failed: %s (%s:%d)", cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
-static inline int kbo_reserve(kbo_handle* h, DevBuf& b, size_t bytes) {
-  if (bytes <= b.cap) return KBO_OK;
-  if (b.p) cudaFree(b.p);
-  b.p = nullptr;
-  b.cap = 0;
-  cudaError_t e = cudaMalloc(&b.p, bytes);
-  if (e != cudaSuccess) KBO_FAIL(h, KBO_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
-  b.cap = bytes;
-  return KBO_OK;
-}
 #define KBO_TRY(expr)          \
   do {                         \
     int _r = (expr);           \
     if (_r != KBO_OK) return _r; \
   } while (0)
-// bytes of host data into b (at least 4 bytes reserved, so an empty list still has a device pointer)
-static inline int kbo_upload(kbo_handle* h, DevBuf& b, const void* host, size_t bytes) {
-  KBO_TRY(kbo_reserve(h, b, bytes > 4 ? bytes : 4));
-  if (bytes) KBO_CUDA(h, cudaMemcpy(b.p, host, bytes, cudaMemcpyHostToDevice));
+// Room for n elements in b: grow-only, and the old contents are not kept.
+template <class T>
+static inline int kbo_reserve(kbo_handle* h, DevBuf<T>& b, size_t n) {
+  if (n <= b.cap) return KBO_OK;
+  if (b.p) cudaFree(b.p);
+  b.p = nullptr;
+  b.cap = 0;
+  const size_t bytes = sizeof(T) * n;
+  cudaError_t e = cudaMalloc(&b.p, bytes);
+  if (e != cudaSuccess) KBO_FAIL(h, KBO_ERR_NOMEM, "cudaMalloc(%zu) failed: %s", bytes, cudaGetErrorString(e));
+  b.cap = n;
   return KBO_OK;
+}
+// n elements of host data into b, synchronously (at least 4 bytes reserved, so an empty list still has a device pointer)
+template <class T>
+static inline int kbo_upload(kbo_handle* h, DevBuf<T>& b, const T* host, size_t n) {
+  KBO_TRY(kbo_reserve(h, b, std::max(n, (4 + sizeof(T) - 1) / sizeof(T))));
+  if (n) KBO_CUDA(h, cudaMemcpy(b.p, host, sizeof(T) * n, cudaMemcpyHostToDevice));
+  return KBO_OK;
+}
+// n elements from src to dst on s (cudaMemcpyAsync); the element types must agree
+template <class T>
+static inline cudaError_t kbo_copy(T* dst, const T* src, size_t n, cudaMemcpyKind kind, cudaStream_t s) {
+  return cudaMemcpyAsync(dst, src, sizeof(T) * n, kind, s);
+}
+// n elements of device data to out on s (cudaMemcpyAsync), or nothing when the caller passed no out
+template <class T>
+static inline cudaError_t kbo_d2h(T* out, const T* src, size_t n, cudaStream_t s) {
+  return out ? cudaMemcpyAsync(out, src, sizeof(T) * n, cudaMemcpyDeviceToHost, s) : cudaSuccess;
 }
 
 static inline int round_up(int x, int m) { return (x + m - 1) / m * m; }

@@ -158,12 +158,12 @@ static int tpe_history_append(kbo_handle* h, Sampler* t, const double* X, const 
   const size_t D = t->D;
   if (t->n + n_new > t->cap) {
     const int cap = std::max({2 * t->cap, t->n + n_new, 64});
-    DevBuf v, l;
-    KBO_TRY(kbo_reserve(h, v, 8 * D * cap));
-    KBO_TRY(kbo_reserve(h, l, 8 * (size_t)cap));
+    DevBuf<double> v, l;
+    KBO_TRY(kbo_reserve(h, v, D * cap));
+    KBO_TRY(kbo_reserve(h, l, (size_t)cap));
     if (t->n) {
-      KBO_CUDA(h, cudaMemcpyAsync(v.p, t->vals.p, 8 * D * t->n, cudaMemcpyDeviceToDevice, s));
-      KBO_CUDA(h, cudaMemcpyAsync(l.p, t->loss.p, 8 * (size_t)t->n, cudaMemcpyDeviceToDevice, s));
+      KBO_CUDA(h, kbo_copy(v.p, t->vals.p, D * t->n, cudaMemcpyDeviceToDevice, s));
+      KBO_CUDA(h, kbo_copy(l.p, t->loss.p, (size_t)t->n, cudaMemcpyDeviceToDevice, s));
       KBO_CUDA(h, cudaStreamSynchronize(s));
     }
     t->vals = std::move(v);
@@ -171,7 +171,7 @@ static int tpe_history_append(kbo_handle* h, Sampler* t, const double* X, const 
     t->cap = cap;
   }
   const cudaMemcpyKind kind = on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-  KBO_CUDA(h, cudaMemcpyAsync((double*)t->vals.p + D * t->n, X, 8 * D * n_new, kind, s));
-  KBO_CUDA(h, cudaMemcpyAsync((double*)t->loss.p + t->n, loss, 8 * (size_t)n_new, kind, s));
+  KBO_CUDA(h, kbo_copy(t->vals.p + D * t->n, X, D * n_new, kind, s));
+  KBO_CUDA(h, kbo_copy(t->loss.p + t->n, loss, (size_t)n_new, kind, s));
   return KBO_OK;
 }

@@ -163,16 +163,16 @@ extern "C" int kbo_lml_grad(kbo_handle* h, double* grad_host, int32_t n_out, voi
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   // Wt = Wᵀ into the trtri scratch, K⁻¹ (lower) into the K* fp64 scratch
-  KBO_TRY(kbo_reserve(h, h->T, sizeof(double) * (size_t)N * ld));
-  KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)N * ld));
+  KBO_TRY(kbo_reserve(h, h->T, (size_t)N * ld));
+  KBO_TRY(kbo_reserve(h, h->Ks64, (size_t)N * ld));
   const int nb = (N + 63) / 64;
-  KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * ((size_t)nb * nb * ncomp + ncomp)));
-  double* grad_dev = (double*)h->part.p + (size_t)nb * nb * ncomp;
-  KBO_TRY(kbo_i_lml_grad_from_w(h, (const double*)h->Xs.p, N, D, h->prm.kernel, h->prm.amplitude, h->prm.noise, (const double*)h->alpha.p,
-                                (const double*)h->W.p, (double*)h->T.p, (double*)h->Ks64.p, ld, P, (double*)h->part.p, grad_dev, s));
+  KBO_TRY(kbo_reserve(h, h->part, (size_t)nb * nb * ncomp + ncomp));
+  double* grad_dev = h->part.p + (size_t)nb * nb * ncomp;
+  KBO_TRY(kbo_i_lml_grad_from_w(h, h->Xs.p, N, D, h->prm.kernel, h->prm.amplitude, h->prm.noise, h->alpha.p,
+                                h->W.p, h->T.p, h->Ks64.p, ld, P, h->part.p, grad_dev, s));
   int inf = 0;
   KBO_CUDA(h, cudaMemcpyAsync(grad_host, grad_dev, sizeof(double) * ncomp, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&inf, h->info.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&inf, h->info.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   // a failed fit leaves L (and so K⁻¹) partly unfactored: the gradient built from it is meaningless
   if (inf != 0) KBO_FAIL(h, KBO_ERR_NOT_PD, "kernel matrix is not positive definite (pivot %d); increase `noise`", inf);

@@ -72,11 +72,22 @@ struct kbo_mvtpe {
   uint64_t seed = 0;
   uint32_t asks = 0;
   int n = 0, cap = 0, built_n = -1, nb = 0, mcap = 0;
-  DevBuf d_prm, d_flt, d_dsc, d_tabd;
-  DevBuf vals, loss, err;
-  DevBuf lkey, lkey2, lidx, lidx2, below, grp, pos, tmp;
-  DevBuf idx, w, c64, c2, mu32, dv, sg, fs, tab32, tab64, hdr;
-  DevBuf draws, prior, sc, lb, surv, bb;
+  DevBuf<MvParam> d_prm;
+  DevBuf<int> d_flt, d_dsc, d_tabd;
+  DevBuf<double> vals, loss;
+  DevBuf<int> err;
+  DevBuf<uint64_t> lkey, lkey2;
+  DevBuf<int> lidx, lidx2, below, grp, pos;
+  DevBuf<unsigned char> tmp;
+  DevBuf<int> idx, dv;
+  DevBuf<double> w, c64, sg, fs, tab64;
+  DevBuf<float> c2, mu32, tab32;
+  DevBuf<MvHdr> hdr;
+  DevBuf<double> draws, prior;
+  DevBuf<float2> sc;
+  DevBuf<unsigned> lb;
+  DevBuf<int> surv;
+  DevBuf<TpeBest> bb;
   std::vector<int> last_surv;
   EventSet<5> ev;
   float last_ms[4] = {};
@@ -582,21 +593,21 @@ static double host_log_gauss_mass_central(double h) { return std::log(std::erf(h
 
 static MvModels mv_models(kbo_mvtpe* t) {
   MvModels md;
-  md.prm = (const MvParam*)t->d_prm.p;
-  md.flt = (const int*)t->d_flt.p;
-  md.dsc = (const int*)t->d_dsc.p;
-  md.idx = (const int*)t->idx.p;
-  md.dv = (const int*)t->dv.p;
-  md.vals = (const double*)t->vals.p;
-  md.w = (const double*)t->w.p;
-  md.c64 = (const double*)t->c64.p;
-  md.sg = (const double*)t->sg.p;
-  md.fs = (const double*)t->fs.p;
-  md.tab64 = (const double*)t->tab64.p;
-  md.c2 = (const float*)t->c2.p;
-  md.mu32 = (const float*)t->mu32.p;
-  md.tab32 = (const float*)t->tab32.p;
-  md.hdr = (const MvHdr*)t->hdr.p;
+  md.prm = t->d_prm.p;
+  md.flt = t->d_flt.p;
+  md.dsc = t->d_dsc.p;
+  md.idx = t->idx.p;
+  md.dv = t->dv.p;
+  md.vals = t->vals.p;
+  md.w = t->w.p;
+  md.c64 = t->c64.p;
+  md.sg = t->sg.p;
+  md.fs = t->fs.p;
+  md.tab64 = t->tab64.p;
+  md.c2 = t->c2.p;
+  md.mu32 = t->mu32.p;
+  md.tab32 = t->tab32.p;
+  md.hdr = t->hdr.p;
   md.D = t->D;
   md.Df = t->Df;
   md.Dd = t->Dd;
@@ -619,17 +630,17 @@ static int mv_build(kbo_handle* h, kbo_mvtpe* t, cudaStream_t s) {
   const int nb = t->nb, m[2] = {nb, n - nb};
   t->mcap = round_up(std::max(n, 1), MV_BN);
   const size_t mc = t->mcap;
-  KBO_TRY(kbo_reserve(h, t->idx, 4 * 2 * mc));
-  KBO_TRY(kbo_reserve(h, t->w, 8 * 2 * (mc + 1)));
-  KBO_TRY(kbo_reserve(h, t->c64, 8 * 2 * mc));
-  KBO_TRY(kbo_reserve(h, t->c2, 4 * 2 * mc));
-  KBO_TRY(kbo_reserve(h, t->mu32, 4 * 2 * mc * std::max(t->Df, 1)));
-  KBO_TRY(kbo_reserve(h, t->dv, 4 * 2 * mc * std::max(t->Dd, 1)));
-  KBO_TRY(kbo_reserve(h, t->sg, 8 * 2 * (size_t)D));
-  KBO_TRY(kbo_reserve(h, t->fs, 8 * 2 * (size_t)std::max(t->Df, 1)));
-  KBO_TRY(kbo_reserve(h, t->tab64, 8 * 2 * (size_t)std::max(t->ltab, 1ll)));
-  KBO_TRY(kbo_reserve(h, t->tab32, 4 * 2 * (size_t)std::max(t->ltab, 1ll)));
-  KBO_TRY(kbo_reserve(h, t->hdr, sizeof(MvHdr) * 2));
+  KBO_TRY(kbo_reserve(h, t->idx, mc * 2));
+  KBO_TRY(kbo_reserve(h, t->w, (mc + 1) * 2));
+  KBO_TRY(kbo_reserve(h, t->c64, mc * 2));
+  KBO_TRY(kbo_reserve(h, t->c2, mc * 2));
+  KBO_TRY(kbo_reserve(h, t->mu32, mc * std::max(t->Df, 1) * 2));
+  KBO_TRY(kbo_reserve(h, t->dv, mc * std::max(t->Dd, 1) * 2));
+  KBO_TRY(kbo_reserve(h, t->sg, (size_t)D * 2));
+  KBO_TRY(kbo_reserve(h, t->fs, (size_t)std::max(t->Df, 1) * 2));
+  KBO_TRY(kbo_reserve(h, t->tab64, (size_t)std::max(t->ltab, 1ll) * 2));
+  KBO_TRY(kbo_reserve(h, t->tab32, (size_t)std::max(t->ltab, 1ll) * 2));
+  KBO_TRY(kbo_reserve(h, t->hdr, 2));
   // per group: sigma, the float scales, and the error-bound constants the host knows
   std::vector<double> sg(2 * D, NAN), fs(2 * std::max(t->Df, 1), 0.0);
   MvHdr hd[2];
@@ -653,44 +664,44 @@ static int mv_build(kbo_handle* h, kbo_mvtpe* t, cudaStream_t s) {
     hd[g].Bsum = (float)(bs * 1.0001);
     hd[g].XM = (float)(xm * 1.0001);
   }
-  KBO_CUDA(h, cudaMemcpyAsync(t->sg.p, sg.data(), 8 * sg.size(), cudaMemcpyHostToDevice, s));
-  KBO_CUDA(h, cudaMemcpyAsync(t->fs.p, fs.data(), 8 * fs.size(), cudaMemcpyHostToDevice, s));
-  KBO_CUDA(h, cudaMemcpyAsync(t->hdr.p, hd, sizeof hd, cudaMemcpyHostToDevice, s));
+  KBO_CUDA(h, kbo_copy(t->sg.p, sg.data(), sg.size(), cudaMemcpyHostToDevice, s));
+  KBO_CUDA(h, kbo_copy(t->fs.p, fs.data(), fs.size(), cudaMemcpyHostToDevice, s));
+  KBO_CUDA(h, kbo_copy(t->hdr.p, hd, 2, cudaMemcpyHostToDevice, s));
   if (n > 0) {
-    KBO_TRY(kbo_reserve(h, t->lkey, 8 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->lkey2, 8 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->lidx, 4 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->lidx2, 4 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->below, 4 * TPE_LF));
-    KBO_TRY(kbo_reserve(h, t->grp, 4 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->pos, 4 * (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->lkey, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->lkey2, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->lidx, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->lidx2, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->below, TPE_LF));
+    KBO_TRY(kbo_reserve(h, t->grp, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->pos, (size_t)n));
     size_t b1 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, b1, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int*)nullptr, (int*)nullptr, n, 0, 64, s);
     KBO_TRY(kbo_reserve(h, t->tmp, std::max<size_t>(b1, 16)));
     // the stable loss order (NumPy's argsort(kind='stable'); NaN losses are refused by tell)
-    tpe_loss_keys_kernel<<<(n + 255) / 256, 256, 0, s>>>((const double*)t->loss.p, n, (uint64_t*)t->lkey.p, (int*)t->lidx.p);
+    tpe_loss_keys_kernel<<<(n + 255) / 256, 256, 0, s>>>(t->loss.p, n, t->lkey.p, t->lidx.p);
     KBO_LAUNCH_CHECK(h);
     size_t bytes = t->tmp.cap;
-    KBO_CUDA(h, cub::DeviceRadixSort::SortPairs(t->tmp.p, bytes, (const uint64_t*)t->lkey.p, (uint64_t*)t->lkey2.p, (const int*)t->lidx.p,
-                                               (int*)t->lidx2.p, n, 0, 64, s));
-    tpe_split_kernel<<<1, 32, 0, s>>>((const int*)t->lidx2.p, nb, (int*)t->below.p);
+    KBO_CUDA(h, cub::DeviceRadixSort::SortPairs(t->tmp.p, bytes, t->lkey.p, t->lkey2.p, t->lidx.p,
+                                               t->lidx2.p, n, 0, 64, s));
+    tpe_split_kernel<<<1, 32, 0, s>>>(t->lidx2.p, nb, t->below.p);
     KBO_LAUNCH_CHECK(h);
-    tpe_group_kernel<<<(n + 255) / 256, 256, 0, s>>>((const int*)t->below.p, nb, n, (int*)t->grp.p, (int*)t->pos.p);
+    tpe_group_kernel<<<(n + 255) / 256, 256, 0, s>>>(t->below.p, nb, n, t->grp.p, t->pos.p);
     KBO_LAUNCH_CHECK(h);
-    mvtpe_members_kernel<<<(n + 255) / 256, 256, 0, s>>>((const int*)t->grp.p, (const int*)t->pos.p, n, t->mcap, (int*)t->idx.p);
+    mvtpe_members_kernel<<<(n + 255) / 256, 256, 0, s>>>(t->grp.p, t->pos.p, n, t->mcap, t->idx.p);
     KBO_LAUNCH_CHECK(h);
   }
-  mvtpe_weights_kernel<<<2, 256, 0, s>>>(t->mcap, (MvHdr*)t->hdr.p, (double*)t->w.p);
+  mvtpe_weights_kernel<<<2, 256, 0, s>>>(t->mcap, t->hdr.p, t->w.p);
   KBO_LAUNCH_CHECK(h);
   const MvModels md = mv_models(t);
   if (n > 0) {
-    mvtpe_model_kernel<<<dim3((n + 255) / 256, 2), 256, 0, s>>>(md, (double*)t->c64.p, (float*)t->c2.p, (float*)t->mu32.p, (int*)t->dv.p,
-                                                               (MvHdr*)t->hdr.p);
+    mvtpe_model_kernel<<<dim3((n + 255) / 256, 2), 256, 0, s>>>(md, t->c64.p, t->c2.p, t->mu32.p, t->dv.p,
+                                                               t->hdr.p);
     KBO_LAUNCH_CHECK(h);
   }
   if (!t->tabd.empty()) {
-    mvtpe_table_kernel<<<dim3((t->lmax + 255) / 256, (unsigned)t->tabd.size(), 2), 256, 0, s>>>(md, (const int*)t->d_tabd.p, (double*)t->tab64.p,
-                                                                                               (float*)t->tab32.p);
+    mvtpe_table_kernel<<<dim3((t->lmax + 255) / 256, (unsigned)t->tabd.size(), 2), 256, 0, s>>>(md, t->d_tabd.p, t->tab64.p,
+                                                                                               t->tab32.p);
     KBO_LAUNCH_CHECK(h);
   }
   KBO_CUDA(h, cudaStreamSynchronize(s));   // the host vectors above are read by the copies
@@ -760,11 +771,11 @@ int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* k
     P.ps = P.hi2 - P.lo2;
     P.lpm = lpm;
   }
-  KBO_TRY(kbo_upload(h, t->d_prm, t->prm.data(), sizeof(MvParam) * D));
-  KBO_TRY(kbo_upload(h, t->d_flt, t->flt.data(), 4 * t->flt.size()));
-  KBO_TRY(kbo_upload(h, t->d_dsc, t->dsc.data(), 4 * t->dsc.size()));
-  KBO_TRY(kbo_upload(h, t->d_tabd, t->tabd.data(), 4 * t->tabd.size()));
-  KBO_TRY(kbo_reserve(h, t->err, 4));
+  KBO_TRY(kbo_upload(h, t->d_prm, t->prm.data(), D));
+  KBO_TRY(kbo_upload(h, t->d_flt, t->flt.data(), t->flt.size()));
+  KBO_TRY(kbo_upload(h, t->d_dsc, t->dsc.data(), t->dsc.size()));
+  KBO_TRY(kbo_upload(h, t->d_tabd, t->tabd.data(), t->tabd.size()));
+  KBO_TRY(kbo_reserve(h, t->err, 1));
   KBO_TRY(t->ev.create());
   *out = t.release();
   return KBO_OK;
@@ -783,13 +794,13 @@ int kbo_mvtpe_tell(kbo_handle* h, kbo_mvtpe* t, const double* X, const double* l
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
   KBO_TRY(tpe_history_append(h, t, X, loss, n_new, on_host, s));
-  const double* Xn = (const double*)t->vals.p + (size_t)t->D * t->n;   // the new rows: checked before n counts them
-  const double* Ln = (const double*)t->loss.p + t->n;
-  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, 4, s));
-  mvtpe_check_kernel<<<(n_new + 255) / 256, 256, 0, s>>>((const MvParam*)t->d_prm.p, t->D, Xn, Ln, n_new, (int*)t->err.p);
+  const double* Xn = t->vals.p + (size_t)t->D * t->n;   // the new rows: checked before n counts them
+  const double* Ln = t->loss.p + t->n;
+  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, sizeof *t->err.p, s));
+  mvtpe_check_kernel<<<(n_new + 255) / 256, 256, 0, s>>>(t->d_prm.p, t->D, Xn, Ln, n_new, t->err.p);
   KBO_LAUNCH_CHECK(h);
   int err = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(&err, t->err.p, 4, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&err, t->err.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (err == 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_tell: a trial has a NaN loss (nothing was told)");
   if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_tell: a value is outside its parameter's domain: floats in [lo, hi], integers on their grid, category indices in range (nothing was told)");
@@ -811,43 +822,43 @@ int kbo_mvtpe_ask(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t M, const doubl
   const int D = t->D;
   const size_t KM = (size_t)k * M;
   const int nbb = (M + 255) / 256;
-  KBO_TRY(kbo_reserve(h, t->surv, 4 * (size_t)k));
-  KBO_TRY(kbo_reserve(h, t->bb, sizeof(TpeBest) * (size_t)k * nbb));
-  KBO_TRY(kbo_reserve(h, t->prior, 8 * KM));
-  KBO_TRY(kbo_reserve(h, t->sc, sizeof(float2) * KM));
-  KBO_TRY(kbo_reserve(h, t->lb, 4 * (size_t)k));
-  KBO_CUDA(h, cudaMemsetAsync(t->surv.p, 0, 4 * (size_t)k, s));
-  KBO_CUDA(h, cudaMemsetAsync(t->lb.p, 0, 4 * (size_t)k, s));
-  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, 4, s));
+  KBO_TRY(kbo_reserve(h, t->surv, (size_t)k));
+  KBO_TRY(kbo_reserve(h, t->bb, (size_t)k * nbb));
+  KBO_TRY(kbo_reserve(h, t->prior, KM));
+  KBO_TRY(kbo_reserve(h, t->sc, KM));
+  KBO_TRY(kbo_reserve(h, t->lb, (size_t)k));
+  KBO_CUDA(h, cudaMemsetAsync(t->surv.p, 0, sizeof *t->surv.p * (size_t)k, s));
+  KBO_CUDA(h, cudaMemsetAsync(t->lb.p, 0, sizeof *t->lb.p * (size_t)k, s));
+  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, sizeof *t->err.p, s));
   const MvModels md = mv_models(t);
   double* Xw = cand_out_dev;   // the working candidates: the caller's output buffer if it wants them, else the handle's
   if (!Xw) {
-    KBO_TRY(kbo_reserve(h, t->draws, 8 * KM * D));
-    Xw = (double*)t->draws.p;
+    KBO_TRY(kbo_reserve(h, t->draws, KM * D));
+    Xw = t->draws.p;
   }
   const dim3 gm((M + 255) / 256, k);
   if (!cand_dev) {
     mvtpe_draw_kernel<<<gm, 256, 0, s>>>(md, M, t->seed, ask, Xw);
     KBO_LAUNCH_CHECK(h);
   }
-  mvtpe_prep_kernel<<<gm, 256, 0, s>>>(md, M, cand_dev ? cand_dev : Xw, Xw, (double*)t->prior.p, (int*)t->err.p);
+  mvtpe_prep_kernel<<<gm, 256, 0, s>>>(md, M, cand_dev ? cand_dev : Xw, Xw, t->prior.p, t->err.p);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[1], s);
-  mvtpe_score_kernel<<<dim3((M + MV_BM - 1) / MV_BM, k), 256, 0, s>>>(md, M, Xw, (const double*)t->prior.p, (float2*)t->sc.p, score_out_dev,
-                                                                       (unsigned*)t->lb.p);
+  mvtpe_score_kernel<<<dim3((M + MV_BM - 1) / MV_BM, k), 256, 0, s>>>(md, M, Xw, t->prior.p, t->sc.p, score_out_dev,
+                                                                       t->lb.p);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[2], s);
-  mvtpe_decide_kernel<<<dim3(nbb, k), 256, 0, s>>>(md, M, Xw, (const double*)t->prior.p, (const float2*)t->sc.p, (const unsigned*)t->lb.p,
-                                                   (TpeBest*)t->bb.p, nbb, (int*)t->surv.p);
+  mvtpe_decide_kernel<<<dim3(nbb, k), 256, 0, s>>>(md, M, Xw, t->prior.p, t->sc.p, t->lb.p,
+                                                   t->bb.p, nbb, t->surv.p);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[3], s);
-  mvtpe_final_kernel<<<k, 256, 0, s>>>(D, M, Xw, (const TpeBest*)t->bb.p, nbb, x_dev, (long long*)idx_dev);
+  mvtpe_final_kernel<<<k, 256, 0, s>>>(D, M, Xw, t->bb.p, nbb, x_dev, (long long*)idx_dev);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[4], s);
   t->last_surv.assign(k, 0);
   int err = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(t->last_surv.data(), t->surv.p, 4 * (size_t)k, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&err, t->err.p, 4, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(t->last_surv.data(), t->surv.p, (size_t)k, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&err, t->err.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   for (int i = 0; i < 4; i++) cudaEventElapsedTime(&t->last_ms[i], t->ev[i], t->ev[i + 1]);
   if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: a supplied candidate is outside its parameter's domain (a float outside [lo, hi] or an invalid category index)");
@@ -862,14 +873,14 @@ int kbo_mvtpe_state(kbo_handle* h, kbo_mvtpe* t, int32_t group, double* w, doubl
   KBO_CUDA(h, cudaSetDevice(h->device));
   if (t->built_n != t->n) KBO_TRY(mv_build(h, t, s));
   const int D = t->D, m = group ? t->n - t->nb : t->nb, c = std::min(cap, m);
-  if (w) KBO_CUDA(h, cudaMemcpyAsync(w, (double*)t->w.p + (size_t)group * (t->mcap + 1), 8 * (size_t)std::min(cap, m + 1), cudaMemcpyDeviceToHost, s));
-  if (sigma) KBO_CUDA(h, cudaMemcpyAsync(sigma, (double*)t->sg.p + (size_t)group * D, 8 * (size_t)D, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_d2h(w, t->w.p + (size_t)group * (t->mcap + 1), (size_t)std::min(cap, m + 1), s));
+  KBO_CUDA(h, kbo_d2h(sigma, t->sg.p + (size_t)group * D, (size_t)D, s));
   if (mu && c > 0) {
     std::vector<int> idx(c);
-    KBO_CUDA(h, cudaMemcpyAsync(idx.data(), (int*)t->idx.p + (size_t)group * t->mcap, 4 * (size_t)c, cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, kbo_copy(idx.data(), t->idx.p + (size_t)group * t->mcap, (size_t)c, cudaMemcpyDeviceToHost, s));
     KBO_CUDA(h, cudaStreamSynchronize(s));
     for (int k = 0; k < c; k++)
-      KBO_CUDA(h, cudaMemcpyAsync(mu + (size_t)k * D, (double*)t->vals.p + (size_t)idx[k] * D, 8 * (size_t)D, cudaMemcpyDeviceToHost, s));
+      KBO_CUDA(h, kbo_copy(mu + (size_t)k * D, t->vals.p + (size_t)idx[k] * D, (size_t)D, cudaMemcpyDeviceToHost, s));
   }
   if (cat_rows)
     for (int d = 0; d < D; d++) {

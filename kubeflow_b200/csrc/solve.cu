@@ -222,17 +222,17 @@ __global__ void sv_col_kernel(const double* __restrict__ src, int N, int stride_
 
 #define SV_GMAX 8   // groups of 8 right-hand sides per forward launch (16 KB of shared memory each)
 static int sv_bar_reset(kbo_handle* h, cudaStream_t s) {
-  KBO_TRY(kbo_reserve(h, h->sv_bar, 256));
-  KBO_CUDA(h, cudaMemsetAsync(h->sv_bar.p, 0, sizeof(unsigned), s));
+  KBO_TRY(kbo_reserve(h, h->sv_bar, 64));
+  KBO_CUDA(h, cudaMemsetAsync(h->sv_bar.p, 0, sizeof *h->sv_bar.p, s));
   return KBO_OK;
 }
 // B (G groups of N × 8, overwritten: scratch) -> V = L⁻¹·B.  Needs the diagonal-block inverses in W's diagonal 256-blocks.
 int kbo_i_solve_fwd(kbo_handle* h, double* B, double* V, cudaStream_t s, int G, size_t gstride) {
   KBO_TRY(sv_bar_reset(h, s));
-  const double* L = (const double*)h->K.p;
-  const double* W = (const double*)h->W.p;
+  const double* L = h->K.p;
+  const double* W = h->W.p;
   int N = h->N, ld = h->ld;
-  unsigned* bar = (unsigned*)h->sv_bar.p;
+  unsigned* bar = h->sv_bar.p;
   const size_t smem = sizeof(double) * (size_t)G * SV_R * SV_P;
   static bool attr = false;
   if (!attr) {
@@ -247,10 +247,10 @@ int kbo_i_solve_fwd(kbo_handle* h, double* B, double* V, cudaStream_t s, int G, 
 // Z (N × 8, overwritten) -> A = L⁻ᵀ·Z (N × 8)
 int kbo_i_solve_bwd(kbo_handle* h, double* Z, double* A, cudaStream_t s) {
   KBO_TRY(sv_bar_reset(h, s));
-  const double* L = (const double*)h->K.p;
-  const double* W = (const double*)h->W.p;
+  const double* L = h->K.p;
+  const double* W = h->W.p;
   int N = h->N, ld = h->ld;
-  unsigned* bar = (unsigned*)h->sv_bar.p;
+  unsigned* bar = h->sv_bar.p;
   void* args[] = {(void*)&L, (void*)&W, (void*)&N, (void*)&ld, (void*)&Z, (void*)&A, (void*)&bar};
   KBO_CUDA(h, cudaLaunchCooperativeKernel((const void*)sv_backward_kernel, dim3(h->sm_count), dim3(256), args, 0, s));
   return KBO_OK;
@@ -294,16 +294,16 @@ __global__ void __launch_bounds__(256) sv_zupdate_kernel(const double* __restric
 }
 }  // namespace
 int kbo_i_zsolve_begin(kbo_handle* h, cudaStream_t s) {
-  KBO_TRY(kbo_reserve(h, h->zf, sizeof(double) * 2 * (size_t)(h->N + SV_P)));
-  KBO_CUDA(h, cudaMemcpyAsync(h->zf.p, h->yn.p, sizeof(double) * h->N, cudaMemcpyDeviceToDevice, s));
+  KBO_TRY(kbo_reserve(h, h->zf, (size_t)(h->N + SV_P) * 2));
+  KBO_CUDA(h, kbo_copy(h->zf.p, h->yn.p, h->N, cudaMemcpyDeviceToDevice, s));
   h->z_ready = false;
   return KBO_OK;
 }
 // panel [K0, K0 + Wd): z_P = W_PP·b_P (needs W's diagonal 256-block) ...
 int kbo_i_zsolve_diag(kbo_handle* h, int K0, int Wd, cudaStream_t s) {
-  double* b = (double*)h->zf.p;
+  double* b = h->zf.p;
   double* z = b + h->N + SV_P;
-  sv_zdiag_kernel<<<(Wd + 7) / 8, 256, 0, s>>>((const double*)h->W.p + (size_t)K0 * h->ld + K0, h->ld, Wd, b + K0, z + K0);
+  sv_zdiag_kernel<<<(Wd + 7) / 8, 256, 0, s>>>(h->W.p + (size_t)K0 * h->ld + K0, h->ld, Wd, b + K0, z + K0);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }
@@ -311,9 +311,9 @@ int kbo_i_zsolve_diag(kbo_handle* h, int K0, int Wd, cudaStream_t s) {
 int kbo_i_zsolve_update(kbo_handle* h, int K0, int Wd, cudaStream_t s) {
   const int N = h->N, rows = N - (K0 + Wd);
   if (rows <= 0) return KBO_OK;
-  double* b = (double*)h->zf.p;
+  double* b = h->zf.p;
   double* z = b + N + SV_P;
-  sv_zupdate_kernel<<<(rows + 7) / 8, 256, 0, s>>>((const double*)h->K.p + (size_t)(K0 + Wd) * h->ld + K0, h->ld, rows, Wd, z + K0, b + K0 + Wd);
+  sv_zupdate_kernel<<<(rows + 7) / 8, 256, 0, s>>>(h->K.p + (size_t)(K0 + Wd) * h->ld + K0, h->ld, rows, Wd, z + K0, b + K0 + Wd);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }
@@ -321,23 +321,23 @@ int kbo_i_zsolve_update(kbo_handle* h, int K0, int Wd, cudaStream_t s) {
 // alpha = L⁻ᵀ(L⁻¹·yn) into h->alpha (what fit_finish computes as Wᵀ(W·yn) when W is formed)
 int kbo_i_alpha_by_solves(kbo_handle* h, cudaStream_t s) {
   const int N = h->N;
-  KBO_TRY(kbo_reserve(h, h->sv_B, sizeof(double) * (size_t)(N + SV_P) * SV_R));
-  KBO_TRY(kbo_reserve(h, h->sv_V, sizeof(double) * (size_t)(N + SV_P) * SV_R));
-  double* B = (double*)h->sv_B.p;
-  double* V = (double*)h->sv_V.p;
+  KBO_TRY(kbo_reserve(h, h->sv_B, (size_t)(N + SV_P) * SV_R));
+  KBO_TRY(kbo_reserve(h, h->sv_V, (size_t)(N + SV_P) * SV_R));
+  double* B = h->sv_B.p;
+  double* V = h->sv_V.p;
   if (h->z_ready) {   // the factorisation already carried z = L⁻¹·yn along (kbo_i_zsolve_*)
     KBO_CUDA(h, cudaMemsetAsync(V, 0, sizeof(double) * (size_t)N * SV_R, s));
-    sv_col_kernel<<<(N + 255) / 256, 256, 0, s>>>((const double*)h->zf.p + N + SV_P, N, 1, V, SV_R);
+    sv_col_kernel<<<(N + 255) / 256, 256, 0, s>>>(h->zf.p + N + SV_P, N, 1, V, SV_R);
     KBO_LAUNCH_CHECK(h);
     h->z_ready = false;
   } else {
     KBO_CUDA(h, cudaMemsetAsync(B, 0, sizeof(double) * (size_t)N * SV_R, s));
-    sv_col_kernel<<<(N + 255) / 256, 256, 0, s>>>((const double*)h->yn.p, N, 1, B, SV_R);
+    sv_col_kernel<<<(N + 255) / 256, 256, 0, s>>>(h->yn.p, N, 1, B, SV_R);
     KBO_LAUNCH_CHECK(h);
     KBO_TRY(kbo_i_solve_fwd(h, B, V, s, 1, 0));      // V[:,0] = z
   }
   KBO_TRY(kbo_i_solve_bwd(h, V, B, s));      // B[:,0] = alpha (V is consumed)
-  sv_col_kernel<<<(N + 255) / 256, 256, 0, s>>>(B, N, SV_R, (double*)h->alpha.p, 1);
+  sv_col_kernel<<<(N + 255) / 256, 256, 0, s>>>(B, N, SV_R, h->alpha.p, 1);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }
@@ -346,10 +346,10 @@ int kbo_i_alpha_by_solves(kbo_handle* h, cudaStream_t s) {
 int kbo_i_variance_by_solves(kbo_handle* h, const double* Ks, int n, double* varn64, cudaStream_t s) {
   const int N = h->N, ld = h->ld;
   const size_t gstride = (size_t)(N + SV_P) * SV_R;
-  KBO_TRY(kbo_reserve(h, h->sv_B, sizeof(double) * gstride * SV_GMAX));
-  KBO_TRY(kbo_reserve(h, h->sv_V, sizeof(double) * gstride * SV_GMAX));
-  double* B = (double*)h->sv_B.p;
-  double* V = (double*)h->sv_V.p;
+  KBO_TRY(kbo_reserve(h, h->sv_B, gstride * SV_GMAX));
+  KBO_TRY(kbo_reserve(h, h->sv_V, gstride * SV_GMAX));
+  double* B = h->sv_B.p;
+  double* V = h->sv_V.p;
   for (int c0 = 0; c0 < n; c0 += SV_R * SV_GMAX) {
     const int nc = n - c0 < SV_R * SV_GMAX ? n - c0 : SV_R * SV_GMAX, G = (nc + SV_R - 1) / SV_R;
     for (int g = 0; g < G; g++) {

@@ -677,13 +677,14 @@ static int launch_acq(kbo_handle* h, const T* mun, const T* varn, int64_t M, int
                       cudaStream_t s) {
   const int g = acq_grid(h, M);
   if (h->blockbest.cap == 0) {
-    KBO_TRY(kbo_reserve(h, h->blockbest, sizeof(BlockBest) * (size_t)h->sm_count * 8 + 64));
-    KBO_CUDA(h, cudaMemsetAsync(h->blockbest.p, 0, h->blockbest.cap, s));
+    KBO_TRY(kbo_reserve(h, h->blockbest, (size_t)h->sm_count * 8 + 4));
+    KBO_CUDA(h, cudaMemsetAsync(h->blockbest.p, 0, sizeof *h->blockbest.p * h->blockbest.cap, s));
   }
-  unsigned int* ticket = (unsigned int*)((BlockBest*)h->blockbest.p + (size_t)h->sm_count * 8);
+  // the last-block ticket lives in the 64 bytes past the partials (BlockBest entries are 16-byte aligned)
+  unsigned int* ticket = reinterpret_cast<unsigned int*>(h->blockbest.p + (size_t)h->sm_count * 8);
 #define KBO_ACQ_LAUNCH(FA)                                                                                                     \
   acq_kernel<T, FA><<<g, 256, 0, s>>>(mun, varn, M, goff, acq, ymean, ystd, yopt, scal_dev, xi, kappa, mu_out, std_out, acq_out, \
-                                      acq_out32, (BlockBest*)h->blockbest.p, ticket, best_dev)
+                                      acq_out32, h->blockbest.p, ticket, best_dev)
   if (sizeof(T) == 4 && !mu_out && !std_out) {
     if (acq == KBO_ACQ_EI) KBO_ACQ_LAUNCH(KBO_ACQ_EI);
     else if (acq == KBO_ACQ_LCB) KBO_ACQ_LAUNCH(KBO_ACQ_LCB);
@@ -726,12 +727,12 @@ static int launch_cross(kbo_handle* h, const XT* Xc, int64_t rows, int64_t rows_
   if (gx < 2u * h->sm_count) nsplit = (int)min((unsigned)min(ntiles, 16), max(1u, 2u * h->sm_count / gx));
   double* part = nullptr;
   if (nsplit > 1) {
-    KBO_TRY(kbo_reserve(h, h->mu_part, sizeof(double) * (size_t)nsplit * rows));
-    part = (double*)h->mu_part.p;
+    KBO_TRY(kbo_reserve(h, h->mu_part, (size_t)nsplit * rows));
+    part = h->mu_part.p;
   }
   cross_mean_kernel<XT, MT, MODE><<<dim3(gx, nsplit), 256, smem, s>>>(
-      Xc, rows, h->D, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(), (const double*)h->XsT.p, h->ld, (const double*)h->nx.p, h->N,
-      (const double*)h->alpha.p, h->prm.kernel, h->prm.amplitude, Ks64, ldks, Ksh, Ksl, h->Npad, mun, part);
+      Xc, rows, h->D, h->d_inv_ls.p, (int)h->inv_ls.size(), h->XsT.p, h->ld, h->nx.p, h->N,
+      h->alpha.p, h->prm.kernel, h->prm.amplitude, Ks64, ldks, Ksh, Ksl, h->Npad, mun, part);
   KBO_LAUNCH_CHECK(h);
   if (nsplit > 1) {
     mu_parts_kernel<MT><<<(unsigned)((rows + 255) / 256), 256, 0, s>>>(part, rows, nsplit, mun);
@@ -811,43 +812,43 @@ static int refine_union(kbo_handle* h, const void* Xc, int xc_dtype, int64_t gof
     up.n[k] = (int)sp.list[k].size();
     for (int idx : sp.list[k]) host.push_back((int)(std::lower_bound(U.begin(), U.end(), idx) - U.begin()));
   }
-  KBO_TRY(kbo_reserve(h, h->un_idx, sizeof(int) * host.size()));
-  KBO_TRY(kbo_reserve(h, h->un_mv, sizeof(double) * 2 * (size_t)nu));
-  int* uidx = (int*)h->un_idx.p;
-  double* mun64 = (double*)h->un_mv.p;
+  KBO_TRY(kbo_reserve(h, h->un_idx, host.size()));
+  KBO_TRY(kbo_reserve(h, h->un_mv, (size_t)nu * 2));
+  int* uidx = h->un_idx.p;
+  double* mun64 = h->un_mv.p;
   double* varn64 = mun64 + nu;
   KBO_CUDA(h, cudaMemcpyAsync(uidx, host.data(), sizeof(int) * host.size(), cudaMemcpyHostToDevice, s));
   const int njt = (N + 7) / 8;   // row blocks of refine_var_kernel (8 rows of W per CTA)
   for (int b0 = 0; b0 < nu; b0 += KBO_UNION_BATCH) {
     const int m = nu - b0 < KBO_UNION_BATCH ? nu - b0 : KBO_UNION_BATCH;
-    KBO_TRY(kbo_reserve(h, h->refine_x, sizeof(double) * (size_t)m * D));
-    KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)m * ld));
-    KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * (size_t)m * njt));
-    double* Xg = (double*)h->refine_x.p;
+    KBO_TRY(kbo_reserve(h, h->refine_x, (size_t)m * D));
+    KBO_TRY(kbo_reserve(h, h->Ks64, (size_t)m * ld));
+    KBO_TRY(kbo_reserve(h, h->part, (size_t)m * njt));
+    double* Xg = h->refine_x.p;
     if (xc_dtype == KBO_F64)
       gather_rows_kernel<double><<<m, 64, 0, s>>>((const double*)Xc, D, uidx + b0, m, Xg);
     else
       gather_rows_kernel<float><<<m, 64, 0, s>>>((const float*)Xc, D, uidx + b0, m, Xg);
     KBO_LAUNCH_CHECK(h);
-    refine_cross_kernel<<<dim3((N + 255) / 256, m), 256, 0, s>>>(Xg, D, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(), (const double*)h->XsT.p, ld, N,
-                                                                 h->prm.kernel, h->prm.amplitude, (double*)h->Ks64.p);
+    refine_cross_kernel<<<dim3((N + 255) / 256, m), 256, 0, s>>>(Xg, D, h->d_inv_ls.p, (int)h->inv_ls.size(), h->XsT.p, ld, N,
+                                                                 h->prm.kernel, h->prm.amplitude, h->Ks64.p);
     KBO_LAUNCH_CHECK(h);
-    refine_mu_kernel<<<m, 256, 0, s>>>((const double*)h->Ks64.p, ld, N, (const double*)h->alpha.p, mun64 + b0);
+    refine_mu_kernel<<<m, 256, 0, s>>>(h->Ks64.p, ld, N, h->alpha.p, mun64 + b0);
     KBO_LAUNCH_CHECK(h);
     if (!h->w_full) {
       // lazy inverse: ‖L⁻¹k*‖² by panel solves with the factor itself (solve.cu) — no W
-      KBO_TRY(kbo_i_variance_by_solves(h, (const double*)h->Ks64.p, m, varn64 + b0, s));
+      KBO_TRY(kbo_i_variance_by_solves(h, h->Ks64.p, m, varn64 + b0, s));
     } else {
       if (m <= 2)   // the usual case: one contender — no point carrying eight accumulators through the triangle of W
-        refine_var_kernel<1><<<dim3(njt, m), 256, 0, s>>>((const double*)h->W.p, ld, N, (const double*)h->Ks64.p, m, (double*)h->part.p, njt);
+        refine_var_kernel<1><<<dim3(njt, m), 256, 0, s>>>(h->W.p, ld, N, h->Ks64.p, m, h->part.p, njt);
       else
-        refine_var_kernel<8><<<dim3(njt, (m + 7) / 8), 256, 0, s>>>((const double*)h->W.p, ld, N, (const double*)h->Ks64.p, m, (double*)h->part.p, njt);
+        refine_var_kernel<8><<<dim3(njt, (m + 7) / 8), 256, 0, s>>>(h->W.p, ld, N, h->Ks64.p, m, h->part.p, njt);
       KBO_LAUNCH_CHECK(h);
-      var_from_parts_kernel<<<(m + 255) / 256, 256, 0, s>>>((const double*)h->part.p, m, njt, h->prm.amplitude, varn64 + b0);
+      var_from_parts_kernel<<<(m + 255) / 256, 256, 0, s>>>(h->part.p, m, njt, h->prm.amplitude, varn64 + b0);
       KBO_LAUNCH_CHECK(h);
     }
   }
-  refine_best_union_kernel<<<sp.nk, 1024, 0, s>>>(mun64, varn64, uidx, uidx + nu, up, (const double*)h->scal.p, h->prm.xi, h->prm.kappa, goff);
+  refine_best_union_kernel<<<sp.nk, 1024, 0, s>>>(mun64, varn64, uidx, uidx + nu, up, h->scal.p, h->prm.xi, h->prm.kappa, goff);
   KBO_LAUNCH_CHECK(h);
   // the host copies above must outlive the asynchronous H2D copy
   KBO_CUDA(h, cudaStreamSynchronize(s));
@@ -891,9 +892,9 @@ static int record_stage(kbo_handle* h, int stage, int acq, int cal_n, const floa
 
 // contenders of the three-product sweep's window (see below) for one acquisition; a list that fits is handed to sp
 static int refine_suggestion(kbo_handle* h, int64_t M, int64_t goff, AcqDecision& d, StagePicks& sp, cudaStream_t s) {
-  const double* scal = (const double*)h->scal.p;
-  KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
-  int* list = (int*)h->refine.p;
+  const double* scal = h->scal.p;
+  KBO_TRY(kbo_reserve(h, h->refine, KBO_REFINE_CAP + 16));
+  int* list = h->refine.p;
   int* count = list + KBO_REFINE_CAP;
   // contenders: within delta of the fp32 maximum, in normalised units (2e-4·y_std on the raw scale; for LCB the raw value is
   // ≈ −y_mean, whose fp32 ulp alone can exceed any absolute window).  2e-4 is ≥ 10× the tensor-core mode's acquisition error
@@ -906,7 +907,7 @@ static int refine_suggestion(kbo_handle* h, int64_t M, int64_t goff, AcqDecision
   d.unrefined = 0;
   for (int round = 0; round < 24; round++) {
     KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
-    contender_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa,
+    contender_kernel<<<acq_grid(h, M), 256, 0, s>>>(kbo_view<float>(h->mun), kbo_view<float>(h->varn), M, d.acq, scal, h->prm.xi, h->prm.kappa,
                                                     d.best, goff, delta, list, count);
     KBO_LAUNCH_CHECK(h);
     KBO_CUDA(h, cudaMemcpyAsync(&n, count, sizeof(int), cudaMemcpyDeviceToHost, s));
@@ -1124,13 +1125,13 @@ static int prefix_grid_pass(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
     h->tim.chunks++;
     {
       KBO_TIME_BEGIN(ev_cross, ev_cross_used);
-      KBO_TRY(kbo_i_tc_kstar(h, xc, xc_dtype, rows, (__half*)h->Ksh.p, (float*)h->mun.p + c0, s, P1 * 512));
+      KBO_TRY(kbo_i_tc_kstar(h, xc, xc_dtype, rows, h->Ksh.p, kbo_view<float>(h->mun) + c0, s, P1 * 512));
       KBO_TIME_END();
     }
     {
       KBO_TIME_BEGIN(ev_var, ev_var_used);
-      KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, round_up64(rows, 256), (const __half*)h->Wh.p, h->Npad, h->prm.amplitude,
-                            (float*)h->varn.p + c0, s, 0, P1));
+      KBO_TRY(kbo_i_tc_rank(h, h->Ksh.p, round_up64(rows, 256), h->Wh.p, h->Npad, h->prm.amplitude,
+                            kbo_view<float>(h->varn) + c0, s, 0, P1));
       KBO_TIME_END();
     }
   }
@@ -1160,25 +1161,25 @@ static int read_bounds(kbo_handle* h, const int* count, int* n, cudaStream_t s) 
 static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int64_t chunk, AcqDecision* dec, int n_acq,
                             cudaStream_t s) {
   const int Npad = h->Npad;
-  const double* scal = (const double*)h->scal.p;
+  const double* scal = h->scal.p;
   const int P1 = kbo_prefix_pairs(h);
   if (P1 < 1 || P1 >= kbo_tile_pairs(Npad) || P1 * 512 > h->w_lead) return KBO_OK;
-  KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
-  int* count = (int*)h->refine.p + KBO_REFINE_CAP;
-  float* fs = (float*)(count + 4);
-  KBO_TRY(kbo_reserve(h, h->pr_list, sizeof(int) * (KBO_PRUNE_CAP + 16)));
-  int* plist = (int*)h->pr_list.p;
+  KBO_TRY(kbo_reserve(h, h->refine, KBO_REFINE_CAP + 16));
+  int* count = h->refine.p + KBO_REFINE_CAP;
+  float* fs = reinterpret_cast<float*>(count + 4);   // the bounds after the count (see h->refine)
+  KBO_TRY(kbo_reserve(h, h->pr_list, KBO_PRUNE_CAP + 16));
+  int* plist = h->pr_list.p;
   int* pcount = plist + KBO_PRUNE_CAP;
   int cal_n = 0;
   {
     KBO_TIME_BEGIN(ev_cal, ev_cal_used);
     KBO_TRY(calibration_rows(h, Xc, xc_dtype, M, &cal_n, s, 2 * P1));   // cal_mu exact, var_cal = exact prefix bound
     const int64_t cal_pad = round_up64(cal_n, 256);
-    KBO_TRY(kbo_reserve(h, h->cal_mu_rk, sizeof(float) * (size_t)(cal_pad + 256)));
-    KBO_TRY(kbo_reserve(h, h->cal_var_rk, sizeof(float) * (size_t)(cal_pad + 256)));
-    KBO_TRY(kbo_i_tc_kstar(h, h->cal_x.p, KBO_F64, cal_n, (__half*)h->Ksh.p, (float*)h->cal_mu_rk.p, s, P1 * 512));
-    KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, cal_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->cal_var_rk.p, s, 0, P1));
-    calib_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p,
+    KBO_TRY(kbo_reserve(h, h->cal_mu_rk, (size_t)(cal_pad + 256)));
+    KBO_TRY(kbo_reserve(h, h->cal_var_rk, (size_t)(cal_pad + 256)));
+    KBO_TRY(kbo_i_tc_kstar(h, h->cal_x.p, KBO_F64, cal_n, h->Ksh.p, h->cal_mu_rk.p, s, P1 * 512));
+    KBO_TRY(kbo_i_tc_rank(h, h->Ksh.p, cal_pad, h->Wh.p, Npad, h->prm.amplitude, h->cal_var_rk.p, s, 0, P1));
+    calib_kernel<<<1, 1024, 0, s>>>(h->cal_var_rk.p, h->var_cal.p, h->cal_mu_rk.p, h->cal_mu.p,
                                     nullptr, cal_n, -1, nullptr, 0.0, 0.0, fs);
     KBO_LAUNCH_CHECK(h);
     KBO_TIME_END();
@@ -1191,9 +1192,9 @@ static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
     if (d.done) continue;
     KBO_CUDA(h, cudaMemsetAsync(pcount, 0, sizeof(int), s));
     KBO_CUDA(h, cudaMemsetAsync(fs + 1, 0, sizeof(float), s));   // this kind's lower bound starts below every ordered value
-    grid_lower_bound_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+    grid_lower_bound_kernel<<<acq_grid(h, M), 256, 0, s>>>(kbo_view<float>(h->mun), kbo_view<float>(h->varn), M, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
     KBO_LAUNCH_CHECK(h);
-    prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
+    prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>(kbo_view<float>(h->mun), kbo_view<float>(h->varn), M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
                                                          pcount, KBO_PRUNE_CAP);
     KBO_LAUNCH_CHECK(h);
     int n1 = 0;
@@ -1218,25 +1219,25 @@ static int prune_sweep_lead(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
 static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int64_t goff, int cal_n, int64_t chunk, AcqDecision* dec, int n_acq,
                        cudaStream_t s) {
   const int D = h->D, Npad = h->Npad;
-  const double* scal = (const double*)h->scal.p;
+  const double* scal = h->scal.p;
   int P1 = kbo_prefix_pairs(h);
   if (P1 < 1) P1 = 1;
   if (P1 >= kbo_tile_pairs(Npad)) return KBO_OK;   // nothing to save: the caller's full pass is the prefix
-  KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
-  int* list = (int*)h->refine.p;
+  KBO_TRY(kbo_reserve(h, h->refine, KBO_REFINE_CAP + 16));
+  int* list = h->refine.p;
   int* count = list + KBO_REFINE_CAP;
-  float* fs = (float*)(count + 4);
-  KBO_TRY(kbo_reserve(h, h->pr_list, sizeof(int) * (KBO_PRUNE_CAP + 16)));
-  int* plist = (int*)h->pr_list.p;
+  float* fs = reinterpret_cast<float*>(count + 4);   // the bounds after the count (see h->refine)
+  KBO_TRY(kbo_reserve(h, h->pr_list, KBO_PRUNE_CAP + 16));
+  int* plist = h->pr_list.p;
   int* pcount = plist + KBO_PRUNE_CAP;
   const int64_t cal_pad = round_up64(cal_n, 256);
-  KBO_TRY(kbo_reserve(h, h->cal_mu_rk, sizeof(float) * (size_t)(cal_pad + 256)));
-  KBO_TRY(kbo_reserve(h, h->cal_var_rk, sizeof(float) * (size_t)(cal_pad + 256)));
+  KBO_TRY(kbo_reserve(h, h->cal_mu_rk, (size_t)(cal_pad + 256)));
+  KBO_TRY(kbo_reserve(h, h->cal_var_rk, (size_t)(cal_pad + 256)));
   {
     KBO_TIME_BEGIN(ev_cal, ev_cal_used);
     // the ranking arithmetic on the calibration rows (all tile pairs): what E and Emu are measured from
-    KBO_TRY(kbo_i_tc_kstar(h, h->cal_x.p, KBO_F64, cal_n, (__half*)h->Ksh.p, (float*)h->cal_mu_rk.p, s));
-    KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, cal_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->cal_var_rk.p, s));
+    KBO_TRY(kbo_i_tc_kstar(h, h->cal_x.p, KBO_F64, cal_n, h->Ksh.p, h->cal_mu_rk.p, s));
+    KBO_TRY(kbo_i_tc_rank(h, h->Ksh.p, cal_pad, h->Wh.p, Npad, h->prm.amplitude, h->cal_var_rk.p, s));
     KBO_TIME_END();
   }
   // pass 1 over the grid: mean over all trials, variance bound from the first P1 tile pairs
@@ -1247,11 +1248,11 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     AcqDecision& d = dec[k];
     if (d.done) continue;
     // E, Emu and this kind's lower bound on the maximum from the calibration rows (one CTA over one wave of rows)
-    calib_kernel<<<1, 1024, 0, s>>>((const float*)h->cal_var_rk.p, (const float*)h->var_cal.p, (const float*)h->cal_mu_rk.p, (const float*)h->cal_mu.p,
+    calib_kernel<<<1, 1024, 0, s>>>(h->cal_var_rk.p, h->var_cal.p, h->cal_mu_rk.p, h->cal_mu.p,
                                     nullptr, cal_n, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
     KBO_LAUNCH_CHECK(h);
     KBO_CUDA(h, cudaMemsetAsync(pcount, 0, sizeof(int), s));
-    prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
+    prefix_survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>(kbo_view<float>(h->mun), kbo_view<float>(h->varn), M, d.acq, scal, h->prm.xi, h->prm.kappa, fs, plist,
                                                          pcount, KBO_PRUNE_CAP);
     KBO_LAUNCH_CHECK(h);
     int n1 = 0;
@@ -1262,21 +1263,21 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
     if (n1 < 1 || n1 > KBO_PRUNE_CAP) continue;
     // pass 2: the survivors' rows through the whole ranking pass, then the interval test and the FP64 decision
     const int64_t n1_pad = round_up64(n1, 256);
-    KBO_TRY(kbo_reserve(h, h->pr_x, sizeof(double) * (size_t)n1_pad * D));
-    KBO_TRY(kbo_reserve(h, h->pr_mu, sizeof(float) * (size_t)(n1_pad + 256)));
-    KBO_TRY(kbo_reserve(h, h->pr_var, sizeof(float) * (size_t)(n1_pad + 256)));
+    KBO_TRY(kbo_reserve(h, h->pr_x, (size_t)n1_pad * D));
+    KBO_TRY(kbo_reserve(h, h->pr_mu, (size_t)(n1_pad + 256)));
+    KBO_TRY(kbo_reserve(h, h->pr_var, (size_t)(n1_pad + 256)));
     if (xc_dtype == KBO_F64)
-      gather_rows_kernel<double><<<n1, 64, 0, s>>>((const double*)Xc, D, plist, n1, (double*)h->pr_x.p);
+      gather_rows_kernel<double><<<n1, 64, 0, s>>>((const double*)Xc, D, plist, n1, h->pr_x.p);
     else
-      gather_rows_kernel<float><<<n1, 64, 0, s>>>((const float*)Xc, D, plist, n1, (double*)h->pr_x.p);
+      gather_rows_kernel<float><<<n1, 64, 0, s>>>((const float*)Xc, D, plist, n1, h->pr_x.p);
     KBO_LAUNCH_CHECK(h);
-    KBO_TRY(kbo_i_tc_kstar(h, h->pr_x.p, KBO_F64, n1, (__half*)h->Ksh.p, (float*)h->pr_mu.p, s));
-    KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, n1_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->pr_var.p, s));
+    KBO_TRY(kbo_i_tc_kstar(h, h->pr_x.p, KBO_F64, n1, h->Ksh.p, h->pr_mu.p, s));
+    KBO_TRY(kbo_i_tc_rank(h, h->Ksh.p, n1_pad, h->Wh.p, Npad, h->prm.amplitude, h->pr_var.p, s));
     KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
     const int g2 = (n1 + 255) / 256;
-    bound_max_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+    bound_max_kernel<<<g2, 256, 0, s>>>(h->pr_mu.p, h->pr_var.p, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
     KBO_LAUNCH_CHECK(h);
-    survivor_kernel<<<g2, 256, 0, s>>>((const float*)h->pr_mu.p, (const float*)h->pr_var.p, plist, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs, list,
+    survivor_kernel<<<g2, 256, 0, s>>>(h->pr_mu.p, h->pr_var.p, plist, n1, d.acq, scal, h->prm.xi, h->prm.kappa, fs, list,
                                        count);
     KBO_LAUNCH_CHECK(h);
     int n2 = 0;
@@ -1296,18 +1297,18 @@ static int prune_sweep(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, i
 // The interval test of the full ranking pass for one acquisition; survivors that fit go to sp.  Not handed over: they do not
 // fit (the caller redoes the sweep with three products).
 static int fast_pick(kbo_handle* h, int64_t M, int cal_n, AcqDecision& d, StagePicks& sp, cudaStream_t s) {
-  const double* scal = (const double*)h->scal.p;
-  KBO_TRY(kbo_reserve(h, h->refine, sizeof(int) * (KBO_REFINE_CAP + 16)));
-  int* list = (int*)h->refine.p;
+  const double* scal = h->scal.p;
+  KBO_TRY(kbo_reserve(h, h->refine, KBO_REFINE_CAP + 16));
+  int* list = h->refine.p;
   int* count = list + KBO_REFINE_CAP;
-  float* fs = (float*)(count + 4);
+  float* fs = reinterpret_cast<float*>(count + 4);   // the bounds after the count (see h->refine)
   KBO_CUDA(h, cudaMemsetAsync(count, 0, sizeof(int), s));
-  calib_kernel<<<1, 1024, 0, s>>>((const float*)h->varn.p, (const float*)h->var_cal.p, (const float*)h->mun.p, (const float*)h->cal_mu.p,
-                                  (const int*)h->cal_idx.p, cal_n, -1, nullptr, 0.0, 0.0, fs);
+  calib_kernel<<<1, 1024, 0, s>>>(kbo_view<float>(h->varn), h->var_cal.p, kbo_view<float>(h->mun), h->cal_mu.p,
+                                  h->cal_idx.p, cal_n, -1, nullptr, 0.0, 0.0, fs);
   KBO_LAUNCH_CHECK(h);
-  bound_max_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
+  bound_max_kernel<<<acq_grid(h, M), 256, 0, s>>>(kbo_view<float>(h->mun), kbo_view<float>(h->varn), M, d.acq, scal, h->prm.xi, h->prm.kappa, fs);
   KBO_LAUNCH_CHECK(h);
-  survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>((const float*)h->mun.p, (const float*)h->varn.p, nullptr, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs,
+  survivor_kernel<<<acq_grid(h, M), 256, 0, s>>>(kbo_view<float>(h->mun), kbo_view<float>(h->varn), nullptr, M, d.acq, scal, h->prm.xi, h->prm.kappa, fs,
                                                  list, count);
   KBO_LAUNCH_CHECK(h);
   int n = 0;
@@ -1329,22 +1330,22 @@ static int calibration_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t
   int64_t want = (int64_t)h->sm_count * 64;
   const int cal_n = (int)(M < want ? M : want);
   const int64_t cal_pad = round_up64(cal_n, 128);
-  KBO_TRY(kbo_reserve(h, h->cal_idx, sizeof(int) * (size_t)cal_pad));
-  KBO_TRY(kbo_reserve(h, h->cal_x, sizeof(double) * (size_t)cal_pad * h->D));
-  KBO_TRY(kbo_reserve(h, h->cal_mu, sizeof(float) * (size_t)cal_pad));
-  KBO_TRY(kbo_reserve(h, h->var_cal, sizeof(float) * (size_t)cal_pad));
-  cal_index_kernel<<<(cal_n + 255) / 256, 256, 0, s>>>((int*)h->cal_idx.p, cal_n, M);
+  KBO_TRY(kbo_reserve(h, h->cal_idx, (size_t)cal_pad));
+  KBO_TRY(kbo_reserve(h, h->cal_x, (size_t)cal_pad * h->D));
+  KBO_TRY(kbo_reserve(h, h->cal_mu, (size_t)cal_pad));
+  KBO_TRY(kbo_reserve(h, h->var_cal, (size_t)cal_pad));
+  cal_index_kernel<<<(cal_n + 255) / 256, 256, 0, s>>>(h->cal_idx.p, cal_n, M);
   KBO_LAUNCH_CHECK(h);
   if (xc_dtype == KBO_F64)
-    gather_rows_kernel<double><<<cal_n, 64, 0, s>>>((const double*)Xc, h->D, (const int*)h->cal_idx.p, cal_n, (double*)h->cal_x.p);
+    gather_rows_kernel<double><<<cal_n, 64, 0, s>>>((const double*)Xc, h->D, h->cal_idx.p, cal_n, h->cal_x.p);
   else
-    gather_rows_kernel<float><<<cal_n, 64, 0, s>>>((const float*)Xc, h->D, (const int*)h->cal_idx.p, cal_n, (double*)h->cal_x.p);
+    gather_rows_kernel<float><<<cal_n, 64, 0, s>>>((const float*)Xc, h->D, h->cal_idx.p, cal_n, h->cal_x.p);
   KBO_LAUNCH_CHECK(h);
-  KBO_TRY((launch_cross<double, float, 1>(h, (const double*)h->cal_x.p, cal_n, cal_pad, nullptr, 0, (__half*)h->Ksh.p, (__half*)h->Ksl.p,
-                                          (float*)h->cal_mu.p, s)));
+  KBO_TRY((launch_cross<double, float, 1>(h, h->cal_x.p, cal_n, cal_pad, nullptr, 0, h->Ksh.p, h->Ksl.p,
+                                          h->cal_mu.p, s)));
   // jtiles > 0: the exact variance bound from a PREFIX of the trial tiles (needs the leading rows of W only)
-  KBO_TRY(kbo_i_tc_variance(h, (const __half*)h->Ksh.p, (const __half*)h->Ksl.p, cal_pad, (const __half*)h->Wh.p, (const __half*)h->Wl.p, h->Npad,
-                            0.0, h->prm.amplitude, (float*)h->var_cal.p, h->prm.tc_k_span, s, 3, jtiles));
+  KBO_TRY(kbo_i_tc_variance(h, h->Ksh.p, h->Ksl.p, cal_pad, h->Wh.p, h->Wl.p, h->Npad,
+                            0.0, h->prm.amplitude, h->var_cal.p, h->prm.tc_k_span, s, 3, jtiles));
   *cal_n_out = cal_n;
   return KBO_OK;
 }
@@ -1355,8 +1356,8 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
 int kbo_i_debug_cross_planes(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, cudaStream_t s) {
   const int64_t rows_pad = round_up64(M, 128);
   if (xc_dtype == KBO_F64)
-    return launch_cross<double, float, 1>(h, (const double*)Xc, M, rows_pad, nullptr, 0, (__half*)h->Ksh.p, (__half*)h->Ksl.p, (float*)h->mun.p, s);
-  return launch_cross<float, float, 1>(h, (const float*)Xc, M, rows_pad, nullptr, 0, (__half*)h->Ksh.p, (__half*)h->Ksl.p, (float*)h->mun.p, s);
+    return launch_cross<double, float, 1>(h, (const double*)Xc, M, rows_pad, nullptr, 0, h->Ksh.p, h->Ksl.p, kbo_view<float>(h->mun), s);
+  return launch_cross<float, float, 1>(h, (const float*)Xc, M, rows_pad, nullptr, 0, h->Ksh.p, h->Ksl.p, kbo_view<float>(h->mun), s);
 }
 
 // Test hook: the ranking arithmetic of M rows as the pruning pass (tile_pairs >= 1: the first tile_pairs pairs of trial tiles, only
@@ -1370,13 +1371,14 @@ int kbo_i_debug_rank_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M
   const int P1 = (tile_pairs < 0 || tile_pairs > n_pairs) ? n_pairs : tile_pairs;
   if (!h->w_full && (P1 == n_pairs || P1 * 512 > h->w_lead)) KBO_TRY(kbo_i_ensure_w(h, s));
   const int64_t rows_pad = round_up64(M, 256);
-  KBO_TRY(kbo_reserve(h, h->Ksh, sizeof(__half) * (size_t)rows_pad * Npad));
-  KBO_TRY(kbo_reserve(h, h->mun, sizeof(float) * (size_t)(rows_pad + 256)));
-  KBO_TRY(kbo_reserve(h, h->varn, sizeof(float) * (size_t)(rows_pad + 256)));
-  KBO_TRY(kbo_i_tc_kstar(h, Xc, xc_dtype, M, (__half*)h->Ksh.p, (float*)h->mun.p, s, P1 < n_pairs ? P1 * 512 : -1));
-  KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, rows_pad, (const __half*)h->Wh.p, Npad, h->prm.amplitude, (float*)h->varn.p, s, 0, P1));
-  KBO_CUDA(h, cudaMemcpyAsync(mun_out, h->mun.p, sizeof(float) * (size_t)M, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, cudaMemcpyAsync(varn_out, h->varn.p, sizeof(float) * (size_t)M, cudaMemcpyDeviceToDevice, s));
+  KBO_TRY(kbo_reserve(h, h->Ksh, (size_t)rows_pad * Npad));
+  const size_t bytes = sizeof(float) * (size_t)(rows_pad + 256);
+  KBO_TRY(kbo_reserve(h, h->mun, bytes));
+  KBO_TRY(kbo_reserve(h, h->varn, bytes));
+  KBO_TRY(kbo_i_tc_kstar(h, Xc, xc_dtype, M, h->Ksh.p, kbo_view<float>(h->mun), s, P1 < n_pairs ? P1 * 512 : -1));
+  KBO_TRY(kbo_i_tc_rank(h, h->Ksh.p, rows_pad, h->Wh.p, Npad, h->prm.amplitude, kbo_view<float>(h->varn), s, 0, P1));
+  KBO_CUDA(h, kbo_copy(mun_out, kbo_view<float>(h->mun), M, cudaMemcpyDeviceToDevice, s));
+  KBO_CUDA(h, kbo_copy(varn_out, kbo_view<float>(h->varn), M, cudaMemcpyDeviceToDevice, s));
   return KBO_OK;
 }
 
@@ -1441,7 +1443,7 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
                                  (h->prm.var_mode == KBO_VAR_AUTO && (amp <= 10.0 || !arrays) && h->have_planes &&
                                   (double)M * h->N * h->N > 2e11));
   const size_t esz = xc_dtype == KBO_F64 ? 8 : 4;
-  const double* scal = (const double*)h->scal.p;
+  const double* scal = h->scal.p;
   // array-free tensor-core sweeps rank with one fp16 product and let the FP64 refinement decide (fast_pick above)
   const bool fast = tc && !force_three && h->tc_fast && !mu_out && !std_out && !acq_out && M < 0x7fffffff;
   // ... and, by default, build that pass's K̃* on the tensor cores and contract it with wgmma MMAs (tc_kstar.cu, tc_rank.cu)
@@ -1459,8 +1461,8 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
       int64_t rows_sh = chunk > round_up64(cal_pad, 256) ? chunk : round_up64(cal_pad, 256);
       const int64_t prune_rows = round_up64(M < 16384 ? M : 16384, 256);          // the pruning pass re-runs up to 16384 survivors in one go
       if (rows_sh < prune_rows) rows_sh = prune_rows;
-      KBO_TRY(kbo_reserve(h, h->Ksh, sizeof(__half) * (size_t)rows_sh * Npad));
-      KBO_TRY(kbo_reserve(h, h->Ksl, sizeof(__half) * (size_t)cal_pad * Npad));   // the lo plane exists for the calibration rows only
+      KBO_TRY(kbo_reserve(h, h->Ksh, (size_t)rows_sh * Npad));
+      KBO_TRY(kbo_reserve(h, h->Ksl, (size_t)cal_pad * Npad));   // the lo plane exists for the calibration rows only
     } else {
       // wave-aligned chunks: the variance kernel runs one 128-row CTA per SM, the K* kernel two — a chunk that is a multiple
       // of sm_count·128 rows leaves no partial wave
@@ -1469,19 +1471,21 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
       if (chunk < 128) chunk = 128;
       if (chunk > round_up64(M, 128)) chunk = round_up64(M, 128);
       const int64_t rows_sh = chunk > cal_pad ? chunk : cal_pad;
-      KBO_TRY(kbo_reserve(h, h->Ksh, sizeof(__half) * (size_t)rows_sh * Npad));
-      KBO_TRY(kbo_reserve(h, h->Ksl, sizeof(__half) * (size_t)rows_sh * Npad));
+      KBO_TRY(kbo_reserve(h, h->Ksh, (size_t)rows_sh * Npad));
+      KBO_TRY(kbo_reserve(h, h->Ksl, (size_t)rows_sh * Npad));
     }
-    KBO_TRY(kbo_reserve(h, h->mun, sizeof(float) * (size_t)(round_up64(M, 256) + 256)));
-    KBO_TRY(kbo_reserve(h, h->varn, sizeof(float) * (size_t)(round_up64(M, 256) + 256)));
+    const size_t bytes = sizeof(float) * (size_t)(round_up64(M, 256) + 256);
+    KBO_TRY(kbo_reserve(h, h->mun, bytes));
+    KBO_TRY(kbo_reserve(h, h->varn, bytes));
   } else {
     chunk = (int64_t)(h->scratch_limit / ((size_t)ld * 8)) / 64 * 64;
     if (chunk < 64) chunk = 64;
     if (chunk > round_up64(M, 64)) chunk = round_up64(M, 64);
-    KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)chunk * ld));
-    KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * (size_t)chunk * ((N + 63) / 64)));
-    KBO_TRY(kbo_reserve(h, h->mun, sizeof(double) * (size_t)M));
-    KBO_TRY(kbo_reserve(h, h->varn, sizeof(double) * (size_t)M));
+    KBO_TRY(kbo_reserve(h, h->Ks64, (size_t)chunk * ld));
+    KBO_TRY(kbo_reserve(h, h->part, (size_t)chunk * ((N + 63) / 64)));
+    const size_t bytes = sizeof(double) * (size_t)M;
+    KBO_TRY(kbo_reserve(h, h->mun, bytes));
+    KBO_TRY(kbo_reserve(h, h->varn, bytes));
   }
   h->tim.chunks = 0;
   auto all_done = [&]() {
@@ -1517,50 +1521,50 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
     if (rank_tc) {
       {
         KBO_TIME_BEGIN(ev_cross, ev_cross_used);
-        KBO_TRY(kbo_i_tc_kstar(h, xc, xc_dtype, rows, (__half*)h->Ksh.p, (float*)h->mun.p + c0, s));
+        KBO_TRY(kbo_i_tc_kstar(h, xc, xc_dtype, rows, h->Ksh.p, kbo_view<float>(h->mun) + c0, s));
         KBO_TIME_END();
       }
       {
         KBO_TIME_BEGIN(ev_var, ev_var_used);
-        KBO_TRY(kbo_i_tc_rank(h, (const __half*)h->Ksh.p, round_up64(rows, 256), (const __half*)h->Wh.p, Npad, h->prm.amplitude,
-                              (float*)h->varn.p + c0, s));
+        KBO_TRY(kbo_i_tc_rank(h, h->Ksh.p, round_up64(rows, 256), h->Wh.p, Npad, h->prm.amplitude,
+                              kbo_view<float>(h->varn) + c0, s));
         KBO_TIME_END();
       }
     } else if (tc) {
       const int64_t rows_pad = round_up64(rows, 128);
-      float* mun = (float*)h->mun.p + c0;
+      float* mun = kbo_view<float>(h->mun) + c0;
       {
         KBO_TIME_BEGIN(ev_cross, ev_cross_used);
         if (xc_dtype == KBO_F64)
-          KBO_TRY((launch_cross<double, float, 1>(h, (const double*)xc, rows, rows_pad, nullptr, 0, (__half*)h->Ksh.p, (__half*)h->Ksl.p, mun, s)));
+          KBO_TRY((launch_cross<double, float, 1>(h, (const double*)xc, rows, rows_pad, nullptr, 0, h->Ksh.p, h->Ksl.p, mun, s)));
         else
-          KBO_TRY((launch_cross<float, float, 1>(h, (const float*)xc, rows, rows_pad, nullptr, 0, (__half*)h->Ksh.p, (__half*)h->Ksl.p, mun, s)));
+          KBO_TRY((launch_cross<float, float, 1>(h, (const float*)xc, rows, rows_pad, nullptr, 0, h->Ksh.p, h->Ksl.p, mun, s)));
         KBO_TIME_END();
       }
       {
         KBO_TIME_BEGIN(ev_var, ev_var_used);
-        KBO_TRY(kbo_i_tc_variance(h, (const __half*)h->Ksh.p, (const __half*)h->Ksl.p, rows_pad, (const __half*)h->Wh.p, (const __half*)h->Wl.p,
-                                  Npad, 0.0, h->prm.amplitude, (float*)h->varn.p + c0, fast ? 1024 : h->prm.tc_k_span, s, fast ? 1 : 3));
+        KBO_TRY(kbo_i_tc_variance(h, h->Ksh.p, h->Ksl.p, rows_pad, h->Wh.p, h->Wl.p,
+                                  Npad, 0.0, h->prm.amplitude, kbo_view<float>(h->varn) + c0, fast ? 1024 : h->prm.tc_k_span, s, fast ? 1 : 3));
         KBO_TIME_END();
       }
     } else {
-      double* mun = (double*)h->mun.p + c0;
+      double* mun = kbo_view<double>(h->mun) + c0;
       {
         KBO_TIME_BEGIN(ev_cross, ev_cross_used);
         if (xc_dtype == KBO_F64)
-          KBO_TRY((launch_cross<double, double, 0>(h, (const double*)xc, rows, rows, (double*)h->Ks64.p, ld, nullptr, nullptr, mun, s)));
+          KBO_TRY((launch_cross<double, double, 0>(h, (const double*)xc, rows, rows, h->Ks64.p, ld, nullptr, nullptr, mun, s)));
         else
-          KBO_TRY((launch_cross<float, double, 0>(h, (const float*)xc, rows, rows, (double*)h->Ks64.p, ld, nullptr, nullptr, mun, s)));
+          KBO_TRY((launch_cross<float, double, 0>(h, (const float*)xc, rows, rows, h->Ks64.p, ld, nullptr, nullptr, mun, s)));
         KBO_TIME_END();
       }
       {
         KBO_TIME_BEGIN(ev_var, ev_var_used);
         const int njt = (N + 63) / 64;
-        dgemm64_launch<true, EPI_ROWSUMSQ>(s, (int)rows, N, N, (const double*)h->Ks64.p, ld, (const double*)h->W.p, ld, (double*)h->part.p, njt,
+        dgemm64_launch<true, EPI_ROWSUMSQ>(s, (int)rows, N, N, h->Ks64.p, ld, h->W.p, ld, h->part.p, njt,
                                            1.0, 0.0, KM_UPTO_N, 0, TS_NONE);
         KBO_LAUNCH_CHECK(h);
-        var_from_parts_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>((const double*)h->part.p, rows, njt, h->prm.amplitude,
-                                                                            (double*)h->varn.p + c0);
+        var_from_parts_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>(h->part.p, rows, njt, h->prm.amplitude,
+                                                                            kbo_view<double>(h->varn) + c0);
         KBO_LAUNCH_CHECK(h);
         KBO_TIME_END();
       }
@@ -1584,7 +1588,7 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
       AcqDecision& d = dec[k];
       if (d.done) continue;
       if (tc) {
-        KBO_TRY(launch_acq<float>(h, (const float*)h->mun.p, (const float*)h->varn.p, M, goff, d.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
+        KBO_TRY(launch_acq<float>(h, kbo_view<float>(h->mun), kbo_view<float>(h->varn), M, goff, d.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
                                   h->prm.kappa, mu_out, std_out, acq_out, nullptr, d.best, s));
         d.unrefined = 2;
         if (M < 0x7fffffff)
@@ -1593,7 +1597,7 @@ static int sweep_impl(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, in
           d.done = true;
       } else {
         d.unrefined = 0;
-        KBO_TRY(launch_acq<double>(h, (const double*)h->mun.p, (const double*)h->varn.p, M, goff, d.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
+        KBO_TRY(launch_acq<double>(h, kbo_view<double>(h->mun), kbo_view<double>(h->varn), M, goff, d.acq, 0.0, 1.0, 0.0, scal, h->prm.xi,
                                    h->prm.kappa, mu_out, std_out, acq_out, nullptr, d.best, s));
         d.done = true;
       }
@@ -1623,11 +1627,11 @@ int kbo_i_predict_mean(kbo_handle* h, const void* X, int x_dtype, int n, double*
   if (h->D > 256) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_predict_mean: D <= 256 supported (got %d)", h->D);
   const int N = h->N, D = h->D, ld = h->ld;
   const int B = n < 1024 ? n : 1024;   // rows per batch: K* scratch of B × ld doubles
-  KBO_TRY(kbo_reserve(h, h->refine_x, sizeof(double) * (size_t)B * D));
-  KBO_TRY(kbo_reserve(h, h->Ks64, sizeof(double) * (size_t)B * ld));
-  KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * 2 * (size_t)B));
-  double* Xg = (double*)h->refine_x.p;
-  double* mun = (double*)h->part.p;
+  KBO_TRY(kbo_reserve(h, h->refine_x, (size_t)B * D));
+  KBO_TRY(kbo_reserve(h, h->Ks64, (size_t)B * ld));
+  KBO_TRY(kbo_reserve(h, h->part, (size_t)B * 2));
+  double* Xg = h->refine_x.p;
+  double* mun = h->part.p;
   double* mu = mun + B;
   const size_t esz = x_dtype == KBO_F64 ? 8 : 4;
   for (int r0 = 0; r0 < n; r0 += B) {
@@ -1639,18 +1643,18 @@ int kbo_i_predict_mean(kbo_handle* h, const void* X, int x_dtype, int n, double*
     else
       rows_to_f64_kernel<float><<<g, 256, 0, s>>>((const float*)x, m, D, Xg);
     KBO_LAUNCH_CHECK(h);
-    refine_cross_kernel<<<dim3((N + 255) / 256, m), 256, 0, s>>>(Xg, D, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(), (const double*)h->XsT.p, ld, N,
-                                                                 h->prm.kernel, h->prm.amplitude, (double*)h->Ks64.p);
+    refine_cross_kernel<<<dim3((N + 255) / 256, m), 256, 0, s>>>(Xg, D, h->d_inv_ls.p, (int)h->inv_ls.size(), h->XsT.p, ld, N,
+                                                                 h->prm.kernel, h->prm.amplitude, h->Ks64.p);
     KBO_LAUNCH_CHECK(h);
-    refine_mu_kernel<<<m, 256, 0, s>>>((const double*)h->Ks64.p, ld, N, (const double*)h->alpha.p, mun);
+    refine_mu_kernel<<<m, 256, 0, s>>>(h->Ks64.p, ld, N, h->alpha.p, mun);
     KBO_LAUNCH_CHECK(h);
-    raw_mean_kernel<<<(m + 255) / 256, 256, 0, s>>>(mun, m, (const double*)h->scal.p, mu);
+    raw_mean_kernel<<<(m + 255) / 256, 256, 0, s>>>(mun, m, h->scal.p, mu);
     KBO_LAUNCH_CHECK(h);
     KBO_CUDA(h, cudaMemcpyAsync(mu_host + r0, mu, sizeof(double) * (size_t)m, cudaMemcpyDeviceToHost, s));
     KBO_CUDA(h, cudaStreamSynchronize(s));
   }
   int inf = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(&inf, h->info.p, sizeof(int), cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&inf, h->info.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (inf != 0) KBO_FAIL(h, KBO_ERR_NOT_PD, "kernel matrix is not positive definite (pivot %d); increase `noise`", inf);
   return KBO_OK;

@@ -297,17 +297,17 @@ int kbo_i_tc_trials_prep(kbo_handle* h, bool new_center, cudaStream_t s) {
   const int N = h->N, D = h->D, Dp = round_up(D, KS_BK), Np = round_up(N, KS_BN);
   h->ks_ready = false;
   if (D > KS_MAX_SLABS * KS_BK) return KBO_OK;   // the FP64 K* kernel serves wider spaces
-  KBO_TRY(kbo_reserve(h, h->ks_center, sizeof(double) * 512));
-  KBO_TRY(kbo_reserve(h, h->ks_Xh, sizeof(__half) * (size_t)Np * Dp));
-  KBO_TRY(kbo_reserve(h, h->ks_Xl, sizeof(__half) * (size_t)Np * Dp));
-  KBO_TRY(kbo_reserve(h, h->ks_nxal, sizeof(float) * 2 * (size_t)Np));
+  KBO_TRY(kbo_reserve(h, h->ks_center, 512));
+  KBO_TRY(kbo_reserve(h, h->ks_Xh, (size_t)Np * Dp));
+  KBO_TRY(kbo_reserve(h, h->ks_Xl, (size_t)Np * Dp));
+  KBO_TRY(kbo_reserve(h, h->ks_nxal, (size_t)Np * 2));
   if (new_center) {
-    ks_center_kernel<<<D, 256, 0, s>>>((const double*)h->XsT.p, h->ld, N, (double*)h->ks_center.p);
+    ks_center_kernel<<<D, 256, 0, s>>>(h->XsT.p, h->ld, N, h->ks_center.p);
     KBO_LAUNCH_CHECK(h);
   }
-  ks_split_rows_kernel<double, true><<<(unsigned)((Np + 7) / 8), 256, 0, s>>>((const double*)h->Xs.p, N, Np, D, Dp, nullptr, 1, (const double*)h->ks_center.p,
-                                                                          ks_kscale(h->prm.kernel), (__half*)h->ks_Xh.p, (__half*)h->ks_Xl.p,
-                                                                          (float*)h->ks_nxal.p, 2, (const double*)h->alpha.p);
+  ks_split_rows_kernel<double, true><<<(unsigned)((Np + 7) / 8), 256, 0, s>>>(h->Xs.p, N, Np, D, Dp, nullptr, 1, h->ks_center.p,
+                                                                          ks_kscale(h->prm.kernel), h->ks_Xh.p, h->ks_Xl.p,
+                                                                          h->ks_nxal.p, 2, h->alpha.p);
   KBO_LAUNCH_CHECK(h);
   h->ks_ready = true;
   return KBO_OK;
@@ -319,18 +319,18 @@ int kbo_i_tc_kstar(kbo_handle* h, const void* Xc, int xc_dtype, int64_t rows, __
   const int N = h->N, D = h->D, Dp = round_up(D, KS_BK), Np = round_up(N, KS_BN), ns = Dp / KS_BK;
   const int64_t rows_pad = round_up64(rows, 256);
   if (h->Npad % KS_BN != 0 || h->Npad < Np) KBO_FAIL(h, KBO_ERR_STATE, "tc_kstar: Npad %d does not cover N %d", h->Npad, N);
-  KBO_TRY(kbo_reserve(h, h->ks_Ch, sizeof(__half) * (size_t)rows_pad * Dp));
-  KBO_TRY(kbo_reserve(h, h->ks_Cl, sizeof(__half) * (size_t)rows_pad * Dp));
-  KBO_TRY(kbo_reserve(h, h->ks_nc, sizeof(float) * (size_t)rows_pad));
+  KBO_TRY(kbo_reserve(h, h->ks_Ch, (size_t)rows_pad * Dp));
+  KBO_TRY(kbo_reserve(h, h->ks_Cl, (size_t)rows_pad * Dp));
+  KBO_TRY(kbo_reserve(h, h->ks_nc, (size_t)rows_pad));
   const unsigned g = (unsigned)((rows_pad + 7) / 8);
   if (xc_dtype == KBO_F64)
-    ks_split_rows_kernel<double, false><<<g, 256, 0, s>>>((const double*)Xc, rows, rows_pad, D, Dp, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(),
-                                                         (const double*)h->ks_center.p, ks_kscale(h->prm.kernel), (__half*)h->ks_Ch.p, (__half*)h->ks_Cl.p,
-                                                         (float*)h->ks_nc.p, 1, nullptr);
+    ks_split_rows_kernel<double, false><<<g, 256, 0, s>>>((const double*)Xc, rows, rows_pad, D, Dp, h->d_inv_ls.p, (int)h->inv_ls.size(),
+                                                         h->ks_center.p, ks_kscale(h->prm.kernel), h->ks_Ch.p, h->ks_Cl.p,
+                                                         h->ks_nc.p, 1, nullptr);
   else
-    ks_split_rows_kernel<float, false><<<g, 256, 0, s>>>((const float*)Xc, rows, rows_pad, D, Dp, (const double*)h->d_inv_ls.p, (int)h->inv_ls.size(),
-                                                        (const double*)h->ks_center.p, ks_kscale(h->prm.kernel), (__half*)h->ks_Ch.p, (__half*)h->ks_Cl.p,
-                                                        (float*)h->ks_nc.p, 1, nullptr);
+    ks_split_rows_kernel<float, false><<<g, 256, 0, s>>>((const float*)Xc, rows, rows_pad, D, Dp, h->d_inv_ls.p, (int)h->inv_ls.size(),
+                                                        h->ks_center.p, ks_kscale(h->prm.kernel), h->ks_Ch.p, h->ks_Cl.p,
+                                                        h->ks_nc.p, 1, nullptr);
   KBO_LAUNCH_CHECK(h);
   CUtensorMap tmCh, tmCl, tmXh, tmXl;
   KBO_TRY(kbo_i_encode_map_f16(h, &tmCh, h->ks_Ch.p, (uint64_t)Dp, (uint64_t)rows_pad, KS_BK, KS_BM));
@@ -341,14 +341,16 @@ int kbo_i_tc_kstar(kbo_handle* h, const void* Xc, int xc_dtype, int64_t rows, __
   const float log2amp = (float)log2(h->prm.amplitude);
   const int ntiles = h->Npad / KS_BN;   // tiles past Np read out-of-bounds trial rows (TMA zero fill) and are masked to 0
   const int store_tiles = (store_cols < 0 || store_cols >= h->Npad) ? ntiles : (store_cols + KS_BN - 1) / KS_BN;
+  // two trials' (|x̂|², alpha) pairs per float4: device allocations are 256-byte aligned, so each group of four floats is 16-byte aligned
+  const float4* nxal = reinterpret_cast<const float4*>(h->ks_nxal.p);
   if (h->prm.kernel == KBO_KERNEL_RBF) {
     KBO_CUDA(h, cudaFuncSetAttribute(tc_kstar_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_kstar_kernel<0><<<(unsigned)(rows_pad / KS_BM), KS_THREADS, smem, s>>>(tmCh, tmCl, tmXh, tmXl, ns, ntiles, N, (const float*)h->ks_nc.p,
-                                                                            (const float4*)h->ks_nxal.p, Np / KS_BN, log2amp, Ksh, h->Npad, mun, store_tiles);
+    tc_kstar_kernel<0><<<(unsigned)(rows_pad / KS_BM), KS_THREADS, smem, s>>>(tmCh, tmCl, tmXh, tmXl, ns, ntiles, N, h->ks_nc.p,
+                                                                            nxal, Np / KS_BN, log2amp, Ksh, h->Npad, mun, store_tiles);
   } else {
     KBO_CUDA(h, cudaFuncSetAttribute(tc_kstar_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    tc_kstar_kernel<1><<<(unsigned)(rows_pad / KS_BM), KS_THREADS, smem, s>>>(tmCh, tmCl, tmXh, tmXl, ns, ntiles, N, (const float*)h->ks_nc.p,
-                                                                            (const float4*)h->ks_nxal.p, Np / KS_BN, log2amp, Ksh, h->Npad, mun, store_tiles);
+    tc_kstar_kernel<1><<<(unsigned)(rows_pad / KS_BM), KS_THREADS, smem, s>>>(tmCh, tmCl, tmXh, tmXl, ns, ntiles, N, h->ks_nc.p,
+                                                                            nxal, Np / KS_BN, log2amp, Ksh, h->Npad, mun, store_tiles);
   }
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;

@@ -156,7 +156,7 @@ __global__ void rank_finish_kernel(const float* __restrict__ part, int p_begin, 
 int rk_schedule(kbo_handle* h, int n_rg, int n_jtiles, int ctas, int p_begin, int p_end, const int** sched_dev, cudaStream_t s) {
   for (auto& e : h->rk_sched)
     if (e.key[0] == n_rg && e.key[1] == n_jtiles && e.key[2] == ctas && e.key[3] == p_begin && e.key[4] == p_end) {
-      *sched_dev = (const int*)e.dev.p;
+      *sched_dev = e.dev.p;
       return KBO_OK;
     }
   kbo_handle::RkSched& e = h->rk_sched[h->rk_sched_next];
@@ -181,15 +181,15 @@ int rk_schedule(kbo_handle* h, int n_rg, int n_jtiles, int ctas, int p_begin, in
   }
   e.host[ctas] = off;
   for (int c = 0; c < ctas; c++) e.host.insert(e.host.end(), lists[c].begin(), lists[c].end());
-  KBO_TRY(kbo_reserve(h, e.dev, sizeof(int) * e.host.size()));
+  KBO_TRY(kbo_reserve(h, e.dev, e.host.size()));
   // pageable source: the runtime stages it before returning, and earlier launches reading this buffer precede the copy on s
-  KBO_CUDA(h, cudaMemcpyAsync(e.dev.p, e.host.data(), sizeof(int) * e.host.size(), cudaMemcpyHostToDevice, s));
+  KBO_CUDA(h, kbo_copy(e.dev.p, e.host.data(), e.host.size(), cudaMemcpyHostToDevice, s));
   e.key[0] = n_rg;
   e.key[1] = n_jtiles;
   e.key[2] = ctas;
   e.key[3] = p_begin;
   e.key[4] = p_end;
-  *sched_dev = (const int*)e.dev.p;
+  *sched_dev = e.dev.p;
   return KBO_OK;
 }
 
@@ -213,14 +213,14 @@ int kbo_i_tc_rank(kbo_handle* h, const __half* Ksh, int64_t rows, const __half* 
   if (p_end < 0 || p_end > n_pairs) p_end = n_pairs;
   if (p_begin < 0 || p_begin >= p_end) KBO_FAIL(h, KBO_ERR_INVALID, "tc_rank: empty tile-pair range [%d, %d)", p_begin, p_end);
   if (n_pairs > 256 || n_rg >= (1 << 23)) KBO_FAIL(h, KBO_ERR_INVALID, "tc_rank: problem too large for the item encoding (Npad %d, rows %lld)", Npad, (long long)rows);
-  KBO_TRY(kbo_reserve(h, h->rk_part, sizeof(float) * (size_t)n_pairs * rows));
+  KBO_TRY(kbo_reserve(h, h->rk_part, (size_t)n_pairs * rows));
   int ctas = h->sm_count;
   if ((int64_t)ctas > n_rg * (p_end - p_begin)) ctas = (int)(n_rg * (p_end - p_begin));
   const int* sched = nullptr;
   KBO_TRY(rk_schedule(h, (int)n_rg, n_jtiles, ctas, p_begin, p_end, &sched, s));
-  tc_rank_kernel<<<(unsigned)ctas, RK_THREADS, RK_SMEM_BYTES, s>>>(tmA, tmW, n_jtiles, sched, (float*)h->rk_part.p, rows);
+  tc_rank_kernel<<<(unsigned)ctas, RK_THREADS, RK_SMEM_BYTES, s>>>(tmA, tmW, n_jtiles, sched, h->rk_part.p, rows);
   KBO_LAUNCH_CHECK(h);
-  rank_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>((const float*)h->rk_part.p, p_begin, p_end, rows, (const double*)h->scal.p + 6, amp, var_n_out);
+  rank_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>(h->rk_part.p, p_begin, p_end, rows, h->scal.p + S_WSCALE, amp, var_n_out);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }

@@ -226,7 +226,7 @@ int tc_launch(kbo_handle* h, const __half* Ksh, const __half* Ksl, int64_t rows,
     h->attr_tc = true;
   }
   // a 2-CTA cluster per 128-row panel: each K* chunk is read once for both CTAs (half the K* panel re-reads)
-  KBO_TRY(kbo_reserve(h, h->part, sizeof(double) * 2 * (size_t)rows));
+  KBO_TRY(kbo_reserve(h, h->part, (size_t)rows * 2));
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -239,9 +239,9 @@ int tc_launch(kbo_handle* h, const __half* Ksh, const __half* Ksl, int64_t rows,
   cfg.stream = s;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  KBO_CUDA(h, cudaLaunchKernelEx(&cfg, tc_variance_kernel, tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, nprod, (double*)h->part.p, rows));
+  KBO_CUDA(h, cudaLaunchKernelEx(&cfg, tc_variance_kernel, tmAh, tmAl, tmBh, tmBl, n_jt, span_chunks, nprod, h->part.p, rows));
   KBO_LAUNCH_CHECK(h);
-  tc_variance_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>((const double*)h->part.p, rows, w_scale_dev, amp, var_out, sumsq_out);
+  tc_variance_finish_kernel<<<(unsigned)((rows + 255) / 256), 256, 0, s>>>(h->part.p, rows, w_scale_dev, amp, var_out, sumsq_out);
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }
@@ -274,7 +274,7 @@ int kbo_i_encode_map_f16(kbo_handle* h, CUtensorMap* out, const void* base, uint
 
 int kbo_i_tc_variance(kbo_handle* h, const __half* Ksh, const __half* Ksl, int64_t rows, const __half* Wh, const __half* Wl, int Npad,
                       double /*unused*/, double amp, float* var_n_out, int k_span, cudaStream_t s, int nprod, int jtiles) {
-  return tc_launch(h, Ksh, Ksl, rows, Wh, Wl, Npad, (const double*)h->scal.p + 6, amp, var_n_out, nullptr, k_span, s, nprod, jtiles);
+  return tc_launch(h, Ksh, Ksl, rows, Wh, Wl, Npad, h->scal.p + S_WSCALE, amp, var_n_out, nullptr, k_span, s, nprod, jtiles);
 }
 
 // Raw entry for the kernel-level parity test: caller supplies fp16 planes and the scale pair on the device.

@@ -61,11 +61,20 @@ struct kbo_tpe {
   uint64_t seed = 0;
   uint32_t asks = 0;
   int n = 0, cap = 0, built_n = -1, nb = 0, ms = 0;
-  DevBuf d_prm, d_cont, d_disc, d_num, d_cat;
-  DevBuf vals, loss;
-  DevBuf lkey, lkey2, lidx, lidx2, below, grp, pos, skey, skey2, sval, sval2, segb, sege, tmp;
-  DevBuf w, mu, sg, lc, f4, cdf, hdr, cat_p, cat_sc, cat_cum;
-  DevBuf draws, sc, lb, surv, bb, first, err;
+  DevBuf<TpeParam> d_prm;
+  DevBuf<int> d_cont, d_disc, d_num, d_cat;
+  DevBuf<double> vals, loss;
+  DevBuf<uint64_t> lkey, lkey2, skey, skey2;
+  DevBuf<int> lidx, lidx2, below, grp, pos, sval, sval2, segb, sege;
+  DevBuf<unsigned char> tmp;
+  DevBuf<double> w, mu, sg, lc, cdf, cat_p, cat_sc, cat_cum;
+  DevBuf<float4> f4;
+  DevBuf<TpeHdr> hdr;
+  DevBuf<double> draws;
+  DevBuf<float2> sc;
+  DevBuf<unsigned> lb, first;
+  DevBuf<int> surv, err;
+  DevBuf<TpeBest> bb;
   std::vector<int> last_surv;
   EventSet<6> ev;
   float last_ms[5] = {};
@@ -525,16 +534,16 @@ __global__ void __launch_bounds__(256) tpe_final_kernel(TpeModels md, int D, int
 // ------------------------------------------------------------------------------------------------ host side
 static TpeModels tpe_models(kbo_tpe* t) {
   TpeModels md;
-  md.prm = (const TpeParam*)t->d_prm.p;
-  md.w = (const double*)t->w.p;
-  md.mu = (const double*)t->mu.p;
-  md.sg = (const double*)t->sg.p;
-  md.lc = (const double*)t->lc.p;
-  md.cdf = (const double*)t->cdf.p;
-  md.f4 = (const float4*)t->f4.p;
-  md.hdr = (const TpeHdr*)t->hdr.p;
-  md.cat_sc = (const double*)t->cat_sc.p;
-  md.cat_cum = (const double*)t->cat_cum.p;
+  md.prm = t->d_prm.p;
+  md.w = t->w.p;
+  md.mu = t->mu.p;
+  md.sg = t->sg.p;
+  md.lc = t->lc.p;
+  md.cdf = t->cdf.p;
+  md.f4 = t->f4.p;
+  md.hdr = t->hdr.p;
+  md.cat_sc = t->cat_sc.p;
+  md.cat_cum = t->cat_cum.p;
   md.ms = t->ms;
   md.lcat = t->lcat;
   return md;
@@ -546,31 +555,31 @@ static int tpe_build(kbo_handle* h, kbo_tpe* t, cudaStream_t s) {
   const int nb = t->nb, nn = std::max(n, 1);
   t->ms = TPE_CB + round_up(n + 1, 32);
   const size_t slots = (size_t)std::max(t->Dnum, 1) * t->ms;
-  KBO_TRY(kbo_reserve(h, t->w, 8 * slots));
-  KBO_TRY(kbo_reserve(h, t->mu, 8 * slots));
-  KBO_TRY(kbo_reserve(h, t->sg, 8 * slots));
-  KBO_TRY(kbo_reserve(h, t->lc, 8 * slots));
-  KBO_TRY(kbo_reserve(h, t->cdf, 8 * slots));
-  KBO_TRY(kbo_reserve(h, t->f4, 16 * slots));
-  KBO_TRY(kbo_reserve(h, t->hdr, sizeof(TpeHdr) * 2 * std::max(t->Dnum, 1)));
-  KBO_TRY(kbo_reserve(h, t->cat_p, 8 * 2 * (size_t)std::max(t->Dcat, 1) * t->lcat));
-  KBO_TRY(kbo_reserve(h, t->cat_sc, 8 * (size_t)std::max(t->Dcat, 1) * t->lcat));
-  KBO_TRY(kbo_reserve(h, t->cat_cum, 8 * (size_t)std::max(t->Dcat, 1) * t->lcat));
-  KBO_TRY(kbo_reserve(h, t->grp, 4 * (size_t)nn));
-  KBO_TRY(kbo_reserve(h, t->pos, 4 * (size_t)nn));
+  KBO_TRY(kbo_reserve(h, t->w, slots));
+  KBO_TRY(kbo_reserve(h, t->mu, slots));
+  KBO_TRY(kbo_reserve(h, t->sg, slots));
+  KBO_TRY(kbo_reserve(h, t->lc, slots));
+  KBO_TRY(kbo_reserve(h, t->cdf, slots));
+  KBO_TRY(kbo_reserve(h, t->f4, slots));
+  KBO_TRY(kbo_reserve(h, t->hdr, std::max(t->Dnum, 1) * 2));
+  KBO_TRY(kbo_reserve(h, t->cat_p, (size_t)std::max(t->Dcat, 1) * t->lcat * 2));
+  KBO_TRY(kbo_reserve(h, t->cat_sc, (size_t)std::max(t->Dcat, 1) * t->lcat));
+  KBO_TRY(kbo_reserve(h, t->cat_cum, (size_t)std::max(t->Dcat, 1) * t->lcat));
+  KBO_TRY(kbo_reserve(h, t->grp, (size_t)nn));
+  KBO_TRY(kbo_reserve(h, t->pos, (size_t)nn));
   const size_t ns = (size_t)std::max(t->Dnum, 1) * nn;
-  KBO_TRY(kbo_reserve(h, t->skey, 8 * ns));
-  KBO_TRY(kbo_reserve(h, t->skey2, 8 * ns));
-  KBO_TRY(kbo_reserve(h, t->sval, 4 * ns));
-  KBO_TRY(kbo_reserve(h, t->sval2, 4 * ns));
+  KBO_TRY(kbo_reserve(h, t->skey, ns));
+  KBO_TRY(kbo_reserve(h, t->skey2, ns));
+  KBO_TRY(kbo_reserve(h, t->sval, ns));
+  KBO_TRY(kbo_reserve(h, t->sval2, ns));
   if (n > 0) {
-    KBO_TRY(kbo_reserve(h, t->lkey, 8 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->lkey2, 8 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->lidx, 4 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->lidx2, 4 * (size_t)n));
-    KBO_TRY(kbo_reserve(h, t->below, 4 * TPE_LF));
-    KBO_TRY(kbo_reserve(h, t->segb, 4 * 2 * (size_t)std::max(t->Dnum, 1)));
-    KBO_TRY(kbo_reserve(h, t->sege, 4 * 2 * (size_t)std::max(t->Dnum, 1)));
+    KBO_TRY(kbo_reserve(h, t->lkey, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->lkey2, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->lidx, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->lidx2, (size_t)n));
+    KBO_TRY(kbo_reserve(h, t->below, TPE_LF));
+    KBO_TRY(kbo_reserve(h, t->segb, (size_t)std::max(t->Dnum, 1) * 2));
+    KBO_TRY(kbo_reserve(h, t->sege, (size_t)std::max(t->Dnum, 1) * 2));
     size_t b1 = 0, b2 = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, b1, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int*)nullptr, (int*)nullptr, n, 0, 64, s);
     if (t->Dnum)
@@ -578,14 +587,14 @@ static int tpe_build(kbo_handle* h, kbo_tpe* t, cudaStream_t s) {
                                                 t->Dnum * n, 2 * t->Dnum, (const int*)nullptr, (const int*)nullptr, s);
     KBO_TRY(kbo_reserve(h, t->tmp, std::max<size_t>(std::max(b1, b2), 16)));
     // the stable loss order (NumPy's argsort(kind='mergesort'), NaN last)
-    tpe_loss_keys_kernel<<<(n + 255) / 256, 256, 0, s>>>((const double*)t->loss.p, n, (uint64_t*)t->lkey.p, (int*)t->lidx.p);
+    tpe_loss_keys_kernel<<<(n + 255) / 256, 256, 0, s>>>(t->loss.p, n, t->lkey.p, t->lidx.p);
     KBO_LAUNCH_CHECK(h);
     size_t bytes = t->tmp.cap;
-    KBO_CUDA(h, cub::DeviceRadixSort::SortPairs(t->tmp.p, bytes, (const uint64_t*)t->lkey.p, (uint64_t*)t->lkey2.p, (const int*)t->lidx.p,
-                                               (int*)t->lidx2.p, n, 0, 64, s));
-    tpe_split_kernel<<<1, 32, 0, s>>>((const int*)t->lidx2.p, nb, (int*)t->below.p);
+    KBO_CUDA(h, cub::DeviceRadixSort::SortPairs(t->tmp.p, bytes, t->lkey.p, t->lkey2.p, t->lidx.p,
+                                               t->lidx2.p, n, 0, 64, s));
+    tpe_split_kernel<<<1, 32, 0, s>>>(t->lidx2.p, nb, t->below.p);
     KBO_LAUNCH_CHECK(h);
-    tpe_group_kernel<<<(n + 255) / 256, 256, 0, s>>>((const int*)t->below.p, nb, n, (int*)t->grp.p, (int*)t->pos.p);
+    tpe_group_kernel<<<(n + 255) / 256, 256, 0, s>>>(t->below.p, nb, n, t->grp.p, t->pos.p);
     KBO_LAUNCH_CHECK(h);
     if (t->Dnum) {
       std::vector<int> sb(2 * t->Dnum), se(2 * t->Dnum);
@@ -595,29 +604,29 @@ static int tpe_build(kbo_handle* h, kbo_tpe* t, cudaStream_t s) {
         sb[2 * j + 1] = j * n + nb;
         se[2 * j + 1] = (j + 1) * n;
       }
-      KBO_CUDA(h, cudaMemcpyAsync(t->segb.p, sb.data(), 4 * sb.size(), cudaMemcpyHostToDevice, s));
-      KBO_CUDA(h, cudaMemcpyAsync(t->sege.p, se.data(), 4 * se.size(), cudaMemcpyHostToDevice, s));
-      tpe_seg_fill_kernel<<<dim3((n + 255) / 256, t->Dnum), 256, 0, s>>>((const double*)t->vals.p, n, nb, D, (const int*)t->d_num.p,
-                                                                        (const int*)t->grp.p, (const int*)t->pos.p, (uint64_t*)t->skey2.p,
-                                                                        (int*)t->sval2.p);
+      KBO_CUDA(h, kbo_copy(t->segb.p, sb.data(), sb.size(), cudaMemcpyHostToDevice, s));
+      KBO_CUDA(h, kbo_copy(t->sege.p, se.data(), se.size(), cudaMemcpyHostToDevice, s));
+      tpe_seg_fill_kernel<<<dim3((n + 255) / 256, t->Dnum), 256, 0, s>>>(t->vals.p, n, nb, D, t->d_num.p,
+                                                                        t->grp.p, t->pos.p, t->skey2.p,
+                                                                        t->sval2.p);
       KBO_LAUNCH_CHECK(h);
       bytes = t->tmp.cap;
-      KBO_CUDA(h, cub::DeviceSegmentedSort::StableSortPairs(t->tmp.p, bytes, (const uint64_t*)t->skey2.p, (uint64_t*)t->skey.p,
-                                                            (const int*)t->sval2.p, (int*)t->sval.p, t->Dnum * n, 2 * t->Dnum,
-                                                            (const int*)t->segb.p, (const int*)t->sege.p, s));
+      const int *segb = t->segb.p, *sege = t->sege.p;   // the offset types the size query above was made with
+      KBO_CUDA(h, cub::DeviceSegmentedSort::StableSortPairs(t->tmp.p, bytes, t->skey2.p, t->skey.p,
+                                                            t->sval2.p, t->sval.p, t->Dnum * n, 2 * t->Dnum, segb, sege, s));
       // the host vectors above must outlive the copies (pageable memory: staged before cudaMemcpyAsync returns)
     }
   }
   if (t->Dnum) {
-    tpe_model_kernel<<<dim3(t->Dnum, 2), 256, 0, s>>>((const TpeParam*)t->d_prm.p, (const int*)t->d_num.p, n, nb, (const uint64_t*)t->skey.p,
-                                                      (const int*)t->sval.p, t->ms, t->pw, (double*)t->w.p, (double*)t->mu.p, (double*)t->sg.p,
-                                                      (double*)t->lc.p, (float4*)t->f4.p, (double*)t->cdf.p, (TpeHdr*)t->hdr.p);
+    tpe_model_kernel<<<dim3(t->Dnum, 2), 256, 0, s>>>(t->d_prm.p, t->d_num.p, n, nb, t->skey.p,
+                                                      t->sval.p, t->ms, t->pw, t->w.p, t->mu.p, t->sg.p,
+                                                      t->lc.p, t->f4.p, t->cdf.p, t->hdr.p);
     KBO_LAUNCH_CHECK(h);
   }
   if (t->Dcat) {
-    tpe_cat_kernel<<<t->Dcat, 256, 0, s>>>((const TpeParam*)t->d_prm.p, (const int*)t->d_cat.p, n, nb, D, (const double*)t->vals.p,
-                                           (const int*)t->grp.p, (const int*)t->pos.p, t->pw, t->lcat, (double*)t->cat_p.p,
-                                           (double*)t->cat_sc.p, (double*)t->cat_cum.p);
+    tpe_cat_kernel<<<t->Dcat, 256, 0, s>>>(t->d_prm.p, t->d_cat.p, n, nb, D, t->vals.p,
+                                           t->grp.p, t->pos.p, t->pw, t->lcat, t->cat_p.p,
+                                           t->cat_sc.p, t->cat_cum.p);
     KBO_LAUNCH_CHECK(h);
   }
   t->built_n = n;
@@ -680,11 +689,11 @@ int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds
   }
   t->Dc = (int)t->cont.size();
   t->Dd = (int)t->disc.size();
-  KBO_TRY(kbo_upload(h, t->d_prm, t->prm.data(), sizeof(TpeParam) * D));
-  KBO_TRY(kbo_upload(h, t->d_cont, t->cont.data(), 4 * t->cont.size()));
-  KBO_TRY(kbo_upload(h, t->d_disc, t->disc.data(), 4 * t->disc.size()));
-  KBO_TRY(kbo_upload(h, t->d_num, t->num.data(), 4 * t->num.size()));
-  KBO_TRY(kbo_upload(h, t->d_cat, t->cat.data(), 4 * t->cat.size()));
+  KBO_TRY(kbo_upload(h, t->d_prm, t->prm.data(), D));
+  KBO_TRY(kbo_upload(h, t->d_cont, t->cont.data(), t->cont.size()));
+  KBO_TRY(kbo_upload(h, t->d_disc, t->disc.data(), t->disc.size()));
+  KBO_TRY(kbo_upload(h, t->d_num, t->num.data(), t->num.size()));
+  KBO_TRY(kbo_upload(h, t->d_cat, t->cat.data(), t->cat.size()));
   KBO_TRY(t->ev.create());
   *out = t.release();
   return KBO_OK;
@@ -723,18 +732,18 @@ int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* c
   const uint32_t ask = t->asks++;
   const int D = t->D, KD = k * D;
   const int nbb = (std::max(M, t->Dd ? t->lt : 1) + 255) / 256;
-  KBO_TRY(kbo_reserve(h, t->surv, 4 * (size_t)KD));
-  KBO_TRY(kbo_reserve(h, t->bb, sizeof(TpeBest) * (size_t)KD * nbb));
-  KBO_TRY(kbo_reserve(h, t->err, 4));
-  KBO_CUDA(h, cudaMemsetAsync(t->surv.p, 0, 4 * (size_t)KD, s));
-  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, 4, s));
+  KBO_TRY(kbo_reserve(h, t->surv, (size_t)KD));
+  KBO_TRY(kbo_reserve(h, t->bb, (size_t)KD * nbb));
+  KBO_TRY(kbo_reserve(h, t->err, 1));
+  KBO_CUDA(h, cudaMemsetAsync(t->surv.p, 0, sizeof *t->surv.p * (size_t)KD, s));
+  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, sizeof *t->err.p, s));
   const TpeModels md = tpe_models(t);
   const double* X = cand_dev;
   if (!X) {   // the draws go to the caller's buffer if it wants them, else to the handle's
     double* Xw = cand_out_dev;
     if (!Xw) {
-      KBO_TRY(kbo_reserve(h, t->draws, 8 * (size_t)KD * M));
-      Xw = (double*)t->draws.p;
+      KBO_TRY(kbo_reserve(h, t->draws, (size_t)KD * M));
+      Xw = t->draws.p;
     }
     tpe_draw_kernel<<<dim3((M + 255) / 256, KD), 256, 0, s>>>(md, D, M, t->seed, ask, Xw);
     KBO_LAUNCH_CHECK(h);
@@ -745,15 +754,15 @@ int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* c
   cudaEventRecord(t->ev[1], s);
   if (t->Dc) {
     const int pairs = k * t->Dc;
-    KBO_TRY(kbo_reserve(h, t->sc, sizeof(float2) * (size_t)pairs * M));
-    KBO_TRY(kbo_reserve(h, t->lb, 4 * (size_t)pairs));
-    KBO_CUDA(h, cudaMemsetAsync(t->lb.p, 0, 4 * (size_t)pairs, s));
+    KBO_TRY(kbo_reserve(h, t->sc, (size_t)pairs * M));
+    KBO_TRY(kbo_reserve(h, t->lb, (size_t)pairs));
+    KBO_CUDA(h, cudaMemsetAsync(t->lb.p, 0, sizeof *t->lb.p * (size_t)pairs, s));
     tpe_score_kernel<<<dim3((M + TPE_THREADS * TPE_CPT - 1) / (TPE_THREADS * TPE_CPT), pairs), TPE_THREADS, 0, s>>>(
-        md, (const int*)t->d_cont.p, t->Dc, D, M, X, (float2*)t->sc.p, score_out_dev, (unsigned*)t->lb.p);
+        md, t->d_cont.p, t->Dc, D, M, X, t->sc.p, score_out_dev, t->lb.p);
     KBO_LAUNCH_CHECK(h);
     cudaEventRecord(t->ev[2], s);
-    tpe_decide_kernel<<<dim3(nbb, pairs), 256, 0, s>>>(md, (const int*)t->d_cont.p, t->Dc, D, M, X, (const float2*)t->sc.p,
-                                                       (const unsigned*)t->lb.p, (TpeBest*)t->bb.p, nbb, (int*)t->surv.p);
+    tpe_decide_kernel<<<dim3(nbb, pairs), 256, 0, s>>>(md, t->d_cont.p, t->Dc, D, M, X, t->sc.p,
+                                                       t->lb.p, t->bb.p, nbb, t->surv.p);
     KBO_LAUNCH_CHECK(h);
   } else {
     cudaEventRecord(t->ev[2], s);
@@ -761,22 +770,22 @@ int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* c
   cudaEventRecord(t->ev[3], s);
   if (t->Dd) {
     const int pairs = k * t->Dd;
-    KBO_TRY(kbo_reserve(h, t->first, 4 * (size_t)pairs * t->lt));
-    KBO_CUDA(h, cudaMemsetAsync(t->first.p, 0xFF, 4 * (size_t)pairs * t->lt, s));
-    tpe_level_kernel<<<dim3((M + 255) / 256, pairs), 256, 0, s>>>(md, (const int*)t->d_disc.p, t->Dd, D, M, X, (unsigned*)t->first.p, t->lt,
-                                                                  (int*)t->err.p);
+    KBO_TRY(kbo_reserve(h, t->first, (size_t)pairs * t->lt));
+    KBO_CUDA(h, cudaMemsetAsync(t->first.p, 0xFF, sizeof *t->first.p * (size_t)pairs * t->lt, s));
+    tpe_level_kernel<<<dim3((M + 255) / 256, pairs), 256, 0, s>>>(md, t->d_disc.p, t->Dd, D, M, X, t->first.p, t->lt,
+                                                                  t->err.p);
     KBO_LAUNCH_CHECK(h);
-    tpe_disc_score_kernel<<<dim3(nbb, pairs), 256, 0, s>>>(md, (const int*)t->d_disc.p, t->Dd, D, M, X, (const unsigned*)t->first.p, t->lt, (TpeBest*)t->bb.p, nbb, (int*)t->surv.p);
+    tpe_disc_score_kernel<<<dim3(nbb, pairs), 256, 0, s>>>(md, t->d_disc.p, t->Dd, D, M, X, t->first.p, t->lt, t->bb.p, nbb, t->surv.p);
     KBO_LAUNCH_CHECK(h);
   }
   cudaEventRecord(t->ev[4], s);
-  tpe_final_kernel<<<KD, 256, 0, s>>>(md, D, M, X, (const TpeBest*)t->bb.p, nbb, x_dev, (long long*)idx_dev);
+  tpe_final_kernel<<<KD, 256, 0, s>>>(md, D, M, X, t->bb.p, nbb, x_dev, (long long*)idx_dev);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[5], s);
   t->last_surv.assign(KD, 0);
   int err = 0;
-  KBO_CUDA(h, cudaMemcpyAsync(t->last_surv.data(), t->surv.p, 4 * (size_t)KD, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaMemcpyAsync(&err, t->err.p, 4, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(t->last_surv.data(), t->surv.p, (size_t)KD, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, kbo_copy(&err, t->err.p, 1, cudaMemcpyDeviceToHost, s));
   KBO_CUDA(h, cudaStreamSynchronize(s));
   for (int i = 0; i < 5; i++) cudaEventElapsedTime(&t->last_ms[i], t->ev[i], t->ev[i + 1]);
   if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: a supplied candidate of a quantized or categorical parameter is outside its levels");
@@ -795,18 +804,18 @@ int kbo_tpe_state(kbo_handle* h, kbo_tpe* t, int32_t param, int32_t group, doubl
   double pa = 1.0;
   if (P.kind == KBO_TPE_CHOICE) {
     nc = P.levels;
-    if (w) KBO_CUDA(h, cudaMemcpyAsync(w, (double*)t->cat_p.p + ((size_t)P.slot * 2 + group) * t->lcat, 8 * (size_t)std::min(cap, nc),
+    if (w) KBO_CUDA(h, kbo_copy(w, t->cat_p.p + ((size_t)P.slot * 2 + group) * t->lcat, (size_t)std::min(cap, nc),
                                        cudaMemcpyDeviceToHost, s));
   } else {
     TpeHdr hd;
-    KBO_CUDA(h, cudaMemcpyAsync(&hd, (TpeHdr*)t->hdr.p + 2 * P.slot + group, sizeof hd, cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, kbo_copy(&hd, t->hdr.p + 2 * P.slot + group, 1, cudaMemcpyDeviceToHost, s));
     KBO_CUDA(h, cudaStreamSynchronize(s));
     nc = hd.ncomp;
     pa = hd.p_acc;
     const size_t o = (size_t)P.slot * t->ms + (group ? TPE_CB : 0), c = (size_t)std::min(cap, nc);
-    if (w) KBO_CUDA(h, cudaMemcpyAsync(w, (double*)t->w.p + o, 8 * c, cudaMemcpyDeviceToHost, s));
-    if (mu) KBO_CUDA(h, cudaMemcpyAsync(mu, (double*)t->mu.p + o, 8 * c, cudaMemcpyDeviceToHost, s));
-    if (sigma) KBO_CUDA(h, cudaMemcpyAsync(sigma, (double*)t->sg.p + o, 8 * c, cudaMemcpyDeviceToHost, s));
+    KBO_CUDA(h, kbo_d2h(w, t->w.p + o, c, s));
+    KBO_CUDA(h, kbo_d2h(mu, t->mu.p + o, c, s));
+    KBO_CUDA(h, kbo_d2h(sigma, t->sg.p + o, c, s));
   }
   KBO_CUDA(h, cudaStreamSynchronize(s));
   if (ncomp) *ncomp = nc;

@@ -20,8 +20,19 @@ def test_device_memory_is_allocated_and_freed_only_by_devbuf():
     assert not outside, f"device memory managed outside DevBuf: {outside}"
 
 
+# `DevBuf* bufs[] = {...}` arrays, and loops over a braced list of buffers (`for (DevBuf* b : {&x, &y})`), with or without
+# the element type (`DevBuf<double>* bufs[]`)
+FREE_LIST = re.compile(r"DevBuf\s*(?:<[^<>;]*(?:<[^<>;]*>[^<>;]*)*>)?\s*\*\s*\w+\s*(?:\[\s*\]|:\s*\{)")
+
+
+def test_free_list_pattern_matches_typed_and_untyped_lists():
+    for sample in ("DevBuf* bufs[] = {&a, &b};", "DevBuf<double>* bufs[] = {&a, &b};", "DevBuf < unsigned char > *bufs[] = {&a};",
+                   "for (DevBuf* b : {&x, &y})", "for (DevBuf<int>* b : {&x, &y})", "DevBuf<std::pair<int, int>>* bufs[] = {&a};"):
+        assert FREE_LIST.search(sample), sample
+    for sample in ("DevBuf<double> a, b;", "DevBuf<double>& b", "template <class T> static int kbo_reserve(kbo_handle* h, DevBuf<T>& b, size_t n)"):
+        assert not FREE_LIST.search(sample), sample
+
+
 def test_no_hand_kept_free_lists():
-    # `DevBuf* bufs[] = {...}` arrays, and loops over a braced list of buffers (`for (DevBuf* b : {&x, &y})`)
-    pat = re.compile(r"DevBuf\s*\*\s*\w+\s*(?:\[\s*\]|:\s*\{)")
-    lists = {name: len(pat.findall(txt)) for name, txt in _sources().items()}
+    lists = {name: len(FREE_LIST.findall(txt)) for name, txt in _sources().items()}
     assert not any(lists.values()), f"DevBuf* free lists: { {k: v for k, v in lists.items() if v} }"
