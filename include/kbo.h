@@ -361,6 +361,30 @@ int kbo_cma_set_lr_adapt(kbo_handle* h, kbo_cma* c, int32_t on);
 int kbo_cma_lra_state(kbo_handle* h, kbo_cma* c, double* E_mean_host, double* E_Sigma_host, double* V_host, double* eta_host,
                       void* stream);
 
+/* ---- separable CMA-ES (`cmaes` with use_separable_cma; Ros & Hansen, PPSN 2008, as CyberAgent `cmaes`' SepCMA) ------
+ * A separate object from kbo_cma: C is kept as its diagonal and d = √C, so sampling and update are O(lambda·D) and no D×D
+ * object exists (oracle/sepcma_oracle.py states each rule).  Positive recombination weights only (μ = ⌊lambda/2⌋);
+ * c_c = 4/(D+4), c1 = 2/((D+1.3)² + μ_eff) and the rank-μ rate scaled by (D+2)/3, capped at 1 − c1 − 1e-8.
+ *   kbo_sepcma_ask : X (lambda×D, device, fp64) = m + sigma·(d∘z); z from the built-in Philox stream (the same convention
+ *                    and never-reset draw counter as kbo_cma_ask) or from z_in_dev (lambda×D device, may be NULL).
+ *   kbo_sepcma_tell: fitness (lambda, device, minimised, ranked in kbo_cma_tell's NumPy order) for the X of the last ask →
+ *                    mean, p_σ, σ (capped at 1e32), h_σ, p_c, C and d = √C (C_j <= 0 floored at 1e-8 under the root).  It
+ *                    ends with kbo_cma_tell's termination test without NOEFFECTAXIS (bit 16 is never set): TOLFUN, TOLX
+ *                    (all σ·C_j and σ·p_c,j < 1e-12·σ0), TOLXUP, NOEFFECTCOORD (some m_j == m_j + 0.2σ·√C_j), CONDITIONCOV.
+ * Limits: 1 <= D <= 4096, 4 <= lambda <= 8192.  kbo_sepcma_state copies mean, sigma, the diagonal C_diag, p_sigma, p_c, d and
+ * the last ask's steps Y (lambda×D) to HOST buffers (any may be NULL) and synchronises; `generation` is the strategy
+ * generation of the current run.  kbo_sepcma_stop_flags and kbo_sepcma_restart behave as kbo_cma_stop_flags and
+ * kbo_cma_restart (restart: C = d = 1, zero paths, history and flags, generation 0; the draw counter goes on). */
+typedef struct kbo_sepcma kbo_sepcma;
+int kbo_sepcma_create(kbo_handle* h, kbo_sepcma** out, int32_t D, int32_t lambda, const double* mean0_host, double sigma0, uint64_t seed);
+void kbo_sepcma_destroy(kbo_sepcma* c);
+int kbo_sepcma_ask(kbo_handle* h, kbo_sepcma* c, double* X_dev, const double* z_in_dev, void* stream);
+int kbo_sepcma_tell(kbo_handle* h, kbo_sepcma* c, const double* fitness_dev, void* stream);
+int kbo_sepcma_state(kbo_handle* h, kbo_sepcma* c, double* mean, double* sigma, double* C_diag, double* p_sigma, double* p_c, double* d,
+                     double* Y_last, int64_t* generation, void* stream);
+int kbo_sepcma_stop_flags(kbo_handle* h, kbo_sepcma* c, uint32_t* flags_host, double* funhist_host, int32_t* term_host, void* stream);
+int kbo_sepcma_restart(kbo_handle* h, kbo_sepcma* c, int32_t lambda, const double* mean0_host, double sigma0);
+
 /* ---- TPE (Katib algorithm `tpe`: hyperopt's tpe.suggest on a flat space; FP64 restatement oracle/tpe_oracle.py) -------
  * Parameter kinds: UNIFORM = uniform(lo, hi); QUNIFORM = quniform(lo, hi, q), values rint(x/q)·q; CHOICE = choice over
  * `levels` categories, observed and reported as the category index.

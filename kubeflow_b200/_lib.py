@@ -60,6 +60,8 @@ EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_se
            "kbo_cma_create", "kbo_cma_destroy", "kbo_cma_ask", "kbo_cma_tell", "kbo_cma_state", "kbo_cma_run_synthetic",
            "kbo_cma_stop_flags", "kbo_cma_restart", "kbo_cma_set_margin", "kbo_cma_margin_state", "kbo_cma_set_lr_adapt",
            "kbo_cma_lra_state",
+           "kbo_sepcma_create", "kbo_sepcma_destroy", "kbo_sepcma_ask", "kbo_sepcma_tell", "kbo_sepcma_state", "kbo_sepcma_stop_flags",
+           "kbo_sepcma_restart",
            "kbo_tpe_create", "kbo_tpe_destroy", "kbo_tpe_tell", "kbo_tpe_ask", "kbo_tpe_state", "kbo_tpe_last_survivors", "kbo_tpe_last_timings",
            "kbo_mvtpe_create", "kbo_mvtpe_destroy", "kbo_mvtpe_tell", "kbo_mvtpe_ask", "kbo_mvtpe_state", "kbo_mvtpe_last_survivors",
            "kbo_mvtpe_last_timings",
@@ -166,6 +168,14 @@ def load() -> C.CDLL:
     lib.kbo_cma_margin_state.argtypes = [vp, vp, vp, vp, pd, vp]
     lib.kbo_cma_set_lr_adapt.argtypes = [vp, vp, i32]
     lib.kbo_cma_lra_state.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+    lib.kbo_sepcma_create.argtypes = [vp, C.POINTER(vp), i32, i32, pd, dbl, C.c_uint64]
+    lib.kbo_sepcma_destroy.argtypes = [vp]
+    lib.kbo_sepcma_destroy.restype = None
+    lib.kbo_sepcma_ask.argtypes = [vp, vp, vp, vp, vp]
+    lib.kbo_sepcma_tell.argtypes = [vp, vp, vp, vp]
+    lib.kbo_sepcma_state.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(i64), vp]
+    lib.kbo_sepcma_stop_flags.argtypes = [vp, vp, C.POINTER(C.c_uint32), vp, C.POINTER(i32), vp]
+    lib.kbo_sepcma_restart.argtypes = [vp, vp, i32, pd, dbl]
     lib.kbo_tpe_create.argtypes = [vp, C.POINTER(vp), i32, vp, vp, vp, vp, vp, dbl, dbl, C.c_uint64]
     lib.kbo_tpe_destroy.argtypes = [vp]
     lib.kbo_tpe_destroy.restype = None

@@ -720,6 +720,165 @@ static int cma_lra_blend(kbo_handle* h, kbo_cma* c, cudaStream_t s) {
   return KBO_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ separable CMA-ES (sep-CMA)
+// sep-CMA-ES (Ros & Hansen, PPSN 2008) as CyberAgent `cmaes`' SepCMA: oracle/sepcma_oracle.py states each rule.  C is kept
+// as its diagonal and d = √C, so a generation is O(λ·D) and D goes to SEP_MAXD.  The ask is cma_normal_kernel,
+// cma_scale_kernel (y = d∘z; its ‖z‖² is not used) and cma_x_kernel; the tell is cma_sort_kernel and the three kernels
+// below.  Every reduction has a fixed order and there are no atomics, so a run replays bit for bit.
+#define SEP_MAXD 4096
+#define SEP_UPD_THREADS 256
+#define SEP_FIN_THREADS 1024
+#define SEP_STOP_THREADS 256
+#define SEP_SIGMA_MAX 1e32
+
+struct kbo_sepcma {
+  int D = 0, lambda = 0, mu = 0, lam_pow2 = 0, nparts = 0;  // nparts: CTAs of sepcma_update_kernel
+  uint64_t seed = 0;
+  long long gen = 0;    // strategy generation: back to 0 at every restart
+  long long draws = 0;  // Philox counter of the built-in sampler: one per tell, never reset
+  double mu_eff, c1, cmu, cm, c_sigma, d_sigma, cc, chi_n;
+  int term = 0;
+  double tolx = 0.0;
+  DevBuf<double> mean, C, Dv, ps, pc, weights, Z, Y, zn2, scal, yw, wy2, part, hist;  // C, Dv: the diagonal and √ of it
+  DevBuf<int> order;
+  DevBuf<unsigned> flags;
+  bool asked = false;
+};
+
+struct SepConst {
+  double mu_eff, c1, cmu, cm, c_sigma, d_sigma, cc, chi_n;
+};
+
+// One thread per dimension j: over the μ best samples in rank order, y_w,j = Σ w_r y_r,j and Σ w_r y_r,j²; then
+// m_j ← m_j + c_m·σ·y_w,j and p_σ,j ← (1 − c_σ)·p_σ,j + √(c_σ(2 − c_σ)μ_eff)·y_w,j/d_j (d from before the tell).  Each CTA
+// writes its Σ p_σ,j² by a fixed tree to part[blockIdx.x].
+__global__ void __launch_bounds__(SEP_UPD_THREADS) sepcma_update_kernel(const double* __restrict__ Y, const int* __restrict__ order,
+                                                                        const double* __restrict__ w, int D, int mu, SepConst k,
+                                                                        double* __restrict__ mean, const double* __restrict__ Dv,
+                                                                        double* __restrict__ ps, const double* __restrict__ scal,
+                                                                        double* __restrict__ yw, double* __restrict__ wy2,
+                                                                        double* __restrict__ part) {
+  __shared__ double red[SEP_UPD_THREADS];
+  const int t = threadIdx.x, j = blockIdx.x * SEP_UPD_THREADS + t;
+  double v2 = 0.0;
+  if (j < D) {
+    double a = 0.0, b = 0.0;
+#pragma unroll 4
+    for (int r = 0; r < mu; r++) {
+      const double y = Y[(size_t)order[r] * D + j], wr = w[r];
+      a = fma(wr, y, a);
+      b = fma(wr * y, y, b);
+    }
+    yw[j] = a;
+    wy2[j] = b;
+    mean[j] = fma(k.cm * scal[CS_SIGMA], a, mean[j]);
+    const double v = (1.0 - k.c_sigma) * ps[j] + sqrt(k.c_sigma * (2.0 - k.c_sigma) * k.mu_eff) * (a / Dv[j]);
+    ps[j] = v;
+    v2 = v * v;
+  }
+  red[t] = v2;
+  __syncthreads();
+  for (int o = SEP_UPD_THREADS / 2; o > 0; o >>= 1) {
+    if (t < o) red[t] += red[t + o];
+    __syncthreads();
+  }
+  if (t == 0) part[blockIdx.x] = red[0];
+}
+
+// One CTA: ‖p_σ‖ from the partials in CTA order, then σ (capped), h_σ, and per dimension p_c, C and d = √C (C_j ≤ 0
+// floored at CMA_EPS under the root, as the oracle does).
+__global__ void __launch_bounds__(SEP_FIN_THREADS) sepcma_finish_kernel(const double* __restrict__ part, int nparts, int D, SepConst k,
+                                                                        long long gen, const double* __restrict__ yw,
+                                                                        const double* __restrict__ wy2, double* __restrict__ pc,
+                                                                        double* __restrict__ C, double* __restrict__ Dv,
+                                                                        double* __restrict__ scal) {
+  __shared__ double s_h;
+  const int t = threadIdx.x;
+  if (t == 0) {
+    double a = 0.0;
+    for (int i = 0; i < nparts; i++) a += part[i];
+    const double norm_ps = sqrt(a);
+    const double h_left = norm_ps / sqrt(1.0 - pow(1.0 - k.c_sigma, 2.0 * (double)(gen + 1)));
+    s_h = h_left < (1.4 + 2.0 / (D + 1.0)) * k.chi_n ? 1.0 : 0.0;
+    const double sigma = scal[CS_SIGMA] * exp((k.c_sigma / k.d_sigma) * (norm_ps / k.chi_n - 1.0));
+    scal[CS_SIGMA] = sigma > SEP_SIGMA_MAX ? SEP_SIGMA_MAX : sigma;
+  }
+  __syncthreads();
+  const double h = s_h;
+  const double a = 1.0 + k.c1 * ((1.0 - h) * k.cc * (2.0 - k.cc)) - k.c1 - k.cmu;
+  const double pcoef = h * sqrt(k.cc * (2.0 - k.cc) * k.mu_eff);
+  for (int j = t; j < D; j += SEP_FIN_THREADS) {
+    const double p = (1.0 - k.cc) * pc[j] + pcoef * yw[j];
+    pc[j] = p;
+    const double c = a * C[j] + k.c1 * (p * p) + k.cmu * wy2[j];
+    C[j] = c;
+    Dv[j] = sqrt(c <= 0.0 ? CMA_EPS : c);
+  }
+}
+
+// One CTA striding over D, after the tell: the history ring and five of cma_stop_kernel's criteria with its rounding
+// rules (no NOEFFECTAXIS: there is no basis).  TOLX tests σ·C_j, as cma_stop_kernel tests σ·C_ii.
+__global__ void __launch_bounds__(SEP_STOP_THREADS) sepcma_should_stop_kernel(const double* __restrict__ f, const int* __restrict__ order,
+                                                                       int lambda, int D, const double* __restrict__ mean,
+                                                                       const double* __restrict__ C, const double* __restrict__ Dv,
+                                                                       const double* __restrict__ pc, const double* __restrict__ scal,
+                                                                       double* hist, int term, long long g, double tolx,
+                                                                       unsigned* __restrict__ flags) {
+  constexpr int NW = SEP_STOP_THREADS / 32;
+  __shared__ double s_hi[NW], s_lo[NW], s_dhi[NW], s_dlo[NW];
+  __shared__ int s_nan[NW], s_dnan[NW];
+  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+  const int slot = (int)(2 * (g % term));
+  if (t == 0) hist[slot] = f[order[0]];
+  if (t == 1) hist[slot + 1] = f[order[lambda - 1]];
+  __syncthreads();
+  int hnan = 0, dnan = 0;
+  double hi = -INFINITY, lo = INFINITY, dhi = -INFINITY, dlo = INFINITY;
+  for (int i = t; i < 2 * term; i += SEP_STOP_THREADS) {
+    const double v = hist[i];
+    hnan |= v != v;
+    hi = fmax(hi, v);
+    lo = fmin(lo, v);
+  }
+  const double sigma = scal[CS_SIGMA];
+  const double s02 = __dmul_rn(0.2, sigma);
+  bool tolx_all = true, coord_any = false;
+  for (int j = t; j < D; j += SEP_STOP_THREADS) {
+    const double c = C[j], m = mean[j], d = Dv[j];
+    dnan |= d != d;
+    dhi = fmax(dhi, d);
+    dlo = fmin(dlo, d);
+    tolx_all &= __dmul_rn(sigma, c) < tolx && __dmul_rn(sigma, pc[j]) < tolx;
+    coord_any |= m == __dadd_rn(m, __dmul_rn(s02, cma_sqrt_rn(c)));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    hnan |= __shfl_xor_sync(0xffffffffu, hnan, o);
+    dnan |= __shfl_xor_sync(0xffffffffu, dnan, o);
+    hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+    dhi = fmax(dhi, __shfl_xor_sync(0xffffffffu, dhi, o));
+    dlo = fmin(dlo, __shfl_xor_sync(0xffffffffu, dlo, o));
+  }
+  if (lane == 0) { s_hi[w] = hi; s_lo[w] = lo; s_dhi[w] = dhi; s_dlo[w] = dlo; s_nan[w] = hnan; s_dnan[w] = dnan; }
+  tolx_all = __syncthreads_and(tolx_all);
+  coord_any = __syncthreads_or(coord_any);
+  if (t == 0) {
+    for (int i = 1; i < NW; i++) {
+      hi = fmax(hi, s_hi[i]); lo = fmin(lo, s_lo[i]); dhi = fmax(dhi, s_dhi[i]); dlo = fmin(dlo, s_dlo[i]);
+      hnan |= s_nan[i]; dnan |= s_dnan[i];
+    }
+    unsigned fl = 0;
+    if (g > term && !hnan && __dadd_rn(hi, -lo) < CMA_TOLFUN) fl |= STOP_TOLFUN;
+    if (tolx_all) fl |= STOP_TOLX;
+    if (!dnan && __dmul_rn(sigma, dhi) > CMA_TOLXUP) fl |= STOP_TOLXUP;
+    if (coord_any) fl |= STOP_NOEFFECTCOORD;
+    if (!dnan && (dhi > 1.7976931348623157e308 ? dlo <= 1.7976931348623157e308 : cma_div_rn(dhi, dlo) > CMA_TOLCONDCOV))
+      fl |= STOP_CONDITIONCOV;
+    *flags = fl;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 static int cma_generation_tell(kbo_handle* h, kbo_cma* c, const double* fitness, cudaStream_t s) {
   const int D = c->D, lam = c->lambda;
@@ -1106,6 +1265,195 @@ int kbo_cma_run_synthetic(kbo_handle* h, kbo_cma* c, int32_t fitness_kind, int32
   if (best_f_host) *best_f_host = sc[CS_BEST_F];
   if (jacobi_sweeps_last) *jacobi_sweeps_last = sc[CS_SWEEPS];
   if (elapsed_ms) cudaEventElapsedTime(elapsed_ms, h->ev[5], h->ev[6]);
+  return KBO_OK;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ separable CMA-ES: host side
+// Strategy parameters for population λ (positive weights only; sep-CMA's c_c, c1 and (D + 2)/3-scaled cμ, capped at
+// 1 − c1 − 1e-8 as the full path caps it), the buffers
+// they size, and the termination constants of a run starting at σ0.  Shared by create and restart.
+static int sepcma_configure(kbo_handle* h, kbo_sepcma* c, int lambda, double sigma0) {
+  const int D = c->D, mu = lambda / 2;
+  const double n = D;
+  c->lambda = lambda;
+  c->mu = mu;
+  int p2 = 1;
+  while (p2 < lambda) p2 <<= 1;
+  c->lam_pow2 = p2;
+  c->nparts = (D + SEP_UPD_THREADS - 1) / SEP_UPD_THREADS;
+  std::vector<double> w(mu);
+  double s1 = 0, s2 = 0;
+  for (int i = 0; i < mu; i++) {
+    w[i] = log((lambda + 1) / 2.0) - log((double)(i + 1));
+    s1 += w[i];
+  }
+  for (int i = 0; i < mu; i++) {
+    w[i] /= s1;
+    s2 += w[i] * w[i];
+  }
+  const double mu_eff = 1.0 / s2;
+  c->mu_eff = mu_eff;
+  c->cm = 1.0;
+  c->c_sigma = (mu_eff + 2) / (n + mu_eff + 5);
+  const double t = sqrt((mu_eff - 1) / (n + 1)) - 1;
+  c->d_sigma = 1 + 2 * (t > 0 ? t : 0) + c->c_sigma;
+  c->cc = 4.0 / (n + 4.0);
+  c->c1 = 2.0 / ((n + 1.3) * (n + 1.3) + mu_eff);
+  const double r = (2 * mu_eff - 1) / ((n + 2) * (n + 2) + mu_eff);
+  c->cmu = (n + 2) / 3.0 * (2.0 / mu_eff / ((n + sqrt(2.0)) * (n + sqrt(2.0))) + (1 - 1 / mu_eff) * (r < 1 ? r : 1.0));
+  if (c->cmu > 1 - c->c1 - 1e-8) c->cmu = 1 - c->c1 - 1e-8;   // past 1 at large λ, C's own coefficient would turn negative
+  c->chi_n = sqrt(n) * (1.0 - 1.0 / (4.0 * n) + 1.0 / (21.0 * n * n));
+  c->term = 10 + (30 * D + lambda - 1) / lambda;   // 10 + ⌈30·n/λ⌉
+  c->tolx = 1e-12 * sigma0;
+  const size_t LD = (size_t)lambda * D;
+  KBO_TRY(kbo_reserve(h, c->mean, D));
+  KBO_TRY(kbo_reserve(h, c->C, D));
+  KBO_TRY(kbo_reserve(h, c->Dv, D));
+  KBO_TRY(kbo_reserve(h, c->ps, D));
+  KBO_TRY(kbo_reserve(h, c->pc, D));
+  KBO_TRY(kbo_reserve(h, c->Z, LD + 2));
+  KBO_TRY(kbo_reserve(h, c->Y, LD));
+  KBO_TRY(kbo_reserve(h, c->zn2, lambda));
+  KBO_TRY(kbo_reserve(h, c->order, lambda));
+  KBO_TRY(kbo_reserve(h, c->scal, CS_COUNT));
+  KBO_TRY(kbo_reserve(h, c->yw, D));
+  KBO_TRY(kbo_reserve(h, c->wy2, D));
+  KBO_TRY(kbo_reserve(h, c->part, c->nparts));
+  KBO_TRY(kbo_reserve(h, c->hist, (size_t)c->term * 2));
+  KBO_TRY(kbo_reserve(h, c->flags, 1));
+  KBO_TRY(kbo_upload(h, c->weights, w.data(), mu));
+  return KBO_OK;
+}
+
+// A run's starting state: mean0, σ0, C = d = 1, zero paths, history and flags, strategy generation 0 (synchronous).
+static int sepcma_start_run(kbo_handle* h, kbo_sepcma* c, const double* mean0, double sigma0) {
+  const int D = c->D;
+  const double sc[CS_COUNT] = {sigma0, 0, 0, 0, 0, 0, 0, 0};
+  const std::vector<double> ones(D, 1.0);
+  KBO_CUDA(h, cudaMemcpy(c->mean.p, mean0, sizeof *c->mean.p * D, cudaMemcpyHostToDevice));
+  KBO_CUDA(h, cudaMemcpy(c->scal.p, sc, sizeof sc, cudaMemcpyHostToDevice));
+  KBO_CUDA(h, cudaMemcpy(c->C.p, ones.data(), sizeof *c->C.p * D, cudaMemcpyHostToDevice));
+  KBO_CUDA(h, cudaMemcpy(c->Dv.p, ones.data(), sizeof *c->Dv.p * D, cudaMemcpyHostToDevice));
+  KBO_CUDA(h, cudaMemset(c->ps.p, 0, sizeof *c->ps.p * D));
+  KBO_CUDA(h, cudaMemset(c->pc.p, 0, sizeof *c->pc.p * D));
+  KBO_CUDA(h, cudaMemset(c->hist.p, 0, sizeof *c->hist.p * 2 * (size_t)c->term));
+  KBO_CUDA(h, cudaMemset(c->flags.p, 0, sizeof *c->flags.p));
+  KBO_CUDA(h, cudaDeviceSynchronize());
+  c->gen = 0;
+  c->asked = false;
+  return KBO_OK;
+}
+
+static int sepcma_generation_ask(kbo_handle* h, kbo_sepcma* c, double* X, const double* z_in, cudaStream_t s) {
+  const int D = c->D, lam = c->lambda;
+  const int64_t n = (int64_t)lam * D;
+  const double* Z = z_in;
+  if (!Z) {
+    cma_normal_kernel<<<(unsigned)((n / 2 + 1 + 255) / 256), 256, 0, s>>>(c->Z.p, n, c->seed, (uint64_t)c->draws);
+    KBO_LAUNCH_CHECK(h);
+    Z = c->Z.p;
+  }
+  cma_scale_kernel<<<(lam + 7) / 8, 256, 0, s>>>(Z, c->Dv.p, lam, D, c->Y.p, c->zn2.p);   // Y = d∘z
+  KBO_LAUNCH_CHECK(h);
+  cma_x_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(c->Y.p, c->mean.p, c->scal.p, n, D, X);
+  KBO_LAUNCH_CHECK(h);
+  c->asked = true;
+  return KBO_OK;
+}
+
+static int sepcma_generation_tell(kbo_handle* h, kbo_sepcma* c, const double* fitness, cudaStream_t s) {
+  const int D = c->D, lam = c->lambda;
+  const SepConst k{c->mu_eff, c->c1, c->cmu, c->cm, c->c_sigma, c->d_sigma, c->cc, c->chi_n};
+  cma_sort_kernel<<<1, 1024, c->lam_pow2 * 12, s>>>(fitness, lam, c->lam_pow2, c->order.p, c->scal.p);
+  KBO_LAUNCH_CHECK(h);
+  sepcma_update_kernel<<<c->nparts, SEP_UPD_THREADS, 0, s>>>(c->Y.p, c->order.p, c->weights.p, D, c->mu, k, c->mean.p, c->Dv.p,
+                                                             c->ps.p, c->scal.p, c->yw.p, c->wy2.p, c->part.p);
+  KBO_LAUNCH_CHECK(h);
+  sepcma_finish_kernel<<<1, SEP_FIN_THREADS, 0, s>>>(c->part.p, c->nparts, D, k, c->gen, c->yw.p, c->wy2.p, c->pc.p, c->C.p,
+                                                     c->Dv.p, c->scal.p);
+  KBO_LAUNCH_CHECK(h);
+  sepcma_should_stop_kernel<<<1, SEP_STOP_THREADS, 0, s>>>(fitness, c->order.p, lam, D, c->mean.p, c->C.p, c->Dv.p, c->pc.p, c->scal.p,
+                                                    c->hist.p, c->term, c->gen + 1, c->tolx, c->flags.p);
+  KBO_LAUNCH_CHECK(h);
+  c->gen++;
+  c->draws++;
+  c->asked = false;
+  return KBO_OK;
+}
+
+extern "C" {
+
+int kbo_sepcma_create(kbo_handle* h, kbo_sepcma** out, int32_t D, int32_t lambda, const double* mean0, double sigma0, uint64_t seed) {
+  if (!h || !out) return KBO_ERR_INVALID;
+  *out = nullptr;
+  if (D < 1 || D > SEP_MAXD) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sepcma_create: 1 <= D <= %d supported (got %d)", SEP_MAXD, D);
+  if (lambda < 4 || lambda > 8192) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sepcma_create: 4 <= lambda <= 8192 supported (got %d)", lambda);
+  if (!mean0 || !(sigma0 > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sepcma_create: mean0 must be given and sigma0 > 0");
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  std::unique_ptr<kbo_sepcma> c(new (std::nothrow) kbo_sepcma());
+  if (!c) return KBO_ERR_NOMEM;
+  c->D = D;
+  c->seed = seed;
+  KBO_TRY(sepcma_configure(h, c.get(), lambda, sigma0));
+  cudaFuncSetAttribute(cma_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 12);
+  KBO_TRY(sepcma_start_run(h, c.get(), mean0, sigma0));
+  *out = c.release();
+  return KBO_OK;
+}
+
+void kbo_sepcma_destroy(kbo_sepcma* c) {
+  if (c) delete c;
+}
+
+int kbo_sepcma_restart(kbo_handle* h, kbo_sepcma* c, int32_t lambda, const double* mean0, double sigma0) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (lambda < 4 || lambda > 8192) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sepcma_restart: 4 <= lambda <= 8192 supported (got %d)", lambda);
+  if (!mean0 || !(sigma0 > 0.0)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sepcma_restart: mean0 must be given and sigma0 > 0");
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  KBO_CUDA(h, cudaDeviceSynchronize());            // the last tell may still be reading buffers that are about to grow
+  KBO_TRY(sepcma_configure(h, c, lambda, sigma0));
+  return sepcma_start_run(h, c, mean0, sigma0);
+}
+
+int kbo_sepcma_ask(kbo_handle* h, kbo_sepcma* c, double* X_dev, const double* z_in_dev, void* stream) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (!X_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sepcma_ask: null output");
+  return sepcma_generation_ask(h, c, X_dev, z_in_dev, (cudaStream_t)stream);
+}
+
+int kbo_sepcma_tell(kbo_handle* h, kbo_sepcma* c, const double* fitness_dev, void* stream) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  if (!fitness_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_sepcma_tell: null fitness");
+  if (!c->asked) KBO_FAIL(h, KBO_ERR_STATE, "kbo_sepcma_tell: call kbo_sepcma_ask first (tell ranks the samples of the last ask)");
+  return sepcma_generation_tell(h, c, fitness_dev, (cudaStream_t)stream);
+}
+
+int kbo_sepcma_state(kbo_handle* h, kbo_sepcma* c, double* mean, double* sigma, double* C_diag, double* p_sigma, double* p_c, double* Dv,
+                     double* Y_last, int64_t* generation, void* stream) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t D = c->D;
+  KBO_CUDA(h, kbo_d2h(mean, c->mean.p, D, s));
+  KBO_CUDA(h, kbo_d2h(sigma, c->scal.p, 1, s));
+  KBO_CUDA(h, kbo_d2h(C_diag, c->C.p, D, s));
+  KBO_CUDA(h, kbo_d2h(p_sigma, c->ps.p, D, s));
+  KBO_CUDA(h, kbo_d2h(p_c, c->pc.p, D, s));
+  KBO_CUDA(h, kbo_d2h(Dv, c->Dv.p, D, s));
+  KBO_CUDA(h, kbo_d2h(Y_last, c->Y.p, D * c->lambda, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (generation) *generation = c->gen;
+  return KBO_OK;
+}
+
+int kbo_sepcma_stop_flags(kbo_handle* h, kbo_sepcma* c, uint32_t* flags_host, double* funhist_host, int32_t* term_host, void* stream) {
+  if (!h || !c) return KBO_ERR_INVALID;
+  cudaStream_t s = (cudaStream_t)stream;
+  KBO_CUDA(h, kbo_d2h(flags_host, c->flags.p, 1, s));
+  KBO_CUDA(h, kbo_d2h(funhist_host, c->hist.p, (size_t)c->term * 2, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (term_host) *term_host = c->term;
   return KBO_OK;
 }
 

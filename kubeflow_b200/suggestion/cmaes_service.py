@@ -22,6 +22,11 @@ With ``lr_adapt: true`` the sampler runs CMA-ES with learning-rate adaptation (O
 when the signal-to-noise ratio of their updates falls, as on a noisy or multimodal objective, instead of asking for a
 larger ``popsize``.  It works with ``popsize``, ``sigma`` and ``restart_strategy`` (each restart starts the adaptation
 afresh) and is refused beside ``with_margin: true``.
+With ``use_separable_cma: true`` the sampler runs separable CMA-ES (Optuna's ``CmaEsSampler(use_separable_cma=True)``,
+``oracle/sepcma_oracle.py``): C is kept as its diagonal, so a generation costs O(λ·D) and spaces of up to 4096 parameters
+are served (the full sampler stops at 128); per-coordinate scales are learnt faster, correlations between parameters are
+not learnt at all.  It works with ``popsize``, ``sigma``, ``random_state`` and ``restart_strategy`` and is refused beside
+``with_margin: true`` and beside ``lr_adapt: true``, as Optuna refuses both.
 
 Each experiment's sampler is kept for one fingerprint of its search space, objective and settings: an experiment recreated
 under the same name with a changed space or changed settings starts a new run, and the old sampler is closed.  At most
@@ -39,6 +44,8 @@ from .internal import (CATEGORICAL, DISCRETE, DOUBLE, INTEGER, MAX_GOAL, Algorit
 from .cma_margin import discrete_dims, encode, parse_with_margin
 from .cma_restart import STRATEGIES, Schedule
 from .service import _Base, _reply_from, experiment_fingerprint
+
+SEP_MAX_PARAMS = 4096          # kbo_sepcma_create's limit
 
 
 def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
@@ -59,7 +66,7 @@ def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
                     raise AlgorithmSettingsError(f"popsize must be in [4, 8192], got {v}")
             elif k in ("restart_strategy", "device"):
                 out[k] = v
-            elif k in ("with_margin", "lr_adapt"):
+            elif k in ("with_margin", "lr_adapt", "use_separable_cma"):
                 out[k] = parse_with_margin(v, k)
             elif k == "margin":
                 out[k] = float(v)
@@ -73,6 +80,12 @@ def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
         raise AlgorithmSettingsError("margin needs with_margin: true")
     if out.get("lr_adapt", False) and out.get("with_margin", False):
         raise AlgorithmSettingsError("lr_adapt: true cannot be combined with with_margin: true")
+    if out.get("use_separable_cma", False):
+        for other in ("with_margin", "lr_adapt"):
+            if out.get(other, False):
+                raise AlgorithmSettingsError(f"use_separable_cma: true cannot be combined with {other}: true")
+        if n_params > SEP_MAX_PARAMS:
+            raise AlgorithmSettingsError(f"use_separable_cma supports at most {SEP_MAX_PARAMS} parameters, got {n_params}")
     if out.get("restart_strategy", "none") not in STRATEGIES:
         raise AlgorithmSettingsError(f"restart_strategy must be one of {', '.join(STRATEGIES)}, got {out['restart_strategy']!r}")
     if n_params < 2:
@@ -82,8 +95,9 @@ def validate_cmaes_settings(settings: dict, n_params: int) -> dict:
 
 class _Experiment:
     def __init__(self, space, D, settings):
-        from ..cmaes import CmaEs
-        self.es = CmaEs(np.full(D, 0.5), settings.get("sigma", 1.0 / 6.0), popsize=settings.get("popsize"),
+        from .. import cmaes
+        self.sep = settings.get("use_separable_cma", False)
+        self.es = (cmaes.SepCmaEs if self.sep else cmaes.CmaEs)(np.full(D, 0.5), settings.get("sigma", 1.0 / 6.0), popsize=settings.get("popsize"),
                         seed=settings.get("random_state", 0), device=int(settings.get("device", 0)))
         self.queue = []          # [(sample index, assignments)] of the current generation not handed out yet
         self.assign = {}         # sample index -> assignments of the current generation
@@ -201,6 +215,8 @@ class CmaesService(_Base):
                     if st.levels:
                         x = s["mean"] + s["sigma"] * (st.es.margin_state()["A"] * (s["B"] @ (s["d"] * z)))
                         lists.append(self._to_assignments(ss, encode(st.levels, x), st.levels))
+                    elif st.sep:
+                        lists.append(self._to_assignments(ss, s["mean"] + s["sigma"] * (s["d"] * z)))
                     else:
                         lists.append(self._to_assignments(ss, s["mean"] + s["sigma"] * (s["B"] @ (s["d"] * z))))
         return _reply_from(lists)

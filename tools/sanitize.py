@@ -52,6 +52,17 @@ print(es.run_synthetic("rastrigin", 3), es.lr_state()["eta_mean"])
 es.restart(40, np.full(9, 0.5), 0.3)                 # an LRA restart with a larger λ, then a tell of the new run
 print(es.run_synthetic("sphere", 2), es.lr_state()["eta_mean"])
 es.close()
+from kubeflow_b200.cmaes import SepCmaEs              # separable CMA-ES: two CTAs of the update at D = 300, a restart to a larger λ
+for D, lam in ((9, 20), (300, 16)):
+    es = SepCmaEs(np.zeros(D), 1.0, popsize=lam, seed=1)
+    for _ in range(3):
+        X = es.ask()
+        es.tell((X * X).sum(1))
+    es.restart(2 * lam, np.full(D, 0.5), 0.3)
+    X = es.ask()
+    es.tell((X * X).sum(1))
+    print(D, lam, es.stop_flags()[0], es.state()["sigma"])
+    es.close()
 from kubeflow_b200.tpe import Tpe                     # TPE: model build (radix + segmented sorts), draws, FP32 score + FP64 decision, levels
 _r = np.random.default_rng(3)
 tp = Tpe([("uniform", -1.0, 3.0), ("quniform", 3.0, 48.0, 5.0), ("choice", 5), ("quniform", 0.0, 1e6, 1.0)], seed=9)
