@@ -499,6 +499,41 @@ int kbo_forest_export(kbo_handle* h, kbo_forest* f, int32_t tree, int32_t* featu
                       void* stream);
 int kbo_forest_last_timings(kbo_handle* h, kbo_forest* f, float* ms, int32_t n);
 
+/* ---- GBRT (Katib algorithm `bayesianoptimization` with skopt's GBRT surrogate: GradientBoostingQuantileRegressor, three
+ * GradientBoostingRegressor(loss="quantile", n_estimators) chains; FP64 restatement oracle/gbrt_oracle.py) ------------------------
+ * Each chain follows scikit-learn 1.9.0: init np.percentile(y, 100·α) (linear); per stage a squared-error tree of depth <= 3 on
+ * the negative gradient (α where y >= raw, α − 1 elsewhere) over float32 X, its leaves replaced by the inverted-CDF percentile of
+ * the residuals y − raw, and raw += fl(0.1·value).  Splits maximise (pl²·nr + pr²·nl) / (nl·nr) exactly (counts of rows going
+ * left / right and of those with y >= raw); ties go to the lowest feature, then the lowest threshold; a node whose rows are all
+ * on one side of raw is a leaf.
+ *   kbo_gbrt_create: quantiles (3 increasing values in (0, 1), NULL: skopt's 0.16, 0.5, 0.84), n_estimators (1..128).
+ *   kbo_gbrt_fit    : X (N×D fp32), y (N fp64), device pointers, 1 <= N <= 65536, 1 <= D <= 1024.  NaN or infinite X or y:
+ *                   KBO_ERR_INVALID.  Synchronises.
+ *   kbo_gbrt_sweep  : skopt's predict with return_std: mean = chain 1, sigma = fl(chain 2 − chain 0) / 2, negative where the quantiles cross; then n_acq (0-3, distinct kbo_acq_kind, HOST
+ *                   acqs) acquisitions on them (EI / PI with y_opt and xi, 0 where sigma <= 0; LCB with kappa and sigma as it
+ *                   is) over M fp32 candidates Xc (M×D, device).  best_dev: n_acq device kbo_best, the first-index argmax of
+ *                   each, with global_offset added to the index.  mu_out / sigma_out (M) and quantiles_out (3×M, chain-major):
+ *                   optional device fp64 arrays.  Asynchronous.
+ *   kbo_gbrt_predict: mean, sigma and the three chains as above at n points (device, or host with x_on_host = 1) into HOST
+ *                   arrays (any may be NULL).  Synchronises.
+ *   kbo_gbrt_export : one stage's tree of one chain into HOST buffers (any may be NULL) in sklearn's tree_ layout (depth-first
+ *                   preorder, left first): feature (-2 at leaves), threshold (-2 at leaves), left / right (-1 at leaves), value
+ *                   (leaves: the replaced value; inner nodes: the mean negative gradient), n_node_samples, n_pos (rows with
+ *                   y >= raw).  n_nodes receives the node count; with cap < n_nodes only n_nodes and init are written.  init: the
+ *                   chain's init.  Synchronises.
+ *   kbo_gbrt_last_timings: milliseconds of the last fit and the last sweep, CUDA events on their streams.  Returns 2. */
+typedef struct kbo_gbrt kbo_gbrt;
+int kbo_gbrt_create(kbo_handle* h, kbo_gbrt** out, const double* quantiles, int32_t n_estimators);
+void kbo_gbrt_destroy(kbo_gbrt* g);
+int kbo_gbrt_fit(kbo_handle* h, kbo_gbrt* g, const float* X, const double* y, int32_t N, int32_t D, void* stream);
+int kbo_gbrt_sweep(kbo_handle* h, kbo_gbrt* g, const float* Xc, int64_t M, int64_t global_offset, int32_t n_acq, const int32_t* acqs, double y_opt,
+                   double xi, double kappa, kbo_best* best_dev, double* mu_out, double* sigma_out, double* quantiles_out, void* stream);
+int kbo_gbrt_predict(kbo_handle* h, kbo_gbrt* g, const float* X, int32_t n, int x_on_host, double* mu_host, double* sigma_host,
+                     double* quantiles_host, void* stream);
+int kbo_gbrt_export(kbo_handle* h, kbo_gbrt* g, int32_t chain, int32_t stage, int32_t* feature, double* threshold, int32_t* left, int32_t* right,
+                    double* value, int32_t* n_node_samples, int32_t* n_pos, int32_t cap, int32_t* n_nodes, double* init, void* stream);
+int kbo_gbrt_last_timings(kbo_handle* h, kbo_gbrt* g, float* ms, int32_t n);
+
 /* ---- ENAS controller (Katib algorithm `enas`: the macro-search LSTM controller of ENAS and its REINFORCE training; FP64
  * restatement oracle/enas_oracle.py) -----------------------------------------------------------------------------------------
  * Parameters, in this order in every flat buffer (FP32, row-major): w_lstm (2H × 4H; gates i, f, o, g), g_emb (H), w_emb

@@ -67,6 +67,8 @@ EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_se
            "kbo_mvtpe_last_timings",
            "kbo_forest_create", "kbo_forest_destroy", "kbo_forest_fit", "kbo_forest_sweep", "kbo_forest_predict", "kbo_forest_export",
            "kbo_forest_last_timings",
+           "kbo_gbrt_create", "kbo_gbrt_destroy", "kbo_gbrt_fit", "kbo_gbrt_sweep", "kbo_gbrt_predict", "kbo_gbrt_export",
+           "kbo_gbrt_last_timings",
            "kbo_enas_create", "kbo_enas_destroy", "kbo_enas_train", "kbo_enas_sample", "kbo_enas_state", "kbo_enas_set_params",
            "kbo_enas_last_timings"]
 
@@ -200,6 +202,14 @@ def load() -> C.CDLL:
     lib.kbo_forest_predict.argtypes = [vp, vp, vp, i32, C.c_int, vp, vp, vp]
     lib.kbo_forest_export.argtypes = [vp, vp, i32] + [vp] * 9 + [i32, vp, vp, vp]
     lib.kbo_forest_last_timings.argtypes = [vp, vp, vp, i32]
+    lib.kbo_gbrt_create.argtypes = [vp, C.POINTER(vp), vp, i32]
+    lib.kbo_gbrt_destroy.argtypes = [vp]
+    lib.kbo_gbrt_destroy.restype = None
+    lib.kbo_gbrt_fit.argtypes = [vp, vp, vp, vp, i32, i32, vp]
+    lib.kbo_gbrt_sweep.argtypes = [vp, vp, vp, i64, i64, i32, vp, dbl, dbl, dbl, vp, vp, vp, vp, vp]
+    lib.kbo_gbrt_predict.argtypes = [vp, vp, vp, i32, C.c_int, vp, vp, vp, vp]
+    lib.kbo_gbrt_export.argtypes = [vp, vp, i32, i32] + [vp] * 7 + [i32, vp, vp, vp]
+    lib.kbo_gbrt_last_timings.argtypes = [vp, vp, vp, i32]
     lib.kbo_enas_create.argtypes = [vp, C.POINTER(vp), i32, i32, i32, C.POINTER(KboEnasSettings), C.c_uint64]
     lib.kbo_enas_destroy.argtypes = [vp]
     lib.kbo_enas_destroy.restype = None

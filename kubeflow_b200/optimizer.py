@@ -26,7 +26,10 @@ requested assignment).  Differences, stated once:
 * ``ask(n_points=k)`` uses skopt's constant-liar "cl_min" strategy: k sequential asks with the lie y = min(y).
 * ``base_estimator`` "RF" / "ET" use skopt's forests (``kubeflow_b200.forest.ForestEngine``: fit and sweep on the GPU, raw y, no
   θ), refit whenever the history changes — every lie included — and swept over the same candidates, shards, gp_hedge and
-  constant liar as the GP.  Their seed is fixed when the engine is made.  GBRT is not served.
+  constant liar as the GP.  Their seed is fixed when the engine is made.
+* GBRT is served when ``base_estimator`` is a ``kubeflow_b200.gbrt.GbrtEngine`` **instance**, the way skopt's ``gbrt_minimize``
+  passes a ``GradientBoostingQuantileRegressor`` instance; it takes the forests' path (raw y, a refit for every lie, gp_hedge,
+  shards) and stays the caller's: ``close()`` does not close it.  The string ``"GBRT"`` is refused.
 
 ``acq_func="gp_hedge"`` (Katib's and skopt's default) is skopt's portfolio: every model-based ask sweeps ONE candidate set
 for EI, LCB and PI together (``GPEngine.ask_multi``: one posterior, three first-index argmaxes), keeps the three picks, and
@@ -62,12 +65,19 @@ class Optimizer:
                  random_state=None, *, n_points=65536, kernel="matern52", length_scale=None, amplitude=1.0, noise=1e-3, xi=0.01,
                  kappa=1.96, var_mode="auto", theta_grid=1, theta_search=0, theta_fit=None, theta_fit_maxiter=None, theta_restarts=None, ard=False,
                  device=0, engine=None, candidate_backend="torch", incremental=True, shard=False):
-        self.base_estimator = str(base_estimator).upper()
-        if self.base_estimator not in ("GP",) + FOREST_ESTIMATORS:
-            raise ValueError("base_estimator must be GP, RF or ET (GBRT is not part of the GPU path)")
-        self.forest = self.base_estimator in FOREST_ESTIMATORS
+        self._gbrt = None             # a GbrtEngine passed as base_estimator (owned by the caller)
+        if isinstance(base_estimator, str):
+            self.base_estimator = base_estimator.upper()
+            if self.base_estimator not in ("GP",) + FOREST_ESTIMATORS:
+                raise ValueError("base_estimator must be GP, RF or ET, or a kubeflow_b200.gbrt.GbrtEngine instance for GBRT")
+        else:
+            from .gbrt import GbrtEngine
+            if not isinstance(base_estimator, GbrtEngine):
+                raise ValueError(f"base_estimator must be GP, RF, ET or a GbrtEngine instance, got {type(base_estimator).__name__}")
+            self._gbrt, self.base_estimator = base_estimator, "GBRT"
+        self.forest = self.base_estimator in FOREST_ESTIMATORS + ("GBRT",)   # the tree path: raw y, refit on every change
         if self.forest and acq_optimizer == "lbfgs":
-            name = "RandomForestRegressor" if self.base_estimator == "RF" else "ExtraTreesRegressor"
+            name = {"RF": "RandomForestRegressor", "ET": "ExtraTreesRegressor", "GBRT": "GradientBoostingQuantileRegressor"}[self.base_estimator]
             raise ValueError(f"The regressor {name} should run with acq_optimizer='sampling'.")
         self.space = dimensions if isinstance(dimensions, Space) else Space(dimensions)
         self.n_initial_points = int(n_initial_points)
@@ -147,8 +157,9 @@ class Optimizer:
         self.last_best = None
 
     def close(self):
-        """Release the GP or forest engine (its libkbo handle and device memory); a later ask makes a fresh one."""
-        if self._engine is not None:
+        """Release the GP or forest engine (its libkbo handle and device memory); a later ask makes a fresh one.  A GbrtEngine
+        passed as base_estimator is the caller's and stays open."""
+        if self._engine is not None and self._engine is not self._gbrt:
             self._engine.close()
             self._engine = None
         self._fit_state = None
@@ -258,7 +269,12 @@ class Optimizer:
         return base if prev is None else base - eng.predict_mean(prev)
 
     def _get_forest(self):
-        """The RF / ET engine, made on first use with a seed fixed for its lifetime: the same history gives the same forest."""
+        """The RF / ET engine, made on first use with a seed fixed for its lifetime: the same history gives the same forest; or
+        the GbrtEngine passed as base_estimator, set to this optimizer's acquisition."""
+        if self._gbrt is not None:
+            self._engine = g = self._gbrt
+            g.acq, g.xi, g.kappa = self.acq, self.xi, self.kappa
+            return g
         from .forest import ForestEngine
         if self._engine is None:
             seed = int(self._seed) if self._seed is not None else int(self.rng.integers(0, 2 ** 31))

@@ -87,6 +87,12 @@ for _kind in ("RF", "ET"):
     print(fe.ask_multi(_r.random((5000, 5)), ["ei", "lcb", "pi"])[0], fe.predict(_r.random((3, 5)))[0].tolist(),
           len(fe.export(0, with_draws=_kind == "ET")["left"]))
     fe.close()
+from kubeflow_b200.gbrt import GbrtEngine           # GBRT: init, presort, the three-chain fit, staged sweep and predict, export
+ge = GbrtEngine()
+ge.tell(_r.random((300, 5)), _r.random(300))
+print(ge.ask_multi(_r.random((5000, 5)), ["ei", "lcb", "pi"])[0], ge.predict(_r.random((3, 5)), return_std=True)[1].tolist(),
+      len(ge.export(2, 29)["left"]))
+ge.close()
 from kubeflow_b200.enas import EnasController        # ENAS: init, the one-CTA train chain (drawn and imposed arcs), batched draws
 en = EnasController(5, 12, 9, seed=2)
 print(en.sample(6).tolist(), en.train(0.5, 3)[:, 0].tolist())
