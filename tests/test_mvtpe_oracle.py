@@ -196,3 +196,47 @@ def test_torch_restatement_matches_the_oracle(big):
     ref = O.score(space, md, C)
     got = R.score(space, md, torch.tensor(C), chunk=512).numpy()
     np.testing.assert_allclose(got, ref, rtol=0, atol=(1e-9 if big else 1e-11) * (1 + np.abs(ref).max()))
+
+
+@pytest.mark.parametrize("big", [False, True])
+def test_tolerance_covers_the_restatement_against_the_oracle(big):
+    """_mvtpe_ref.tol, the distance two correct FP64 evaluations of a score can lie apart, covers this restatement against the
+    NumPy oracle for every candidate: mixed spaces of 4 and 5 parameters (the second with a 2^18-level integer, whose tail
+    bins are the worst conditioned) and a 40-float space, with candidates at observations and on the bounds.  It is no more
+    than 1e-8 anywhere, so a pick check under it still tells scores apart."""
+    import torch
+    from tests import _mvtpe_ref as R
+    r = np.random.default_rng(19)
+    for space in ([("float", -1.0, 3.0), ("int", 0, 19, 1), ("cat", 5), ("float", 0.0, 1.0)] + ([("int", 0, (1 << 18) - 1, 1)] if big else []),
+                  [("float", 0.0, 1e-3), ("float", -1e6, 1e6), ("int", 3, 48, 5), ("cat", 64)] * (10 if big else 1)):
+        X = np.stack([O.round_int(p, r.uniform(p[1], p[2], 400)) if p[0] == "int" else
+                      r.integers(0, p[1], 400).astype(float) if p[0] == "cat" else r.uniform(p[1], p[2], 400) for p in space], axis=1)
+        md = O.build_models(space, X, r.random(400))
+        C = O.draw(space, md, 2000, r)
+        C[:5] = X[:5]
+        for d, p in enumerate(space[:4]):
+            C[5 + d, d] = p[1] if p[0] != "cat" else p[1] - 1
+        ref = O.score(space, md, C)
+        s, T = R.score_tol(space, md, torch.tensor(C), chunk=512)
+        err, T = np.abs(s.numpy() - ref), T.numpy()
+        assert (err <= T).all(), (len(space), float(np.max(err / T)))
+        assert T.max() < 1e-8 and np.array_equal(T, R.tol(space, md, torch.tensor(C), chunk=512).numpy())
+
+
+def test_pick_check_accepts_ties_and_rejects_gaps():
+    """_mvtpe_ref.pick_ok: within the tolerances a pick may be any candidate, at its first occurrence; past them only the
+    first occurrence of the maximum."""
+    import torch
+    from tests import _mvtpe_ref as R
+    C = torch.tensor([[0.0, 1.0], [1.0, 0.0], [2.0, 0.0], [3.0, 3.0], [1.0, 0.0]], dtype=torch.float64)
+    T = torch.full((5,), 1e-10, dtype=torch.float64)
+    tie = torch.tensor([0.0, 1.0, 1.0 + 1.5e-10, 0.5, 1.0], dtype=torch.float64)      # 1 and 2 closer than T1 + T2
+    assert R.pick_ok(C, tie, T, 2)[0] and R.pick_ok(C, tie, T, 1)[0]
+    ok, _, keys = R.pick_ok(C, tie, T, 4)                             # a copy of 1 after its first occurrence
+    assert not ok and keys == 2
+    assert not R.pick_ok(C, tie, T, 3)[0] and not R.pick_ok(C, tie, T, 0)[0]
+    gap = torch.tensor([0.0, 1.0, 1.0 + 2.5e-10, 0.5, 1.0], dtype=torch.float64)      # 2 wins by more than T1 + T2
+    assert R.pick_ok(C, gap, T, 2)[0] and not R.pick_ok(C, gap, T, 1)[0]
+    dup = torch.tensor([0.0, 1.0, 0.5, 0.5, 1.0], dtype=torch.float64)               # the best twice: the first copy
+    ok, _, keys = R.pick_ok(C, dup, T, 1)
+    assert ok and keys == 1 and not R.pick_ok(C, dup, T, 4)[0]
