@@ -27,11 +27,7 @@
 #include <algorithm>
 #include <vector>
 
-#include <cub/device/device_segmented_radix_sort.cuh>
-
-#include "kbo_internal.cuh"
 #include "kbo_rng.cuh"
-#include "kbo_acq.cuh"
 #include "kbo_tree.cuh"
 
 #define FOREST_FIT_THREADS 1024
@@ -40,43 +36,23 @@
 #define FOREST_MAX_D 1024
 #define FOREST_MAX_T 1024
 
-struct ForestPart;
-
-struct kbo_forest {
+struct kbo_forest : TreeCore {
   int kind = 0, T = 0, msl = 3;
   uint64_t seed = 0;
-  int N = 0, D = 0, n_cap = 0;       // fitted history; node capacity per tree
-  bool fitted = false;
-  DevBuf<float> X;
-  DevBuf<double> y;
-  DevBuf<int> cnt, order, order_in, seg;
-  DevBuf<uint32_t> keys, keys2;
-  DevBuf<unsigned char> sort_tmp;
-  DevBuf<int> cols, tmp, nstart, nend, flag;
+  int n_cap = 0;                     // node capacity per tree
+  DevBuf<int> cnt;
+  DevBuf<int> cols, tmp, nstart, nend;
   DevBuf<unsigned char> side;
   DevBuf<int> feat, left, right, nns, nnodes, nleaves;
   DevBuf<double> thr, value, imp, wn;
   DevBuf<unsigned char> blob;
   DevBuf<long long> tree_off;
-  DevBuf<ForestPart> part;
   DevBuf<uint32_t> ex_mn, ex_mx;
   std::vector<int> h_nnodes, h_nleaves;
   std::vector<long long> h_off;
   size_t max_tree_bytes = 0;
-  float last_ms[2] = {0.f, 0.f};     // fit, sweep
-  EventSet<4> ev;
 };
 
-struct ForestPart {
-  double v;
-  long long i;
-  double mu, sd;
-};
-
-__device__ __forceinline__ uint32_t f32_key(float x) {   // order-preserving map of a float to uint32
-  const uint32_t u = __float_as_uint(x);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 __device__ __forceinline__ float key_f32(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }
 
 // NumPy's random_standard_uniform from two 32-bit words: (a >> 5, b >> 6) → 53 bits / 2^53.
@@ -91,7 +67,7 @@ __device__ __forceinline__ double et_threshold(uint64_t seed, int t, int node, i
   return th;
 }
 
-// ---- bootstrap counts, presort ------------------------------------------------------------------------------------------
+// ---- bootstrap counts --------------------------------------------------------------------------------------------------
 __global__ void forest_bootstrap_kernel(int* __restrict__ cnt, int N, uint64_t seed) {
   const int t = blockIdx.y, d = blockIdx.x * blockDim.x + threadIdx.x;
   if (d >= N) return;
@@ -99,25 +75,6 @@ __global__ void forest_bootstrap_kernel(int* __restrict__ cnt, int N, uint64_t s
   philox4x32_10((uint32_t)d, (uint32_t)t, 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), r);
   const int i = (int)(((uint64_t)r[0] * (uint64_t)N) >> 32);
   atomicAdd(&cnt[(size_t)t * N + i], 1);
-}
-
-__global__ void forest_check_kernel(const float* __restrict__ X, const double* __restrict__ y, int N, int D, int* __restrict__ bad) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < N && !isfinite(y[i])) atomicOr(bad, 1);
-  if (i < (int64_t)N * D && !isfinite(X[i])) atomicOr(bad, 2);
-}
-
-__global__ void forest_keys_kernel(const float* __restrict__ X, int N, int D, uint32_t* __restrict__ keys, int* __restrict__ idx) {
-  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // e = f·N + i: column-major keys
-  if (e >= (int64_t)N * D) return;
-  const int f = (int)(e / N), i = (int)(e % N);
-  keys[e] = f32_key(X[(size_t)i * D + f]);
-  idx[e] = i;
-}
-
-__global__ void forest_seg_kernel(int* __restrict__ seg, int N, int D) {
-  const int f = blockIdx.x * blockDim.x + threadIdx.x;
-  if (f <= D) seg[f] = f * N;
 }
 
 // ---- fit -----------------------------------------------------------------------------------------------------------------
@@ -456,7 +413,7 @@ struct SweepArgs {
   double yopt, xi, kappa;
   double* mu_out;
   double* sd_out;
-  ForestPart* part;
+  kbo_best* part;
 };
 
 template <int CPT, bool STAGED>
@@ -464,8 +421,7 @@ __global__ void __launch_bounds__(256) forest_sweep_kernel(SweepArgs a) {
   extern __shared__ int4 smem[];
   const int tid = threadIdx.x;
   const int64_t ntiles = (a.M + 256 * CPT - 1) / (256 * CPT);
-  double bv[3] = {-INFINITY, -INFINITY, -INFINITY}, bmu[3] = {0, 0, 0}, bsd[3] = {0, 0, 0};
-  long long bi[3] = {0x7fffffffffffffffLL, 0x7fffffffffffffffLL, 0x7fffffffffffffffLL};
+  TreeArgmax best;
   const int acqs[3] = {a.acq0, a.acq1, a.acq2};
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
     int64_t m[CPT];
@@ -532,67 +488,11 @@ __global__ void __launch_bounds__(256) forest_sweep_kernel(SweepArgs a) {
       for (int q = 0; q < 3; q++) {
         if (q >= a.n_acq) break;
         double mo, so;
-        const double v = acq_value<double>(mu, s2, acqs[q], 0.0, 1.0, a.yopt, a.xi, a.kappa, &mo, &so);
-        if (v > bv[q]) {   // indices only grow inside a thread: the first maximum stays
-          bv[q] = v;
-          bi[q] = m[c];
-          bmu[q] = mu;
-          bsd[q] = sd;
-        }
+        best.keep(q, acq_value<double>(mu, s2, acqs[q], 0.0, 1.0, a.yopt, a.xi, a.kappa, &mo, &so), m[c], mu, sd);
       }
     }
   }
-  if (a.n_acq == 0) return;
-  __shared__ ForestPart sp[3][8];
-#pragma unroll
-  for (int q = 0; q < 3; q++) {
-    if (q >= a.n_acq) break;
-    double v = bv[q], mu = bmu[q], sd = bsd[q];
-    long long i = bi[q];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double ov = __shfl_xor_sync(0xffffffffu, v, o), omu = __shfl_xor_sync(0xffffffffu, mu, o), osd = __shfl_xor_sync(0xffffffffu, sd, o);
-      const long long oi = __shfl_xor_sync(0xffffffffu, i, o);
-      if (better(ov, oi, v, i)) {
-        v = ov;
-        i = oi;
-        mu = omu;
-        sd = osd;
-      }
-    }
-    if ((tid & 31) == 0) sp[q][tid >> 5] = ForestPart{v, i, mu, sd};
-  }
-  __syncthreads();
-  if (tid < a.n_acq) {
-    ForestPart b = sp[tid][0];
-    for (int w = 1; w < 8; w++)
-      if (better(sp[tid][w].v, sp[tid][w].i, b.v, b.i)) b = sp[tid][w];
-    a.part[(size_t)blockIdx.x * 3 + tid] = b;
-  }
-}
-
-__global__ void forest_reduce_kernel(const ForestPart* __restrict__ part, int nblocks, int n_acq, int64_t goff, kbo_best* __restrict__ best) {
-  const int q = blockIdx.x;
-  ForestPart b{-INFINITY, 0x7fffffffffffffffLL, 0.0, 0.0};
-  for (int k = threadIdx.x; k < nblocks; k += 32) {
-    const ForestPart& p = part[(size_t)k * 3 + q];
-    if (better(p.v, p.i, b.v, b.i)) b = p;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    ForestPart o2;
-    o2.v = __shfl_xor_sync(0xffffffffu, b.v, o);
-    o2.i = __shfl_xor_sync(0xffffffffu, b.i, o);
-    o2.mu = __shfl_xor_sync(0xffffffffu, b.mu, o);
-    o2.sd = __shfl_xor_sync(0xffffffffu, b.sd, o);
-    if (better(o2.v, o2.i, b.v, b.i)) b = o2;
-  }
-  if (threadIdx.x == 0 && q < n_acq) {
-    best[q].value = b.v;
-    best[q].index = goff + b.i;
-    best[q].mu = b.mu;
-    best[q].std = b.sd;
-  }
+  best.write(a.n_acq, a.part);
 }
 
 // ---- export: the per-node min / max of each feature over the node's samples, to restate the ET draws --------------------
@@ -687,24 +587,10 @@ int kbo_forest_fit(kbo_handle* h, kbo_forest* f, const float* X, const double* y
   if (counts && f->kind != KBO_FOREST_RF) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_fit: bootstrap counts are for RF forests only");
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
-  f->fitted = false;
+  KBO_TRY(tree_fit_begin(h, f, X, y, N, D, "kbo_forest_fit", s));
   const int T = f->T;
   const bool rf = f->kind == KBO_FOREST_RF;
   const size_t ND = (size_t)N * D;
-  KBO_TRY(kbo_reserve(h, f->X, ND));
-  KBO_TRY(kbo_reserve(h, f->y, (size_t)N));
-  KBO_TRY(kbo_reserve(h, f->flag, 1));
-  KBO_CUDA(h, cudaEventRecord(f->ev[0], s));
-  KBO_CUDA(h, kbo_copy(f->X.p, X, ND, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, kbo_copy(f->y.p, y, (size_t)N, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, cudaMemsetAsync(f->flag.p, 0, sizeof *f->flag.p, s));
-  forest_check_kernel<<<(unsigned)((ND + 255) / 256), 256, 0, s>>>(f->X.p, f->y.p, N, D, f->flag.p);
-  KBO_LAUNCH_CHECK(h);
-  int bad = 0;
-  KBO_CUDA(h, kbo_copy(&bad, f->flag.p, 1, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));
-  if (bad & 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_fit: y contains NaN or infinity");
-  if (bad & 2) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_fit: X contains NaN or infinity");
   if (rf) {
     KBO_TRY(kbo_reserve(h, f->cnt, (size_t)T * N));
     if (counts) {
@@ -714,23 +600,7 @@ int kbo_forest_fit(kbo_handle* h, kbo_forest* f, const float* X, const double* y
       forest_bootstrap_kernel<<<dim3((N + 255) / 256, T), 256, 0, s>>>(f->cnt.p, N, f->seed);
       KBO_LAUNCH_CHECK(h);
     }
-    // presort every column once: stable segmented radix sort of (order-preserving key, sample index)
-    KBO_TRY(kbo_reserve(h, f->keys, ND));
-    KBO_TRY(kbo_reserve(h, f->keys2, ND));
-    KBO_TRY(kbo_reserve(h, f->order_in, ND));
-    KBO_TRY(kbo_reserve(h, f->order, ND));
-    KBO_TRY(kbo_reserve(h, f->seg, (size_t)(D + 1)));
-    forest_keys_kernel<<<(unsigned)((ND + 255) / 256), 256, 0, s>>>(f->X.p, N, D, f->keys.p, f->order_in.p);
-    KBO_LAUNCH_CHECK(h);
-    forest_seg_kernel<<<(D + 1 + 255) / 256, 256, 0, s>>>(f->seg.p, N, D);
-    KBO_LAUNCH_CHECK(h);
-    size_t tb = 0;
-    const int* seg = f->seg.p;
-    KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb, f->keys.p, f->keys2.p, f->order_in.p,
-                                                         f->order.p, (int)ND, D, seg, seg + 1, 0, 32, s));
-    KBO_TRY(kbo_reserve(h, f->sort_tmp, std::max<size_t>(tb, 16)));
-    KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(f->sort_tmp.p, tb, f->keys.p, f->keys2.p, f->order_in.p,
-                                                         f->order.p, (int)ND, D, seg, seg + 1, 0, 32, s));
+    KBO_TRY(tree_presort(h, f, N, D, s));
   }
   // node capacity: every leaf holds >= min_samples_leaf samples (or is the root)
   const int cap = 2 * std::max(1, N / f->msl) + 1;
@@ -784,52 +654,24 @@ int kbo_forest_fit(kbo_handle* h, kbo_forest* f, const float* X, const double* y
                                         f->imp.p, f->nnodes.p, f->nleaves.p, cap,
                                         f->tree_off.p, f->blob.p);
   KBO_LAUNCH_CHECK(h);
-  KBO_CUDA(h, cudaEventRecord(f->ev[1], s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));   // the host copy of tree_off must outlive its transfer
-  KBO_CUDA(h, cudaEventElapsedTime(&f->last_ms[0], f->ev[0], f->ev[1]));
-  f->N = N;
-  f->D = D;
-  f->fitted = true;
-  return KBO_OK;
+  return tree_fit_end(h, f, N, D, s);   // synchronises: the host copy of tree_off must outlive its transfer
 }
 
 int kbo_forest_sweep(kbo_handle* h, kbo_forest* f, const float* Xc, int64_t M, int64_t global_offset, int32_t n_acq, const int32_t* acqs, double y_opt,
                      double xi, double kappa, kbo_best* best_dev, double* mu_out, double* sigma_out, void* stream) {
   if (!h || !f || !Xc) return KBO_ERR_INVALID;
-  if (!f->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_forest_sweep: the forest is not fitted");
-  if (M < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_sweep: M must be >= 1 (got %lld)", (long long)M);
-  if (n_acq < 0 || n_acq > 3 || (n_acq > 0 && (!acqs || !best_dev))) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_sweep: 0 <= n_acq <= 3 with acqs and best_dev");
-  for (int i = 0; i < n_acq; i++) {
-    if (acqs[i] < KBO_ACQ_EI || acqs[i] > KBO_ACQ_PI) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_sweep: unknown acquisition %d", acqs[i]);
-    for (int j = 0; j < i; j++)
-      if (acqs[j] == acqs[i]) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_sweep: acquisition %d given twice", acqs[i]);
-  }
-  if (!std::isfinite(y_opt)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_forest_sweep: y_opt must be finite");
   cudaStream_t s = (cudaStream_t)stream;
-  KBO_CUDA(h, cudaSetDevice(h->device));
-  KBO_CUDA(h, cudaEventRecord(f->ev[2], s));
+  KBO_TRY(tree_sweep_begin(h, f, M, n_acq, acqs, y_opt, best_dev, "kbo_forest_sweep", "the forest", s));
   int nb = 0;
   KBO_TRY(forest_sweep_launch(h, f, Xc, M, n_acq, acqs, y_opt, xi, kappa, mu_out, sigma_out, &nb, s));
-  if (n_acq > 0) {
-    forest_reduce_kernel<<<n_acq, 32, 0, s>>>(f->part.p, nb, n_acq, global_offset, best_dev);
-    KBO_LAUNCH_CHECK(h);
-  }
-  KBO_CUDA(h, cudaEventRecord(f->ev[3], s));
-  return KBO_OK;
+  return tree_sweep_end(h, f, nb, n_acq, global_offset, best_dev, s);
 }
 
 int kbo_forest_predict(kbo_handle* h, kbo_forest* f, const float* X, int32_t n, int x_on_host, double* mu_host, double* sigma_host, void* stream) {
   if (!h || !f || !X || n < 1) return KBO_ERR_INVALID;
-  if (!f->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_forest_predict: the forest is not fitted");
   cudaStream_t s = (cudaStream_t)stream;
-  KBO_CUDA(h, cudaSetDevice(h->device));
-  const float* Xd = X;
-  if (x_on_host) {
-    const size_t bytes = (size_t)n * f->D * sizeof(float);
-    KBO_TRY(kbo_reserve(h, h->stage_Xc, bytes));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_Xc.p, X, bytes, cudaMemcpyHostToDevice, s));
-    Xd = kbo_view<float>(h->stage_Xc);
-  }
+  const float* Xd = nullptr;
+  KBO_TRY(tree_predict_rows(h, f, X, n, x_on_host, &Xd, "kbo_forest_predict", "the forest", s));
   KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)n * 2));
   double* mu = h->stage_y.p;
   int nb = 0;
@@ -890,13 +732,6 @@ int kbo_forest_export(kbo_handle* h, kbo_forest* f, int32_t tree, int32_t* featu
   return KBO_OK;
 }
 
-int kbo_forest_last_timings(kbo_handle* h, kbo_forest* f, float* ms, int32_t n) {
-  if (!h || !f) return KBO_ERR_INVALID;
-  float sweep = 0.f;
-  if (cudaEventQuery(f->ev[3]) == cudaSuccess && cudaEventElapsedTime(&sweep, f->ev[2], f->ev[3]) == cudaSuccess) f->last_ms[1] = sweep;
-  cudaGetLastError();
-  for (int i = 0; ms && i < n && i < 2; i++) ms[i] = f->last_ms[i];
-  return 2;
-}
+int kbo_forest_last_timings(kbo_handle* h, kbo_forest* f, float* ms, int32_t n) { return tree_last_timings(h, f, ms, n); }
 
 }  // extern "C"

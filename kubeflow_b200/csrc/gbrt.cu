@@ -27,10 +27,7 @@
 #include <vector>
 
 #include <cub/device/device_radix_sort.cuh>
-#include <cub/device/device_segmented_radix_sort.cuh>
 
-#include "kbo_internal.cuh"
-#include "kbo_acq.cuh"
 #include "kbo_tree.cuh"
 
 #define GBRT_FIT_THREADS 1024
@@ -42,37 +39,20 @@
 #define GBRT_MAX_D 1024
 #define GBRT_MAX_STAGES 128
 
-struct GbrtPart {
-  double v;
-  long long i;
-  double mu, sd;
-};
-
-struct kbo_gbrt {
+struct kbo_gbrt : TreeCore {
   int S = 30;
   double alpha[GBRT_CHAINS] = {0.16, 0.5, 0.84};
-  int N = 0, D = 0;
-  bool fitted = false;
-  DevBuf<float> X;
-  DevBuf<double> y, ysort, raw, alpha_dev, init;
-  DevBuf<uint32_t> keys, keys2;
-  DevBuf<int> order_in, order, seg, cols, tmp, flag;
-  DevBuf<unsigned char> pos, side, leaf, sort_tmp;
+  DevBuf<double> ysort, raw, alpha_dev, init;
+  DevBuf<int> cols, tmp;
+  DevBuf<unsigned char> pos, side, leaf, ysort_tmp;
   DevBuf<unsigned long long> rkey;
   // per (chain, stage, slot): the tree in heap layout (export) and the packed model (sweep)
   DevBuf<int> feat, nn, np_;
   DevBuf<double> thr, value, mval;
   DevBuf<uint2> mnode;
-  DevBuf<GbrtPart> part;
   double h_init[GBRT_CHAINS] = {0.0, 0.0, 0.0};
-  float last_ms[2] = {0.f, 0.f};     // fit, sweep
-  EventSet<4> ev;
 };
 
-__device__ __forceinline__ uint32_t gbrt_f32_key(float x) {   // order-preserving map of a float to uint32
-  const uint32_t u = __float_as_uint(x);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
 __device__ __forceinline__ unsigned long long gbrt_f64_key(double x) {   // order-preserving, -0.0 taken as +0.0
   const unsigned long long u = (unsigned long long)__double_as_longlong(x == 0.0 ? 0.0 : x);
   return (u >> 63) ? ~u : (u | 0x8000000000000000ull);
@@ -81,23 +61,7 @@ __device__ __forceinline__ double gbrt_key_f64(unsigned long long k) {
   return __longlong_as_double((long long)((k >> 63) ? (k & 0x7FFFFFFFFFFFFFFFull) : ~k));
 }
 
-// ---- checks, presort, init ------------------------------------------------------------------------------------------------
-__global__ void gbrt_check_kernel(const float* __restrict__ X, const double* __restrict__ y, int N, int D, int* __restrict__ bad) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < N && !isfinite(y[i])) atomicOr(bad, 1);
-  if (i < (int64_t)N * D && !isfinite(X[i])) atomicOr(bad, 2);
-}
-
-__global__ void gbrt_keys_kernel(const float* __restrict__ X, int N, int D, uint32_t* __restrict__ keys, int* __restrict__ idx,
-                                 int* __restrict__ seg) {
-  const int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;   // e = f·N + i: column-major keys
-  if (e <= D) seg[e] = (int)e * N;
-  if (e >= (int64_t)N * D) return;
-  const int f = (int)(e / N), i = (int)(e % N);
-  keys[e] = gbrt_f32_key(X[(size_t)i * D + f]);
-  idx[e] = i;
-}
-
+// ---- init -------------------------------------------------------------------------------------------------------------------
 // np.percentile(y, 100·α) with the linear rule (numpy/lib/_function_base_impl.py _quantile / _lerp): virtual index (n − 1)·q,
 // q = fl(100·α) / 100; γ its fractional part; a + (b − a)·γ, or b − (b − a)·(1 − γ) where γ >= 0.5; the last value past n − 1.
 __global__ void gbrt_init_kernel(const double* __restrict__ ys, int N, const double* __restrict__ alpha, double* __restrict__ init) {
@@ -370,7 +334,7 @@ struct GbrtSweepArgs {
   double* mu_out;
   double* sd_out;
   double* q_out;         // 3 × M chain predictions
-  GbrtPart* part;
+  kbo_best* part;
 };
 
 // ACQ = false (predict): the chain sums alone, so the instance's SASS shows they are never contracted into a DFMA.
@@ -387,8 +351,7 @@ __global__ void __launch_bounds__(256) gbrt_sweep_kernel(GbrtSweepArgs a) {
     nodes[i] = a.mnode[i];
   }
   const double init0 = a.init[0], init1 = a.init[1], init2 = a.init[2];
-  double bv[3] = {-INFINITY, -INFINITY, -INFINITY}, bmu[3] = {0, 0, 0}, bsd[3] = {0, 0, 0};
-  long long bi[3] = {0x7fffffffffffffffLL, 0x7fffffffffffffffLL, 0x7fffffffffffffffLL};
+  TreeArgmax best;
   const int acqs[3] = {a.acq0, a.acq1, a.acq2};
   const int64_t ntiles = (a.M + 255) / 256;
   for (int64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
@@ -436,69 +399,11 @@ __global__ void __launch_bounds__(256) gbrt_sweep_kernel(GbrtSweepArgs a) {
 #pragma unroll
       for (int qq = 0; qq < 3; qq++) {
         if (qq >= a.n_acq) break;
-        const double v = acq_of_sd<double>(mu, sd, acqs[qq], a.yopt, a.xi, a.kappa);
-        if (v > bv[qq]) {   // indices only grow inside a thread: the first maximum stays
-          bv[qq] = v;
-          bi[qq] = m;
-          bmu[qq] = mu;
-          bsd[qq] = sd;
-        }
+        best.keep(qq, acq_of_sd<double>(mu, sd, acqs[qq], a.yopt, a.xi, a.kappa), m, mu, sd);
       }
     }
   }
-  if constexpr (ACQ) {   // the per-CTA first-index argmax of each acquisition
-    if (a.n_acq == 0) return;
-    __shared__ GbrtPart sp[3][8];
-#pragma unroll
-    for (int qq = 0; qq < 3; qq++) {
-      if (qq >= a.n_acq) break;
-      double v = bv[qq], mu = bmu[qq], sd = bsd[qq];
-      long long i = bi[qq];
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const double ov = __shfl_xor_sync(0xffffffffu, v, o), omu = __shfl_xor_sync(0xffffffffu, mu, o), osd = __shfl_xor_sync(0xffffffffu, sd, o);
-        const long long oi = __shfl_xor_sync(0xffffffffu, i, o);
-        if (better(ov, oi, v, i)) {
-          v = ov;
-          i = oi;
-          mu = omu;
-          sd = osd;
-        }
-      }
-      if ((tid & 31) == 0) sp[qq][tid >> 5] = GbrtPart{v, i, mu, sd};
-    }
-    __syncthreads();
-    if (tid < a.n_acq) {
-      GbrtPart b = sp[tid][0];
-      for (int w = 1; w < 8; w++)
-        if (better(sp[tid][w].v, sp[tid][w].i, b.v, b.i)) b = sp[tid][w];
-      a.part[(size_t)blockIdx.x * 3 + tid] = b;
-    }
-  }
-}
-
-__global__ void gbrt_reduce_kernel(const GbrtPart* __restrict__ part, int nblocks, int n_acq, int64_t goff, kbo_best* __restrict__ best) {
-  const int q = blockIdx.x;
-  GbrtPart b{-INFINITY, 0x7fffffffffffffffLL, 0.0, 0.0};
-  for (int k = threadIdx.x; k < nblocks; k += 32) {
-    const GbrtPart& p = part[(size_t)k * 3 + q];
-    if (better(p.v, p.i, b.v, b.i)) b = p;
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    GbrtPart o2;
-    o2.v = __shfl_xor_sync(0xffffffffu, b.v, o);
-    o2.i = __shfl_xor_sync(0xffffffffu, b.i, o);
-    o2.mu = __shfl_xor_sync(0xffffffffu, b.mu, o);
-    o2.sd = __shfl_xor_sync(0xffffffffu, b.sd, o);
-    if (better(o2.v, o2.i, b.v, b.i)) b = o2;
-  }
-  if (threadIdx.x == 0 && q < n_acq) {
-    best[q].value = b.v;
-    best[q].index = goff + b.i;
-    best[q].mu = b.mu;
-    best[q].std = b.sd;
-  }
+  if constexpr (ACQ) best.write(a.n_acq, a.part);
 }
 
 // ---- C ABI ------------------------------------------------------------------------------------------------------------------
@@ -561,44 +466,18 @@ int kbo_gbrt_fit(kbo_handle* h, kbo_gbrt* g, const float* X, const double* y, in
   if (D < 1 || D > GBRT_MAX_D) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_fit: 1 <= D <= %d (got %d)", GBRT_MAX_D, D);
   cudaStream_t s = (cudaStream_t)stream;
   KBO_CUDA(h, cudaSetDevice(h->device));
-  g->fitted = false;
+  KBO_TRY(tree_fit_begin(h, g, X, y, N, D, "kbo_gbrt_fit", s));
   const size_t ND = (size_t)N * D;
-  KBO_TRY(kbo_reserve(h, g->X, ND));
-  KBO_TRY(kbo_reserve(h, g->y, (size_t)N));
-  KBO_TRY(kbo_reserve(h, g->flag, 1));
-  KBO_CUDA(h, cudaEventRecord(g->ev[0], s));
-  KBO_CUDA(h, kbo_copy(g->X.p, X, ND, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, kbo_copy(g->y.p, y, (size_t)N, cudaMemcpyDeviceToDevice, s));
-  KBO_CUDA(h, cudaMemsetAsync(g->flag.p, 0, sizeof *g->flag.p, s));
-  gbrt_check_kernel<<<(unsigned)((ND + 255) / 256), 256, 0, s>>>(g->X.p, g->y.p, N, D, g->flag.p);
-  KBO_LAUNCH_CHECK(h);
-  int bad = 0;
-  KBO_CUDA(h, kbo_copy(&bad, g->flag.p, 1, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));
-  if (bad & 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_fit: y contains NaN or infinity");
-  if (bad & 2) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_fit: X contains NaN or infinity");
   // init: y sorted once, the linear percentile per chain
   KBO_TRY(kbo_reserve(h, g->ysort, (size_t)N));
   KBO_TRY(kbo_reserve(h, g->init, GBRT_CHAINS));
-  size_t tb = 0, tb2 = 0;
+  size_t tb = 0;
   KBO_CUDA(h, cub::DeviceRadixSort::SortKeys(nullptr, tb, g->y.p, g->ysort.p, N, 0, 64, s));
-  // presort every column once: stable segmented radix sort of (order-preserving key, row index)
-  KBO_TRY(kbo_reserve(h, g->keys, ND));
-  KBO_TRY(kbo_reserve(h, g->keys2, ND));
-  KBO_TRY(kbo_reserve(h, g->order_in, ND));
-  KBO_TRY(kbo_reserve(h, g->order, ND));
-  KBO_TRY(kbo_reserve(h, g->seg, (size_t)(D + 1)));
-  const int* seg = g->seg.p;
-  KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(nullptr, tb2, g->keys.p, g->keys2.p, g->order_in.p, g->order.p, (int)ND, D, seg,
-                                                       seg + 1, 0, 32, s));
-  KBO_TRY(kbo_reserve(h, g->sort_tmp, std::max<size_t>(std::max(tb, tb2), 16)));
-  KBO_CUDA(h, cub::DeviceRadixSort::SortKeys(g->sort_tmp.p, tb, g->y.p, g->ysort.p, N, 0, 64, s));
+  KBO_TRY(kbo_reserve(h, g->ysort_tmp, std::max<size_t>(tb, 16)));
+  KBO_CUDA(h, cub::DeviceRadixSort::SortKeys(g->ysort_tmp.p, tb, g->y.p, g->ysort.p, N, 0, 64, s));
   gbrt_init_kernel<<<1, 32, 0, s>>>(g->ysort.p, N, g->alpha_dev.p, g->init.p);
   KBO_LAUNCH_CHECK(h);
-  gbrt_keys_kernel<<<(unsigned)((std::max(ND, (size_t)D + 1) + 255) / 256), 256, 0, s>>>(g->X.p, N, D, g->keys.p, g->order_in.p, g->seg.p);
-  KBO_LAUNCH_CHECK(h);
-  KBO_CUDA(h, cub::DeviceSegmentedRadixSort::SortPairs(g->sort_tmp.p, tb2, g->keys.p, g->keys2.p, g->order_in.p, g->order.p, (int)ND, D,
-                                                       seg, seg + 1, 0, 32, s));
+  KBO_TRY(tree_presort(h, g, N, D, s));
   const size_t C = GBRT_CHAINS, TS = C * g->S * GBRT_SLOTS;
   KBO_TRY(kbo_reserve(h, g->cols, C * ND));
   KBO_TRY(kbo_reserve(h, g->tmp, C * ND));
@@ -619,53 +498,25 @@ int kbo_gbrt_fit(kbo_handle* h, kbo_gbrt* g, const float* X, const double* y, in
   gbrt_fit_kernel<<<GBRT_CHAINS, GBRT_FIT_THREADS, 0, s>>>(a);
   KBO_LAUNCH_CHECK(h);
   KBO_CUDA(h, kbo_copy(g->h_init, g->init.p, GBRT_CHAINS, cudaMemcpyDeviceToHost, s));
-  KBO_CUDA(h, cudaEventRecord(g->ev[1], s));
-  KBO_CUDA(h, cudaStreamSynchronize(s));
-  KBO_CUDA(h, cudaEventElapsedTime(&g->last_ms[0], g->ev[0], g->ev[1]));
-  g->N = N;
-  g->D = D;
-  g->fitted = true;
-  return KBO_OK;
+  return tree_fit_end(h, g, N, D, s);
 }
 
 int kbo_gbrt_sweep(kbo_handle* h, kbo_gbrt* g, const float* Xc, int64_t M, int64_t global_offset, int32_t n_acq, const int32_t* acqs, double y_opt,
                    double xi, double kappa, kbo_best* best_dev, double* mu_out, double* sigma_out, double* quantiles_out, void* stream) {
   if (!h || !g || !Xc) return KBO_ERR_INVALID;
-  if (!g->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_gbrt_sweep: the model is not fitted");
-  if (M < 1) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_sweep: M must be >= 1 (got %lld)", (long long)M);
-  if (n_acq < 0 || n_acq > 3 || (n_acq > 0 && (!acqs || !best_dev))) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_sweep: 0 <= n_acq <= 3 with acqs and best_dev");
-  for (int i = 0; i < n_acq; i++) {
-    if (acqs[i] < KBO_ACQ_EI || acqs[i] > KBO_ACQ_PI) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_sweep: unknown acquisition %d", acqs[i]);
-    for (int j = 0; j < i; j++)
-      if (acqs[j] == acqs[i]) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_sweep: acquisition %d given twice", acqs[i]);
-  }
-  if (!std::isfinite(y_opt)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_gbrt_sweep: y_opt must be finite");
   cudaStream_t s = (cudaStream_t)stream;
-  KBO_CUDA(h, cudaSetDevice(h->device));
-  KBO_CUDA(h, cudaEventRecord(g->ev[2], s));
+  KBO_TRY(tree_sweep_begin(h, g, M, n_acq, acqs, y_opt, best_dev, "kbo_gbrt_sweep", "the model", s));
   int nb = 0;
   KBO_TRY(gbrt_sweep_launch(h, g, Xc, M, n_acq, acqs, y_opt, xi, kappa, mu_out, sigma_out, quantiles_out, &nb, s));
-  if (n_acq > 0) {
-    gbrt_reduce_kernel<<<n_acq, 32, 0, s>>>(g->part.p, nb, n_acq, global_offset, best_dev);
-    KBO_LAUNCH_CHECK(h);
-  }
-  KBO_CUDA(h, cudaEventRecord(g->ev[3], s));
-  return KBO_OK;
+  return tree_sweep_end(h, g, nb, n_acq, global_offset, best_dev, s);
 }
 
 int kbo_gbrt_predict(kbo_handle* h, kbo_gbrt* g, const float* X, int32_t n, int x_on_host, double* mu_host, double* sigma_host,
                      double* quantiles_host, void* stream) {
   if (!h || !g || !X || n < 1) return KBO_ERR_INVALID;
-  if (!g->fitted) KBO_FAIL(h, KBO_ERR_STATE, "kbo_gbrt_predict: the model is not fitted");
   cudaStream_t s = (cudaStream_t)stream;
-  KBO_CUDA(h, cudaSetDevice(h->device));
-  const float* Xd = X;
-  if (x_on_host) {
-    const size_t bytes = (size_t)n * g->D * sizeof(float);
-    KBO_TRY(kbo_reserve(h, h->stage_Xc, bytes));
-    KBO_CUDA(h, cudaMemcpyAsync(h->stage_Xc.p, X, bytes, cudaMemcpyHostToDevice, s));
-    Xd = kbo_view<float>(h->stage_Xc);
-  }
+  const float* Xd = nullptr;
+  KBO_TRY(tree_predict_rows(h, g, X, n, x_on_host, &Xd, "kbo_gbrt_predict", "the model", s));
   KBO_TRY(kbo_reserve(h, h->stage_y, (size_t)n * 5));
   double* mu = h->stage_y.p;
   int nb = 0;
@@ -723,13 +574,6 @@ int kbo_gbrt_export(kbo_handle* h, kbo_gbrt* g, int32_t chain, int32_t stage, in
   return KBO_OK;
 }
 
-int kbo_gbrt_last_timings(kbo_handle* h, kbo_gbrt* g, float* ms, int32_t n) {
-  if (!h || !g) return KBO_ERR_INVALID;
-  float sweep = 0.f;
-  if (cudaEventQuery(g->ev[3]) == cudaSuccess && cudaEventElapsedTime(&sweep, g->ev[2], g->ev[3]) == cudaSuccess) g->last_ms[1] = sweep;
-  cudaGetLastError();
-  for (int i = 0; ms && i < n && i < 2; i++) ms[i] = g->last_ms[i];
-  return 2;
-}
+int kbo_gbrt_last_timings(kbo_handle* h, kbo_gbrt* g, float* ms, int32_t n) { return tree_last_timings(h, g, ms, n); }
 
 }  // extern "C"

@@ -229,7 +229,8 @@ def predict(trees, X, min_variance=0.0):
 
 
 def acquisition(kind, mu, std, y_opt, xi=0.01, kappa=1.96):
-    """EI / PI (0 where std = 0) and LCB as a value to maximise, -(mu - kappa·std): skopt.acquisition.gaussian_*."""
+    """EI / PI (0 where std <= 0) and LCB as a value to maximise, -(mu - kappa·std) with std as it is (GBRT's may be negative):
+    skopt.acquisition.gaussian_*."""
     mu, std = np.asarray(mu, np.float64), np.asarray(std, np.float64)
     if kind == "lcb":
         return -(mu - kappa * std)

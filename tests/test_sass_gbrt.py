@@ -1,6 +1,7 @@
-"""CPU: the GBRT kernels in the built libkbo.so (cuobjdump -sass; no GPU needed).  No kernel touches local memory; the staged
-sweep reads the model and the candidate tile from shared memory; the predict instances of the sweep — the chain sums alone —
-hold no DFMA, so every stage's fl(0.1·v) is added with a plain DADD as sklearn adds it."""
+"""CPU: the GBRT kernels in the built libkbo.so (cuobjdump -sass; no GPU needed).  No kernel the GBRT path launches touches
+local memory, its own or the tree_*_kernel it shares with the forests (kbo_tree.cuh); the staged sweep reads the model and the
+candidate tile from shared memory; the predict instances of the sweep — the chain sums alone — hold no DFMA, so every stage's
+fl(0.1·v) is added with a plain DADD as sklearn adds it."""
 import re
 import shutil
 import subprocess
@@ -31,9 +32,9 @@ def built():
     build.build()
 
 
-def test_no_gbrt_kernel_uses_local_memory(built):
-    kernels = _ops(r"gbrt_")
-    assert len(kernels) >= 8, sorted(kernels)
+def test_no_gbrt_path_kernel_uses_local_memory(built):
+    kernels = _ops(r"gbrt_|tree_(check|keys|reduce)_kernel")
+    assert len(kernels) == 9, sorted(kernels)      # init, fit, 4 sweep instances; check, keys, reduce
     for name, ops in kernels.items():
         assert not any(o.startswith(("LDL", "STL")) for o in ops), name
 

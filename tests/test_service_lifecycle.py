@@ -122,6 +122,7 @@ def _engines():
     from kubeflow_b200.cmaes import CmaEs
     from kubeflow_b200.enas import EnasController
     from kubeflow_b200.forest import ForestEngine
+    from kubeflow_b200.gbrt import GbrtEngine
     from kubeflow_b200.gp import GPEngine
     from kubeflow_b200.mvtpe import MvTpe
     from kubeflow_b200.tpe import Tpe
@@ -130,6 +131,7 @@ def _engines():
             "mvtpe": lambda: MvTpe([("float", 0.0, 1.0), ("cat", 3)]),
             "cma": lambda: CmaEs(np.zeros(2), 0.5, popsize=4),
             "forest": lambda: ForestEngine(0),
+            "gbrt": lambda: GbrtEngine(0),
             "enas": lambda: EnasController(2, 8, 3)}
 
 
@@ -146,7 +148,7 @@ def fake_cuda(monkeypatch):
     return use
 
 
-@pytest.mark.parametrize("kind", [None, "tpe", "mvtpe", "cma", "forest", "enas"])
+@pytest.mark.parametrize("kind", [None, "tpe", "mvtpe", "cma", "forest", "gbrt", "enas"])
 def test_close_destroys_the_object_then_the_handle_once(fake_cuda, kind):
     lib = fake_cuda(_FakeLib())
     e = _engines()[kind]()
@@ -161,7 +163,7 @@ def test_close_destroys_the_object_then_the_handle_once(fake_cuda, kind):
     assert len(lib.calls) == n
 
 
-@pytest.mark.parametrize("kind", ["tpe", "mvtpe", "cma", "forest", "enas"])
+@pytest.mark.parametrize("kind", ["tpe", "mvtpe", "cma", "forest", "gbrt", "enas"])
 def test_failed_object_create_destroys_the_handle_and_reports_its_error(fake_cuda, kind):
     lib = fake_cuda(_FakeLib(fail=f"kbo_{kind}_create"))
     try:
@@ -173,7 +175,7 @@ def test_failed_object_create_destroys_the_handle_and_reports_its_error(fake_cud
         pytest.fail("no KboError")
 
 
-@pytest.mark.parametrize("kind", ["tpe", "mvtpe", "cma", "forest", "enas"])    # GPEngine's text, now every engine's
+@pytest.mark.parametrize("kind", ["tpe", "mvtpe", "cma", "forest", "gbrt", "enas"])    # GPEngine's text, now every engine's
 def test_failed_kbo_create_has_one_message_and_nothing_to_destroy(fake_cuda, kind):
     lib = fake_cuda(_FakeLib(fail="kbo_create"))
     with pytest.raises(L.KboError, match=r"kbo_create failed \(no usable CUDA device\?\)"):
