@@ -407,7 +407,17 @@ int kbo_sepcma_restart(kbo_handle* h, kbo_sepcma* c, int32_t lambda, const doubl
  *   kbo_tpe_last_survivors: per (point, parameter) of the last ask, the candidates decided in FP64 (continuous) or the
  *                   distinct values scored (quantized, categorical).  Returns k·D, fills up to n entries.
  *   kbo_tpe_last_timings: milliseconds of the last ask's phases (models, FP32 score, FP64 decision, discrete parameters, final
- *                   reduction), CUDA events on its stream.  Returns 5, fills up to n entries. */
+ *                   reduction), CUDA events on its stream.  Returns 5, fills up to n entries.
+ *   kbo_tpe_ask_shard: one shard of an ask sharded over ranks: as kbo_tpe_ask, but only candidates [lo, hi) of n_candidates
+ *                   are drawn (keyed by their global index) and scored; quantized and categorical parameters score the
+ *                   distinct values present in the shard.  Per (point, parameter) it writes the shard's winner to val_dev
+ *                   (k×D fp64, device: its FP64 score) and idx_dev (k×D, device: its global index).  lo == hi is an empty
+ *                   shard, which writes (-inf, n_candidates) and never wins.  The ask counter advances as one kbo_tpe_ask
+ *                   advances it.  cand_dev must be NULL.  Synchronises.  The exchange of (value, index) pairs is the
+ *                   caller's: the first index of the maximum over all shards is the winner one kbo_tpe_ask would pick.
+ *   kbo_tpe_pick  : after a shard ask and before the next tell, the values of the winning global indices idx_dev (k×D,
+ *                   device, each in [0, n_candidates)), regenerated from Philox and quantized as kbo_tpe_ask does, to x_dev
+ *                   (k×D fp64, device).  k must be the shard ask's.  Synchronises. */
 typedef enum kbo_tpe_kind { KBO_TPE_UNIFORM = 0, KBO_TPE_QUNIFORM = 1, KBO_TPE_CHOICE = 2 } kbo_tpe_kind;
 typedef struct kbo_tpe kbo_tpe;
 int kbo_tpe_create(kbo_handle* h, kbo_tpe** out, int32_t D, const int32_t* kinds, const double* lo, const double* hi, const double* q,
@@ -420,6 +430,9 @@ int kbo_tpe_state(kbo_handle* h, kbo_tpe* t, int32_t param, int32_t group, doubl
                   int32_t* ncomp, double* p_accept, int32_t* n_below, void* stream);
 int kbo_tpe_last_survivors(kbo_handle* h, kbo_tpe* t, int32_t* out, int32_t n);
 int kbo_tpe_last_timings(kbo_handle* h, kbo_tpe* t, float* ms, int32_t n);
+int kbo_tpe_ask_shard(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t n_candidates, int32_t lo, int32_t hi, const double* cand_dev,
+                      double* val_dev, int64_t* idx_dev, void* stream);
+int kbo_tpe_pick(kbo_handle* h, kbo_tpe* t, int32_t k, const int64_t* idx_dev, double* x_dev, void* stream);
 
 /* ---- multivariate TPE (Katib algorithm `multivariate-tpe`: Optuna's TPESampler(multivariate=True) on a flat space; FP64
  * restatement oracle/mvtpe_oracle.py) ------------------------------------------------------------------------------------
@@ -446,7 +459,15 @@ int kbo_tpe_last_timings(kbo_handle* h, kbo_tpe* t, float* ms, int32_t n);
  *                   row's entry at its own category and elsewhere; NaN for other kinds), n_obs, n_below.  Synchronises.
  *   kbo_mvtpe_last_survivors: per point of the last ask, the candidates decided in FP64.  Returns k, fills up to n entries.
  *   kbo_mvtpe_last_timings: milliseconds of the last ask's phases (models and draws, FP32 score, FP64 decision, final
- *                   reduction), CUDA events on its stream.  Returns 4, fills up to n entries. */
+ *                   reduction), CUDA events on its stream.  Returns 4, fills up to n entries.
+ *   kbo_mvtpe_ask_shard: one shard of an ask sharded over ranks: as kbo_mvtpe_ask, but only candidates [lo, hi) of
+ *                   n_candidates are drawn (keyed by their global index) and scored.  Per point it writes the shard's winner
+ *                   to val_dev (k fp64, device: its FP64 score) and idx_dev (k, device: its global index).  lo == hi is an
+ *                   empty shard, which writes (-inf, n_candidates) and never wins.  The ask counter advances as one
+ *                   kbo_mvtpe_ask advances it.  cand_dev must be NULL.  Synchronises.
+ *   kbo_mvtpe_pick  : after a shard ask and before the next tell, the vectors of the winning global indices idx_dev (k,
+ *                   device, each in [0, n_candidates)), regenerated from Philox as kbo_mvtpe_ask draws them, to x_dev (k×D
+ *                   fp64, device).  k must be the shard ask's.  Synchronises. */
 typedef enum kbo_mvtpe_kind { KBO_MVTPE_FLOAT = 0, KBO_MVTPE_INT = 1, KBO_MVTPE_CAT = 2 } kbo_mvtpe_kind;
 typedef struct kbo_mvtpe kbo_mvtpe;
 int kbo_mvtpe_create(kbo_handle* h, kbo_mvtpe** out, int32_t D, const int32_t* kinds, const double* lo, const double* hi, const double* q,
@@ -459,6 +480,9 @@ int kbo_mvtpe_state(kbo_handle* h, kbo_mvtpe* t, int32_t group, double* w, doubl
                     int32_t* n_obs, int32_t* n_below, void* stream);
 int kbo_mvtpe_last_survivors(kbo_handle* h, kbo_mvtpe* t, int32_t* out, int32_t n);
 int kbo_mvtpe_last_timings(kbo_handle* h, kbo_mvtpe* t, float* ms, int32_t n);
+int kbo_mvtpe_ask_shard(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t n_candidates, int32_t lo, int32_t hi, const double* cand_dev,
+                        double* val_dev, int64_t* idx_dev, void* stream);
+int kbo_mvtpe_pick(kbo_handle* h, kbo_mvtpe* t, int32_t k, const int64_t* idx_dev, double* x_dev, void* stream);
 
 /* ---- tree forests (Katib algorithm `bayesianoptimization` with base_estimator RF / ET: skopt's RandomForestRegressor /
  * ExtraTreesRegressor surrogates; FP64 restatement oracle/forest_oracle.py) --------------------------------------------------

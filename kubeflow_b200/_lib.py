@@ -63,8 +63,9 @@ EXPORTS = ["kbo_version", "kbo_create", "kbo_destroy", "kbo_last_error", "kbo_se
            "kbo_sepcma_create", "kbo_sepcma_destroy", "kbo_sepcma_ask", "kbo_sepcma_tell", "kbo_sepcma_state", "kbo_sepcma_stop_flags",
            "kbo_sepcma_restart",
            "kbo_tpe_create", "kbo_tpe_destroy", "kbo_tpe_tell", "kbo_tpe_ask", "kbo_tpe_state", "kbo_tpe_last_survivors", "kbo_tpe_last_timings",
+           "kbo_tpe_ask_shard", "kbo_tpe_pick",
            "kbo_mvtpe_create", "kbo_mvtpe_destroy", "kbo_mvtpe_tell", "kbo_mvtpe_ask", "kbo_mvtpe_state", "kbo_mvtpe_last_survivors",
-           "kbo_mvtpe_last_timings",
+           "kbo_mvtpe_last_timings", "kbo_mvtpe_ask_shard", "kbo_mvtpe_pick",
            "kbo_forest_create", "kbo_forest_destroy", "kbo_forest_fit", "kbo_forest_sweep", "kbo_forest_predict", "kbo_forest_export",
            "kbo_forest_last_timings",
            "kbo_gbrt_create", "kbo_gbrt_destroy", "kbo_gbrt_fit", "kbo_gbrt_sweep", "kbo_gbrt_predict", "kbo_gbrt_export",
@@ -186,6 +187,8 @@ def load() -> C.CDLL:
     lib.kbo_tpe_state.argtypes = [vp, vp, i32, i32, vp, vp, vp, i32, vp, vp, vp, vp]
     lib.kbo_tpe_last_survivors.argtypes = [vp, vp, vp, i32]
     lib.kbo_tpe_last_timings.argtypes = [vp, vp, vp, i32]
+    lib.kbo_tpe_ask_shard.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp]
+    lib.kbo_tpe_pick.argtypes = [vp, vp, i32, vp, vp, vp]
     lib.kbo_mvtpe_create.argtypes = [vp, C.POINTER(vp), i32, vp, vp, vp, vp, vp, C.c_uint64]
     lib.kbo_mvtpe_destroy.argtypes = [vp]
     lib.kbo_mvtpe_destroy.restype = None
@@ -194,6 +197,8 @@ def load() -> C.CDLL:
     lib.kbo_mvtpe_state.argtypes = [vp, vp, i32, vp, vp, vp, vp, i32, vp, vp, vp]
     lib.kbo_mvtpe_last_survivors.argtypes = [vp, vp, vp, i32]
     lib.kbo_mvtpe_last_timings.argtypes = [vp, vp, vp, i32]
+    lib.kbo_mvtpe_ask_shard.argtypes = [vp, vp, i32, i32, i32, i32, vp, vp, vp, vp]
+    lib.kbo_mvtpe_pick.argtypes = [vp, vp, i32, vp, vp, vp]
     lib.kbo_forest_create.argtypes = [vp, C.POINTER(vp), i32, i32, i32, C.c_uint64]
     lib.kbo_forest_destroy.argtypes = [vp]
     lib.kbo_forest_destroy.restype = None

@@ -72,6 +72,23 @@ __device__ __forceinline__ TpeBest tpe_block_best(TpeBest b) {
   __syncthreads();
   return b;  // valid in thread 0
 }
+// a shard ask's result per row (tpe: (point, parameter); mvtpe: point): the winner over the row's nbb per-block results as
+// (FP64 value, global index lo + local index).  A row with no candidate (nbb = 0: an empty shard) reports (-inf, sentinel):
+// sentinel is n_candidates, past every real index, so it loses even to a real -inf under the first-index rule.
+static __global__ void __launch_bounds__(256) tpe_shard_best_kernel(const TpeBest* __restrict__ bb, int nbb, long long lo, long long sentinel,
+                                                                    double* __restrict__ val, long long* __restrict__ idx) {
+  const int r = blockIdx.x;
+  TpeBest best{0.0, -1};
+  for (int i = threadIdx.x; i < nbb; i += blockDim.x) {
+    const TpeBest b = bb[(size_t)r * nbb + i];
+    if (tpe_better(b.s, b.i, best)) best = b;
+  }
+  best = tpe_block_best(best);
+  if (threadIdx.x == 0) {
+    val[r] = best.i >= 0 ? best.s : -INFINITY;
+    idx[r] = best.i >= 0 ? lo + best.i : sentinel;
+  }
+}
 template <bool MAX>
 __device__ __forceinline__ double tpe_block_reduce(double v) {
   __shared__ double red[32];

@@ -72,6 +72,8 @@ struct kbo_mvtpe {
   uint64_t seed = 0;
   uint32_t asks = 0;
   int n = 0, cap = 0, built_n = -1, nb = 0, mcap = 0;
+  uint32_t pick_ask = 0;            // the last shard ask: its ask number, k, n_candidates and history size, for kbo_mvtpe_pick
+  int pick_k = 0, pick_M = 0, pick_n = -1;
   DevBuf<MvParam> d_prm;
   DevBuf<int> d_flt, d_dsc, d_tabd;
   DevBuf<double> vals, loss;
@@ -209,10 +211,8 @@ __global__ void mvtpe_table_kernel(MvModels md, const int* __restrict__ tabd, do
 // ------------------------------------------------------------------------------------------------ ask: candidates
 // candidate m of point p: a component of the below mixture ∝ w_k (slot 0), then every parameter from that component (slot
 // 1 + d): floats and integers by the truncated normal's inverse CDF (integers on [lo2, hi2), then rounded to the grid and
-// clipped), categories from the component's row
-__global__ void mvtpe_draw_kernel(MvModels md, int M, uint64_t seed, uint32_t ask, double* __restrict__ X) {
-  const int p = blockIdx.y, m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m >= M) return;
+// clipped), categories from the component's row; parameter d goes to x[d * stride]
+__device__ __forceinline__ void mv_draw(const MvModels& md, uint64_t seed, uint32_t ask, int p, int m, double* __restrict__ x_out, size_t stride) {
   const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
   uint32_t r[4];
   philox4x32_10((uint32_t)m, 0u, (uint32_t)p, ask, k0, k1, r);
@@ -247,8 +247,29 @@ __global__ void mvtpe_draw_kernel(MvModels md, int M, uint64_t seed, uint32_t as
       x = tpe_truncnorm_draw(P.lo2, P.hi2, mu, sg, u2);
       if (P.kind == KBO_MVTPE_INT) x = mv_grid(P, min(max((int)rint((x - P.lo) / P.q), 0), P.levels - 1));
     }
-    X[((size_t)p * md.D + d) * M + m] = x;
+    x_out[d * stride] = x;
   }
+}
+// every candidate of every point: local candidate m is global candidate m0 + m (m0 = 0 but for a shard ask)
+__global__ void mvtpe_draw_kernel(MvModels md, int M, int m0, uint64_t seed, uint32_t ask, double* __restrict__ X) {
+  const int p = blockIdx.y, m = blockIdx.x * blockDim.x + threadIdx.x;
+  if (m >= M) return;
+  mv_draw(md, seed, ask, p, m0 + m, X + (size_t)p * md.D * M + m, (size_t)M);
+}
+// a shard ask's winners, regenerated from their global indices (the draw's values are already those mvtpe_prep_kernel keeps);
+// an index outside [0, M) is an error
+__global__ void mvtpe_pick_kernel(MvModels md, int k, int M, uint64_t seed, uint32_t ask, const long long* __restrict__ idx,
+                                  double* __restrict__ x_out, int* __restrict__ err) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= k) return;
+  const long long m = idx[p];
+  double* x = x_out + (size_t)p * md.D;
+  if (!(m >= 0 && m < M)) {
+    atomicExch(err, 1);
+    for (int d = 0; d < md.D; d++) x[d] = NAN;
+    return;
+  }
+  mv_draw(md, seed, ask, p, (int)m, x, 1);
 }
 // every candidate into the working buffer (integers rounded to the grid and clipped; floats outside [lo, hi] and invalid
 // category indices are an error) with the prior component's log density in FP64 (without its weight, which is per group)
@@ -808,18 +829,30 @@ int kbo_mvtpe_tell(kbo_handle* h, kbo_mvtpe* t, const double* X, const double* l
   return KBO_OK;
 }
 
-int kbo_mvtpe_ask(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t M, const double* cand_dev, double* x_dev, int64_t* idx_dev, double* cand_out_dev,
-                  float* score_out_dev, void* stream) {
-  if (!h || !t) return KBO_ERR_INVALID;
-  if (!x_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: null output");
-  if (k < 1 || k > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: 1 <= k <= 65535 supported (got %d)", k);
-  if (M < 1 || M > MV_MAXM) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: 1 <= n_candidates <= 2^24 supported (got %d)", M);
-  cudaStream_t s = (cudaStream_t)stream;
+// One ask over local candidates [0, M), which are global candidates [m0, m0 + M) of n_candidates = Mall.  With val_dev null
+// it is kbo_mvtpe_ask (m0 = 0, M = Mall): the winners' vectors go to x_dev.  With val_dev it is a shard ask: each point
+// writes its FP64 winner and global index to val_dev / idx_dev, and M = 0 (an empty shard) is legal.
+static int mv_ask_run(kbo_handle* h, kbo_mvtpe* t, int k, int M, int m0, int Mall, const double* cand_dev, double* x_dev, int64_t* idx_dev,
+                      double* cand_out_dev, float* score_out_dev, double* val_dev, cudaStream_t s) {
   KBO_CUDA(h, cudaSetDevice(h->device));
   cudaEventRecord(t->ev[0], s);
   if (t->built_n != t->n) KBO_TRY(mv_build(h, t, s));
   const uint32_t ask = t->asks++;
   const int D = t->D;
+  if (val_dev) {
+    t->pick_ask = ask;
+    t->pick_k = k;
+    t->pick_M = Mall;
+    t->pick_n = t->n;
+    if (M == 0) {
+      tpe_shard_best_kernel<<<k, 256, 0, s>>>(nullptr, 0, m0, Mall, val_dev, (long long*)idx_dev);
+      KBO_LAUNCH_CHECK(h);
+      t->last_surv.assign(k, 0);
+      std::fill(t->last_ms, t->last_ms + 4, 0.f);
+      KBO_CUDA(h, cudaStreamSynchronize(s));
+      return KBO_OK;
+    }
+  }
   const size_t KM = (size_t)k * M;
   const int nbb = (M + 255) / 256;
   KBO_TRY(kbo_reserve(h, t->surv, (size_t)k));
@@ -838,7 +871,7 @@ int kbo_mvtpe_ask(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t M, const doubl
   }
   const dim3 gm((M + 255) / 256, k);
   if (!cand_dev) {
-    mvtpe_draw_kernel<<<gm, 256, 0, s>>>(md, M, t->seed, ask, Xw);
+    mvtpe_draw_kernel<<<gm, 256, 0, s>>>(md, M, m0, t->seed, ask, Xw);
     KBO_LAUNCH_CHECK(h);
   }
   mvtpe_prep_kernel<<<gm, 256, 0, s>>>(md, M, cand_dev ? cand_dev : Xw, Xw, t->prior.p, t->err.p);
@@ -852,7 +885,8 @@ int kbo_mvtpe_ask(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t M, const doubl
                                                    t->bb.p, nbb, t->surv.p);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[3], s);
-  mvtpe_final_kernel<<<k, 256, 0, s>>>(D, M, Xw, t->bb.p, nbb, x_dev, (long long*)idx_dev);
+  if (val_dev) tpe_shard_best_kernel<<<k, 256, 0, s>>>(t->bb.p, nbb, m0, Mall, val_dev, (long long*)idx_dev);
+  else mvtpe_final_kernel<<<k, 256, 0, s>>>(D, M, Xw, t->bb.p, nbb, x_dev, (long long*)idx_dev);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[4], s);
   t->last_surv.assign(k, 0);
@@ -862,6 +896,44 @@ int kbo_mvtpe_ask(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t M, const doubl
   KBO_CUDA(h, cudaStreamSynchronize(s));
   for (int i = 0; i < 4; i++) cudaEventElapsedTime(&t->last_ms[i], t->ev[i], t->ev[i + 1]);
   if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: a supplied candidate is outside its parameter's domain (a float outside [lo, hi] or an invalid category index)");
+  return KBO_OK;
+}
+
+int kbo_mvtpe_ask(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t M, const double* cand_dev, double* x_dev, int64_t* idx_dev, double* cand_out_dev,
+                  float* score_out_dev, void* stream) {
+  if (!h || !t) return KBO_ERR_INVALID;
+  if (!x_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: null output");
+  if (k < 1 || k > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: 1 <= k <= 65535 supported (got %d)", k);
+  if (M < 1 || M > MV_MAXM) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask: 1 <= n_candidates <= 2^24 supported (got %d)", M);
+  return mv_ask_run(h, t, k, M, 0, M, cand_dev, x_dev, idx_dev, cand_out_dev, score_out_dev, nullptr, (cudaStream_t)stream);
+}
+
+int kbo_mvtpe_ask_shard(kbo_handle* h, kbo_mvtpe* t, int32_t k, int32_t M, int32_t lo, int32_t hi, const double* cand_dev, double* val_dev,
+                        int64_t* idx_dev, void* stream) {
+  if (!h || !t) return KBO_ERR_INVALID;
+  if (cand_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask_shard: caller-supplied candidates are not accepted (the shards draw their own)");
+  if (!val_dev || !idx_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask_shard: null output");
+  if (k < 1 || k > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask_shard: 1 <= k <= 65535 supported (got %d)", k);
+  if (M < 1 || M > MV_MAXM) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask_shard: 1 <= n_candidates <= 2^24 supported (got %d)", M);
+  if (!(0 <= lo && lo <= hi && hi <= M)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_ask_shard: need 0 <= lo <= hi <= n_candidates (got [%d, %d) of %d)", lo, hi, M);
+  return mv_ask_run(h, t, k, hi - lo, lo, M, nullptr, nullptr, idx_dev, nullptr, nullptr, val_dev, (cudaStream_t)stream);
+}
+
+int kbo_mvtpe_pick(kbo_handle* h, kbo_mvtpe* t, int32_t k, const int64_t* idx_dev, double* x_dev, void* stream) {
+  if (!h || !t) return KBO_ERR_INVALID;
+  if (!idx_dev || !x_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_pick: null argument");
+  if (t->pick_k == 0 || t->pick_n != t->n) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_pick: no shard ask since the last tell");
+  if (k != t->pick_k) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_pick: k must be the last shard ask's (%d, got %d)", t->pick_k, k);
+  cudaStream_t s = (cudaStream_t)stream;
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, sizeof *t->err.p, s));
+  mvtpe_pick_kernel<<<(k + 255) / 256, 256, 0, s>>>(mv_models(t), k, t->pick_M, t->seed, t->pick_ask, (const long long*)idx_dev, x_dev,
+                                                    t->err.p);
+  KBO_LAUNCH_CHECK(h);
+  int err = 0;
+  KBO_CUDA(h, kbo_copy(&err, t->err.p, 1, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_mvtpe_pick: a winning index is outside [0, n_candidates)");
   return KBO_OK;
 }
 

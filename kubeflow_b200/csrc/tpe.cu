@@ -61,6 +61,8 @@ struct kbo_tpe {
   uint64_t seed = 0;
   uint32_t asks = 0;
   int n = 0, cap = 0, built_n = -1, nb = 0, ms = 0;
+  uint32_t pick_ask = 0;            // the last shard ask: its ask number, k, n_candidates and history size, for kbo_tpe_pick
+  int pick_k = 0, pick_M = 0, pick_n = -1;
   DevBuf<TpeParam> d_prm;
   DevBuf<int> d_cont, d_disc, d_num, d_cat;
   DevBuf<double> vals, loss;
@@ -106,11 +108,30 @@ __device__ double tpe_draw(const TpeModels& md, const TpeParam& P, uint64_t seed
   while (k < nc - 1 && !(u1 < md.cdf[o + k])) k++;
   return tpe_truncnorm_draw(P.lo, P.hi, md.mu[o + k], md.sg[o + k], u2);
 }
-// every candidate of every (point, parameter), before quantization
-__global__ void tpe_draw_kernel(TpeModels md, int D, int M, uint64_t seed, uint32_t ask, double* __restrict__ X) {
+// every candidate of every (point, parameter), before quantization: local candidate m is global candidate m0 + m (m0 = 0
+// but for a shard ask)
+__global__ void tpe_draw_kernel(TpeModels md, int D, int M, int m0, uint64_t seed, uint32_t ask, double* __restrict__ X) {
   const int pd = blockIdx.y, p = pd / D, d = pd % D;
   const int m = blockIdx.x * blockDim.x + threadIdx.x;
-  if (m < M) X[(size_t)pd * M + m] = tpe_draw(md, md.prm[d], seed, ask, p, d, m);
+  if (m < M) X[(size_t)pd * M + m] = tpe_draw(md, md.prm[d], seed, ask, p, d, m0 + m);
+}
+// a shard ask's winners, regenerated from their global indices and taken to their values as tpe_final_kernel does;
+// an index outside [0, M) is an error
+__global__ void tpe_pick_kernel(TpeModels md, int KD, int D, int M, uint64_t seed, uint32_t ask, const long long* __restrict__ idx,
+                                double* __restrict__ x_out, int* __restrict__ err) {
+  const int pd = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pd >= KD) return;
+  const int p = pd / D, d = pd % D;
+  const long long m = idx[pd];
+  if (!(m >= 0 && m < M)) {
+    atomicExch(err, 1);
+    x_out[pd] = NAN;
+    return;
+  }
+  const TpeParam P = md.prm[d];
+  double x = tpe_draw(md, P, seed, ask, p, d, (int)m);
+  if (P.kind == KBO_TPE_QUNIFORM) x = rint(x / P.q) * P.q;
+  x_out[pd] = x;
 }
 // level index of a candidate of a quantized (rint(x/q) - rint(lo/q)) or categorical (the index itself) parameter; -1 if invalid
 __device__ __forceinline__ long long tpe_level(const TpeParam& P, double x) {
@@ -717,20 +738,30 @@ int kbo_tpe_tell(kbo_handle* h, kbo_tpe* t, const double* X, const double* loss,
   return KBO_OK;
 }
 
-int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* cand_dev, double* x_dev, int64_t* idx_dev, double* cand_out_dev,
-                float* score_out_dev, void* stream) {
-  if (!h || !t) return KBO_ERR_INVALID;
-  if (!x_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: null output");
-  if (k < 1 || k > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: 1 <= k <= 65535 supported (got %d)", k);
-  if (M < 1 || M > TPE_MAXM) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: 1 <= n_candidates <= 2^24 supported (got %d)", M);
-  if ((int64_t)k * t->D > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: k * D must be <= 65535");
-  if ((int64_t)k * t->D * M > (1ll << 31)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: k * D * n_candidates must be <= 2^31");
-  cudaStream_t s = (cudaStream_t)stream;
+// One ask over local candidates [0, M), which are global candidates [m0, m0 + M) of n_candidates = Mall.  With val_dev null
+// it is kbo_tpe_ask (m0 = 0, M = Mall): the winners' values go to x_dev.  With val_dev it is a shard ask: each (point,
+// parameter) writes its FP64 winner and global index to val_dev / idx_dev, and M = 0 (an empty shard) is legal.
+static int tpe_ask_run(kbo_handle* h, kbo_tpe* t, int k, int M, int m0, int Mall, const double* cand_dev, double* x_dev, int64_t* idx_dev,
+                       double* cand_out_dev, float* score_out_dev, double* val_dev, cudaStream_t s) {
   KBO_CUDA(h, cudaSetDevice(h->device));
   cudaEventRecord(t->ev[0], s);
   if (t->built_n != t->n) KBO_TRY(tpe_build(h, t, s));
   const uint32_t ask = t->asks++;
   const int D = t->D, KD = k * D;
+  if (val_dev) {
+    t->pick_ask = ask;
+    t->pick_k = k;
+    t->pick_M = Mall;
+    t->pick_n = t->n;
+    if (M == 0) {
+      tpe_shard_best_kernel<<<KD, 256, 0, s>>>(nullptr, 0, m0, Mall, val_dev, (long long*)idx_dev);
+      KBO_LAUNCH_CHECK(h);
+      t->last_surv.assign(KD, 0);
+      std::fill(t->last_ms, t->last_ms + 5, 0.f);
+      KBO_CUDA(h, cudaStreamSynchronize(s));
+      return KBO_OK;
+    }
+  }
   const int nbb = (std::max(M, t->Dd ? t->lt : 1) + 255) / 256;
   KBO_TRY(kbo_reserve(h, t->surv, (size_t)KD));
   KBO_TRY(kbo_reserve(h, t->bb, (size_t)KD * nbb));
@@ -745,7 +776,7 @@ int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* c
       KBO_TRY(kbo_reserve(h, t->draws, (size_t)KD * M));
       Xw = t->draws.p;
     }
-    tpe_draw_kernel<<<dim3((M + 255) / 256, KD), 256, 0, s>>>(md, D, M, t->seed, ask, Xw);
+    tpe_draw_kernel<<<dim3((M + 255) / 256, KD), 256, 0, s>>>(md, D, M, m0, t->seed, ask, Xw);
     KBO_LAUNCH_CHECK(h);
     X = Xw;
   } else if (cand_out_dev) {
@@ -779,7 +810,8 @@ int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* c
     KBO_LAUNCH_CHECK(h);
   }
   cudaEventRecord(t->ev[4], s);
-  tpe_final_kernel<<<KD, 256, 0, s>>>(md, D, M, X, t->bb.p, nbb, x_dev, (long long*)idx_dev);
+  if (val_dev) tpe_shard_best_kernel<<<KD, 256, 0, s>>>(t->bb.p, nbb, m0, Mall, val_dev, (long long*)idx_dev);
+  else tpe_final_kernel<<<KD, 256, 0, s>>>(md, D, M, X, t->bb.p, nbb, x_dev, (long long*)idx_dev);
   KBO_LAUNCH_CHECK(h);
   cudaEventRecord(t->ev[5], s);
   t->last_surv.assign(KD, 0);
@@ -789,6 +821,50 @@ int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* c
   KBO_CUDA(h, cudaStreamSynchronize(s));
   for (int i = 0; i < 5; i++) cudaEventElapsedTime(&t->last_ms[i], t->ev[i], t->ev[i + 1]);
   if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: a supplied candidate of a quantized or categorical parameter is outside its levels");
+  return KBO_OK;
+}
+
+int kbo_tpe_ask(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, const double* cand_dev, double* x_dev, int64_t* idx_dev, double* cand_out_dev,
+                float* score_out_dev, void* stream) {
+  if (!h || !t) return KBO_ERR_INVALID;
+  if (!x_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: null output");
+  if (k < 1 || k > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: 1 <= k <= 65535 supported (got %d)", k);
+  if (M < 1 || M > TPE_MAXM) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: 1 <= n_candidates <= 2^24 supported (got %d)", M);
+  if ((int64_t)k * t->D > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: k * D must be <= 65535");
+  if ((int64_t)k * t->D * M > (1ll << 31)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask: k * D * n_candidates must be <= 2^31");
+  return tpe_ask_run(h, t, k, M, 0, M, cand_dev, x_dev, idx_dev, cand_out_dev, score_out_dev, nullptr, (cudaStream_t)stream);
+}
+
+int kbo_tpe_ask_shard(kbo_handle* h, kbo_tpe* t, int32_t k, int32_t M, int32_t lo, int32_t hi, const double* cand_dev, double* val_dev,
+                      int64_t* idx_dev, void* stream) {
+  if (!h || !t) return KBO_ERR_INVALID;
+  if (cand_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask_shard: caller-supplied candidates are not accepted (the shards draw their own)");
+  if (!val_dev || !idx_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask_shard: null output");
+  if (k < 1 || k > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask_shard: 1 <= k <= 65535 supported (got %d)", k);
+  if (M < 1 || M > TPE_MAXM) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask_shard: 1 <= n_candidates <= 2^24 supported (got %d)", M);
+  if (!(0 <= lo && lo <= hi && hi <= M)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask_shard: need 0 <= lo <= hi <= n_candidates (got [%d, %d) of %d)", lo, hi, M);
+  if ((int64_t)k * t->D > 65535) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask_shard: k * D must be <= 65535");
+  if ((int64_t)k * t->D * (hi - lo) > (1ll << 31)) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_ask_shard: k * D * (hi - lo) must be <= 2^31");
+  return tpe_ask_run(h, t, k, hi - lo, lo, M, nullptr, nullptr, idx_dev, nullptr, nullptr, val_dev, (cudaStream_t)stream);
+}
+
+int kbo_tpe_pick(kbo_handle* h, kbo_tpe* t, int32_t k, const int64_t* idx_dev, double* x_dev, void* stream) {
+  if (!h || !t) return KBO_ERR_INVALID;
+  if (!idx_dev || !x_dev) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_pick: null argument");
+  if (t->pick_k == 0 || t->pick_n != t->n) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_pick: no shard ask since the last tell");
+  if (k != t->pick_k) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_pick: k must be the last shard ask's (%d, got %d)", t->pick_k, k);
+  cudaStream_t s = (cudaStream_t)stream;
+  KBO_CUDA(h, cudaSetDevice(h->device));
+  KBO_TRY(kbo_reserve(h, t->err, 1));
+  KBO_CUDA(h, cudaMemsetAsync(t->err.p, 0, sizeof *t->err.p, s));
+  const int KD = k * t->D;
+  tpe_pick_kernel<<<(KD + 255) / 256, 256, 0, s>>>(tpe_models(t), KD, t->D, t->pick_M, t->seed, t->pick_ask, (const long long*)idx_dev,
+                                                   x_dev, t->err.p);
+  KBO_LAUNCH_CHECK(h);
+  int err = 0;
+  KBO_CUDA(h, kbo_copy(&err, t->err.p, 1, cudaMemcpyDeviceToHost, s));
+  KBO_CUDA(h, cudaStreamSynchronize(s));
+  if (err) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_tpe_pick: a winning index is outside [0, n_candidates)");
   return KBO_OK;
 }
 

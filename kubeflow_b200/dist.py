@@ -61,3 +61,29 @@ def global_argmax(best: Best | list[Best] | None, group=None, device=None, faile
         win = max((table[r][j] for r in range(world)), key=lambda r: (r[0], -r[1]))
         out.append(Best(float(win[0]), int(win[1]), float(win[2]), float(win[3])))
     return out if multi else out[0]
+
+
+def rank0_seed() -> int:
+    """A seed drawn from fresh entropy on rank 0 and broadcast: every rank of the default process group gets the same one."""
+    import numpy as np
+    box = [int(np.random.default_rng().integers(1 << 62))]
+    if dist.is_initialized() and dist.get_world_size() > 1:
+        dist.broadcast_object_list(box, src=0)
+    return box[0]
+
+
+def sharded_ask(shard_ask, pick, n_candidates: int, rows: int, device):
+    """An ask over candidates sharded by index (``tpe`` / ``multivariate-tpe``): this rank's ``shard_ask(lo, hi)`` returns
+    its (FP64 value, global index) winner per row (NumPy arrays of ``rows``); one ``global_argmax`` over the rows gives
+    every rank the first index of the global maximum, and ``pick(indices)`` regenerates those candidates locally, so no row
+    has to be broadcast.  A rank whose shard ask raises still joins the exchange and every rank raises ``RankFailure``.
+    An empty shard's (-inf, n_candidates) entries are ordinary entries that never win."""
+    lo, hi = shard_rows(n_candidates, dist.get_rank(), dist.get_world_size())
+    bests, failed = None, None
+    try:
+        val, idx = shard_ask(lo, hi)
+        bests = [Best(float(v), int(i), 0.0, 0.0) for v, i in zip(val.ravel().tolist(), idx.ravel().tolist())]
+    except Exception as e:  # noqa: BLE001 — every rank raises RankFailure in the exchange, none is left waiting
+        failed = f"{type(e).__name__}: {e}"
+    bests = global_argmax(bests, device=device, failed=failed, n=rows)
+    return pick([b.index for b in bests])

@@ -12,6 +12,7 @@ Katib's Optuna service is unpinned).
 * Batches (``current_request_number`` = k > 1): k independent draws against the same model, with no lies in between, as k
   calls of Optuna's ``study.ask`` with the pending trials ignored.
 * Draws are keyed by (random_state, ask counter, point, candidate, slot): the same request sequence gives the same replies.
+* Under the SPMD server every rank scores its block of each request's candidates, as for ``tpe`` (tpe_service.py).
 """
 from __future__ import annotations
 
@@ -19,7 +20,7 @@ import numpy as np
 
 from .internal import DOUBLE, INTEGER, AlgorithmSettingsError, HyperParameterSearchSpace, parse_settings
 from .service import _Base, _reply_from, experiment_fingerprint
-from .tpe_service import _Experiment
+from .tpe_service import _Experiment, sharded_points
 
 NAME = "multivariate-tpe"
 MAX_EI_CANDIDATES = 1 << 24
@@ -121,4 +122,4 @@ class MultivariateTpeService(_Base):
             def make_engine():
                 from ..mvtpe import MvTpe
                 return MvTpe(st.space, seed=st.seed, device=int(settings.get("device", 0)))
-            return _reply_from(st.points(k, settings["n_startup_trials"], settings["n_ei_candidates"], make_engine))
+            return _reply_from(sharded_points(self, exp.name, st, k, settings["n_startup_trials"], settings["n_ei_candidates"], make_engine))

@@ -87,7 +87,8 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
         dev = {"device": local}
         inner = DispatchService([SkoptService({**dev, "shard": True}), RandomService(), SobolService(), CmaesService(dev),
-                                 TpeService(dev), MultivariateTpeService(dev), EnasService(dev), HyperbandService(), PbtService()])
+                                 TpeService({**dev, "shard": True}), MultivariateTpeService({**dev, "shard": True}), EnasService(dev),
+                                 HyperbandService(), PbtService()])
         spmd = SpmdServicer(inner)
         if dist.get_rank() == 0:
             server, port = serve(spmd, args.port)

@@ -5,7 +5,10 @@ endpoint Katib talks to; for every ``GetSuggestions`` it broadcasts the request'
 servicer call in lockstep — same trials told, same seed, same constant lies — so their optimizers stay identical without
 any state exchange.  Inside the call the optimizer (``shard=True``) gives each rank ``n_points / world`` candidates, the
 fit is replicated, and the only data-path collectives are the 32-byte all-gather of the per-rank argmax
-(``dist.global_argmax``) and the broadcast of the winning row from its owner.  Ranks > 0 sit in ``worker_loop``.
+(``dist.global_argmax``) and the broadcast of the winning row from its owner.  ``tpe`` and ``multivariate-tpe`` shard the
+same way: each rank draws and scores its block of every point's candidates (keyed by their global index), one all-gather
+of the per-rank (FP64 value, global index) winners decides, and every rank regenerates the winners itself
+(``dist.sharded_ask``), so the replies are bit for bit those of one GPU.  Ranks > 0 sit in ``worker_loop``.
 Calls are serialised on rank 0 (collectives need one order); ValidateAlgorithmSettings touches no GPU and stays on rank 0.
 """
 from __future__ import annotations
@@ -21,7 +24,7 @@ logger = logging.getLogger(__name__)
 
 
 class SpmdServicer:
-    sharded_algorithms = ("", "bayesianoptimization")
+    sharded_algorithms = ("", "bayesianoptimization", "tpe", "multivariate-tpe")
 
     def __init__(self, inner):
         if not dist.is_initialized():
@@ -43,7 +46,7 @@ class SpmdServicer:
 
     def GetSuggestions(self, request, context):
         if request.experiment.spec.algorithm.algorithm_name not in self.sharded_algorithms:
-            return self.inner.GetSuggestions(request, context)      # nothing to shard (random, sobol, cmaes, tpe, multivariate-tpe, enas, hyperband, pbt): rank 0 alone
+            return self.inner.GetSuggestions(request, context)      # nothing to shard (random, sobol, cmaes, enas, hyperband, pbt): rank 0 alone
         data = request._data if isinstance(request, LazyRequest) else request.SerializeToString()
         with self._lock:
             self._bcast(("GetSuggestions", data))

@@ -13,6 +13,10 @@ the GPU engine ``kubeflow_b200.tpe`` (contract: oracle/tpe_oracle.py).
   ``n_startup_jobs = current_request_number`` to it, where this service honours the ``n_startup_jobs`` setting.
 * Draws are keyed by (random_state, ask counter, point, parameter, candidate): the same request sequence gives the same
   replies.
+* Under the SPMD server (engine default ``shard``, never an Experiment setting) every rank holds the same experiment and
+  scores its block of each request's candidates; the replies are those of one GPU.  A seed drawn from fresh entropy is drawn
+  on rank 0 and broadcast, and an experiment whose sharded ask failed on any rank is closed on every rank, so the next
+  request rebuilds it identically everywhere.
 """
 from __future__ import annotations
 
@@ -84,7 +88,11 @@ class _Experiment:
         self.ss, self.settings = ss, settings
         self.space = tpe_space(ss)
         self.rows, self.losses, self.told = [], [], set()
-        self.rng = np.random.default_rng(settings.get("random_state"))       # start-up phase (None: fresh entropy)
+        entropy = settings.get("random_state")
+        if entropy is None and settings.get("shard"):      # the ranks' engines must draw the same candidates
+            from ..dist import rank0_seed
+            entropy = rank0_seed()
+        self.rng = np.random.default_rng(entropy)       # start-up phase (None: fresh entropy)
         self.seed = settings["random_state"] if "random_state" in settings else int(self.rng.integers(1 << 62))
         self.engine = None       # kubeflow_b200.tpe.Tpe, created at the first model-based ask
         self.n_engine = 0        # rows told to the engine
@@ -130,9 +138,9 @@ class _Experiment:
         self.losses += losses
         self.told.update(names)
 
-    def points(self, k: int, n_startup: int, n_candidates: int, make_engine) -> list:
+    def points(self, k: int, n_startup: int, n_candidates: int, make_engine, shard: bool = False) -> list:
         """k assignment lists: start-up points from the prior (no engine) while fewer than ``n_startup`` trials are told, else
-        the engine's (made by ``make_engine()`` on first use), told every trial it has not seen."""
+        the engine's (made by ``make_engine()`` on first use), told every trial it has not seen; ``shard``: its sharded ask."""
         if k == 0:
             return []
         if len(self.rows) < n_startup:
@@ -143,7 +151,7 @@ class _Experiment:
         if self.n_engine < len(self.rows):
             self.engine.tell(np.asarray(self.rows[self.n_engine:]), np.asarray(self.losses[self.n_engine:]))
             self.n_engine = len(self.rows)
-        return [self.assignments(x) for x in self.engine.ask(k, n_candidates)]
+        return [self.assignments(x) for x in self.engine.ask(k, n_candidates, shard=shard)]
 
     def assignments(self, x) -> list:
         out = []
@@ -162,6 +170,18 @@ def _same_number(a: str, b: str) -> bool:
         return float(a) == float(b)
     except ValueError:
         return False
+
+
+def sharded_points(service, name: str, st, *args) -> list:
+    """``st.points(*args)`` with the service's ``shard`` default; a ``RankFailure`` closes the experiment's entry, which every
+    rank does together, so the next request rebuilds it identically everywhere.  Call with ``service._lock`` held."""
+    from ..dist import RankFailure
+    try:
+        return st.points(*args, shard=bool(service.engine_defaults.get("shard")))
+    except RankFailure:
+        if service._exps.get(name) is st:
+            service._exps.pop(name).close()
+        raise
 
 
 class TpeService(_Base):
@@ -188,4 +208,4 @@ class TpeService(_Base):
                 from ..tpe import Tpe
                 return Tpe(st.space, gamma=settings["gamma"], prior_weight=settings["prior_weight"], seed=st.seed,
                            device=int(settings.get("device", 0)))
-            return _reply_from(st.points(k, settings["n_startup_jobs"], settings["n_EI_candidates"], make_engine))
+            return _reply_from(sharded_points(self, exp.name, st, k, settings["n_startup_jobs"], settings["n_EI_candidates"], make_engine))

@@ -46,11 +46,22 @@ class Tpe(L.Handle):
             self.check(self.lib.kbo_tpe_tell(self._h, self._o, X.ctypes.data, y.ctypes.data, X.shape[0], 1, self._stream()))
             self.n += X.shape[0]
 
-    def ask(self, k: int = 1, n_candidates: int = 24, candidates: torch.Tensor | None = None, return_details: bool = False):
+    def ask(self, k: int = 1, n_candidates: int = 24, candidates: torch.Tensor | None = None, return_details: bool = False,
+            shard: bool = False):
         """k suggestions (k × D float64 NumPy array).  ``candidates``: optional k × D × n_candidates float64 CUDA tensor (numeric
         values before quantization, category indices for choices).  ``return_details``: also the winning indices, the
-        candidates (CUDA tensor) and the FP32 scores with their bounds (k × D × n_candidates × 2 CUDA tensor)."""
+        candidates (CUDA tensor) and the FP32 scores with their bounds (k × D × n_candidates × 2 CUDA tensor).  ``shard``: when the default process group has
+        more than one rank, every rank draws and scores its ``shard_rows`` block of the candidates and one exchange gives all
+        ranks the suggestions a one-GPU ask would make (``dist.sharded_ask``); every rank must then make the same calls."""
         k, M = int(k), int(n_candidates)
+        if shard:
+            if candidates is not None or return_details:
+                raise ValueError("candidates and return_details cannot be combined with shard")
+            import torch.distributed as dist
+            if dist.is_initialized() and dist.get_world_size() > 1:
+                from .dist import sharded_ask
+                cdev = torch.device("cuda", self.device) if dist.get_backend() == "nccl" else torch.device("cpu")
+                return sharded_ask(lambda lo, hi: self.ask_shard(k, M, lo, hi), lambda idx: self.pick(k, idx), M, k * self.D, cdev)
         dev = f"cuda:{self.device}"
         cp = None
         if candidates is not None:
@@ -86,6 +97,26 @@ class Tpe(L.Handle):
                 ent["n_below"] = nb.value
             out.append(ent)
         return out
+
+    def ask_shard(self, k: int, n_candidates: int, lo: int, hi: int):
+        """One shard of a sharded ask: candidates [lo, hi) of n_candidates, drawn by their global index.  Returns this shard's
+        winner per (point, parameter) as (FP64 values, global indices) NumPy arrays; an empty shard (lo == hi) gives (-inf, n_candidates).
+        The ask counter advances as one ``ask`` advances it."""
+        dev = f"cuda:{self.device}"
+        val = torch.empty((int(k), self.D), dtype=torch.float64, device=dev)
+        idx = torch.empty((int(k), self.D), dtype=torch.int64, device=dev)
+        self.check(self.lib.kbo_tpe_ask_shard(self._h, self._o, int(k), int(n_candidates), int(lo), int(hi), None, val.data_ptr(),
+                                              idx.data_ptr(), self._stream()))
+        return val.cpu().numpy(), idx.cpu().numpy()
+
+    def pick(self, k: int, index) -> np.ndarray:
+        """The suggestions (k × D) at the winning global indices ``index`` (k × D) of the last shard ask, regenerated from
+        their draws: what ``ask`` returns when those candidates win."""
+        dev = f"cuda:{self.device}"
+        idx = torch.as_tensor(np.asarray(index, dtype=np.int64).reshape((int(k), self.D))).to(dev)
+        x = torch.empty(int(k), self.D, dtype=torch.float64, device=dev)
+        self.check(self.lib.kbo_tpe_pick(self._h, self._o, int(k), idx.data_ptr(), x.data_ptr(), self._stream()))
+        return x.cpu().numpy()
 
     def last_survivors(self) -> np.ndarray:
         return self._last_survivors()
