@@ -532,6 +532,22 @@ int kbo_debug_record_stages(kbo_handle* h, int32_t on) {
   h->stage_recs.clear();
   return KBO_OK;
 }
+// Test hooks (not in kbo.h): with on != 0, kbo_fit enqueues its factorisation call by call instead of replaying the cached graph
+// (the path KBO_FIT_TRACE measures).  stats[8] = graph captures, executable updates, instantiations, replays since the handle was
+// made; then the cached graph's kernel nodes in the chain's green context, in the rest's, elsewhere; kernel launches per replay.
+int kbo_debug_fit_stream_path(kbo_handle* h, int32_t on) {
+  if (!h) return KBO_ERR_INVALID;
+  h->fit_stream_path = on != 0;
+  return KBO_OK;
+}
+int kbo_debug_fit_graph(kbo_handle* h, int32_t* stats) {
+  if (!h) return KBO_ERR_INVALID;
+  if (!stats) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_fit_graph: bad argument");
+  cudaSetDevice(h->device);
+  for (int i = 0; i < 4; i++) stats[i] = h->fit_graph_stat[i];
+  stats[7] = h->fit_graph_launches;
+  return kbo_i_fit_graph_nodes(h, stats + 4);
+}
 int kbo_debug_stage_count(kbo_handle* h) { return h ? (int)h->stage_recs.size() : KBO_ERR_INVALID; }
 // ints[4] = (stage, acquisition, calibration rows, survivors counted), floats[7] = (E, Eμ, raw max |dσ²|, raw max |dμ|, lower bound,
 // threshold, window delta); the first min(cap, list length) survivors go to list.  Returns the list length.

@@ -167,18 +167,25 @@ dgemm_sm90_kernel(int M, int N, int K, const double* __restrict__ A, int lda, co
     }
 }
 
+// More than 48 KB of dynamic shared memory needs the opt-in, once per instantiation and device.  Callers that capture launches
+// into a CUDA graph call this before the capture begins: no attribute call may run inside one.
 template <bool TRANSB>
-static inline void dgemm_sm90_launch(cudaStream_t s, int M, int N, int K, const double* A, int lda, const double* B, int ldb, double* C,
-                                     int ldc, double alpha, double beta, int kmode, int kbegin, int tileskip, int batch = 1,
-                                     long long strideA = 0, long long strideB = 0, long long strideC = 0) {
-  dim3 grid((N + DG_BN - 1) / DG_BN, (M + DG_BM - 1) / DG_BM, batch);
-  static bool attr_set[16] = {};   // per instantiation and device: more than 48 KB of dynamic shared memory needs the opt-in
+static inline void dgemm_sm90_opt_in() {
+  static bool attr_set[16] = {};
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 16 && !attr_set[dev]) {
     cudaFuncSetAttribute(dgemm_sm90_kernel<TRANSB>, cudaFuncAttributeMaxDynamicSharedMemorySize, DS_SMEM_BYTES);
     attr_set[dev] = true;
   }
+}
+
+template <bool TRANSB>
+static inline void dgemm_sm90_launch(cudaStream_t s, int M, int N, int K, const double* A, int lda, const double* B, int ldb, double* C,
+                                     int ldc, double alpha, double beta, int kmode, int kbegin, int tileskip, int batch = 1,
+                                     long long strideA = 0, long long strideB = 0, long long strideC = 0) {
+  dim3 grid((N + DG_BN - 1) / DG_BN, (M + DG_BM - 1) / DG_BM, batch);
+  dgemm_sm90_opt_in<TRANSB>();
   dgemm_sm90_kernel<TRANSB><<<grid, 256, DS_SMEM_BYTES, s>>>(M, N, K, A, lda, B, ldb, C, ldc, alpha, beta, kmode, kbegin, tileskip, strideA,
                                                              strideB, strideC);
 }

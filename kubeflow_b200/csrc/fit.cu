@@ -444,7 +444,11 @@ static int fit_partition(kbo_handle* h, bool partitioned, cudaStream_t (&out)[FI
   for (int i = 0; i < FIT_NSTREAMS; i++) out[i] = h->s3p[i];
   return KBO_OK;
 }
+static void fit_graph_drop(kbo_handle* h);
 void kbo_i_fit_partition_free(kbo_handle* h) {
+  fit_graph_drop(h);   // its kernel nodes belong to the green contexts below
+  if (h->s_cap) cudaStreamDestroy(h->s_cap);
+  h->s_cap = nullptr;
   for (auto* set : {&h->s3g, &h->s3p})
     for (auto& st : *set)
       if (st) {
@@ -456,10 +460,56 @@ void kbo_i_fit_partition_free(kbo_handle* h) {
   h->gctx_chain = h->gctx_rest = nullptr;
 }
 
+// The Gram matrix's columns past its first `tile0` 64-column tiles (which hold everything the first panel's chain and shadows read).
+struct GramRest {
+  const double* Xs;
+  int N, D, kind;
+  double amp, noise;
+  double* K;
+  int ldk, tile0;
+  dim3 grid() const { return dim3((N + 63) / 64 - tile0, (N + 63) / 64); }
+};
+
+// Set the graph's Gram node to this fit's arguments: θ (amp, noise) is passed by value, and a replay must not reuse a stale one.
+static int gram_node_set(kbo_handle* h, const GramRest& g) {
+  void* args[] = {(void*)&g.Xs, (void*)&g.N, (void*)&g.D, (void*)&g.kind, (void*)&g.amp, (void*)&g.noise, (void*)&g.K, (void*)&g.ldk, (void*)&g.tile0};
+  cudaKernelNodeParams p = {};
+  p.func = (void*)gram_kernel;
+  p.gridDim = g.grid();
+  p.blockDim = dim3(256);
+  p.kernelParams = args;
+  KBO_CUDA(h, cudaGraphExecKernelNodeSetParams(h->fit_exec, h->fit_gram_node, &p));
+  return KBO_OK;
+}
+
+static int fit_graph_replay(kbo_handle* h, cudaStream_t s, const GramRest* gram, bool zsolve) {
+  if (gram) KBO_TRY(gram_node_set(h, *gram));
+  KBO_CUDA(h, cudaGraphLaunch(h->fit_exec, s));
+  h->launches += h->fit_graph_launches;
+  h->fit_graph_stat[3]++;
+  if (zsolve) h->z_ready = true;
+  return KBO_OK;
+}
+
+static void fit_graph_drop(kbo_handle* h) {
+  if (h->fit_exec) cudaGraphExecDestroy(h->fit_exec);
+  if (h->fit_graph) cudaGraphDestroy(h->fit_graph);
+  h->fit_exec = nullptr;
+  h->fit_graph = nullptr;
+  h->fit_gram_node = nullptr;
+  h->fit_key.clear();
+}
+
+// The factorisation is ~3000 launches, event records and waits over ten streams.  Enqueued call by call, the host is barely ahead
+// of the chain: the GPU is idle when a fit starts (every ask ends in a synchronisation), and the chain needs a panel's launches about
+// as fast as the host issues them.  So the schedule is captured once into a CUDA graph and replayed with one cudaGraphLaunch for as
+// long as what it bakes in holds (the key below): the same kernels, arguments and dependencies, so the same results bit for bit.
+// KBO_FIT_TRACE and kbo_debug_fit_stream_path enqueue it call by call.
 static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double* W, int ldw, int* info_dev, cudaStream_t s, int lead,
-                                cudaEvent_t e_early = nullptr) {
-  // e_early (optional): the first column block of A is complete and info / W are zeroed (the caller did both); the rest of A follows
-  // on s.  The chain-side streams then start on e_early; everything that touches other column blocks waits for the whole matrix.
+                                const GramRest* gram = nullptr) {
+  // gram (optional): the first column block of A is complete and info / W are zeroed (the caller did both on s); this launches the
+  // rest of A.  The chain-side streams then start on the first column block; everything that touches other column blocks waits for
+  // the whole matrix.
   // panel width 256: four 64-blocks per panel
   const int OW = 256, NB = KBO_NB, n_panels = (N + OW - 1) / OW;
   // look-ahead depth: column blocks at distance 1..Dn from the panel get their own GEMM (and stream) per panel, the bulk of the
@@ -486,6 +536,25 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
     KBO_CUDA(h, cudaFuncSetAttribute(diag_inv_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     h->attr_fit = true;
   }
+  dgemm_sm90_opt_in<true>();
+  dgemm_sm90_opt_in<false>();
+  // a lazy fit takes alpha from triangular solves: the forward one (z = L⁻¹·yn) is carried along, one panel behind (solve.cu)
+  const bool zsolve = lead < N && A == h->K.p && W == h->W.p && N == h->N && lda == h->ld;
+  if (zsolve) KBO_TRY(kbo_i_zsolve_reserve(h));
+  if (gram && !h->ev_gram) KBO_CUDA(h, cudaEventCreateWithFlags(&h->ev_gram, cudaEventDisableTiming));
+  static const bool trace = getenv("KBO_FIT_TRACE") != nullptr;
+  const bool graph = !trace && !h->fit_stream_path;
+  if (graph && !h->s_cap) KBO_CUDA(h, cudaStreamCreateWithFlags(&h->s_cap, cudaStreamNonBlocking));
+  // Everything above allocates or sets attributes; nothing below may (a capture forbids it).
+  std::vector<intptr_t> key;
+  if (graph) {
+    key = {N, lda, ldw, lead, zsolve, gram != nullptr, partitioned, (intptr_t)A, (intptr_t)W, (intptr_t)h->T.p, (intptr_t)h->T2.p, (intptr_t)h->Linv4.p,
+           (intptr_t)info_dev, zsolve ? (intptr_t)h->zf.p : 0, zsolve ? (intptr_t)h->yn.p : 0, gram ? gram->tile0 : 0};
+    if (h->fit_exec && key == h->fit_key) return fit_graph_replay(h, s, gram, zsolve);
+  }
+  // the caller's stream, or the capture's origin stream: the graph is then launched on s
+  const cudaStream_t so = graph ? h->s_cap : s;
+  const cudaEvent_t e_early = gram ? h->ev_gram : nullptr;
   double* T = h->T.p;
   double* T2 = h->T2.p;
   // the 64×64 inverses of a panel's diagonal blocks, two sets: the chain of panel P+1 starts when the NEAR shadow of panel P is done,
@@ -506,7 +575,6 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   std::vector<cudaStream_t> all_streams = {sc, sn, ss, sb, si, sw};
   cudaEvent_t* ev_wpp = ev_x + 32;   // [n_panels] W_PP complete
   for (int k = 1; k <= Dn + 1; k++) all_streams.push_back(colS[k]);
-  static const bool trace = getenv("KBO_FIT_TRACE") != nullptr;
   cudaEvent_t tr[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   std::vector<cudaEvent_t> tp;   // per panel on the chain stream: enqueued | column block ready | diagonal block done
   auto mark = [&]() {
@@ -531,14 +599,29 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
     for (auto& e : tr) cudaEventCreate(&e);
     cudaEventRecord(tr[0], s);
   }
-  if (!e_early) {
-    KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, 2 * sizeof(int), s));   // h->info: the pivot and who set it
-    KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, s));   // on the caller's stream: all SMs, not the chain's 8
+  const int launches0 = h->launches;
+  if (graph) KBO_CUDA(h, cudaStreamBeginCapture(so, cudaStreamCaptureModeThreadLocal));
+  cudaGraphNode_t gram_node = nullptr;
+  double host_ms = 0.0;
+  const int rc = [&]() -> int {
+  if (gram) {
+    KBO_CUDA(h, cudaEventRecord(e_early, so));
+    gram_kernel<<<gram->grid(), 256, 0, so>>>(gram->Xs, gram->N, gram->D, gram->kind, gram->amp, gram->noise, gram->K, gram->ldk, gram->tile0);
+    KBO_LAUNCH_CHECK(h);
+    if (graph) {
+      cudaStreamCaptureStatus cs;
+      const cudaGraphNode_t* deps = nullptr;
+      size_t nd = 0;
+      KBO_CUDA(h, cudaStreamGetCaptureInfo(so, &cs, nullptr, nullptr, &deps, &nd));
+      if (nd != 1) KBO_FAIL(h, KBO_ERR_CUDA, "fit graph capture: the Gram launch is not the origin stream's last node");
+      gram_node = deps[0];
+    }
+  } else {
+    KBO_CUDA(h, cudaMemsetAsync(info_dev, 0, 2 * sizeof(int), so));   // h->info: the pivot and who set it
+    KBO_CUDA(h, cudaMemsetAsync(W, 0, sizeof(double) * (size_t)N * ldw, so));   // on the caller's stream: all SMs, not the chain's 8
   }
-  // a lazy fit takes alpha from triangular solves: the forward one (z = L⁻¹·yn) is carried along, one panel behind (solve.cu)
-  const bool zsolve = lead < N && A == h->K.p && W == h->W.p && N == h->N && lda == h->ld;
-  if (zsolve) KBO_TRY(kbo_i_zsolve_begin(h, s));
-  KBO_CUDA(h, cudaEventRecord(e_start, s));
+  if (zsolve) KBO_TRY(kbo_i_zsolve_begin(h, so));
+  KBO_CUDA(h, cudaEventRecord(e_start, so));
   for (cudaStream_t st : all_streams) {
     const bool chain_side = st == sc || st == sn || st == sw;
     KBO_CUDA(h, cudaStreamWaitEvent(st, e_early && chain_side ? e_early : e_start, 0));
@@ -711,7 +794,9 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
         const int P0 = rp0, Pw = done - rp0;
         rp0 = done;
         if (P > 0) {   // rows [P0, done) of L left of this panel: the earlier panels' shadows
-          KBO_CUDA(h, cudaStreamWaitEvent(si, ev_solve[P - 1], 0));
+          // (panel P − 1 had far rows only if more than one 256-row block lay below it: a graph capture may wait only on events
+          // recorded inside it)
+          if (N - K0 > OW) KBO_CUDA(h, cudaStreamWaitEvent(si, ev_solve[P - 1], 0));
           KBO_CUDA(h, cudaStreamWaitEvent(si, ev_nsolve[P - 1], 0));
         }
         double* Wrp = W + (size_t)P0 * ldw + P0;
@@ -740,14 +825,50 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   };
   const auto host_t0 = std::chrono::steady_clock::now();
   const int rc = body();
-  const double host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
+  host_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - host_t0).count();
   {
     int j = 0;
     for (cudaStream_t st : all_streams) {
       cudaEventRecord(e_join[j], st);
-      cudaStreamWaitEvent(s, e_join[j], 0);
+      cudaStreamWaitEvent(so, e_join[j], 0);
       j++;
     }
+  }
+  return rc;
+  }();
+  if (graph) {
+    cudaGraph_t g = nullptr;
+    const cudaError_t e = cudaStreamEndCapture(so, &g);
+    if (rc != KBO_OK) {
+      if (g) cudaGraphDestroy(g);
+      return rc;
+    }
+    if (e != cudaSuccess) KBO_FAIL(h, KBO_ERR_CUDA, "fit graph capture failed: %s", cudaGetErrorString(e));
+    h->fit_graph_stat[0]++;
+    h->fit_graph_launches = h->launches - launches0;
+    h->launches = launches0;   // counted again by the replay
+    // the same schedule over moved buffers keeps its topology: update the executable graph in place; otherwise instantiate anew
+    cudaGraphExecUpdateResultInfo ui;
+    if (h->fit_exec && (!gram) == (!h->fit_gram_node) && cudaGraphExecUpdate(h->fit_exec, g, &ui) == cudaSuccess) {
+      cudaGraphDestroy(g);   // the nodes of the graph fit_exec was instantiated from still address it (fit_gram_node)
+      h->fit_graph_stat[1]++;
+    } else {
+      cudaGetLastError();
+      fit_graph_drop(h);
+      // node priorities: the chain's streams are the most urgent, and a graph otherwise runs every node at the priority of the
+      // stream it is launched into
+      const cudaError_t ei = cudaGraphInstantiateWithFlags(&h->fit_exec, g, cudaGraphInstantiateFlagUseNodePriority);
+      if (ei != cudaSuccess) {
+        cudaGraphDestroy(g);
+        h->fit_exec = nullptr;
+        KBO_FAIL(h, KBO_ERR_CUDA, "fit graph instantiation failed: %s", cudaGetErrorString(ei));
+      }
+      h->fit_graph = g;
+      h->fit_gram_node = gram_node;
+      h->fit_graph_stat[2]++;
+    }
+    h->fit_key = key;
+    return fit_graph_replay(h, s, gram, zsolve);
   }
   if (tr[0]) {
     int j = 1;
@@ -785,6 +906,35 @@ static int factor_and_invert_v3(kbo_handle* h, double* A, int N, int lda, double
   (void)host_ms;
   if (zsolve && rc == KBO_OK) h->z_ready = true;
   return rc;
+}
+
+// Test hook: the cached graph's kernel nodes by the context they run in — counts[0] the chain's green context, [1] the rest's,
+// [2] any other (the plain streams of an unpartitioned fit, and the Gram launch on the caller's side).  No graph: all zero.
+int kbo_i_fit_graph_nodes(kbo_handle* h, int32_t* counts) {
+  counts[0] = counts[1] = counts[2] = 0;
+  if (!h->fit_graph) return KBO_OK;
+  CUresult (*node_params)(CUgraphNode, CUDA_KERNEL_NODE_PARAMS*) = nullptr;
+  CUresult (*from_green)(CUcontext*, CUgreenCtx) = nullptr;
+  cudaDriverEntryPointQueryResult q;
+  KBO_CUDA(h, cudaGetDriverEntryPoint("cuGraphKernelNodeGetParams", (void**)&node_params, cudaEnableDefault, &q));
+  KBO_CUDA(h, cudaGetDriverEntryPoint("cuCtxFromGreenCtx", (void**)&from_green, cudaEnableDefault, &q));
+  if (!node_params || !from_green) KBO_FAIL(h, KBO_ERR_CUDA, "kbo_debug_fit_graph: driver entry points missing");
+  CUcontext chain = nullptr, rest = nullptr;
+  if (h->gctx_chain && (from_green(&chain, (CUgreenCtx)h->gctx_chain) != CUDA_SUCCESS || from_green(&rest, (CUgreenCtx)h->gctx_rest) != CUDA_SUCCESS))
+    KBO_FAIL(h, KBO_ERR_CUDA, "kbo_debug_fit_graph: cuCtxFromGreenCtx failed");
+  size_t n = 0;
+  KBO_CUDA(h, cudaGraphGetNodes(h->fit_graph, nullptr, &n));
+  std::vector<cudaGraphNode_t> nodes(n);
+  KBO_CUDA(h, cudaGraphGetNodes(h->fit_graph, nodes.data(), &n));
+  for (cudaGraphNode_t nd : nodes) {
+    cudaGraphNodeType t;
+    KBO_CUDA(h, cudaGraphNodeGetType(nd, &t));
+    if (t != cudaGraphNodeTypeKernel) continue;
+    CUDA_KERNEL_NODE_PARAMS p = {};
+    if (node_params((CUgraphNode)nd, &p) != CUDA_SUCCESS) KBO_FAIL(h, KBO_ERR_CUDA, "kbo_debug_fit_graph: cuGraphKernelNodeGetParams failed");
+    counts[chain && p.ctx == chain ? 0 : rest && p.ctx == rest ? 1 : 2]++;
+  }
+  return KBO_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -891,21 +1041,6 @@ int kbo_i_gram(kbo_handle* h, const double* Xs, int N, int D, int kernel, double
   KBO_LAUNCH_CHECK(h);
   return KBO_OK;
 }
-// The Gram matrix in two launches: the first `tiles_first` 64-column tiles (all the first panel's chain and shadows read), an event,
-// then the rest — the factorisation starts earlier (fit.cu: factor_and_invert_v3, e_early).
-static int gram_two_parts(kbo_handle* h, const double* Xs, int N, int D, int kernel, double amp, double noise, double* K, int ldk, int tiles_first,
-                          cudaEvent_t e_first, cudaStream_t s) {
-  const int nt = (N + 63) / 64, t1 = min(tiles_first, nt);
-  gram_kernel<<<dim3(t1, nt), 256, 0, s>>>(Xs, N, D, kernel, amp, noise, K, ldk, 0);
-  KBO_LAUNCH_CHECK(h);
-  KBO_CUDA(h, cudaEventRecord(e_first, s));
-  if (nt > t1) {
-    gram_kernel<<<dim3(nt - t1, nt), 256, 0, s>>>(Xs, N, D, kernel, amp, noise, K, ldk, t1);
-    KBO_LAUNCH_CHECK(h);
-  }
-  return KBO_OK;
-}
-
 // alpha = Wᵀ(W yn), LML, and (when the tensor-core sweep may be used) the fp16 hi/lo planes of W — shared by fit and append
 static int fit_finish(kbo_handle* h, cudaStream_t s, bool new_center) {
   const int N = h->N, ld = h->ld;
@@ -1026,12 +1161,14 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
   if (trace) cudaEventRecord(te[0], s);
   // the one-stream reference: Cholesky, then recursive-doubling inverse (kbo_potrf, kbo_trtri)
   static const bool serial = getenv("KBO_FIT_SERIAL") != nullptr;
-  const bool early = !serial && N >= 1024;   // v3 starts on the first column block of the Gram matrix
+  // v3 starts on the first column block of the Gram matrix: the first 8 64-column tiles are launched here, the rest by v3
+  const bool early = !serial && N >= 1024;
+  const GramRest gram_rest{h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, h->K.p, ld, 8};
   if (early) {
     KBO_CUDA(h, cudaMemsetAsync(h->info.p, 0, sizeof *h->info.p * 2, s));
     KBO_CUDA(h, cudaMemsetAsync(h->W.p, 0, sizeof *h->W.p * N * ld, s));
-    if (!h->ev_gram) KBO_CUDA(h, cudaEventCreateWithFlags(&h->ev_gram, cudaEventDisableTiming));
-    KBO_TRY(gram_two_parts(h, h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, h->K.p, ld, 8, h->ev_gram, s));
+    gram_kernel<<<dim3(gram_rest.tile0, (N + 63) / 64), 256, 0, s>>>(h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, h->K.p, ld, 0);
+    KBO_LAUNCH_CHECK(h);
   } else {
     KBO_TRY(kbo_i_gram(h, h->Xs.p, N, D, p->kernel, p->amplitude, p->noise, h->K.p, ld, s));
   }
@@ -1053,7 +1190,7 @@ int kbo_i_fit(kbo_handle* h, const double* X, const double* y, int N, int D, con
         const int P1 = kbo_prefix_pairs(h);
         if (P1 >= 1 && P1 < kbo_tile_pairs(h->Npad) && P1 * 512 + 512 <= N) lead = round_up(P1 * 512, 512);
       }
-      KBO_TRY(factor_and_invert_v3(h, h->K.p, N, ld, h->W.p, ld, h->info.p, s, lead, early ? h->ev_gram : nullptr));
+      KBO_TRY(factor_and_invert_v3(h, h->K.p, N, ld, h->W.p, ld, h->info.p, s, lead, early ? &gram_rest : nullptr));
       h->w_lead = lead < N ? lead : N;
       h->w_full = lead >= N;
     }

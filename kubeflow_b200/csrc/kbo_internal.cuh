@@ -166,6 +166,16 @@ struct kbo_handle {
   DevBuf<double> Linv4;             // the four 64×64 block inverses of the current panel
   std::vector<cudaEvent_t> ev_panel;
   cudaEvent_t ev_gram = nullptr;   // the first column block of the Gram matrix is complete (the factorisation starts on it)
+  // The factorisation as one CUDA graph (fit.cu, factor_and_invert_v3): captured on s_cap (the caller's stream may be the legacy
+  // default stream, which cannot capture), replayed on the caller's stream while the key (shape, mode, device pointers) holds.
+  cudaStream_t s_cap = nullptr;
+  cudaGraph_t fit_graph = nullptr;          // the graph fit_exec was instantiated from (its nodes address fit_exec's)
+  cudaGraphExec_t fit_exec = nullptr;
+  cudaGraphNode_t fit_gram_node = nullptr;  // the Gram matrix's second launch: θ by value, set before every replay
+  std::vector<intptr_t> fit_key;
+  int fit_graph_launches = 0;               // kernel launches in the graph (counted into `launches` on every replay)
+  bool fit_stream_path = false;             // kbo_debug_fit_stream_path: enqueue the factorisation call by call
+  int fit_graph_stat[4] = {};               // captures, executable updates, instantiations, replays
   // ---- lazy inverse (fit.cu, solve.cu): the product path never needs all of W = L⁻¹ -----------------------------------------
   bool lazy_w = true;              // kbo_set_lazy_inverse: tensor-core fits form only the leading rows of W the pruning pass reads
   bool w_full = true;              // all rows of W (and the full fp16 planes) exist
@@ -270,6 +280,7 @@ int kbo_i_lml_grad_batch(kbo_handle* h, const double* X_dev, const double* y_dev
 size_t kbo_i_lml_grad_lane_bytes(int N, int D, int P);   // device memory one θ of kbo_lml_grad_batch takes
 void kbo_i_lml_batch_free(kbo_handle* h);
 void kbo_i_fit_partition_free(kbo_handle* h);
+int kbo_i_fit_graph_nodes(kbo_handle* h, int32_t* counts);   // test hook: kernel nodes of the cached graph per context
 int kbo_i_ensure_w(kbo_handle* h, cudaStream_t s);   // form the rest of W and the full planes if the fit left them out
 int kbo_i_debug_rank_rows(kbo_handle* h, const void* Xc, int xc_dtype, int64_t M, int tile_pairs, float* mun_out, float* varn_out, cudaStream_t s);
 // ---- lmlgrad.cu ---------------------------------------------------------------------------------
@@ -278,6 +289,7 @@ int kbo_i_lml_grad_from_w(kbo_handle* h, const double* Xs, int N, int D, int kin
 // ---- solve.cu ----------------------------------------------------------------------------------
 int kbo_i_alpha_by_solves(kbo_handle* h, cudaStream_t s);
 int kbo_i_variance_by_solves(kbo_handle* h, const double* Ks, int n, double* varn64, cudaStream_t s);
+int kbo_i_zsolve_reserve(kbo_handle* h);
 int kbo_i_zsolve_begin(kbo_handle* h, cudaStream_t s);
 int kbo_i_zsolve_diag(kbo_handle* h, int K0, int Wd, cudaStream_t s);
 int kbo_i_zsolve_update(kbo_handle* h, int K0, int Wd, cudaStream_t s);

@@ -293,8 +293,9 @@ __global__ void __launch_bounds__(256) sv_zupdate_kernel(const double* __restric
   if (lane == 0) b[r] -= a;
 }
 }  // namespace
+int kbo_i_zsolve_reserve(kbo_handle* h) { return kbo_reserve(h, h->zf, (size_t)(h->N + SV_P) * 2); }
+// after kbo_i_zsolve_reserve: it allocates nothing, so a graph capture may contain it
 int kbo_i_zsolve_begin(kbo_handle* h, cudaStream_t s) {
-  KBO_TRY(kbo_reserve(h, h->zf, (size_t)(h->N + SV_P) * 2));
   KBO_CUDA(h, kbo_copy(h->zf.p, h->yn.p, h->N, cudaMemcpyDeviceToDevice, s));
   h->z_ready = false;
   return KBO_OK;
