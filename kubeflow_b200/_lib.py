@@ -140,6 +140,7 @@ def load() -> C.CDLL:
     lib.kbo_debug_stage.argtypes = [vp, i32, vp, vp, vp, i32]
     lib.kbo_debug_fit_stream_path.argtypes = [vp, i32]
     lib.kbo_debug_fit_graph.argtypes = [vp, vp]
+    lib.kbo_debug_forest_sweep.argtypes = [vp, vp, vp]
     lib.kbo_debug_fp64_peak.argtypes = [vp, pd]
     lib.kbo_debug_dgemm_sm90.argtypes = [vp, i32, i32, i32, i32, vp, i32, vp, i32, vp, i32, dbl, dbl, i32, i32, i32, vp]
     lib.kbo_fit.argtypes = [vp, vp, vp, i32, i32, C.POINTER(KboParams), C.c_int, vp]
@@ -228,7 +229,7 @@ def load() -> C.CDLL:
     lib.kbo_tc_variance_raw.argtypes = [vp, vp, vp, i64, vp, vp, i32, vp, dbl, vp, vp, i32, vp]
     for name in EXPORTS + ["kbo_tc_variance_raw", "kbo_debug_rank_pass", "kbo_debug_kstar", "kbo_debug_rank_rows", "kbo_debug_record_stages",
                            "kbo_debug_stage_count", "kbo_debug_stage", "kbo_debug_fp64_peak", "kbo_debug_dgemm_sm90",
-                           "kbo_debug_fit_stream_path", "kbo_debug_fit_graph"]:
+                           "kbo_debug_fit_stream_path", "kbo_debug_fit_graph", "kbo_debug_forest_sweep"]:
         fn = getattr(lib, name)
         if fn.restype is C.c_int and name not in ("kbo_version",):
             fn.restype = C.c_int

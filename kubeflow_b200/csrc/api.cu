@@ -22,6 +22,7 @@ int kbo_create(kbo_handle** out, int device) {
   if (!h) return KBO_ERR_NOMEM;
   h->device = device;
   h->sm_count = prop.multiProcessorCount;
+  h->smem_optin = (int)prop.sharedMemPerBlockOptin;   // cudaDevAttrMaxSharedMemoryPerBlockOptin
   if (prop.major != 9) {
     // sm_90a cubin only: refuse politely instead of failing at the first launch
     h->err = "libkbo is built for sm_90a (H100) only";

@@ -51,6 +51,7 @@ struct kbo_forest : TreeCore {
   std::vector<int> h_nnodes, h_nleaves;
   std::vector<long long> h_off;
   size_t max_tree_bytes = 0;
+  int last_launch[6] = {};           // the last sweep's (staged, CPT, CTAs per SM, CTAs, static smem, opt-in limit)
 };
 
 __device__ __forceinline__ float key_f32(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }
@@ -528,30 +529,30 @@ __global__ void forest_draws_kernel(const uint32_t* __restrict__ mn, const uint3
 // ---- C ABI ------------------------------------------------------------------------------------------------------------------
 static int forest_sweep_launch(kbo_handle* h, kbo_forest* f, const float* Xc, int64_t M, int n_acq, const int32_t* acqs, double yopt, double xi,
                                double kappa, double* mu_out, double* sd_out, int* nblocks_out, cudaStream_t s) {
-  const size_t smem = f->max_tree_bytes;
-  const bool staged = smem <= 227 * 1024;
-  const int occ = !staged ? 4 : smem <= 113 * 1024 ? 2 : 1;
   const int cpt = (M + 1023) / 1024 >= 2 * h->sm_count ? 4 : 1;
+  // The largest tree is staged in shared memory when it fits there beside the kernel's own static shared memory (TreeArgmax's
+  // partials): a block may opt in to smem_optin bytes of both together.  Larger trees are walked in global memory.
+  void (*k)(SweepArgs) = cpt == 4 ? forest_sweep_kernel<4, true> : forest_sweep_kernel<1, true>;
+  cudaFuncAttributes fa;
+  KBO_CUDA(h, cudaFuncGetAttributes(&fa, k));
+  const bool staged = f->max_tree_bytes + fa.sharedSizeBytes <= (size_t)h->smem_optin;
+  const size_t sm = staged ? f->max_tree_bytes : 0;
+  if (staged) {
+    KBO_CUDA(h, cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+  } else {
+    k = cpt == 4 ? forest_sweep_kernel<4, false> : forest_sweep_kernel<1, false>;
+  }
+  int occ = 0;
+  KBO_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, 256, sm));
   const int64_t ntiles = (M + 256 * cpt - 1) / (256 * cpt);
-  const int nb = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * occ);
+  const int nb = (int)std::min<int64_t>(ntiles, (int64_t)h->sm_count * std::max(occ, 1));
   KBO_TRY(kbo_reserve(h, f->part, (size_t)nb * 3));
   SweepArgs a{f->blob.p, f->tree_off.p, f->nleaves.p, f->T, Xc, M, f->D, n_acq,
               n_acq > 0 ? acqs[0] : 0, n_acq > 1 ? acqs[1] : 0, n_acq > 2 ? acqs[2] : 0, yopt, xi, kappa, mu_out, sd_out, f->part.p};
-  const size_t sm = staged ? smem : 0;
-  if (staged) {
-    if (cpt == 4) {
-      KBO_CUDA(h, cudaFuncSetAttribute(forest_sweep_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-      forest_sweep_kernel<4, true><<<nb, 256, sm, s>>>(a);
-    } else {
-      KBO_CUDA(h, cudaFuncSetAttribute(forest_sweep_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-      forest_sweep_kernel<1, true><<<nb, 256, sm, s>>>(a);
-    }
-  } else if (cpt == 4) {
-    forest_sweep_kernel<4, false><<<nb, 256, 0, s>>>(a);
-  } else {
-    forest_sweep_kernel<1, false><<<nb, 256, 0, s>>>(a);
-  }
+  k<<<nb, 256, sm, s>>>(a);
   KBO_LAUNCH_CHECK(h);
+  const int launch[6] = {staged ? 1 : 0, cpt, occ, nb, (int)fa.sharedSizeBytes, h->smem_optin};
+  std::copy(launch, launch + 6, f->last_launch);
   *nblocks_out = nb;
   return KBO_OK;
 }
@@ -733,5 +734,14 @@ int kbo_forest_export(kbo_handle* h, kbo_forest* f, int32_t tree, int32_t* featu
 }
 
 int kbo_forest_last_timings(kbo_handle* h, kbo_forest* f, float* ms, int32_t n) { return tree_last_timings(h, f, ms, n); }
+
+// Test hook: how the last sweep or predict was launched, stats[6] = (staged, CPT, CTAs per SM, CTAs, the kernel's static shared
+// memory, the device's per-block opt-in limit).
+int kbo_debug_forest_sweep(kbo_handle* h, kbo_forest* f, int32_t* stats) {
+  if (!h || !f) return KBO_ERR_INVALID;
+  if (!stats) KBO_FAIL(h, KBO_ERR_INVALID, "kbo_debug_forest_sweep: bad argument");
+  std::copy(f->last_launch, f->last_launch + 6, stats);
+  return KBO_OK;
+}
 
 }  // extern "C"

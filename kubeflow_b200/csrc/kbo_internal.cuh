@@ -71,6 +71,7 @@ struct BlockBest;  // sweep.cu
 struct kbo_handle {
   int device = 0;
   int sm_count = 132;
+  int smem_optin = 227 * 1024;  // shared memory a block may opt in to, static and dynamic together
   std::string err;
   uint64_t scratch_limit = 4ull << 30;
 
