@@ -25,7 +25,7 @@ import logging
 import numpy as np
 
 from . import api_pb as api
-from .internal import AlgorithmSettingsError, Assignment, parse_settings
+from .internal import AlgorithmSettingsError, Assignment, parse_settings, spec_values
 from .service import _Base, _reply_from
 
 logger = logging.getLogger(__name__)
@@ -91,32 +91,10 @@ def validate_enas_settings(settings: dict) -> dict:
 
 
 def _spec_values(op_type: str, p) -> list:
-    fs = p.feasible_space
-    if p.parameter_type == api.CATEGORICAL:
-        if not len(fs.list):
-            raise AlgorithmSettingsError(f"operation {op_type!r}, parameter {p.name!r}: a CATEGORICAL spec needs a non-empty list")
-        return [str(x) for x in fs.list]
-    if p.parameter_type not in (api.INT, api.DOUBLE):
-        raise AlgorithmSettingsError(f"operation {op_type!r}, parameter {p.name!r}: only INT, DOUBLE and CATEGORICAL specs are supported")
-    if not (fs.min and fs.max and fs.step):
-        raise AlgorithmSettingsError(f"operation {op_type!r}, parameter {p.name!r}: INT and DOUBLE specs need min, max and step")
-    try:
-        if p.parameter_type == api.INT:
-            lo, hi, st = int(fs.min), int(fs.max), int(fs.step)
-        else:
-            lo, hi, st = float(fs.min), float(fs.max), float(fs.step)
-    except ValueError:
-        raise AlgorithmSettingsError(f"operation {op_type!r}, parameter {p.name!r}: min, max and step must be numbers")
-    if not (st > 0 and lo <= hi and np.isfinite(lo) and np.isfinite(hi) and np.isfinite(st)):
-        raise AlgorithmSettingsError(f"operation {op_type!r}, parameter {p.name!r}: need step > 0 and min <= max")
-    if (hi - lo) / st >= MAX_OPS:
-        raise AlgorithmSettingsError(f"operation {op_type!r}, parameter {p.name!r}: more than this engine's limit of {MAX_OPS} values")
-    if p.parameter_type == api.INT:
-        return list(range(lo, hi + 1, st))
-    vals = np.arange(lo, hi + st, st)
-    if vals[-1] > hi:
-        vals = vals[:-1]
-    return [float(x) for x in vals]
+    where = f"operation {op_type!r}, parameter {p.name!r}"
+    if p.parameter_type not in (api.INT, api.DOUBLE, api.CATEGORICAL):
+        raise AlgorithmSettingsError(f"{where}: only INT, DOUBLE and CATEGORICAL specs are supported")
+    return spec_values(p, where, MAX_OPS)
 
 
 def expand_operations(operations) -> list:

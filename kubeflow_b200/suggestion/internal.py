@@ -6,6 +6,8 @@ from __future__ import annotations
 
 from dataclasses import dataclass, field
 
+import numpy as np
+
 from . import api_pb as api
 
 INTEGER, DOUBLE, CATEGORICAL, DISCRETE = "int", "double", "categorical", "discrete"
@@ -136,3 +138,37 @@ class Trial:
 
 def parse_settings(experiment) -> dict:
     return {s.name: s.value for s in experiment.spec.algorithm.algorithm_settings}
+
+
+def spec_values(p, where: str, limit: int) -> list:
+    """The values of one ``ParameterSpec``, in order [RECALL: Katib's ENAS Operation.py and its Optuna service's grid search]:
+    INT → range(min, max + 1, step), DOUBLE → np.arange(min, max + step, step) with an endpoint above max dropped,
+    CATEGORICAL and DISCRETE → the feasible list as strings.  AlgorithmSettingsError, prefixed by ``where``, for a spec with no
+    such values or with more than ``limit`` of them (checked before any list is built)."""
+    fs = p.feasible_space
+    if p.parameter_type in (api.CATEGORICAL, api.DISCRETE):
+        if not len(fs.list):
+            kind = "CATEGORICAL" if p.parameter_type == api.CATEGORICAL else "DISCRETE"
+            raise AlgorithmSettingsError(f"{where}: a {kind} spec needs a non-empty list")
+        return [str(x) for x in fs.list]
+    if p.parameter_type not in (api.INT, api.DOUBLE):
+        raise AlgorithmSettingsError(f"{where}: only INT, DOUBLE, CATEGORICAL and DISCRETE specs have values")
+    if not (fs.min and fs.max and fs.step):
+        raise AlgorithmSettingsError(f"{where}: INT and DOUBLE specs need min, max and step")
+    try:
+        if p.parameter_type == api.INT:
+            lo, hi, st = int(fs.min), int(fs.max), int(fs.step)
+        else:
+            lo, hi, st = float(fs.min), float(fs.max), float(fs.step)
+    except ValueError:
+        raise AlgorithmSettingsError(f"{where}: min, max and step must be numbers")
+    if not (st > 0 and lo <= hi and np.isfinite(lo) and np.isfinite(hi) and np.isfinite(st)):
+        raise AlgorithmSettingsError(f"{where}: need step > 0 and min <= max")
+    if (hi - lo) / st >= limit:
+        raise AlgorithmSettingsError(f"{where}: more than this engine's limit of {limit} values")
+    if p.parameter_type == api.INT:
+        return list(range(lo, hi + 1, st))
+    vals = np.arange(lo, hi + st, st)
+    if vals[-1] > hi:
+        vals = vals[:-1]
+    return [float(x) for x in vals]

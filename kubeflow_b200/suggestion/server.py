@@ -61,14 +61,25 @@ class SuggestionStub:
                                                response_deserializer=lambda b: b)
 
 
-def main():
+def services(dev: dict, shard: bool = False) -> list:
+    """The servicers ``main`` routes to, one per algorithm name Katib ships; ``dev`` holds the engine defaults (``device``), and
+    ``shard`` makes the algorithms that shard their candidates over the ranks of an SPMD run (suggestion/spmd.py) do so."""
     from .cmaes_service import CmaesService
+    from .darts_service import DartsService
     from .enas_service import EnasService
+    from .grid_service import GridService
     from .hyperband import HyperbandService
     from .mvtpe_service import MultivariateTpeService
     from .pbt_service import PbtService
-    from .service import DispatchService, RandomService, SkoptService, SobolService
+    from .service import RandomService, SkoptService, SobolService
     from .tpe_service import TpeService
+    sharded = {**dev, "shard": True} if shard else dev
+    return [SkoptService(sharded), RandomService(), SobolService(), CmaesService(dev), TpeService(sharded),
+            MultivariateTpeService(sharded), EnasService(dev), HyperbandService(), PbtService(), GridService(), DartsService()]
+
+
+def main():
+    from .service import DispatchService
     ap = argparse.ArgumentParser()
     ap.add_argument("--port", type=int, default=DEFAULT_PORT)
     ap.add_argument("--device", type=int, default=0)
@@ -85,11 +96,7 @@ def main():
         local = int(os.environ.get("LOCAL_RANK", "0"))
         torch.cuda.set_device(local)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-        dev = {"device": local}
-        inner = DispatchService([SkoptService({**dev, "shard": True}), RandomService(), SobolService(), CmaesService(dev),
-                                 TpeService({**dev, "shard": True}), MultivariateTpeService({**dev, "shard": True}), EnasService(dev),
-                                 HyperbandService(), PbtService()])
-        spmd = SpmdServicer(inner)
+        spmd = SpmdServicer(DispatchService(services({"device": local}, shard=True)))
         if dist.get_rank() == 0:
             server, port = serve(spmd, args.port)
             logging.info("api.v1.beta1.Suggestion listening on :%d, %d ranks", port, dist.get_world_size())
@@ -101,9 +108,7 @@ def main():
             spmd.worker_loop()
         dist.destroy_process_group()
         return
-    dev = {"device": args.device}
-    server, port = serve(DispatchService([SkoptService(dev), RandomService(), SobolService(), CmaesService(dev), TpeService(dev),
-                                          MultivariateTpeService(dev), EnasService(dev), HyperbandService(), PbtService()]), args.port)
+    server, port = serve(DispatchService(services({"device": args.device})), args.port)
     logging.info("api.v1.beta1.Suggestion listening on :%d", port)
     server.wait_for_termination()
 
